@@ -303,6 +303,59 @@ GS_API int gs_sort_pairs_host(GsContext *ctx, uint32_t *keys, uint32_t *payload,
 GS_API int gs_export_splats(GsContext *ctx, GsAsset *asset, const GsCutout *cutouts, uint32_t cutout_count,
                             uint32_t bake_transform, void *dst);
 
+/* ---- asset packer on the GPU (CreateAsset, E/GaussianSplatAssetCreator.cs:248-330) ----------------------------------
+ * The device twin of gsa_create_asset (include/gsplat_asset.h, the host packer): bounds, Morton reorder, SH palette
+ * clustering (mini-batch k-means with k-means++ seeding), chunk quantisation, the format encodes and BC7.  For finite input
+ * the five blobs and the bounds are the same bytes the host packer writes.  Input containing NaN or Inf still yields a
+ * well-formed asset of the right size, without faulting, but its bytes are not guaranteed to match the host packer's. */
+
+/* InputSplatData (E/Utils/GaussianFileReader.cs:17-26), 62 floats / 248 bytes, after LinearizeData: the same layout as
+ * GsaInputSplat of gsplat_asset.h, restated so that this header stands alone. */
+typedef struct GsInputSplat {
+  float pos[3];
+  float nor[3];
+  float dc0[3];
+  float sh[45]; /* sh1..shF, each rgb */
+  float opacity;
+  float scale[3];
+  float rot[4];
+} GsInputSplat;
+
+typedef struct GsPackSizes {   /* byte sizes of the five blobs (the gsa_calc_sizes values) and the colour texture */
+  uint64_t pos_bytes, other_bytes, color_bytes, sh_bytes, chunk_bytes;
+  uint32_t tex_width, tex_height;
+} GsPackSizes;
+
+typedef struct GsPackDesc {
+  const GsInputSplat *splats;   /* splat_count records; read only, never modified */
+  uint32_t splat_count;
+  uint32_t memory;              /* GsMemory: where `splats` lives (device memory must belong to the context's device) */
+  uint32_t pos_format, scale_format, color_format, sh_format;   /* GsVectorFormat x2, GsColorFormat, GsSHFormat */
+} GsPackDesc;
+
+typedef struct GsPackedAsset {
+  void *pos, *other, *color, *sh, *chunks;   /* caller's buffers of gs_pack_sizes bytes each; chunks may be NULL when chunk_bytes is 0 */
+  uint32_t memory;                           /* GsMemory of the five buffers */
+  uint32_t reserved;
+  float bounds_min[3], bounds_max[3];        /* out: position bounds of the input */
+} GsPackedAsset;
+
+/* gsa_calc_sizes' arithmetic and rules: GS_ERR_UNSUPPORTED_FORMAT for an unknown format or a clustered SH format with no
+ * more splats than palette entries. */
+GS_API int gs_pack_sizes(uint32_t splat_count, uint32_t pos_format, uint32_t scale_format, uint32_t color_format,
+                         uint32_t sh_format, GsPackSizes *out);
+/* Packs desc->splats on the context's device.  blobs_out (may be NULL) receives the blobs in host or device memory;
+ * asset_out (may be NULL) receives a ready GsAsset, as gs_asset_upload makes it (draw order reset, blobs in HBM), built
+ * without a host copy of the blobs.  At least one of the two must be given.  Blocks until the results are complete. */
+GS_API int gs_pack_asset(GsContext *ctx, const GsPackDesc *desc, GsPackedAsset *blobs_out, GsAsset **asset_out);
+/* The device twin of gsa_kmeans (gsplat_asset.h): the same means and labels, bit for bit.  Host pointers: data
+ * n x dim floats, means_out k x dim, labels_out n.  dim must be 1..128. Blocks. */
+GS_API int gs_kmeans(GsContext *ctx, uint32_t dim, const float *data, uint32_t n, uint32_t batch, float passes,
+                     float *means_out, uint32_t k, int32_t *labels_out);
+/* Counters of the last gs_pack_asset: [0] scale^(1/8) values recomputed on the host because the device's double pow
+ * result lay next to a float rounding midpoint (see DESIGN.md), [1] k-means mini-batch iterations, [2] k-means++ rounds. */
+GS_API int gs_debug_pack_stats(GsContext *ctx, uint64_t out[4]);
+
 /* ---- test hooks (blocking device->host reads) ----------------------------------- */
 GS_API int gs_readback_order(GsAsset *asset, uint32_t *dst);      /* _SplatSortKeys, N words */
 GS_API int gs_readback_keys(GsAsset *asset, uint32_t *dst);       /* _SplatSortDistances, N words (sorted after gs_sort) */

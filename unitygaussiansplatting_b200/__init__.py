@@ -6,8 +6,9 @@ from .asset import (ColorFormat, GaussianSplatAsset, SHFormat, VectorFormat, QUA
 from .camera import Camera, look_rotation, trs, quat_to_mat
 from .renderer import (GaussianSplatContext, GaussianSplatRenderer, GatherSplatsForCamera, SortAndRenderSplatsMulti,
                        make_frame_params)
+from .pack import pack_asset
 from ._native import GsError
 
 __all__ = ["ColorFormat", "GaussianSplatAsset", "SHFormat", "VectorFormat", "QUALITY", "SCENE_CLUSTERED", "SCENE_LATTICE",
            "SCENE_UNIFORM", "create_asset", "generate_input_splats", "read_ply", "read_spz", "write_ply", "save_asset", "load_asset", "synthetic_asset", "Camera", "look_rotation", "trs",
-           "quat_to_mat", "GaussianSplatContext", "GaussianSplatRenderer", "GatherSplatsForCamera", "SortAndRenderSplatsMulti", "make_frame_params", "GsError"]
+           "quat_to_mat", "GaussianSplatContext", "GaussianSplatRenderer", "GatherSplatsForCamera", "SortAndRenderSplatsMulti", "make_frame_params", "pack_asset", "GsError"]

@@ -96,6 +96,21 @@ class GsStageTimes(C.Structure):
                 ("reserved", C.c_uint32)]
 
 
+class GsPackSizes(C.Structure):
+    _fields_ = [("pos_bytes", C.c_uint64), ("other_bytes", C.c_uint64), ("color_bytes", C.c_uint64), ("sh_bytes", C.c_uint64),
+                ("chunk_bytes", C.c_uint64), ("tex_width", C.c_uint32), ("tex_height", C.c_uint32)]
+
+
+class GsPackDesc(C.Structure):
+    _fields_ = [("splats", C.c_void_p), ("splat_count", C.c_uint32), ("memory", C.c_uint32), ("pos_format", C.c_uint32),
+                ("scale_format", C.c_uint32), ("color_format", C.c_uint32), ("sh_format", C.c_uint32)]
+
+
+class GsPackedAsset(C.Structure):
+    _fields_ = [("pos", C.c_void_p), ("other", C.c_void_p), ("color", C.c_void_p), ("sh", C.c_void_p), ("chunks", C.c_void_p),
+                ("memory", C.c_uint32), ("reserved", C.c_uint32), ("bounds_min", C.c_float * 3), ("bounds_max", C.c_float * 3)]
+
+
 class GsaSizes(C.Structure):
     _fields_ = [("pos_bytes", C.c_uint64), ("other_bytes", C.c_uint64), ("color_bytes", C.c_uint64), ("sh_bytes", C.c_uint64),
                 ("chunk_bytes", C.c_uint64), ("tex_width", C.c_uint32), ("tex_height", C.c_uint32)]
@@ -146,6 +161,11 @@ NATIVE_SYMBOLS = {
     "gs_debug_raster_stats": (C.c_int, [C.c_void_p, C.c_void_p]),
     "gs_context_stream": (C.c_void_p, [C.c_void_p]),
     "gs_asset_device_ptr": (C.c_void_p, [C.c_void_p, C.c_int]),
+    "gs_pack_sizes": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(GsPackSizes)]),
+    "gs_pack_asset": (C.c_int, [C.c_void_p, C.POINTER(GsPackDesc), C.POINTER(GsPackedAsset), C.POINTER(C.c_void_p)]),
+    "gs_kmeans": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_float, C.c_void_p, C.c_uint32,
+                            C.c_void_p]),
+    "gs_debug_pack_stats": (C.c_int, [C.c_void_p, C.c_void_p]),
 }
 
 ASSET_SYMBOLS = {

@@ -23,7 +23,7 @@ CSRC = PKG / "csrc"
 NATIVE_LIB = PKG / "libgsplat_b200.so"
 ASSET_LIB = PKG / "libgsplat_asset.so"
 
-CU_SOURCES = ["gs_api.cu", "gs_group.cu", "gs_view.cu", "gs_sort.cu", "gs_raster.cu", "gs_export.cu"]
+CU_SOURCES = ["gs_api.cu", "gs_group.cu", "gs_view.cu", "gs_sort.cu", "gs_raster.cu", "gs_export.cu", "gs_pack.cu"]
 CU_HEADERS = ["gs_common.cuh", "gs_kernels.cuh", "gs_internal.cuh", "gs_nccl.h", "gs_bc7.cuh", "bc7_tables.h", "../../include/gsplat_b200.h"]
 
 

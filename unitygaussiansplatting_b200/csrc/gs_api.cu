@@ -368,6 +368,26 @@ static int init_staging(GsContext *ctx, const GsRenderOptions &opt, void *d_rt, 
   return GS_OK;
 }
 
+cudaError_t asset_init_work(GsContext *ctx, GsAsset *as, uint32_t n, uint32_t pos_fmt, uint32_t scale_fmt, uint32_t sh_fmt,
+                            uint32_t col_fmt, uint32_t chunk_count) {
+  cudaError_t e = cudaSuccess;
+  if ((e = cudaMalloc(&as->order, (size_t)n * 4)) != cudaSuccess || (e = cudaMalloc(&as->keys, (size_t)n * 4)) != cudaSuccess ||
+      (e = cudaMalloc(&as->key_table, (size_t)n * 4)) != cudaSuccess || (e = cudaMalloc(&as->draw, (size_t)n * 48)) != cudaSuccess ||
+      (e = cudaMalloc(&as->view, (size_t)n * kViewStride + 16)) != cudaSuccess || (e = cudaMalloc(&as->rect, (size_t)n * 4)) != cudaSuccess ||
+      (e = cudaMalloc(&as->d_n, 4)) != cudaSuccess || (e = cudaMalloc(&as->block_bits, block_bits_words(n) * 4 + 64)) != cudaSuccess)
+    return e;
+  if ((e = cudaMemcpyAsync(as->d_n, &n, 4, cudaMemcpyHostToDevice, ctx->stream)) != cudaSuccess) return e;
+  as->av.n = n;
+  as->av.posFmt = pos_fmt; as->av.scaleFmt = scale_fmt; as->av.shFmt = sh_fmt; as->av.colFmt = col_fmt;
+  as->av.chunkCount = chunk_count;
+  as->av.pos = (const uint8_t *)as->d_pos; as->av.other = (const uint8_t *)as->d_other; as->av.sh = (const uint8_t *)as->d_sh;
+  as->av.color = (const uint8_t *)as->d_color; as->av.chunks = (const Chunk *)as->d_chunks;
+  launch_set_indices(as->order, as->av.n, ctx->stream);  // CSSetIndices
+  ctx->launches += 1;
+  // `n` is a stack value: the copy above must have left it before this returns
+  return cudaStreamSynchronize(ctx->stream);
+}
+
 static int check_bin_overflow(GsContext *ctx) {
   uint32_t ec[2] = {0, 0};
   GS_CUDA_TRY(ctx, cudaMemcpyAsync(ec, ctx->bin.entry_count, 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -529,22 +549,10 @@ int gs_asset_upload(GsContext *ctx, const GsAssetDesc *d, GsAsset **out) {
   if ((e = up(&as->d_pos, d->pos, d->pos_bytes)) != cudaSuccess || (e = up(&as->d_other, d->other, d->other_bytes)) != cudaSuccess ||
       (e = up(&as->d_sh, d->sh, d->sh_bytes, sh_min)) != cudaSuccess || (e = up(&as->d_color, d->color, d->color_bytes)) != cudaSuccess ||
       (chunk_count && (e = up(&as->d_chunks, d->chunks, (uint64_t)chunk_count * 64)) != cudaSuccess) ||
-      (e = cudaMalloc(&as->order, n * 4)) != cudaSuccess || (e = cudaMalloc(&as->keys, n * 4)) != cudaSuccess ||
-      (e = cudaMalloc(&as->key_table, n * 4)) != cudaSuccess || (e = cudaMalloc(&as->draw, n * 48)) != cudaSuccess ||
-      (e = cudaMalloc(&as->view, n * kViewStride + 16)) != cudaSuccess || (e = cudaMalloc(&as->rect, n * 4)) != cudaSuccess ||
-      (e = cudaMalloc(&as->d_n, 4)) != cudaSuccess || (e = cudaMalloc(&as->block_bits, block_bits_words(d->splat_count) * 4 + 64)) != cudaSuccess) {
+      (e = asset_init_work(ctx, as, d->splat_count, d->pos_format, d->scale_format, d->sh_format, d->color_format, chunk_count)) != cudaSuccess) {
     gs_asset_destroy(as);
     return fail_cuda(ctx, e, "asset upload", __FILE__, __LINE__);
   }
-  uint32_t n32 = d->splat_count;
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(as->d_n, &n32, 4, cudaMemcpyHostToDevice, ctx->stream));
-  as->av.n = d->splat_count;
-  as->av.posFmt = d->pos_format; as->av.scaleFmt = d->scale_format; as->av.shFmt = d->sh_format; as->av.colFmt = d->color_format;
-  as->av.chunkCount = chunk_count;
-  as->av.pos = (const uint8_t *)as->d_pos; as->av.other = (const uint8_t *)as->d_other; as->av.sh = (const uint8_t *)as->d_sh;
-  as->av.color = (const uint8_t *)as->d_color; as->av.chunks = (const Chunk *)as->d_chunks;
-  launch_set_indices(as->order, as->av.n, ctx->stream);  // CSSetIndices
-  ctx->launches += 1;
   GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // host blobs are only borrowed for this call
   *out = as;
   return GS_OK;

@@ -65,6 +65,7 @@ struct GsContext {
   size_t depth_bytes = 0;
   const float *cur_depth = nullptr;  // what the compositor tests against this frame (nullptr: no depth test)
   uint32_t launches = 0;
+  uint64_t pack_stats[4] = {0, 0, 0, 0};   // gs_debug_pack_stats
 };
 
 struct GsAsset {
@@ -98,6 +99,10 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
 int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRenderOptions &opt, void *d_rt, uint32_t pitch, uint32_t fmt);
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch);
 uint32_t pix_bytes(uint32_t fmt);
+// The per-asset work buffers (order, keys, view data, ...) of an asset whose blobs as->d_* are already in HBM, the format
+// fields of as->av, and CSSetIndices: what gs_asset_upload and gs_pack_asset share.
+cudaError_t asset_init_work(GsContext *ctx, GsAsset *as, uint32_t n, uint32_t pos_fmt, uint32_t scale_fmt, uint32_t sh_fmt,
+                            uint32_t col_fmt, uint32_t chunk_count);
 void rec(GsContext *ctx, int e);
 void launch_row_costs(const uint32_t *cost, uint32_t ntx, uint32_t t0, uint32_t t1, uint32_t *row_cost, cudaStream_t s);   // gs_raster.cu
 }  // namespace gs

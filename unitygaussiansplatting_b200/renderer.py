@@ -219,6 +219,22 @@ def make_frame_params(cam: Camera, localToWorld=None, splat_scale=1.0, opacity_s
 
 class GaussianSplatRenderer:
     def __init__(self, asset: GaussianSplatAsset, context: Optional[GaussianSplatContext] = None):
+        self._init_state(asset, context)
+        d = asset.desc()
+        h = C.c_void_p()
+        N.check(self.context.handle, self._lib.gs_asset_upload(self.context.handle, C.byref(d), C.byref(h)))
+        self._asset = h
+
+    @classmethod
+    def from_device_asset(cls, asset: GaussianSplatAsset, handle: C.c_void_p, context: GaussianSplatContext):
+        """A renderer on a GsAsset that is already in HBM (gs_pack_asset's asset_out); it takes ownership of `handle`.
+        `asset` is the host copy of the same blobs."""
+        self = cls.__new__(cls)
+        self._init_state(asset, context)
+        self._asset = handle
+        return self
+
+    def _init_state(self, asset: GaussianSplatAsset, context: Optional[GaussianSplatContext]):
         self.context = context or GaussianSplatContext(0)
         self._lib = self.context._lib
         self.m_Asset = asset
@@ -243,10 +259,7 @@ class GaussianSplatRenderer:
         self.rows = (0, 0)           # contiguous partition: 16-pixel rows [begin, end) (GsRenderOptions.row_begin/row_end)
         self.load_rt = False         # GS_FLAG_LOAD_RT: blend under what the target already holds (several renderers, one RT)
         self.async_readback = False  # host render targets are filled asynchronously (pinned memory; context.sync() completes them)
-        d = asset.desc()
-        h = C.c_void_p()
-        N.check(self.context.handle, self._lib.gs_asset_upload(self.context.handle, C.byref(d), C.byref(h)))
-        self._asset = h
+        self._asset = None
         self._keep = None
 
     # -- resources ---------------------------------------------------------------------------
