@@ -343,6 +343,25 @@ __device__ __forceinline__ void bulk_copy_g2s(void *smem_dst, const void *gmem_s
                "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
+// Can any pixel centre of the 8x4 block centred on (bcx, bcy) lie inside the splat's quad, |qa| <= 2 and |qb| <= 2 with
+// q = (dot(d, i1), dot(d, i2))?  (A = cx, cy, i1x, i1y; i2 = (i2x, i2y).)  The pixel centres lie within 3.5 / 1.5 pixels of
+// the block's centre, so each q of a pixel differs from its value at the centre by at most r = 3.5 |ix| + 1.5 |iy|.  Both
+// evaluations round, by far less than 1e-5 of the magnitudes involved, and that much is added to the bound.  A candidate
+// this test drops is one for which the per-pixel test finds no pixel inside, so the candidates that are evaluated, and
+// their order, are unchanged; it only saves the candidate loop's quad test for splats whose box touches the block but
+// whose quad does not.  A NaN keeps the candidate.
+__device__ __forceinline__ bool block_may_touch_quad(const float4 &A, float i2x, float i2y, float bcx, float bcy) {
+  const float dxc = bcx - A.x, dyc = A.y - bcy;   // as the per-pixel test: pixel y grows down, NDC y up
+  auto axis_ok = [&](float ix, float iy) {
+    const float tx = dxc * ix, ty = dyc * iy;
+    const float r = 3.5f * fabsf(ix) + 1.5f * fabsf(iy);
+    const float bound = 2.0f + r;
+    const float slack = 1e-5f * (fabsf(tx) + fabsf(ty) + bound);
+    return !(fabsf(tx + ty) > bound + slack);
+  };
+  return axis_ok(A.z, A.w) && axis_ok(i2x, i2y);
+}
+
 // SEL ("extras"): a separate instantiation for frames with an edit selection and / or a scene depth buffer bound, so that
 // ordinary frames pay nothing.  Selected splats (records with opacity -1) take the pixel shader's other branch
 // (S/RenderGaussianSplats.shader:87-101); with `scene_depth` every fragment is depth-tested like the pass's ZTest LEqual
@@ -465,6 +484,10 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
         const float4 A = s_a[e * ES];
         const float hx = s_b[e * ES].w, hy = s_c[e * ES].w;
         hit = (fabsf(A.x - bcx) <= hx + 3.5f) && (fabsf(A.y - bcy) <= hy + 1.5f);
+        if (hit) {
+          const float4 B = s_b[e * ES];
+          hit = block_may_touch_quad(A, B.x, B.y, bcx, bcy);
+        }
       }
       uint32_t mask = __ballot_sync(0xffffffffu, hit);
       while (mask) {
