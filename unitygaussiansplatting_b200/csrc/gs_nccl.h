@@ -23,8 +23,6 @@ struct NcclApi {
   ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
   ncclResult_t (*AllGather)(const void *, void *, size_t, ncclDataType_t, ncclComm_t, cudaStream_t) = nullptr;
   ncclResult_t (*Broadcast)(const void *, void *, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
-  ncclResult_t (*Send)(const void *, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
-  ncclResult_t (*Recv)(void *, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
   ncclResult_t (*GroupStart)() = nullptr;
   ncclResult_t (*GroupEnd)() = nullptr;
   const char *(*GetErrorString)(ncclResult_t) = nullptr;
@@ -47,14 +45,12 @@ inline const NcclApi &nccl_api() {
     GS_NCCL_SYM(CommDestroy, "ncclCommDestroy");
     GS_NCCL_SYM(AllGather, "ncclAllGather");
     GS_NCCL_SYM(Broadcast, "ncclBroadcast");
-    GS_NCCL_SYM(Send, "ncclSend");
-    GS_NCCL_SYM(Recv, "ncclRecv");
     GS_NCCL_SYM(GroupStart, "ncclGroupStart");
     GS_NCCL_SYM(GroupEnd, "ncclGroupEnd");
     GS_NCCL_SYM(GetErrorString, "ncclGetErrorString");
     GS_NCCL_SYM(GetVersion, "ncclGetVersion");
 #undef GS_NCCL_SYM
-    if (a.GetUniqueId && a.CommInitRank && a.CommInitAll && a.CommDestroy && a.AllGather && a.Broadcast && a.Send && a.Recv &&
+    if (a.GetUniqueId && a.CommInitRank && a.CommInitAll && a.CommDestroy && a.AllGather && a.Broadcast &&
         a.GroupStart && a.GroupEnd && a.GetErrorString)
       a.lib = h;
     return a;

@@ -318,31 +318,6 @@ void launch_row_costs(const uint32_t *cost, uint32_t ntx, uint32_t t0, uint32_t 
   if (t1 > t0) k_row_costs<<<(t1 - t0 + 7) / 8, 256, 0, s>>>(cost, ntx, t0, t1, row_cost);
 }
 
-// ---- TMA (bulk async copy) staging: one 48-byte cp.async.bulk per record, completion counted in bytes on an mbarrier ----
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t *bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "GS_WAIT:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra GS_DONE;\n\t"
-      "bra GS_WAIT;\n\t"
-      "GS_DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_copy_g2s(void *smem_dst, const void *gmem_src, uint32_t bytes, uint64_t *bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
-               "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
 // Can any pixel centre of the 8x4 block centred on (bcx, bcy) lie inside the splat's quad, |qa| <= 2 and |qb| <= 2 with
 // q = (dot(d, i1), dot(d, i2))?  (A = cx, cy, i1x, i1y; i2 = (i2x, i2y).)  The pixel centres lie within 3.5 / 1.5 pixels of
 // the block's centre, so each q of a pixel differs from its value at the centre by at most r = 3.5 |ix| + 1.5 |iy|.  Both
@@ -366,7 +341,7 @@ __device__ __forceinline__ bool block_may_touch_quad(const float4 &A, float i2x,
 // ordinary frames pay nothing.  Selected splats (records with opacity -1) take the pixel shader's other branch
 // (S/RenderGaussianSplats.shader:87-101); with `scene_depth` every fragment is depth-tested like the pass's ZTest LEqual
 // (reversed Z: quad depth >= stored depth), the per-splat quad depths being staged beside the records.
-template <bool FP16_ROP, int OUT_FMT, bool STATS, bool TMA, bool SEL = false>
+template <bool FP16_ROP, int OUT_FMT, bool STATS, bool SEL = false>
 __global__ void __launch_bounds__(256)
 k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const uint2 *__restrict__ bin_ranges,
          const uint32_t *__restrict__ tile_vals, const uint32_t *__restrict__ tile_order, uint32_t *__restrict__ tile_cost, uint32_t ntx,
@@ -375,22 +350,11 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   uint32_t st_batches = 0, st_culls = 0, st_cand = 0, st_eval = 0, st_blend = 0;   // GS_RASTER_STATS diagnostics (per warp)
   unsigned long long st_t0 = 0;
   if (STATS) asm volatile("mov.u64 %0, %globaltimer;" : "=l"(st_t0));
-  // two staging buffers of 256 raster records (3 x float4 each): batch k+1 lands asynchronously while batch k is composited.
-  // cp.async path: planar [buf][plane][entry]; TMA path: the 48-byte records as they are, [buf][entry][plane].
+  // two staging buffers of 256 raster records (3 x float4 each, planar [buf][plane][entry]): batch k+1 lands
+  // asynchronously while batch k is composited
   __shared__ __align__(128) float4 s_rec[2][3][256];  // plane 0: cx, cy, i1x, i1y   1: i2x, i2y, opacity, hx   2: r, g, b, hy
-  __shared__ __align__(8) uint64_t s_bar[2];
   __shared__ float s_z[SEL ? 2 : 1][SEL ? 256 : 1];   // quad depths of the staged batch (depth test only)
   const bool depth_test = SEL && scene_depth != nullptr;
-  constexpr int ES = TMA ? 3 : 1;     // float4 stride between consecutive entries of one plane
-  constexpr int PS = TMA ? 1 : 256;   // float4 stride between the planes of one entry
-  if (TMA) {
-    if (threadIdx.x == 0) {
-      mbar_init(&s_bar[0], 256);
-      mbar_init(&s_bar[1], 256);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-  }
 
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   // 1-D grid over raster tiles: tile = (16-pixel column, R * own 64-pixel bin row + tile row inside that bin row)
@@ -433,17 +397,6 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   // three-deep pipeline: splat ids of batch k+2 (register) -> records of batch k+1 (cp.async in flight) -> batch k (composited)
   auto load_id = [&](uint32_t e) -> uint32_t { return e < range.y ? __ldg(tile_vals + e) : 0xFFFFFFFFu; };
   auto stage = [&](int buf, uint32_t id) {
-    float4 *base_f4 = &s_rec[buf][0][0];
-    if (TMA) {
-      // every thread arrives once per stage; a thread with a record first announces its 48 bytes, then issues the bulk copy
-      if (id != 0xFFFFFFFFu) {
-        mbar_arrive_expect_tx(&s_bar[buf], 48u);
-        bulk_copy_g2s(base_f4 + (size_t)tid * 3, draw + (size_t)id * 3, 48u, &s_bar[buf]);
-      } else {
-        mbar_arrive(&s_bar[buf]);
-      }
-      return;
-    }
     if (id != 0xFFFFFFFFu) {
       const float4 *src = draw + (size_t)id * 3;
       cp_async16(&s_rec[buf][0][tid], src);
@@ -455,21 +408,15 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   };
   uint32_t id_next = load_id(range.x + tid);
   stage(0, id_next);
-  uint32_t issued = 0;   // index of the newest stage handed to the copy engine
   id_next = load_id(range.x + 256 + tid);
 
   int buf = 0;
-  uint32_t kbatch = 0;   // stage index: stage s lives in buffer s&1 and completes phase (s>>1)&1 of that buffer's mbarrier
-  for (uint32_t base = range.x; base < range.y; base += 256, buf ^= 1, ++kbatch) {
-    stage(buf ^ 1, id_next); issued = kbatch + 1;  // batch k+1 -> other buffer (free since the barrier that ended batch k-1)
+  for (uint32_t base = range.x; base < range.y; base += 256, buf ^= 1) {
+    stage(buf ^ 1, id_next);                       // batch k+1 -> other buffer (free since the barrier that ended batch k-1)
     id_next = load_id(base + 512 + tid);           // ids of batch k+2
-    if (TMA) {
-      mbar_wait(&s_bar[buf], (kbatch >> 1) & 1u);  // all 256 arrivals + every announced byte of batch k have landed
-    } else {
-      cp_async_wait<1>();                          // batch k has landed (this thread's copies) ...
-      __syncthreads();                             // ... and everyone else's
-    }
-    const float4 *s_a = &s_rec[buf][0][0], *s_b = s_a + PS, *s_c = s_a + 2 * PS;
+    cp_async_wait<1>();                            // batch k has landed (this thread's copies) ...
+    __syncthreads();                               // ... and everyone else's
+    const float4 *s_a = s_rec[buf][0], *s_b = s_rec[buf][1], *s_c = s_rec[buf][2];
 
     const uint32_t cnt = min(256u, range.y - base);
     ++st_batches;
@@ -481,11 +428,11 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
       const uint32_t e = c0 + lane;
       bool hit = false;
       if (e < cnt) {
-        const float4 A = s_a[e * ES];
-        const float hx = s_b[e * ES].w, hy = s_c[e * ES].w;
+        const float4 A = s_a[e];
+        const float hx = s_b[e].w, hy = s_c[e].w;
         hit = (fabsf(A.x - bcx) <= hx + 3.5f) && (fabsf(A.y - bcy) <= hy + 1.5f);
         if (hit) {
-          const float4 B = s_b[e * ES];
+          const float4 B = s_b[e];
           hit = block_may_touch_quad(A, B.x, B.y, bcx, bcy);
         }
       }
@@ -494,7 +441,7 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
         const uint32_t j = c0 + __ffs(mask) - 1;
         mask &= mask - 1;
         if (STATS) ++st_cand;
-        const float4 A = s_a[j * ES], B = s_b[j * ES];
+        const float4 A = s_a[j], B = s_b[j];
         const float dx = pxc - A.x, dy = A.y - pyc;  // pixel y grows down, NDC y up
         const float qa = fmaf(dy, A.w, dx * A.z), qb = fmaf(dy, B.y, dx * B.x);
         const bool inside = (fabsf(qa) <= 2.0f) && (fabsf(qb) <= 2.0f);  // quad corners at +-2 (:54-55)
@@ -516,7 +463,7 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
         if (SEL && depth_test) pass = pass && (s_z[SEL ? buf : 0][SEL ? j : 0] >= zscene);   // ZTest LEqual, reversed Z
         if (pass) {
           if (STATS) ++st_blend;
-          float4 C = s_c[j * ES];
+          float4 C = s_c[j];
           if (SEL && tint) {
             if (outline) { C.x = 1.0f; C.y = 0.0f; C.z = 1.0f; }
             C.x = lerpf(C.x, 1.0f, 0.5f); C.y = lerpf(C.y, 0.0f, 0.5f); C.z = lerpf(C.z, 1.0f, 0.5f);
@@ -536,12 +483,7 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
     // frees this batch's buffer for the copies issued at the top of the next-but-one iteration.
     if (__syncthreads_and(d3 == 1.0f || !in_image)) break;
   }
-  if (TMA) {
-    // exactly one issued stage has not been waited for (the look-ahead one, or stage 0 of an empty list): drain it
-    mbar_wait(&s_bar[issued & 1u], (issued >> 1) & 1u);
-  } else {
-    cp_async_wait<0>();
-  }
+  cp_async_wait<0>();
   // this tile's cost for next frame's launch order: the slowest warp's work (evaluations dominate, culls and batches add)
   if (lane == 0) atomicMax(&s_cost, st_eval * 4 + st_batches * 16 + 1);
   __syncthreads();
@@ -573,7 +515,6 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
 }
 
 unsigned long long *g_raster_stats = nullptr;
-static constexpr int kRasterTmaDefault = 0;
 
 void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const BinScratch &bs, void *rt,
                    uint32_t rt_pitch_bytes, uint32_t rt_format, cudaStream_t s, const float *zndc, const float *scene_depth) {
@@ -591,19 +532,15 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const floa
   if (want < 0) { const char *e = getenv("GS_RASTER_STATS"); want = (e && e[0] == '1') ? 1 : 0; }
   if (want && !stats) { cudaMalloc(&stats, 64); g_raster_stats = stats; }
   if (stats) cudaMemsetAsync(stats, 0, 64, s);
-  // GS_RASTER_TMA=0/1: record staging by per-thread cp.async (16 B x 3) or by cp.async.bulk + mbarrier (48 B x 1)
-  static int tma = -1;
-  if (tma < 0) { const char *e = getenv("GS_RASTER_TMA"); tma = e ? (e[0] == '1') : kRasterTmaDefault; }
   const uint32_t bins = fc.binsX * fc.binsY;
   uint2 *ranges = reinterpret_cast<uint2 *>(bs.bin_ranges);
   const uint32_t packed = part.range ? 0u : opt.band_packed, load = (opt.flags & GS_FLAG_LOAD_RT) ? 1u : 0u;
   k_bin_ranges<<<(bins + 7) / 8, 256, 0, s>>>(bs.tile_keys, bs.entry_count, bins, ranges);
 #define GS_LAUNCH_RASTER(ROP, FMT)                                                                                              \
   do {                                                                                                                         \
-    if (fc.selValid || scene_depth) k_raster<ROP, FMT, false, false, true><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, packed, load, stats, zndc, scene_depth); \
-    else if (tma) k_raster<ROP, FMT, false, true><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, packed, load, stats, nullptr, nullptr); \
-    else if (stats) k_raster<ROP, FMT, true, false><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, packed, load, stats, nullptr, nullptr); \
-    else k_raster<ROP, FMT, false, false><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, packed, load, stats, nullptr, nullptr); \
+    if (fc.selValid || scene_depth) k_raster<ROP, FMT, false, true><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, packed, load, stats, zndc, scene_depth); \
+    else if (stats) k_raster<ROP, FMT, true><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, packed, load, stats, nullptr, nullptr); \
+    else k_raster<ROP, FMT, false><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, packed, load, stats, nullptr, nullptr); \
   } while (0)
   if (rt_format == GS_PIX_RGBA16F) {
     if (rop) GS_LAUNCH_RASTER(true, GS_PIX_RGBA16F); else GS_LAUNCH_RASTER(false, GS_PIX_RGBA16F);

@@ -21,7 +21,6 @@
 // The digit width is a template parameter: depth keys use 4 x 8 bits, the tile binner sorts
 // 12..16-bit tile ids in 2 passes of 6..8 bits.
 // No tensor-core path: there is no contraction here, only byte/integer traffic.
-#include <cstdio>
 #include <cstdlib>
 
 #include "gs_kernels.cuh"
@@ -29,6 +28,7 @@
 namespace gs {
 
 enum : uint32_t { kFlagLocal = 1u << 30, kFlagIncl = 2u << 30, kValMask = (1u << 30) - 1u };
+constexpr int kSortKpt = 16;   // keys per thread
 
 size_t sort_lookback_words(uint32_t capacity, int passes) {
   size_t tiles = ((size_t)capacity + kSortTileItems - 1) / kSortTileItems;
@@ -106,22 +106,18 @@ __device__ __forceinline__ uint32_t match_digit(uint32_t d) {
 }
 
 // ---- one digit pass -------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t gtime() { uint64_t t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-#define GS_TRACE(slot) do { if (trace && tid == 0) trace[(size_t)tile * 8 + (slot)] = gtime(); } while (0)
-
 // GATHER: the keys of this pass are keys_src[payload] (pass 0 of the depth sort reads the per-splat key
 // table through last frame's order, S/SplatUtilities.compute:76-81, without a separate gather pass).
 // PERSIST: a fixed grid whose CTAs keep taking tiles until the (device-side) count is exhausted -- for lists whose length
 // the host does not know when it launches (the binner's entry list): no capacity-sized grid of idle CTAs.
-// KPT: keys per thread (a tile is THREADS * KPT pairs): 16 for big sorts; 8 when the whole sort is about one wave of tiles, where a
-// pass costs one tile latency and half-size tiles have a shorter one.
-template <int BITS, bool GATHER, int THREADS, bool PERSIST, int KPT>
+// THREADS: 256, or 512 with GS_SORT_THREADS=512.  A tile is THREADS * kSortKpt pairs.
+template <int BITS, bool GATHER, int THREADS, bool PERSIST>
 __global__ void __launch_bounds__(THREADS, 1024 / THREADS)
 k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_v, uint32_t *__restrict__ dst_k,
            uint32_t *__restrict__ dst_v, const uint32_t *__restrict__ d_count, int shift, const uint32_t *__restrict__ ghist,
-           volatile uint32_t *lookback, uint32_t *ticket, uint64_t *trace) {
+           volatile uint32_t *lookback, uint32_t *ticket) {
   constexpr uint32_t NB = 1u << BITS;
-  constexpr uint32_t kTileItems = THREADS * KPT;
+  constexpr uint32_t kTileItems = THREADS * kSortKpt;
   constexpr int kSortWarps = THREADS / 32;
   constexpr int kSortThreads = THREADS;
   extern __shared__ __align__(16) uint8_t s_dyn[];
@@ -146,26 +142,25 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
   const uint32_t tile = s_tile;
   if (tile >= num_tiles) return;
   const uint32_t tile_base = tile * kTileItems;
-  GS_TRACE(0);
   const bool full_tile = tile_base + kTileItems <= n;
 
   // warp-striped load: warp w owns 512 consecutive pairs, item i of lane l is base + i*32 + l
-  uint32_t key[KPT], val[KPT];
-  const uint32_t wbase = tile_base + warp * (32 * KPT) + lane;
+  uint32_t key[kSortKpt], val[kSortKpt];
+  const uint32_t wbase = tile_base + warp * (32 * kSortKpt) + lane;
   if (GATHER) {
 #pragma unroll
-    for (int i = 0; i < KPT; ++i) {
+    for (int i = 0; i < kSortKpt; ++i) {
       const uint32_t idx = wbase + i * 32;
       val[i] = (idx < n) ? __ldg(src_v + idx) : 0xFFFFFFFFu;
     }
 #pragma unroll
-    for (int i = 0; i < KPT; ++i) key[i] = (val[i] != 0xFFFFFFFFu) ? __ldg(src_k + val[i]) : 0xFFFFFFFFu;
+    for (int i = 0; i < kSortKpt; ++i) key[i] = (val[i] != 0xFFFFFFFFu) ? __ldg(src_k + val[i]) : 0xFFFFFFFFu;
   } else if (full_tile) {
 #pragma unroll
-    for (int i = 0; i < KPT; ++i) key[i] = __ldg(src_k + wbase + i * 32);
+    for (int i = 0; i < kSortKpt; ++i) key[i] = __ldg(src_k + wbase + i * 32);
   } else {
 #pragma unroll
-    for (int i = 0; i < KPT; ++i) {
+    for (int i = 0; i < kSortKpt; ++i) {
       const uint32_t idx = wbase + i * 32;
       key[i] = (idx < n) ? __ldg(src_k + idx) : 0xFFFFFFFFu;  // pads sort last (S/SortCommon.hlsl:244-247 does the same)
     }
@@ -173,7 +168,7 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
 
   // 1. tile digit histogram (cheap, before ranking) so that the LOCAL count is published as early as possible
 #pragma unroll
-  for (int i = 0; i < KPT; ++i) {
+  for (int i = 0; i < kSortKpt; ++i) {
     const uint32_t d = (key[i] >> shift) & (NB - 1);
     const uint32_t d0 = __shfl_sync(0xffffffffu, d, 0);
     if (__all_sync(0xffffffffu, d == d0)) {   // skewed digits (high bytes of depth keys): one add per warp
@@ -183,7 +178,6 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
     }
   }
   __syncthreads();
-  GS_TRACE(1);
 
   // 2. publish, then resolve the exclusive prefix over earlier tiles with 4 status probes in flight
   uint32_t prefix = 0, tile_total = 0;
@@ -220,14 +214,13 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
     }
   }
   __syncwarp();   // the spin loop above ends per thread: tell the compiler the warp is whole again before the ballots
-  GS_TRACE(2);
   if (!GATHER) {  // payloads: issued now, consumed at the scatter
     if (full_tile) {
 #pragma unroll
-      for (int i = 0; i < KPT; ++i) val[i] = __ldg(src_v + wbase + i * 32);
+      for (int i = 0; i < kSortKpt; ++i) val[i] = __ldg(src_v + wbase + i * 32);
     } else {
 #pragma unroll
-      for (int i = 0; i < KPT; ++i) {
+      for (int i = 0; i < kSortKpt; ++i) {
         const uint32_t idx = wbase + i * 32;
         val[i] = (idx < n) ? __ldg(src_v + idx) : 0u;
       }
@@ -235,10 +228,10 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
   }
 
   // 3. stable in-warp ranking; ranks (< 4096) are packed two per register
-  uint32_t rank2[KPT / 2];
+  uint32_t rank2[kSortKpt / 2];
   const uint32_t lt_mask = (1u << lane) - 1u;
 #pragma unroll
-  for (int i = 0; i < KPT; ++i) {
+  for (int i = 0; i < kSortKpt; ++i) {
     const uint32_t d = (key[i] >> shift) & (NB - 1);
     const uint32_t m = match_digit<BITS>(d);
     // every lane reads its digit's running count (lanes of one digit read one word: a broadcast), then the lowest lane of
@@ -254,7 +247,6 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
     __syncwarp();
   }
   __syncthreads();
-  GS_TRACE(3);
 
   // 4. thread `tid` < NB owns digit `tid`: exclusive prefix over warps, tile/global digit bases
   if (tid < NB) {
@@ -273,18 +265,16 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
     s_off[tid] = gbase + prefix - dig_start;
   }
   __syncthreads();
-  GS_TRACE(4);
 
   // 5. scatter into digit order inside shared memory
 #pragma unroll
-  for (int i = 0; i < KPT; ++i) {
+  for (int i = 0; i < kSortKpt; ++i) {
     const uint32_t d = (key[i] >> shift) & (NB - 1);
     const uint32_t r = (i & 1) ? (rank2[i >> 1] >> 16) : (rank2[i >> 1] & 0xffffu);
     const uint32_t pos = s_dig_start[d] + s_whist[warp][d] + r;
     s_kv[pos] = make_uint2(key[i], val[i]);
   }
   __syncthreads();
-  GS_TRACE(5);
 
   const uint32_t valid = full_tile ? kTileItems : n - tile_base;
 #pragma unroll 4
@@ -294,7 +284,6 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
     dst_k[dst] = kv.x;
     dst_v[dst] = kv.y;
   }
-  GS_TRACE(6);
   } while (PERSIST);
 }
 
@@ -422,10 +411,6 @@ uint32_t sm_count() {
   return cached[dev];
 }
 
-// optional per-tile phase trace of the first pass (debug/profiling aid): GS_SORT_TRACE=<file>
-static uint64_t *g_trace = nullptr;
-static uint32_t g_trace_tiles = 0;
-
 static int sort_threads() {
   static int v = 0;
   if (!v) { const char *e = getenv("GS_SORT_THREADS"); v = (e && atoi(e) == 512) ? 512 : 256; }
@@ -433,11 +418,11 @@ static int sort_threads() {
 }
 
 template <int BITS>
-static void launch_pass(uint32_t count_bound, bool persist, bool small_tiles, cudaStream_t s, const uint32_t *sk, const uint32_t *sv, uint32_t *dk,
+static void launch_pass(uint32_t count_bound, bool persist, cudaStream_t s, const uint32_t *sk, const uint32_t *sv, uint32_t *dk,
                         uint32_t *dv, const uint32_t *d_count, int shift, const uint32_t *ghist, uint32_t *lookback, uint32_t *ticket,
-                        uint64_t *trace, bool gather) {
-  auto go = [&](auto kern, int threads, int kpt) {
-    const size_t smem = (size_t)threads * kpt * 8 + (size_t)(threads / 32) * (1u << BITS) * 4;
+                        bool gather) {
+  auto go = [&](auto kern, int threads) {
+    const size_t smem = (size_t)threads * kSortKpt * 8 + (size_t)(threads / 32) * (1u << BITS) * 4;
     // the opt-in for > 48 KB dynamic shared memory is per function AND per device
     struct Seen { const void *fn; int dev; };
     static thread_local Seen configured[64];
@@ -450,19 +435,17 @@ static void launch_pass(uint32_t count_bound, bool persist, bool small_tiles, cu
       cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (nconf < 64) configured[nconf++] = Seen{(const void *)kern, dev};
     }
-    const uint32_t per = (uint32_t)threads * kpt;
+    const uint32_t per = (uint32_t)threads * kSortKpt;
     uint32_t grid = (uint32_t)(((uint64_t)count_bound + per - 1) / per);
     if (persist) grid = min(grid, sm_count() * (1024u / (uint32_t)threads));
-    kern<<<grid, threads, smem, s>>>(sk, sv, dk, dv, d_count, shift, ghist, lookback, ticket, trace);
+    kern<<<grid, threads, smem, s>>>(sk, sv, dk, dv, d_count, shift, ghist, lookback, ticket);
   };
   if (persist) {
-    if (gather) go(k_onesweep<BITS, true, 256, true, 16>, 256, 16); else go(k_onesweep<BITS, false, 256, true, 16>, 256, 16);
-  } else if (small_tiles) {
-    if (gather) go(k_onesweep<BITS, true, 256, false, 8>, 256, 8); else go(k_onesweep<BITS, false, 256, false, 8>, 256, 8);
+    if (gather) go(k_onesweep<BITS, true, 256, true>, 256); else go(k_onesweep<BITS, false, 256, true>, 256);
   } else if (sort_threads() == 512) {
-    if (gather) go(k_onesweep<BITS, true, 512, false, 16>, 512, 16); else go(k_onesweep<BITS, false, 512, false, 16>, 512, 16);
+    if (gather) go(k_onesweep<BITS, true, 512, false>, 512); else go(k_onesweep<BITS, false, 512, false>, 512);
   } else {
-    if (gather) go(k_onesweep<BITS, true, 256, false, 16>, 256, 16); else go(k_onesweep<BITS, false, 256, false, 16>, 256, 16);
+    if (gather) go(k_onesweep<BITS, true, 256, false>, 256); else go(k_onesweep<BITS, false, 256, false>, 256);
   }
 }
 
@@ -476,16 +459,8 @@ void launch_sort_pairs(uint32_t *keys, uint32_t *vals, const uint32_t *d_count, 
   // length lives on the device only (the binner's entries): a persistent grid, and the look-back rows actually needed are
   // cleared by a kernel that reads the count.
   const bool persist = !count_is_capacity;
-  // Half-size tiles for exact, smallish counts (a slab of a group's sort) were tried -- twice the CTAs, shorter tiles -- and
-  // measured SLOWER: a pass is bound by its fixed per-tile work, not by
-  // the tile count.  Kept behind GS_SORT_SMALL_TILES=1 for experiments.
-  static int small_env = -1;
-  if (small_env < 0) { const char *e = getenv("GS_SORT_SMALL_TILES"); small_env = (e && e[0] == '1') ? 1 : 0; }
-  const bool small_tiles = small_env && !persist && capacity <= 4u * 1024u * 1024u && sort_threads() != 512 &&
-                           (size_t)tiles * 2 * nb * passes <= sc.lookback_words;
-  const uint32_t rows = small_tiles ? (capacity + kSortTileItems / 2 - 1) / (kSortTileItems / 2) : tiles;
   if (persist) k_zero_rows<<<sm_count(), 256, 0, s>>>(sc.lookback, d_count, kSortTileItems, nb, nb, (uint32_t)passes, tiles * nb);
-  else cudaMemsetAsync(sc.lookback, 0, (size_t)rows * nb * passes * sizeof(uint32_t), s);
+  else cudaMemsetAsync(sc.lookback, 0, (size_t)tiles * nb * passes * sizeof(uint32_t), s);
   cudaMemsetAsync(sc.tickets, 0, 4 * sizeof(uint32_t), s);
   if (!hist_ready) {
     cudaMemsetAsync(sc.ghist, 0, 4 * 256 * sizeof(uint32_t), s);
@@ -497,36 +472,20 @@ void launch_sort_pairs(uint32_t *keys, uint32_t *vals, const uint32_t *d_count, 
     else k_sort_hist<2, 8><<<grid, 256, 0, s>>>(keys, d_count, sc.ghist);
   }
   uint32_t *sk = keys, *sv = vals, *dk = sc.alt_keys, *dv = sc.alt_vals;
-  const char *trace_path = getenv("GS_SORT_TRACE");
-  if (trace_path && passes == 4 && g_trace_tiles < tiles) {
-    cudaFree(g_trace);
-    cudaMalloc(&g_trace, (size_t)tiles * 8 * sizeof(uint64_t));
-    g_trace_tiles = tiles;
-  }
   for (int p = 0; p < passes; ++p) {
-    uint64_t *trace = (trace_path && passes == 4 && p == 1 && !small_tiles) ? g_trace : nullptr;
-    if (trace) cudaMemsetAsync(trace, 0, (size_t)tiles * 8 * sizeof(uint64_t), s);
     if (pass_events) cudaEventRecord(pass_events[p], s);
-    uint32_t *lb = sc.lookback + (size_t)p * rows * nb;
+    uint32_t *lb = sc.lookback + (size_t)p * tiles * nb;
     const bool gather = key_table != nullptr && p == 0;   // pass 0 reads key_table[vals[i]] instead of keys[i]
     const uint32_t *src_keys = gather ? key_table : sk;
     if (p == passes - 1 && final_keys && final_vals) { dk = final_keys; dv = final_vals; }   // the last pass lands where the caller wants it
-    if (bits == 5) launch_pass<5>(capacity, persist, small_tiles, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, trace, gather);
-    else if (bits == 6) launch_pass<6>(capacity, persist, small_tiles, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, trace, gather);
-    else if (bits == 7) launch_pass<7>(capacity, persist, small_tiles, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, trace, gather);
-    else launch_pass<8>(capacity, persist, small_tiles, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, trace, gather);
+    if (bits == 5) launch_pass<5>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
+    else if (bits == 6) launch_pass<6>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
+    else if (bits == 7) launch_pass<7>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
+    else launch_pass<8>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
     uint32_t *t = sk; sk = dk; dk = t;
     t = sv; sv = dv; dv = t;
   }
   if (pass_events) cudaEventRecord(pass_events[passes], s);
-  if (trace_path && passes == 4) {
-    cudaStreamSynchronize(s);
-    uint64_t *h = (uint64_t *)malloc((size_t)tiles * 64);
-    cudaMemcpy(h, g_trace, (size_t)tiles * 64, cudaMemcpyDeviceToHost);
-    FILE *f = fopen(trace_path, "wb");
-    if (f) { fwrite(h, 64, tiles, f); fclose(f); }
-    free(h);
-  }
 }
 
 }  // namespace gs
