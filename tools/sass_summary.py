@@ -13,9 +13,10 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parents[1]
 LIB = ROOT / "unitygaussiansplatting_b200" / "libgsplat_b200.so"
-WANT = [("k_onesweep<8, gather, 256, one-shot> (depth sort pass 0)", r"k_onesweepILi8ELb1ELi256ELb0E"),
-        ("k_onesweep<8, no gather, 256, one-shot> (depth sort passes 1-3, slab sorts)", r"k_onesweepILi8ELb0ELi256ELb0E"),
-        ("k_onesweep<8, no gather, 256, persistent> (the bin sort)", r"k_onesweepILi8ELb0ELi256ELb1E"),
+WANT = [("k_onesweep<8, gather, one-shot> (depth sort pass 0)", r"k_onesweepILi8ELb1ELb0E"),
+        ("k_onesweep<8, no gather, one-shot> (depth sort passes 1-3, slab sorts)", r"k_onesweepILi8ELb0ELb0E"),
+        ("k_onesweep<9, no gather, persistent> (the bin sort at 257-512 bins)", r"k_onesweepILi9ELb0ELb1E"),
+        ("k_onesweep<8, no gather, persistent> (the bin sort at 129-256 bins)", r"k_onesweepILi8ELb0ELb1E"),
         ("k_raster<fp16 ROP, RGBA16F, no stats, no extras> (default)", r"k_rasterILb1ELi0ELb0ELb0E"),
         ("k_raster<fp16 ROP, RGBA16F, no stats, EXTRAS> (selected splats / scene depth test)", r"k_rasterILb1ELi0ELb0ELb1E"),
         ("k_calc_view<3, true, false> (Norm6 SH, fused cull: the Medium frame)", r"k_calc_viewILi3ELb1ELb0E"),

@@ -258,8 +258,8 @@ static int do_sort(GsContext *ctx, GsAsset *as, const FrameConsts &fc) {
   launch_calc_distances(as->av, fc, as->key_table, ctx->sort.ghist, ctx->stream);
   rec(ctx, EV_DIST);
   cudaEvent_t pe[5] = {ctx->ev[EV_SORT0], ctx->ev[EV_SORT1], ctx->ev[EV_SORT2], ctx->ev[EV_SORT3], ctx->ev[EV_SORT4]};
-  launch_sort_pairs(as->keys, as->order, as->d_n, as->av.n, 4, 8, true, ctx->sort, ctx->stream, ctx->timing ? pe : nullptr,
-                    as->key_table);
+  GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order, as->d_n, as->av.n, 4, 8, true, ctx->sort, ctx->stream, ctx->timing ? pe : nullptr,
+                                     as->key_table));
   if (ctx->timing) for (int e = EV_SORT0; e <= EV_SORT4; ++e) ctx->ev_valid[e] = true;
   ctx->launches += 1 + 4;
   GS_CUDA_TRY(ctx, cudaGetLastError());
@@ -322,7 +322,9 @@ int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRender
     }
   }
   int bin_launches = 0;
-  const BinScratch lists = launch_binning(fc, opt, as->av.n, as->order, as->rect, as->block_bits, ctx->bin, ctx->sort, ctx->stream, &bin_launches);
+  BinScratch lists;
+  GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->av.n, as->order, as->rect, as->block_bits, ctx->bin, ctx->sort, ctx->stream, &lists,
+                                  &bin_launches));
   rec(ctx, EV_BIN1);
   launch_raster(fc, opt, as->draw, lists, d_rt, pitch, fmt, ctx->stream, ctx->cur_depth ? as->zndc : nullptr, ctx->cur_depth);
   rec(ctx, EV_RASTER1);
@@ -754,7 +756,7 @@ int gs_sort_pairs_device(GsContext *ctx, uint32_t *d_keys, uint32_t *d_payload, 
   for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
   cudaEvent_t pe[5] = {ctx->ev[EV_SORT0], ctx->ev[EV_SORT1], ctx->ev[EV_SORT2], ctx->ev[EV_SORT3], ctx->ev[EV_SORT4]};
   rec(ctx, EV_BEGIN);
-  launch_sort_pairs(d_keys, d_payload, ctx->d_scalar, count, 4, 8, false, ctx->sort, ctx->stream, ctx->timing ? pe : nullptr);
+  GS_CUDA_TRY(ctx, launch_sort_pairs(d_keys, d_payload, ctx->d_scalar, count, 4, 8, false, ctx->sort, ctx->stream, ctx->timing ? pe : nullptr));
   if (ctx->timing) for (int e = EV_SORT0; e <= EV_SORT4; ++e) ctx->ev_valid[e] = true;
   ctx->launches += 5;
   GS_CUDA_TRY(ctx, cudaGetLastError());

@@ -645,13 +645,14 @@ int gs_group_frame(GsGroup *g, GsAsset *const *assets, const GsFrameParams *fp, 
       GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
       const uint32_t cnt = g->slab_cnt[mb.rank], off = g->slab_off[mb.rank];
       if (G == 1) {
-        launch_sort_pairs(as->keys, as->order, as->d_n, N, 4, 8, true, ctx->sort, ctx->stream, nullptr, as->key_table);
+        GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order, as->d_n, N, 4, 8, true, ctx->sort, ctx->stream, nullptr, as->key_table));
         ctx->launches += 4;
       } else if (cnt) {
         launch_compact_order(as->order, N, as->slab_mask, as->slab_group_bits, as->key_table, as->order_tmp, as->keys, mb.d_cmp_status, mb.d_slab_count,
                              ctx->stream);
-        launch_sort_pairs(as->keys, as->order_tmp, mb.d_slab_count, cnt, 4, 8, true, ctx->sort, ctx->stream, nullptr, nullptr, true,
-                          as->keys + off, use_p2p ? p2p_new + off : use_gather ? mb.d_gather + (size_t)mb.rank * cap : as->order + off);
+        GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order_tmp, mb.d_slab_count, cnt, 4, 8, true, ctx->sort, ctx->stream, nullptr, nullptr,
+                                           true, as->keys + off,
+                                           use_p2p ? p2p_new + off : use_gather ? mb.d_gather + (size_t)mb.rank * cap : as->order + off));
         ctx->launches += 5;
       }
       if (use_p2p) {

@@ -140,21 +140,23 @@ void launch_calc_view(const AssetView &a, const FrameConsts &fc, const GsCutout 
 // Radix sort (gs_sort.cu).  Scratch layout is owned by the caller (gs_api.cu).
 struct SortScratch {
   uint32_t *alt_keys, *alt_vals;  // ping-pong buffers, >= capacity elements each
-  uint32_t *ghist;                // 4*256 digit counts (one row per pass)
-  uint32_t *lookback;             // passes * max_tiles * 256 status words
+  uint32_t *ghist;                // 4*256 digit counts (one row of 256 per pass; a single 9-bit pass uses the first 512)
+  uint32_t *lookback;             // max_tiles * 1024 status words: per tile, 4 passes x 256 digits or 1 pass x 512
   uint32_t *tickets;              // passes counters
   uint32_t max_tiles;             // capacity / kSortTileItems rounded up
   size_t lookback_words;          // size of `lookback`
 };
-constexpr uint32_t kSortTileItems = 4096;  // 256 threads x 16 keys
+constexpr uint32_t kSortTileItems = 8192;  // 512 threads x 16 keys
 size_t sort_lookback_words(uint32_t capacity, int passes);
-// Stable ascending LSD sort of (key,val) pairs on bits [0, bits*passes), bits in {5..8}.  The count is read from d_count
-// (device).  count_is_capacity: the host passes the exact count as `capacity` (exact grid); otherwise `capacity` only bounds
-// the buffers and a persistent grid serves whatever d_count holds.
-// ghist must already hold the per-pass digit counts when hist_ready, otherwise it is computed.
+// Stable ascending LSD sort of (key,val) pairs on bits [0, bits*passes), bits in {5..8}, or one pass of 9 bits.  The count
+// is read from d_count (device).  count_is_capacity: the host passes the exact count as `capacity` (exact grid); otherwise
+// `capacity` only bounds the buffers and a persistent grid serves whatever d_count holds.
+// ghist must already hold the per-pass digit counts when hist_ready, otherwise it is computed (4 x 8 or 1..2 x 5..8 bits
+// only: a 9-bit pass needs hist_ready).  Each pass of a tile publishes 2^bits status words; `lookback` must hold
+// passes * 2^bits words per 8192-pair tile.  An unsupported request launches nothing and returns cudaErrorInvalidValue.
 // After an even number of passes the result is back in keys/vals -- unless final_keys/final_vals name where the last pass
 // writes.  key_table != nullptr: the input keys are key_table[vals[i]] (gathered inside pass 0; `keys` is then output only).
-void launch_sort_pairs(uint32_t *keys, uint32_t *vals, const uint32_t *d_count, uint32_t capacity, int passes, int bits, bool hist_ready,
+cudaError_t launch_sort_pairs(uint32_t *keys, uint32_t *vals, const uint32_t *d_count, uint32_t capacity, int passes, int bits, bool hist_ready,
                        const SortScratch &sc, cudaStream_t s, cudaEvent_t *pass_events = nullptr, const uint32_t *key_table = nullptr,
                        bool count_is_capacity = true, uint32_t *final_keys = nullptr, uint32_t *final_vals = nullptr);
 // (out_ids, out_keys) = (id, key_table[id]) of the ids of order[0..n) whose mask bit is set, order kept; *count_out = how many.
@@ -173,9 +175,10 @@ struct BinScratch {
   uint32_t *tile_cost, *tile_order;   // per raster tile: last frame's cost, this frame's launch order
   uint32_t capacity;
 };
-// returns the scratch view whose tile_keys / tile_vals hold the bin-sorted lists (launch_raster's input)
-BinScratch launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, uint32_t n, const uint32_t *order, const uint32_t *rect,
-                          const uint32_t *block_bits, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, int *launches);
+// *sorted: the scratch view whose tile_keys / tile_vals hold the bin-sorted lists (launch_raster's input)
+cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, uint32_t n, const uint32_t *order, const uint32_t *rect,
+                           const uint32_t *block_bits, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted,
+                           int *launches);
 // zndc / scene_depth: per-splat quad depth and the W x H depth buffer to test it against (both nullptr: no depth test)
 void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const BinScratch &bs, void *rt,
                    uint32_t rt_pitch_bytes, uint32_t rt_format, cudaStream_t s, const float *zndc = nullptr, const float *scene_depth = nullptr);

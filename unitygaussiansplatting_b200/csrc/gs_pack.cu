@@ -951,9 +951,9 @@ int gs_pack_asset(GsContext *ctx, const GsPackDesc *desc, GsPackedAsset *blobs_o
   int rc = ensure_sort_scratch(ctx, n);
   if (rc) return rc;
   GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_scalar, &n, 4, cudaMemcpyHostToDevice, st));
-  launch_sort_pairs(lo, idx, ctx->d_scalar, n, 4, 8, false, ctx->sort, st);
+  GS_CUDA_TRY(ctx, launch_sort_pairs(lo, idx, ctx->d_scalar, n, 4, 8, false, ctx->sort, st));
   k_gather_u32<<<blocks_for(n, 256), 256, 0, st>>>(hi, idx, n, lo);
-  launch_sort_pairs(lo, idx, ctx->d_scalar, n, 4, 8, false, ctx->sort, st);
+  GS_CUDA_TRY(ctx, launch_sort_pairs(lo, idx, ctx->d_scalar, n, 4, 8, false, ctx->sort, st));
   ctx->launches += 5 + 2 * 5;
   GS_CUDA_TRY(ctx, cudaGetLastError());
   float *recs;

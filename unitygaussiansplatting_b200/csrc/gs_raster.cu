@@ -8,9 +8,10 @@
 //               64x64-pixel bin its visible footprint can touch (rect written by k_calc_view).
 //               Bins are coarser than the 16x16 raster tiles on purpose: 2.5x fewer entries to
 //               emit and sort, and the per-warp ballot cull below makes a foreign entry cost 1/32
-//               of an evaluation.  Emission order == depth order, so one STABLE 16-bit radix sort
-//               by tile id (2 onesweep passes) yields per-tile lists that are already in
-//               draw order.  No 64-bit (tile|depth) re-sort of duplicated keys.
+//               of an evaluation.  Emission order == depth order, so one STABLE radix sort by
+//               bin id (one onesweep pass up to 512 bins, e.g. 1920x1080 = 510 bins, else 2
+//               passes) yields per-bin lists that are already in draw order.  No 64-bit
+//               (tile|depth) re-sort of duplicated keys.
 //   2. raster-- one CTA per tile, one pixel per thread.  The tile's list is consumed in
 //               batches of 256 raster-ready records (written by k_calc_view) that land in shared
 //               memory by cp.async, double buffered; every warp owns an 8x4 pixel block and
@@ -52,7 +53,8 @@ __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ o
   extern __shared__ uint32_t s_bits[];   // the view kernel's block bitmap (bits_words words), or nothing when it is too large to hold
   __shared__ uint32_t s_w[8];
   __shared__ uint32_t s_block, s_excl;
-  __shared__ uint32_t s_dh[512];   // digit histograms of the two sort passes over the tile ids we emit
+  __shared__ uint32_t s_dh[512];   // digit histograms of the sort by the bin ids we emit: [0,256) pass 0 and [256,512) pass 1
+                                   // of two passes, or all 512 for one pass of up to 9 bits (ghist's layout)
   __shared__ uint2 s_items[kBinBlock];     // per warp: its drawable ranks, squeezed together in order
   __shared__ uint32_t s_pre[kBinBlock];
   const uint32_t nblocks = (n + kBinBlock - 1) / kBinBlock;
@@ -186,20 +188,22 @@ __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ o
   }
 }
 
-// digit width and pass count of the stable sort by bin id: one pass while the bin count fits a digit (<= 256 bins, e.g.
-// 1200x797 = 19x13), else two passes of the narrowest digit that covers it
+// digit width and pass count of the stable sort by bin id: one pass while the bin count fits a digit (<= 512 bins, e.g.
+// 1200x797 = 19x13 in 8 bits, 1920x1080 = 30x17 in 9), else two passes of the narrowest digit that covers it
 static void bin_sort_plan(uint32_t bins, int *bits, int *passes) {
-  if (bins <= 256u) { *passes = 1; *bits = bins <= 32u ? 5 : bins <= 64u ? 6 : bins <= 128u ? 7 : 8; return; }
+  if (bins <= 512u) { *passes = 1; *bits = bins <= 32u ? 5 : bins <= 64u ? 6 : bins <= 128u ? 7 : bins <= 256u ? 8 : 9; return; }
   *passes = 2;
   *bits = bins <= 1024u ? 5 : bins <= 4096u ? 6 : bins <= 16384u ? 7 : 8;
 }
 
-BinScratch launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, uint32_t n, const uint32_t *order, const uint32_t *rect,
-                          const uint32_t *block_bits, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, int *launches) {
+cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, uint32_t n, const uint32_t *order, const uint32_t *rect,
+                           const uint32_t *block_bits, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted,
+                           int *launches) {
   const Partition part = make_partition(opt);
   const uint32_t tiles = fc.binsX * fc.binsY;
+  *sorted = bs;
   if (launches) *launches = 0;
-  if (!n) { cudaMemsetAsync(bs.entry_count, 0, 16, s); return bs; }
+  if (!n) return cudaMemsetAsync(bs.entry_count, 0, 16, s);
   const uint32_t nblocks = (n + kBinBlock - 1) / kBinBlock;
   cudaMemsetAsync(bs.block_sums, 0, ((size_t)nblocks + 1) * sizeof(uint32_t), s);   // [0] ticket, [1..] look-back status
   int bits, passes;
@@ -215,11 +219,12 @@ BinScratch launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, uin
   k_bin_emit<<<nblocks, 256, words * 4u, s>>>(order, rect, block_bits, words, n, part, fc.binsX, bs.block_sums + 1, bs.block_sums, bs.capacity,
                                      bs.tile_keys, bs.tile_vals, bs.entry_count, sc.ghist, (uint32_t)bits, passes == 2);
   // the entry count lives on the device: a persistent grid sorts whatever it is (no capacity-sized grid or memset)
-  launch_sort_pairs(bs.tile_keys, bs.tile_vals, bs.entry_count, bs.capacity, passes, bits, true, sc, s, nullptr, nullptr,
-                    /*count_is_capacity=*/false);
-  BinScratch sorted = bs;   // an odd number of passes leaves the sorted lists in the sorter's ping-pong buffers
-  if (passes & 1) { sorted.tile_keys = sc.alt_keys; sorted.tile_vals = sc.alt_vals; }
-  return sorted;
+  const cudaError_t e = launch_sort_pairs(bs.tile_keys, bs.tile_vals, bs.entry_count, bs.capacity, passes, bits, true, sc, s, nullptr,
+                                          nullptr, /*count_is_capacity=*/false);
+  if (e != cudaSuccess) return e;
+  // an odd number of passes leaves the sorted lists in the sorter's ping-pong buffers
+  if (passes & 1) { sorted->tile_keys = sc.alt_keys; sorted->tile_vals = sc.alt_vals; }
+  return cudaSuccess;
 }
 
 // ---- 2. raster ---------------------------------------------------------------------------------

@@ -8,8 +8,8 @@
 // reduce-then-scan's two reads per pass:
 //   * digit histograms for all passes come from one read of the keys (or for free from
 //     k_calc_distances, which wrote the keys in the first place);
-//   * each CTA takes a 4096-pair tile by atomic ticket (so a tile's predecessors are
-//     always resident: look-back cannot deadlock), ranks its keys with warp-level digit
+//   * each CTA (512 threads x 16 keys) takes an 8192-pair tile by atomic ticket (so a tile's
+//     predecessors are always resident: look-back cannot deadlock), ranks its keys with warp-level digit
 //     matching (the match mask of equal digits gives the stable rank as a popc of the lower
 //     lanes; one lane bumps the warp-private shared histogram), publishes the tile's
 //     per-digit count with a LOCAL flag, walks back over predecessors' status words until
@@ -17,9 +17,9 @@
 //   * keys and payloads are first scattered inside shared memory into digit order, then
 //     written out in runs, so global stores are coalesced per digit run;
 //   * payloads are fetched only after ranking (their latency hides behind the look-back),
-//     which keeps the kernel at <= 64 registers and 4 CTAs/SM.
-// The digit width is a template parameter: depth keys use 4 x 8 bits, the tile binner sorts
-// 12..16-bit tile ids in 2 passes of 6..8 bits.
+//     which keeps the kernel at <= 64 registers and 2 CTAs/SM.
+// The digit width is a template parameter: depth keys use 4 x 8 bits; the binner sorts bin ids
+// in one pass of 5..9 bits up to 512 bins, else in 2 passes of 5..8 bits.
 // No tensor-core path: there is no contraction here, only byte/integer traffic.
 #include <cstdlib>
 
@@ -28,8 +28,14 @@
 namespace gs {
 
 enum : uint32_t { kFlagLocal = 1u << 30, kFlagIncl = 2u << 30, kValMask = (1u << 30) - 1u };
-constexpr int kSortKpt = 16;   // keys per thread
+constexpr int kSortKpt = 16;                       // keys per thread
+constexpr int kSortThreads = kSortTileItems / kSortKpt;   // 512: thread `tid` owns digit `tid`, so digits are at most 9 bits
+constexpr int kSortWarps = kSortThreads / 32;
 
+// Look-back status words for `passes` passes of 8 bits: a pass of 2^bits digits keeps one row of 2^bits words per tile.  The
+// context allocates for 4 passes (1024 words per 8192-pair tile).  A single 9-bit pass (the bin sort up to 512 bins) needs
+// 512 of them -- per pair, as many as one 8-bit pass needed over 4096-pair tiles -- and two passes of up to 8 bits at most
+// 512, so every plan fits the allocation; launch_sort_pairs checks it.
 size_t sort_lookback_words(uint32_t capacity, int passes) {
   size_t tiles = ((size_t)capacity + kSortTileItems - 1) / kSortTileItems;
   return tiles * 256 * (size_t)passes;
@@ -68,7 +74,7 @@ __global__ void __launch_bounds__(256) k_sort_hist(const uint32_t *__restrict__ 
   }
 }
 
-// ---- block-wide exclusive scan of one value per thread (256 threads) ------------------------
+// ---- block-wide exclusive scan of one value per thread (WARPS <= 32 warps) ------------------
 template <int WARPS>
 __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *s_warp /*WARPS*/) {
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -110,16 +116,16 @@ __device__ __forceinline__ uint32_t match_digit(uint32_t d) {
 // table through last frame's order, S/SplatUtilities.compute:76-81, without a separate gather pass).
 // PERSIST: a fixed grid whose CTAs keep taking tiles until the (device-side) count is exhausted -- for lists whose length
 // the host does not know when it launches (the binner's entry list): no capacity-sized grid of idle CTAs.
-// THREADS: 256, or 512 with GS_SORT_THREADS=512.  A tile is THREADS * kSortKpt pairs.
-template <int BITS, bool GATHER, int THREADS, bool PERSIST>
-__global__ void __launch_bounds__(THREADS, 1024 / THREADS)
+// Shared memory per CTA at BITS = 9: 64 KB of pairs + 16 warps x 512 x 4 B = 32 KB of warp histograms (dynamic) + 6 KB of
+// static digit arrays = 102 KB, so two CTAs fit an SM's 228 KB.
+template <int BITS, bool GATHER, bool PERSIST>
+__global__ void __launch_bounds__(kSortThreads, 2)
 k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_v, uint32_t *__restrict__ dst_k,
            uint32_t *__restrict__ dst_v, const uint32_t *__restrict__ d_count, int shift, const uint32_t *__restrict__ ghist,
            volatile uint32_t *lookback, uint32_t *ticket) {
   constexpr uint32_t NB = 1u << BITS;
-  constexpr uint32_t kTileItems = THREADS * kSortKpt;
-  constexpr int kSortWarps = THREADS / 32;
-  constexpr int kSortThreads = THREADS;
+  static_assert(NB <= (uint32_t)kSortThreads, "steps 2 and 4 give each digit its own thread");
+  constexpr uint32_t kTileItems = kSortTileItems;
   extern __shared__ __align__(16) uint8_t s_dyn[];
   uint2 *s_kv = reinterpret_cast<uint2 *>(s_dyn);                                         // [kTileItems]
   uint32_t (*s_whist)[NB] = reinterpret_cast<uint32_t (*)[NB]>(s_dyn + kTileItems * 8);    // [kSortWarps][NB]
@@ -227,7 +233,7 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
     }
   }
 
-  // 3. stable in-warp ranking; ranks (< 4096) are packed two per register
+  // 3. stable in-warp ranking; a warp ranks its own 512 pairs, so ranks (< 512) are packed two per register
   uint32_t rank2[kSortKpt / 2];
   const uint32_t lt_mask = (1u << lane) - 1u;
 #pragma unroll
@@ -411,18 +417,12 @@ uint32_t sm_count() {
   return cached[dev];
 }
 
-static int sort_threads() {
-  static int v = 0;
-  if (!v) { const char *e = getenv("GS_SORT_THREADS"); v = (e && atoi(e) == 512) ? 512 : 256; }
-  return v;
-}
-
 template <int BITS>
 static void launch_pass(uint32_t count_bound, bool persist, cudaStream_t s, const uint32_t *sk, const uint32_t *sv, uint32_t *dk,
                         uint32_t *dv, const uint32_t *d_count, int shift, const uint32_t *ghist, uint32_t *lookback, uint32_t *ticket,
                         bool gather) {
-  auto go = [&](auto kern, int threads) {
-    const size_t smem = (size_t)threads * kSortKpt * 8 + (size_t)(threads / 32) * (1u << BITS) * 4;
+  auto go = [&](auto kern) {
+    const size_t smem = (size_t)kSortTileItems * 8 + (size_t)kSortWarps * (1u << BITS) * 4;
     // the opt-in for > 48 KB dynamic shared memory is per function AND per device
     struct Seen { const void *fn; int dev; };
     static thread_local Seen configured[64];
@@ -435,26 +435,28 @@ static void launch_pass(uint32_t count_bound, bool persist, cudaStream_t s, cons
       cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (nconf < 64) configured[nconf++] = Seen{(const void *)kern, dev};
     }
-    const uint32_t per = (uint32_t)threads * kSortKpt;
-    uint32_t grid = (uint32_t)(((uint64_t)count_bound + per - 1) / per);
-    if (persist) grid = min(grid, sm_count() * (1024u / (uint32_t)threads));
-    kern<<<grid, threads, smem, s>>>(sk, sv, dk, dv, d_count, shift, ghist, lookback, ticket);
+    uint32_t grid = (uint32_t)(((uint64_t)count_bound + kSortTileItems - 1) / kSortTileItems);
+    if (persist) grid = min(grid, sm_count() * 2u);   // the 2 CTAs per SM that __launch_bounds__ asks for
+    kern<<<grid, kSortThreads, smem, s>>>(sk, sv, dk, dv, d_count, shift, ghist, lookback, ticket);
   };
   if (persist) {
-    if (gather) go(k_onesweep<BITS, true, 256, true>, 256); else go(k_onesweep<BITS, false, 256, true>, 256);
-  } else if (sort_threads() == 512) {
-    if (gather) go(k_onesweep<BITS, true, 512, false>, 512); else go(k_onesweep<BITS, false, 512, false>, 512);
+    if (gather) go(k_onesweep<BITS, true, true>); else go(k_onesweep<BITS, false, true>);
   } else {
-    if (gather) go(k_onesweep<BITS, true, 256, false>, 256); else go(k_onesweep<BITS, false, 256, false>, 256);
+    if (gather) go(k_onesweep<BITS, true, false>); else go(k_onesweep<BITS, false, false>);
   }
 }
 
-void launch_sort_pairs(uint32_t *keys, uint32_t *vals, const uint32_t *d_count, uint32_t capacity, int passes, int bits,
-                       bool hist_ready, const SortScratch &sc, cudaStream_t s, cudaEvent_t *pass_events, const uint32_t *key_table,
-                       bool count_is_capacity, uint32_t *final_keys, uint32_t *final_vals) {
-  if (capacity == 0) return;
+cudaError_t launch_sort_pairs(uint32_t *keys, uint32_t *vals, const uint32_t *d_count, uint32_t capacity, int passes, int bits,
+                              bool hist_ready, const SortScratch &sc, cudaStream_t s, cudaEvent_t *pass_events, const uint32_t *key_table,
+                              bool count_is_capacity, uint32_t *final_keys, uint32_t *final_vals) {
+  if (capacity == 0) return cudaSuccess;
   const uint32_t tiles = (capacity + kSortTileItems - 1) / kSortTileItems;
   const uint32_t nb = 1u << bits;
+  // ghist has one row of 256 words per pass, so a 9-bit digit (512 words) is only possible as a single pass; k_sort_hist
+  // counts 4 x 8 or 2 x 5..8 bits, so a 9-bit digit needs the caller's histogram.  Nothing is launched for any other request.
+  const bool shape_ok = passes >= 1 && passes <= 4 && bits >= 5 && (bits <= 8 || (bits == 9 && passes == 1));
+  const bool hist_ok = hist_ready || (passes == 4 && bits == 8) || (passes <= 2 && bits <= 8);
+  if (!shape_ok || !hist_ok || (size_t)tiles * nb * passes > sc.lookback_words) return cudaErrorInvalidValue;
   // count_is_capacity: the host knows the exact count (depth sort, slab sort) -> exact grid, exact memset.  Otherwise the list
   // length lives on the device only (the binner's entries): a persistent grid, and the look-back rows actually needed are
   // cleared by a kernel that reads the count.
@@ -469,7 +471,7 @@ void launch_sort_pairs(uint32_t *keys, uint32_t *vals, const uint32_t *d_count, 
     else if (bits == 5) k_sort_hist<2, 5><<<grid, 256, 0, s>>>(keys, d_count, sc.ghist);
     else if (bits == 6) k_sort_hist<2, 6><<<grid, 256, 0, s>>>(keys, d_count, sc.ghist);
     else if (bits == 7) k_sort_hist<2, 7><<<grid, 256, 0, s>>>(keys, d_count, sc.ghist);
-    else k_sort_hist<2, 8><<<grid, 256, 0, s>>>(keys, d_count, sc.ghist);
+    else k_sort_hist<2, 8><<<grid, 256, 0, s>>>(keys, d_count, sc.ghist);   // bits == 8: hist_ok rules out 9
   }
   uint32_t *sk = keys, *sv = vals, *dk = sc.alt_keys, *dv = sc.alt_vals;
   for (int p = 0; p < passes; ++p) {
@@ -481,11 +483,13 @@ void launch_sort_pairs(uint32_t *keys, uint32_t *vals, const uint32_t *d_count, 
     if (bits == 5) launch_pass<5>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
     else if (bits == 6) launch_pass<6>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
     else if (bits == 7) launch_pass<7>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
-    else launch_pass<8>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
+    else if (bits == 8) launch_pass<8>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
+    else launch_pass<9>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
     uint32_t *t = sk; sk = dk; dk = t;
     t = sv; sv = dv; dv = t;
   }
   if (pass_events) cudaEventRecord(pass_events[passes], s);
+  return cudaSuccess;
 }
 
 }  // namespace gs
