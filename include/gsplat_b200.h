@@ -114,14 +114,26 @@ typedef enum GsPixelFormat {
   GS_PIX_RGBA32F = 1
 } GsPixelFormat;
 
-typedef enum GsMemory { GS_MEM_HOST = 0, GS_MEM_DEVICE = 1 } GsMemory;
+/* GS_MEM_ARRAY (images only, not GsPackDesc / GsPackedAsset): `data` is a cudaArray_t -- a 2-D CUDA array (mip level 0) on the
+ * context's device, e.g. a Vulkan / D3D12 render texture imported with cudaImportExternalMemory +
+ * cudaExternalMemoryGetMappedMipmappedArray + cudaGetMipmappedArrayLevel(.., 0), or a GL / D3D11 one from
+ * cudaGraphicsSubResourceGetMappedArray.  The library reads and writes it in place through surface objects, so:
+ *   - the array must have been created with cudaArraySurfaceLoadStore (for an imported image: ask for that flag in
+ *     cudaExternalMemoryMipmappedArrayDesc.flags);
+ *   - its channel format must be the image's: 4 x 16-bit float for GS_PIX_RGBA16F, 4 x 32-bit float for GS_PIX_RGBA32F
+ *     (else GS_ERR_UNSUPPORTED_FORMAT);
+ *   - its extent must be width x height with depth 0, and row_pitch_bytes must be 0 (else GS_ERR_INVALID_ARGUMENT).
+ * The import itself and the graphics API's semaphores stay with the host: wait / signal them on gs_context_stream(ctx).
+ * Not accepted (GS_ERR_INVALID_ARGUMENT): band_packed output and gs_unshuffle_bands output.  GS_FLAG_ASYNC_READBACK has no
+ * effect on an array render target (it applies to host images only). */
+typedef enum GsMemory { GS_MEM_HOST = 0, GS_MEM_DEVICE = 1, GS_MEM_ARRAY = 2 } GsMemory;
 
 typedef struct GsImage {
-  void *data;
+  void *data;                /* host pointer, device pointer, or cudaArray_t (GS_MEM_ARRAY) */
   uint32_t width, height;
-  uint32_t row_pitch_bytes;  /* 0 = tightly packed */
+  uint32_t row_pitch_bytes;  /* 0 = tightly packed (and always 0 for GS_MEM_ARRAY) */
   uint32_t format;           /* GsPixelFormat */
-  uint32_t memory;           /* GsMemory: where `data` lives */
+  uint32_t memory;           /* GsMemory: where `data` lives; a value above GS_MEM_ARRAY is GS_ERR_INVALID_ARGUMENT */
 } GsImage;
 
 /* How the render-target blend is evaluated.
@@ -150,7 +162,7 @@ typedef struct GsRenderOptions {
 } GsRenderOptions;
 
 typedef enum GsRenderFlags {
-  /* gs_frame with a HOST render target returns as soon as the read-back is ENQUEUED (on a second stream, double-buffered
+  /* gs_frame with a HOST render target (the flag has no effect on device or array targets) returns as soon as the read-back is ENQUEUED (on a second stream, double-buffered
    * device staging): frame k's copy overlaps frame k+1's kernels.  The image must be pinned (cudaHostRegister /
    * cudaMallocHost) and must not be read, nor handed to another frame, until gs_sync (or two later frames) -- the
    * managed-side analogue is AsyncGPUReadback.  Errors of the frame (e.g. a truncated bin list) surface at gs_sync. */
@@ -272,8 +284,9 @@ GS_API GsContext *gs_group_context(GsGroup *group, uint32_t local_index);
 /* CreateResourcesForAsset on every local member (R/GaussianSplatRenderer.cs:373-445): assets_out[local_count]. */
 GS_API int gs_group_asset_upload(GsGroup *group, const GsAssetDesc *desc, GsAsset **assets_out);
 /* SortAndRenderSplats (R/GaussianSplatRenderer.cs:108-169) on the group.  assets[i] / rts[i] belong to local member i;
- * rts[i] is a full-size image (device or host memory; NULL = this member keeps the frame in library scratch only).  Every
- * non-NULL rts[i] ends up holding the COMPLETE render target.  `opt`: blend_mode, and GS_FLAG_ASYNC_READBACK for host images
+ * rts[i] is a full-size image (device, host or CUDA-array memory; NULL = this member keeps the frame in library scratch only).
+ * Every non-NULL rts[i] ends up holding the COMPLETE render target; an array is filled by one copy of the assembled frame on the
+ * member's transfer stream, complete after gs_group_sync.  `opt`: blend_mode, and GS_FLAG_ASYNC_READBACK for host images
  * (the call returns with the read-back enqueued; gs_group_sync completes it).  Collective: every process of the
  * group must call it with the same parameters. */
 GS_API int gs_group_frame(GsGroup *group, GsAsset *const *assets, const GsFrameParams *fp, const GsRenderOptions *opt, int do_sort,

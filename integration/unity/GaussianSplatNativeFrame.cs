@@ -73,10 +73,11 @@ namespace GaussianSplatting.Runtime
             dst.CopyFrom(src);
         }
 
-        /// Records the native frame into `cmb`.  `rtDevicePtr` is the CUDA mapping of the linear RGBA16F buffer that backs
-        /// _GaussianSplatRT (external-memory interop, INTEGRATION.md section 3); the composite draw that follows in the
-        /// reference (:206-210) stays as it is and reads that buffer.
-        public void Record(CommandBuffer cmb, GaussianSplatRenderer gs, Camera cam, IntPtr ctx, IntPtr asset, IntPtr rtDevicePtr,
+        /// Records the native frame into `cmb`.  `rtArray` is the cudaArray_t of _GaussianSplatRT's R16G16B16A16_SFloat image
+        /// that the graphics-interop plugin imported (cudaImportExternalMemory -> cudaExternalMemoryGetMappedMipmappedArray with
+        /// cudaArraySurfaceLoadStore -> cudaGetMipmappedArrayLevel 0; INTEGRATION.md section 3).  The library renders into it in
+        /// place; the composite draw that follows in the reference (:206-210) stays as it is and samples that texture.
+        public void Record(CommandBuffer cmb, GaussianSplatRenderer gs, Camera cam, IntPtr ctx, IntPtr asset, IntPtr rtArray,
                            int rtWidth, int rtHeight, NativeArray<uint> hostDeletedBits = default, NativeArray<uint> hostSelectedBits = default)
         {
             // results of the event recorded kInFlight frames ago: log and skip, like the reference (:655)
@@ -128,8 +129,8 @@ namespace GaussianSplatting.Runtime
             ev->has_rt = 1; ev->has_camera_target = 0;
             ev->rt = new GaussianSplatNative.GsImage
             {
-                data = (void*)rtDevicePtr, width = (uint)rtWidth, height = (uint)rtHeight,
-                row_pitch_bytes = 0, format = 0 /* GS_PIX_RGBA16F */, memory = 1 /* GS_MEM_DEVICE */
+                data = (void*)rtArray, width = (uint)rtWidth, height = (uint)rtHeight,
+                row_pitch_bytes = 0, format = 0 /* GS_PIX_RGBA16F */, memory = 2 /* GS_MEM_ARRAY */
             };
             ++gs.m_FrameCounter;
             cmb.IssuePluginEventAndData(s_EventFunc, kEventFrame, (IntPtr)ev);

@@ -1,0 +1,411 @@
+"""CUDA arrays as images (GS_MEM_ARRAY): what a graphics API's render texture looks like once it is imported into CUDA
+(cudaExternalMemoryGetMappedMipmappedArray / cudaGraphicsSubResourceGetMappedArray).  The library renders into and composites
+onto such an array in place, through surface objects.
+
+Arrays are made here with the CUDA runtime torch already loaded (a runtime cudaArray_t is a driver CUarray in the device's
+primary context, so the library's own runtime can use it).  Every GPU test compares the array result byte for byte with the
+same call on a torch device tensor: the linear path is pinned to the oracle elsewhere, so equality is the parity contract."""
+import ctypes as C
+import re
+import sys
+from pathlib import Path
+
+import numpy as np
+import pytest
+
+from util import camera
+
+ROOT = Path(__file__).resolve().parents[1]
+GOLD = Path(__file__).parent / "golden"
+
+# cudaChannelFormatKind / cudaArray flags / cudaMemcpyKind (cuda_runtime_api.h)
+_KIND_UNSIGNED, _KIND_FLOAT = 1, 2
+_SURFACE_LOAD_STORE = 0x02
+_H2D, _D2H = 1, 2
+
+
+def test_header_and_python_agree_on_gs_mem_array():
+    from unitygaussiansplatting_b200 import _native as N
+    text = (ROOT / "include" / "gsplat_b200.h").read_text()
+    m = re.search(r"typedef enum GsMemory \{([^}]*)\} GsMemory;", text)
+    assert m, "GsMemory enum not found in the header"
+    values = dict((k, int(v)) for k, v in re.findall(r"(GS_MEM_\w+)\s*=\s*(\d+)", m.group(1)))
+    assert values == {"GS_MEM_HOST": N.GS_MEM_HOST, "GS_MEM_DEVICE": N.GS_MEM_DEVICE, "GS_MEM_ARRAY": N.GS_MEM_ARRAY}
+    assert N.GS_MEM_ARRAY == 2
+
+
+class _ChannelDesc(C.Structure):
+    _fields_ = [("x", C.c_int), ("y", C.c_int), ("z", C.c_int), ("w", C.c_int), ("f", C.c_int)]
+
+
+class _Cudart:
+    """cudaMallocArray / cudaMemcpy2D{To,From}Array / cudaFreeArray through the runtime torch loaded."""
+
+    def __init__(self):
+        import torch
+        torch.cuda.init()
+        self.lib = C.CDLL("libcudart.so.12")   # resolves to the copy torch already loaded (same soname)
+        self.lib.cudaMallocArray.argtypes = [C.POINTER(C.c_void_p), C.POINTER(_ChannelDesc), C.c_size_t, C.c_size_t, C.c_uint]
+        self.lib.cudaMemcpy2DToArray.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
+        self.lib.cudaMemcpy2DFromArray.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
+        self.lib.cudaFreeArray.argtypes = [C.c_void_p]
+        self.live = []
+
+    def _check(self, rc, what):
+        assert rc == 0, "%s failed with CUDA error %d" % (what, rc)
+
+    def array(self, width, height, bits=16, kind=_KIND_FLOAT, flags=_SURFACE_LOAD_STORE):
+        h = C.c_void_p()
+        desc = _ChannelDesc(bits, bits, bits, bits, kind)
+        self._check(self.lib.cudaMallocArray(C.byref(h), C.byref(desc), width, height, flags), "cudaMallocArray")
+        self.live.append(h.value)
+        return h.value
+
+    def upload(self, handle, host):
+        host = np.ascontiguousarray(host)
+        row = host.shape[1] * host.shape[2] * host.itemsize
+        self._check(self.lib.cudaMemcpy2DToArray(handle, 0, 0, host.ctypes.data, row, row, host.shape[0], _H2D), "cudaMemcpy2DToArray")
+
+    def download(self, handle, shape, dtype):
+        out = np.empty(shape, dtype)
+        row = shape[1] * shape[2] * out.itemsize
+        self._check(self.lib.cudaMemcpy2DFromArray(out.ctypes.data, row, handle, 0, 0, row, shape[0], _D2H), "cudaMemcpy2DFromArray")
+        return out
+
+    def free_all(self):
+        for h in self.live:
+            self.lib.cudaFreeArray(h)
+        self.live = []
+
+
+@pytest.fixture
+def rt_arrays(ctx):
+    ca = _Cudart()
+    yield ca
+    ctx.sync()
+    ca.free_all()
+
+
+def _image_array(g, ca, w, h, dtype=np.float16, fill=None):
+    """A CudaArrayImage of (h, w) RGBA texels, pre-filled with `fill` (default: random halves / floats)."""
+    handle = ca.array(w, h, 16 if dtype == np.float16 else 32)
+    if fill is None:
+        fill = np.random.default_rng(w * 7919 + h).random((h, w, 4), np.float32).astype(dtype)
+    ca.upload(handle, np.broadcast_to(np.asarray(fill, dtype), (h, w, 4)))
+    return g.CudaArrayImage(handle, w, h, dtype)
+
+
+def _read(ctx, ca, im):
+    ctx.sync()   # the library's stream does not synchronise with the legacy default stream the copy runs on
+    return ca.download(im.handle, im.shape, im.dtype)
+
+
+def _tensor(h, w, dtype=np.float16, fill=None):
+    import torch
+    t = torch.zeros((h, w, 4), dtype=torch.float16 if dtype == np.float16 else torch.float32, device="cuda")
+    if fill is not None:
+        t.copy_(torch.from_numpy(np.array(np.broadcast_to(np.asarray(fill, dtype), (h, w, 4)))))
+    return t
+
+
+def _host(ctx, t):
+    import torch
+    ctx.sync()
+    torch.cuda.synchronize()
+    return t.cpu().numpy()
+
+
+def _bits(a):
+    return a.view(np.uint16) if a.dtype == np.float16 else a.view(np.uint32)
+
+
+def _lattice_case(g):
+    sys.path.insert(0, str(GOLD))
+    import make_golden
+    kind, n, seed, quality, _w, _h, pos, sh = make_golden.CASES["lattice_1k_medium"]
+    return g.synthetic_asset(kind, n, seed, quality), camera(g, 256, 256, pos=pos), sh
+
+
+# ---- 1, 2: gs_frame into an array --------------------------------------------------------------------------------------------
+@pytest.mark.gpu
+@pytest.mark.parametrize("scene", ["lattice_1k_medium_256x256", "clustered_333x211"])
+def test_frame_into_rgba16f_array_equals_tensor(g, O, ctx, rt_arrays, scene):
+    if scene.startswith("lattice"):
+        asset, cam, sh = _lattice_case(g)
+    else:
+        asset, cam, sh = g.synthetic_asset(g.SCENE_CLUSTERED, 30000, 0x5EED00A1, "Medium"), camera(g, 333, 211), 3
+    h, w = cam.pixelHeight, cam.pixelWidth
+    r = g.GaussianSplatRenderer(asset, ctx)
+    r.m_SHOrder = sh
+    t = _tensor(h, w)
+    r.SortAndRenderSplats(cam, rt=t)
+    want = _host(ctx, t)
+    r.ResetOrder()
+    im = _image_array(g, rt_arrays, w, h)     # random content: every pixel must be overwritten
+    r.SortAndRenderSplats(cam, rt=im)
+    got = _read(ctx, rt_arrays, im)
+    assert want.any()
+    assert np.array_equal(_bits(got), _bits(want))
+    if scene.startswith("lattice"):   # and straight against the oracle
+        fp, _keep = g.make_frame_params(cam, sh_order=sh)
+        ref = O.frame(asset, fp, threads=O.max_threads())
+        assert np.array_equal(got.astype(np.float32), ref["rt"])
+    r.Dispose()
+
+
+@pytest.mark.gpu
+def test_frame_into_rgba32f_array_fp32_blend_equals_tensor(g, ctx, rt_arrays):
+    asset = g.synthetic_asset(g.SCENE_CLUSTERED, 30000, 0x5EED00A2, "Medium")
+    cam = camera(g, 333, 211)
+    r = g.GaussianSplatRenderer(asset, ctx)
+    r.blend_mode = 1
+    t = _tensor(211, 333, np.float32)
+    r.SortAndRenderSplats(cam, rt=t)
+    want = _host(ctx, t)
+    r.ResetOrder()
+    im = _image_array(g, rt_arrays, 333, 211, np.float32)
+    r.SortAndRenderSplats(cam, rt=im)
+    got = _read(ctx, rt_arrays, im)
+    assert want.any() and np.array_equal(_bits(got), _bits(want))
+    r.Dispose()
+
+
+# ---- 3: GS_FLAG_LOAD_RT ------------------------------------------------------------------------------------------------------
+@pytest.mark.gpu
+def test_two_renderers_share_one_array_render_target(g, ctx, rt_arrays):
+    a = g.synthetic_asset(g.SCENE_CLUSTERED, 30000, 0x5EED0091, "Medium")
+    b = g.synthetic_asset(g.SCENE_CLUSTERED, 20000, 0x5EED0092, "VeryHigh")
+    cam = camera(g, 400, 300)
+
+    def draw(rt):
+        ra, rb = g.GaussianSplatRenderer(a, ctx), g.GaussianSplatRenderer(b, ctx)
+        ra.localToWorldMatrix = g.trs(position=(1.5, 0.0, 3.0)).astype(np.float32)
+        rb.localToWorldMatrix = g.trs(position=(-1.0, 0.2, 0.5), scale=(0.7, 0.7, 0.7)).astype(np.float32)
+        active = g.SortAndRenderSplatsMulti([ra, rb], cam, rt)
+        assert active == [rb, ra]
+        return ra, rb
+
+    t = _tensor(300, 400)
+    keep = draw(t)
+    want = _host(ctx, t)
+    im = _image_array(g, rt_arrays, 400, 300)
+    keep += draw(im)
+    got = _read(ctx, rt_arrays, im)
+    assert want.any() and np.array_equal(_bits(got), _bits(want))
+    for r in keep:
+        r.Dispose()
+
+
+# ---- 4: the extras variant (selection + scene depth) ---------------------------------------------------------------------------
+@pytest.mark.gpu
+def test_selection_and_scene_depth_into_array(g, ctx, rt_arrays):
+    asset = g.synthetic_asset(g.SCENE_CLUSTERED, 40000, 0x5EED00A4, "Medium")
+    n = asset.splatCount
+    sel = np.zeros((n + 31) // 32, np.uint32)
+    ids = np.arange(0, n, 5)
+    np.bitwise_or.at(sel, ids >> 5, np.uint32(1) << (ids & 31).astype(np.uint32))
+    cam = camera(g, 400, 300)
+    P = cam.gpuProjectionMatrix(True).astype(np.float64)
+    clip = P @ np.array([0.0, 0.0, -6.0, 1.0])
+    depth = np.zeros((300, 400), np.float32)
+    depth[:, :240] = np.float32(clip[2] / clip[3])
+    r = g.GaussianSplatRenderer(asset, ctx)
+    r.m_SelectedBits, r.sceneDepth = sel, depth
+    t = _tensor(300, 400)
+    r.SortAndRenderSplats(cam, rt=t)
+    want = _host(ctx, t)
+    r.ResetOrder()
+    im = _image_array(g, rt_arrays, 400, 300)
+    r.SortAndRenderSplats(cam, rt=im)
+    got = _read(ctx, rt_arrays, im)
+    assert want.any() and np.array_equal(_bits(got), _bits(want))
+    r.Dispose()
+
+
+# ---- 5: staged calls -------------------------------------------------------------------------------------------------------------
+@pytest.mark.gpu
+def test_staged_render_into_array_equals_fused_frame(g, ctx, rt_arrays):
+    asset = g.synthetic_asset(g.SCENE_CLUSTERED, 30000, 0x5EED0006, "Medium")
+    cam = camera(g, 300, 200)
+    a, b = g.GaussianSplatRenderer(asset, ctx), g.GaussianSplatRenderer(asset, ctx)
+    t = _tensor(200, 300)
+    a.SortAndRenderSplats(cam, rt=t)
+    want = _host(ctx, t)
+    im = _image_array(g, rt_arrays, 300, 200)
+    b.SortPoints(cam); b.CalcViewData(cam); b.DrawSplats(cam, im)
+    got = _read(ctx, rt_arrays, im)
+    assert want.any() and np.array_equal(_bits(got), _bits(want))
+    a.Dispose(); b.Dispose()
+
+
+# ---- 6: composite --------------------------------------------------------------------------------------------------------------
+@pytest.mark.gpu
+@pytest.mark.parametrize("tgt_dtype", [np.float16, np.float32])
+def test_composite_all_four_target_kinds(g, ctx, rt_arrays, tgt_dtype):
+    asset = g.synthetic_asset(g.SCENE_CLUSTERED, 20000, 0x5EED0002, "Medium")
+    cam = camera(g, 320, 200)
+    r = g.GaussianSplatRenderer(asset, ctx)
+    rt_t = _tensor(200, 320)
+    r.SortAndRenderSplats(cam, rt=rt_t)
+    rt_np = _host(ctx, rt_t)
+    assert (rt_np[..., 3] == 0).any() and (rt_np[..., 3] > 0).any()   # both sides of the SrcAlpha == 0 early-out occur
+    rt_a = _image_array(g, rt_arrays, 320, 200, fill=rt_np)
+    bg = np.random.default_rng(11).random((200, 320, 4), np.float32).astype(np.float16).astype(tgt_dtype)
+    want = None
+    for src in (rt_t, rt_a):
+        for kind in ("tensor", "array"):
+            tgt = _tensor(200, 320, tgt_dtype, fill=bg) if kind == "tensor" else _image_array(g, rt_arrays, 320, 200, tgt_dtype, fill=bg)
+            r.Composite(src, tgt)
+            got = _host(ctx, tgt) if kind == "tensor" else _read(ctx, rt_arrays, tgt)
+            if want is None:
+                want = got
+                untouched = rt_np[..., 3] == 0
+                assert np.array_equal(_bits(got)[untouched], _bits(bg)[untouched]) and not np.array_equal(got, bg)
+            assert np.array_equal(_bits(got), _bits(want)), "rt %s, target %s" % ("tensor" if src is rt_t else "array", kind)
+    # gs_frame with an array camera target, with the render target in library scratch and with an array render target
+    for with_rt in (False, True):
+        r.ResetOrder(); r.m_FrameCounter = 0
+        tgt = _image_array(g, rt_arrays, 320, 200, tgt_dtype, fill=bg)
+        rt = _image_array(g, rt_arrays, 320, 200) if with_rt else None
+        r.SortAndRenderSplats(cam, rt=rt, camera_target=tgt)
+        assert np.array_equal(_bits(_read(ctx, rt_arrays, tgt)), _bits(want)), "gs_frame, rt %s" % ("array" if with_rt else "scratch")
+        if with_rt:
+            assert np.array_equal(_bits(_read(ctx, rt_arrays, rt)), _bits(rt_np))
+    r.Dispose()
+
+
+# ---- 7: row ranges ---------------------------------------------------------------------------------------------------------------
+@pytest.mark.gpu
+def test_row_range_into_array_keeps_other_rows(g, ctx, rt_arrays):
+    asset = g.synthetic_asset(g.SCENE_CLUSTERED, 30000, 0x5EED00A7, "Medium")
+    cam = camera(g, 333, 211)
+    r = g.GaussianSplatRenderer(asset, ctx)
+    full_t = _tensor(211, 333)
+    r.SortAndRenderSplats(cam, rt=full_t)
+    full = _host(ctx, full_t)
+    sentinel = np.float16(-7.5)
+    r.rows = (3, 11)                          # 16-pixel rows 3..10: pixel rows [48, 176)
+    r.ResetOrder(); r.m_FrameCounter = 0
+    t = _tensor(211, 333, fill=sentinel)
+    r.SortAndRenderSplats(cam, rt=t)
+    want = _host(ctx, t)
+    r.ResetOrder(); r.m_FrameCounter = 0
+    im = _image_array(g, rt_arrays, 333, 211, fill=sentinel)
+    r.SortAndRenderSplats(cam, rt=im)
+    got = _read(ctx, rt_arrays, im)
+    assert np.array_equal(_bits(got), _bits(want))
+    assert np.array_equal(_bits(got[48:176]), _bits(full[48:176])) and full[48:176].any()
+    assert (got[:48] == sentinel).all() and (got[176:] == sentinel).all()
+    r.Dispose()
+
+
+# ---- 8: the Unity render-thread event ------------------------------------------------------------------------------------------
+@pytest.mark.gpu
+def test_unity_event_with_array_rt_equals_direct_frame(g, ctx, rt_arrays):
+    from unitygaussiansplatting_b200 import _native as N
+    asset = g.synthetic_asset(g.SCENE_CLUSTERED, 20000, 0x5EED0051, "Medium")
+    cam = camera(g, 200, 150)
+    r = g.GaussianSplatRenderer(asset, ctx)
+    direct = np.zeros((150, 200, 4), np.float16)
+    r.SortAndRenderSplats(cam, rt=direct)
+    r.ResetOrder()
+    im = _image_array(g, rt_arrays, 200, 150)
+    fp, _keep = g.make_frame_params(cam, r.localToWorldMatrix, r.m_SplatScale, r.m_OpacityScale, r.m_SHOrder, r.m_SHOnly)
+    ev = N.GsUnityFrameEvent()
+    ev.ctx, ev.asset = C.cast(ctx.handle, C.c_void_p).value, C.cast(r._asset, C.c_void_p).value
+    C.memmove(C.byref(ev.params), C.byref(fp), C.sizeof(fp))
+    ev.options.blend_mode = 0
+    ev.do_sort, ev.status = 1, -5
+    ev.has_rt, ev.has_camera_target = 1, 0
+    ev.rt.data, ev.rt.width, ev.rt.height = im.handle, 200, 150
+    ev.rt.row_pitch_bytes, ev.rt.format, ev.rt.memory = 0, N.GS_PIX_RGBA16F, N.GS_MEM_ARRAY
+    fn = N.native().gs_unity_get_render_event_func()
+    fn(N.GS_UNITY_EVENT_FRAME, C.addressof(ev))
+    assert ev.status == 0
+    fn(N.GS_UNITY_EVENT_SYNC, C.addressof(ev))
+    assert ev.status == 0
+    got = _read(ctx, rt_arrays, im)
+    assert direct.any() and np.array_equal(_bits(got), _bits(direct))
+    r.Dispose()
+
+
+# ---- 9: groups -----------------------------------------------------------------------------------------------------------------
+@pytest.mark.gpu
+@pytest.mark.parametrize("members", [2, 3])
+def test_emulated_group_with_array_members_equals_one_gpu(g, ctx, rt_arrays, members):
+    from unitygaussiansplatting_b200.multigpu import GaussianSplatGroup
+    asset = g.synthetic_asset(g.SCENE_CLUSTERED, 40000, 0x5EED00A9, "Medium")
+    cam = camera(g, 400, 300)
+    r = g.GaussianSplatRenderer(asset, ctx)
+    want = np.zeros((300, 400, 4), np.float16)
+    r.SortAndRenderSplats(cam, rt=want)
+    r.Dispose()
+    grp = GaussianSplatGroup.create(asset, [0] * members, emulate=True)
+    arrays = [_image_array(g, rt_arrays, 400, 300) for _ in range(members - 1)]   # rts[0] (and rts[1] for 3 members)
+    rest = [np.zeros_like(want)]
+    grp.SortAndRenderSplats(cam, rts=arrays + rest)
+    grp.sync()
+    assert want.any()
+    for im in arrays:
+        assert np.array_equal(_bits(_read(ctx, rt_arrays, im)), _bits(want))
+    assert np.array_equal(_bits(rest[0]), _bits(want))
+    grp.close()
+
+
+# ---- 10: rejections ------------------------------------------------------------------------------------------------------------
+@pytest.mark.gpu
+def test_array_rejections_leave_the_array_untouched(g, ctx, rt_arrays):
+    import torch
+    from unitygaussiansplatting_b200 import _native as N
+    lib = N.native()
+    asset = g.synthetic_asset(g.SCENE_CLUSTERED, 20000, 0x5EED00AA, "Medium")
+    cam = camera(g, 128, 128)
+    r = g.GaussianSplatRenderer(asset, ctx)
+    fp = r.frame_params(cam)
+
+    def frame(handle, fmt=N.GS_PIX_RGBA16F, memory=N.GS_MEM_ARRAY, pitch=0, band_packed=0):
+        im = N.GsImage(handle, 128, 128, pitch, fmt, memory)
+        opt = r._options()
+        opt.band_packed = band_packed
+        return lib.gs_frame(ctx.handle, r._asset, C.byref(fp), C.byref(opt), 1, C.byref(im), None)
+
+    pattern = np.random.default_rng(3).random((128, 128, 4), np.float32).astype(np.float16)
+
+    def filled(width=128, bits=16, kind=_KIND_FLOAT, flags=_SURFACE_LOAD_STORE, fill=pattern):
+        h = rt_arrays.array(width, 128, bits, kind, flags)
+        rt_arrays.upload(h, fill)
+        return h
+
+    def unchanged(h, fill=pattern, width=128):
+        return np.array_equal(rt_arrays.download(h, (128, width, 4), fill.dtype).view(np.uint8), fill.view(np.uint8))
+
+    bytes8 = np.random.default_rng(4).integers(0, 256, (128, 128, 4), np.uint8)
+    h = filled(bits=8, kind=_KIND_UNSIGNED, fill=bytes8)                      # uint8 x 4
+    assert frame(h) == -4 and "channel format" in lib.gs_last_error(ctx.handle).decode()
+    ctx.sync()
+    assert unchanged(h, bytes8)
+    wide = np.concatenate([pattern, pattern[:, :1]], axis=1)
+    h = filled(width=129, fill=wide)                                           # 129 x 128 for a 128 x 128 image
+    assert frame(h) == -1
+    ctx.sync()
+    assert unchanged(h, wide, 129)
+    h = filled(flags=0)                                                        # no cudaArraySurfaceLoadStore
+    assert frame(h) == -1 and "cudaArraySurfaceLoadStore" in lib.gs_last_error(ctx.handle).decode()
+    good = filled()
+    assert frame(good, pitch=128 * 8) == -1                                    # non-zero pitch
+    assert frame(good, memory=3) == -1                                         # unknown memory kind
+    opt = r._options()                                                         # band-packed output (all of one partition's rows)
+    opt.partition_index, opt.partition_count, opt.band_rows, opt.band_packed = 0, 2, 1, 1
+    im = N.GsImage(good, 128, 64, 0, N.GS_PIX_RGBA16F, N.GS_MEM_ARRAY)
+    assert lib.gs_frame(ctx.handle, r._asset, C.byref(fp), C.byref(opt), 1, C.byref(im), None) == -1
+    assert "band_packed" in lib.gs_last_error(ctx.handle).decode()
+    gathered = torch.zeros((2, 64, 128, 4), dtype=torch.float16, device="cuda")   # gs_unshuffle_bands into an array
+    im = N.GsImage(good, 128, 128, 0, N.GS_PIX_RGBA16F, N.GS_MEM_ARRAY)
+    assert lib.gs_unshuffle_bands(ctx.handle, C.c_void_p(gathered.data_ptr()), 2, 1, 64, N.GS_PIX_RGBA16F, C.byref(im)) == -1
+    ctx.sync()
+    assert unchanged(good) and unchanged(rt_arrays.live[2])
+    # and the same array, correctly described, is accepted
+    assert frame(good) == 0
+    ctx.sync()
+    assert not unchanged(good)
+    r.Dispose()

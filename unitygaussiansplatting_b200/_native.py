@@ -15,7 +15,7 @@ ASSET_LIB = PKG / "libgsplat_asset.so"
 GS_OK = 0
 GS_ERR_NO_DEVICE = -6
 GS_PIX_RGBA16F, GS_PIX_RGBA32F = 0, 1
-GS_MEM_HOST, GS_MEM_DEVICE = 0, 1
+GS_MEM_HOST, GS_MEM_DEVICE, GS_MEM_ARRAY = 0, 1, 2
 GS_BLEND_FP16_ROP, GS_BLEND_FP32 = 0, 1
 
 

@@ -184,6 +184,67 @@ static int ensure_async_readback(GsContext *ctx) {
 
 uint32_t pix_bytes(uint32_t fmt) { return fmt == GS_PIX_RGBA16F ? 8u : 16u; }
 
+// ---- GS_MEM_ARRAY images -----------------------------------------------------------------------------
+// Destroys the held surface objects whose last use has completed (every one when `all`: the caller has synchronised the stream).
+static void release_surfaces(GsContext *ctx, bool all) {
+  auto &held = ctx->held_surfaces;
+  size_t keep = 0;
+  for (size_t i = 0; i < held.size(); ++i) {
+    bool done = all;
+    if (!done) {
+      const cudaError_t q = cudaEventQuery(held[i].done);
+      done = q != cudaErrorNotReady;   // completed, or failed: either way nothing will use the surfaces any more
+      if (!done && cudaPeekAtLastError() == cudaErrorNotReady) cudaGetLastError();
+    }
+    if (done) {
+      for (cudaSurfaceObject_t so : held[i].surfs) cudaDestroySurfaceObject(so);
+      ctx->spare_events.push_back(held[i].done);
+    } else {
+      if (keep != i) held[keep] = std::move(held[i]);
+      ++keep;
+    }
+  }
+  held.resize(keep);
+}
+
+// The surface objects one call creates for its GS_MEM_ARRAY images.  When the call returns they are handed to the context behind
+// an event recorded on its stream after their last use.  They are never cached by cudaArray_t value: a freed array's handle can be
+// reused by the next allocation.
+class CallSurfaces {
+ public:
+  explicit CallSurfaces(GsContext *ctx) : ctx_(ctx) {}
+  CallSurfaces(const CallSurfaces &) = delete;
+  CallSurfaces &operator=(const CallSurfaces &) = delete;
+  ~CallSurfaces() {
+    if (made_.empty()) return;
+    cudaEvent_t ev = nullptr;
+    if (!ctx_->spare_events.empty()) { ev = ctx_->spare_events.back(); ctx_->spare_events.pop_back(); }
+    else if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) ev = nullptr;
+    if (ev && cudaEventRecord(ev, ctx_->stream) == cudaSuccess) {
+      ctx_->held_surfaces.push_back({ev, std::move(made_)});
+      return;
+    }
+    cudaStreamSynchronize(ctx_->stream);   // no event to wait for: wait for the stream itself
+    for (cudaSurfaceObject_t so : made_) cudaDestroySurfaceObject(so);
+    if (ev) ctx_->spare_events.push_back(ev);
+  }
+  // `im` has passed image_ok as a GS_MEM_ARRAY image
+  int make(const GsImage *im, cudaSurfaceObject_t *out) {
+    if (made_.empty()) release_surfaces(ctx_, false);
+    cudaResourceDesc rd;
+    memset(&rd, 0, sizeof(rd));
+    rd.resType = cudaResourceTypeArray;
+    rd.res.array.array = static_cast<cudaArray_t>(im->data);
+    GS_CUDA_TRY(ctx_, cudaCreateSurfaceObject(out, &rd));
+    made_.push_back(*out);
+    return GS_OK;
+  }
+
+ private:
+  GsContext *ctx_;
+  std::vector<cudaSurfaceObject_t> made_;
+};
+
 int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t stream) {
   if (fp->cutouts && fp->cutout_count) {
     if (fp->cutout_count > ctx->cutout_cap) {
@@ -299,7 +360,7 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
 
 // binning + raster into a device image
 int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRenderOptions &opt, void *d_rt, uint32_t pitch,
-                     uint32_t fmt) {
+                     uint32_t fmt, cudaSurfaceObject_t surf) {
   GsNvtxRange nvtx("GaussianSplat.Draw");
   const uint32_t tiles = fc.binsX * fc.binsY;
   int rc = ensure_bin_scratch(ctx, as->av.n, tiles, 0);
@@ -326,7 +387,7 @@ int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRender
   GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->av.n, as->order, as->rect, as->block_bits, ctx->bin, ctx->sort, ctx->stream, &lists,
                                   &bin_launches));
   rec(ctx, EV_BIN1);
-  launch_raster(fc, opt, as->draw, lists, d_rt, pitch, fmt, ctx->stream, ctx->cur_depth ? as->zndc : nullptr, ctx->cur_depth);
+  launch_raster(fc, opt, as->draw, lists, d_rt, pitch, fmt, surf, ctx->stream, ctx->cur_depth ? as->zndc : nullptr, ctx->cur_depth);
   rec(ctx, EV_RASTER1);
   ctx->launches += bin_launches + 3;  // bin_emit, look-back clear, 1-2 sort passes; bin_ranges, tile_order, raster
   GS_CUDA_TRY(ctx, cudaGetLastError());
@@ -337,7 +398,25 @@ int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRender
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch) {
   if (!im || !im->data) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image is null");
   if (im->format > GS_PIX_RGBA32F) return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "unsupported pixel format");
+  if (im->memory > GS_MEM_ARRAY) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "unknown image memory kind");
   if (im->width != W || im->height != H) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image size does not match screen size");
+  if (im->memory == GS_MEM_ARRAY) {   // a 2-D CUDA array: data is a cudaArray_t
+    if (im->row_pitch_bytes) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "row_pitch_bytes must be 0 for a CUDA array image");
+    cudaChannelFormatDesc cd;
+    cudaExtent ext;
+    unsigned int flags = 0;
+    const cudaError_t e = cudaArrayGetInfo(&cd, &ext, &flags, static_cast<cudaArray_t>(im->data));
+    if (e != cudaSuccess) { cudaGetLastError(); return fail(ctx, GS_ERR_INVALID_ARGUMENT, std::string("not a CUDA array: ") + cudaGetErrorString(e)); }
+    const int bits = im->format == GS_PIX_RGBA16F ? 16 : 32;
+    if (cd.f != cudaChannelFormatKindFloat || cd.x != bits || cd.y != bits || cd.z != bits || cd.w != bits)
+      return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "the CUDA array's channel format does not match the image's pixel format");
+    if (ext.width != W || ext.height != H || ext.depth != 0)
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array is not a 2-D array of the image's size");
+    if (!(flags & cudaArraySurfaceLoadStore))
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array was not created with cudaArraySurfaceLoadStore");
+    *pitch = 0;
+    return GS_OK;
+  }
   uint32_t p = im->row_pitch_bytes ? im->row_pitch_bytes : W * pix_bytes(im->format);
   if (p < W * pix_bytes(im->format) || (p % pix_bytes(im->format)) != 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "bad row pitch");
   *pitch = p;
@@ -466,6 +545,8 @@ void gs_destroy(GsContext *ctx) {
     if (ctx->ev_copy_done[i]) cudaEventDestroy(ctx->ev_copy_done[i]);
   }
   for (int i = 0; i < EV_COUNT; ++i) if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
+  release_surfaces(ctx, true);   // the stream is idle (synchronised above)
+  for (cudaEvent_t e : ctx->spare_events) cudaEventDestroy(e);
   if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
 }
@@ -479,6 +560,8 @@ int gs_sync(GsContext *ctx) {
     GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->copy_stream));
     ctx->copy_pending[0] = ctx->copy_pending[1] = false;
   }
+  GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  release_surfaces(ctx, true);
   return rc;
 }
 
@@ -611,12 +694,20 @@ int gs_render(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRend
       return fail(ctx, GS_ERR_NOT_READY, "the last gs_frame prepared draw records for another tile partition; run gs_calc_view");
   }
   const uint32_t H = opt.band_packed ? partition_own_bin_rows(opt, fc.binsY) * kBin : (uint32_t)fp->screen_h;
+  if (opt.band_packed && rt && rt->memory == GS_MEM_ARRAY)
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, "band_packed output is the send buffer of an all-gather: it must be linear memory, not a CUDA array");
   if ((rc = image_ok(ctx, rt, W, H, &pitch))) return rc;
   for (int e = EV_BIN1; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
   if ((rc = bind_depth(ctx, fp, ctx->stream))) return rc;
   if (ctx->cur_depth && !as->zndc_valid) return fail(ctx, GS_ERR_NOT_READY, "a scene depth buffer needs the quad depths: run gs_calc_view with scene_depth set");
   rec(ctx, EV_VIEW1);
   if (rt->memory == GS_MEM_DEVICE) return do_render(ctx, as, fc, opt, rt->data, pitch, rt->format);
+  if (rt->memory == GS_MEM_ARRAY) {
+    CallSurfaces surfs(ctx);
+    cudaSurfaceObject_t so = 0;
+    if ((rc = surfs.make(rt, &so))) return rc;
+    return do_render(ctx, as, fc, opt, nullptr, 0, rt->format, so);
+  }
   const uint32_t tight = W * pix_bytes(rt->format);
   if ((rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)tight * H))) return rc;
   if ((rc = init_staging(ctx, opt, ctx->rt_scratch, tight, W, H, rt->format, rt, pitch))) return rc;
@@ -625,40 +716,53 @@ int gs_render(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRend
   return check_bin_overflow(ctx);
 }
 
-static int composite_impl(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H) {
+// d_rt == nullptr: the render target is the CUDA array behind rt_surf
+static int composite_impl(GsContext *ctx, CallSurfaces &surfs, const void *d_rt, uint32_t rt_pitch, cudaSurfaceObject_t rt_surf,
+                          uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H) {
   GsNvtxRange nvtx("GaussianSplat.Compose");
   uint32_t tp = 0;
   int rc = image_ok(ctx, tgt, W, H, &tp);
   if (rc) return rc;
   if (tgt->memory == GS_MEM_DEVICE) {
-    launch_composite(d_rt, rt_pitch, rt_fmt, tgt->data, tp, tgt->format, W, H, ctx->stream);
+    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, tgt->data, tp, 0, tgt->format, W, H, ctx->stream);
+  } else if (tgt->memory == GS_MEM_ARRAY) {
+    cudaSurfaceObject_t so = 0;
+    if ((rc = surfs.make(tgt, &so))) return rc;
+    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, nullptr, 0, so, tgt->format, W, H, ctx->stream);
   } else {
     const uint32_t tight = W * pix_bytes(tgt->format);
     if ((rc = grow(ctx, &ctx->tgt_scratch, &ctx->tgt_bytes, (size_t)tight * H))) return rc;
     GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->tgt_scratch, tight, tgt->data, tp, tight, H, cudaMemcpyHostToDevice, ctx->stream));
-    launch_composite(d_rt, rt_pitch, rt_fmt, ctx->tgt_scratch, tight, tgt->format, W, H, ctx->stream);
+    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, ctx->tgt_scratch, tight, 0, tgt->format, W, H, ctx->stream);
     GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(tgt->data, tp, ctx->tgt_scratch, tight, tight, H, cudaMemcpyDeviceToHost, ctx->stream));
   }
   rec(ctx, EV_COMP1);
   ctx->launches += 1;
   GS_CUDA_TRY(ctx, cudaGetLastError());
-  if (tgt->memory != GS_MEM_DEVICE) GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (tgt->memory == GS_MEM_HOST) GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return GS_OK;
 }
 
 int gs_composite(GsContext *ctx, const GsImage *rt, GsImage *tgt) {
   if (!ctx || !rt || !tgt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null argument");
+  GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));   // array images are inspected and bound on the context's device
   uint32_t rp = 0;
   int rc = image_ok(ctx, rt, rt->width, rt->height, &rp);
   if (rc) return rc;
   const uint32_t W = rt->width, H = rt->height;
   ctx->ev_valid[EV_COMP1] = false;
   rec(ctx, EV_RASTER1);
-  if (rt->memory == GS_MEM_DEVICE) return composite_impl(ctx, rt->data, rp, rt->format, tgt, W, H);
+  CallSurfaces surfs(ctx);
+  if (rt->memory == GS_MEM_DEVICE) return composite_impl(ctx, surfs, rt->data, rp, 0, rt->format, tgt, W, H);
+  if (rt->memory == GS_MEM_ARRAY) {
+    cudaSurfaceObject_t so = 0;
+    if ((rc = surfs.make(rt, &so))) return rc;
+    return composite_impl(ctx, surfs, nullptr, 0, so, rt->format, tgt, W, H);
+  }
   const uint32_t tight = W * pix_bytes(rt->format);
   if ((rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)tight * H))) return rc;
   GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->rt_scratch, tight, rt->data, rp, tight, H, cudaMemcpyHostToDevice, ctx->stream));
-  return composite_impl(ctx, ctx->rt_scratch, tight, rt->format, tgt, W, H);
+  return composite_impl(ctx, surfs, ctx->rt_scratch, tight, 0, rt->format, tgt, W, H);
 }
 
 int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRenderOptions *opt_in, int do_sort_flag, GsImage *rt,
@@ -673,17 +777,24 @@ int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRende
   if ((rc = check_options(ctx, fc, opt))) return rc;
   const uint32_t H = opt.band_packed ? partition_own_bin_rows(opt, fc.binsY) * kBin : (uint32_t)fp->screen_h;
   if (opt.band_packed && tgt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "band_packed output cannot be composited before the gather");
+  if (opt.band_packed && rt && rt->memory == GS_MEM_ARRAY)
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, "band_packed output is the send buffer of an all-gather: it must be linear memory, not a CUDA array");
   if (rt) { if ((rc = image_ok(ctx, rt, W, H, &rt_pitch))) return rc; rt_fmt = rt->format; }
   for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
   if (do_sort_flag && (rc = do_sort(ctx, as, fc))) return rc;
   if ((rc = do_view(ctx, as, fp, fc, true, opt, ctx->stream))) return rc;   // fused frame: colour of never-drawn splats is dead code
   void *d_rt;
   uint32_t d_pitch;
-  const bool rt_dev = rt && rt->memory == GS_MEM_DEVICE;
-  const bool async_rb = rt && !rt_dev && !tgt && (opt.flags & GS_FLAG_ASYNC_READBACK) != 0;
+  cudaSurfaceObject_t rt_surf = 0;
+  CallSurfaces surfs(ctx);
+  const bool rt_dev = rt && rt->memory == GS_MEM_DEVICE, rt_arr = rt && rt->memory == GS_MEM_ARRAY, rt_host = rt && rt->memory == GS_MEM_HOST;
+  const bool async_rb = rt_host && !tgt && (opt.flags & GS_FLAG_ASYNC_READBACK) != 0;
   int slot = 0;
   if (rt_dev) { d_rt = rt->data; d_pitch = rt_pitch; }
-  else if (async_rb) {
+  else if (rt_arr) {   // rendered into in place, through a surface
+    d_rt = nullptr; d_pitch = 0;
+    if ((rc = surfs.make(rt, &rt_surf))) return rc;
+  } else if (async_rb) {
     if ((rc = ensure_async_readback(ctx))) return rc;
     slot = ctx->rt_flip;
     ctx->rt_flip ^= 1;
@@ -701,7 +812,7 @@ int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRende
     if ((rc = init_staging(ctx, opt, d_rt, d_pitch, W, H, rt_fmt, rt, rt_pitch))) return rc;
   }
   if ((rc = bind_depth(ctx, fp, ctx->stream))) return rc;
-  if ((rc = do_render(ctx, as, fc, opt, d_rt, d_pitch, rt_fmt))) return rc;
+  if ((rc = do_render(ctx, as, fc, opt, d_rt, d_pitch, rt_fmt, rt_surf))) return rc;
   bool synced = false;
   if (async_rb) {
     GS_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_rt_ready[slot], ctx->stream));
@@ -711,20 +822,21 @@ int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRende
     ctx->copy_pending[slot] = true;
     return GS_OK;   // completion and the bin-list check: gs_sync
   }
-  if (rt && !rt_dev) {
+  if (rt_host) {
     GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, rt_pitch, d_rt, d_pitch, (size_t)W * pix_bytes(rt_fmt), H, cudaMemcpyDeviceToHost, ctx->stream));
   }
   if (tgt) {
-    if ((rc = composite_impl(ctx, d_rt, d_pitch, rt_fmt, tgt, W, H))) return rc;
-    synced = tgt->memory != GS_MEM_DEVICE;
+    if ((rc = composite_impl(ctx, surfs, d_rt, d_pitch, rt_surf, rt_fmt, tgt, W, H))) return rc;
+    synced = tgt->memory == GS_MEM_HOST;
   }
-  if ((rt && !rt_dev) || synced) return check_bin_overflow(ctx);
+  if (rt_host || synced) return check_bin_overflow(ctx);
   return GS_OK;
 }
 
 int gs_unshuffle_bands(GsContext *ctx, const void *gathered, uint32_t parts, uint32_t band_rows, uint32_t rows_pp, uint32_t fmt,
                        GsImage *out) {
   if (!ctx || !gathered || !out || parts == 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null argument");
+  if (out->memory == GS_MEM_ARRAY) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_unshuffle_bands writes host or linear device memory, not a CUDA array");
   uint32_t pitch = 0;
   int rc = image_ok(ctx, out, out->width, out->height, &pitch);
   if (rc) return rc;

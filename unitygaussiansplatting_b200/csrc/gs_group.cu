@@ -776,10 +776,13 @@ int gs_group_frame(GsGroup *g, GsAsset *const *assets, const GsFrameParams *fp, 
     GS_CUDA_TRY(ctx, cudaMemcpyAsync(mb.h_row_cost[slot], mb.d_row_cost, (size_t)rows * 4, cudaMemcpyDeviceToHost, mb.xfer));
     GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_cost[slot], mb.xfer));
     GsImage *rt = rts ? rts[i] : nullptr;
-    if (rt && rt->memory != GS_MEM_DEVICE) {
+    if (rt && rt->memory == GS_MEM_HOST) {
       const uint32_t hp = rt->row_pitch_bytes ? rt->row_pitch_bytes : W * pix_bytes(fmt);
       GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, hp, img[i], pitches[i], (size_t)W * pix_bytes(fmt), H, cudaMemcpyDeviceToHost, mb.xfer));
       host_out = true;
+    } else if (rt && rt->memory == GS_MEM_ARRAY) {   // e.g. the display GPU's imported render texture: one copy of the assembled frame
+      GS_CUDA_TRY(ctx, cudaMemcpy2DToArrayAsync(static_cast<cudaArray_t>(rt->data), 0, 0, img[i], pitches[i], (size_t)W * pix_bytes(fmt), H,
+                                                cudaMemcpyDeviceToDevice, mb.xfer));
     }
     GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_image, mb.xfer));
     mb.image_pending = true;

@@ -2,6 +2,7 @@
 // the context / asset objects and the per-stage drivers.
 #pragma once
 #include <string>
+#include <vector>
 
 #include <nvtx3/nvToolsExt.h>   // header-only; costs one predicted-not-taken branch per range when no tool is attached
 
@@ -66,6 +67,14 @@ struct GsContext {
   const float *cur_depth = nullptr;  // what the compositor tests against this frame (nullptr: no depth test)
   uint32_t launches = 0;
   uint64_t pack_stats[4] = {0, 0, 0, 0};   // gs_debug_pack_stats
+  // surface objects of GS_MEM_ARRAY images, one per array per call: each batch is destroyed once `done` (recorded behind the
+  // call's last use on `stream`) has completed, or at gs_sync / gs_destroy
+  struct HeldSurfaces {
+    cudaEvent_t done;
+    std::vector<cudaSurfaceObject_t> surfs;
+  };
+  std::vector<HeldSurfaces> held_surfaces;
+  std::vector<cudaEvent_t> spare_events;
 };
 
 struct GsAsset {
@@ -96,7 +105,9 @@ int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cu
 int bind_depth(GsContext *ctx, const GsFrameParams *fp, cudaStream_t stream);   // sets ctx->cur_depth for the draw that follows
 int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameConsts &fc, bool cull, const GsRenderOptions &opt,
             cudaStream_t stream);
-int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRenderOptions &opt, void *d_rt, uint32_t pitch, uint32_t fmt);
+// d_rt == nullptr: the target is the CUDA array behind `surf`
+int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRenderOptions &opt, void *d_rt, uint32_t pitch, uint32_t fmt,
+              cudaSurfaceObject_t surf = 0);
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch);
 uint32_t pix_bytes(uint32_t fmt);
 // The per-asset work buffers (order, keys, view data, ...) of an asset whose blobs as->d_* are already in HBM, the format

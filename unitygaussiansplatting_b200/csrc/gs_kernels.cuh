@@ -179,15 +179,17 @@ struct BinScratch {
 cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, uint32_t n, const uint32_t *order, const uint32_t *rect,
                            const uint32_t *block_bits, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted,
                            int *launches);
-// zndc / scene_depth: per-splat quad depth and the W x H depth buffer to test it against (both nullptr: no depth test)
+// zndc / scene_depth: per-splat quad depth and the W x H depth buffer to test it against (both nullptr: no depth test).
+// Images here are linear device memory (pointer, pitch) or, when the pointer is null, a CUDA array behind a surface object.
 void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const BinScratch &bs, void *rt,
-                   uint32_t rt_pitch_bytes, uint32_t rt_format, cudaStream_t s, const float *zndc = nullptr, const float *scene_depth = nullptr);
+                   uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s, const float *zndc = nullptr,
+                   const float *scene_depth = nullptr);
 extern unsigned long long *g_raster_stats;   // diagnostics, see GS_RASTER_STATS
 uint32_t partition_own_bin_rows(const GsRenderOptions &opt, uint32_t binsY);
 uint32_t partition_own_tile_rows(const GsRenderOptions &opt, uint32_t binsY);
 void launch_unshuffle(const void *gathered, uint32_t parts, uint32_t band, uint32_t rows_pp, uint32_t fmt, void *out, uint32_t pitch,
                       uint32_t W, uint32_t H, cudaStream_t s);
-void launch_composite(const void *rt, uint32_t rt_pitch, uint32_t rt_format, void *target, uint32_t tgt_pitch, uint32_t tgt_format,
-                      uint32_t W, uint32_t H, cudaStream_t s);
+void launch_composite(const void *rt, uint32_t rt_pitch, cudaSurfaceObject_t rt_surf, uint32_t rt_format, void *target, uint32_t tgt_pitch,
+                      cudaSurfaceObject_t tgt_surf, uint32_t tgt_format, uint32_t W, uint32_t H, cudaStream_t s);
 
 }  // namespace gs

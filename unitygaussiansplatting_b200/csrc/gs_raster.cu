@@ -346,12 +346,14 @@ __device__ __forceinline__ bool block_may_touch_quad(const float4 &A, float i2x,
 // ordinary frames pay nothing.  Selected splats (records with opacity -1) take the pixel shader's other branch
 // (S/RenderGaussianSplats.shader:87-101); with `scene_depth` every fragment is depth-tested like the pass's ZTest LEqual
 // (reversed Z: quad depth >= stored depth), the per-splat quad depths being staged beside the records.
-template <bool FP16_ROP, int OUT_FMT, bool STATS, bool SEL = false>
+// SURF: the target is a CUDA array (GS_MEM_ARRAY), read and written through the surface object `surf` instead of `rt`/`pitch`; a
+// separate instantiation so that the linear ones keep their code.
+template <bool FP16_ROP, int OUT_FMT, bool STATS, bool SEL = false, bool SURF = false>
 __global__ void __launch_bounds__(256)
 k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const uint2 *__restrict__ bin_ranges,
          const uint32_t *__restrict__ tile_vals, const uint32_t *__restrict__ tile_order, uint32_t *__restrict__ tile_cost, uint32_t ntx,
-         uint8_t *__restrict__ rt, uint32_t pitch, uint32_t band_packed, uint32_t load_rt, unsigned long long *stats,
-         const float *__restrict__ zndc, const float *__restrict__ scene_depth) {
+         uint8_t *__restrict__ rt, uint32_t pitch, cudaSurfaceObject_t surf, uint32_t band_packed, uint32_t load_rt,
+         unsigned long long *stats, const float *__restrict__ zndc, const float *__restrict__ scene_depth) {
   uint32_t st_batches = 0, st_culls = 0, st_cand = 0, st_eval = 0, st_blend = 0;   // GS_RASTER_STATS diagnostics (per warp)
   unsigned long long st_t0 = 0;
   if (STATS) asm volatile("mov.u64 %0, %globaltimer;" : "=l"(st_t0));
@@ -391,10 +393,14 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
     // (R/GaussianSplatRenderer.cs:111-168 loops the active splat objects over ONE _GaussianSplatRT); blend under what is there
     const uint8_t *row = rt + (size_t)out_row * pitch;
     if (OUT_FMT == GS_PIX_RGBA16F) {
-      const uint2 v = reinterpret_cast<const uint2 *>(row)[px];
+      uint2 v;
+      if (SURF) surf2Dread(&v, surf, (int)(px * 8u), (int)out_row);
+      else v = reinterpret_cast<const uint2 *>(row)[px];
       d0 = f16lo(v.x); d1 = f16hi(v.x); d2 = f16lo(v.y); d3 = f16hi(v.y);
     } else {
-      const float4 v = reinterpret_cast<const float4 *>(row)[px];
+      float4 v;
+      if (SURF) surf2Dread(&v, surf, (int)(px * 16u), (int)out_row);
+      else v = reinterpret_cast<const float4 *>(row)[px];
       d0 = v.x; d1 = v.y; d2 = v.z; d3 = v.w;
     }
   }
@@ -514,9 +520,11 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
       uint2 o;
       o.x = f32tof16(d0) | (f32tof16(d1) << 16);
       o.y = f32tof16(d2) | (f32tof16(d3) << 16);
-      reinterpret_cast<uint2 *>(row)[px] = o;
+      if (SURF) surf2Dwrite(o, surf, (int)(px * 8u), (int)out_row);
+      else reinterpret_cast<uint2 *>(row)[px] = o;
     } else {
-      reinterpret_cast<float4 *>(row)[px] = make_float4(d0, d1, d2, d3);
+      if (SURF) surf2Dwrite(make_float4(d0, d1, d2, d3), surf, (int)(px * 16u), (int)out_row);
+      else reinterpret_cast<float4 *>(row)[px] = make_float4(d0, d1, d2, d3);
     }
   }
 }
@@ -524,7 +532,8 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
 unsigned long long *g_raster_stats = nullptr;
 
 void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const BinScratch &bs, void *rt,
-                   uint32_t rt_pitch_bytes, uint32_t rt_format, cudaStream_t s, const float *zndc, const float *scene_depth) {
+                   uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s, const float *zndc,
+                   const float *scene_depth) {
   const Partition part = make_partition(opt);
   const uint32_t rows = part.own_tile_rows(fc.binsY);
   if (!rows || !fc.binsX) return;
@@ -543,17 +552,23 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const floa
   uint2 *ranges = reinterpret_cast<uint2 *>(bs.bin_ranges);
   const uint32_t packed = part.range ? 0u : opt.band_packed, load = (opt.flags & GS_FLAG_LOAD_RT) ? 1u : 0u;
   k_bin_ranges<<<(bins + 7) / 8, 256, 0, s>>>(bs.tile_keys, bs.entry_count, bins, ranges);
-#define GS_LAUNCH_RASTER(ROP, FMT)                                                                                              \
+#define GS_LAUNCH_RASTER(ROP, FMT, SURF)                                                                                        \
   do {                                                                                                                         \
-    if (fc.selValid || scene_depth) k_raster<ROP, FMT, false, true><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, packed, load, stats, zndc, scene_depth); \
-    else if (stats) k_raster<ROP, FMT, true><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, packed, load, stats, nullptr, nullptr); \
-    else k_raster<ROP, FMT, false><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, packed, load, stats, nullptr, nullptr); \
+    if (fc.selValid || scene_depth) k_raster<ROP, FMT, false, true, SURF><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed, load, stats, zndc, scene_depth); \
+    else if (stats) k_raster<ROP, FMT, true, false, SURF><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed, load, stats, nullptr, nullptr); \
+    else k_raster<ROP, FMT, false, false, SURF><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed, load, stats, nullptr, nullptr); \
+  } while (0)
+  // a null `rt` means the target is a CUDA array behind rt_surf
+#define GS_LAUNCH_RASTER_TARGET(ROP, FMT)                                                                                       \
+  do {                                                                                                                         \
+    if (out) GS_LAUNCH_RASTER(ROP, FMT, false); else GS_LAUNCH_RASTER(ROP, FMT, true);                                          \
   } while (0)
   if (rt_format == GS_PIX_RGBA16F) {
-    if (rop) GS_LAUNCH_RASTER(true, GS_PIX_RGBA16F); else GS_LAUNCH_RASTER(false, GS_PIX_RGBA16F);
+    if (rop) GS_LAUNCH_RASTER_TARGET(true, GS_PIX_RGBA16F); else GS_LAUNCH_RASTER_TARGET(false, GS_PIX_RGBA16F);
   } else {
-    if (rop) GS_LAUNCH_RASTER(true, GS_PIX_RGBA32F); else GS_LAUNCH_RASTER(false, GS_PIX_RGBA32F);
+    if (rop) GS_LAUNCH_RASTER_TARGET(true, GS_PIX_RGBA32F); else GS_LAUNCH_RASTER_TARGET(false, GS_PIX_RGBA32F);
   }
+#undef GS_LAUNCH_RASTER_TARGET
 #undef GS_LAUNCH_RASTER
 }
 
@@ -588,26 +603,28 @@ __device__ __forceinline__ float gamma_to_linear(float x) {  // UnityCG.cginc Ga
   return x * fmaf(x, fmaf(x, 0.305306011f, 0.682171111f), 0.012522878f);
 }
 
-__global__ void __launch_bounds__(256) k_composite(const uint8_t *__restrict__ rt, uint32_t rt_pitch, uint32_t rt_fmt,
-                                                   uint8_t *__restrict__ tgt, uint32_t tgt_pitch, uint32_t tgt_fmt, uint32_t W,
-                                                   uint32_t H) {
+// one pixel of an RGBA16F / RGBA32F image: linear memory at (base, pitch), or, when base is null, a CUDA array behind `surf`
+__device__ __forceinline__ float4 load_px(const uint8_t *base, uint32_t pitch, cudaSurfaceObject_t surf, uint32_t fmt, uint32_t x, uint32_t y) {
+  if (fmt == GS_PIX_RGBA16F) {
+    uint2 v;
+    if (base) v = reinterpret_cast<const uint2 *>(base + (size_t)y * pitch)[x];
+    else surf2Dread(&v, surf, (int)(x * 8u), (int)y);
+    return make_float4(f16lo(v.x), f16hi(v.x), f16lo(v.y), f16hi(v.y));
+  }
+  float4 c;
+  if (base) c = reinterpret_cast<const float4 *>(base + (size_t)y * pitch)[x];
+  else surf2Dread(&c, surf, (int)(x * 16u), (int)y);
+  return c;
+}
+
+__global__ void __launch_bounds__(256) k_composite(const uint8_t *__restrict__ rt, uint32_t rt_pitch, cudaSurfaceObject_t rt_surf,
+                                                   uint32_t rt_fmt, uint8_t *__restrict__ tgt, uint32_t tgt_pitch,
+                                                   cudaSurfaceObject_t tgt_surf, uint32_t tgt_fmt, uint32_t W, uint32_t H) {
   const uint32_t x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= W || y >= H) return;
-  float4 c;
-  if (rt_fmt == GS_PIX_RGBA16F) {
-    uint2 v = reinterpret_cast<const uint2 *>(rt + (size_t)y * rt_pitch)[x];
-    c = make_float4(f16lo(v.x), f16hi(v.x), f16lo(v.y), f16hi(v.y));
-  } else {
-    c = reinterpret_cast<const float4 *>(rt + (size_t)y * rt_pitch)[x];
-  }
+  const float4 c = load_px(rt, rt_pitch, rt_surf, rt_fmt, x, y);
   if (!(c.w > 0.0f)) return;  // SrcAlpha == 0 leaves the target untouched
-  float4 d;
-  if (tgt_fmt == GS_PIX_RGBA16F) {
-    uint2 v = reinterpret_cast<const uint2 *>(tgt + (size_t)y * tgt_pitch)[x];
-    d = make_float4(f16lo(v.x), f16hi(v.x), f16lo(v.y), f16hi(v.y));
-  } else {
-    d = reinterpret_cast<const float4 *>(tgt + (size_t)y * tgt_pitch)[x];
-  }
+  const float4 d = load_px(tgt, tgt_pitch, tgt_surf, tgt_fmt, x, y);
   const float a = c.w, om = 1.0f - a;
   float4 o;
   o.x = fmaf(gamma_to_linear(__fdiv_rn(c.x, a)), a, d.x * om);
@@ -618,18 +635,20 @@ __global__ void __launch_bounds__(256) k_composite(const uint8_t *__restrict__ r
     uint2 v;
     v.x = f32tof16(o.x) | (f32tof16(o.y) << 16);
     v.y = f32tof16(o.z) | (f32tof16(o.w) << 16);
-    reinterpret_cast<uint2 *>(tgt + (size_t)y * tgt_pitch)[x] = v;
+    if (tgt) reinterpret_cast<uint2 *>(tgt + (size_t)y * tgt_pitch)[x] = v;
+    else surf2Dwrite(v, tgt_surf, (int)(x * 8u), (int)y);
   } else {
-    reinterpret_cast<float4 *>(tgt + (size_t)y * tgt_pitch)[x] = o;
+    if (tgt) reinterpret_cast<float4 *>(tgt + (size_t)y * tgt_pitch)[x] = o;
+    else surf2Dwrite(o, tgt_surf, (int)(x * 16u), (int)y);
   }
 }
 
-void launch_composite(const void *rt, uint32_t rt_pitch, uint32_t rt_format, void *target, uint32_t tgt_pitch, uint32_t tgt_format,
-                      uint32_t W, uint32_t H, cudaStream_t s) {
+void launch_composite(const void *rt, uint32_t rt_pitch, cudaSurfaceObject_t rt_surf, uint32_t rt_format, void *target, uint32_t tgt_pitch,
+                      cudaSurfaceObject_t tgt_surf, uint32_t tgt_format, uint32_t W, uint32_t H, cudaStream_t s) {
   if (!W || !H) return;
   dim3 grid((W + 31) / 32, (H + 7) / 8);
-  k_composite<<<grid, 256, 0, s>>>(reinterpret_cast<const uint8_t *>(rt), rt_pitch, rt_format, reinterpret_cast<uint8_t *>(target),
-                                   tgt_pitch, tgt_format, W, H);
+  k_composite<<<grid, 256, 0, s>>>(reinterpret_cast<const uint8_t *>(rt), rt_pitch, rt_surf, rt_format, reinterpret_cast<uint8_t *>(target),
+                                   tgt_pitch, tgt_surf, tgt_format, W, H);
 }
 
 }  // namespace gs

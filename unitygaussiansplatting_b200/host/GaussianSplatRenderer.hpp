@@ -21,6 +21,21 @@ struct CameraState {               // what the C# code reads from UnityEngine.Ca
   float position[3];               // :592
 };
 
+// An image that is a 2-D CUDA array (GS_MEM_ARRAY): `array` is the cudaArray_t of RGBA16F / RGBA32F texels, created with
+// cudaArraySurfaceLoadStore -- e.g. the render texture a graphics-interop plugin imported (cudaExternalMemoryGetMappedMipmappedArray,
+// level 0).  It is rendered into / composited onto in place.
+inline GsImage ArrayImage(void *array, uint32_t width, uint32_t height, uint32_t format = GS_PIX_RGBA16F) {
+  GsImage im;
+  std::memset(&im, 0, sizeof(im));
+  im.data = array;
+  im.width = width;
+  im.height = height;
+  im.row_pitch_bytes = 0;
+  im.format = format;
+  im.memory = GS_MEM_ARRAY;
+  return im;
+}
+
 class GaussianSplatRenderer {
  public:
   // serialized knobs, :225-251
@@ -127,7 +142,7 @@ class GaussianSplatRendererGroup {
     if (m_Group) gs_group_destroy(m_Group);
     m_Group = nullptr;
   }
-  // rts[i]: the image of local member i (device or host memory) or nullptr
+  // rts[i]: the image of local member i (device, host or CUDA-array memory) or nullptr
   bool SortAndRenderSplats(const CameraState &cam, GsImage *const *rts) {
     const int doSort = (m_FrameCounter % (m_SortNthFrame > 0 ? m_SortNthFrame : 1)) == 0;
     ++m_FrameCounter;

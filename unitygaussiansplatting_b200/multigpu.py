@@ -183,7 +183,8 @@ class GaussianSplatGroup:
         return fp
 
     def SortAndRenderSplats(self, cam, rts=None, fp=None):
-        """rts: one image per LOCAL member (numpy host array, torch CUDA tensor, or None); each receives the whole frame."""
+        """rts: one image per LOCAL member (numpy host array, torch CUDA tensor, CudaArrayImage, or None); each receives the
+        whole frame."""
         from .renderer import _image
         do_sort = 1 if (self.m_FrameCounter % max(1, int(self.m_SortNthFrame)) == 0) else 0
         self.m_FrameCounter += 1

@@ -83,10 +83,33 @@ class GaussianSplatContext:
             pass
 
 
+class CudaArrayImage:
+    """A 2-D CUDA array (cudaArray_t, e.g. an imported graphics render texture) of RGBA float16 or float32 texels, given to the
+    library as an image (GS_MEM_ARRAY): it is rendered into / composited onto in place.  The host creates the array, with
+    cudaArraySurfaceLoadStore, and keeps it alive; the library never allocates or frees one."""
+
+    def __init__(self, handle: int, width: int, height: int, dtype=np.float16):
+        self.handle = int(handle)
+        self.width, self.height = int(width), int(height)
+        self.dtype = np.dtype(dtype)
+        if self.dtype not in (np.float16, np.float32):
+            raise ValueError("CudaArrayImage dtype must be float16 or float32")
+
+    @property
+    def shape(self):
+        return (self.height, self.width, 4)
+
+
 def _image(arr, width: int, height: int) -> N.GsImage:
-    """numpy (host) array or torch CUDA tensor of shape (H, W, 4), float16/float32 -> GsImage."""
+    """numpy (host) array or torch CUDA tensor of shape (H, W, 4), float16/float32, or a CudaArrayImage -> GsImage."""
     im = N.GsImage()
     im.width, im.height = width, height
+    if isinstance(arr, CudaArrayImage):
+        if arr.shape != (height, width, 4):
+            raise ValueError("CUDA array is %dx%d, the image must be %dx%d" % (arr.width, arr.height, width, height))
+        im.format = N.GS_PIX_RGBA16F if arr.dtype == np.float16 else N.GS_PIX_RGBA32F
+        im.data, im.memory, im.row_pitch_bytes = arr.handle, N.GS_MEM_ARRAY, 0
+        return im
     if isinstance(arr, np.ndarray):
         if arr.shape != (height, width, 4) or not arr.flags.c_contiguous:
             raise ValueError("image must be C-contiguous (H, W, 4)")
