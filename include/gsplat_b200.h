@@ -291,11 +291,45 @@ GS_API int gs_group_asset_upload(GsGroup *group, const GsAssetDesc *desc, GsAsse
  * group must call it with the same parameters. */
 GS_API int gs_group_frame(GsGroup *group, GsAsset *const *assets, const GsFrameParams *fp, const GsRenderOptions *opt, int do_sort,
                           GsImage *const *rts);
+/* One camera's frame with several splat objects on the group: OnPreCullCamera (R/GaussianSplatRenderer.cs:187-211) -- the
+ * render target cleared once, every active object sorted, view-calculated and drawn into it in the caller's order
+ * (GatherSplatsForCamera, :73-105, loop :111-168), then the composite onto the camera target.  Every member ends with exactly
+ * what one GPU leaves after gs_frame per object (GS_FLAG_LOAD_RT from the second on) and gs_composite.
+ *   assets          [object_count][local_count]: object k's asset on local member i is assets[k * local_count + i]
+ *                   (each uploaded with gs_group_asset_upload; an asset may appear in one object only);
+ *   fps, do_sort    [object_count]: each object's uniforms (transform, knobs, bits, cutouts, scene depth) and its
+ *                   m_FrameCounter % m_SortNthFrame == 0.  All objects must share screen_w / screen_h;
+ *   opt             blend_mode and GS_FLAG_ASYNC_READBACK, as gs_group_frame; GS_FLAG_LOAD_RT is refused;
+ *   rts             as gs_group_frame;
+ *   camera_targets  [local_count], may be NULL or hold NULLs: member i's camera target (host, device or CUDA-array memory,
+ *                   width x height) receives the composite pass of the assembled frame, on the member's transfer stream after
+ *                   the row exchange.  A device or array target is complete after gs_group_sync (or before the next call's
+ *                   draw touches the image); a host target is complete when the call returns.  gs_sync on a member's
+ *                   context also waits for that member's composite onto a CUDA-array camera target.
+ * Per call: each object is sorted with its own splitters, slab table and order exchange (its order persists in its asset);
+ * all objects' distance kernels and view-calcs are queued first and the host waits once for all slab tables.  Each object
+ * blends under the earlier ones on the member's own rows; there is ONE row split (balanced on the summed measured cost of the
+ * objects) and ONE row exchange per call.  After gs_group_join only the first object ever sorted on the group uses the
+ * peer-to-peer order exchange; the others use the all-gather or in-place exchange.  GsGroupStats of such a call: the times
+ * span the whole call (slab_sort_ms runs to the end of the last object's slab sort, order_exchange_ms is its exchange,
+ * bin_ms sums every object's binning); slab_counts are summed over the objects the call sorted.
+ * GS_ERR_INVALID_ARGUMENT, with nothing written: a NULL group / assets / fps / do_sort, object_count 0, a NULL asset, one
+ * asset listed for two objects, members of one object holding different splat counts, objects of different screen sizes,
+ * GS_FLAG_LOAD_RT, or an image / camera target of the wrong size (bad formats: the image errors of gs_frame).
+ * gs_group_frame is this call with one object and no camera targets.  Collective, as gs_group_frame. */
+GS_API int gs_group_frame_objects(GsGroup *group, uint32_t object_count, GsAsset *const *assets, const GsFrameParams *fps,
+                                  const int32_t *do_sort, const GsRenderOptions *opt, GsImage *const *rts,
+                                  GsImage *const *camera_targets);
 GS_API int gs_group_sync(GsGroup *group);
 GS_API int gs_group_get_stats(GsGroup *group, GsGroupStats *out);
 /* The row balancer by itself (host arithmetic, no GPU): splits `rows` 16-pixel rows with the given measured costs into
  * `parts` contiguous ranges of near-equal cost; bounds_out[parts + 1], bounds_out[0] = 0, bounds_out[parts] = rows. */
 GS_API int gs_group_balance_rows(const uint32_t *row_cost, uint32_t rows, uint32_t parts, uint32_t *bounds_out);
+/* The per-row costs the last gs_group_frame / gs_group_frame_objects call measured: for every 16-pixel row, the summed
+ * raster-tile cost of all the objects it drew.  The row split two calls later is gs_group_balance_rows of this vector.
+ * row_cost_out[rows], where rows is the number of 16-pixel rows of that call's screen (else GS_ERR_INVALID_ARGUMENT).  Blocks
+ * until the vector is on the host.  GS_ERR_NOT_READY before the first call at the current screen size. */
+GS_API int gs_group_row_costs(GsGroup *group, uint32_t *row_cost_out, uint32_t rows);
 
 /* ---- stand-alone sorter (GpuSorting.Dispatch, R/GpuSorting.cs:142-198) ----------- */
 /* Stable ascending sort of `count` (uint32 key, uint32 payload) pairs in place in DEVICE

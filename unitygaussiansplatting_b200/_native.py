@@ -146,9 +146,12 @@ NATIVE_SYMBOLS = {
     "gs_group_asset_upload": (C.c_int, [C.c_void_p, C.POINTER(GsAssetDesc), C.POINTER(C.c_void_p)]),
     "gs_group_frame": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(GsFrameParams), C.POINTER(GsRenderOptions), C.c_int,
                                  C.POINTER(C.POINTER(GsImage))]),
+    "gs_group_frame_objects": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(GsFrameParams), C.POINTER(C.c_int32),
+                                         C.POINTER(GsRenderOptions), C.POINTER(C.POINTER(GsImage)), C.POINTER(C.POINTER(GsImage))]),
     "gs_group_sync": (C.c_int, [C.c_void_p]),
     "gs_group_get_stats": (C.c_int, [C.c_void_p, C.POINTER(GsGroupStats)]),
     "gs_group_balance_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
+    "gs_group_row_costs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32]),
     "gs_sort_pairs_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
     "gs_sort_pairs_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
     "gs_readback_order": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -185,13 +185,17 @@ static int ensure_async_readback(GsContext *ctx) {
 uint32_t pix_bytes(uint32_t fmt) { return fmt == GS_PIX_RGBA16F ? 8u : 16u; }
 
 // ---- GS_MEM_ARRAY images -----------------------------------------------------------------------------
-// Destroys the held surface objects whose last use has completed (every one when `all`: the caller has synchronised the stream).
+// Destroys the held surface objects whose last use has completed; with `all`, every one, after waiting for its event.  The
+// event, not the context stream, is what guards a batch: the group path composites onto CUDA-array camera targets on a
+// member's transfer stream, which the context stream never waits for.
 static void release_surfaces(GsContext *ctx, bool all) {
   auto &held = ctx->held_surfaces;
   size_t keep = 0;
   for (size_t i = 0; i < held.size(); ++i) {
     bool done = all;
-    if (!done) {
+    if (all) {
+      if (cudaEventSynchronize(held[i].done) != cudaSuccess) cudaGetLastError();   // failed: nothing will use the surfaces any more
+    } else {
       const cudaError_t q = cudaEventQuery(held[i].done);
       done = q != cudaErrorNotReady;   // completed, or failed: either way nothing will use the surfaces any more
       if (!done && cudaPeekAtLastError() == cudaErrorNotReady) cudaGetLastError();
@@ -208,11 +212,11 @@ static void release_surfaces(GsContext *ctx, bool all) {
 }
 
 // The surface objects one call creates for its GS_MEM_ARRAY images.  When the call returns they are handed to the context behind
-// an event recorded on its stream after their last use.  They are never cached by cudaArray_t value: a freed array's handle can be
-// reused by the next allocation.
+// an event recorded on the stream that used them (the context's, unless another is named) after their last use.  They are never
+// cached by cudaArray_t value: a freed array's handle can be reused by the next allocation.
 class CallSurfaces {
  public:
-  explicit CallSurfaces(GsContext *ctx) : ctx_(ctx) {}
+  explicit CallSurfaces(GsContext *ctx, cudaStream_t stream = nullptr) : ctx_(ctx), stream_(stream ? stream : ctx->stream) {}
   CallSurfaces(const CallSurfaces &) = delete;
   CallSurfaces &operator=(const CallSurfaces &) = delete;
   ~CallSurfaces() {
@@ -220,11 +224,11 @@ class CallSurfaces {
     cudaEvent_t ev = nullptr;
     if (!ctx_->spare_events.empty()) { ev = ctx_->spare_events.back(); ctx_->spare_events.pop_back(); }
     else if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) ev = nullptr;
-    if (ev && cudaEventRecord(ev, ctx_->stream) == cudaSuccess) {
+    if (ev && cudaEventRecord(ev, stream_) == cudaSuccess) {
       ctx_->held_surfaces.push_back({ev, std::move(made_)});
       return;
     }
-    cudaStreamSynchronize(ctx_->stream);   // no event to wait for: wait for the stream itself
+    cudaStreamSynchronize(stream_);   // no event to wait for: wait for the stream itself
     for (cudaSurfaceObject_t so : made_) cudaDestroySurfaceObject(so);
     if (ev) ctx_->spare_events.push_back(ev);
   }
@@ -242,42 +246,48 @@ class CallSurfaces {
 
  private:
   GsContext *ctx_;
+  cudaStream_t stream_;
   std::vector<cudaSurfaceObject_t> made_;
 };
 
+int reserve_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t busy) {
+  auto drain = [&]() {
+    cudaStreamSynchronize(ctx->stream);
+    if (busy) cudaStreamSynchronize(busy);
+  };
+  if (fp->cutouts && fp->cutout_count && fp->cutout_count > ctx->cutout_cap) {
+    drain();
+    cudaFree(ctx->d_cutouts);
+    ctx->d_cutouts = nullptr;
+    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->d_cutouts, sizeof(GsCutout) * fp->cutout_count));
+    ctx->cutout_cap = fp->cutout_count;
+  }
+  const size_t words = ((size_t)as->av.n + 31) / 32;
+  if (fp->deleted_bits && words > ctx->deleted_words) {
+    drain();
+    cudaFree(ctx->d_deleted);
+    ctx->d_deleted = nullptr;
+    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->d_deleted, words * 4));
+    ctx->deleted_words = words;
+  }
+  if (fp->selected_bits && words > ctx->selected_words) {
+    drain();
+    cudaFree(ctx->d_selected);
+    ctx->d_selected = nullptr;
+    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->d_selected, words * 4));
+    ctx->selected_words = words;
+  }
+  return GS_OK;
+}
+
 int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t stream) {
-  if (fp->cutouts && fp->cutout_count) {
-    if (fp->cutout_count > ctx->cutout_cap) {
-      cudaStreamSynchronize(ctx->stream);
-      cudaFree(ctx->d_cutouts);
-      ctx->d_cutouts = nullptr;
-      GS_CUDA_TRY(ctx, cudaMalloc(&ctx->d_cutouts, sizeof(GsCutout) * fp->cutout_count));
-      ctx->cutout_cap = fp->cutout_count;
-    }
+  int rc = reserve_frame_inputs(ctx, as, fp);
+  if (rc) return rc;
+  const size_t words = ((size_t)as->av.n + 31) / 32;
+  if (fp->cutouts && fp->cutout_count)
     GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_cutouts, fp->cutouts, sizeof(GsCutout) * fp->cutout_count, cudaMemcpyHostToDevice, stream));
-  }
-  if (fp->deleted_bits) {
-    size_t words = ((size_t)as->av.n + 31) / 32;
-    if (words > ctx->deleted_words) {
-      cudaStreamSynchronize(ctx->stream);
-      cudaFree(ctx->d_deleted);
-      ctx->d_deleted = nullptr;
-      GS_CUDA_TRY(ctx, cudaMalloc(&ctx->d_deleted, words * 4));
-      ctx->deleted_words = words;
-    }
-    GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_deleted, fp->deleted_bits, words * 4, cudaMemcpyHostToDevice, stream));
-  }
-  if (fp->selected_bits) {
-    size_t words = ((size_t)as->av.n + 31) / 32;
-    if (words > ctx->selected_words) {
-      cudaStreamSynchronize(ctx->stream);
-      cudaFree(ctx->d_selected);
-      ctx->d_selected = nullptr;
-      GS_CUDA_TRY(ctx, cudaMalloc(&ctx->d_selected, words * 4));
-      ctx->selected_words = words;
-    }
-    GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_selected, fp->selected_bits, words * 4, cudaMemcpyHostToDevice, stream));
-  }
+  if (fp->deleted_bits) GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_deleted, fp->deleted_bits, words * 4, cudaMemcpyHostToDevice, stream));
+  if (fp->selected_bits) GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_selected, fp->selected_bits, words * 4, cudaMemcpyHostToDevice, stream));
   return GS_OK;
 }
 
@@ -360,7 +370,7 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
 
 // binning + raster into a device image
 int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRenderOptions &opt, void *d_rt, uint32_t pitch,
-                     uint32_t fmt, cudaSurfaceObject_t surf) {
+                     uint32_t fmt, cudaSurfaceObject_t surf, cudaEvent_t bin_done) {
   GsNvtxRange nvtx("GaussianSplat.Draw");
   const uint32_t tiles = fc.binsX * fc.binsY;
   int rc = ensure_bin_scratch(ctx, as->av.n, tiles, 0);
@@ -387,6 +397,7 @@ int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRender
   GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->av.n, as->order, as->rect, as->block_bits, ctx->bin, ctx->sort, ctx->stream, &lists,
                                   &bin_launches));
   rec(ctx, EV_BIN1);
+  if (bin_done) cudaEventRecord(bin_done, ctx->stream);
   launch_raster(fc, opt, as->draw, lists, d_rt, pitch, fmt, surf, ctx->stream, ctx->cur_depth ? as->zndc : nullptr, ctx->cur_depth);
   rec(ctx, EV_RASTER1);
   ctx->launches += bin_launches + 3;  // bin_emit, look-back clear, 1-2 sort passes; bin_ranges, tile_order, raster
@@ -545,7 +556,7 @@ void gs_destroy(GsContext *ctx) {
     if (ctx->ev_copy_done[i]) cudaEventDestroy(ctx->ev_copy_done[i]);
   }
   for (int i = 0; i < EV_COUNT; ++i) if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
-  release_surfaces(ctx, true);   // the stream is idle (synchronised above)
+  release_surfaces(ctx, true);   // waits for each batch's event (a group's transfer stream may still hold one)
   for (cudaEvent_t e : ctx->spare_events) cudaEventDestroy(e);
   if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
@@ -561,7 +572,7 @@ int gs_sync(GsContext *ctx) {
     ctx->copy_pending[0] = ctx->copy_pending[1] = false;
   }
   GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  release_surfaces(ctx, true);
+  release_surfaces(ctx, true);   // also waits for surfaces a group's transfer stream still uses (camera targets)
   return rc;
 }
 
@@ -716,30 +727,31 @@ int gs_render(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRend
   return check_bin_overflow(ctx);
 }
 
-// d_rt == nullptr: the render target is the CUDA array behind rt_surf
+// d_rt == nullptr: the render target is the CUDA array behind rt_surf.  Enqueued on `s`: the context's stream, or the group
+// path's transfer stream (surfs must then hand its surfaces over on `s` as well).
 static int composite_impl(GsContext *ctx, CallSurfaces &surfs, const void *d_rt, uint32_t rt_pitch, cudaSurfaceObject_t rt_surf,
-                          uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H) {
+                          uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H, cudaStream_t s) {
   GsNvtxRange nvtx("GaussianSplat.Compose");
   uint32_t tp = 0;
   int rc = image_ok(ctx, tgt, W, H, &tp);
   if (rc) return rc;
   if (tgt->memory == GS_MEM_DEVICE) {
-    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, tgt->data, tp, 0, tgt->format, W, H, ctx->stream);
+    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, tgt->data, tp, 0, tgt->format, W, H, s);
   } else if (tgt->memory == GS_MEM_ARRAY) {
     cudaSurfaceObject_t so = 0;
     if ((rc = surfs.make(tgt, &so))) return rc;
-    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, nullptr, 0, so, tgt->format, W, H, ctx->stream);
+    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, nullptr, 0, so, tgt->format, W, H, s);
   } else {
     const uint32_t tight = W * pix_bytes(tgt->format);
     if ((rc = grow(ctx, &ctx->tgt_scratch, &ctx->tgt_bytes, (size_t)tight * H))) return rc;
-    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->tgt_scratch, tight, tgt->data, tp, tight, H, cudaMemcpyHostToDevice, ctx->stream));
-    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, ctx->tgt_scratch, tight, 0, tgt->format, W, H, ctx->stream);
-    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(tgt->data, tp, ctx->tgt_scratch, tight, tight, H, cudaMemcpyDeviceToHost, ctx->stream));
+    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->tgt_scratch, tight, tgt->data, tp, tight, H, cudaMemcpyHostToDevice, s));
+    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, ctx->tgt_scratch, tight, 0, tgt->format, W, H, s);
+    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(tgt->data, tp, ctx->tgt_scratch, tight, tight, H, cudaMemcpyDeviceToHost, s));
   }
-  rec(ctx, EV_COMP1);
+  if (s == ctx->stream) rec(ctx, EV_COMP1);
   ctx->launches += 1;
   GS_CUDA_TRY(ctx, cudaGetLastError());
-  if (tgt->memory == GS_MEM_HOST) GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (tgt->memory == GS_MEM_HOST) GS_CUDA_TRY(ctx, cudaStreamSynchronize(s));
   return GS_OK;
 }
 
@@ -753,16 +765,16 @@ int gs_composite(GsContext *ctx, const GsImage *rt, GsImage *tgt) {
   ctx->ev_valid[EV_COMP1] = false;
   rec(ctx, EV_RASTER1);
   CallSurfaces surfs(ctx);
-  if (rt->memory == GS_MEM_DEVICE) return composite_impl(ctx, surfs, rt->data, rp, 0, rt->format, tgt, W, H);
+  if (rt->memory == GS_MEM_DEVICE) return composite_impl(ctx, surfs, rt->data, rp, 0, rt->format, tgt, W, H, ctx->stream);
   if (rt->memory == GS_MEM_ARRAY) {
     cudaSurfaceObject_t so = 0;
     if ((rc = surfs.make(rt, &so))) return rc;
-    return composite_impl(ctx, surfs, nullptr, 0, so, rt->format, tgt, W, H);
+    return composite_impl(ctx, surfs, nullptr, 0, so, rt->format, tgt, W, H, ctx->stream);
   }
   const uint32_t tight = W * pix_bytes(rt->format);
   if ((rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)tight * H))) return rc;
   GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->rt_scratch, tight, rt->data, rp, tight, H, cudaMemcpyHostToDevice, ctx->stream));
-  return composite_impl(ctx, surfs, ctx->rt_scratch, tight, 0, rt->format, tgt, W, H);
+  return composite_impl(ctx, surfs, ctx->rt_scratch, tight, 0, rt->format, tgt, W, H, ctx->stream);
 }
 
 int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRenderOptions *opt_in, int do_sort_flag, GsImage *rt,
@@ -826,7 +838,7 @@ int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRende
     GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, rt_pitch, d_rt, d_pitch, (size_t)W * pix_bytes(rt_fmt), H, cudaMemcpyDeviceToHost, ctx->stream));
   }
   if (tgt) {
-    if ((rc = composite_impl(ctx, surfs, d_rt, d_pitch, rt_surf, rt_fmt, tgt, W, H))) return rc;
+    if ((rc = composite_impl(ctx, surfs, d_rt, d_pitch, rt_surf, rt_fmt, tgt, W, H, ctx->stream))) return rc;
     synced = tgt->memory == GS_MEM_HOST;
   }
   if (rt_host || synced) return check_bin_overflow(ctx);
@@ -973,3 +985,11 @@ void *gs_asset_device_ptr(GsAsset *as, int which) {
 }
 
 }  // extern "C"
+
+namespace gs {
+int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H,
+                        cudaStream_t s) {
+  CallSurfaces surfs(ctx, s);
+  return composite_impl(ctx, surfs, d_rt, rt_pitch, 0, rt_fmt, tgt, W, H, s);
+}
+}  // namespace gs

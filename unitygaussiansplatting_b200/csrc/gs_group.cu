@@ -22,6 +22,7 @@
 // one ncclAllGather of equal slots + G device copies; badly unbalanced slabs -> grouped NCCL broadcasts of the exact sizes in
 // place.  Row exchange: grouped NCCL broadcasts in place.  In GS_GROUP_EMULATE, or without NCCL in a single process, plain
 // device-to-device copies ordered by events stand in for every exchange.
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -55,8 +56,24 @@ struct Member {
   size_t cmp_words = 0;
   uint32_t rows_cap = 0;
   uint32_t *h_info = nullptr, *h_row_cost[2] = {nullptr, nullptr};   // pinned
+  uint32_t info_slots = 1;             // slab tables d_info / h_info hold: one per splat object of a call
+  uint32_t *d_ghist_more = nullptr;    // the distance kernel's digit histograms of objects 1.. of a call (object 0: the context's)
+  uint32_t ghist_more_slots = 0;
+  std::vector<cudaEvent_t> obj_tev;    // timing, per object of the last call: [2k] its draw begins, [2k + 1] its binning ends
+  uint32_t obj_timed = 0;              // objects of the last call whose draw was timed here
   void *rt_scratch = nullptr;
   size_t rt_bytes = 0;
+};
+
+// One splat object of a gs_group_frame_objects call: its assets on the local members, its uniforms, and what the call derives
+// for it (every member derives the same slab table).
+struct GroupObject {
+  GsAsset *const *assets = nullptr;   // [local_count]
+  const GsFrameParams *fp = nullptr;
+  FrameConsts fc{};
+  bool sort = false;
+  uint32_t n = 0;
+  uint32_t slab_off[GS_GROUP_MAX_GPUS + 1]{}, slab_cnt[GS_GROUP_MAX_GPUS]{};
 };
 
 }  // namespace
@@ -85,7 +102,7 @@ struct GsGroup {
   uint32_t hist_w = 0, hist_h = 0;
   uint64_t hist_frames = 0;   // frames rendered at (hist_w, hist_h): the cost of frame k is usable from frame k+2 on
   uint32_t bounds[GS_GROUP_MAX_GPUS + 1]{};
-  uint32_t slab_off[GS_GROUP_MAX_GPUS + 1]{}, slab_cnt[GS_GROUP_MAX_GPUS]{};
+  uint32_t slab_cnt[GS_GROUP_MAX_GPUS]{};   // splats each rank sorted in the last call that sorted, summed over its objects
   bool timed = false;
 };
 
@@ -134,6 +151,8 @@ void member_free(Member &mb) {
   cudaEvent_t evs[] = {mb.ev_begin, mb.ev_view, mb.ev_info, mb.ev_cost[0], mb.ev_cost[1], mb.ev_produced, mb.ev_consumed, mb.ev_raster, mb.ev_image};
   for (cudaEvent_t e : evs) if (e) cudaEventDestroy(e);
   for (int i = 0; i < GT_COUNT; ++i) if (mb.tev[i]) cudaEventDestroy(mb.tev[i]);
+  for (cudaEvent_t e : mb.obj_tev) cudaEventDestroy(e);
+  cudaFree(mb.d_ghist_more);
   cudaFree(mb.d_info); cudaFree(mb.d_slab_count); cudaFree(mb.d_cmp_status); cudaFree(mb.d_row_cost); cudaFree(mb.rt_scratch); cudaFree(mb.d_gather);
   cudaFreeHost(mb.h_info); cudaFreeHost(mb.h_row_cost[0]); cudaFreeHost(mb.h_row_cost[1]);
   if (mb.comm && nccl_api().ok()) nccl_api().CommDestroy(mb.comm);
@@ -169,6 +188,33 @@ int member_asset(Member &mb, GsAsset *as) {   // per-asset buffers only the grou
     mb.cmp_words = words;
   }
   return ensure_sort_scratch(ctx, n);
+}
+
+// per-object scratch of a call with `objects` splat objects: slab tables, digit histograms, timing events
+int member_objects(Member &mb, uint32_t objects, bool timing) {
+  GsContext *ctx = mb.ctx;
+  const size_t table = 2 * kMaxSlabs * 4;
+  if (objects > mb.info_slots) {
+    cudaStreamSynchronize(ctx->stream);
+    cudaFree(mb.d_info); cudaFreeHost(mb.h_info);
+    mb.d_info = nullptr; mb.h_info = nullptr; mb.info_slots = 0;
+    GS_CUDA_TRY(ctx, cudaMalloc(&mb.d_info, objects * table));
+    GS_CUDA_TRY(ctx, cudaMallocHost(&mb.h_info, objects * table));
+    mb.info_slots = objects;
+  }
+  if (objects - 1 > mb.ghist_more_slots) {
+    cudaStreamSynchronize(ctx->stream);
+    cudaFree(mb.d_ghist_more);
+    mb.d_ghist_more = nullptr; mb.ghist_more_slots = 0;
+    GS_CUDA_TRY(ctx, cudaMalloc(&mb.d_ghist_more, (size_t)(objects - 1) * 4 * 256 * 4));
+    mb.ghist_more_slots = objects - 1;
+  }
+  while (timing && mb.obj_tev.size() < 2 * (size_t)objects) {
+    cudaEvent_t e = nullptr;
+    GS_CUDA_TRY(ctx, cudaEventCreate(&e));
+    mb.obj_tev.push_back(e);
+  }
+  return GS_OK;
 }
 
 // ---- the exchange: every member ends up with every segment ------------------------------------------------------------
@@ -382,6 +428,18 @@ int gs_group_balance_rows(const uint32_t *row_cost, uint32_t rows, uint32_t part
   return GS_OK;
 }
 
+int gs_group_row_costs(GsGroup *g, uint32_t *out, uint32_t rows) {
+  if (!g || !out) return fail(nullptr, GS_ERR_INVALID_ARGUMENT, "null argument");
+  Member &m0 = g->m[0];
+  if (g->hist_frames == 0) return fail(m0.ctx, GS_ERR_NOT_READY, "no call has measured row costs at the current screen size");
+  if (rows != (g->hist_h + kTile - 1) / kTile) return fail(m0.ctx, GS_ERR_INVALID_ARGUMENT, "rows is not the last call's number of 16-pixel rows");
+  const int slot = (int)((g->hist_frames - 1) & 1u);   // written by the last call, after its row exchange
+  GS_CUDA_TRY(m0.ctx, cudaSetDevice(m0.ctx->device));
+  GS_CUDA_TRY(m0.ctx, cudaEventSynchronize(m0.ev_cost[slot]));
+  memcpy(out, m0.h_row_cost[slot], (size_t)rows * 4);
+  return GS_OK;
+}
+
 int gs_group_unique_id(void *id_out) {
   if (!id_out) return fail(nullptr, GS_ERR_INVALID_ARGUMENT, "null id");
   if (!nccl_api().ok()) return fail(nullptr, GS_ERR_NOT_READY, "libnccl.so.2 not found: a multi-process group needs NCCL");
@@ -506,19 +564,35 @@ int gs_group_sync(GsGroup *g) {
   return rc;
 }
 
-int gs_group_frame(GsGroup *g, GsAsset *const *assets, const GsFrameParams *fp, const GsRenderOptions *opt_in, int do_sort_flag,
-                   GsImage *const *rts) {
-  if (!g || !assets || !fp) return fail(nullptr, GS_ERR_INVALID_ARGUMENT, "null argument");
+// One camera's frame of K splat objects on the group (gs_group_frame_objects; gs_group_frame is K = 1).  assets: [K][local
+// count].  strict: the new entry point's rules (GS_FLAG_LOAD_RT is refused); gs_group_frame ignores the flag, as it always has.
+static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsFrameParams *fps, const int32_t *do_sort,
+                       const GsRenderOptions *opt_in, GsImage *const *rts, GsImage *const *cams, bool strict) {
   const uint32_t G = g->size;
   const size_t L = g->m.size();
   int rc;
-  for (size_t i = 0; i < L; ++i) {
-    if (!assets[i]) return fail(g->m[i].ctx, GS_ERR_INVALID_ARGUMENT, "null asset");
-    if ((rc = check_params(g->m[i].ctx, assets[i], fp))) return rc;
-    if (assets[i]->av.n != assets[0]->av.n) return fail(g->m[i].ctx, GS_ERR_INVALID_ARGUMENT, "members hold different assets");
+  // ---- validation: everything is checked before anything is enqueued, so a rejected call writes nothing -----------------
+  if (strict && opt_in && (opt_in->flags & GS_FLAG_LOAD_RT))
+    return fail(g->m[0].ctx, GS_ERR_INVALID_ARGUMENT, "GS_FLAG_LOAD_RT: the first object starts from a cleared target, each later one blends under it");
+  std::vector<GroupObject> obj(K);
+  for (uint32_t k = 0; k < K; ++k) {
+    GroupObject &o = obj[k];
+    o.assets = assets + (size_t)k * L;
+    o.fp = fps + k;
+    o.sort = do_sort[k] != 0;
+    for (size_t i = 0; i < L; ++i) {
+      GsAsset *as = o.assets[i];
+      if (!as) return fail(g->m[i].ctx, GS_ERR_INVALID_ARGUMENT, "null asset");
+      if ((rc = check_params(g->m[i].ctx, as, o.fp))) return rc;
+      if (as->av.n != o.assets[0]->av.n) return fail(g->m[i].ctx, GS_ERR_INVALID_ARGUMENT, "members hold different assets");
+      for (size_t j = 0; j < (size_t)k * L; ++j)
+        if (assets[j] == as) return fail(g->m[i].ctx, GS_ERR_INVALID_ARGUMENT, "an asset is listed for two objects");
+    }
+    if (o.fp->screen_w != fps[0].screen_w || o.fp->screen_h != fps[0].screen_h)
+      return fail(g->m[0].ctx, GS_ERR_INVALID_ARGUMENT, "the objects of one camera differ in screen size");
+    o.n = o.assets[0]->av.n;
   }
-  const FrameConsts fc = make_frame_consts(fp);
-  const uint32_t W = (uint32_t)fp->screen_w, H = (uint32_t)fp->screen_h, N = assets[0]->av.n;
+  const uint32_t W = (uint32_t)fps[0].screen_w, H = (uint32_t)fps[0].screen_h;
   const uint32_t rows = (H + kTile - 1) / kTile, ntx = (W + kTile - 1) / kTile;
   GsRenderOptions base;
   memset(&base, 0, sizeof(base));
@@ -526,194 +600,251 @@ int gs_group_frame(GsGroup *g, GsAsset *const *assets, const GsFrameParams *fp, 
   if (base.blend_mode > GS_BLEND_FP32) return fail(g->m[0].ctx, GS_ERR_INVALID_ARGUMENT, "bad blend mode");
   uint32_t fmt = GS_PIX_RGBA16F;
   for (size_t i = 0; i < L; ++i) if (rts && rts[i]) { fmt = rts[i]->format; break; }
+  std::vector<uint32_t> pitches(L);
+  std::vector<void *> dev_rt(L, nullptr);   // a device rt is composited into in place; other members use library scratch
+  for (size_t i = 0; i < L; ++i) {
+    GsContext *ctx = g->m[i].ctx;
+    GsImage *rt = rts ? rts[i] : nullptr;
+    pitches[i] = W * pix_bytes(fmt);
+    if (rt) {
+      uint32_t p = 0;
+      if ((rc = image_ok(ctx, rt, W, H, &p))) return rc;
+      if (rt->format != fmt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "members' images differ in pixel format");
+      if (rt->memory == GS_MEM_DEVICE) { dev_rt[i] = rt->data; pitches[i] = p; }
+    }
+    if (G > 1 && pitches[i] != pitches[0]) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "members' images differ in row pitch");
+    GsImage *ct = cams ? cams[i] : nullptr;
+    uint32_t tp = 0;
+    if (ct && (rc = image_ok(ctx, ct, W, H, &tp))) return rc;
+  }
+  const FrameConsts fc0 = make_frame_consts(obj[0].fp);
+  for (uint32_t k = 0; k < K; ++k) obj[k].fc = k ? make_frame_consts(obj[k].fp) : fc0;
+  bool any_sort = false;
+  for (const GroupObject &o : obj) any_sort |= o.sort;
 
-  // ---- row ranges of this frame: from the row costs measured two frames ago (the last ones every GPU surely holds) ----
+  // ---- row ranges of this call: from the row costs measured two calls ago (the last ones every GPU surely holds), summed
+  // over that call's objects ------------------------------------------------------------------------------------------
   if (g->hist_w != W || g->hist_h != H) { g->hist_w = W; g->hist_h = H; g->hist_frames = 0; }
   const int slot = (int)(g->hist_frames & 1u);
-  for (Member &mb : g->m) { cudaSetDevice(mb.ctx->device); if ((rc = member_rows(mb, rows))) return rc; }
+  const bool timing = g->m[0].ctx->timing;
+  for (Member &mb : g->m) {
+    cudaSetDevice(mb.ctx->device);
+    if ((rc = member_rows(mb, rows)) || (rc = member_objects(mb, K, timing))) return rc;
+  }
   if (G == 1) { g->bounds[0] = 0; g->bounds[1] = rows; }
   else if (g->hist_frames >= 2) {
     Member &m0 = g->m[0];
-    GS_CUDA_TRY(m0.ctx, cudaEventSynchronize(m0.ev_cost[slot]));   // written by frame hist_frames - 2: long done
+    GS_CUDA_TRY(m0.ctx, cudaEventSynchronize(m0.ev_cost[slot]));   // written by call hist_frames - 2: long done
     balance_rows(m0.h_row_cost[slot], rows, G, g->bounds);
   } else {
     balance_rows(nullptr, rows, G, g->bounds);
   }
 
-  const bool timing = g->m[0].ctx->timing;
   g->timed = timing;
   GsNvtxRange nvtx_frame("GaussianSplat.GroupFrame");
-  // ---- phase A: distances + slab table on the context stream; view-calc on the second stream --------------------------
+  // ---- phase A: every object's distances + slab table on the context stream; every object's view-calc on the second stream
   for (size_t i = 0; i < L; ++i) {
     Member &mb = g->m[i];
     GsContext *ctx = mb.ctx;
-    GsAsset *as = assets[i];
     GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    if ((rc = member_asset(mb, as))) return rc;
+    // the objects' cutouts / bits share the context's buffers: sized for all of them before the first view-calc is queued, so
+    // the uploads (behind each other on the second stream) never reallocate under a view-calc that reads them
+    for (GroupObject &o : obj)
+      if ((rc = member_asset(mb, o.assets[i])) || (rc = reserve_frame_inputs(ctx, o.assets[i], o.fp, mb.aux))) return rc;
     for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
     GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_begin, ctx->stream));
     if (timing) cudaEventRecord(mb.tev[GT_BEGIN], ctx->stream);
-    if (do_sort_flag) {
-      SlabArgs sl;
-      memset(&sl, 0, sizeof(sl));
-      sl.count = G; sl.index = mb.rank; sl.order_prev = as->order; sl.mask = as->slab_mask; sl.group_bits = as->slab_group_bits; sl.info = mb.d_info;
-      for (uint32_t j = 0; j + 1 < G; ++j) sl.qpos[j] = (uint32_t)(((uint64_t)N * (j + 1)) / G);
-      GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->sort.ghist, 0, 4 * 256 * 4, ctx->stream));
-      GS_CUDA_TRY(ctx, cudaMemsetAsync(mb.d_info, 0, 2 * kMaxSlabs * 4, ctx->stream));
-      launch_calc_distances(as->av, fc, as->key_table, ctx->sort.ghist, ctx->stream, &sl);
-      ctx->launches += 1;
-      if (G > 1) {
-        GS_CUDA_TRY(ctx, cudaMemcpyAsync(mb.h_info, mb.d_info, 2 * kMaxSlabs * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_info, ctx->stream));
+    GsRenderOptions opt = base;
+    opt.row_begin = g->bounds[mb.rank]; opt.row_end = g->bounds[mb.rank + 1];
+    const bool draws = opt.row_end > opt.row_begin || G == 1;
+    if (G == 1) opt.row_begin = opt.row_end = 0;
+    for (uint32_t k = 0; k < K; ++k) {
+      GroupObject &o = obj[k];
+      GsAsset *as = o.assets[i];
+      if (o.sort) {
+        // each object has its own digit histograms and slab table: all distance kernels run before the one host wait
+        uint32_t *ghist = k ? mb.d_ghist_more + (size_t)(k - 1) * 4 * 256 : ctx->sort.ghist;
+        uint32_t *info = mb.d_info + (size_t)k * 2 * kMaxSlabs;
+        SlabArgs sl;
+        memset(&sl, 0, sizeof(sl));
+        sl.count = G; sl.index = mb.rank; sl.order_prev = as->order; sl.mask = as->slab_mask; sl.group_bits = as->slab_group_bits; sl.info = info;
+        for (uint32_t j = 0; j + 1 < G; ++j) sl.qpos[j] = (uint32_t)(((uint64_t)o.n * (j + 1)) / G);
+        GS_CUDA_TRY(ctx, cudaMemsetAsync(ghist, 0, 4 * 256 * 4, ctx->stream));
+        GS_CUDA_TRY(ctx, cudaMemsetAsync(info, 0, 2 * kMaxSlabs * 4, ctx->stream));
+        launch_calc_distances(as->av, o.fc, as->key_table, ghist, ctx->stream, &sl);
+        ctx->launches += 1;
+        if (G > 1) {
+          GS_CUDA_TRY(ctx, cudaMemcpyAsync(mb.h_info + (size_t)k * 2 * kMaxSlabs, info, 2 * kMaxSlabs * 4, cudaMemcpyDeviceToHost, ctx->stream));
+          GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_info, ctx->stream));
+        }
+      }
+      // View-calc reads nothing the sort writes: it runs on the helper stream (lowest priority), right behind the object's
+      // distance kernel (started together, its 24 k blocks crowd the distance kernel out), and so fills what the sort chain
+      // leaves idle: the host's wait for the slab tables, the sort's tails and the exchange
+      cudaEvent_t after = mb.ev_begin;
+      if (o.sort) { GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_produced, ctx->stream)); after = mb.ev_produced; }
+      if (draws) {
+        GS_CUDA_TRY(ctx, cudaStreamWaitEvent(mb.aux, after, 0));
+        if (timing && k == 0) cudaEventRecord(mb.tev[GT_V0], mb.aux);
+        if ((rc = do_view(ctx, as, o.fp, o.fc, true, opt, mb.aux))) return rc;
       }
     }
     if (timing) cudaEventRecord(mb.tev[GT_DIST], ctx->stream);
-    // View-calc reads nothing the sort writes: it runs on the helper stream (lowest priority), right behind the distance
-    // kernel (started together, its 24 k blocks crowd the distance kernel out), and so fills what the sort chain leaves
-    // idle: the host's wait for the slab table, the sort's tails and the exchange
-    cudaEvent_t after = mb.ev_begin;
-    if (do_sort_flag) { GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_produced, ctx->stream)); after = mb.ev_produced; }
-    GsRenderOptions opt = base;
-    opt.row_begin = g->bounds[mb.rank]; opt.row_end = g->bounds[mb.rank + 1];
-    if (opt.row_end > opt.row_begin || G == 1) {
-      if (G == 1) opt.row_begin = opt.row_end = 0;
-      GS_CUDA_TRY(ctx, cudaStreamWaitEvent(mb.aux, after, 0));
-      if (timing) cudaEventRecord(mb.tev[GT_V0], mb.aux);
-      if ((rc = do_view(ctx, as, fp, fc, true, opt, mb.aux))) return rc;
+    if (draws) {
       if (timing) cudaEventRecord(mb.tev[GT_V1], mb.aux);
       GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_view, mb.aux));
     }
   }
 
-  // ---- slab sizes: the one host wait of the frame (the GPUs are busy with view-calc) ----------------------------------
-  if (do_sort_flag) {
-    if (G == 1) { g->slab_off[0] = 0; g->slab_off[1] = N; g->slab_cnt[0] = N; }
-    for (size_t i = 0; i < L && G > 1; ++i) {
-      Member &mb = g->m[i];
-      GS_CUDA_TRY(mb.ctx, cudaSetDevice(mb.ctx->device));
-      GS_CUDA_TRY(mb.ctx, cudaEventSynchronize(mb.ev_info));
+  // ---- slab sizes: the one host wait of the call, for every object's table at once (the GPUs are busy with view-calc) ----
+  for (GroupObject &o : obj) {
+    if (!o.sort || G > 1) continue;
+    o.slab_off[0] = 0; o.slab_off[1] = o.n; o.slab_cnt[0] = o.n;
+  }
+  for (size_t i = 0; i < L && G > 1 && any_sort; ++i) {
+    Member &mb = g->m[i];
+    GS_CUDA_TRY(mb.ctx, cudaSetDevice(mb.ctx->device));
+    GS_CUDA_TRY(mb.ctx, cudaEventSynchronize(mb.ev_info));
+    for (uint32_t k = 0; k < K; ++k) {
+      GroupObject &o = obj[k];
+      if (!o.sort) continue;
+      const uint32_t *info = mb.h_info + (size_t)k * 2 * kMaxSlabs;
       uint32_t off[GS_GROUP_MAX_GPUS + 1];
       off[0] = 0;
       for (uint32_t c = 1; c < G; ++c) {
-        const uint32_t ge = mb.h_info[kMaxSlabs + c - 1];   // #{key >= splitter c-1 (ascending)}
-        if (ge > N) return fail(mb.ctx, GS_ERR_CUDA, "slab table corrupt");
-        off[c] = N - ge;
+        const uint32_t ge = info[kMaxSlabs + c - 1];   // #{key >= splitter c-1 (ascending)}
+        if (ge > o.n) return fail(mb.ctx, GS_ERR_CUDA, "slab table corrupt");
+        off[c] = o.n - ge;
       }
-      off[G] = N;
+      off[G] = o.n;
       for (uint32_t c = 0; c < G; ++c) if (off[c + 1] < off[c]) return fail(mb.ctx, GS_ERR_CUDA, "slab table not monotone");
-      if (i == 0) memcpy(g->slab_off, off, sizeof(uint32_t) * (G + 1));
-      else if (memcmp(g->slab_off, off, sizeof(uint32_t) * (G + 1)) != 0) return fail(mb.ctx, GS_ERR_CUDA, "members disagree on the slab table");
+      if (i == 0) memcpy(o.slab_off, off, sizeof(uint32_t) * (G + 1));
+      else if (memcmp(o.slab_off, off, sizeof(uint32_t) * (G + 1)) != 0) return fail(mb.ctx, GS_ERR_CUDA, "members disagree on the slab table");
+      for (uint32_t c = 0; c < G; ++c) o.slab_cnt[c] = o.slab_off[c + 1] - o.slab_off[c];
     }
-    for (uint32_t c = 0; c < G; ++c) g->slab_cnt[c] = g->slab_off[c + 1] - g->slab_off[c];
+  }
 
-    // ---- phase C: compact my slab out of last frame's order, sort it into its place of the new order ------------------
+  // ---- phase C, object after object: compact my slab out of last frame's order, sort it into its place, exchange the slabs
+  if (any_sort) {
     GsNvtxRange nvtx_sort("GaussianSplat.Sort");
-    // equal slots + one all-gather while the slabs are reasonably balanced (they are after the first frame); a frame whose
-    // largest slab is far above N/G exchanges the exact sizes in place instead (no G x cap staging)
-    uint32_t cap = 0;
-    for (uint32_t c = 0; c < G; ++c) cap = g->slab_cnt[c] > cap ? g->slab_cnt[c] : cap;
-    cap = (cap + 3u) & ~3u;
-    // one process per GPU: slabs go peer to peer (set up on the first sorted frame)
-    if (G > 1 && g->use_nccl && L == 1 && !g->link.tried) { if ((rc = peer_link_setup(g, assets[0]))) return rc; }
-    const bool use_p2p = G > 1 && L == 1 && g->link.ready && g->link.asset == assets[0];
-    uint32_t *p2p_new = nullptr;
-    int p2p_idx = 0;
-    if (use_p2p) {   // the two order buffers alternate: last frame's order is read, the other one is assembled
-      p2p_idx = assets[0]->order == g->link.buf[0] ? 1 : 0;
-      p2p_new = g->link.buf[p2p_idx];
+    for (uint32_t c = 0; c < G; ++c) g->slab_cnt[c] = 0;
+    for (const GroupObject &o : obj)
+      if (o.sort) for (uint32_t c = 0; c < G; ++c) g->slab_cnt[c] += o.slab_cnt[c];
+    // one process per GPU: the first object sorted on the group gets the peer-to-peer links (set up on its first sorted call);
+    // every other object exchanges its order through the all-gather or in place
+    if (G > 1 && g->use_nccl && L == 1 && !g->link.tried)
+      for (const GroupObject &o : obj)
+        if (o.sort) { if ((rc = peer_link_setup(g, o.assets[0]))) return rc; break; }
+    // per object: equal slots + one all-gather while the slabs are reasonably balanced (they are after the first frame); an
+    // object whose largest slab is far above N/G exchanges the exact sizes in place instead (no G x cap staging).  The staging
+    // is one buffer, sized for the largest object, that the objects use one after the other.
+    std::vector<uint32_t> caps(K, 0);
+    std::vector<char> p2p(K, 0), gather(K, 0);
+    size_t need = 0, words = 0;
+    for (uint32_t k = 0; k < K; ++k) {
+      const GroupObject &o = obj[k];
+      if (!o.sort) continue;
+      uint32_t cap = 0;
+      for (uint32_t c = 0; c < G; ++c) cap = o.slab_cnt[c] > cap ? o.slab_cnt[c] : cap;
+      caps[k] = (cap + 3u) & ~3u;
+      p2p[k] = G > 1 && L == 1 && g->link.ready && g->link.asset == o.assets[0];
+      gather[k] = !p2p[k] && G > 1 && (uint64_t)caps[k] * G <= (uint64_t)o.n + (uint64_t)o.n / 2 + 64u * G;
+      if (gather[k]) {
+        need = std::max(need, (size_t)caps[k] * G);
+        words = std::max(words, (size_t)o.n + (size_t)o.n / 2 + 64u * G);   // the largest staging this object ever uses
+      }
     }
-    const bool use_gather = !use_p2p && G > 1 && (uint64_t)cap * G <= (uint64_t)N + (uint64_t)N / 2 + 64u * G;
-    if (use_gather) {
+    for (size_t i = 0; i < L && need; ++i) {
+      Member &mb = g->m[i];
+      if (need <= mb.gather_words) continue;
+      GS_CUDA_TRY(mb.ctx, cudaSetDevice(mb.ctx->device));
+      cudaStreamSynchronize(mb.ctx->stream);
+      cudaFree(mb.d_gather);
+      mb.d_gather = nullptr; mb.gather_words = 0;
+      GS_CUDA_TRY(mb.ctx, cudaMalloc(&mb.d_gather, words * 4));
+      mb.gather_words = words;
+    }
+    for (uint32_t k = 0; k < K; ++k) {
+      const GroupObject &o = obj[k];
+      if (!o.sort) continue;
+      const uint32_t N = o.n, cap = caps[k];
+      const bool use_p2p = p2p[k], use_gather = gather[k];
+      uint32_t *p2p_new = nullptr;
+      int p2p_idx = 0;
+      if (use_p2p) {   // the two order buffers alternate: last frame's order is read, the other one is assembled
+        p2p_idx = o.assets[0]->order == g->link.buf[0] ? 1 : 0;
+        p2p_new = g->link.buf[p2p_idx];
+      }
       for (size_t i = 0; i < L; ++i) {
         Member &mb = g->m[i];
-        const size_t need = (size_t)cap * G;
-        if (need > mb.gather_words) {
-          GS_CUDA_TRY(mb.ctx, cudaSetDevice(mb.ctx->device));
-          cudaStreamSynchronize(mb.ctx->stream);
-          cudaFree(mb.d_gather);
-          mb.d_gather = nullptr; mb.gather_words = 0;
-          const size_t words = (size_t)N + (size_t)N / 2 + 64u * G;   // the largest staging this path ever uses
-          GS_CUDA_TRY(mb.ctx, cudaMalloc(&mb.d_gather, words * 4));
-          mb.gather_words = words;
+        GsContext *ctx = mb.ctx;
+        GsAsset *as = o.assets[i];
+        GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+        SortScratch sc = ctx->sort;   // this object's digit histograms (the rest of the scratch is used in stream order)
+        if (k) sc.ghist = mb.d_ghist_more + (size_t)(k - 1) * 4 * 256;
+        const uint32_t cnt = o.slab_cnt[mb.rank], off = o.slab_off[mb.rank];
+        if (G == 1) {
+          GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order, as->d_n, N, 4, 8, true, sc, ctx->stream, nullptr, as->key_table));
+          ctx->launches += 4;
+        } else if (cnt) {
+          launch_compact_order(as->order, N, as->slab_mask, as->slab_group_bits, as->key_table, as->order_tmp, as->keys, mb.d_cmp_status, mb.d_slab_count,
+                               ctx->stream);
+          GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order_tmp, mb.d_slab_count, cnt, 4, 8, true, sc, ctx->stream, nullptr, nullptr,
+                                             true, as->keys + off,
+                                             use_p2p ? p2p_new + off : use_gather ? mb.d_gather + (size_t)mb.rank * cap : as->order + off));
+          ctx->launches += 5;
         }
-      }
-    }
-    for (size_t i = 0; i < L; ++i) {
-      Member &mb = g->m[i];
-      GsContext *ctx = mb.ctx;
-      GsAsset *as = assets[i];
-      GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-      const uint32_t cnt = g->slab_cnt[mb.rank], off = g->slab_off[mb.rank];
-      if (G == 1) {
-        GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order, as->d_n, N, 4, 8, true, ctx->sort, ctx->stream, nullptr, as->key_table));
-        ctx->launches += 4;
-      } else if (cnt) {
-        launch_compact_order(as->order, N, as->slab_mask, as->slab_group_bits, as->key_table, as->order_tmp, as->keys, mb.d_cmp_status, mb.d_slab_count,
-                             ctx->stream);
-        GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order_tmp, mb.d_slab_count, cnt, 4, 8, true, ctx->sort, ctx->stream, nullptr, nullptr,
-                                           true, as->keys + off,
-                                           use_p2p ? p2p_new + off : use_gather ? mb.d_gather + (size_t)mb.rank * cap : as->order + off));
-        ctx->launches += 5;
-      }
-      if (use_p2p) {
-        PeerLink &k = g->link;
-        const uint32_t tag = ++k.sort_frames;
-        PushArgs pa;
-        memset(&pa, 0, sizeof(pa));
-        for (uint32_t c = 0; c < G; ++c)
-          if (c != mb.rank) { pa.dst[pa.npeers] = k.peer_buf[p2p_idx][c] + off; pa.flag[pa.npeers] = k.peer_flags[c] + mb.rank; ++pa.npeers; }
-        k_push_slab<<<sm_count(), 512, 0, ctx->stream>>>(p2p_new + off, cnt, pa, tag, k.d_done);
-        k_wait_slabs<<<1, 32, 0, ctx->stream>>>(k.flags, G, mb.rank, tag);
-        ctx->launches += 2;
-        // from here on the assembled buffer IS the draw order; last frame's becomes the next frame's target
-        as->order_alt = as->order;
-        as->order = p2p_new;
-      }
-      GS_CUDA_TRY(ctx, cudaGetLastError());
-      if (timing) cudaEventRecord(mb.tev[GT_SORT], ctx->stream);
-    }
-    if (G > 1) {
-      std::vector<uint8_t *> bufs(L);
-      size_t off[GS_GROUP_MAX_GPUS], cnt[GS_GROUP_MAX_GPUS];
-      for (uint32_t c = 0; c < G; ++c) { off[c] = (size_t)g->slab_off[c] * 4; cnt[c] = (size_t)g->slab_cnt[c] * 4; }
-      if (use_p2p) {
-        // delivered by k_push_slab / awaited by k_wait_slabs above
-      } else if (use_gather) {
-        for (size_t i = 0; i < L; ++i) bufs[i] = reinterpret_cast<uint8_t *>(g->m[i].d_gather);
-        if ((rc = exchange_allgather(g, bufs.data(), (size_t)cap * 4, cnt))) return rc;
-        for (size_t i = 0; i < L; ++i) {   // slot c's ids -> their place in the order: G device copies (a copy kernel that found
-          Member &mb = g->m[i];            // each element's slab was measured slower than the copy engine)
-          GS_CUDA_TRY(mb.ctx, cudaSetDevice(mb.ctx->device));
+        if (use_p2p) {
+          PeerLink &lk = g->link;
+          const uint32_t tag = ++lk.sort_frames;
+          PushArgs pa;
+          memset(&pa, 0, sizeof(pa));
           for (uint32_t c = 0; c < G; ++c)
-            if (g->slab_cnt[c])
-              GS_CUDA_TRY(mb.ctx, cudaMemcpyAsync(assets[i]->order + g->slab_off[c], mb.d_gather + (size_t)c * cap, (size_t)g->slab_cnt[c] * 4,
-                                                  cudaMemcpyDeviceToDevice, mb.ctx->stream));
+            if (c != mb.rank) { pa.dst[pa.npeers] = lk.peer_buf[p2p_idx][c] + off; pa.flag[pa.npeers] = lk.peer_flags[c] + mb.rank; ++pa.npeers; }
+          k_push_slab<<<sm_count(), 512, 0, ctx->stream>>>(p2p_new + off, cnt, pa, tag, lk.d_done);
+          k_wait_slabs<<<1, 32, 0, ctx->stream>>>(lk.flags, G, mb.rank, tag);
+          ctx->launches += 2;
+          // from here on the assembled buffer IS the draw order; last frame's becomes the next frame's target
+          as->order_alt = as->order;
+          as->order = p2p_new;
         }
-      } else {
-        for (size_t i = 0; i < L; ++i) bufs[i] = reinterpret_cast<uint8_t *>(assets[i]->order);
-        if ((rc = exchange_begin(g)) || (rc = exchange_add(g, bufs.data(), off, cnt)) || (rc = exchange_end(g))) return rc;
+        GS_CUDA_TRY(ctx, cudaGetLastError());
+        if (timing) cudaEventRecord(mb.tev[GT_SORT], ctx->stream);
+      }
+      if (G > 1) {
+        std::vector<uint8_t *> bufs(L);
+        size_t off[GS_GROUP_MAX_GPUS], cnt[GS_GROUP_MAX_GPUS];
+        for (uint32_t c = 0; c < G; ++c) { off[c] = (size_t)o.slab_off[c] * 4; cnt[c] = (size_t)o.slab_cnt[c] * 4; }
+        if (use_p2p) {
+          // delivered by k_push_slab / awaited by k_wait_slabs above
+        } else if (use_gather) {
+          for (size_t i = 0; i < L; ++i) bufs[i] = reinterpret_cast<uint8_t *>(g->m[i].d_gather);
+          if ((rc = exchange_allgather(g, bufs.data(), (size_t)cap * 4, cnt))) return rc;
+          for (size_t i = 0; i < L; ++i) {   // slot c's ids -> their place in the order: G device copies (a copy kernel that found
+            Member &mb = g->m[i];            // each element's slab was measured slower than the copy engine)
+            GS_CUDA_TRY(mb.ctx, cudaSetDevice(mb.ctx->device));
+            for (uint32_t c = 0; c < G; ++c)
+              if (o.slab_cnt[c])
+                GS_CUDA_TRY(mb.ctx, cudaMemcpyAsync(o.assets[i]->order + o.slab_off[c], mb.d_gather + (size_t)c * cap, (size_t)o.slab_cnt[c] * 4,
+                                                    cudaMemcpyDeviceToDevice, mb.ctx->stream));
+          }
+        } else {
+          for (size_t i = 0; i < L; ++i) bufs[i] = reinterpret_cast<uint8_t *>(o.assets[i]->order);
+          if ((rc = exchange_begin(g)) || (rc = exchange_add(g, bufs.data(), off, cnt)) || (rc = exchange_end(g))) return rc;
+        }
       }
     }
   }
-  if (timing) for (Member &mb : g->m) { cudaSetDevice(mb.ctx->device); if (!do_sort_flag) cudaEventRecord(mb.tev[GT_SORT], mb.ctx->stream); cudaEventRecord(mb.tev[GT_ORDER], mb.ctx->stream); }
+  if (timing) for (Member &mb : g->m) { cudaSetDevice(mb.ctx->device); if (!any_sort) cudaEventRecord(mb.tev[GT_SORT], mb.ctx->stream); cudaEventRecord(mb.tev[GT_ORDER], mb.ctx->stream); }
 
-  // ---- phase D: bin + composite my rows, then exchange rows and row costs ---------------------------------------------
+  // ---- phase D: bin + composite my rows, object after object into the one image, then exchange rows and row costs ---------
   std::vector<uint8_t *> img(L), costs(L);
-  std::vector<uint32_t> pitches(L);
   for (size_t i = 0; i < L; ++i) {
     Member &mb = g->m[i];
     GsContext *ctx = mb.ctx;
-    GsAsset *as = assets[i];
     GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    GsImage *rt = rts ? rts[i] : nullptr;
-    uint32_t pitch = W * pix_bytes(fmt);
-    void *d_rt = nullptr;
-    if (rt) {
-      uint32_t p = 0;
-      if ((rc = image_ok(ctx, rt, W, H, &p))) return rc;
-      if (rt->format != fmt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "members' images differ in pixel format");
-      if (rt->memory == GS_MEM_DEVICE) { d_rt = rt->data; pitch = p; }
-    }
+    const uint32_t pitch = pitches[i];
+    void *d_rt = dev_rt[i];
     if (!d_rt) {
       if (mb.rt_bytes < (size_t)pitch * H) {
         cudaStreamSynchronize(ctx->stream);
@@ -725,39 +856,47 @@ int gs_group_frame(GsGroup *g, GsAsset *const *assets, const GsFrameParams *fp, 
       d_rt = mb.rt_scratch;
     }
     img[i] = reinterpret_cast<uint8_t *>(d_rt);
-    pitches[i] = pitch;
     costs[i] = reinterpret_cast<uint8_t *>(mb.d_row_cost);
     GsRenderOptions opt = base;
     opt.row_begin = g->bounds[mb.rank]; opt.row_end = g->bounds[mb.rank + 1];
+    mb.obj_timed = 0;
     if (opt.row_end > opt.row_begin || G == 1) {
       if (G == 1) opt.row_begin = opt.row_end = 0;
       GS_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, mb.ev_view, 0));
-      // the previous frame's row exchange (transfer stream) may still be filling this image: composite only after it
+      // the previous call's row exchange (transfer stream) may still be filling this image: composite only after it
       if (mb.image_pending) GS_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, mb.ev_image, 0));
       if (timing) cudaEventRecord(mb.tev[GT_VIEWWAIT], ctx->stream);
-      rec(ctx, EV_VIEW1);
-      if ((rc = bind_depth(ctx, fp, ctx->stream))) return rc;
-      if ((rc = do_render(ctx, as, fc, opt, d_rt, pitch, fmt))) return rc;
-      ctx->launches += 1;   // k_row_costs, launched on the transfer stream below
+      for (uint32_t k = 0; k < K; ++k) {
+        GroupObject &o = obj[k];
+        // object 0 starts from a cleared target, each later one blends under what the earlier ones left in my rows
+        opt.flags = k ? (uint32_t)GS_FLAG_LOAD_RT : 0u;
+        rec(ctx, EV_VIEW1);
+        if (timing) cudaEventRecord(mb.obj_tev[2 * k], ctx->stream);
+        if ((rc = bind_depth(ctx, o.fp, ctx->stream))) return rc;
+        if ((rc = do_render(ctx, o.assets[i], o.fc, opt, d_rt, pitch, fmt, 0, timing ? mb.obj_tev[2 * k + 1] : nullptr))) return rc;
+        ctx->launches += 1;   // k_row_costs: here for every object but the last (before the next one's raster overwrites the
+                              // tile costs), on the transfer stream below for the last
+        if (k + 1 < K) launch_row_costs(ctx->bin.tile_cost, ntx, g->bounds[mb.rank], g->bounds[mb.rank + 1], mb.d_row_cost, ctx->stream, k > 0);
+      }
+      mb.obj_timed = timing ? K : 0;
     } else if (timing) {
       cudaEventRecord(mb.tev[GT_VIEWWAIT], ctx->stream);
     }
     if (timing) cudaEventRecord(mb.tev[GT_RASTER], ctx->stream);
   }
   // The exchange of the composited rows (and of their measured costs) goes to the transfer stream: it needs no SM to speak
-  // of, and the next frame's distance / sort chain does not depend on it, so the two overlap; the next frame's compositor
+  // of, and the next call's distance / sort chain does not depend on it, so the two overlap; the next call's compositor
   // waits for it (above), gs_group_sync / a host image complete it.
   for (size_t i = 0; i < L; ++i) {
     Member &mb = g->m[i];
     GS_CUDA_TRY(mb.ctx, cudaSetDevice(mb.ctx->device));
     GS_CUDA_TRY(mb.ctx, cudaEventRecord(mb.ev_raster, mb.ctx->stream));
     GS_CUDA_TRY(mb.ctx, cudaStreamWaitEvent(mb.xfer, mb.ev_raster, 0));
-    if (g->bounds[mb.rank + 1] > g->bounds[mb.rank] || G == 1)   // the measured cost of my rows, for the balancer two frames on
-      launch_row_costs(mb.ctx->bin.tile_cost, ntx, g->bounds[mb.rank], g->bounds[mb.rank + 1], mb.d_row_cost, mb.xfer);
+    if (g->bounds[mb.rank + 1] > g->bounds[mb.rank] || G == 1)   // the measured cost of my rows, for the balancer two calls on
+      launch_row_costs(mb.ctx->bin.tile_cost, ntx, g->bounds[mb.rank], g->bounds[mb.rank + 1], mb.d_row_cost, mb.xfer, K > 1);
   }
   if (G > 1) {
     size_t off[GS_GROUP_MAX_GPUS], cnt[GS_GROUP_MAX_GPUS], coff[GS_GROUP_MAX_GPUS], ccnt[GS_GROUP_MAX_GPUS];
-    for (size_t i = 1; i < L; ++i) if (pitches[i] != pitches[0]) return fail(g->m[i].ctx, GS_ERR_INVALID_ARGUMENT, "members' images differ in row pitch");
     for (uint32_t c = 0; c < G; ++c) {
       const uint32_t y0 = min(g->bounds[c] * kTile, H), y1 = min(g->bounds[c + 1] * kTile, H);
       off[c] = (size_t)y0 * pitches[0]; cnt[c] = (size_t)(y1 - y0) * pitches[0];
@@ -784,20 +923,39 @@ int gs_group_frame(GsGroup *g, GsAsset *const *assets, const GsFrameParams *fp, 
       GS_CUDA_TRY(ctx, cudaMemcpy2DToArrayAsync(static_cast<cudaArray_t>(rt->data), 0, 0, img[i], pitches[i], (size_t)W * pix_bytes(fmt), H,
                                                 cudaMemcpyDeviceToDevice, mb.xfer));
     }
+    // the composite pass onto this member's camera target, from the assembled image, still on the transfer stream (a host
+    // camera target is uploaded, blended and read back before the call returns, as gs_composite does)
+    GsImage *ct = cams ? cams[i] : nullptr;
+    if (ct && (rc = composite_device_rt(ctx, img[i], pitches[i], fmt, ct, W, H, mb.xfer))) return rc;
     GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_image, mb.xfer));
     mb.image_pending = true;
-    // the row-cost vector is rewritten by the next frame's k_row_costs on the context stream: that must follow this exchange too
-    // (it does: k_row_costs runs after the compositor, which waits for ev_image)
+    // the row-cost vector is rewritten by the next call's k_row_costs: on the context stream after the compositor, which
+    // waits for ev_image, or on this stream
   }
   g->frame++;
   g->hist_frames++;
   // host images: filled by the transfer stream.  By default the call blocks until they are (like gs_frame); with
   // GS_FLAG_ASYNC_READBACK it returns now and gs_group_sync completes them -- the images must be pinned and must not be
-  // reused before that (alternate two).  The next frame's compositor waits for this frame's copy before it touches the
+  // reused before that (alternate two).  The next call's compositor waits for this call's copy before it touches the
   // device image, so no second device image is needed.
   const bool async_rb = opt_in && (opt_in->flags & GS_FLAG_ASYNC_READBACK) != 0;
   if (host_out && !async_rb) return gs_group_sync(g);
   return GS_OK;
+}
+
+int gs_group_frame(GsGroup *g, GsAsset *const *assets, const GsFrameParams *fp, const GsRenderOptions *opt_in, int do_sort_flag,
+                   GsImage *const *rts) {
+  if (!g || !assets || !fp) return fail(nullptr, GS_ERR_INVALID_ARGUMENT, "null argument");
+  const int32_t do_sort = do_sort_flag;
+  return group_frame(g, 1, assets, fp, &do_sort, opt_in, rts, nullptr, false);
+}
+
+int gs_group_frame_objects(GsGroup *g, uint32_t object_count, GsAsset *const *assets, const GsFrameParams *fps, const int32_t *do_sort,
+                           const GsRenderOptions *opt, GsImage *const *rts, GsImage *const *camera_targets) {
+  if (!g) return fail(nullptr, GS_ERR_INVALID_ARGUMENT, "null group");
+  if (object_count == 0) return fail(g->m[0].ctx, GS_ERR_INVALID_ARGUMENT, "object_count is 0");
+  if (!assets || !fps || !do_sort) return fail(g->m[0].ctx, GS_ERR_INVALID_ARGUMENT, "null argument");
+  return group_frame(g, object_count, assets, fps, do_sort, opt, rts, camera_targets, true);
 }
 
 int gs_group_get_stats(GsGroup *g, GsGroupStats *out) {
@@ -817,8 +975,12 @@ int gs_group_get_stats(GsGroup *g, GsGroupStats *out) {
     out->slab_sort_ms = tev_ms(mb, GT_DIST, GT_SORT);
     out->order_exchange_ms = tev_ms(mb, GT_SORT, GT_ORDER);
     out->view_ms = tev_ms(mb, GT_V0, GT_V1);
-    float bin = 0.0f;
-    if (mb.ctx->ev_valid[EV_VIEW1] && mb.ctx->ev_valid[EV_BIN1] && cudaEventElapsedTime(&bin, mb.ctx->ev[EV_VIEW1], mb.ctx->ev[EV_BIN1]) != cudaSuccess) { cudaGetLastError(); bin = 0.0f; }
+    float bin = 0.0f;   // binning of every object drawn, summed; the raster is the rest of the compositing span
+    for (uint32_t k = 0; k < mb.obj_timed; ++k) {
+      float ms = 0.0f;
+      if (cudaEventElapsedTime(&ms, mb.obj_tev[2 * k], mb.obj_tev[2 * k + 1]) != cudaSuccess) { cudaGetLastError(); ms = 0.0f; }
+      bin += ms;
+    }
     out->bin_ms = bin;
     out->raster_ms = tev_ms(mb, GT_VIEWWAIT, GT_RASTER) - bin;
     out->image_exchange_ms = tev_ms(mb, GT_RASTER, GT_IMAGE);

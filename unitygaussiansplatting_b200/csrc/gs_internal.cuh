@@ -101,13 +101,20 @@ FrameConsts make_frame_consts(const GsFrameParams *fp);
 int check_params(GsContext *ctx, GsAsset *as, const GsFrameParams *fp);
 int check_options(GsContext *ctx, const FrameConsts &fc, GsRenderOptions &opt);
 int ensure_sort_scratch(GsContext *ctx, uint32_t capacity);
+// Grows the context's cutout / deleted / selected buffers to what fp needs for `as`; a buffer is only reallocated once
+// ctx->stream and `busy` (when given: another stream whose view-calc may still read it) have drained.  Uploads nothing.
+int reserve_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t busy = nullptr);
 int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t stream);
 int bind_depth(GsContext *ctx, const GsFrameParams *fp, cudaStream_t stream);   // sets ctx->cur_depth for the draw that follows
 int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameConsts &fc, bool cull, const GsRenderOptions &opt,
             cudaStream_t stream);
-// d_rt == nullptr: the target is the CUDA array behind `surf`
+// d_rt == nullptr: the target is the CUDA array behind `surf`.  bin_done (optional) is recorded on ctx->stream when binning ends.
 int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRenderOptions &opt, void *d_rt, uint32_t pitch, uint32_t fmt,
-              cudaSurfaceObject_t surf = 0);
+              cudaSurfaceObject_t surf = 0, cudaEvent_t bin_done = nullptr);
+// The composite pass (gs_composite) of a linear device render target onto `tgt` (host, device or CUDA-array memory, already
+// validated as W x H), enqueued on `s`.  A host target is uploaded and read back, and the call waits for `s`.
+int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H,
+                        cudaStream_t s);
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch);
 uint32_t pix_bytes(uint32_t fmt);
 // The per-asset work buffers (order, keys, view data, ...) of an asset whose blobs as->d_* are already in HBM, the format
@@ -115,5 +122,6 @@ uint32_t pix_bytes(uint32_t fmt);
 cudaError_t asset_init_work(GsContext *ctx, GsAsset *as, uint32_t n, uint32_t pos_fmt, uint32_t scale_fmt, uint32_t sh_fmt,
                             uint32_t col_fmt, uint32_t chunk_count);
 void rec(GsContext *ctx, int e);
-void launch_row_costs(const uint32_t *cost, uint32_t ntx, uint32_t t0, uint32_t t1, uint32_t *row_cost, cudaStream_t s);   // gs_raster.cu
+void launch_row_costs(const uint32_t *cost, uint32_t ntx, uint32_t t0, uint32_t t1, uint32_t *row_cost, cudaStream_t s,
+                      bool accumulate = false);   // gs_raster.cu
 }  // namespace gs

@@ -308,19 +308,20 @@ __global__ void __launch_bounds__(1024) k_tile_order(const uint32_t *__restrict_
   }
 }
 
-// per raster-tile row: the sum of its tiles' costs (what the group path balances its row ranges with)
+// per raster-tile row: the sum of its tiles' costs (what the group path balances its row ranges with).  accumulate != 0 adds
+// the sums to what row_cost holds: several splat objects drawn into one target are balanced on their summed cost.
 __global__ void __launch_bounds__(256) k_row_costs(const uint32_t *__restrict__ cost, uint32_t ntx, uint32_t t0, uint32_t t1,
-                                                   uint32_t *__restrict__ row_cost) {
+                                                   uint32_t *__restrict__ row_cost, uint32_t accumulate) {
   const uint32_t row = t0 + blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (row >= t1) return;
   uint32_t acc = 0;
   for (uint32_t x = lane; x < ntx; x += 32) acc += cost[row * ntx + x];
 #pragma unroll
   for (int o = 16; o; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if (lane == 0) row_cost[row] = acc;
+  if (lane == 0) row_cost[row] = accumulate ? row_cost[row] + acc : acc;
 }
-void launch_row_costs(const uint32_t *cost, uint32_t ntx, uint32_t t0, uint32_t t1, uint32_t *row_cost, cudaStream_t s) {
-  if (t1 > t0) k_row_costs<<<(t1 - t0 + 7) / 8, 256, 0, s>>>(cost, ntx, t0, t1, row_cost);
+void launch_row_costs(const uint32_t *cost, uint32_t ntx, uint32_t t0, uint32_t t1, uint32_t *row_cost, cudaStream_t s, bool accumulate) {
+  if (t1 > t0) k_row_costs<<<(t1 - t0 + 7) / 8, 256, 0, s>>>(cost, ntx, t0, t1, row_cost, accumulate ? 1u : 0u);
 }
 
 // Can any pixel centre of the 8x4 block centred on (bcx, bcy) lie inside the splat's quad, |qa| <= 2 and |qb| <= 2 with

@@ -4,6 +4,7 @@
 // host language used instead.  Same member names and call order as the C# class for the hot path;
 // errors never throw: like the reference (:361-369,:655) a failed call logs and returns false.
 #pragma once
+#include <algorithm>
 #include <cstdio>
 #include <cstring>
 #include <vector>
@@ -114,38 +115,23 @@ class GaussianSplatRenderer {
   int m_FrameCounter = 0;
 };
 
-// The same renderer on several GPUs of one box, one process driving all of them (gs_group_create / gs_group_frame):
-// identical knobs; every non-null image receives the complete frame, bit-identical to what one GPU renders.
-class GaussianSplatRendererGroup {
- public:
+// One splat object on a group: the renderer's knobs and its asset on every local member.  The group itself is one
+// (GaussianSplatRendererGroup derives from it); AddObject makes more.
+struct GaussianSplatGroupObject {
   float m_SplatScale = 1.0f, m_OpacityScale = 1.0f;
   int m_SHOrder = 3;
   bool m_SHOnly = false;
   int m_SortNthFrame = 1;
+  int m_RenderOrder = 0;   // :236, higher values draw first
   Matrix4x4 localToWorldMatrix{{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}};
   Matrix4x4 worldToLocalMatrix{{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}};
-  GsRenderOptions options{};
+  std::vector<GsCutout> m_Cutouts;
+  const uint32_t *deletedBits = nullptr, *selectedBits = nullptr;   // host, ceil(N/32) words, or nullptr
+  const float *sceneDepth = nullptr;                                 // host, width x height, or nullptr
+  int m_FrameCounter = 0;
+  std::vector<GsAsset *> m_Assets;                                   // [local member]
 
-  ~GaussianSplatRendererGroup() { OnDisable(); }
-
-  bool OnEnable(const GsAssetDesc &asset, const std::vector<int> &cudaDevices, uint32_t flags = 0) {
-    OnDisable();
-    if (!ok(gs_group_create(cudaDevices.data(), (uint32_t)cudaDevices.size(), flags, &m_Group))) return false;
-    m_Assets.assign(gs_group_local_count(m_Group), nullptr);
-    if (!ok(gs_group_asset_upload(m_Group, &asset, m_Assets.data()))) return false;
-    m_FrameCounter = 0;
-    return true;
-  }
-  void OnDisable() {
-    for (GsAsset *a : m_Assets) if (a) gs_asset_destroy(a);   // the library owns the contexts: assets go first
-    m_Assets.clear();
-    if (m_Group) gs_group_destroy(m_Group);
-    m_Group = nullptr;
-  }
-  // rts[i]: the image of local member i (device, host or CUDA-array memory) or nullptr
-  bool SortAndRenderSplats(const CameraState &cam, GsImage *const *rts) {
-    const int doSort = (m_FrameCounter % (m_SortNthFrame > 0 ? m_SortNthFrame : 1)) == 0;
-    ++m_FrameCounter;
+  GsFrameParams params(const CameraState &cam) const {
     GsFrameParams fp;
     std::memset(&fp, 0, sizeof(fp));
     std::memcpy(fp.mat_object_to_world, localToWorldMatrix.m, 64);
@@ -159,7 +145,84 @@ class GaussianSplatRendererGroup {
     fp.opacity_scale = m_OpacityScale;
     fp.sh_order = (uint32_t)m_SHOrder;
     fp.sh_only = m_SHOnly ? 1u : 0u;
+    fp.cutouts = m_Cutouts.empty() ? nullptr : m_Cutouts.data();
+    fp.cutout_count = (uint32_t)m_Cutouts.size();
+    fp.deleted_bits = deletedBits;
+    fp.selected_bits = selectedBits;
+    fp.scene_depth = sceneDepth;
+    return fp;
+  }
+  int nextDoSort() {   // :120-121
+    const int doSort = (m_FrameCounter % (m_SortNthFrame > 0 ? m_SortNthFrame : 1)) == 0;
+    ++m_FrameCounter;
+    return doSort;
+  }
+};
+
+// The same renderer on several GPUs of one box, one process driving all of them (gs_group_create / gs_group_frame):
+// identical knobs; every non-null image receives the complete frame, bit-identical to what one GPU renders.
+class GaussianSplatRendererGroup : public GaussianSplatGroupObject {
+ public:
+  GsRenderOptions options{};
+
+  ~GaussianSplatRendererGroup() { OnDisable(); }
+
+  bool OnEnable(const GsAssetDesc &asset, const std::vector<int> &cudaDevices, uint32_t flags = 0) {
+    OnDisable();
+    if (!ok(gs_group_create(cudaDevices.data(), (uint32_t)cudaDevices.size(), flags, &m_Group))) return false;
+    m_Assets.assign(gs_group_local_count(m_Group), nullptr);
+    if (!ok(gs_group_asset_upload(m_Group, &asset, m_Assets.data()))) return false;
+    m_FrameCounter = 0;
+    return true;
+  }
+  void OnDisable() {
+    // the library owns the contexts: every object's assets go first
+    for (GaussianSplatGroupObject *o : m_Objects) { for (GsAsset *a : o->m_Assets) if (a) gs_asset_destroy(a); delete o; }
+    m_Objects.clear();
+    for (GsAsset *a : m_Assets) if (a) gs_asset_destroy(a);
+    m_Assets.clear();
+    if (m_Group) gs_group_destroy(m_Group);
+    m_Group = nullptr;
+  }
+  // Another splat object on the group (its asset uploaded to every member); owned by the group, nullptr on failure.
+  GaussianSplatGroupObject *AddObject(const GsAssetDesc &asset) {
+    GaussianSplatGroupObject *o = new GaussianSplatGroupObject();
+    o->m_Assets.assign(gs_group_local_count(m_Group), nullptr);
+    if (!m_Group || !ok(gs_group_asset_upload(m_Group, &asset, o->m_Assets.data()))) { delete o; return nullptr; }
+    m_Objects.push_back(o);
+    return o;
+  }
+  // rts[i]: the image of local member i (device, host or CUDA-array memory) or nullptr
+  bool SortAndRenderSplats(const CameraState &cam, GsImage *const *rts) {
+    const int doSort = nextDoSort();
+    GsFrameParams fp = params(cam);
     return ok(gs_group_frame(m_Group, m_Assets.data(), &fp, &options, doSort, rts));
+  }
+  // OnPreCullCamera on the group (R/GaussianSplatRenderer.cs:187-211): `objects` (this group and / or AddObject's) drawn in
+  // GatherSplatsForCamera order (:73-105) into one target, then composited onto cameraTargets[i] (may be nullptr / hold nullptrs).
+  bool SortAndRenderSplatsMulti(const CameraState &cam, std::vector<GaussianSplatGroupObject *> objects, GsImage *const *rts,
+                                GsImage *const *cameraTargets = nullptr) {
+    auto depth = [&](const GaussianSplatGroupObject *o) {   // camera-space z of the object's position, +z forward
+      const float *v = cam.worldToCameraMatrix.m, *p = o->localToWorldMatrix.m + 12;
+      return -(v[2] * p[0] + v[6] * p[1] + v[10] * p[2] + v[14]);
+    };
+    if (objects.empty()) return true;   // no active splat object: OnPreCullCamera draws nothing
+    const size_t L = m_Assets.size();
+    for (const GaussianSplatGroupObject *o : objects)   // checked before any object's frame counter moves
+      if (!o || o->m_Assets.size() != L) return false;
+    std::stable_sort(objects.begin(), objects.end(), [&](const GaussianSplatGroupObject *a, const GaussianSplatGroupObject *b) {
+      if (a->m_RenderOrder != b->m_RenderOrder) return a->m_RenderOrder > b->m_RenderOrder;
+      return depth(a) < depth(b);
+    });
+    std::vector<GsAsset *> assets;
+    std::vector<GsFrameParams> fps;
+    std::vector<int32_t> doSort;
+    for (GaussianSplatGroupObject *o : objects) {
+      assets.insert(assets.end(), o->m_Assets.begin(), o->m_Assets.end());
+      fps.push_back(o->params(cam));
+      doSort.push_back(o->nextDoSort());
+    }
+    return ok(gs_group_frame_objects(m_Group, (uint32_t)objects.size(), assets.data(), fps.data(), doSort.data(), &options, rts, cameraTargets));
   }
   bool Sync() { return ok(gs_group_sync(m_Group)); }
   GsGroup *group() const { return m_Group; }
@@ -172,8 +235,7 @@ class GaussianSplatRendererGroup {
     return false;
   }
   GsGroup *m_Group = nullptr;
-  std::vector<GsAsset *> m_Assets;
-  int m_FrameCounter = 0;
+  std::vector<GaussianSplatGroupObject *> m_Objects;
 };
 
 }  // namespace GaussianSplatting

@@ -142,16 +142,11 @@ class GaussianSplatGroup:
         self.size = int(lib.gs_group_size(handle))
         self.local_count = int(lib.gs_group_local_count(handle))
         self.contexts = [GaussianSplatContext.from_handle(lib.gs_group_context(handle, i)) for i in range(self.local_count)]
-        d = asset.desc()
-        self._assets = (C.c_void_p * self.local_count)()
-        N.check(None, lib.gs_group_asset_upload(handle, C.byref(d), self._assets))
-        self.m_SplatScale, self.m_OpacityScale, self.m_SHOrder, self.m_SHOnly = 1.0, 1.0, 3, False
-        self.m_SortNthFrame, self.m_FrameCounter = 1, 0
-        self.localToWorldMatrix = None
-        self.m_Cutouts, self.m_DeletedBits, self.m_SelectedBits, self.sceneDepth = [], None, None, None
+        self._assets = _upload(lib, handle, asset, self.local_count)
+        _init_knobs(self)
         self.blend_mode = N.GS_BLEND_FP16_ROP
         self.async_readback = False  # host images are filled asynchronously (pinned memory; sync() completes them)
-        self._keep = None
+        self._objects = []           # further splat objects (add_object), drawn with SortAndRenderSplatsMulti
 
     @classmethod
     def join(cls, asset, context, rank: int, world: int, unique_id: bytes):
@@ -177,36 +172,95 @@ class GaussianSplatGroup:
         return self.m_Asset.splatCount
 
     def frame_params(self, cam):
-        from .renderer import make_frame_params
-        fp, self._keep = make_frame_params(cam, self.localToWorldMatrix, self.m_SplatScale, self.m_OpacityScale, self.m_SHOrder,
-                                           self.m_SHOnly, self.m_Cutouts, self.m_DeletedBits, self.splatCount, self.m_SelectedBits, self.sceneDepth)
+        fp, self._keep = _frame_params(self, cam)
         return fp
+
+    def add_object(self, asset) -> "GaussianSplatGroupObject":
+        """Another splat object on the group: `asset` is uploaded to every member (gs_group_asset_upload).  The returned object
+        carries the renderer's knobs; draw it with SortAndRenderSplatsMulti.  The group itself stays usable as an object."""
+        o = GaussianSplatGroupObject(self, asset)
+        self._objects.append(o)
+        return o
 
     def SortAndRenderSplats(self, cam, rts=None, fp=None):
         """rts: one image per LOCAL member (numpy host array, torch CUDA tensor, CudaArrayImage, or None); each receives the
         whole frame."""
-        from .renderer import _image
         do_sort = 1 if (self.m_FrameCounter % max(1, int(self.m_SortNthFrame)) == 0) else 0
         self.m_FrameCounter += 1
         if fp is None:
             fp = self.frame_params(cam)
+        opt = self._options()
+        ims = []
+        ptrs = self._images(rts, cam, ims)
+        N.check(self.contexts[0].handle, self._lib.gs_group_frame(self.handle, self._assets, C.byref(fp), C.byref(opt), do_sort, ptrs))
+
+    def SortAndRenderSplatsMulti(self, objects, cam, rts=None, camera_targets=None):
+        """One camera's frame with several splat objects (the group itself and / or add_object's objects): ordered by
+        GatherSplatsForCamera, the first drawn into a cleared target and each later one under it, one row exchange, then the
+        composite onto every given camera target (gs_group_frame_objects).  rts / camera_targets: one image per LOCAL member
+        or None, as in SortAndRenderSplats.  Returns the objects in the order they were drawn.  With no objects nothing is
+        drawn or composited, as OnPreCullCamera returns early when the camera has no active splat object."""
+        from .renderer import GatherSplatsForCamera
+        objects = list(objects)
+        for k, o in enumerate(objects):   # checked before any object's frame counter moves
+            if o._group() is not self:
+                raise ValueError("object %d belongs to another group" % k)
+        if len(set(map(id, objects))) != len(objects):
+            raise ValueError("an object is listed twice")
+        if not objects:
+            return []
+        active = GatherSplatsForCamera(objects, cam)
+        K, L = len(active), self.local_count
+        assets = (C.c_void_p * (K * L))()
+        fps = (N.GsFrameParams * K)()
+        do_sort = (C.c_int32 * K)()
+        keep = []
+        for k, o in enumerate(active):
+            for i in range(L):
+                assets[k * L + i] = o._assets[i]
+            fps[k], kp = _frame_params(o, cam)
+            keep.append(kp)
+            do_sort[k] = 1 if (o.m_FrameCounter % max(1, int(o.m_SortNthFrame)) == 0) else 0
+        opt = self._options()
+        ims = []
+        ptrs, cptrs = self._images(rts, cam, ims), self._images(camera_targets, cam, ims)
+        for o in active:   # the uniforms and images were accepted: now the frame counts (:120-121)
+            o.m_FrameCounter += 1
+        N.check(self.contexts[0].handle, self._lib.gs_group_frame_objects(self.handle, K, assets, fps, do_sort, C.byref(opt), ptrs, cptrs))
+        return active
+
+    def _group(self):
+        return self
+
+    def _options(self) -> N.GsRenderOptions:
         opt = N.GsRenderOptions()
         opt.blend_mode = self.blend_mode
         opt.flags = N.GS_FLAG_ASYNC_READBACK if self.async_readback else 0
+        return opt
+
+    def _images(self, images, cam, keep):
+        from .renderer import _image
         ptrs = (C.POINTER(N.GsImage) * self.local_count)()
-        ims = []
-        if rts is not None:
-            if not isinstance(rts, (list, tuple)):
-                rts = [rts]
-            for i, rt in enumerate(rts):
-                if rt is not None:
-                    im = _image(rt, cam.pixelWidth, cam.pixelHeight)
-                    ims.append(im)
+        if images is not None:
+            if not isinstance(images, (list, tuple)):
+                images = [images]
+            for i, a in enumerate(images):
+                if a is not None:
+                    im = _image(a, cam.pixelWidth, cam.pixelHeight)
+                    keep.append(im)
                     ptrs[i] = C.pointer(im)
-        N.check(self.contexts[0].handle, self._lib.gs_group_frame(self.handle, self._assets, C.byref(fp), C.byref(opt), do_sort, ptrs))
+        return ptrs
 
     def sync(self):
         N.check(self.contexts[0].handle, self._lib.gs_group_sync(self.handle))
+
+    def row_costs(self, rows: int):
+        """gs_group_row_costs: the per-row costs the last call measured, summed over its objects (what the row split two calls
+        later is balanced on)."""
+        import numpy as np
+        out = np.zeros(rows, np.uint32)
+        N.check(self.contexts[0].handle, self._lib.gs_group_row_costs(self.handle, out.ctypes.data, rows))
+        return out
 
     def stats(self) -> N.GsGroupStats:
         st = N.GsGroupStats()
@@ -222,10 +276,11 @@ class GaussianSplatGroup:
     def close(self):
         if self.handle:
             def free_assets():
-                for i in range(self.local_count):
-                    if self._assets[i]:
-                        self._lib.gs_asset_destroy(self._assets[i])
-                        self._assets[i] = None
+                for holder in [self] + self._objects:
+                    for i in range(self.local_count):
+                        if holder._assets[i]:
+                            self._lib.gs_asset_destroy(holder._assets[i])
+                            holder._assets[i] = None
             if getattr(self, "_owner_ctx", None) is not None:
                 # joined group: the context is the caller's and outlives the group; the group goes first so that the peers'
                 # mappings of this process's order buffers are closed before the buffers are freed
@@ -242,6 +297,56 @@ class GaussianSplatGroup:
             self.close()
         except Exception:
             pass
+
+
+class GaussianSplatGroupObject:
+    """A further splat object on a GaussianSplatGroup (GaussianSplatGroup.add_object): the renderer's knobs and the object's
+    asset on every local member.  Its assets are freed by the group's close()."""
+
+    def __init__(self, group: GaussianSplatGroup, asset):
+        import weakref
+        self._group = weakref.ref(group)
+        self._lib = group._lib
+        self.m_Asset = asset
+        self._assets = _upload(group._lib, group.handle, asset, group.local_count)
+        _init_knobs(self)
+
+    @property
+    def splatCount(self) -> int:
+        return self.m_Asset.splatCount
+
+    def frame_params(self, cam):
+        fp, self._keep = _frame_params(self, cam)
+        return fp
+
+    def readback_order(self, local: int = 0):
+        import numpy as np
+        out = np.empty(self.splatCount, np.uint32)
+        N.check(None, self._lib.gs_readback_order(self._assets[local], out.ctypes.data))
+        return out
+
+
+def _upload(lib, handle, asset, local_count):
+    d = asset.desc()
+    assets = (C.c_void_p * local_count)()
+    N.check(None, lib.gs_group_asset_upload(handle, C.byref(d), assets))
+    return assets
+
+
+def _init_knobs(o):
+    """The serialized knobs of GaussianSplatRenderer (R/GaussianSplatRenderer.cs:225-251) on a group object."""
+    o.m_SplatScale, o.m_OpacityScale, o.m_SHOrder, o.m_SHOnly = 1.0, 1.0, 3, False
+    o.m_SortNthFrame, o.m_FrameCounter = 1, 0
+    o.m_RenderOrder = 0          # higher values draw first (GatherSplatsForCamera)
+    o.localToWorldMatrix = None  # None: identity
+    o.m_Cutouts, o.m_DeletedBits, o.m_SelectedBits, o.sceneDepth = [], None, None, None
+    o._keep = None
+
+
+def _frame_params(o, cam):
+    from .renderer import make_frame_params
+    return make_frame_params(cam, o.localToWorldMatrix, o.m_SplatScale, o.m_OpacityScale, o.m_SHOrder, o.m_SHOnly, o.m_Cutouts,
+                             o.m_DeletedBits, o.splatCount, o.m_SelectedBits, o.sceneDepth)
 
 
 def balance_rows(row_cost, parts: int):

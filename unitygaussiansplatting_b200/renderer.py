@@ -395,7 +395,8 @@ def GatherSplatsForCamera(renderers, cam: Camera):
     w2c = cam.worldToCameraMatrix.astype(np.float64)
 
     def depth(r):
-        p = np.asarray(r.localToWorldMatrix, np.float64)[:3, 3]
+        m = r.localToWorldMatrix   # None (a group object's default): identity
+        p = np.asarray(_EYE4 if m is None else m, np.float64)[:3, 3]
         return -float((w2c @ np.r_[p, 1.0])[2])     # camTr.InverseTransformPoint(pos).z: +z forward (the view matrix looks down -z)
     return sorted(renderers, key=lambda r: (-int(r.m_RenderOrder), depth(r)))
 
