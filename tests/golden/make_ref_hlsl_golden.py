@@ -8,8 +8,9 @@ oracle/refhlsl/build_ref_hlsl.py.  `reference(name)` returns its output for case
 library is present, otherwise read from the fixture.  The scene-sized cases are stored for a fixed seeded sample of their
 splats (the whole scenes would make fixtures of ~0.7 MB each); `idx` names the sampled splats (or sorted positions) and is
 every one of them when the library computes the case.
-Run from the repo root:  python tests/golden/make_ref_hlsl_golden.py
+Run from the repo root:  python tests/golden/make_ref_hlsl_golden.py [case ...]   (every case when none is named)
 """
+import dataclasses
 import hashlib
 import sys
 from pathlib import Path
@@ -21,15 +22,20 @@ ROOT = GOLD.parents[1]
 sys.path.insert(0, str(ROOT))
 sys.path.insert(0, str(ROOT / "tests"))
 
+from util import FORMAT_CASES  # noqa: E402
+
 # ---- the GPU comparison: CSCalcViewData + CSCalcDistances with the renderer's defaults (ref_hlsl_<quality>.npz) ----------
 QUALITIES = ("Medium", "VeryHigh")
 N, SEED, WIDTH, HEIGHT = 20000, 0x5EED0091, 320, 240
 SAMPLE, SAMPLE_SEED = 2048, 0x5EED0095
 
 # ---- the oracle comparisons (ref_hlsl_<case>.npz) --------------------------------------------------------------------------
-VIEW_QUALITIES = ("Medium", "VeryHigh", "High", "Low", "custom-f16sh", "custom-norm6pos")
+# "custom-<name>" is the format case <name> of tests/util.py FORMAT_CASES; BC7 colour is left out of the view cases because
+# its block decode belongs to the texture unit, not to the reference's code (tests/golden/bc7_blocks.npz covers it)
+VIEW_QUALITIES = ("Medium", "VeryHigh", "High", "Low", "custom-f16sh", "custom-norm6pos") + \
+    tuple("custom-" + c.name for c in FORMAT_CASES if c.formats[2] != 3)
 VIEW_SAMPLE = 512
-KEY_QUALITIES = ("Medium", "VeryHigh")
+KEY_QUALITIES = ("Medium", "VeryHigh", "custom-norm6pos-f16sh", "custom-f32pos-bc7-f16sh")   # + Norm6, chunked Float32 positions
 KEY_N, KEY_SAMPLE = 30000, 4096
 EXPORT_N, EXPORT_SAMPLE = 3000, 128
 DRAW_W, DRAW_H = 200, 150
@@ -57,11 +63,14 @@ def sample_ids(n=N, k=SAMPLE, seed=SAMPLE_SEED):
 def view_case(quality):
     """(asset, (fp, keep)): object transform, splat / opacity scale, a cutout box and deleted bits on a clustered scene."""
     import unitygaussiansplatting_b200 as g
-    from util import camera
-    if quality.startswith("custom"):     # format combinations no preset uses: Float16 SH, Norm6 positions, Norm16 scale
+    from util import camera, case_asset, format_case, palette_backed
+    if quality in ("custom-f16sh", "custom-norm6pos"):     # Float16 SH; Norm6 positions with Norm16 scale
         fmts = {"custom-f16sh": (g.VectorFormat.Norm16, g.VectorFormat.Norm6, g.ColorFormat.Float16x4, g.SHFormat.Float16),
                 "custom-norm6pos": (g.VectorFormat.Norm6, g.VectorFormat.Norm16, g.ColorFormat.Float32x4, g.SHFormat.Norm11)}[quality]
         asset = g.create_asset(g.generate_input_splats(g.SCENE_CLUSTERED, N, 0x5EED0091), formats=fmts)
+    elif quality.startswith("custom-"):
+        # a clustered palette padded to the 65536 entries a u16 index can name, as the device backs it
+        asset = palette_backed(case_asset(g, format_case(quality[len("custom-"):]), N, 0x5EED0091))
     else:
         asset = g.synthetic_asset(g.SCENE_CLUSTERED, N, 0x5EED0091, quality)
     T = np.eye(4, dtype=np.float32)
@@ -77,8 +86,11 @@ def view_case(quality):
 def key_case(quality):
     """(asset, (fp, keep), order): CSCalcDistances through a random permutation."""
     import unitygaussiansplatting_b200 as g
-    from util import camera
-    asset = g.synthetic_asset(g.SCENE_CLUSTERED, KEY_N, 0x5EED0092, quality)
+    from util import camera, case_asset, format_case
+    if quality.startswith("custom-"):
+        asset = case_asset(g, format_case(quality[len("custom-"):]), KEY_N, 0x5EED0092)
+    else:
+        asset = g.synthetic_asset(g.SCENE_CLUSTERED, KEY_N, 0x5EED0092, quality)
     order = np.random.default_rng(1).permutation(KEY_N).astype(np.uint32)
     return asset, g.make_frame_params(camera(g, 320, 240)), order
 
@@ -128,7 +140,7 @@ def rotation_quats():
 
 CASES = (["gpu_" + q.lower() for q in QUALITIES] + ["view_" + q.lower() for q in VIEW_QUALITIES] +
          ["keys_" + q.lower() for q in KEY_QUALITIES] + ["export", "draw", "draw_selected", "rotation"])
-_NAMES = {q.lower(): q for q in VIEW_QUALITIES}
+_NAMES = {q.lower(): q for q in VIEW_QUALITIES + KEY_QUALITIES}
 
 
 def compute(name):
@@ -144,7 +156,9 @@ def compute(name):
         return {"idx": np.arange(N, dtype=np.uint32), "view": O.ref_calc_view(asset, fp), "asset_sha256": asset_digest(asset)}
     if kind == "keys":
         asset, (fp, _keep), order = key_case(_NAMES[q])
-        return {"idx": np.arange(KEY_N, dtype=np.uint32), "keys": O.ref_calc_distances(asset, fp, order), "asset_sha256": asset_digest(asset)}
+        # CSCalcDistances reads positions only, and the compiled reference refuses a BC7 asset as a whole: call it Norm8x4
+        pos_only = dataclasses.replace(asset, colorFormat=2) if asset.colorFormat == 3 else asset
+        return {"idx": np.arange(KEY_N, dtype=np.uint32), "keys": O.ref_calc_distances(pos_only, fp, order), "asset_sha256": asset_digest(asset)}
     if name == "export":
         asset, (fp, _k), (fpT, _k2), _T, rq, rs = export_case()
         return {"idx": np.arange(EXPORT_N, dtype=np.uint32), "plain": O.ref_export(asset, fp),
@@ -207,7 +221,10 @@ if __name__ == "__main__":
     from oracle import gs_oracle_py as O
     if O.ref_hlsl() is None:
         raise SystemExit("oracle/_ref/libref_hlsl.so is not built")
-    for name in CASES:
+    unknown = sorted(set(sys.argv[1:]) - set(CASES))
+    if unknown:
+        raise SystemExit("unknown case(s) %s; the cases are %s" % (unknown, CASES))
+    for name in sys.argv[1:] or CASES:
         data = stored(name)
         np.savez_compressed(fixture(name), **data)
         print(name, {k: v.shape for k, v in data.items()})

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 from conftest import default_camera
+from util import FORMAT_CASES
 
 pytestmark = pytest.mark.gpu
 
@@ -75,6 +76,8 @@ CUSTOM = [
     (2, 1, 3, 2),    # Norm11, Norm16, BC7, Norm11
     (0, 0, 0, 7),    # all float, Cluster8k
 ]
+# ... and every combination of tests/util.py FORMAT_CASES the host packer makes itself (not the 64k / 32k / 16k palettes)
+CUSTOM += [f for f in dict.fromkeys(c.formats for c in FORMAT_CASES) if f[3] not in (4, 5, 6) and f not in CUSTOM]
 
 
 @pytest.mark.parametrize("formats", CUSTOM)

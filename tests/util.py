@@ -1,4 +1,7 @@
 """Shared scene builders for the tests."""
+import dataclasses
+from collections import namedtuple
+
 import numpy as np
 
 
@@ -79,3 +82,69 @@ def view_fields(view):
         return (x & 0xFFFF).astype(np.uint16).view(np.float16).astype(np.float32)
     return {"pos": f[:, 0:4], "axis1": f[:, 4:6], "axis2": f[:, 6:8], "r": h(col[:, 0] >> 16), "g": h(col[:, 0]), "b": h(col[:, 1] >> 16),
             "a": h(col[:, 1])}
+
+
+# ---- asset format combinations no preset uses ------------------------------------------------------------------------------
+# The importer's Custom quality lets a user pick any (position, scale, colour, SH) format.  One list of combinations, chosen so
+# that between them they reach every decode path of the view, distance and export kernels (tests/test_format_cases.py checks
+# that they still do); tests/test_gpu_formats.py, tests/test_gpu_pack.py and the reference-shader fixtures all draw from it.
+# Codes: vector 0 Float32, 1 Norm16, 2 Norm11, 3 Norm6; colour 0 Float32x4, 1 Float16x4, 2 Norm8x4, 3 BC7;
+# SH 0 Float32, 1 Float16, 2 Norm11, 3 Norm6, 4..8 Cluster64k..Cluster4k.
+# `n` is the splat count of the GPU comparison; `indices`: the clustered palette indices are rewritten over all of 0..65535.
+FormatCase = namedtuple("FormatCase", "name formats n indices")
+FORMAT_CASES = (
+    FormatCase("norm6pos-f16sh", (3, 3, 0, 1), 4865, False),      # Norm6 position; 6-byte `other`; chunked Float32x4 colour
+    FormatCase("f32pos-bc7-f16sh", (0, 1, 3, 1), 5003, False),    # chunked Float32 position; Float16 SH with BC7
+    FormatCase("f32sh-bc7", (1, 0, 3, 0), 3001, False),           # 16-byte `other`; chunked but not lerped Float32 SH
+    FormatCase("norm11sh-bc7", (2, 3, 3, 2), 2819, False),        # 6-byte `other`; Norm11 SH with BC7
+    FormatCase("norm6sh-bc7", (3, 2, 3, 3), 4098, False),         # 8-byte `other`; Norm6 SH with BC7; the one even count
+    FormatCase("f32sh-chunked", (0, 2, 0, 0), 2305, False),       # Float32 SH and colour, chunked because scale is Norm11
+    FormatCase("norm11sh-f16col", (2, 2, 1, 2), 2561, False),     # Norm11 SH without BC7
+    FormatCase("norm6sh-norm8col", (1, 3, 2, 3), 3331, False),    # Norm6 SH without BC7; 6-byte `other`
+    FormatCase("cluster64k", (0, 0, 1, 4), 4099, True),           # clustered 18-byte `other` (Float32 scale at 2-aligned)
+    FormatCase("cluster32k", (1, 2, 0, 5), 4353, True),           # clustered 10-byte `other`
+    FormatCase("cluster16k", (1, 3, 1, 6), 4611, True),           # clustered 8-byte `other` with Norm6 scale
+    FormatCase("cluster8k", (2, 1, 2, 7), 8195, False),           # clustered 12-byte `other`, packed by the host
+    FormatCase("cluster4k", (3, 0, 1, 8), 4097, False),           # clustered 18-byte `other` with Norm6 position
+    FormatCase("cluster4k-oob-bc7", (3, 0, 3, 8), 4391, True),    # ... with BC7, and indices past the 4096-entry palette
+)
+FORMAT_SEED = 0x5EED0C00
+
+
+def format_case(name):
+    return next(c for c in FORMAT_CASES if c.name == name)
+
+
+def case_asset(g, case, n=None, seed=FORMAT_SEED):
+    """The asset of a FormatCase: a clustered scene of `n` (default case.n) splats packed by the host.  Host k-means at 16k,
+    32k and 64k entries is too slow for a test, so those are a host-packed Cluster4k asset with the same vector and colour
+    formats whose palette is replaced by a seeded one of that size; where case.indices is set, every splat's palette index
+    (the trailing u16 of its `other` record) is replaced by a seeded value in 0..65535, a quarter or more of them >= 32768."""
+    pf, sf, cf, shf = case.formats
+    n = case.n if n is None else n
+    host_sh = 8 if shf in (4, 5, 6) else shf
+    asset = g.create_asset(g.generate_input_splats(1, n, seed), formats=(pf, sf, cf, host_sh))   # 1: SCENE_CLUSTERED
+    rng = np.random.default_rng(seed + case.formats[3])
+    if shf != host_sh:
+        entries = 65536 >> (shf - 4)
+        pal = np.zeros((entries, 48), np.float16)            # SHTableItemFloat16: 45 halfs + 3 of padding = 96 bytes
+        pal[:, :45] = rng.uniform(-0.6, 0.6, (entries, 45))
+        asset.shData = pal.view(np.uint8).reshape(-1)
+        asset.shFormat = g.SHFormat(shf)
+    if case.indices:
+        stride = 4 + (12, 6, 4, 2)[sf] + 2
+        rec = asset.otherData[:n * stride].reshape(n, stride)
+        idx = rng.integers(0, 65536, n, dtype=np.uint16)
+        assert (idx >= 32768).mean() >= 0.25
+        rec[:, stride - 2:] = idx.view(np.uint8).reshape(n, 2)
+    return asset
+
+
+def palette_backed(asset):
+    """`asset` with a clustered palette zero-padded to 65536 entries: any u16 index names an entry, and the device backs all
+    of them with zeros (gs_asset_upload), so this is the asset a host-side decoder has to read to see the same splats."""
+    if asset.shFormat <= 3 or asset.shData.nbytes >= 65536 * 96:
+        return asset
+    sh = np.zeros(65536 * 96, np.uint8)
+    sh[:asset.shData.nbytes] = asset.shData
+    return dataclasses.replace(asset, shData=sh)
