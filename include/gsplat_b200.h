@@ -410,6 +410,11 @@ GS_API int gs_upload_order(GsAsset *asset, const uint32_t *src);  /* seed a prev
 /* Diagnostics: with GS_RASTER_STATS=1 in the environment the compositor counts, per frame, [0] warp-batches,
  * [1] warp cull ballots, [2] warp candidates, [3] warp evaluations, [4] pixel blends, [5] list entries x warps. */
 GS_API int gs_debug_raster_stats(GsContext *ctx, uint64_t out[8]);
+/* Diagnostics: with GS_SORT_PHASES=1 in the environment the depth sort records, per pass and 8192-pair tile, 8 words:
+ * %globaltimer ns at [0] tile start, [1] keys landed, [2] prefix resolved, [3] scatter done; [4] look-back status words read and
+ * [5] status words summed (max over digits); [6] the tile; [7] CTA << 32 | SM.  Pass p's tile t is at (p * tiles + t) * 8;
+ * *tiles = tiles per pass.  Copies min(max_words, 32 * tiles) words of the last depth sort. */
+GS_API int gs_debug_sort_phases(GsContext *ctx, uint64_t *out, uint32_t max_words, uint32_t *tiles);
 
 /* ---- Unity render-thread entry (SURVEY 8f N2) -------------------------------------- */
 /* Unity executes native GPU work on its render thread through CommandBuffer.IssuePluginEventAndData(func, eventId, data)

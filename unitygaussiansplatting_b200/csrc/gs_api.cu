@@ -978,6 +978,17 @@ int gs_debug_raster_stats(GsContext *ctx, uint64_t out[8]) {
   return GS_OK;
 }
 
+int gs_debug_sort_phases(GsContext *ctx, uint64_t *out, uint32_t max_words, uint32_t *tiles) {
+  if (!ctx || !tiles) return GS_ERR_INVALID_ARGUMENT;
+  *tiles = g_sort_phase_tiles;
+  if (!g_sort_phases) return GS_ERR_NOT_READY;
+  const size_t all = (size_t)4 * g_sort_phase_tiles * 8, words = max_words < all ? max_words : all;
+  if (words && !out) return GS_ERR_INVALID_ARGUMENT;
+  GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (words) GS_CUDA_TRY(ctx, cudaMemcpy(out, g_sort_phases, words * 8, cudaMemcpyDeviceToHost));
+  return GS_OK;
+}
+
 void *gs_context_stream(GsContext *ctx) { return ctx ? (void *)ctx->stream : nullptr; }
 void *gs_asset_device_ptr(GsAsset *as, int which) {
   if (!as) return nullptr;

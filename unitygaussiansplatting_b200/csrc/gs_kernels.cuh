@@ -148,6 +148,8 @@ struct SortScratch {
 };
 constexpr uint32_t kSortTileItems = 8192;  // 512 threads x 16 keys
 size_t sort_lookback_words(uint32_t capacity, int passes);
+extern unsigned long long *g_sort_phases;   // diagnostics, see GS_SORT_PHASES
+extern uint32_t g_sort_phase_tiles;
 // Stable ascending LSD sort of (key,val) pairs on bits [0, bits*passes), bits in {5..8}, or one pass of 9 bits.  The count
 // is read from d_count (device).  count_is_capacity: the host passes the exact count as `capacity` (exact grid); otherwise
 // `capacity` only bounds the buffers and a persistent grid serves whatever d_count holds.

@@ -9,15 +9,16 @@
 //   * digit histograms for all passes come from one read of the keys (or for free from
 //     k_calc_distances, which wrote the keys in the first place);
 //   * each CTA (512 threads x 16 keys) takes an 8192-pair tile by atomic ticket (so a tile's
-//     predecessors are always resident: look-back cannot deadlock), ranks its keys with warp-level digit
+//     predecessors are always resident: look-back cannot deadlock), publishes the tile's per-digit
+//     count with a LOCAL flag as soon as its keys have landed, ranks its keys with warp-level digit
 //     matching (the match mask of equal digits gives the stable rank as a popc of the lower
-//     lanes; one lane bumps the warp-private shared histogram), publishes the tile's
-//     per-digit count with a LOCAL flag, walks back over predecessors' status words until
-//     it meets an INCLUSIVE one, then publishes its own inclusive prefix;
+//     lanes; one lane bumps the warp-private shared histogram), and only then walks back over
+//     predecessors' status words until it meets an INCLUSIVE one and publishes its own inclusive
+//     prefix: ranking does not need the prefix, so the predecessors' progress overlaps it;
 //   * keys and payloads are first scattered inside shared memory into digit order, then
 //     written out in runs, so global stores are coalesced per digit run;
-//   * payloads are fetched only after ranking (their latency hides behind the look-back),
-//     which keeps the kernel at <= 64 registers and 2 CTAs/SM.
+//   * payloads are fetched after the tile's count is published and consumed at the scatter, which
+//     keeps the kernel at <= 64 registers and 2 CTAs/SM.
 // The digit width is a template parameter: depth keys use 4 x 8 bits; the binner sorts bin ids
 // in one pass of 5..9 bits up to 512 bins, else in 2 passes of 5..8 bits.
 // No tensor-core path: there is no contraction here, only byte/integer traffic.
@@ -39,6 +40,18 @@ constexpr int kSortWarps = kSortThreads / 32;
 size_t sort_lookback_words(uint32_t capacity, int passes) {
   size_t tiles = ((size_t)capacity + kSortTileItems - 1) / kSortTileItems;
   return tiles * 256 * (size_t)passes;
+}
+
+// Diagnostics (tools/time_sort_phases.py): with GS_SORT_PHASES=1 the depth sort runs an instantiation of k_onesweep that
+// records, per tile, %globaltimer at tile start / keys landed / prefix resolved / scatter done, the look-back's status words
+// read and summed, the tile, the CTA and its SM (kPhaseWords words per tile, one row of g_sort_phase_tiles tiles per pass).
+constexpr int kPhaseWords = 8;
+unsigned long long *g_sort_phases = nullptr;
+uint32_t g_sort_phase_tiles = 0;
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
 }
 
 // ---- digit histograms of all passes in one read -------------------------------------------
@@ -114,15 +127,16 @@ __device__ __forceinline__ uint32_t match_digit(uint32_t d) {
 // ---- one digit pass -------------------------------------------------------------------------
 // GATHER: the keys of this pass are keys_src[payload] (pass 0 of the depth sort reads the per-splat key
 // table through last frame's order, S/SplatUtilities.compute:76-81, without a separate gather pass).
+// PHASES: the diagnostic instantiation that fills `phases` (see g_sort_phases); the product never launches it.
 // PERSIST: a fixed grid whose CTAs keep taking tiles until the (device-side) count is exhausted -- for lists whose length
 // the host does not know when it launches (the binner's entry list): no capacity-sized grid of idle CTAs.
 // Shared memory per CTA at BITS = 9: 64 KB of pairs + 16 warps x 512 x 4 B = 32 KB of warp histograms (dynamic) + 6 KB of
 // static digit arrays = 102 KB, so two CTAs fit an SM's 228 KB.
-template <int BITS, bool GATHER, bool PERSIST>
+template <int BITS, bool GATHER, bool PERSIST, bool PHASES>
 __global__ void __launch_bounds__(kSortThreads, 2)
 k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_v, uint32_t *__restrict__ dst_k,
            uint32_t *__restrict__ dst_v, const uint32_t *__restrict__ d_count, int shift, const uint32_t *__restrict__ ghist,
-           volatile uint32_t *lookback, uint32_t *ticket) {
+           volatile uint32_t *lookback, uint32_t *ticket, unsigned long long *phases) {
   constexpr uint32_t NB = 1u << BITS;
   static_assert(NB <= (uint32_t)kSortThreads, "steps 2 and 4 give each digit its own thread");
   constexpr uint32_t kTileItems = kSortTileItems;
@@ -134,6 +148,7 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
   __shared__ uint32_t s_off[NB];
   __shared__ uint32_t s_scan[kSortWarps];
   __shared__ uint32_t s_tile;
+  __shared__ unsigned long long s_ph[3];
 
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t n = *d_count;
@@ -144,9 +159,11 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
   for (uint32_t d = tid; d < NB; d += kSortThreads) s_hist[d] = 0;
 #pragma unroll
   for (uint32_t d = lane; d < NB; d += 32) s_whist[warp][d] = 0;
+  if (PHASES && tid < 3) s_ph[tid] = 0;
   __syncthreads();
   const uint32_t tile = s_tile;
   if (tile >= num_tiles) return;
+  const unsigned long long t_start = PHASES ? globaltimer() : 0ull;
   const uint32_t tile_base = tile * kTileItems;
   const bool full_tile = tile_base + kTileItems <= n;
 
@@ -184,42 +201,18 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
     }
   }
   __syncthreads();
+  const unsigned long long t_keys = PHASES ? globaltimer() : 0ull;
 
-  // 2. publish, then resolve the exclusive prefix over earlier tiles with 4 status probes in flight
-  uint32_t prefix = 0, tile_total = 0;
+  // 2. publish the tile's per-digit count; its exclusive prefix over earlier tiles is resolved only after ranking (step 4),
+  // which does not need it: predecessors get the ranking's time to publish, and the wait overlaps work in every warp
+  uint32_t tile_total = 0, pub = 0;
+  volatile uint32_t *lb = lookback + (size_t)tile * NB + tid;
   if (tid < NB) {
     tile_total = s_hist[tid];  // includes pads (only the last digit of the last tile)
-    uint32_t pub = tile_total;
+    pub = tile_total;
     if (tid == NB - 1 && !full_tile) pub -= (tile_base + kTileItems - n);
-    volatile uint32_t *lb = lookback + (size_t)tile * NB + tid;
-    if (tile == 0) {
-      *lb = kFlagIncl | pub;
-    } else {
-      *lb = kFlagLocal | pub;
-      int t = (int)tile - 1;
-      bool done = false;
-      constexpr int kProbe = 4;   // status probes in flight per round (8 measured slower: more polling traffic, same wait)
-      while (!done) {
-        uint32_t v[kProbe];
-#pragma unroll
-        for (int q = 0; q < kProbe; ++q) v[q] = (t - q >= 0) ? lookback[(size_t)(t - q) * NB + tid] : (uint32_t)kFlagIncl;
-        int used = 0;
-#pragma unroll
-        for (int q = 0; q < kProbe; ++q) {
-          if (!done && used == q) {
-            if (v[q] != 0) {
-              prefix += v[q] & kValMask;
-              used = q + 1;
-              if (v[q] & kFlagIncl) done = true;
-            }
-          }
-        }
-        t -= used;
-      }
-      *lb = kFlagIncl | (prefix + pub);
-    }
+    *lb = (tile == 0 ? kFlagIncl : kFlagLocal) | pub;
   }
-  __syncwarp();   // the spin loop above ends per thread: tell the compiler the warp is whole again before the ballots
   if (!GATHER) {  // payloads: issued now, consumed at the scatter
     if (full_tile) {
 #pragma unroll
@@ -254,7 +247,8 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
   }
   __syncthreads();
 
-  // 4. thread `tid` < NB owns digit `tid`: exclusive prefix over warps, tile/global digit bases
+  // 4. thread `tid` < NB owns digit `tid`: exclusive prefix over warps, tile digit bases, then the look-back (4 status
+  // probes in flight per round) for the tile's global digit bases
   if (tid < NB) {
     uint32_t run = 0;
 #pragma unroll
@@ -266,6 +260,38 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
   }
   const uint32_t dig_start = block_excl_scan<kSortWarps>(tile_total, s_scan);
   const uint32_t gbase = block_excl_scan<kSortWarps>(tid < NB ? __ldg(ghist + tid) : 0u, s_scan);
+  uint32_t prefix = 0;
+  if (tid < NB && tile != 0) {
+    int t = (int)tile - 1;
+    bool done = false;
+    uint32_t polls = 0, steps = 0;
+    constexpr int kProbe = 4;   // status probes in flight per round (8 measured slower: more polling traffic, same wait)
+    while (!done) {
+      uint32_t v[kProbe];
+#pragma unroll
+      for (int q = 0; q < kProbe; ++q) v[q] = (t - q >= 0) ? lookback[(size_t)(t - q) * NB + tid] : (uint32_t)kFlagIncl;
+      int used = 0;
+      if (PHASES) polls += kProbe;
+#pragma unroll
+      for (int q = 0; q < kProbe; ++q) {
+        if (!done && used == q) {
+          if (v[q] != 0) {
+            prefix += v[q] & kValMask;
+            used = q + 1;
+            if (v[q] & kFlagIncl) done = true;
+          }
+        }
+      }
+      t -= used;
+      if (PHASES) steps += used;
+    }
+    *lb = kFlagIncl | (prefix + pub);
+    if (PHASES) {
+      atomicMax(&s_ph[0], globaltimer());
+      atomicMax(&s_ph[1], (unsigned long long)polls);
+      atomicMax(&s_ph[2], (unsigned long long)steps);
+    }
+  }
   if (tid < NB) {
     s_dig_start[tid] = dig_start;
     s_off[tid] = gbase + prefix - dig_start;
@@ -289,6 +315,17 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
     const uint32_t dst = j + s_off[(kv.x >> shift) & (NB - 1)];
     dst_k[dst] = kv.x;
     dst_v[dst] = kv.y;
+  }
+  if (PHASES) {
+    __syncthreads();
+    if (tid == 0) {
+      unsigned long long *rec = phases + (size_t)tile * kPhaseWords;
+      uint32_t smid;
+      asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+      rec[0] = t_start; rec[1] = t_keys; rec[2] = tile ? s_ph[0] : t_keys; rec[3] = globaltimer();
+      rec[4] = s_ph[1]; rec[5] = s_ph[2]; rec[6] = tile; rec[7] = ((unsigned long long)blockIdx.x << 32) | smid;
+      s_ph[0] = s_ph[1] = s_ph[2] = 0;
+    }
   }
   } while (PERSIST);
 }
@@ -420,7 +457,7 @@ uint32_t sm_count() {
 template <int BITS>
 static void launch_pass(uint32_t count_bound, bool persist, cudaStream_t s, const uint32_t *sk, const uint32_t *sv, uint32_t *dk,
                         uint32_t *dv, const uint32_t *d_count, int shift, const uint32_t *ghist, uint32_t *lookback, uint32_t *ticket,
-                        bool gather) {
+                        bool gather, unsigned long long *phases) {
   auto go = [&](auto kern) {
     const size_t smem = (size_t)kSortTileItems * 8 + (size_t)kSortWarps * (1u << BITS) * 4;
     // the opt-in for > 48 KB dynamic shared memory is per function AND per device
@@ -437,12 +474,15 @@ static void launch_pass(uint32_t count_bound, bool persist, cudaStream_t s, cons
     }
     uint32_t grid = (uint32_t)(((uint64_t)count_bound + kSortTileItems - 1) / kSortTileItems);
     if (persist) grid = min(grid, sm_count() * 2u);   // the 2 CTAs per SM that __launch_bounds__ asks for
-    kern<<<grid, kSortThreads, smem, s>>>(sk, sv, dk, dv, d_count, shift, ghist, lookback, ticket);
+    kern<<<grid, kSortThreads, smem, s>>>(sk, sv, dk, dv, d_count, shift, ghist, lookback, ticket, phases);
   };
+  if constexpr (BITS == 8) {   // the depth sort's digit width: the only one the phase diagnostics record
+    if (phases) { if (gather) go(k_onesweep<BITS, true, false, true>); else go(k_onesweep<BITS, false, false, true>); return; }
+  }
   if (persist) {
-    if (gather) go(k_onesweep<BITS, true, true>); else go(k_onesweep<BITS, false, true>);
+    if (gather) go(k_onesweep<BITS, true, true, false>); else go(k_onesweep<BITS, false, true, false>);
   } else {
-    if (gather) go(k_onesweep<BITS, true, false>); else go(k_onesweep<BITS, false, false>);
+    if (gather) go(k_onesweep<BITS, true, false, false>); else go(k_onesweep<BITS, false, false, false>);
   }
 }
 
@@ -473,18 +513,33 @@ cudaError_t launch_sort_pairs(uint32_t *keys, uint32_t *vals, const uint32_t *d_
     else if (bits == 7) k_sort_hist<2, 7><<<grid, 256, 0, s>>>(keys, d_count, sc.ghist);
     else k_sort_hist<2, 8><<<grid, 256, 0, s>>>(keys, d_count, sc.ghist);   // bits == 8: hist_ok rules out 9
   }
+  // GS_SORT_PHASES=1: the depth sort (the sort that gathers its keys through key_table) records its tiles' phases
+  static int want_phases = -1;
+  if (want_phases < 0) { const char *e = getenv("GS_SORT_PHASES"); want_phases = (e && e[0] == '1') ? 1 : 0; }
+  const bool phases = want_phases && key_table && bits == 8;
+  if (phases) {
+    if (g_sort_phase_tiles < tiles) {
+      cudaFree(g_sort_phases);
+      g_sort_phases = nullptr;
+      g_sort_phase_tiles = 0;
+      if (cudaMalloc(&g_sort_phases, (size_t)4 * tiles * kPhaseWords * 8) != cudaSuccess) return cudaErrorMemoryAllocation;
+      g_sort_phase_tiles = tiles;
+    }
+    cudaMemsetAsync(g_sort_phases, 0, (size_t)4 * g_sort_phase_tiles * kPhaseWords * 8, s);
+  }
   uint32_t *sk = keys, *sv = vals, *dk = sc.alt_keys, *dv = sc.alt_vals;
   for (int p = 0; p < passes; ++p) {
     if (pass_events) cudaEventRecord(pass_events[p], s);
     uint32_t *lb = sc.lookback + (size_t)p * tiles * nb;
+    unsigned long long *ph = phases ? g_sort_phases + (size_t)p * g_sort_phase_tiles * kPhaseWords : nullptr;
     const bool gather = key_table != nullptr && p == 0;   // pass 0 reads key_table[vals[i]] instead of keys[i]
     const uint32_t *src_keys = gather ? key_table : sk;
     if (p == passes - 1 && final_keys && final_vals) { dk = final_keys; dv = final_vals; }   // the last pass lands where the caller wants it
-    if (bits == 5) launch_pass<5>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
-    else if (bits == 6) launch_pass<6>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
-    else if (bits == 7) launch_pass<7>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
-    else if (bits == 8) launch_pass<8>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
-    else launch_pass<9>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather);
+    if (bits == 5) launch_pass<5>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather, ph);
+    else if (bits == 6) launch_pass<6>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather, ph);
+    else if (bits == 7) launch_pass<7>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather, ph);
+    else if (bits == 8) launch_pass<8>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather, ph);
+    else launch_pass<9>(capacity, persist, s, src_keys, sv, dk, dv, d_count, bits * p, sc.ghist + 256 * p, lb, sc.tickets + p, gather, ph);
     uint32_t *t = sk; sk = dk; dk = t;
     t = sv; sv = dv; dv = t;
   }
