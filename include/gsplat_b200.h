@@ -234,6 +234,32 @@ GS_API int gs_composite(GsContext *ctx, const GsImage *rt, GsImage *camera_targe
  * returns GS_ERR_NOT_READY -- call gs_calc_view when the buffer itself is wanted. */
 GS_API int gs_frame(GsContext *ctx, GsAsset *asset, const GsFrameParams *fp,
                     const GsRenderOptions *opt, int do_sort, GsImage *rt, GsImage *camera_target);
+/* GaussianSplatRenderSystem.SortAndRenderSplats for one camera on one context (R/GaussianSplatRenderer.cs:73-105,108-169,
+ * 187-211): the render target cleared once, every object drawn into it in the caller's order (GatherSplatsForCamera), then
+ * one composite onto the camera target.
+ *   Result: rt, camera_target and every object's persistent draw order are bit-identical to gs_frame(assets[0], flags 0),
+ *   then gs_frame(assets[k], GS_FLAG_LOAD_RT) for k >= 1, then gs_composite(rt, camera_target) when camera_target is given --
+ *   for both blend modes and both pixel formats.
+ *   assets, fps, do_sort  [object_count]: each object's asset (of this context, each listed once), uniforms and
+ *                   m_FrameCounter % m_SortNthFrame == 0.  All objects must share screen_w / screen_h.
+ *   opt             blend_mode and GS_FLAG_ASYNC_READBACK (as gs_frame); may be NULL.
+ *   rt, camera_target  host, device or CUDA-array memory, screen-sized; at least one must be given.
+ * Per object, in order, on the context stream: the sort (when do_sort[k]) and the view-calc, as gs_frame.  Then consecutive
+ * objects are drawn together as one run: their bin-list entries go into one list, object after object, which is sorted once
+ * by bin id and drawn by one raster pass.  A run holds at most 16 objects, each with fewer than 2^28 splats, binding at most
+ * one scene depth buffer (the same scene_depth pointer and memory); a new run starts where one of these would break, and
+ * blends under what the earlier runs drew.  Any object count is accepted.  With one object the call does the device work of
+ * gs_frame.  The bin-list capacity of a run is clamp(8 x its summed splat count, 4 Mi, 768 Mi) entries; a run that needs more
+ * reports GS_ERR_OUT_OF_MEMORY as gs_frame does (at gs_sync when nothing is read back to the host).
+ * GsStageTimes after this call: bin_ms, raster_ms, composite_ms and tile_entries are those of the call's draw when it forms one
+ * run; with several runs, bin_ms runs from the end of the last view-calc to the end of the last run's bin sort, and raster_ms
+ * and tile_entries are the last run's.  distances_ms, sort_ms, sort_pass_ms and view_ms are those of the last object that
+ * was sorted / view-calculated; total_ms spans the whole call; kernel_launches counts every kernel.
+ * GS_ERR_INVALID_ARGUMENT, with nothing enqueued and nothing written: a NULL ctx, assets, fps or do_sort; object_count 0;
+ * a NULL asset; an asset listed twice or of another context; objects of different screen sizes; GS_FLAG_LOAD_RT, a
+ * partition, row_begin / row_end or band_packed in opt.  Image errors are reported as gs_frame reports them. */
+GS_API int gs_frame_objects(GsContext *ctx, uint32_t object_count, GsAsset *const *assets, const GsFrameParams *fps,
+                            const int32_t *do_sort, const GsRenderOptions *opt, GsImage *rt, GsImage *camera_target);
 
 /* Multi-GPU epilogue (SURVEY 8e.1): `gathered` is the all-gather of every partition's band-packed
  * render target, [partition_count][rows_per_partition][width] pixels in DEVICE memory, where
@@ -424,7 +450,9 @@ GS_API int gs_debug_sort_phases(GsContext *ctx, uint64_t *out, uint32_t max_word
  * the requested entry point and stores its GsStatus in `status` -- "log and skip", never a throw across the boundary. */
 typedef enum GsUnityEvent {
   GS_UNITY_EVENT_FRAME = 1,   /* gs_frame(ctx, asset, &params, &options, do_sort, has_rt ? &rt : NULL, has_camera_target ? &camera_target : NULL) */
-  GS_UNITY_EVENT_SYNC = 2     /* gs_sync(ctx) */
+  GS_UNITY_EVENT_SYNC = 2,    /* gs_sync(ctx) */
+  GS_UNITY_EVENT_FRAME_OBJECTS = 3   /* data is a GsUnityFrameObjectsEvent: gs_frame_objects(ctx, object_count, assets, fps,
+                                        do_sort, &options, has_rt ? &rt : NULL, has_camera_target ? &camera_target : NULL) */
 } GsUnityEvent;
 
 typedef struct GsUnityFrameEvent {
@@ -438,9 +466,24 @@ typedef struct GsUnityFrameEvent {
   GsImage rt, camera_target;
 } GsUnityFrameEvent;
 
+/* One camera's splat objects (GS_UNITY_EVENT_FRAME_OBJECTS).  The three arrays are the managed side's, kept alive (pinned)
+ * with the payload until the command buffer has executed. */
+typedef struct GsUnityFrameObjectsEvent {
+  GsContext *ctx;
+  uint32_t object_count, reserved0;
+  GsAsset *const *assets;     /* [object_count] */
+  const GsFrameParams *fps;   /* [object_count] */
+  const int32_t *do_sort;     /* [object_count] */
+  GsRenderOptions options;
+  int32_t status;             /* out: GsStatus of the call (GS_ERR_NOT_READY until the event has run) */
+  uint32_t has_rt, has_camera_target, reserved1;
+  GsImage rt, camera_target;
+} GsUnityFrameObjectsEvent;
+
 typedef void (*GsUnityRenderEventAndDataFunc)(int event_id, void *data);
 GS_API GsUnityRenderEventAndDataFunc gs_unity_get_render_event_func(void);
 GS_API uint32_t gs_unity_frame_event_size(void);   /* sizeof(GsUnityFrameEvent), for the managed side's layout check */
+GS_API uint32_t gs_unity_frame_objects_event_size(void);   /* sizeof(GsUnityFrameObjectsEvent) */
 
 /* ---- device-pointer access for zero-copy hosts (torch / CUDA-Vulkan interop) ----- */
 GS_API void *gs_context_stream(GsContext *ctx);

@@ -5,8 +5,11 @@
 // What it replaces: the per-renderer body of GaussianSplatRenderSystem.SortAndRenderSplats
 // (package/Runtime/GaussianSplatRenderer.cs:118-166: SortPoints + CalcViewData + DrawProcedural) by ONE native event on
 // Unity's render thread.  The native side of the event (gs_unity_get_render_event_func, GsUnityFrameEvent in
-// include/gsplat_b200.h) is built and tested here (tests/test_zz_unity_event.py).
+// include/gsplat_b200.h) is built and tested here (tests/test_zz_unity_event.py).  GaussianSplatNativeCameraFrame below
+// records ONE event for all of a camera's active splat objects (GS_UNITY_EVENT_FRAME_OBJECTS -> gs_frame_objects; tested in
+// tests/test_gpu_frame_objects.py).
 using System;
+using System.Collections.Generic;
 using System.Runtime.InteropServices;
 using Unity.Collections;
 using Unity.Collections.LowLevel.Unsafe;
@@ -33,7 +36,7 @@ namespace GaussianSplatting.Runtime
         [DllImport("gsplat_b200")] static extern uint gs_unity_frame_event_size();
 
         const int kEventFrame = 1;                                  // GS_UNITY_EVENT_FRAME
-        const int kInFlight = 3;                                    // command buffers may execute up to 2 frames late
+        internal const int kInFlight = 3;                                   // command buffers may execute up to 2 frames late
         NativeArray<GsUnityFrameEvent> m_Events;                    // persistent => stable address, no GC pinning needed
         // The reference binds _SplatCutouts / _SplatDeletedBits / _SplatSelectedBits on every CalcViewData (SetAssetDataOnCS,
         // R/GaussianSplatRenderer.cs:485-509).  The native frame takes them as HOST arrays borrowed until the event has run,
@@ -43,7 +46,7 @@ namespace GaussianSplatting.Runtime
         NativeArray<GaussianCutout.ShaderData>[] m_Cutouts = new NativeArray<GaussianCutout.ShaderData>[kInFlight];
         NativeArray<uint>[] m_Deleted = new NativeArray<uint>[kInFlight], m_Selected = new NativeArray<uint>[kInFlight];
         int m_Next;
-        static readonly IntPtr s_EventFunc = gs_unity_get_render_event_func();
+        internal static readonly IntPtr s_EventFunc = gs_unity_get_render_event_func();
 
         public GaussianSplatNativeFrame()
         {
@@ -73,6 +76,7 @@ namespace GaussianSplatting.Runtime
             dst.CopyFrom(src);
         }
 
+
         /// Records the native frame into `cmb`.  `rtArray` is the cudaArray_t of _GaussianSplatRT's R16G16B16A16_SFloat image
         /// that the graphics-interop plugin imported (cudaImportExternalMemory -> cudaExternalMemoryGetMappedMipmappedArray with
         /// cudaArraySurfaceLoadStore -> cudaGetMipmappedArrayLevel 0; INTEGRATION.md section 3).  The library renders into it in
@@ -85,10 +89,30 @@ namespace GaussianSplatting.Runtime
             if (ev->ctx != IntPtr.Zero && ev->status != 0 && ev->status != -5)
                 GaussianSplatNative.Check(ev->ctx, ev->status);
 
-            var tr = gs.transform;
             ev->ctx = ctx;
             ev->asset = asset;
-            ev->fp = new GaussianSplatNative.GsFrameParams
+            ev->fp = FillParams(m_Next, gs, cam, rtWidth, rtHeight, hostDeletedBits, hostSelectedBits);
+            ev->options = default;                                                    // fp16-ROP blend, whole image
+            ev->do_sort = gs.m_FrameCounter % gs.m_SortNthFrame == 0 ? 1 : 0;         // :120-121
+            ev->status = -5;                                                          // GS_ERR_NOT_READY until it has run
+            ev->has_rt = 1; ev->has_camera_target = 0;
+            ev->rt = new GaussianSplatNative.GsImage
+            {
+                data = (void*)rtArray, width = (uint)rtWidth, height = (uint)rtHeight,
+                row_pitch_bytes = 0, format = 0 /* GS_PIX_RGBA16F */, memory = 2 /* GS_MEM_ARRAY */
+            };
+            ++gs.m_FrameCounter;
+            cmb.IssuePluginEventAndData(s_EventFunc, kEventFrame, (IntPtr)ev);
+            m_Next = (m_Next + 1) % kInFlight;
+        }
+
+        /// The renderer's uniforms for in-flight slot `slot`.  The cutouts and bits they point to are this object's copies for
+        /// that slot, alive until the slot is used again kInFlight events later.
+        internal GaussianSplatNative.GsFrameParams FillParams(int slot, GaussianSplatRenderer gs, Camera cam, int rtWidth, int rtHeight,
+                                                              NativeArray<uint> hostDeletedBits, NativeArray<uint> hostSelectedBits)
+        {
+            var tr = gs.transform;
+            var fp = new GaussianSplatNative.GsFrameParams
             {
                 mat_object_to_world = tr.localToWorldMatrix,
                 mat_world_to_object = tr.worldToLocalMatrix,
@@ -101,39 +125,123 @@ namespace GaussianSplatting.Runtime
             };
             // cutouts: the ShaderData records UpdateCutoutsBuffer builds (R/GaussianSplatRenderer.cs:511-531), matrix = cutout
             // worldToLocal * renderer localToWorld (R/GaussianCutout.cs:26-40)
-            int slot = m_Next;
-            ev->fp.cutouts = null; ev->fp.cutout_count = 0; ev->fp.deleted_bits = null; ev->fp.selected_bits = null;
+            fp.cutouts = null; fp.cutout_count = 0; fp.deleted_bits = null; fp.selected_bits = null;
             if (gs.m_Cutouts != null && gs.m_Cutouts.Length > 0)
             {
                 var data = new NativeArray<GaussianCutout.ShaderData>(gs.m_Cutouts.Length, Allocator.Temp);
                 for (int i = 0; i < gs.m_Cutouts.Length; ++i) data[i] = GaussianCutout.GetShaderData(gs.m_Cutouts[i], tr.localToWorldMatrix);
                 CopyInto(ref m_Cutouts[slot], data);
                 data.Dispose();
-                ev->fp.cutouts = (GaussianCutout.ShaderData*)m_Cutouts[slot].GetUnsafePtr();
-                ev->fp.cutout_count = (uint)m_Cutouts[slot].Length;
+                fp.cutouts = (GaussianCutout.ShaderData*)m_Cutouts[slot].GetUnsafePtr();
+                fp.cutout_count = (uint)m_Cutouts[slot].Length;
             }
             int words = (gs.splatCount + 31) / 32;
             if (hostDeletedBits.IsCreated && hostDeletedBits.Length >= words)
             {
                 CopyInto(ref m_Deleted[slot], hostDeletedBits);
-                ev->fp.deleted_bits = (uint*)m_Deleted[slot].GetUnsafePtr();
+                fp.deleted_bits = (uint*)m_Deleted[slot].GetUnsafePtr();
             }
             if (hostSelectedBits.IsCreated && hostSelectedBits.Length >= words)
             {
                 CopyInto(ref m_Selected[slot], hostSelectedBits);
-                ev->fp.selected_bits = (uint*)m_Selected[slot].GetUnsafePtr();
+                fp.selected_bits = (uint*)m_Selected[slot].GetUnsafePtr();
             }
-            ev->options = default;                                                    // fp16-ROP blend, whole image
-            ev->do_sort = gs.m_FrameCounter % gs.m_SortNthFrame == 0 ? 1 : 0;         // :120-121
-            ev->status = -5;                                                          // GS_ERR_NOT_READY until it has run
+            return fp;
+        }
+    }
+
+    /// One per camera: the camera's active splat objects, in GatherSplatsForCamera order, drawn by ONE native event
+    /// (GS_UNITY_EVENT_FRAME_OBJECTS -> gs_frame_objects): _GaussianSplatRT cleared once, one bin list and one raster for all
+    /// of them, instead of one event per object.  Each object keeps its GaussianSplatNativeFrame for its cutout and bit
+    /// copies; every asset must live on `ctx`.
+    internal sealed unsafe class GaussianSplatNativeCameraFrame : IDisposable
+    {
+        [StructLayout(LayoutKind.Sequential)]
+        struct GsUnityFrameObjectsEvent                             // include/gsplat_b200.h (size checked against gs_unity_frame_objects_event_size)
+        {
+            public IntPtr ctx;
+            public uint object_count, reserved0;
+            public IntPtr* assets;
+            public GaussianSplatNative.GsFrameParams* fps;
+            public int* do_sort;
+            public GaussianSplatNative.GsRenderOptions options;
+            public int status;
+            public uint has_rt, has_camera_target, reserved1;
+            public GaussianSplatNative.GsImage rt, camera_target;
+        }
+
+        [DllImport("gsplat_b200")] static extern uint gs_unity_frame_objects_event_size();
+
+        const int kEventFrameObjects = 3;                           // GS_UNITY_EVENT_FRAME_OBJECTS
+        const int kInFlight = GaussianSplatNativeFrame.kInFlight;
+        NativeArray<GsUnityFrameObjectsEvent> m_Events;
+        // what each in-flight event points to: the library reads these arrays on the render thread
+        NativeArray<IntPtr>[] m_Assets = new NativeArray<IntPtr>[kInFlight];
+        NativeArray<GaussianSplatNative.GsFrameParams>[] m_Params = new NativeArray<GaussianSplatNative.GsFrameParams>[kInFlight];
+        NativeArray<int>[] m_DoSort = new NativeArray<int>[kInFlight];
+        int m_Next;
+
+        public GaussianSplatNativeCameraFrame()
+        {
+            if (gs_unity_frame_objects_event_size() != (uint)UnsafeUtility.SizeOf<GsUnityFrameObjectsEvent>())
+                throw new InvalidOperationException("GsUnityFrameObjectsEvent layout mismatch between C# and libgsplat_b200");
+            m_Events = new NativeArray<GsUnityFrameObjectsEvent>(kInFlight, Allocator.Persistent);
+        }
+
+        public void Dispose()
+        {
+            if (m_Events.IsCreated) m_Events.Dispose();
+            for (int i = 0; i < kInFlight; ++i)
+            {
+                if (m_Assets[i].IsCreated) m_Assets[i].Dispose();
+                if (m_Params[i].IsCreated) m_Params[i].Dispose();
+                if (m_DoSort[i].IsCreated) m_DoSort[i].Dispose();
+            }
+        }
+
+        static void Ensure<T>(ref NativeArray<T> a, int n) where T : unmanaged
+        {
+            if (a.IsCreated && a.Length == n) return;
+            if (a.IsCreated) a.Dispose();
+            a = new NativeArray<T>(n, Allocator.Persistent, NativeArrayOptions.UninitializedMemory);
+        }
+
+        /// Records the camera's frame into `cmb`: `active` in GatherSplatsForCamera order (R/GaussianSplatRenderer.cs:73-105), each
+        /// object with its storage and its asset on `ctx`; `rtArray` as in GaussianSplatNativeFrame.Record.  The composite draw
+        /// that follows in the reference (:206-210) stays as it is.
+        public void Record(CommandBuffer cmb, List<(GaussianSplatRenderer gs, GaussianSplatNativeFrame storage, IntPtr asset)> active,
+                           Camera cam, IntPtr ctx, IntPtr rtArray, int rtWidth, int rtHeight)
+        {
+            if (active.Count == 0) return;   // no active splat object: OnPreCullCamera draws nothing
+            var ev = (GsUnityFrameObjectsEvent*)m_Events.GetUnsafePtr() + m_Next;
+            if (ev->ctx != IntPtr.Zero && ev->status != 0 && ev->status != -5)
+                GaussianSplatNative.Check(ev->ctx, ev->status);
+            int slot = m_Next, n = active.Count;
+            Ensure(ref m_Assets[slot], n);
+            Ensure(ref m_Params[slot], n);
+            Ensure(ref m_DoSort[slot], n);
+            for (int i = 0; i < n; ++i)
+            {
+                var (gs, storage, asset) = active[i];
+                m_Assets[slot][i] = asset;
+                m_Params[slot][i] = storage.FillParams(slot, gs, cam, rtWidth, rtHeight, default, default);
+                m_DoSort[slot][i] = gs.m_FrameCounter % gs.m_SortNthFrame == 0 ? 1 : 0;   // :120-121
+                ++gs.m_FrameCounter;
+            }
+            ev->ctx = ctx;
+            ev->object_count = (uint)n;
+            ev->assets = (IntPtr*)m_Assets[slot].GetUnsafePtr();
+            ev->fps = (GaussianSplatNative.GsFrameParams*)m_Params[slot].GetUnsafePtr();
+            ev->do_sort = (int*)m_DoSort[slot].GetUnsafePtr();
+            ev->options = default;                                  // fp16-ROP blend, whole image; the call clears the target once
+            ev->status = -5;                                        // GS_ERR_NOT_READY until it has run
             ev->has_rt = 1; ev->has_camera_target = 0;
             ev->rt = new GaussianSplatNative.GsImage
             {
                 data = (void*)rtArray, width = (uint)rtWidth, height = (uint)rtHeight,
                 row_pitch_bytes = 0, format = 0 /* GS_PIX_RGBA16F */, memory = 2 /* GS_MEM_ARRAY */
             };
-            ++gs.m_FrameCounter;
-            cmb.IssuePluginEventAndData(s_EventFunc, kEventFrame, (IntPtr)ev);
+            cmb.IssuePluginEventAndData(GaussianSplatNativeFrame.s_EventFunc, kEventFrameObjects, (IntPtr)ev);
             m_Next = (m_Next + 1) % kInFlight;
         }
     }

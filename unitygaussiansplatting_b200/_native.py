@@ -85,7 +85,14 @@ class GsUnityFrameEvent(C.Structure):   # include/gsplat_b200.h: the payload of 
                 ("rt", GsImage), ("camera_target", GsImage)]
 
 
-GS_UNITY_EVENT_FRAME, GS_UNITY_EVENT_SYNC = 1, 2
+class GsUnityFrameObjectsEvent(C.Structure):   # the payload of GS_UNITY_EVENT_FRAME_OBJECTS
+    _fields_ = [("ctx", C.c_void_p), ("object_count", C.c_uint32), ("reserved0", C.c_uint32), ("assets", C.c_void_p),
+                ("fps", C.c_void_p), ("do_sort", C.c_void_p), ("options", GsRenderOptions), ("status", C.c_int32),
+                ("has_rt", C.c_uint32), ("has_camera_target", C.c_uint32), ("reserved1", C.c_uint32),
+                ("rt", GsImage), ("camera_target", GsImage)]
+
+
+GS_UNITY_EVENT_FRAME, GS_UNITY_EVENT_SYNC, GS_UNITY_EVENT_FRAME_OBJECTS = 1, 2, 3
 GsUnityRenderEventAndDataFunc = C.CFUNCTYPE(None, C.c_int, C.c_void_p)
 
 
@@ -135,6 +142,8 @@ NATIVE_SYMBOLS = {
     "gs_composite": (C.c_int, [C.c_void_p, C.POINTER(GsImage), C.POINTER(GsImage)]),
     "gs_frame": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(GsFrameParams), C.POINTER(GsRenderOptions), C.c_int,
                            C.POINTER(GsImage), C.POINTER(GsImage)]),
+    "gs_frame_objects": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(GsFrameParams), C.POINTER(C.c_int32),
+                                   C.POINTER(GsRenderOptions), C.POINTER(GsImage), C.POINTER(GsImage)]),
     "gs_unshuffle_bands": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(GsImage)]),
     "gs_group_unique_id": (C.c_int, [C.c_void_p]),
     "gs_group_join": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_void_p)]),
@@ -160,6 +169,7 @@ NATIVE_SYMBOLS = {
     "gs_upload_order": (C.c_int, [C.c_void_p, C.c_void_p]),
     "gs_unity_get_render_event_func": (GsUnityRenderEventAndDataFunc, []),
     "gs_unity_frame_event_size": (C.c_uint32, []),
+    "gs_unity_frame_objects_event_size": (C.c_uint32, []),
     "gs_export_splats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     "gs_debug_raster_stats": (C.c_int, [C.c_void_p, C.c_void_p]),
     "gs_debug_sort_phases": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]),

@@ -5,6 +5,7 @@
 // InitSortBuffers (R/GaussianSplatRenderer.cs:373-445), CalcViewData (:579-610), SortPoints
 // (:612-639) and SortAndRenderSplats (:108-169).  There is no CPU fallback anywhere: without
 // a CUDA device gs_create fails with GS_ERR_NO_DEVICE.
+#include <algorithm>
 #include <cstdio>
 #include <cstring>
 #include <new>
@@ -368,6 +369,26 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
   return GS_OK;
 }
 
+// raster-tile cost history (launch order); invalidated when the tile grid changes
+static int ensure_raster_tiles(GsContext *ctx, const FrameConsts &fc) {
+  // per-tile state is indexed by the tile's id in the whole image, whatever part of it this context composites
+  const uint32_t rtiles = (((uint32_t)fc.screenW + kTile - 1) / kTile) * fc.binsY * (kBin / kTile);
+  if (rtiles > ctx->raster_tiles_cap) {
+    cudaStreamSynchronize(ctx->stream);
+    cudaFree(ctx->bin.tile_cost); cudaFree(ctx->bin.tile_order);
+    ctx->bin.tile_cost = ctx->bin.tile_order = nullptr;
+    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.tile_cost, (size_t)rtiles * 4));
+    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.tile_order, (size_t)rtiles * 4));
+    ctx->raster_tiles_cap = rtiles;
+    ctx->raster_tiles_cur = 0;
+  }
+  if (rtiles != ctx->raster_tiles_cur) {
+    GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->bin.tile_cost, 0, (size_t)rtiles * 4, ctx->stream));
+    ctx->raster_tiles_cur = rtiles;
+  }
+  return GS_OK;
+}
+
 // binning + raster into a device image
 int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRenderOptions &opt, void *d_rt, uint32_t pitch,
                      uint32_t fmt, cudaSurfaceObject_t surf, cudaEvent_t bin_done) {
@@ -375,23 +396,7 @@ int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRender
   const uint32_t tiles = fc.binsX * fc.binsY;
   int rc = ensure_bin_scratch(ctx, as->av.n, tiles, 0);
   if (rc) return rc;
-  {  // raster-tile cost history (launch order); invalidated when the tile grid changes
-    // per-tile state is indexed by the tile's id in the whole image, whatever part of it this context composites
-    const uint32_t rtiles = (((uint32_t)fc.screenW + kTile - 1) / kTile) * fc.binsY * (kBin / kTile);
-    if (rtiles > ctx->raster_tiles_cap) {
-      cudaStreamSynchronize(ctx->stream);
-      cudaFree(ctx->bin.tile_cost); cudaFree(ctx->bin.tile_order);
-      ctx->bin.tile_cost = ctx->bin.tile_order = nullptr;
-      GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.tile_cost, (size_t)rtiles * 4));
-      GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.tile_order, (size_t)rtiles * 4));
-      ctx->raster_tiles_cap = rtiles;
-      ctx->raster_tiles_cur = 0;
-    }
-    if (rtiles != ctx->raster_tiles_cur) {
-      GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->bin.tile_cost, 0, (size_t)rtiles * 4, ctx->stream));
-      ctx->raster_tiles_cur = rtiles;
-    }
-  }
+  if ((rc = ensure_raster_tiles(ctx, fc))) return rc;
   int bin_launches = 0;
   BinScratch lists;
   GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->av.n, as->order, as->rect, as->block_bits, ctx->bin, ctx->sort, ctx->stream, &lists,
@@ -401,6 +406,43 @@ int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRender
   launch_raster(fc, opt, as->draw, lists, d_rt, pitch, fmt, surf, ctx->stream, ctx->cur_depth ? as->zndc : nullptr, ctx->cur_depth);
   rec(ctx, EV_RASTER1);
   ctx->launches += bin_launches + 3;  // bin_emit, look-back clear, 1-2 sort passes; bin_ranges, tile_order, raster
+  GS_CUDA_TRY(ctx, cudaGetLastError());
+  return GS_OK;
+}
+
+// One run of gs_frame_objects: the objects' entries in one bin list (object after object), one bin sort and one raster.
+// `first`: the run starts from a cleared target and clears the overflow flag; later runs blend under what is there.
+// depth_fp: the frame parameters whose scene depth buffer the run binds (every object of the run that binds one binds it).
+static int render_run(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *const *as, const GsFrameParams *fps,
+                      uint32_t count, bool first, const GsFrameParams *depth_fp, void *d_rt, uint32_t pitch, uint32_t fmt,
+                      cudaSurfaceObject_t surf) {
+  GsNvtxRange nvtx("GaussianSplat.Draw");
+  uint64_t total = 0;
+  BinObject bo[kRunObjects];
+  RasterObjects ro;
+  memset(&ro, 0, sizeof(ro));
+  bool extras = false;
+  for (uint32_t i = 0; i < count; ++i) {
+    const GsAsset *a = as[i];
+    total += a->av.n;
+    bo[i] = BinObject{a->av.n, a->order, a->rect, a->block_bits};
+    ro.draw[i] = a->draw;
+    if (fps[i].scene_depth) { ro.zndc[i] = a->zndc; ro.depth_mask |= 1u << i; }
+    extras |= fps[i].selected_bits != nullptr || fps[i].scene_depth != nullptr;   // what picks the extras raster for one object
+  }
+  int rc = ensure_bin_scratch(ctx, (uint32_t)std::min<uint64_t>(total, 0xFFFFFFFFu), fc.binsX * fc.binsY, 0);
+  if (rc) return rc;
+  if ((rc = ensure_raster_tiles(ctx, fc))) return rc;
+  if ((rc = bind_depth(ctx, depth_fp, ctx->stream))) return rc;
+  BinScratch lists;
+  int bin_launches = 0;
+  GS_CUDA_TRY(ctx, launch_binning_objects(fc, count, bo, first, ctx->bin, ctx->sort, ctx->stream, &lists, &bin_launches));
+  rec(ctx, EV_BIN1);
+  GsRenderOptions o = opt;
+  if (!first) o.flags |= GS_FLAG_LOAD_RT;
+  launch_raster_objects(fc, o, ro, extras, lists, d_rt, pitch, fmt, surf, ctx->stream, ctx->cur_depth);
+  rec(ctx, EV_RASTER1);
+  ctx->launches += bin_launches + 3;  // per object look-back clear + bin_emit, 1-2 sort passes; bin_ranges, tile_order, raster
   GS_CUDA_TRY(ctx, cudaGetLastError());
   return GS_OK;
 }
@@ -777,6 +819,78 @@ int gs_composite(GsContext *ctx, const GsImage *rt, GsImage *tgt) {
   return composite_impl(ctx, surfs, ctx->rt_scratch, tight, 0, rt->format, tgt, W, H, ctx->stream);
 }
 
+}  // extern "C"
+
+namespace gs {
+// The device image a frame draws into: `rt` itself when it is device or array memory, else library scratch (or, with
+// GS_FLAG_ASYNC_READBACK, one of the two asynchronous staging images) that a host `rt` is read back from.
+struct FrameImage {
+  void *d_rt = nullptr;            // nullptr: the CUDA array behind `surf`
+  uint32_t pitch = 0;
+  cudaSurfaceObject_t surf = 0;
+  bool async_rb = false;
+  int slot = 0;
+};
+
+// what gs_frame and gs_frame_objects do between their view-calcs and their draw; rt (when given) has passed image_ok
+static int begin_frame_image(GsContext *ctx, CallSurfaces &surfs, const GsRenderOptions &opt, GsImage *rt, uint32_t rt_pitch,
+                             uint32_t rt_fmt, const GsImage *tgt, uint32_t W, uint32_t H, FrameImage *fi) {
+  int rc = GS_OK;
+  const bool rt_dev = rt && rt->memory == GS_MEM_DEVICE, rt_arr = rt && rt->memory == GS_MEM_ARRAY, rt_host = rt && rt->memory == GS_MEM_HOST;
+  fi->async_rb = rt_host && !tgt && (opt.flags & GS_FLAG_ASYNC_READBACK) != 0;
+  if (rt_dev) { fi->d_rt = rt->data; fi->pitch = rt_pitch; }
+  else if (rt_arr) {   // rendered into in place, through a surface
+    if ((rc = surfs.make(rt, &fi->surf))) return rc;
+  } else if (fi->async_rb) {
+    if ((rc = ensure_async_readback(ctx))) return rc;
+    const int slot = fi->slot = ctx->rt_flip;
+    ctx->rt_flip ^= 1;
+    fi->pitch = W * pix_bytes(rt_fmt);
+    // the staging image of two frames ago: its copy must have left the device before this frame's raster overwrites it
+    if (ctx->copy_pending[slot]) GS_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy_done[slot], 0));
+    if (ctx->rt_async_bytes[slot] < (size_t)fi->pitch * H && ctx->copy_pending[slot]) GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->copy_stream));  // about to be freed
+    if ((rc = grow(ctx, &ctx->rt_async[slot], &ctx->rt_async_bytes[slot], (size_t)fi->pitch * H))) return rc;
+    fi->d_rt = ctx->rt_async[slot];
+    if ((rc = init_staging(ctx, opt, fi->d_rt, fi->pitch, W, H, rt_fmt, rt, rt_pitch))) return rc;
+  } else {
+    fi->pitch = W * pix_bytes(rt_fmt);
+    if ((rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)fi->pitch * H))) return rc;
+    fi->d_rt = ctx->rt_scratch;
+    if ((rc = init_staging(ctx, opt, fi->d_rt, fi->pitch, W, H, rt_fmt, rt, rt_pitch))) return rc;
+  }
+  return GS_OK;
+}
+
+// what follows the draw: the read-back of a host `rt` (enqueued only, with GS_FLAG_ASYNC_READBACK), the composite onto the
+// camera target, and the bin-list check of a call that waits for the device anyway
+static int end_frame_image(GsContext *ctx, CallSurfaces &surfs, GsImage *rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W,
+                           uint32_t H, const FrameImage &fi) {
+  int rc = GS_OK;
+  const bool rt_host = rt && rt->memory == GS_MEM_HOST;
+  if (fi.async_rb) {
+    const int slot = fi.slot;
+    GS_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_rt_ready[slot], ctx->stream));
+    GS_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_rt_ready[slot], 0));
+    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, rt_pitch, fi.d_rt, fi.pitch, (size_t)W * pix_bytes(rt_fmt), H, cudaMemcpyDeviceToHost, ctx->copy_stream));
+    GS_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_copy_done[slot], ctx->copy_stream));
+    ctx->copy_pending[slot] = true;
+    return GS_OK;   // completion and the bin-list check: gs_sync
+  }
+  if (rt_host) {
+    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, rt_pitch, fi.d_rt, fi.pitch, (size_t)W * pix_bytes(rt_fmt), H, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  bool synced = false;
+  if (tgt) {
+    if ((rc = composite_impl(ctx, surfs, fi.d_rt, fi.pitch, fi.surf, rt_fmt, tgt, W, H, ctx->stream))) return rc;
+    synced = tgt->memory == GS_MEM_HOST;
+  }
+  if (rt_host || synced) return check_bin_overflow(ctx);
+  return GS_OK;
+}
+}  // namespace gs
+
+extern "C" {
+
 int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRenderOptions *opt_in, int do_sort_flag, GsImage *rt,
              GsImage *tgt) {
   int rc = check_params(ctx, as, fp);
@@ -795,54 +909,83 @@ int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRende
   for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
   if (do_sort_flag && (rc = do_sort(ctx, as, fc))) return rc;
   if ((rc = do_view(ctx, as, fp, fc, true, opt, ctx->stream))) return rc;   // fused frame: colour of never-drawn splats is dead code
-  void *d_rt;
-  uint32_t d_pitch;
-  cudaSurfaceObject_t rt_surf = 0;
   CallSurfaces surfs(ctx);
-  const bool rt_dev = rt && rt->memory == GS_MEM_DEVICE, rt_arr = rt && rt->memory == GS_MEM_ARRAY, rt_host = rt && rt->memory == GS_MEM_HOST;
-  const bool async_rb = rt_host && !tgt && (opt.flags & GS_FLAG_ASYNC_READBACK) != 0;
-  int slot = 0;
-  if (rt_dev) { d_rt = rt->data; d_pitch = rt_pitch; }
-  else if (rt_arr) {   // rendered into in place, through a surface
-    d_rt = nullptr; d_pitch = 0;
-    if ((rc = surfs.make(rt, &rt_surf))) return rc;
-  } else if (async_rb) {
-    if ((rc = ensure_async_readback(ctx))) return rc;
-    slot = ctx->rt_flip;
-    ctx->rt_flip ^= 1;
-    d_pitch = W * pix_bytes(rt_fmt);
-    // the staging image of two frames ago: its copy must have left the device before this frame's raster overwrites it
-    if (ctx->copy_pending[slot]) GS_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy_done[slot], 0));
-    if (ctx->rt_async_bytes[slot] < (size_t)d_pitch * H && ctx->copy_pending[slot]) GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->copy_stream));  // about to be freed
-    if ((rc = grow(ctx, &ctx->rt_async[slot], &ctx->rt_async_bytes[slot], (size_t)d_pitch * H))) return rc;
-    d_rt = ctx->rt_async[slot];
-    if ((rc = init_staging(ctx, opt, d_rt, d_pitch, W, H, rt_fmt, rt, rt_pitch))) return rc;
-  } else {
-    d_pitch = W * pix_bytes(rt_fmt);
-    if ((rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)d_pitch * H))) return rc;
-    d_rt = ctx->rt_scratch;
-    if ((rc = init_staging(ctx, opt, d_rt, d_pitch, W, H, rt_fmt, rt, rt_pitch))) return rc;
-  }
+  FrameImage fi;
+  if ((rc = begin_frame_image(ctx, surfs, opt, rt, rt_pitch, rt_fmt, tgt, W, H, &fi))) return rc;
   if ((rc = bind_depth(ctx, fp, ctx->stream))) return rc;
-  if ((rc = do_render(ctx, as, fc, opt, d_rt, d_pitch, rt_fmt, rt_surf))) return rc;
-  bool synced = false;
-  if (async_rb) {
-    GS_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_rt_ready[slot], ctx->stream));
-    GS_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_rt_ready[slot], 0));
-    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, rt_pitch, d_rt, d_pitch, (size_t)W * pix_bytes(rt_fmt), H, cudaMemcpyDeviceToHost, ctx->copy_stream));
-    GS_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_copy_done[slot], ctx->copy_stream));
-    ctx->copy_pending[slot] = true;
-    return GS_OK;   // completion and the bin-list check: gs_sync
+  if ((rc = do_render(ctx, as, fc, opt, fi.d_rt, fi.pitch, rt_fmt, fi.surf))) return rc;
+  return end_frame_image(ctx, surfs, rt, rt_pitch, rt_fmt, tgt, W, H, fi);
+}
+
+int gs_frame_objects(GsContext *ctx, uint32_t object_count, GsAsset *const *assets, const GsFrameParams *fps, const int32_t *do_sort_flags,
+                     const GsRenderOptions *opt_in, GsImage *rt, GsImage *tgt) {
+  if (!ctx || !assets || !fps || !do_sort_flags) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null context / assets / fps / do_sort");
+  const uint32_t K = object_count;
+  if (K == 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "object_count is 0");
+  int rc = GS_OK;
+  for (uint32_t k = 0; k < K; ++k) {
+    if (!assets[k]) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null asset");
+    if ((rc = check_params(ctx, assets[k], &fps[k]))) return rc;
+    if (fps[k].screen_w != fps[0].screen_w || fps[k].screen_h != fps[0].screen_h)
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the objects of one call must share screen_w / screen_h");
   }
-  if (rt_host) {
-    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, rt_pitch, d_rt, d_pitch, (size_t)W * pix_bytes(rt_fmt), H, cudaMemcpyDeviceToHost, ctx->stream));
+  {
+    std::vector<GsAsset *> sorted(assets, assets + K);
+    std::sort(sorted.begin(), sorted.end());
+    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "an asset is listed for two objects (its draw order would be sorted twice)");
   }
-  if (tgt) {
-    if ((rc = composite_impl(ctx, surfs, d_rt, d_pitch, rt_surf, rt_fmt, tgt, W, H, ctx->stream))) return rc;
-    synced = tgt->memory == GS_MEM_HOST;
+  if (!rt && !tgt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_frame_objects needs rt and/or camera_target");
+  GsRenderOptions opt = opt_in ? *opt_in : default_opts();
+  if (opt.flags & GS_FLAG_LOAD_RT) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "GS_FLAG_LOAD_RT is not accepted: the call clears the target once itself");
+  if (opt.partition_count > 1 || opt.partition_index || opt.row_begin || opt.row_end || opt.band_packed)
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_frame_objects draws the whole screen: no partition, row range or band packing");
+  std::vector<FrameConsts> fcs(K);
+  for (uint32_t k = 0; k < K; ++k) fcs[k] = make_frame_consts(&fps[k]);
+  if ((rc = check_options(ctx, fcs[0], opt))) return rc;
+  const uint32_t W = (uint32_t)fps[0].screen_w, H = (uint32_t)fps[0].screen_h;
+  uint32_t rt_pitch = 0, tgt_pitch = 0, rt_fmt = GS_PIX_RGBA16F;
+  if (rt) { if ((rc = image_ok(ctx, rt, W, H, &rt_pitch))) return rc; rt_fmt = rt->format; }
+  if (tgt && (rc = image_ok(ctx, tgt, W, H, &tgt_pitch))) return rc;
+  // the objects' cutouts / bits share the context's buffers: sized for all of them before the first view-calc is queued
+  for (uint32_t k = 0; k < K; ++k)
+    if ((rc = reserve_frame_inputs(ctx, assets[k], &fps[k]))) return rc;
+
+  for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
+  for (uint32_t k = 0; k < K; ++k) {
+    if (do_sort_flags[k] && (rc = do_sort(ctx, assets[k], fcs[k]))) return rc;
+    if ((rc = do_view(ctx, assets[k], &fps[k], fcs[k], true, opt, ctx->stream))) return rc;
   }
-  if (rt_host || synced) return check_bin_overflow(ctx);
-  return GS_OK;
+  CallSurfaces surfs(ctx);
+  FrameImage fi;
+  if ((rc = begin_frame_image(ctx, surfs, opt, rt, rt_pitch, rt_fmt, tgt, W, H, &fi))) return rc;
+  // Runs: consecutive objects drawn by one bin list and one raster -- at most kRunObjects, each with fewer than 2^kSlotShift
+  // splats (the slot tag), binding at most one scene depth buffer.  An object that fits no run, and the only object of a
+  // one-object call, is drawn by the kernels of gs_frame.
+  for (uint32_t k = 0; k < K;) {
+    const bool first = k == 0;
+    if (K == 1 || assets[k]->av.n > kLocalIdMask) {
+      // this draw's bin list check overwrites the overflow flag: report an earlier run's truncation first
+      if (!first && (rc = check_bin_overflow(ctx))) return rc;
+      GsRenderOptions o = opt;
+      if (!first) o.flags |= GS_FLAG_LOAD_RT;
+      if ((rc = bind_depth(ctx, &fps[k], ctx->stream))) return rc;
+      if ((rc = do_render(ctx, assets[k], fcs[k], o, fi.d_rt, fi.pitch, rt_fmt, fi.surf))) return rc;
+      ++k;
+      continue;
+    }
+    const GsFrameParams *depth_fp = &fps[k];
+    uint32_t e = k;
+    for (; e < K && e - k < kRunObjects && assets[e]->av.n <= kLocalIdMask; ++e) {
+      const GsFrameParams &f = fps[e];
+      if (!f.scene_depth) continue;
+      if (!depth_fp->scene_depth) depth_fp = &f;
+      else if (f.scene_depth != depth_fp->scene_depth || f.scene_depth_on_device != depth_fp->scene_depth_on_device) break;
+    }
+    if ((rc = render_run(ctx, fcs[k], opt, assets + k, fps + k, e - k, first, depth_fp, fi.d_rt, fi.pitch, rt_fmt, fi.surf))) return rc;
+    k = e;
+  }
+  return end_frame_image(ctx, surfs, rt, rt_pitch, rt_fmt, tgt, W, H, fi);
 }
 
 int gs_unshuffle_bands(GsContext *ctx, const void *gathered, uint32_t parts, uint32_t band_rows, uint32_t rows_pp, uint32_t fmt,
@@ -952,8 +1095,14 @@ int gs_upload_order(GsAsset *as, const uint32_t *src) {
 
 // ---- Unity render-thread entry: IssuePluginEventAndData -> gs_frame / gs_sync ----
 static void gs_unity_on_render_event(int event_id, void *data) {
+  if (!data) return;
+  if (event_id == GS_UNITY_EVENT_FRAME_OBJECTS) {
+    GsUnityFrameObjectsEvent *ev = static_cast<GsUnityFrameObjectsEvent *>(data);
+    ev->status = gs_frame_objects(ev->ctx, ev->object_count, ev->assets, ev->fps, ev->do_sort, &ev->options, ev->has_rt ? &ev->rt : nullptr,
+                                  ev->has_camera_target ? &ev->camera_target : nullptr);
+    return;
+  }
   GsUnityFrameEvent *ev = static_cast<GsUnityFrameEvent *>(data);
-  if (!ev) return;
   switch (event_id) {
     case GS_UNITY_EVENT_FRAME:
       ev->status = gs_frame(ev->ctx, ev->asset, &ev->params, &ev->options, ev->do_sort, ev->has_rt ? &ev->rt : nullptr,
@@ -968,6 +1117,7 @@ static void gs_unity_on_render_event(int event_id, void *data) {
 }
 GsUnityRenderEventAndDataFunc gs_unity_get_render_event_func(void) { return gs_unity_on_render_event; }
 uint32_t gs_unity_frame_event_size(void) { return (uint32_t)sizeof(GsUnityFrameEvent); }
+uint32_t gs_unity_frame_objects_event_size(void) { return (uint32_t)sizeof(GsUnityFrameObjectsEvent); }
 
 int gs_debug_raster_stats(GsContext *ctx, uint64_t out[8]) {
   if (!ctx || !out) return GS_ERR_INVALID_ARGUMENT;

@@ -181,6 +181,28 @@ struct BinScratch {
 cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, uint32_t n, const uint32_t *order, const uint32_t *rect,
                            const uint32_t *block_bits, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted,
                            int *launches);
+// Several splat objects drawn by one bin list and one raster (gs_frame_objects): a run of up to kRunObjects objects, each with
+// fewer than 2^kSlotShift splats.  Every list entry is (slot << kSlotShift) | splat id.
+constexpr uint32_t kRunObjects = 16, kSlotShift = 28, kLocalIdMask = (1u << kSlotShift) - 1u;
+struct BinObject {
+  uint32_t n;
+  const uint32_t *order, *rect, *block_bits;
+};
+// The objects' lists go into one list, object after object (slot k = objs[k]), and are sorted once by bin id.  clear_overflow:
+// this is the call's first run (later runs keep an earlier run's overflow flag).
+cudaError_t launch_binning_objects(const FrameConsts &fc, uint32_t count, const BinObject *objs, bool clear_overflow, const BinScratch &bs,
+                                   const SortScratch &sc, cudaStream_t s, BinScratch *sorted, int *launches);
+struct RasterObjects {
+  const float4 *draw[kRunObjects];   // each slot's raster records
+  const float *zndc[kRunObjects];    // each slot's quad depths, where that object is depth-tested
+  uint32_t depth_mask;               // bit k: slot k is depth-tested against the run's scene depth buffer
+};
+struct NoRasterObjects {};
+// The raster of one run into a full-screen target; `extras`: some object has a selection or a depth buffer.  opt: blend mode
+// and GS_FLAG_LOAD_RT.
+void launch_raster_objects(const FrameConsts &fc, const GsRenderOptions &opt, const RasterObjects &objs, bool extras, const BinScratch &bs,
+                           void *rt, uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s,
+                           const float *scene_depth);
 // zndc / scene_depth: per-splat quad depth and the W x H depth buffer to test it against (both nullptr: no depth test).
 // Images here are linear device memory (pointer, pitch) or, when the pointer is null, a CUDA array behind a surface object.
 void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const BinScratch &bs, void *rt,

@@ -21,6 +21,7 @@
 //               every splat (GS_BLEND_FP16_ROP) -- or kept in float32 (GS_BLEND_FP32).
 //   3. composite (S/GaussianComposite.shader:35-39).
 #include <cstdlib>
+#include <type_traits>
 
 #include "gs_kernels.cuh"
 
@@ -44,15 +45,23 @@ __device__ __forceinline__ uint32_t entry_tile(uint32_t e, uint32_t r, const Par
   return ty * tilesX + x0 + col;
 }
 
+// APPEND (several objects into one list): the entries go behind the entry_count[2] already listed, each value is tagged
+// `tag | splat id` (tag = the object's slot << kSlotShift), and the overflow flag entry_count[1] is sticky.
+template <bool APPEND>
 __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ order, const uint32_t *__restrict__ rect,
                                                   const uint32_t *__restrict__ block_bits, uint32_t bits_words, uint32_t n, Partition part,
                                                   uint32_t tilesX, volatile uint32_t *status,
                                                   uint32_t *ticket, uint32_t capacity, uint32_t *__restrict__ keys,
                                                   uint32_t *__restrict__ vals, uint32_t *__restrict__ entry_count,
-                                                  uint32_t *__restrict__ ghist, uint32_t digit_bits, bool two_pass) {
+                                                  uint32_t *__restrict__ ghist, uint32_t digit_bits, bool two_pass, uint32_t tag) {
   extern __shared__ uint32_t s_bits[];   // the view kernel's block bitmap (bits_words words), or nothing when it is too large to hold
   __shared__ uint32_t s_w[8];
-  __shared__ uint32_t s_block, s_excl;
+  __shared__ uint32_t s_block, s_excl, s_base;
+  if (APPEND && threadIdx.x == 0) {
+    // read before this block publishes its status: the last block writes the new total only after every block has published
+    s_base = *(volatile uint32_t *)(entry_count + 2);
+    __threadfence();
+  }
   __shared__ uint32_t s_dh[512];   // digit histograms of the sort by the bin ids we emit: [0,256) pass 0 and [256,512) pass 1
                                    // of two passes, or all 512 for one pass of up to 9 bits (ghist's layout)
   __shared__ uint2 s_items[kBinBlock];     // per warp: its drawable ranks, squeezed together in order
@@ -136,10 +145,12 @@ __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ o
       if (lane == 0) status[b] = kBinFlagIncl | min(excl + total, (uint32_t)kBinValMask);
     }
     if (lane == 0) {
+      if (APPEND) excl = min(s_base + excl, (uint32_t)kBinValMask);
       s_excl = excl;
       if (b == nblocks - 1) {
         const uint32_t all = min(excl + total, (uint32_t)kBinValMask);
-        entry_count[1] = all > capacity ? 1u : 0u;   // overflow: lists are truncated, the API reports it
+        if (APPEND) { if (all > capacity) entry_count[1] = 1u; }
+        else entry_count[1] = all > capacity ? 1u : 0u;   // overflow: lists are truncated, the API reports it
         entry_count[0] = all > capacity ? capacity : all;
         entry_count[2] = all;
       }
@@ -174,7 +185,7 @@ __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ o
       if (x < T && o < capacity) {
         const uint32_t tile = entry_tile(x - opre, orc, part, tilesX);
         keys[o] = tile;
-        vals[o] = oid;
+        vals[o] = APPEND ? (tag | oid) : oid;
         atomicAdd(&s_dh[tile & dmask], 1u);
         if (two_pass) atomicAdd(&s_dh[256 + ((tile >> digit_bits) & dmask)], 1u);
       }
@@ -216,13 +227,44 @@ cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, ui
   if (bits_global) words = 0;
   if (words * 4u > 16u * 1024u) words = 0;   // beside the kernel's 28 KB of static shared memory only 20 KB of the default 48 remain:
                                               // a larger bitmap (> 33 M splats) is read through L1 instead
-  k_bin_emit<<<nblocks, 256, words * 4u, s>>>(order, rect, block_bits, words, n, part, fc.binsX, bs.block_sums + 1, bs.block_sums, bs.capacity,
-                                     bs.tile_keys, bs.tile_vals, bs.entry_count, sc.ghist, (uint32_t)bits, passes == 2);
+  k_bin_emit<false><<<nblocks, 256, words * 4u, s>>>(order, rect, block_bits, words, n, part, fc.binsX, bs.block_sums + 1, bs.block_sums,
+                                                     bs.capacity, bs.tile_keys, bs.tile_vals, bs.entry_count, sc.ghist, (uint32_t)bits,
+                                                     passes == 2, 0u);
   // the entry count lives on the device: a persistent grid sorts whatever it is (no capacity-sized grid or memset)
   const cudaError_t e = launch_sort_pairs(bs.tile_keys, bs.tile_vals, bs.entry_count, bs.capacity, passes, bits, true, sc, s, nullptr,
                                           nullptr, /*count_is_capacity=*/false);
   if (e != cudaSuccess) return e;
   // an odd number of passes leaves the sorted lists in the sorter's ping-pong buffers
+  if (passes & 1) { sorted->tile_keys = sc.alt_keys; sorted->tile_vals = sc.alt_vals; }
+  return cudaSuccess;
+}
+
+cudaError_t launch_binning_objects(const FrameConsts &fc, uint32_t count, const BinObject *objs, bool clear_overflow, const BinScratch &bs,
+                                   const SortScratch &sc, cudaStream_t s, BinScratch *sorted, int *launches) {
+  const Partition part = make_partition(GsRenderOptions{});
+  const uint32_t tiles = fc.binsX * fc.binsY;
+  *sorted = bs;
+  int bits, passes;
+  bin_sort_plan(tiles, &bits, &passes);
+  *launches = 0;
+  // [0] and [2] start from an empty list; [1] (overflow) is kept across the runs of one call unless clear_overflow
+  cudaMemsetAsync(bs.entry_count + (clear_overflow ? 0 : 2), 0, (clear_overflow ? 3 : 1) * sizeof(uint32_t), s);
+  cudaMemsetAsync(sc.ghist, 0, 4 * 256 * sizeof(uint32_t), s);
+  for (uint32_t k = 0; k < count; ++k) {
+    const BinObject &o = objs[k];
+    const uint32_t nblocks = (o.n + kBinBlock - 1) / kBinBlock;
+    cudaMemsetAsync(bs.block_sums, 0, ((size_t)nblocks + 1) * sizeof(uint32_t), s);   // [0] ticket, [1..] look-back status
+    uint32_t words = (uint32_t)block_bits_words(o.n);
+    if (words * 4u > 16u * 1024u) words = 0;   // as launch_binning: a bitmap above 16 KB is read through L1
+    k_bin_emit<true><<<nblocks, 256, words * 4u, s>>>(o.order, o.rect, o.block_bits, words, o.n, part, fc.binsX, bs.block_sums + 1,
+                                                      bs.block_sums, bs.capacity, bs.tile_keys, bs.tile_vals, bs.entry_count, sc.ghist,
+                                                      (uint32_t)bits, passes == 2, k << kSlotShift);
+    *launches += 2;   // look-back clear, bin_emit
+  }
+  *launches += passes;
+  const cudaError_t e = launch_sort_pairs(bs.tile_keys, bs.tile_vals, bs.entry_count, bs.capacity, passes, bits, true, sc, s, nullptr,
+                                          nullptr, /*count_is_capacity=*/false);
+  if (e != cudaSuccess) return e;
   if (passes & 1) { sorted->tile_keys = sc.alt_keys; sorted->tile_vals = sc.alt_vals; }
   return cudaSuccess;
 }
@@ -349,12 +391,15 @@ __device__ __forceinline__ bool block_may_touch_quad(const float4 &A, float i2x,
 // (reversed Z: quad depth >= stored depth), the per-splat quad depths being staged beside the records.
 // SURF: the target is a CUDA array (GS_MEM_ARRAY), read and written through the surface object `surf` instead of `rt`/`pitch`; a
 // separate instantiation so that the linear ones keep their code.
-template <bool FP16_ROP, int OUT_FMT, bool STATS, bool SEL = false, bool SURF = false>
+// MULTI: the list holds the entries of several objects (one run of gs_frame_objects), each tagged with its slot in `objs`; the
+// records are gathered from that object's buffers, and the result is what drawing the objects one after the other leaves.
+template <bool FP16_ROP, int OUT_FMT, bool STATS, bool SEL = false, bool SURF = false, bool MULTI = false>
 __global__ void __launch_bounds__(256)
 k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const uint2 *__restrict__ bin_ranges,
          const uint32_t *__restrict__ tile_vals, const uint32_t *__restrict__ tile_order, uint32_t *__restrict__ tile_cost, uint32_t ntx,
          uint8_t *__restrict__ rt, uint32_t pitch, cudaSurfaceObject_t surf, uint32_t band_packed, uint32_t load_rt,
-         unsigned long long *stats, const float *__restrict__ zndc, const float *__restrict__ scene_depth) {
+         unsigned long long *stats, const float *__restrict__ zndc, const float *__restrict__ scene_depth,
+         std::conditional_t<MULTI, RasterObjects, NoRasterObjects> objs) {
   uint32_t st_batches = 0, st_culls = 0, st_cand = 0, st_eval = 0, st_blend = 0;   // GS_RASTER_STATS diagnostics (per warp)
   unsigned long long st_t0 = 0;
   if (STATS) asm volatile("mov.u64 %0, %globaltimer;" : "=l"(st_t0));
@@ -363,6 +408,14 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   __shared__ __align__(128) float4 s_rec[2][3][256];  // plane 0: cx, cy, i1x, i1y   1: i2x, i2y, opacity, hx   2: r, g, b, hy
   __shared__ float s_z[SEL ? 2 : 1][SEL ? 256 : 1];   // quad depths of the staged batch (depth test only)
   const bool depth_test = SEL && scene_depth != nullptr;
+  // MULTI: the object table, staged where a slot can index it without local memory, and each staged entry's slot
+  __shared__ const float4 *s_draw[MULTI ? kRunObjects : 1];
+  __shared__ const float *s_zndc[MULTI ? kRunObjects : 1];
+  __shared__ uint8_t s_slot[MULTI ? 2 : 1][MULTI ? 256 : 1];
+  // FP32 blending into an RGBA16F target: drawing the objects one after the other stores (rounds to half) each object's result
+  // and the next object starts from it.  Rounding is idempotent, so rounding at the next object's first candidate is exact.
+  constexpr bool kRoundAtObject = MULTI && !FP16_ROP && OUT_FMT == GS_PIX_RGBA16F;
+  uint32_t depth_mask = 0, cur_slot = 0;
 
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   // 1-D grid over raster tiles: tile = (16-pixel column, R * own 64-pixel bin row + tile row inside that bin row)
@@ -375,6 +428,14 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   if (ty * kTile >= (uint32_t)fc.screenH) { if (threadIdx.x == 0) tile_cost[lin] = 0; return; }
   __shared__ uint32_t s_cost;
   if (threadIdx.x == 0) s_cost = 0;
+  if constexpr (MULTI) {
+    depth_mask = objs.depth_mask;
+    if (threadIdx.x == 0) {
+#pragma unroll
+      for (uint32_t k = 0; k < kRunObjects; ++k) { s_draw[k] = objs.draw[k]; s_zndc[k] = objs.zndc[k]; }
+    }
+    __syncthreads();
+  }
   // [start,end) of this tile's bin in the bin-sorted entry list (k_bin_ranges); R*R tiles share one list
   const uint2 range = __ldg(bin_ranges + brow * fc.binsX + (tx / R));
   const uint32_t bx = tx * kTile + (warp & 1) * 8, by = ty * kTile + (warp >> 1) * 4;
@@ -409,7 +470,17 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   // three-deep pipeline: splat ids of batch k+2 (register) -> records of batch k+1 (cp.async in flight) -> batch k (composited)
   auto load_id = [&](uint32_t e) -> uint32_t { return e < range.y ? __ldg(tile_vals + e) : 0xFFFFFFFFu; };
   auto stage = [&](int buf, uint32_t id) {
-    if (id != 0xFFFFFFFFu) {
+    if constexpr (MULTI) {
+      if (id != 0xFFFFFFFFu) {
+        const uint32_t slot = id >> kSlotShift, lid = id & kLocalIdMask;
+        s_slot[buf][tid] = (uint8_t)slot;
+        const float4 *src = s_draw[slot] + (size_t)lid * 3;
+        cp_async16(&s_rec[buf][0][tid], src);
+        cp_async16(&s_rec[buf][1][tid], src + 1);
+        cp_async16(&s_rec[buf][2][tid], src + 2);
+        if (SEL && depth_test && s_zndc[slot]) cp_async4(&s_z[SEL ? buf : 0][SEL ? tid : 0], s_zndc[slot] + lid);
+      }
+    } else if (id != 0xFFFFFFFFu) {
       const float4 *src = draw + (size_t)id * 3;
       cp_async16(&s_rec[buf][0][tid], src);
       cp_async16(&s_rec[buf][1][tid], src + 1);
@@ -458,6 +529,14 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
         const float qa = fmaf(dy, A.w, dx * A.z), qb = fmaf(dy, B.y, dx * B.x);
         const bool inside = (fabsf(qa) <= 2.0f) && (fabsf(qb) <= 2.0f);  // quad corners at +-2 (:54-55)
         if (!__any_sync(0xffffffffu, inside)) continue;
+        uint32_t slot = 0;
+        if constexpr (MULTI) {
+          slot = s_slot[buf][j];
+          if (kRoundAtObject && slot != cur_slot) {
+            cur_slot = slot;
+            d0 = round_half(d0); d1 = round_half(d1); d2 = round_half(d2); d3 = round_half(d3);
+          }
+        }
         ++st_eval;
         const float power = -fmaf(qb, qb, qa * qa);                       // -dot(i.pos, i.pos) (:81)
         float alpha = exp_neg(power);                                     // half alpha = exp(power) (:82)
@@ -474,7 +553,8 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
         // discard below 1/255 (:103-104); a pixel with dst.a == 1 ignores every later splat, as the early-outs assume: a zero
         // blend factor contributes nothing, even to an inf colour (DESIGN §4)
         bool pass = inside && alpha >= 0.003921569f && d3 != 1.0f;
-        if (SEL && depth_test) pass = pass && (s_z[SEL ? buf : 0][SEL ? j : 0] >= zscene);   // ZTest LEqual, reversed Z
+        if (SEL && depth_test && (!MULTI || ((depth_mask >> slot) & 1u)))
+          pass = pass && (s_z[SEL ? buf : 0][SEL ? j : 0] >= zscene);   // ZTest LEqual, reversed Z (MULTI: objects that bind it)
         if (pass) {
           if (STATS) ++st_blend;
           float4 C = s_c[j];
@@ -555,9 +635,9 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const floa
   k_bin_ranges<<<(bins + 7) / 8, 256, 0, s>>>(bs.tile_keys, bs.entry_count, bins, ranges);
 #define GS_LAUNCH_RASTER(ROP, FMT, SURF)                                                                                        \
   do {                                                                                                                         \
-    if (fc.selValid || scene_depth) k_raster<ROP, FMT, false, true, SURF><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed, load, stats, zndc, scene_depth); \
-    else if (stats) k_raster<ROP, FMT, true, false, SURF><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed, load, stats, nullptr, nullptr); \
-    else k_raster<ROP, FMT, false, false, SURF><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed, load, stats, nullptr, nullptr); \
+    if (fc.selValid || scene_depth) k_raster<ROP, FMT, false, true, SURF><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed, load, stats, zndc, scene_depth, NoRasterObjects{}); \
+    else if (stats) k_raster<ROP, FMT, true, false, SURF><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed, load, stats, nullptr, nullptr, NoRasterObjects{}); \
+    else k_raster<ROP, FMT, false, false, SURF><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed, load, stats, nullptr, nullptr, NoRasterObjects{}); \
   } while (0)
   // a null `rt` means the target is a CUDA array behind rt_surf
 #define GS_LAUNCH_RASTER_TARGET(ROP, FMT)                                                                                       \
@@ -571,6 +651,37 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const floa
   }
 #undef GS_LAUNCH_RASTER_TARGET
 #undef GS_LAUNCH_RASTER
+}
+
+void launch_raster_objects(const FrameConsts &fc, const GsRenderOptions &opt, const RasterObjects &objs, bool extras, const BinScratch &bs,
+                           void *rt, uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s,
+                           const float *scene_depth) {
+  const Partition part = make_partition(GsRenderOptions{});
+  const uint32_t ntx = ((uint32_t)fc.screenW + kTile - 1) / kTile, grid = ntx * part.own_tile_rows(fc.binsY);
+  if (!grid) return;
+  k_tile_order<<<1, 1024, 0, s>>>(bs.tile_cost, grid, ntx, part, bs.tile_order);
+  const uint32_t bins = fc.binsX * fc.binsY;
+  uint2 *ranges = reinterpret_cast<uint2 *>(bs.bin_ranges);
+  k_bin_ranges<<<(bins + 7) / 8, 256, 0, s>>>(bs.tile_keys, bs.entry_count, bins, ranges);
+  const bool rop = opt.blend_mode == GS_BLEND_FP16_ROP;
+  uint8_t *out = reinterpret_cast<uint8_t *>(rt);
+  const uint32_t load = (opt.flags & GS_FLAG_LOAD_RT) ? 1u : 0u;
+#define GS_LAUNCH_RASTER_OBJECTS(ROP, FMT, SURF)                                                                                \
+  do {                                                                                                                         \
+    if (extras) k_raster<ROP, FMT, false, true, SURF, true><<<grid, 256, 0, s>>>(fc, part, nullptr, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, 0u, load, nullptr, nullptr, scene_depth, objs); \
+    else k_raster<ROP, FMT, false, false, SURF, true><<<grid, 256, 0, s>>>(fc, part, nullptr, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, 0u, load, nullptr, nullptr, nullptr, objs); \
+  } while (0)
+#define GS_LAUNCH_RASTER_OBJECTS_TARGET(ROP, FMT)                                                                               \
+  do {                                                                                                                         \
+    if (out) GS_LAUNCH_RASTER_OBJECTS(ROP, FMT, false); else GS_LAUNCH_RASTER_OBJECTS(ROP, FMT, true);                          \
+  } while (0)
+  if (rt_format == GS_PIX_RGBA16F) {
+    if (rop) GS_LAUNCH_RASTER_OBJECTS_TARGET(true, GS_PIX_RGBA16F); else GS_LAUNCH_RASTER_OBJECTS_TARGET(false, GS_PIX_RGBA16F);
+  } else {
+    if (rop) GS_LAUNCH_RASTER_OBJECTS_TARGET(true, GS_PIX_RGBA32F); else GS_LAUNCH_RASTER_OBJECTS_TARGET(false, GS_PIX_RGBA32F);
+  }
+#undef GS_LAUNCH_RASTER_OBJECTS_TARGET
+#undef GS_LAUNCH_RASTER_OBJECTS
 }
 
 uint32_t partition_own_bin_rows(const GsRenderOptions &opt, uint32_t binsY) { return make_partition(opt).own_rows_below(binsY); }

@@ -44,6 +44,7 @@ class GaussianSplatRenderer {
   int m_SHOrder = 3;
   bool m_SHOnly = false;
   int m_SortNthFrame = 1;
+  int m_RenderOrder = 0;   // :236, higher values draw first
   Matrix4x4 localToWorldMatrix{{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}};
   Matrix4x4 worldToLocalMatrix{{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}};
   std::vector<GsCutout> m_Cutouts;
@@ -55,15 +56,27 @@ class GaussianSplatRenderer {
   bool OnEnable(const GsAssetDesc &asset, int cudaDevice = 0, void *stream = nullptr) {
     OnDisable();
     if (!ok(gs_create(cudaDevice, stream, &m_Ctx))) return false;
+    m_OwnsCtx = true;
+    if (!ok(gs_asset_upload(m_Ctx, &asset, &m_Asset))) return false;
+    m_FrameCounter = 0;
+    return true;
+  }
+  // The same on the context of another renderer (which must outlive this one): the splat objects of one camera share a
+  // context so that SortAndRenderSplatsMulti draws them in one call.
+  bool OnEnable(const GsAssetDesc &asset, GsContext *sharedContext) {
+    OnDisable();
+    if (!sharedContext) return false;
+    m_Ctx = sharedContext;
     if (!ok(gs_asset_upload(m_Ctx, &asset, &m_Asset))) return false;
     m_FrameCounter = 0;
     return true;
   }
   void OnDisable() {  // :533-577
     if (m_Asset) gs_asset_destroy(m_Asset);
-    if (m_Ctx) gs_destroy(m_Ctx);
+    if (m_Ctx && m_OwnsCtx) gs_destroy(m_Ctx);
     m_Asset = nullptr;
     m_Ctx = nullptr;
+    m_OwnsCtx = false;
   }
   bool HasValidRenderSetup() const { return m_Ctx && m_Asset; }                           // :369
   bool SortPoints(const CameraState &cam) { GsFrameParams fp = params(cam); return ok(gs_sort(m_Ctx, m_Asset, &fp)); }          // :612
@@ -76,6 +89,36 @@ class GaussianSplatRenderer {
     ++m_FrameCounter;
     GsFrameParams fp = params(cam);
     return ok(gs_frame(m_Ctx, m_Asset, &fp, &options, doSort, rt, cameraTarget));
+  }
+  // GaussianSplatRenderSystem.SortAndRenderSplats for one camera (:73-105,108-169,187-211): `renderers` (all on one context)
+  // drawn in GatherSplatsForCamera order into one target, cleared once, then composited onto cameraTarget (may be nullptr) --
+  // one gs_frame_objects call.  options (blend mode, asynchronous read-back) are the first drawn renderer's.
+  static bool SortAndRenderSplatsMulti(const CameraState &cam, std::vector<GaussianSplatRenderer *> renderers, GsImage *rt,
+                                       GsImage *cameraTarget = nullptr) {
+    auto depth = [&](const GaussianSplatRenderer *r) {   // camera-space z of the object's position, +z forward
+      const float *v = cam.worldToCameraMatrix.m, *p = r->localToWorldMatrix.m + 12;
+      return -(v[2] * p[0] + v[6] * p[1] + v[10] * p[2] + v[14]);
+    };
+    if (renderers.empty()) return true;   // no active splat object: OnPreCullCamera draws nothing
+    for (const GaussianSplatRenderer *r : renderers)   // checked before any renderer's frame counter moves
+      if (!r || !r->HasValidRenderSetup() || r->m_Ctx != renderers[0]->m_Ctx) return false;
+    std::stable_sort(renderers.begin(), renderers.end(), [&](const GaussianSplatRenderer *a, const GaussianSplatRenderer *b) {
+      if (a->m_RenderOrder != b->m_RenderOrder) return a->m_RenderOrder > b->m_RenderOrder;
+      return depth(a) < depth(b);
+    });
+    std::vector<GsAsset *> assets;
+    std::vector<GsFrameParams> fps;
+    std::vector<int32_t> doSort;
+    for (GaussianSplatRenderer *r : renderers) {
+      assets.push_back(r->m_Asset);
+      fps.push_back(r->params(cam));
+      doSort.push_back((r->m_FrameCounter % (r->m_SortNthFrame > 0 ? r->m_SortNthFrame : 1)) == 0);   // :120-121
+      ++r->m_FrameCounter;
+    }
+    GsRenderOptions opt = renderers[0]->options;
+    opt.flags &= ~(uint32_t)GS_FLAG_LOAD_RT;
+    return renderers[0]->ok(gs_frame_objects(renderers[0]->m_Ctx, (uint32_t)renderers.size(), assets.data(), fps.data(), doSort.data(),
+                                             &opt, rt, cameraTarget));
   }
   bool Sync() { return ok(gs_sync(m_Ctx)); }
   // EditExportData, R/GaussianSplatRenderer.cs:936-958: n x 62 floats (the .ply attribute record), cut splats marked by nor = 1
@@ -111,6 +154,7 @@ class GaussianSplatRenderer {
     return false;
   }
   GsContext *m_Ctx = nullptr;
+  bool m_OwnsCtx = false;
   GsAsset *m_Asset = nullptr;
   int m_FrameCounter = 0;
 };

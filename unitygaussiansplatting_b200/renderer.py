@@ -10,6 +10,7 @@ the hot path; everything it does is a call into libgsplat_b200.so (there is no C
   cmb.DrawProcedural(matSplats)       (:165)   DrawSplats(cam, rt)           -> gs_render
   composite DrawProcedural            (:206)   Composite(rt, target)         -> gs_composite
   SortAndRenderSplats(cam, cmb)       (:108)   SortAndRenderSplats(cam, ...) -> gs_frame
+  (several objects of one camera)              SortAndRenderSplatsMulti(...) -> gs_frame_objects
   OnDisable / DisposeResourcesForAsset(:533)   Dispose()
 """
 from __future__ import annotations
@@ -401,11 +402,28 @@ def GatherSplatsForCamera(renderers, cam: Camera):
     return sorted(renderers, key=lambda r: (-int(r.m_RenderOrder), depth(r)))
 
 
-def SortAndRenderSplatsMulti(renderers, cam: Camera, rt):
+def draws_in_one_call(active) -> bool:
+    """Whether gs_frame_objects can draw these renderers: one context, whole-screen options (no partition, row range or band
+    packing) and one blend mode and read-back mode.  Otherwise SortAndRenderSplatsMulti draws them one gs_frame at a time."""
+    r0 = active[0]
+    return all(r.context is r0.context and r.blend_mode == r0.blend_mode and bool(r.async_readback) == bool(r0.async_readback)
+               and int(r.partition[1]) <= 1 and int(r.partition[0]) == 0 and tuple(r.rows) == (0, 0) and not r.band_packed
+               for r in active)
+
+
+def SortAndRenderSplatsMulti(renderers, cam: Camera, rt, camera_target=None):
     """GaussianSplatRenderSystem.SortAndRenderSplats (R/GaussianSplatRenderer.cs:108-169) for several splat objects of one
-    camera: ONE render target, cleared once (:196), every object blended under what the earlier ones left
-    (GS_FLAG_LOAD_RT from the second object on).  All renderers must live on one context."""
+    camera: ONE render target, cleared once (:196), every object blended under what the earlier ones left, then the composite
+    onto camera_target (when given).  One gs_frame_objects call when draws_in_one_call(active); else one gs_frame per object
+    (GS_FLAG_LOAD_RT from the second on) and gs_composite.  Returns the active renderers in draw order."""
     active = GatherSplatsForCamera(renderers, cam)
+    if not active:
+        return active
+    if draws_in_one_call(active):
+        _frame_objects(active, cam, rt, camera_target)
+        return active
+    if rt is None:
+        raise ValueError("drawing the objects one gs_frame at a time needs a render target")
     for i, r in enumerate(active):
         keep = r.load_rt
         r.load_rt = i > 0
@@ -413,4 +431,25 @@ def SortAndRenderSplatsMulti(renderers, cam: Camera, rt):
             r.SortAndRenderSplats(cam, rt=rt)
         finally:
             r.load_rt = keep
+    if camera_target is not None:
+        active[0].Composite(rt, camera_target)
     return active
+
+
+def _frame_objects(active, cam: Camera, rt, camera_target):
+    k = len(active)
+    fps = (N.GsFrameParams * k)()
+    assets = (C.c_void_p * k)()
+    do_sort = (C.c_int32 * k)()
+    for i, r in enumerate(active):
+        do_sort[i] = 1 if (r.m_FrameCounter % max(1, int(r.m_SortNthFrame)) == 0) else 0
+        r.m_FrameCounter += 1
+        fps[i] = r.frame_params(cam)     # r._keep holds the host buffers it points to
+        assets[i] = r._asset.value if isinstance(r._asset, C.c_void_p) else r._asset
+    opt = active[0]._options()
+    opt.flags &= ~N.GS_FLAG_LOAD_RT
+    a = _image(rt, cam.pixelWidth, cam.pixelHeight) if rt is not None else None
+    b = _image(camera_target, cam.pixelWidth, cam.pixelHeight) if camera_target is not None else None
+    ctx = active[0].context
+    N.check(ctx.handle, ctx._lib.gs_frame_objects(ctx.handle, k, assets, fps, do_sort, C.byref(opt), C.byref(a) if a is not None else None,
+                                                  C.byref(b) if b is not None else None))
