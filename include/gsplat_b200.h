@@ -85,7 +85,11 @@ typedef struct GsFrameParams {
   float mat_view[16];             /* cam.worldToCameraMatrix, -z fwd  (:586,:617) */
   float mat_proj_gpu[16];         /* UNITY_MATRIX_P = GL.GetGPUProjectionMatrix(cam.projectionMatrix, true);
                                      an engine global in the reference (S/SplatUtilities.compute:200,236) */
-  float screen_w, screen_h;       /* _VecScreenParams.xy              (:591) */
+  float screen_w, screen_h;       /* _VecScreenParams.xy              (:591).  In [1, 16384] per axis, the largest
+                                     render texture D3D12 makes (a splat's bin rectangle holds 8-bit indices of 64-pixel bins);
+                                     anything else is GS_ERR_INVALID_ARGUMENT.  A screen above 8160 px (128 bins) on either
+                                     axis makes the draw wait for the device once after binning: see "Bin-list capacity"
+                                     below. */
   float cam_pos_world[3];         /* _VecWorldSpaceCameraPos          (:592) */
   float splat_scale;              /* m_SplatScale   [0.1,2]           (:599) */
   float opacity_scale;            /* m_OpacityScale [0.05,20]         (:600) */
@@ -223,6 +227,16 @@ GS_API int gs_render(GsContext *ctx, GsAsset *asset, const GsFrameParams *fp,
 /* Composite pass: GaussianComposite.shader:35-39 with Blend SrcAlpha OneMinusSrcAlpha
  * (R/GaussianSplatRenderer.cs:206-210).  `camera_target` is read-modify-write. */
 GS_API int gs_composite(GsContext *ctx, const GsImage *rt, GsImage *camera_target);
+/* Bin-list capacity.  The draw lists one (bin, splat) entry per 64-pixel bin a splat's footprint touches, in a list of
+ * clamp(8 x splats, 4 Mi, 768 Mi) entries (for gs_frame_objects, 8 x a run's summed splats).  A list that needs more is
+ * truncated and the frame reports GS_ERR_OUT_OF_MEMORY: when the call reads its image back to the host, or else at gs_sync.
+ * Screens above 8160 px (128 bins) on either axis are the exception: the rule was set for smaller screens, and a splat's
+ * footprint in bins grows with the square of the screen size, so after binning the host waits for the device and reads the
+ * entry count back: one wait per draw, per run of gs_frame_objects and per object of a group member's draw, which smaller
+ * screens do not have (their calls return once the work is enqueued).  A list that overflowed is grown to the entries it needs plus a quarter, at most 768 Mi, and the frame is
+ * binned again; the capacity is kept, so the next frames of that size bin once.  Beyond 768 Mi the frame reports GS_ERR_OUT_OF_MEMORY as above.
+ * GsStageTimes.tile_entries is the count of the list the draw used. */
+
 /* SortAndRenderSplats for one renderer, one stream, no host round trips:
  * (do_sort ? gs_sort : nothing) -> gs_calc_view -> gs_render [-> gs_composite if
  * camera_target != NULL].  do_sort == (m_FrameCounter % m_SortNthFrame == 0),
@@ -250,7 +264,8 @@ GS_API int gs_frame(GsContext *ctx, GsAsset *asset, const GsFrameParams *fp,
  * one scene depth buffer (the same scene_depth pointer and memory); a new run starts where one of these would break, and
  * blends under what the earlier runs drew.  Any object count is accepted.  With one object the call does the device work of
  * gs_frame.  The bin-list capacity of a run is clamp(8 x its summed splat count, 4 Mi, 768 Mi) entries; a run that needs more
- * reports GS_ERR_OUT_OF_MEMORY as gs_frame does (at gs_sync when nothing is read back to the host).
+ * reports GS_ERR_OUT_OF_MEMORY as gs_frame does (at gs_sync when nothing is read back to the host), except on screens above
+ * 8160 px, where the list grows first (see "Bin-list capacity").
  * GsStageTimes after this call: bin_ms, raster_ms, composite_ms and tile_entries are those of the call's draw when it forms one
  * run; with several runs, bin_ms runs from the end of the last view-calc to the end of the last run's bin sort, and raster_ms
  * and tile_entries are the last run's.  distances_ms, sort_ms, sort_pass_ms and view_ms are those of the last object that

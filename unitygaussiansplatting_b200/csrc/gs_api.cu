@@ -127,10 +127,16 @@ int ensure_sort_scratch(GsContext *ctx, uint32_t capacity) {
   return GS_OK;
 }
 
+// The bin list holds clamp(8 x splats, 4 Mi, kBinListMax) entries, a rule set for screens of at most kRuleBins bins per axis
+// (8160 px).  A splat's footprint in bins grows with the square of the screen size, so larger frames check their list after
+// binning and grow it (grow_bin_list).
+constexpr uint32_t kBinListMax = 768u << 20;
+constexpr uint32_t kRuleBins = 128;
+
 static int ensure_bin_scratch(GsContext *ctx, uint32_t n, uint32_t tiles, uint32_t min_capacity) {
   uint64_t want = (uint64_t)n * 8;
   if (want < (4u << 20)) want = 4u << 20;
-  if (want > (768u << 20)) want = 768u << 20;
+  if (want > kBinListMax) want = kBinListMax;
   if (want < min_capacity) want = min_capacity;
   if ((uint32_t)want > ctx->bin.capacity) {
     cudaStreamSynchronize(ctx->stream);
@@ -159,6 +165,28 @@ static int ensure_bin_scratch(GsContext *ctx, uint32_t n, uint32_t tiles, uint32
     GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.bin_ranges, (size_t)tiles * 8));
     ctx->tiles_cap = tiles;
   }
+  return GS_OK;
+}
+
+// Screens of more than kRuleBins bins on either axis only: the host waits for the binning just enqueued and reads
+// entry_count back.  A list that overflowed grows to its total plus a quarter (at most kBinListMax) and *again asks the
+// caller to bin once more from the same rectangles (the view-calc output still holds them).  The capacity stays, and the
+// headroom lets the next frames of a moving camera, whose counts drift, bin once instead of growing the list again and again.
+// A total above kBinListMax is left truncated and reported like any overflow, at gs_sync or at the host read-back.
+static int grow_bin_list(GsContext *ctx, const FrameConsts &fc, uint32_t n, bool *again) {
+  *again = false;
+  if (fc.binsX <= kRuleBins && fc.binsY <= kRuleBins) return GS_OK;
+  const uint32_t tiles = fc.binsX * fc.binsY;
+  uint32_t ec[3] = {0, 0, 0};   // clamped count, overflow flag, total (of this run, for gs_frame_objects)
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ec, ctx->bin.entry_count, sizeof(ec), cudaMemcpyDeviceToHost, ctx->stream));
+  GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (ec[2] <= ctx->bin.capacity || ec[2] > kBinListMax) {
+    ctx->bin_overflow = ec[1] != 0;
+    return GS_OK;
+  }
+  const int rc = ensure_bin_scratch(ctx, n, tiles, (uint32_t)std::min<uint64_t>((uint64_t)ec[2] + ec[2] / 4, kBinListMax));
+  if (rc) return rc;
+  *again = true;
   return GS_OK;
 }
 
@@ -315,8 +343,8 @@ int check_params(GsContext *ctx, GsAsset *as, const GsFrameParams *fp) {
   if (!ctx || !as || !fp) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null context/asset/params");
   if (as->ctx != ctx) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "asset belongs to another context");
   GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));   // the caller's current device may be another one
-  if (!(fp->screen_w >= 1.0f) || !(fp->screen_h >= 1.0f) || fp->screen_w > 8160.0f || fp->screen_h > 8160.0f)
-    return fail(ctx, GS_ERR_INVALID_ARGUMENT, "screen size must be in [1,8160] (8-bit bin indices)");
+  if (!(fp->screen_w >= 1.0f) || !(fp->screen_h >= 1.0f) || fp->screen_w > 16384.0f || fp->screen_h > 16384.0f)
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, "screen size must be in [1,16384] (8-bit indices of 64-pixel bins)");
   if (fp->sh_order > 3) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "sh_order must be 0..3");
   return GS_OK;
 }
@@ -397,10 +425,18 @@ int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRender
   int rc = ensure_bin_scratch(ctx, as->av.n, tiles, 0);
   if (rc) return rc;
   if ((rc = ensure_raster_tiles(ctx, fc))) return rc;
-  int bin_launches = 0;
+  int bin_launches = 0, more = 0;
   BinScratch lists;
   GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->av.n, as->order, as->rect, as->block_bits, ctx->bin, ctx->sort, ctx->stream, &lists,
                                   &bin_launches));
+  bool again = false;
+  if ((rc = grow_bin_list(ctx, fc, as->av.n, &again))) return rc;
+  if (again) {
+    GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->av.n, as->order, as->rect, as->block_bits, ctx->bin, ctx->sort, ctx->stream, &lists,
+                                    &more));
+    bin_launches += more;
+    ctx->bin_overflow = false;
+  }
   rec(ctx, EV_BIN1);
   if (bin_done) cudaEventRecord(bin_done, ctx->stream);
   launch_raster(fc, opt, as->draw, lists, d_rt, pitch, fmt, surf, ctx->stream, ctx->cur_depth ? as->zndc : nullptr, ctx->cur_depth);
@@ -430,13 +466,24 @@ static int render_run(GsContext *ctx, const FrameConsts &fc, const GsRenderOptio
     if (fps[i].scene_depth) { ro.zndc[i] = a->zndc; ro.depth_mask |= 1u << i; }
     extras |= fps[i].selected_bits != nullptr || fps[i].scene_depth != nullptr;   // what picks the extras raster for one object
   }
-  int rc = ensure_bin_scratch(ctx, (uint32_t)std::min<uint64_t>(total, 0xFFFFFFFFu), fc.binsX * fc.binsY, 0);
+  const uint32_t n = (uint32_t)std::min<uint64_t>(total, 0xFFFFFFFFu), tiles = fc.binsX * fc.binsY;
+  int rc = ensure_bin_scratch(ctx, n, tiles, 0);
   if (rc) return rc;
   if ((rc = ensure_raster_tiles(ctx, fc))) return rc;
   if ((rc = bind_depth(ctx, depth_fp, ctx->stream))) return rc;
   BinScratch lists;
-  int bin_launches = 0;
+  int bin_launches = 0, more = 0;
   GS_CUDA_TRY(ctx, launch_binning_objects(fc, count, bo, first, ctx->bin, ctx->sort, ctx->stream, &lists, &bin_launches));
+  bool again = false;
+  if ((rc = grow_bin_list(ctx, fc, n, &again))) return rc;
+  if (again) {
+    // the overflow flag this run set is cleared again, unless an earlier run of the call left its list truncated (every run of
+    // the call has the same screen, so every one was checked here)
+    const bool clear = first || !ctx->bin_overflow;
+    GS_CUDA_TRY(ctx, launch_binning_objects(fc, count, bo, clear, ctx->bin, ctx->sort, ctx->stream, &lists, &more));
+    bin_launches += more;
+    if (first) ctx->bin_overflow = false;
+  }
   rec(ctx, EV_BIN1);
   GsRenderOptions o = opt;
   if (!first) o.flags |= GS_FLAG_LOAD_RT;

@@ -42,6 +42,7 @@ struct GsContext {
   // bin scratch
   gs::BinScratch bin{};
   uint32_t bin_blocks_cap = 0, tiles_cap = 0, raster_tiles_cap = 0, raster_tiles_cur = 0;
+  bool bin_overflow = false;   // the bin list's overflow flag as the last read-back of a frame above kLargeFrameBins left it
   // image scratch
   void *rt_scratch = nullptr;
   size_t rt_bytes = 0;

@@ -4,7 +4,9 @@
 
 namespace gs {
 
-constexpr uint32_t kRectEmpty = 0xFFFFFFFFu;  // bin rect sentinel (bin indices are < 255)
+// Bin rect sentinel: x0 = 255 > x1 = 0, which no rectangle footprint_tile_rect makes can be.  (All ones would be the
+// one-bin rectangle at bin (255, 255), which exists on screens wider and taller than 16320 px.)
+constexpr uint32_t kRectEmpty = 0x000000FFu;
 
 // Screen-space footprint of one splat, derived from its SplatViewData exactly the way the
 // draw stage defines it (S/RenderGaussianSplats.shader:35-77; DESIGN.md "Raster rule").
@@ -91,7 +93,8 @@ inline Partition make_partition(const GsRenderOptions &o) {
   return p;
 }
 
-// Pixel rows/cols whose centres can be touched -> inclusive rectangle of kBin-pixel bins packed x0|y0<<8|x1<<16|y1<<24.
+// Pixel rows/cols whose centres can be touched -> inclusive rectangle of kBin-pixel bins packed x0|y0<<8|x1<<16|y1<<24
+// (8 bits per index: 256 bins = 16384 px per axis, the largest screen check_params accepts).
 // Range partitions clip the rows to their own pixel band first, so the rectangle holds own bin rows only.
 __device__ __forceinline__ uint32_t footprint_tile_rect(const SplatFootprint &fp, const FrameConsts &fc, const Partition &part) {
   float x0 = fmaxf(ceilf(fp.cx - fp.hx - 0.5f), 0.0f), x1 = fminf(floorf(fp.cx + fp.hx - 0.5f), fc.screenW - 1.0f);

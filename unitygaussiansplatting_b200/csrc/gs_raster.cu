@@ -200,7 +200,9 @@ __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ o
 }
 
 // digit width and pass count of the stable sort by bin id: one pass while the bin count fits a digit (<= 512 bins, e.g.
-// 1200x797 = 19x13 in 8 bits, 1920x1080 = 30x17 in 9), else two passes of the narrowest digit that covers it
+// 1200x797 = 19x13 in 8 bits, 1920x1080 = 30x17 in 9), else two passes of the narrowest digit that covers it, up to two
+// 8-bit passes for 65536 bins (16384x16384).  The 8-bit plan's digit histograms are ghist's first two rows of 256 and its
+// look-back 2 x 256 words per tile, within the depth sort's allocation (4 x 256).
 static void bin_sort_plan(uint32_t bins, int *bits, int *passes) {
   if (bins <= 512u) { *passes = 1; *bits = bins <= 32u ? 5 : bins <= 64u ? 6 : bins <= 128u ? 7 : bins <= 256u ? 8 : 9; return; }
   *passes = 2;
