@@ -262,10 +262,11 @@ GS_API int gs_frame(GsContext *ctx, GsAsset *asset, const GsFrameParams *fp,
  * objects are drawn together as one run: their bin-list entries go into one list, object after object, which is sorted once
  * by bin id and drawn by one raster pass.  A run holds at most 16 objects, each with fewer than 2^28 splats, binding at most
  * one scene depth buffer (the same scene_depth pointer and memory); a new run starts where one of these would break, and
- * blends under what the earlier runs drew.  Any object count is accepted.  With one object the call does the device work of
- * gs_frame.  The bin-list capacity of a run is clamp(8 x its summed splat count, 4 Mi, 768 Mi) entries; a run that needs more
- * reports GS_ERR_OUT_OF_MEMORY as gs_frame does (at gs_sync when nothing is read back to the host), except on screens above
- * 8160 px, where the list grows first (see "Bin-list capacity").
+ * blends under what the earlier runs drew.  Any object count is accepted.  A run of one object (with one object: the whole
+ * call) does the device work of gs_frame.  The bin-list capacity of a run is clamp(8 x its summed splat count, 4 Mi, 768 Mi)
+ * entries; a run that needs more reports GS_ERR_OUT_OF_MEMORY as gs_frame does (at gs_sync when nothing is read back to the
+ * host), even when a later run's list fits, except on screens above 8160 px, where the list grows first (see "Bin-list
+ * capacity").
  * GsStageTimes after this call: bin_ms, raster_ms, composite_ms and tile_entries are those of the call's draw when it forms one
  * run; with several runs, bin_ms runs from the end of the last view-calc to the end of the last run's bin sort, and raster_ms
  * and tile_entries are the last run's.  distances_ms, sort_ms, sort_pass_ms and view_ms are those of the last object that
@@ -350,7 +351,8 @@ GS_API int gs_group_frame(GsGroup *group, GsAsset *const *assets, const GsFrameP
  * Per call: each object is sorted with its own splitters, slab table and order exchange (its order persists in its asset);
  * all objects' distance kernels and view-calcs are queued first and the host waits once for all slab tables.  Each object
  * blends under the earlier ones on the member's own rows; there is ONE row split (balanced on the summed measured cost of the
- * objects) and ONE row exchange per call.  After gs_group_join only the first object ever sorted on the group uses the
+ * objects) and ONE row exchange per call.  A truncated bin list of any object is reported, as for gs_frame (see "Bin-list
+ * capacity"), even when a later object's list fits.  After gs_group_join only the first object ever sorted on the group uses the
  * peer-to-peer order exchange; the others use the all-gather or in-place exchange.  GsGroupStats of such a call: the times
  * span the whole call (slab_sort_ms runs to the end of the last object's slab sort, order_exchange_ms is its exchange,
  * bin_ms sums every object's binning); slab_counts are summed over the objects the call sorted.

@@ -382,6 +382,56 @@ def test_member_context_sync_with_a_pending_array_camera_target(g, ctx):
         cu.free_all()
 
 
+@pytest.mark.parametrize("image", ["host", "device"])
+def test_truncated_list_of_an_earlier_object_is_reported(g, ctx, image):
+    """A member draws the call's objects one after the other through one bin list.  On a fresh group (a 4 Mi entry list),
+    object 0 is the construction of test_bin_list_exact_capacity_overflow_and_recovery, one splat over capacity, and object 1
+    fits: the call still reports GS_ERR_OUT_OF_MEMORY, when it returns with a host image and at gs_group_sync with a device
+    image.  Deleting the splat that no longer fits makes the next call succeed and equal the per-object gs_frame loop."""
+    import torch
+    import test_gpu_cull_edges as ce
+    from test_gpu_frame_objects import loop_frame
+    W, H = ce.CAP_W, ce.CAP_H
+    cam = camera(g, W, H)
+    assets = [g.create_asset(ce._bin_row_splats(cam, ce.CAP_SPLATS + 1, 0xCA9), "VeryHigh"),
+              g.create_asset(ce._bin_row_splats(cam, 1000, 0xCAA), "VeryHigh")]
+    grp, objs = _group(assets, [{}, {}], 1)
+    rs = []
+    try:
+        def new_rt():
+            return np.zeros((H, W, 4), np.float16) if image == "host" else torch.zeros((H, W, 4), dtype=torch.float16, device="cuda")
+
+        rt = new_rt()
+        if image == "host":
+            with pytest.raises(g.GsError) as e:
+                grp.SortAndRenderSplatsMulti(objs, cam, rts=[rt])
+        else:
+            assert grp.SortAndRenderSplatsMulti(objs, cam, rts=[rt]) == objs   # not checked when it is enqueued ...
+            with pytest.raises(g.GsError) as e:
+                grp.sync()                                                      # ... but at the next synchronising call
+        assert e.value.code == -3 and "tile-list capacity exceeded" in str(e.value)
+
+        last = int(grp.readback_order()[-1])
+        bits = np.zeros((assets[0].splatCount + 31) // 32, np.uint32)
+        bits[last >> 5] |= np.uint32(1 << (last & 31))
+        objs[0].m_DeletedBits = bits
+        rt = new_rt()
+        assert grp.SortAndRenderSplatsMulti(objs, cam, rts=[rt]) == objs
+        grp.sync()
+        got = rt if image == "host" else rt.cpu().numpy()
+        rs = [g.GaussianSplatRenderer(a, ctx) for a in assets]
+        rs[0].m_DeletedBits = bits
+        want = np.zeros((H, W, 4), np.float16)
+        loop_frame(g, ctx, rs, cam, 0, want, None)
+        assert got.any() and np.array_equal(got.view(np.uint16), want.view(np.uint16))
+        for o, r in zip(objs, rs):
+            assert np.array_equal(o.readback_order(), r.readback_order())
+    finally:
+        for r in rs:
+            r.Dispose()
+        grp.close()
+
+
 def test_python_multi_rejects_before_counting_and_draws_nothing_without_objects(g, ctx):
     """SortAndRenderSplatsMulti checks every object before any frame counter moves; with no objects it draws nothing."""
     W, H = 128, 96

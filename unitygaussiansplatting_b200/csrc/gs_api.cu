@@ -320,12 +320,12 @@ int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cu
   return GS_OK;
 }
 
-// The scene depth buffer the splat pass is tested against (GsFrameParams.scene_depth): used in place when it is device
-// memory, uploaded on `stream` when it is host memory.
-int bind_depth(GsContext *ctx, const GsFrameParams *fp, cudaStream_t stream) {
-  ctx->cur_depth = nullptr;
+// The scene depth buffer the splat pass is tested against (GsFrameParams.scene_depth), in *depth (nullptr: none): used in
+// place when it is device memory, uploaded on the context stream when it is host memory.
+static int bind_depth(GsContext *ctx, const GsFrameParams *fp, const float **depth) {
+  *depth = nullptr;
   if (!fp->scene_depth) return GS_OK;
-  if (fp->scene_depth_on_device) { ctx->cur_depth = fp->scene_depth; return GS_OK; }
+  if (fp->scene_depth_on_device) { *depth = fp->scene_depth; return GS_OK; }
   const size_t bytes = (size_t)(uint32_t)fp->screen_w * (uint32_t)fp->screen_h * sizeof(float);
   if (bytes > ctx->depth_bytes) {
     cudaStreamSynchronize(ctx->stream);
@@ -334,8 +334,8 @@ int bind_depth(GsContext *ctx, const GsFrameParams *fp, cudaStream_t stream) {
     GS_CUDA_TRY(ctx, cudaMalloc(&ctx->d_depth, bytes));
     ctx->depth_bytes = bytes;
   }
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_depth, fp->scene_depth, bytes, cudaMemcpyHostToDevice, stream));
-  ctx->cur_depth = ctx->d_depth;
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_depth, fp->scene_depth, bytes, cudaMemcpyHostToDevice, ctx->stream));
+  *depth = ctx->d_depth;
   return GS_OK;
 }
 
@@ -417,77 +417,48 @@ static int ensure_raster_tiles(GsContext *ctx, const FrameConsts &fc) {
   return GS_OK;
 }
 
-// binning + raster into a device image
-int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRenderOptions &opt, void *d_rt, uint32_t pitch,
-                     uint32_t fmt, cudaSurfaceObject_t surf, cudaEvent_t bin_done) {
+int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *const *as, const GsFrameParams *fps,
+            uint32_t count, bool first, void *d_rt, uint32_t pitch, uint32_t fmt, cudaSurfaceObject_t surf, cudaEvent_t bin_done) {
   GsNvtxRange nvtx("GaussianSplat.Draw");
-  const uint32_t tiles = fc.binsX * fc.binsY;
-  int rc = ensure_bin_scratch(ctx, as->av.n, tiles, 0);
-  if (rc) return rc;
-  if ((rc = ensure_raster_tiles(ctx, fc))) return rc;
-  int bin_launches = 0, more = 0;
-  BinScratch lists;
-  GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->av.n, as->order, as->rect, as->block_bits, ctx->bin, ctx->sort, ctx->stream, &lists,
-                                  &bin_launches));
-  bool again = false;
-  if ((rc = grow_bin_list(ctx, fc, as->av.n, &again))) return rc;
-  if (again) {
-    GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->av.n, as->order, as->rect, as->block_bits, ctx->bin, ctx->sort, ctx->stream, &lists,
-                                    &more));
-    bin_launches += more;
-    ctx->bin_overflow = false;
-  }
-  rec(ctx, EV_BIN1);
-  if (bin_done) cudaEventRecord(bin_done, ctx->stream);
-  launch_raster(fc, opt, as->draw, lists, d_rt, pitch, fmt, surf, ctx->stream, ctx->cur_depth ? as->zndc : nullptr, ctx->cur_depth);
-  rec(ctx, EV_RASTER1);
-  ctx->launches += bin_launches + 3;  // bin_emit, look-back clear, 1-2 sort passes; bin_ranges, tile_order, raster
-  GS_CUDA_TRY(ctx, cudaGetLastError());
-  return GS_OK;
-}
-
-// One run of gs_frame_objects: the objects' entries in one bin list (object after object), one bin sort and one raster.
-// `first`: the run starts from a cleared target and clears the overflow flag; later runs blend under what is there.
-// depth_fp: the frame parameters whose scene depth buffer the run binds (every object of the run that binds one binds it).
-static int render_run(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *const *as, const GsFrameParams *fps,
-                      uint32_t count, bool first, const GsFrameParams *depth_fp, void *d_rt, uint32_t pitch, uint32_t fmt,
-                      cudaSurfaceObject_t surf) {
-  GsNvtxRange nvtx("GaussianSplat.Draw");
+  DrawObjects objs;
+  memset(&objs, 0, sizeof(objs));
+  objs.count = count;
+  const GsFrameParams *depth_fp = &fps[0];   // every object that binds a scene depth buffer binds this one
   uint64_t total = 0;
-  BinObject bo[kRunObjects];
-  RasterObjects ro;
-  memset(&ro, 0, sizeof(ro));
-  bool extras = false;
-  for (uint32_t i = 0; i < count; ++i) {
-    const GsAsset *a = as[i];
+  for (uint32_t k = 0; k < count; ++k) {
+    const GsAsset *a = as[k];
+    const GsFrameParams &f = fps[k];
     total += a->av.n;
-    bo[i] = BinObject{a->av.n, a->order, a->rect, a->block_bits};
-    ro.draw[i] = a->draw;
-    if (fps[i].scene_depth) { ro.zndc[i] = a->zndc; ro.depth_mask |= 1u << i; }
-    extras |= fps[i].selected_bits != nullptr || fps[i].scene_depth != nullptr;   // what picks the extras raster for one object
+    objs.n[k] = a->av.n; objs.order[k] = a->order; objs.rect[k] = a->rect; objs.block_bits[k] = a->block_bits; objs.draw[k] = a->draw;
+    if (f.scene_depth) {
+      objs.zndc[k] = a->zndc;
+      objs.depth_mask |= 1u << k;
+      if (!depth_fp->scene_depth) depth_fp = &f;
+    }
+    objs.extras |= f.selected_bits != nullptr || f.scene_depth != nullptr;
   }
-  const uint32_t n = (uint32_t)std::min<uint64_t>(total, 0xFFFFFFFFu), tiles = fc.binsX * fc.binsY;
-  int rc = ensure_bin_scratch(ctx, n, tiles, 0);
+  const uint32_t n = (uint32_t)std::min<uint64_t>(total, 0xFFFFFFFFu);
+  int rc = ensure_bin_scratch(ctx, n, fc.binsX * fc.binsY, 0);
   if (rc) return rc;
   if ((rc = ensure_raster_tiles(ctx, fc))) return rc;
-  if ((rc = bind_depth(ctx, depth_fp, ctx->stream))) return rc;
+  const float *depth = nullptr;
+  if ((rc = bind_depth(ctx, depth_fp, &depth))) return rc;
   BinScratch lists;
   int bin_launches = 0, more = 0;
-  GS_CUDA_TRY(ctx, launch_binning_objects(fc, count, bo, first, ctx->bin, ctx->sort, ctx->stream, &lists, &bin_launches));
+  GS_CUDA_TRY(ctx, launch_binning(fc, opt, objs, first, ctx->bin, ctx->sort, ctx->stream, &lists, &bin_launches));
   bool again = false;
   if ((rc = grow_bin_list(ctx, fc, n, &again))) return rc;
   if (again) {
-    // the overflow flag this run set is cleared again, unless an earlier run of the call left its list truncated (every run of
-    // the call has the same screen, so every one was checked here)
+    // the grown list fits: the flag this draw set is cleared again, unless an earlier draw of the call left its list truncated
+    // (every draw of a call has the same screen, so every one was checked here)
     const bool clear = first || !ctx->bin_overflow;
-    GS_CUDA_TRY(ctx, launch_binning_objects(fc, count, bo, clear, ctx->bin, ctx->sort, ctx->stream, &lists, &more));
+    GS_CUDA_TRY(ctx, launch_binning(fc, opt, objs, clear, ctx->bin, ctx->sort, ctx->stream, &lists, &more));
     bin_launches += more;
-    if (first) ctx->bin_overflow = false;
+    ctx->bin_overflow = !clear;
   }
   rec(ctx, EV_BIN1);
-  GsRenderOptions o = opt;
-  if (!first) o.flags |= GS_FLAG_LOAD_RT;
-  launch_raster_objects(fc, o, ro, extras, lists, d_rt, pitch, fmt, surf, ctx->stream, ctx->cur_depth);
+  if (bin_done) cudaEventRecord(bin_done, ctx->stream);
+  launch_raster(fc, opt, objs, lists, d_rt, pitch, fmt, surf, ctx->stream, depth);
   rec(ctx, EV_RASTER1);
   ctx->launches += bin_launches + 3;  // per object look-back clear + bin_emit, 1-2 sort passes; bin_ranges, tile_order, raster
   GS_CUDA_TRY(ctx, cudaGetLastError());
@@ -797,21 +768,20 @@ int gs_render(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRend
   if (opt.band_packed && rt && rt->memory == GS_MEM_ARRAY)
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "band_packed output is the send buffer of an all-gather: it must be linear memory, not a CUDA array");
   if ((rc = image_ok(ctx, rt, W, H, &pitch))) return rc;
+  if (fp->scene_depth && !as->zndc_valid) return fail(ctx, GS_ERR_NOT_READY, "a scene depth buffer needs the quad depths: run gs_calc_view with scene_depth set");
   for (int e = EV_BIN1; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
-  if ((rc = bind_depth(ctx, fp, ctx->stream))) return rc;
-  if (ctx->cur_depth && !as->zndc_valid) return fail(ctx, GS_ERR_NOT_READY, "a scene depth buffer needs the quad depths: run gs_calc_view with scene_depth set");
   rec(ctx, EV_VIEW1);
-  if (rt->memory == GS_MEM_DEVICE) return do_render(ctx, as, fc, opt, rt->data, pitch, rt->format);
+  if (rt->memory == GS_MEM_DEVICE) return do_draw(ctx, fc, opt, &as, fp, 1, true, rt->data, pitch, rt->format);
   if (rt->memory == GS_MEM_ARRAY) {
     CallSurfaces surfs(ctx);
     cudaSurfaceObject_t so = 0;
     if ((rc = surfs.make(rt, &so))) return rc;
-    return do_render(ctx, as, fc, opt, nullptr, 0, rt->format, so);
+    return do_draw(ctx, fc, opt, &as, fp, 1, true, nullptr, 0, rt->format, so);
   }
   const uint32_t tight = W * pix_bytes(rt->format);
   if ((rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)tight * H))) return rc;
   if ((rc = init_staging(ctx, opt, ctx->rt_scratch, tight, W, H, rt->format, rt, pitch))) return rc;
-  if ((rc = do_render(ctx, as, fc, opt, ctx->rt_scratch, tight, rt->format))) return rc;
+  if ((rc = do_draw(ctx, fc, opt, &as, fp, 1, true, ctx->rt_scratch, tight, rt->format))) return rc;
   GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, pitch, ctx->rt_scratch, tight, tight, H, cudaMemcpyDeviceToHost, ctx->stream));
   return check_bin_overflow(ctx);
 }
@@ -959,8 +929,7 @@ int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRende
   CallSurfaces surfs(ctx);
   FrameImage fi;
   if ((rc = begin_frame_image(ctx, surfs, opt, rt, rt_pitch, rt_fmt, tgt, W, H, &fi))) return rc;
-  if ((rc = bind_depth(ctx, fp, ctx->stream))) return rc;
-  if ((rc = do_render(ctx, as, fc, opt, fi.d_rt, fi.pitch, rt_fmt, fi.surf))) return rc;
+  if ((rc = do_draw(ctx, fc, opt, &as, fp, 1, true, fi.d_rt, fi.pitch, rt_fmt, fi.surf))) return rc;
   return end_frame_image(ctx, surfs, rt, rt_pitch, rt_fmt, tgt, W, H, fi);
 }
 
@@ -1007,20 +976,9 @@ int gs_frame_objects(GsContext *ctx, uint32_t object_count, GsAsset *const *asse
   FrameImage fi;
   if ((rc = begin_frame_image(ctx, surfs, opt, rt, rt_pitch, rt_fmt, tgt, W, H, &fi))) return rc;
   // Runs: consecutive objects drawn by one bin list and one raster -- at most kRunObjects, each with fewer than 2^kSlotShift
-  // splats (the slot tag), binding at most one scene depth buffer.  An object that fits no run, and the only object of a
-  // one-object call, is drawn by the kernels of gs_frame.
+  // splats (the slot tag), binding at most one scene depth buffer.  An object of more splats, and the only object of a
+  // one-object call, is a run of one.  The first run starts from a cleared target, each later one blends under it.
   for (uint32_t k = 0; k < K;) {
-    const bool first = k == 0;
-    if (K == 1 || assets[k]->av.n > kLocalIdMask) {
-      // this draw's bin list check overwrites the overflow flag: report an earlier run's truncation first
-      if (!first && (rc = check_bin_overflow(ctx))) return rc;
-      GsRenderOptions o = opt;
-      if (!first) o.flags |= GS_FLAG_LOAD_RT;
-      if ((rc = bind_depth(ctx, &fps[k], ctx->stream))) return rc;
-      if ((rc = do_render(ctx, assets[k], fcs[k], o, fi.d_rt, fi.pitch, rt_fmt, fi.surf))) return rc;
-      ++k;
-      continue;
-    }
     const GsFrameParams *depth_fp = &fps[k];
     uint32_t e = k;
     for (; e < K && e - k < kRunObjects && assets[e]->av.n <= kLocalIdMask; ++e) {
@@ -1029,7 +987,10 @@ int gs_frame_objects(GsContext *ctx, uint32_t object_count, GsAsset *const *asse
       if (!depth_fp->scene_depth) depth_fp = &f;
       else if (f.scene_depth != depth_fp->scene_depth || f.scene_depth_on_device != depth_fp->scene_depth_on_device) break;
     }
-    if ((rc = render_run(ctx, fcs[k], opt, assets + k, fps + k, e - k, first, depth_fp, fi.d_rt, fi.pitch, rt_fmt, fi.surf))) return rc;
+    e = std::max(e, k + 1);
+    GsRenderOptions o = opt;
+    if (k) o.flags |= GS_FLAG_LOAD_RT;
+    if ((rc = do_draw(ctx, fcs[k], o, assets + k, fps + k, e - k, k == 0, fi.d_rt, fi.pitch, rt_fmt, fi.surf))) return rc;
     k = e;
   }
   return end_frame_image(ctx, surfs, rt, rt_pitch, rt_fmt, tgt, W, H, fi);

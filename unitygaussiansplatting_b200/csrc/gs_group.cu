@@ -872,8 +872,8 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
         opt.flags = k ? (uint32_t)GS_FLAG_LOAD_RT : 0u;
         rec(ctx, EV_VIEW1);
         if (timing) cudaEventRecord(mb.obj_tev[2 * k], ctx->stream);
-        if ((rc = bind_depth(ctx, o.fp, ctx->stream))) return rc;
-        if ((rc = do_render(ctx, o.assets[i], o.fc, opt, d_rt, pitch, fmt, 0, timing ? mb.obj_tev[2 * k + 1] : nullptr))) return rc;
+        if ((rc = do_draw(ctx, o.fc, opt, o.assets + i, o.fp, 1, k == 0, d_rt, pitch, fmt, 0, timing ? mb.obj_tev[2 * k + 1] : nullptr)))
+          return rc;
         ctx->launches += 1;   // k_row_costs: here for every object but the last (before the next one's raster overwrites the
                               // tile costs), on the transfer stream below for the last
         if (k + 1 < K) launch_row_costs(ctx->bin.tile_cost, ntx, g->bounds[mb.rank], g->bounds[mb.rank + 1], mb.d_row_cost, ctx->stream, k > 0);

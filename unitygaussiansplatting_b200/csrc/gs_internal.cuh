@@ -65,7 +65,6 @@ struct GsContext {
   size_t selected_words = 0;
   float *d_depth = nullptr;          // the frame's scene depth buffer when it was handed over in host memory
   size_t depth_bytes = 0;
-  const float *cur_depth = nullptr;  // what the compositor tests against this frame (nullptr: no depth test)
   uint32_t launches = 0;
   uint64_t pack_stats[4] = {0, 0, 0, 0};   // gs_debug_pack_stats
   // surface objects of GS_MEM_ARRAY images, one per array per call: each batch is destroyed once `done` (recorded behind the
@@ -106,12 +105,15 @@ int ensure_sort_scratch(GsContext *ctx, uint32_t capacity);
 // ctx->stream and `busy` (when given: another stream whose view-calc may still read it) have drained.  Uploads nothing.
 int reserve_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t busy = nullptr);
 int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t stream);
-int bind_depth(GsContext *ctx, const GsFrameParams *fp, cudaStream_t stream);   // sets ctx->cur_depth for the draw that follows
 int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameConsts &fc, bool cull, const GsRenderOptions &opt,
             cudaStream_t stream);
-// d_rt == nullptr: the target is the CUDA array behind `surf`.  bin_done (optional) is recorded on ctx->stream when binning ends.
-int do_render(GsContext *ctx, GsAsset *as, const FrameConsts &fc, const GsRenderOptions &opt, void *d_rt, uint32_t pitch, uint32_t fmt,
-              cudaSurfaceObject_t surf = 0, cudaEvent_t bin_done = nullptr);
+// Bins and rasterizes the objects as[0, count), drawn with the uniforms fps[0, count), into a device image (d_rt == nullptr:
+// the CUDA array behind `surf`) on ctx->stream: one object with gs_frame's kernels, or several as one run of gs_frame_objects
+// (DrawObjects).  The scene depth buffer bound is that of the first object that has one.  `first`: the first draw of its
+// public call, whose bin list sets the overflow flag; a later draw of the call only ever sets it, so the call reports every
+// truncated list.  bin_done (optional) is recorded on ctx->stream when binning ends.
+int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *const *as, const GsFrameParams *fps, uint32_t count,
+            bool first, void *d_rt, uint32_t pitch, uint32_t fmt, cudaSurfaceObject_t surf = 0, cudaEvent_t bin_done = nullptr);
 // The composite pass (gs_composite) of a linear device render target onto `tgt` (host, device or CUDA-array memory, already
 // validated as W x H), enqueued on `s`.  A host target is uploaded and read back, and the call waits for `s`.
 int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H,

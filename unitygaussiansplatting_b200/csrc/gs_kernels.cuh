@@ -180,37 +180,31 @@ struct BinScratch {
   uint32_t *tile_cost, *tile_order;   // per raster tile: last frame's cost, this frame's launch order
   uint32_t capacity;
 };
-// *sorted: the scratch view whose tile_keys / tile_vals hold the bin-sorted lists (launch_raster's input)
-cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, uint32_t n, const uint32_t *order, const uint32_t *rect,
-                           const uint32_t *block_bits, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted,
-                           int *launches);
-// Several splat objects drawn by one bin list and one raster (gs_frame_objects): a run of up to kRunObjects objects, each with
-// fewer than 2^kSlotShift splats.  Every list entry is (slot << kSlotShift) | splat id.
+// The splat objects one draw bins and rasterizes, in draw order.  A list of one is drawn by gs_frame's kernels, under any tile
+// partition.  A longer list is a run of gs_frame_objects: at most kRunObjects objects, each with fewer than 2^kSlotShift
+// splats, on the whole screen.  Their entries go into one list, object after object, each tagged (slot << kSlotShift) | splat
+// id; that list is sorted once by bin id and drawn by one k_raster<..., MULTI> pass, whose kernel parameter this is.
 constexpr uint32_t kRunObjects = 16, kSlotShift = 28, kLocalIdMask = (1u << kSlotShift) - 1u;
-struct BinObject {
-  uint32_t n;
-  const uint32_t *order, *rect, *block_bits;
-};
-// The objects' lists go into one list, object after object (slot k = objs[k]), and are sorted once by bin id.  clear_overflow:
-// this is the call's first run (later runs keep an earlier run's overflow flag).
-cudaError_t launch_binning_objects(const FrameConsts &fc, uint32_t count, const BinObject *objs, bool clear_overflow, const BinScratch &bs,
-                                   const SortScratch &sc, cudaStream_t s, BinScratch *sorted, int *launches);
-struct RasterObjects {
-  const float4 *draw[kRunObjects];   // each slot's raster records
-  const float *zndc[kRunObjects];    // each slot's quad depths, where that object is depth-tested
-  uint32_t depth_mask;               // bit k: slot k is depth-tested against the run's scene depth buffer
+struct DrawObjects {
+  const float4 *draw[kRunObjects];   // raster records
+  const float *zndc[kRunObjects];    // quad depths, where the object is depth-tested
+  uint32_t depth_mask;               // bit k: object k is depth-tested against the draw's scene depth buffer
+  uint32_t count;
+  bool extras;                       // some object has a selection or is depth-tested: the raster's SEL instantiation
+  uint32_t n[kRunObjects];           // splats, and what binning reads of them
+  const uint32_t *order[kRunObjects], *rect[kRunObjects], *block_bits[kRunObjects];
 };
 struct NoRasterObjects {};
-// The raster of one run into a full-screen target; `extras`: some object has a selection or a depth buffer.  opt: blend mode
-// and GS_FLAG_LOAD_RT.
-void launch_raster_objects(const FrameConsts &fc, const GsRenderOptions &opt, const RasterObjects &objs, bool extras, const BinScratch &bs,
-                           void *rt, uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s,
-                           const float *scene_depth);
-// zndc / scene_depth: per-splat quad depth and the W x H depth buffer to test it against (both nullptr: no depth test).
-// Images here are linear device memory (pointer, pitch) or, when the pointer is null, a CUDA array behind a surface object.
-void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const BinScratch &bs, void *rt,
-                   uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s, const float *zndc = nullptr,
-                   const float *scene_depth = nullptr);
+// The objects' (bin id, splat id) lists, sorted by bin id.  *sorted: the scratch view whose tile_keys / tile_vals hold them
+// (launch_raster's input).  clear_overflow: this is the first draw of its call, and its list sets the overflow flag
+// entry_count[1] from its own total; otherwise the flag is only ever set, so an earlier draw's truncation stays reported.
+cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, const DrawObjects &objs, bool clear_overflow,
+                           const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted, int *launches);
+// scene_depth: the W x H depth buffer the depth-tested objects are tested against (nullptr: none).  opt: tile partition,
+// band_packed, blend mode and GS_FLAG_LOAD_RT.  Images here are linear device memory (pointer, pitch) or, when the pointer is
+// null, a CUDA array behind a surface object.
+void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const DrawObjects &objs, const BinScratch &bs, void *rt,
+                   uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s, const float *scene_depth);
 extern unsigned long long *g_raster_stats;   // diagnostics, see GS_RASTER_STATS
 uint32_t partition_own_bin_rows(const GsRenderOptions &opt, uint32_t binsY);
 uint32_t partition_own_tile_rows(const GsRenderOptions &opt, uint32_t binsY);

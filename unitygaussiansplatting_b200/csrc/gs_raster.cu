@@ -45,15 +45,17 @@ __device__ __forceinline__ uint32_t entry_tile(uint32_t e, uint32_t r, const Par
   return ty * tilesX + x0 + col;
 }
 
-// APPEND (several objects into one list): the entries go behind the entry_count[2] already listed, each value is tagged
-// `tag | splat id` (tag = the object's slot << kSlotShift), and the overflow flag entry_count[1] is sticky.
+// APPEND (several objects into one list): the entries go behind the entry_count[2] already listed, and each value is tagged
+// `tag | splat id` (tag = the object's slot << kSlotShift).  clear_overflow: the overflow flag entry_count[1] is set from this
+// list's total; otherwise it is only ever set.
 template <bool APPEND>
 __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ order, const uint32_t *__restrict__ rect,
                                                   const uint32_t *__restrict__ block_bits, uint32_t bits_words, uint32_t n, Partition part,
                                                   uint32_t tilesX, volatile uint32_t *status,
                                                   uint32_t *ticket, uint32_t capacity, uint32_t *__restrict__ keys,
                                                   uint32_t *__restrict__ vals, uint32_t *__restrict__ entry_count,
-                                                  uint32_t *__restrict__ ghist, uint32_t digit_bits, bool two_pass, uint32_t tag) {
+                                                  uint32_t *__restrict__ ghist, uint32_t digit_bits, bool two_pass, bool clear_overflow,
+                                                  uint32_t tag) {
   extern __shared__ uint32_t s_bits[];   // the view kernel's block bitmap (bits_words words), or nothing when it is too large to hold
   __shared__ uint32_t s_w[8];
   __shared__ uint32_t s_block, s_excl, s_base;
@@ -149,8 +151,8 @@ __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ o
       s_excl = excl;
       if (b == nblocks - 1) {
         const uint32_t all = min(excl + total, (uint32_t)kBinValMask);
-        if (APPEND) { if (all > capacity) entry_count[1] = 1u; }
-        else entry_count[1] = all > capacity ? 1u : 0u;   // overflow: lists are truncated, the API reports it
+        if (clear_overflow) entry_count[1] = all > capacity ? 1u : 0u;   // overflow: lists are truncated, the API reports it
+        else if (all > capacity) entry_count[1] = 1u;
         entry_count[0] = all > capacity ? capacity : all;
         entry_count[2] = all;
       }
@@ -209,64 +211,41 @@ static void bin_sort_plan(uint32_t bins, int *bits, int *passes) {
   *bits = bins <= 1024u ? 5 : bins <= 4096u ? 6 : bins <= 16384u ? 7 : 8;
 }
 
-cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, uint32_t n, const uint32_t *order, const uint32_t *rect,
-                           const uint32_t *block_bits, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted,
-                           int *launches) {
+cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, const DrawObjects &objs, bool clear_overflow,
+                           const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted, int *launches) {
   const Partition part = make_partition(opt);
-  const uint32_t tiles = fc.binsX * fc.binsY;
+  const bool run = objs.count > 1;
   *sorted = bs;
-  if (launches) *launches = 0;
-  if (!n) return cudaMemsetAsync(bs.entry_count, 0, 16, s);
-  const uint32_t nblocks = (n + kBinBlock - 1) / kBinBlock;
-  cudaMemsetAsync(bs.block_sums, 0, ((size_t)nblocks + 1) * sizeof(uint32_t), s);   // [0] ticket, [1..] look-back status
   int bits, passes;
-  bin_sort_plan(tiles, &bits, &passes);
-  if (launches) *launches = 2 + passes;   // bin_emit, look-back clear, sort passes
+  bin_sort_plan(fc.binsX * fc.binsY, &bits, &passes);
+  *launches = passes;
+  if (run) cudaMemsetAsync(bs.entry_count + 2, 0, sizeof(uint32_t), s);   // the objects append behind an empty list
   cudaMemsetAsync(sc.ghist, 0, 4 * 256 * sizeof(uint32_t), s);
-  uint32_t words = (uint32_t)block_bits_words(n);
   static int bits_global = -1;   // GS_WALK_BITS_GLOBAL=1 forces the large-asset path (bitmap read through L1) for tests
   if (bits_global < 0) { const char *e = getenv("GS_WALK_BITS_GLOBAL"); bits_global = (e && e[0] == '1') ? 1 : 0; }
-  if (bits_global) words = 0;
-  if (words * 4u > 16u * 1024u) words = 0;   // beside the kernel's 28 KB of static shared memory only 20 KB of the default 48 remain:
-                                              // a larger bitmap (> 33 M splats) is read through L1 instead
-  k_bin_emit<false><<<nblocks, 256, words * 4u, s>>>(order, rect, block_bits, words, n, part, fc.binsX, bs.block_sums + 1, bs.block_sums,
-                                                     bs.capacity, bs.tile_keys, bs.tile_vals, bs.entry_count, sc.ghist, (uint32_t)bits,
-                                                     passes == 2, 0u);
+  for (uint32_t k = 0; k < objs.count; ++k) {
+    const uint32_t n = objs.n[k], nblocks = (n + kBinBlock - 1) / kBinBlock;
+    cudaMemsetAsync(bs.block_sums, 0, ((size_t)nblocks + 1) * sizeof(uint32_t), s);   // [0] ticket, [1..] look-back status
+    uint32_t words = (uint32_t)block_bits_words(n);
+    if (bits_global) words = 0;
+    if (words * 4u > 16u * 1024u) words = 0;   // beside the kernel's 28 KB of static shared memory only 20 KB of the default 48
+                                                // remain: a larger bitmap (> 33 M splats) is read through L1 instead
+    const bool clear = clear_overflow && k == 0;   // the later objects' totals include this one's: they can only add overflow
+    if (run)
+      k_bin_emit<true><<<nblocks, 256, words * 4u, s>>>(objs.order[k], objs.rect[k], objs.block_bits[k], words, n, part, fc.binsX,
+                                                        bs.block_sums + 1, bs.block_sums, bs.capacity, bs.tile_keys, bs.tile_vals,
+                                                        bs.entry_count, sc.ghist, (uint32_t)bits, passes == 2, clear, k << kSlotShift);
+    else
+      k_bin_emit<false><<<nblocks, 256, words * 4u, s>>>(objs.order[k], objs.rect[k], objs.block_bits[k], words, n, part, fc.binsX,
+                                                         bs.block_sums + 1, bs.block_sums, bs.capacity, bs.tile_keys, bs.tile_vals,
+                                                         bs.entry_count, sc.ghist, (uint32_t)bits, passes == 2, clear, 0u);
+    *launches += 2;   // look-back clear, bin_emit
+  }
   // the entry count lives on the device: a persistent grid sorts whatever it is (no capacity-sized grid or memset)
   const cudaError_t e = launch_sort_pairs(bs.tile_keys, bs.tile_vals, bs.entry_count, bs.capacity, passes, bits, true, sc, s, nullptr,
                                           nullptr, /*count_is_capacity=*/false);
   if (e != cudaSuccess) return e;
   // an odd number of passes leaves the sorted lists in the sorter's ping-pong buffers
-  if (passes & 1) { sorted->tile_keys = sc.alt_keys; sorted->tile_vals = sc.alt_vals; }
-  return cudaSuccess;
-}
-
-cudaError_t launch_binning_objects(const FrameConsts &fc, uint32_t count, const BinObject *objs, bool clear_overflow, const BinScratch &bs,
-                                   const SortScratch &sc, cudaStream_t s, BinScratch *sorted, int *launches) {
-  const Partition part = make_partition(GsRenderOptions{});
-  const uint32_t tiles = fc.binsX * fc.binsY;
-  *sorted = bs;
-  int bits, passes;
-  bin_sort_plan(tiles, &bits, &passes);
-  *launches = 0;
-  // [0] and [2] start from an empty list; [1] (overflow) is kept across the runs of one call unless clear_overflow
-  cudaMemsetAsync(bs.entry_count + (clear_overflow ? 0 : 2), 0, (clear_overflow ? 3 : 1) * sizeof(uint32_t), s);
-  cudaMemsetAsync(sc.ghist, 0, 4 * 256 * sizeof(uint32_t), s);
-  for (uint32_t k = 0; k < count; ++k) {
-    const BinObject &o = objs[k];
-    const uint32_t nblocks = (o.n + kBinBlock - 1) / kBinBlock;
-    cudaMemsetAsync(bs.block_sums, 0, ((size_t)nblocks + 1) * sizeof(uint32_t), s);   // [0] ticket, [1..] look-back status
-    uint32_t words = (uint32_t)block_bits_words(o.n);
-    if (words * 4u > 16u * 1024u) words = 0;   // as launch_binning: a bitmap above 16 KB is read through L1
-    k_bin_emit<true><<<nblocks, 256, words * 4u, s>>>(o.order, o.rect, o.block_bits, words, o.n, part, fc.binsX, bs.block_sums + 1,
-                                                      bs.block_sums, bs.capacity, bs.tile_keys, bs.tile_vals, bs.entry_count, sc.ghist,
-                                                      (uint32_t)bits, passes == 2, k << kSlotShift);
-    *launches += 2;   // look-back clear, bin_emit
-  }
-  *launches += passes;
-  const cudaError_t e = launch_sort_pairs(bs.tile_keys, bs.tile_vals, bs.entry_count, bs.capacity, passes, bits, true, sc, s, nullptr,
-                                          nullptr, /*count_is_capacity=*/false);
-  if (e != cudaSuccess) return e;
   if (passes & 1) { sorted->tile_keys = sc.alt_keys; sorted->tile_vals = sc.alt_vals; }
   return cudaSuccess;
 }
@@ -401,7 +380,7 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
          const uint32_t *__restrict__ tile_vals, const uint32_t *__restrict__ tile_order, uint32_t *__restrict__ tile_cost, uint32_t ntx,
          uint8_t *__restrict__ rt, uint32_t pitch, cudaSurfaceObject_t surf, uint32_t band_packed, uint32_t load_rt,
          unsigned long long *stats, const float *__restrict__ zndc, const float *__restrict__ scene_depth,
-         std::conditional_t<MULTI, RasterObjects, NoRasterObjects> objs) {
+         std::conditional_t<MULTI, DrawObjects, NoRasterObjects> objs) {
   uint32_t st_batches = 0, st_culls = 0, st_cand = 0, st_eval = 0, st_blend = 0;   // GS_RASTER_STATS diagnostics (per warp)
   unsigned long long st_t0 = 0;
   if (STATS) asm volatile("mov.u64 %0, %globaltimer;" : "=l"(st_t0));
@@ -614,18 +593,18 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
 
 unsigned long long *g_raster_stats = nullptr;
 
-void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const BinScratch &bs, void *rt,
-                   uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s, const float *zndc,
-                   const float *scene_depth) {
+void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const DrawObjects &objs, const BinScratch &bs, void *rt,
+                   uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s, const float *scene_depth) {
   const Partition part = make_partition(opt);
   const uint32_t rows = part.own_tile_rows(fc.binsY);
   if (!rows || !fc.binsX) return;
   const uint32_t ntx = ((uint32_t)fc.screenW + kTile - 1) / kTile, ntiles = ntx * rows;
   const uint32_t grid = ntiles;
   k_tile_order<<<1, 1024, 0, s>>>(bs.tile_cost, ntiles, ntx, part, bs.tile_order);
-  const bool rop = opt.blend_mode == GS_BLEND_FP16_ROP;
+  const bool rop = opt.blend_mode == GS_BLEND_FP16_ROP, run = objs.count > 1;
   uint8_t *out = reinterpret_cast<uint8_t *>(rt);
-  // GS_RASTER_STATS=1: per-frame work counters (diagnostics; printed by tools/raster_stats.py through gs_debug_raster_stats)
+  // GS_RASTER_STATS=1: per-frame work counters of a one-object draw (diagnostics; printed by tools/raster_stats.py through
+  // gs_debug_raster_stats)
   static unsigned long long *stats = nullptr;
   static int want = -1;
   if (want < 0) { const char *e = getenv("GS_RASTER_STATS"); want = (e && e[0] == '1') ? 1 : 0; }
@@ -635,11 +614,17 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const floa
   uint2 *ranges = reinterpret_cast<uint2 *>(bs.bin_ranges);
   const uint32_t packed = part.range ? 0u : opt.band_packed, load = (opt.flags & GS_FLAG_LOAD_RT) ? 1u : 0u;
   k_bin_ranges<<<(bins + 7) / 8, 256, 0, s>>>(bs.tile_keys, bs.entry_count, bins, ranges);
+  // a run's raster reads each object's records and quad depths from `objs`, one object's from the draw / zndc arguments
+#define GS_RASTER_ARGS(OBJS)                                                                                                     \
+  <<<grid, 256, 0, s>>>(fc, part, objs.draw[0], ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, \
+                        packed, load, stats, objs.zndc[0], scene_depth, OBJS)
 #define GS_LAUNCH_RASTER(ROP, FMT, SURF)                                                                                        \
   do {                                                                                                                         \
-    if (fc.selValid || scene_depth) k_raster<ROP, FMT, false, true, SURF><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed, load, stats, zndc, scene_depth, NoRasterObjects{}); \
-    else if (stats) k_raster<ROP, FMT, true, false, SURF><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed, load, stats, nullptr, nullptr, NoRasterObjects{}); \
-    else k_raster<ROP, FMT, false, false, SURF><<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed, load, stats, nullptr, nullptr, NoRasterObjects{}); \
+    if (run && objs.extras) k_raster<ROP, FMT, false, true, SURF, true> GS_RASTER_ARGS(objs);                                   \
+    else if (run) k_raster<ROP, FMT, false, false, SURF, true> GS_RASTER_ARGS(objs);                                            \
+    else if (objs.extras) k_raster<ROP, FMT, false, true, SURF> GS_RASTER_ARGS(NoRasterObjects{});                              \
+    else if (stats) k_raster<ROP, FMT, true, false, SURF> GS_RASTER_ARGS(NoRasterObjects{});                                    \
+    else k_raster<ROP, FMT, false, false, SURF> GS_RASTER_ARGS(NoRasterObjects{});                                              \
   } while (0)
   // a null `rt` means the target is a CUDA array behind rt_surf
 #define GS_LAUNCH_RASTER_TARGET(ROP, FMT)                                                                                       \
@@ -653,37 +638,7 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const floa
   }
 #undef GS_LAUNCH_RASTER_TARGET
 #undef GS_LAUNCH_RASTER
-}
-
-void launch_raster_objects(const FrameConsts &fc, const GsRenderOptions &opt, const RasterObjects &objs, bool extras, const BinScratch &bs,
-                           void *rt, uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s,
-                           const float *scene_depth) {
-  const Partition part = make_partition(GsRenderOptions{});
-  const uint32_t ntx = ((uint32_t)fc.screenW + kTile - 1) / kTile, grid = ntx * part.own_tile_rows(fc.binsY);
-  if (!grid) return;
-  k_tile_order<<<1, 1024, 0, s>>>(bs.tile_cost, grid, ntx, part, bs.tile_order);
-  const uint32_t bins = fc.binsX * fc.binsY;
-  uint2 *ranges = reinterpret_cast<uint2 *>(bs.bin_ranges);
-  k_bin_ranges<<<(bins + 7) / 8, 256, 0, s>>>(bs.tile_keys, bs.entry_count, bins, ranges);
-  const bool rop = opt.blend_mode == GS_BLEND_FP16_ROP;
-  uint8_t *out = reinterpret_cast<uint8_t *>(rt);
-  const uint32_t load = (opt.flags & GS_FLAG_LOAD_RT) ? 1u : 0u;
-#define GS_LAUNCH_RASTER_OBJECTS(ROP, FMT, SURF)                                                                                \
-  do {                                                                                                                         \
-    if (extras) k_raster<ROP, FMT, false, true, SURF, true><<<grid, 256, 0, s>>>(fc, part, nullptr, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, 0u, load, nullptr, nullptr, scene_depth, objs); \
-    else k_raster<ROP, FMT, false, false, SURF, true><<<grid, 256, 0, s>>>(fc, part, nullptr, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, 0u, load, nullptr, nullptr, nullptr, objs); \
-  } while (0)
-#define GS_LAUNCH_RASTER_OBJECTS_TARGET(ROP, FMT)                                                                               \
-  do {                                                                                                                         \
-    if (out) GS_LAUNCH_RASTER_OBJECTS(ROP, FMT, false); else GS_LAUNCH_RASTER_OBJECTS(ROP, FMT, true);                          \
-  } while (0)
-  if (rt_format == GS_PIX_RGBA16F) {
-    if (rop) GS_LAUNCH_RASTER_OBJECTS_TARGET(true, GS_PIX_RGBA16F); else GS_LAUNCH_RASTER_OBJECTS_TARGET(false, GS_PIX_RGBA16F);
-  } else {
-    if (rop) GS_LAUNCH_RASTER_OBJECTS_TARGET(true, GS_PIX_RGBA32F); else GS_LAUNCH_RASTER_OBJECTS_TARGET(false, GS_PIX_RGBA32F);
-  }
-#undef GS_LAUNCH_RASTER_OBJECTS_TARGET
-#undef GS_LAUNCH_RASTER_OBJECTS
+#undef GS_RASTER_ARGS
 }
 
 uint32_t partition_own_bin_rows(const GsRenderOptions &opt, uint32_t binsY) { return make_partition(opt).own_rows_below(binsY); }
