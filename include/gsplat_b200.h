@@ -276,6 +276,47 @@ GS_API int gs_frame(GsContext *ctx, GsAsset *asset, const GsFrameParams *fp,
  * partition, row_begin / row_end or band_packed in opt.  Image errors are reported as gs_frame reports them. */
 GS_API int gs_frame_objects(GsContext *ctx, uint32_t object_count, GsAsset *const *assets, const GsFrameParams *fps,
                             const int32_t *do_sort, const GsRenderOptions *opt, GsImage *rt, GsImage *camera_target);
+/* The camera loop of GaussianSplatRenderSystem (R/GaussianSplatRenderer.cs:187-211): OnPreCullCamera runs for every camera
+ * but CameraType.Preview (:75, :581, :614) -- an editor's Scene and Game views, secondary views, one camera per eye (:590-591)
+ * -- and each camera gathers and draws its own objects (GatherSplatsForCamera :73-105, SortAndRenderSplats :108-169).
+ *   Result: bit-identical to
+ *     for c: gs_frame_objects(ctx, object_counts[c], assets + off_c, fps + off_c, do_sort + off_c, opt, rts[c], camera_targets[c])
+ *   with off_c = object_counts[0] + ... + object_counts[c - 1]: every render target, every camera target, and every asset's
+ *   persistent draw order and sorted keys, for both blend modes and both pixel formats.  An asset's draw order is one buffer
+ *   shared by every camera (m_GpuSortKeys, :142) and m_FrameCounter advances once per camera (:120-122), so a camera's sort
+ *   gathers its distances through the order the previous camera's sort left, and the stable sort breaks ties by it; with
+ *   m_SortNthFrame > 1 a camera that does not sort draws in the previous camera's order.  Both hold here.
+ *   object_counts [camera_count]: the objects of each camera, at least one.
+ *   assets, fps, do_sort: camera-major; camera c's objects, in its GatherSplatsForCamera order, are entries
+ *                   [off_c, off_c + object_counts[c]).  Each camera's objects share that camera's screen size; cameras may
+ *                   have different sizes.  An asset may appear in several cameras but only once within one.
+ *   opt             blend_mode (as gs_frame_objects); may be NULL.
+ *   rts, camera_targets [camera_count]: the cameras' images (host, device or CUDA-array memory, screen-sized); either of a
+ *                   camera's two may be NULL, not both.
+ * Consecutive cameras are drawn together as a camera run: per camera and per object in order, on the context stream, the
+ * sort (when do_sort), the view-calc and that object's bin-list entries (bin ids offset by the camera's first bin in the run);
+ * then one stable sort of the run's list by bin id, one raster pass over the tiles of all its cameras (the longest tiles of
+ * all cameras first), and per camera the host read-back and the composite.  The records of an asset that a later camera of
+ * the run draws again are kept in a context scratch slab until the raster.  A run holds at most 16 (camera, object) pairs,
+ * each object under 2^28 splats, cameras of at most 8160 px per axis and 65536 64-pixel bins in all, at most one scene depth
+ * buffer per camera, and one render-target pixel format (RGBA16F for a camera without rt).  A camera whose rt or camera
+ * target is the render target of an earlier camera of the run starts a new run.  A camera that breaks a limit of its own (a
+ * larger screen, more objects or splats, two depth buffers), and a camera that ends up alone in its run, is drawn by
+ * gs_frame_objects' own work, large screens' bin-list growth included.  A run's bin-list capacity is
+ * clamp(8 x its summed splats over all pairs, 4 Mi, 768 Mi) entries; overflow is reported as gs_frame_objects reports it
+ * (when the call reads a host image back, else at gs_sync), for any run of the call.
+ * GsStageTimes after this call follows gs_frame_objects' rules for several runs: bin_ms runs from the end of the last
+ * view-calc to the end of the last run's bin sort (in a camera run each object's entries are emitted right after its
+ * view-calc, so this holds the last object's emit and the run's sort), raster_ms and tile_entries are the last run's,
+ * composite_ms runs from the end of the last raster to the end of the last composite, total_ms (like gs_frame_objects') from
+ * the start of the last sort or view-calc to the end of the call, and kernel_launches counts every kernel.  With one camera
+ * the call does gs_frame_objects' device work, kernel for kernel.
+ * GS_ERR_INVALID_ARGUMENT, with nothing enqueued and nothing written: everything gs_frame_objects refuses, for any camera; a
+ * NULL object_counts, rts or camera_targets array; camera_count 0; a camera without objects; GS_FLAG_ASYNC_READBACK
+ * (per-camera double-buffered staging is not provided: host images are read back before the call returns). */
+GS_API int gs_frame_cameras(GsContext *ctx, uint32_t camera_count, const uint32_t *object_counts, GsAsset *const *assets,
+                            const GsFrameParams *fps, const int32_t *do_sort, const GsRenderOptions *opt, GsImage *const *rts,
+                            GsImage *const *camera_targets);
 
 /* Multi-GPU epilogue (SURVEY 8e.1): `gathered` is the all-gather of every partition's band-packed
  * render target, [partition_count][rows_per_partition][width] pixels in DEVICE memory, where

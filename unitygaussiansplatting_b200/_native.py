@@ -144,6 +144,9 @@ NATIVE_SYMBOLS = {
                            C.POINTER(GsImage), C.POINTER(GsImage)]),
     "gs_frame_objects": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(GsFrameParams), C.POINTER(C.c_int32),
                                    C.POINTER(GsRenderOptions), C.POINTER(GsImage), C.POINTER(GsImage)]),
+    "gs_frame_cameras": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_void_p), C.POINTER(GsFrameParams),
+                                   C.POINTER(C.c_int32), C.POINTER(GsRenderOptions), C.POINTER(C.POINTER(GsImage)),
+                                   C.POINTER(C.POINTER(GsImage))]),
     "gs_unshuffle_bands": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(GsImage)]),
     "gs_group_unique_id": (C.c_int, [C.c_void_p]),
     "gs_group_join": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_void_p)]),

@@ -373,12 +373,20 @@ static GsRenderOptions default_opts() {
 }
 
 int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameConsts &fc, bool cull, const GsRenderOptions &opt,
-            cudaStream_t stream) {
+            cudaStream_t stream, float4 *draw, float *zndc) {
   GsNvtxRange nvtx("GaussianSplat.CalcView");
   int rc = upload_frame_inputs(ctx, as, fp, stream);
   if (rc) return rc;
   const bool own = stream == ctx->stream;   // the group path runs view-calc beside the sort on a second stream and times it itself
   if (own) rec(ctx, EV_VIEW0);
+  if (draw) {   // a record slab: the asset's own records stay as they are
+    launch_calc_view(as->av, fc, ctx->d_cutouts, ctx->d_deleted, ctx->d_selected, as->view, as->rect, draw, as->block_bits,
+                     fp->scene_depth ? zndc : nullptr, cull, make_partition(opt), stream);
+    if (own) rec(ctx, EV_VIEW1);
+    ctx->launches += 1;
+    GS_CUDA_TRY(ctx, cudaGetLastError());
+    return GS_OK;
+  }
   if (fp->scene_depth && !as->zndc) GS_CUDA_TRY(ctx, cudaMalloc(&as->zndc, (size_t)as->av.n * sizeof(float) + 16));
   as->zndc_valid = fp->scene_depth != nullptr;
   launch_calc_view(as->av, fc, ctx->d_cutouts, ctx->d_deleted, ctx->d_selected, as->view, as->rect, as->draw, as->block_bits,
@@ -414,6 +422,46 @@ static int ensure_raster_tiles(GsContext *ctx, const FrameConsts &fc) {
     GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->bin.tile_cost, 0, (size_t)rtiles * 4, ctx->stream));
     ctx->raster_tiles_cur = rtiles;
   }
+  return GS_OK;
+}
+
+// The tile-cost history of a camera run of gs_frame_cameras, in *cost: one per camera layout ((raster tiles per row, rows) of
+// each camera of the run), kept in cams_tile_cost apart from the single-grid history above, so that the runs of one call and
+// the single-camera draws between calls do not reset each other's.  At most kCameraLayouts layouts are kept; one more starts
+// the cache afresh.  The launch-order scratch bin.tile_order is shared with the single-grid draws.
+constexpr size_t kCameraLayouts = 16;
+static int camera_tile_history(GsContext *ctx, uint32_t tiles, const std::vector<uint32_t> &layout, uint32_t **cost) {
+  if (tiles > ctx->raster_tiles_cap) {
+    cudaStreamSynchronize(ctx->stream);
+    cudaFree(ctx->bin.tile_cost); cudaFree(ctx->bin.tile_order);
+    ctx->bin.tile_cost = ctx->bin.tile_order = nullptr;
+    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.tile_cost, (size_t)tiles * 4));
+    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.tile_order, (size_t)tiles * 4));
+    ctx->raster_tiles_cap = tiles;
+    ctx->raster_tiles_cur = 0;
+  }
+  for (size_t i = 0; i < ctx->cams_layouts.size(); ++i)
+    if (ctx->cams_layouts[i] == layout) { *cost = ctx->cams_tile_cost + ctx->cams_layout_base[i]; return GS_OK; }
+  if (ctx->cams_layouts.size() >= kCameraLayouts) { ctx->cams_layouts.clear(); ctx->cams_layout_base.clear(); ctx->cams_cost_used = 0; }
+  const size_t need = ctx->cams_cost_used + tiles;
+  if (need > ctx->cams_cost_cap) {   // grown with the histories kept
+    uint32_t *grown = nullptr;
+    const size_t cap = std::max(need, 2 * ctx->cams_cost_cap);
+    GS_CUDA_TRY(ctx, cudaMalloc(&grown, cap * 4));
+    const cudaError_t e = ctx->cams_cost_used ? cudaMemcpyAsync(grown, ctx->cams_tile_cost, ctx->cams_cost_used * 4,
+                                                                cudaMemcpyDeviceToDevice, ctx->stream)
+                                              : cudaSuccess;
+    if (e != cudaSuccess) { cudaFree(grown); return fail_cuda(ctx, e, "cudaMemcpyAsync", __FILE__, __LINE__); }
+    cudaStreamSynchronize(ctx->stream);
+    cudaFree(ctx->cams_tile_cost);
+    ctx->cams_tile_cost = grown;
+    ctx->cams_cost_cap = cap;
+  }
+  GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->cams_tile_cost + ctx->cams_cost_used, 0, (size_t)tiles * 4, ctx->stream));
+  ctx->cams_layouts.push_back(layout);
+  ctx->cams_layout_base.push_back(ctx->cams_cost_used);
+  *cost = ctx->cams_tile_cost + ctx->cams_cost_used;
+  ctx->cams_cost_used = need;
   return GS_OK;
 }
 
@@ -609,6 +657,7 @@ void gs_destroy(GsContext *ctx) {
   cudaFree(ctx->sort.ghist); cudaFree(ctx->sort.tickets); cudaFree(ctx->d_scalar);
   cudaFree(ctx->bin.bin_ranges); cudaFree(ctx->bin.tile_cost); cudaFree(ctx->bin.tile_order); cudaFree(ctx->bin.block_sums); cudaFree(ctx->bin.entry_count); cudaFree(ctx->bin.tile_keys); cudaFree(ctx->bin.tile_vals);
   cudaFree(ctx->rt_scratch); cudaFree(ctx->tgt_scratch); cudaFree(ctx->d_cutouts); cudaFree(ctx->d_deleted); cudaFree(ctx->d_selected); cudaFree(ctx->d_depth);
+  cudaFree(ctx->cams_ghist); cudaFree(ctx->cams_scratch); cudaFree(ctx->cams_tile_cost);
   if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
   for (int i = 0; i < 2; ++i) {
     cudaFree(ctx->rt_async[i]);
@@ -880,8 +929,9 @@ static int begin_frame_image(GsContext *ctx, CallSurfaces &surfs, const GsRender
 
 // what follows the draw: the read-back of a host `rt` (enqueued only, with GS_FLAG_ASYNC_READBACK), the composite onto the
 // camera target, and the bin-list check of a call that waits for the device anyway
+// (check_overflow false: the caller checks the bin list once, after its last draw)
 static int end_frame_image(GsContext *ctx, CallSurfaces &surfs, GsImage *rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W,
-                           uint32_t H, const FrameImage &fi) {
+                           uint32_t H, const FrameImage &fi, bool check_overflow = true) {
   int rc = GS_OK;
   const bool rt_host = rt && rt->memory == GS_MEM_HOST;
   if (fi.async_rb) {
@@ -901,7 +951,199 @@ static int end_frame_image(GsContext *ctx, CallSurfaces &surfs, GsImage *rt, uin
     if ((rc = composite_impl(ctx, surfs, fi.d_rt, fi.pitch, fi.surf, rt_fmt, tgt, W, H, ctx->stream))) return rc;
     synced = tgt->memory == GS_MEM_HOST;
   }
-  if (rt_host || synced) return check_bin_overflow(ctx);
+  if (check_overflow && (rt_host || synced)) return check_bin_overflow(ctx);
+  return GS_OK;
+}
+
+// What gs_frame_objects checks of one camera's arguments: the objects, the options (validated into *opt) and the images.
+// Out: the objects' uniforms, the screen size, and the render target's pitch and pixel format (RGBA16F without one).
+static int check_camera(GsContext *ctx, uint32_t K, GsAsset *const *assets, const GsFrameParams *fps, GsRenderOptions *opt,
+                        const GsImage *rt, const GsImage *tgt, std::vector<FrameConsts> *fcs, uint32_t *W, uint32_t *H,
+                        uint32_t *rt_pitch, uint32_t *rt_fmt) {
+  int rc = GS_OK;
+  for (uint32_t k = 0; k < K; ++k) {
+    if (!assets[k]) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null asset");
+    if ((rc = check_params(ctx, assets[k], &fps[k]))) return rc;
+    if (fps[k].screen_w != fps[0].screen_w || fps[k].screen_h != fps[0].screen_h)
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the objects of one call must share screen_w / screen_h");
+  }
+  {
+    std::vector<GsAsset *> sorted(assets, assets + K);
+    std::sort(sorted.begin(), sorted.end());
+    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "an asset is listed for two objects (its draw order would be sorted twice)");
+  }
+  if (!rt && !tgt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_frame_objects needs rt and/or camera_target");
+  if (opt->flags & GS_FLAG_LOAD_RT) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "GS_FLAG_LOAD_RT is not accepted: the call clears the target once itself");
+  if (opt->partition_count > 1 || opt->partition_index || opt->row_begin || opt->row_end || opt->band_packed)
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_frame_objects draws the whole screen: no partition, row range or band packing");
+  fcs->resize(K);
+  for (uint32_t k = 0; k < K; ++k) (*fcs)[k] = make_frame_consts(&fps[k]);
+  if ((rc = check_options(ctx, (*fcs)[0], *opt))) return rc;
+  *W = (uint32_t)fps[0].screen_w; *H = (uint32_t)fps[0].screen_h;
+  uint32_t tgt_pitch = 0;
+  *rt_pitch = 0; *rt_fmt = GS_PIX_RGBA16F;
+  if (rt) { if ((rc = image_ok(ctx, rt, *W, *H, rt_pitch))) return rc; *rt_fmt = rt->format; }
+  if (tgt && (rc = image_ok(ctx, tgt, *W, *H, &tgt_pitch))) return rc;
+  return GS_OK;
+}
+
+// gs_frame_objects' work for one camera whose arguments have passed check_camera and whose frame inputs are reserved: per
+// object the sort and the view-calc, then the runs into the image *fi (set up here).  first: the first draw of its public call.
+static int draw_objects(GsContext *ctx, CallSurfaces &surfs, uint32_t K, GsAsset *const *assets, const GsFrameParams *fps,
+                        const int32_t *do_sort_flags, const std::vector<FrameConsts> &fcs, const GsRenderOptions &opt, GsImage *rt,
+                        uint32_t rt_pitch, uint32_t rt_fmt, const GsImage *tgt, uint32_t W, uint32_t H, bool first, FrameImage *fi) {
+  int rc = GS_OK;
+  for (uint32_t k = 0; k < K; ++k) {
+    if (do_sort_flags[k] && (rc = do_sort(ctx, assets[k], fcs[k]))) return rc;
+    if ((rc = do_view(ctx, assets[k], &fps[k], fcs[k], true, opt, ctx->stream))) return rc;
+  }
+  if ((rc = begin_frame_image(ctx, surfs, opt, rt, rt_pitch, rt_fmt, tgt, W, H, fi))) return rc;
+  // Runs: consecutive objects drawn by one bin list and one raster -- at most kRunObjects, each with fewer than 2^kSlotShift
+  // splats (the slot tag), binding at most one scene depth buffer.  An object of more splats, and the only object of a
+  // one-object call, is a run of one.  The first run starts from a cleared target, each later one blends under it.
+  for (uint32_t k = 0; k < K;) {
+    const GsFrameParams *depth_fp = &fps[k];
+    uint32_t e = k;
+    for (; e < K && e - k < kRunObjects && assets[e]->av.n <= kLocalIdMask; ++e) {
+      const GsFrameParams &f = fps[e];
+      if (!f.scene_depth) continue;
+      if (!depth_fp->scene_depth) depth_fp = &f;
+      else if (f.scene_depth != depth_fp->scene_depth || f.scene_depth_on_device != depth_fp->scene_depth_on_device) break;
+    }
+    e = std::max(e, k + 1);
+    GsRenderOptions o = opt;
+    if (k) o.flags |= GS_FLAG_LOAD_RT;
+    if ((rc = do_draw(ctx, fcs[k], o, assets + k, fps + k, e - k, first && k == 0, fi->d_rt, fi->pitch, rt_fmt, fi->surf))) return rc;
+    k = e;
+  }
+  return GS_OK;
+}
+
+// ---- gs_frame_cameras ---------------------------------------------------------------------------------
+// A camera run holds whole cameras of at most kMaxRunScreen px per axis, kRunObjects (camera, object) pairs and kMaxRunBins
+// bins in all (the largest bin space the bin sort's digit plans cover).
+constexpr uint32_t kMaxRunScreen = 8160, kMaxRunBins = 65536;
+
+struct CameraArgs {
+  uint32_t off, K, W, H, rt_pitch, rt_fmt;
+  std::vector<FrameConsts> fcs;
+  GsImage *rt, *tgt;
+};
+
+static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+// Draws the cameras cams[0, count) as one camera run (see DrawCameras): pair by pair the sort, the view-calc and the bin
+// emit, then one bin sort, one raster over every camera's tiles, and per camera the host read-back and the composite.
+static int draw_camera_run(GsContext *ctx, CallSurfaces &surfs, const CameraArgs *cams, uint32_t count, GsAsset *const *assets,
+                           const GsFrameParams *fps, const int32_t *do_sort_flags, const GsRenderOptions &opt, bool first) {
+  GsNvtxRange nvtx("GaussianSplat.DrawCameras");
+  const uint32_t rt_fmt = cams[0].rt_fmt;
+  DrawCameras dc;
+  memset(&dc, 0, sizeof(dc));
+  dc.count = count;
+  std::vector<uint32_t> layout;
+  uint32_t tiles = 0, bins = 0, pairs = 0;
+  uint64_t total = 0;
+  size_t bytes = 0;
+  std::vector<size_t> slab_at, stage_at(count, 0), depth_at(count, 0);
+  std::vector<const GsFrameParams *> depth_fp(count, nullptr);
+  for (uint32_t i = 0; i < count; ++i) {
+    const CameraArgs &c = cams[i];
+    RasterCamera &rc = dc.cam[i];
+    rc.W = c.W; rc.H = c.H;
+    rc.binsX = c.fcs[0].binsX;
+    rc.ntx = (c.W + kTile - 1) / kTile;
+    const uint32_t rows = c.fcs[0].binsY * (kBin / kTile);
+    rc.tile_base = tiles; rc.bin_base = bins;
+    tiles += rc.ntx * rows;
+    bins += rc.binsX * c.fcs[0].binsY;
+    layout.push_back(rc.ntx); layout.push_back(rows);
+    for (uint32_t k = 0; k < c.K; ++k) {
+      const GsAsset *as = assets[c.off + k];
+      const GsFrameParams &f = fps[c.off + k];
+      total += as->av.n;
+      if (f.scene_depth && !depth_fp[i]) depth_fp[i] = &f;
+      // every appearance of an asset but its last in the run draws from a record slab: a later view-calc overwrites its own
+      bool later = false;
+      for (uint32_t j = i; j < count && !later; ++j)
+        for (uint32_t m = (j == i ? k + 1 : 0); m < cams[j].K; ++m) later |= assets[cams[j].off + m] == as;
+      slab_at.push_back(later ? bytes + 1 : 0);   // 0: the asset's own buffers (offsets are stored + 1)
+      if (later) bytes += align256((size_t)as->av.n * 48) + (f.scene_depth ? align256((size_t)as->av.n * 4 + 16) : 0);
+      ++pairs;
+    }
+    if (!c.rt || c.rt->memory == GS_MEM_HOST) { stage_at[i] = bytes; bytes += align256((size_t)c.W * pix_bytes(rt_fmt) * c.H); }
+    if (depth_fp[i] && !depth_fp[i]->scene_depth_on_device) { depth_at[i] = bytes; bytes += align256((size_t)c.W * c.H * 4); }
+  }
+  int rc = GS_OK;
+  if (bytes && (rc = grow(ctx, &ctx->cams_scratch, &ctx->cams_bytes, bytes))) return rc;
+  if (!ctx->cams_ghist) GS_CUDA_TRY(ctx, cudaMalloc(&ctx->cams_ghist, 4 * 256 * sizeof(uint32_t)));
+  if ((rc = ensure_bin_scratch(ctx, (uint32_t)std::min<uint64_t>(total, 0xFFFFFFFFu), bins, 0))) return rc;
+  uint32_t *tile_cost = nullptr;
+  if ((rc = camera_tile_history(ctx, tiles, layout, &tile_cost))) return rc;
+  uint8_t *scratch = static_cast<uint8_t *>(ctx->cams_scratch);
+  for (uint32_t i = 0; i < count; ++i) {
+    const CameraArgs &c = cams[i];
+    RasterCamera &r = dc.cam[i];
+    if (!c.rt || c.rt->memory == GS_MEM_HOST) { r.rt = scratch + stage_at[i]; r.pitch = c.W * pix_bytes(rt_fmt); }
+    else if (c.rt->memory == GS_MEM_DEVICE) { r.rt = static_cast<uint8_t *>(c.rt->data); r.pitch = c.rt_pitch; }
+    else if ((rc = surfs.make(c.rt, &r.surf))) return rc;
+    if (depth_fp[i] && depth_fp[i]->scene_depth_on_device) r.depth = depth_fp[i]->scene_depth;
+    else if (depth_fp[i]) {
+      r.depth = reinterpret_cast<const float *>(scratch + depth_at[i]);
+      GS_CUDA_TRY(ctx, cudaMemcpyAsync(scratch + depth_at[i], depth_fp[i]->scene_depth, (size_t)c.W * c.H * 4, cudaMemcpyHostToDevice, ctx->stream));
+    }
+  }
+
+  DrawObjects objs;
+  memset(&objs, 0, sizeof(objs));
+  objs.count = pairs;
+  launch_bin_list_begin(ctx->bin, ctx->cams_ghist, ctx->stream);
+  uint32_t p = 0;
+  for (uint32_t i = 0; i < count; ++i) {
+    const CameraArgs &c = cams[i];
+    for (uint32_t k = 0; k < c.K; ++k, ++p) {
+      GsAsset *as = assets[c.off + k];
+      const GsFrameParams &f = fps[c.off + k];
+      float4 *draw = nullptr;
+      float *zndc = nullptr;
+      if (slab_at[p]) {
+        draw = reinterpret_cast<float4 *>(scratch + slab_at[p] - 1);
+        zndc = reinterpret_cast<float *>(scratch + slab_at[p] - 1 + align256((size_t)as->av.n * 48));
+      }
+      if (do_sort_flags[c.off + k] && (rc = do_sort(ctx, as, c.fcs[k]))) return rc;
+      if ((rc = do_view(ctx, as, &f, c.fcs[k], true, opt, ctx->stream, draw, zndc))) return rc;
+      // emitted before the next sort or view-calc of this asset replaces its order, rectangles and block bits
+      launch_bin_emit_pair(as->order, as->rect, as->block_bits, as->av.n, dc.cam[i].binsX, dc.cam[i].bin_base, p, first && p == 0, bins,
+                           ctx->bin, ctx->cams_ghist, ctx->stream);
+      ctx->launches += 2;   // look-back clear, bin_emit
+      objs.n[p] = as->av.n;
+      objs.draw[p] = draw ? draw : as->draw;
+      if (f.scene_depth) {
+        objs.zndc[p] = draw ? zndc : as->zndc;
+        objs.depth_mask |= 1u << p;
+      }
+      objs.extras |= f.selected_bits != nullptr || f.scene_depth != nullptr;
+    }
+  }
+  SortScratch sc = ctx->sort;
+  sc.ghist = ctx->cams_ghist;
+  BinScratch lists;
+  int sort_launches = 0;
+  GS_CUDA_TRY(ctx, launch_bin_list_sort(bins, ctx->bin, sc, ctx->stream, &lists, &sort_launches));
+  lists.tile_cost = tile_cost;
+  rec(ctx, EV_BIN1);
+  launch_raster_cameras(objs, dc, bins, tiles, opt.blend_mode, rt_fmt, lists, ctx->stream);
+  rec(ctx, EV_RASTER1);
+  ctx->launches += sort_launches + 3;   // bin sort passes; bin_ranges, tile_order, raster
+  GS_CUDA_TRY(ctx, cudaGetLastError());
+  for (uint32_t i = 0; i < count; ++i) {
+    const CameraArgs &c = cams[i];
+    const RasterCamera &r = dc.cam[i];
+    if (c.rt && c.rt->memory == GS_MEM_HOST)
+      GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(c.rt->data, c.rt_pitch, r.rt, r.pitch, (size_t)c.W * pix_bytes(rt_fmt), c.H, cudaMemcpyDeviceToHost, ctx->stream));
+    if (c.tgt && (rc = composite_impl(ctx, surfs, r.rt, r.pitch, r.surf, rt_fmt, c.tgt, c.W, c.H, ctx->stream))) return rc;
+  }
   return GS_OK;
 }
 }  // namespace gs
@@ -938,62 +1180,102 @@ int gs_frame_objects(GsContext *ctx, uint32_t object_count, GsAsset *const *asse
   if (!ctx || !assets || !fps || !do_sort_flags) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null context / assets / fps / do_sort");
   const uint32_t K = object_count;
   if (K == 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "object_count is 0");
-  int rc = GS_OK;
-  for (uint32_t k = 0; k < K; ++k) {
-    if (!assets[k]) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null asset");
-    if ((rc = check_params(ctx, assets[k], &fps[k]))) return rc;
-    if (fps[k].screen_w != fps[0].screen_w || fps[k].screen_h != fps[0].screen_h)
-      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the objects of one call must share screen_w / screen_h");
-  }
-  {
-    std::vector<GsAsset *> sorted(assets, assets + K);
-    std::sort(sorted.begin(), sorted.end());
-    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
-      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "an asset is listed for two objects (its draw order would be sorted twice)");
-  }
-  if (!rt && !tgt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_frame_objects needs rt and/or camera_target");
   GsRenderOptions opt = opt_in ? *opt_in : default_opts();
-  if (opt.flags & GS_FLAG_LOAD_RT) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "GS_FLAG_LOAD_RT is not accepted: the call clears the target once itself");
-  if (opt.partition_count > 1 || opt.partition_index || opt.row_begin || opt.row_end || opt.band_packed)
-    return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_frame_objects draws the whole screen: no partition, row range or band packing");
-  std::vector<FrameConsts> fcs(K);
-  for (uint32_t k = 0; k < K; ++k) fcs[k] = make_frame_consts(&fps[k]);
-  if ((rc = check_options(ctx, fcs[0], opt))) return rc;
-  const uint32_t W = (uint32_t)fps[0].screen_w, H = (uint32_t)fps[0].screen_h;
-  uint32_t rt_pitch = 0, tgt_pitch = 0, rt_fmt = GS_PIX_RGBA16F;
-  if (rt) { if ((rc = image_ok(ctx, rt, W, H, &rt_pitch))) return rc; rt_fmt = rt->format; }
-  if (tgt && (rc = image_ok(ctx, tgt, W, H, &tgt_pitch))) return rc;
+  std::vector<FrameConsts> fcs;
+  uint32_t W = 0, H = 0, rt_pitch = 0, rt_fmt = GS_PIX_RGBA16F;
+  int rc = check_camera(ctx, K, assets, fps, &opt, rt, tgt, &fcs, &W, &H, &rt_pitch, &rt_fmt);
+  if (rc) return rc;
   // the objects' cutouts / bits share the context's buffers: sized for all of them before the first view-calc is queued
   for (uint32_t k = 0; k < K; ++k)
     if ((rc = reserve_frame_inputs(ctx, assets[k], &fps[k]))) return rc;
 
   for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
-  for (uint32_t k = 0; k < K; ++k) {
-    if (do_sort_flags[k] && (rc = do_sort(ctx, assets[k], fcs[k]))) return rc;
-    if ((rc = do_view(ctx, assets[k], &fps[k], fcs[k], true, opt, ctx->stream))) return rc;
-  }
   CallSurfaces surfs(ctx);
   FrameImage fi;
-  if ((rc = begin_frame_image(ctx, surfs, opt, rt, rt_pitch, rt_fmt, tgt, W, H, &fi))) return rc;
-  // Runs: consecutive objects drawn by one bin list and one raster -- at most kRunObjects, each with fewer than 2^kSlotShift
-  // splats (the slot tag), binding at most one scene depth buffer.  An object of more splats, and the only object of a
-  // one-object call, is a run of one.  The first run starts from a cleared target, each later one blends under it.
-  for (uint32_t k = 0; k < K;) {
-    const GsFrameParams *depth_fp = &fps[k];
-    uint32_t e = k;
-    for (; e < K && e - k < kRunObjects && assets[e]->av.n <= kLocalIdMask; ++e) {
-      const GsFrameParams &f = fps[e];
-      if (!f.scene_depth) continue;
-      if (!depth_fp->scene_depth) depth_fp = &f;
-      else if (f.scene_depth != depth_fp->scene_depth || f.scene_depth_on_device != depth_fp->scene_depth_on_device) break;
-    }
-    e = std::max(e, k + 1);
-    GsRenderOptions o = opt;
-    if (k) o.flags |= GS_FLAG_LOAD_RT;
-    if ((rc = do_draw(ctx, fcs[k], o, assets + k, fps + k, e - k, k == 0, fi.d_rt, fi.pitch, rt_fmt, fi.surf))) return rc;
-    k = e;
-  }
+  if ((rc = draw_objects(ctx, surfs, K, assets, fps, do_sort_flags, fcs, opt, rt, rt_pitch, rt_fmt, tgt, W, H, true, &fi))) return rc;
   return end_frame_image(ctx, surfs, rt, rt_pitch, rt_fmt, tgt, W, H, fi);
+}
+
+int gs_frame_cameras(GsContext *ctx, uint32_t camera_count, const uint32_t *object_counts, GsAsset *const *assets, const GsFrameParams *fps,
+                     const int32_t *do_sort_flags, const GsRenderOptions *opt_in, GsImage *const *rts, GsImage *const *camera_targets) {
+  if (!ctx || !object_counts || !assets || !fps || !do_sort_flags || !rts || !camera_targets)
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null context / object_counts / assets / fps / do_sort / rts / camera_targets");
+  if (camera_count == 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "camera_count is 0");
+  GsRenderOptions opt = opt_in ? *opt_in : default_opts();
+  if (opt.flags & GS_FLAG_ASYNC_READBACK)
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, "GS_FLAG_ASYNC_READBACK is not accepted by gs_frame_cameras: its host images are read back before it returns");
+  std::vector<CameraArgs> cams(camera_count);
+  uint64_t pairs = 0;
+  int rc = GS_OK;
+  for (uint32_t c = 0; c < camera_count; ++c) {
+    CameraArgs &a = cams[c];
+    if (object_counts[c] == 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "a camera has no objects (leave it out: the reference draws nothing for it)");
+    a.off = (uint32_t)pairs; a.K = object_counts[c]; a.rt = rts[c]; a.tgt = camera_targets[c];
+    pairs += a.K;
+    if (pairs > 0xFFFFFFFFu) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "more than 2^32 - 1 objects in all");
+    GsRenderOptions o = opt;
+    if ((rc = check_camera(ctx, a.K, assets + a.off, fps + a.off, &o, a.rt, a.tgt, &a.fcs, &a.W, &a.H, &a.rt_pitch, &a.rt_fmt))) return rc;
+  }
+  for (uint64_t p = 0; p < pairs; ++p)
+    if ((rc = reserve_frame_inputs(ctx, assets[p], &fps[p]))) return rc;
+
+  for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
+  CallSurfaces surfs(ctx);
+  bool host = false;
+  // May camera `c` join the run cams[c0, c)?  Its own limits, the run's totals, one pixel format, and no image shared with the
+  // run's render targets (two cameras rasterizing into one image at once would race, where the loop draws one after the other).
+  auto joins = [&](uint32_t c0, uint32_t c, uint32_t run_pairs, uint32_t run_bins) {
+    const CameraArgs &a = cams[c];
+    if (a.W > kMaxRunScreen || a.H > kMaxRunScreen || a.K > kRunObjects) return false;
+    const GsFrameParams *depth = nullptr;
+    for (uint32_t k = 0; k < a.K; ++k) {
+      const GsFrameParams &f = fps[a.off + k];
+      if (assets[a.off + k]->av.n > kLocalIdMask) return false;
+      if (!f.scene_depth) continue;
+      if (!depth) depth = &f;
+      else if (f.scene_depth != depth->scene_depth || f.scene_depth_on_device != depth->scene_depth_on_device) return false;
+    }
+    if (c == c0) return true;
+    if (run_pairs + a.K > kRunObjects || run_bins + a.fcs[0].binsX * a.fcs[0].binsY > kMaxRunBins || a.rt_fmt != cams[c0].rt_fmt) return false;
+    for (uint32_t j = c0; j < c; ++j) {
+      const void *rj = cams[j].rt ? cams[j].rt->data : nullptr, *tj = cams[j].tgt ? cams[j].tgt->data : nullptr;
+      if (a.rt && (a.rt->data == rj || a.rt->data == tj)) return false;
+      if (a.tgt && a.tgt->data == rj) return false;
+    }
+    return true;
+  };
+  for (uint32_t c = 0; c < camera_count;) {
+    uint32_t e = c, run_pairs = 0, run_bins = 0;
+    while (e < camera_count && joins(c, e, run_pairs, run_bins)) {
+      run_pairs += cams[e].K;
+      run_bins += cams[e].fcs[0].binsX * cams[e].fcs[0].binsY;
+      ++e;
+    }
+    for (uint32_t j = c; j < std::max(e, c + 1); ++j)
+      host |= (cams[j].rt && cams[j].rt->memory == GS_MEM_HOST) || (cams[j].tgt && cams[j].tgt->memory == GS_MEM_HOST);
+    if (e - c >= 2) {
+      if ((rc = draw_camera_run(ctx, surfs, &cams[c], e - c, assets, fps, do_sort_flags, opt, c == 0))) return rc;
+      c = e;
+      continue;
+    }
+    // a camera on its own: gs_frame_objects' work
+    CameraArgs &a = cams[c];
+    if (c > 0 && (a.fcs[0].binsX > kRuleBins || a.fcs[0].binsY > kRuleBins)) {
+      // a growing bin list clears the overflow flag unless an earlier draw of the call was truncated (do_draw): read it
+      uint32_t flag = 0;
+      GS_CUDA_TRY(ctx, cudaMemcpyAsync(&flag, ctx->bin.entry_count + 1, 4, cudaMemcpyDeviceToHost, ctx->stream));
+      GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+      ctx->bin_overflow = flag != 0;
+    }
+    FrameImage fi;
+    if ((rc = draw_objects(ctx, surfs, a.K, assets + a.off, fps + a.off, do_sort_flags + a.off, a.fcs, opt, a.rt, a.rt_pitch, a.rt_fmt, a.tgt,
+                           a.W, a.H, c == 0, &fi)))
+      return rc;
+    if ((rc = end_frame_image(ctx, surfs, a.rt, a.rt_pitch, a.rt_fmt, a.tgt, a.W, a.H, fi, false))) return rc;
+    ++c;
+  }
+  // overflow is reported as gs_frame_objects reports it: here when a host image was read back, else at gs_sync
+  return host ? check_bin_overflow(ctx) : GS_OK;
 }
 
 int gs_unshuffle_bands(GsContext *ctx, const void *gathered, uint32_t parts, uint32_t band_rows, uint32_t rows_pp, uint32_t fmt,

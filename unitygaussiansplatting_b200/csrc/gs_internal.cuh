@@ -43,6 +43,16 @@ struct GsContext {
   gs::BinScratch bin{};
   uint32_t bin_blocks_cap = 0, tiles_cap = 0, raster_tiles_cap = 0, raster_tiles_cur = 0;
   bool bin_overflow = false;   // the bin list's overflow flag as the last read-back of a frame above kLargeFrameBins left it
+  // gs_frame_cameras: the tile-cost histories of the camera layouts seen ((raster tiles per row, rows) per camera of a run,
+  // each history at its base in cams_tile_cost), the digit histograms of a camera run's bin list (the depth sorts between its
+  // emits use sort.ghist), and one scratch buffer for a run's record slabs, staging images and host depth buffers
+  std::vector<std::vector<uint32_t>> cams_layouts;
+  std::vector<size_t> cams_layout_base;
+  uint32_t *cams_tile_cost = nullptr;
+  size_t cams_cost_cap = 0, cams_cost_used = 0;
+  uint32_t *cams_ghist = nullptr;
+  void *cams_scratch = nullptr;
+  size_t cams_bytes = 0;
   // image scratch
   void *rt_scratch = nullptr;
   size_t rt_bytes = 0;
@@ -105,8 +115,10 @@ int ensure_sort_scratch(GsContext *ctx, uint32_t capacity);
 // ctx->stream and `busy` (when given: another stream whose view-calc may still read it) have drained.  Uploads nothing.
 int reserve_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t busy = nullptr);
 int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t stream);
+// draw / zndc (optional): where the raster records and quad depths go instead of the asset's own buffers (gs_frame_cameras'
+// record slabs); the asset's draw state is then left as it was
 int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameConsts &fc, bool cull, const GsRenderOptions &opt,
-            cudaStream_t stream);
+            cudaStream_t stream, float4 *draw = nullptr, float *zndc = nullptr);
 // Bins and rasterizes the objects as[0, count), drawn with the uniforms fps[0, count), into a device image (d_rt == nullptr:
 // the CUDA array behind `surf`) on ctx->stream: one object with gs_frame's kernels, or several as one run of gs_frame_objects
 // (DrawObjects).  The scene depth buffer bound is that of the first object that has one.  `first`: the first draw of its

@@ -200,6 +200,39 @@ struct NoRasterObjects {};
 // entry_count[1] from its own total; otherwise the flag is only ever set, so an earlier draw's truncation stays reported.
 cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, const DrawObjects &objs, bool clear_overflow,
                            const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted, int *launches);
+
+// A camera run of gs_frame_cameras: consecutive cameras whose (camera, object) pairs, at most kRunObjects in all, share one
+// bin list, one bin sort and one k_raster<..., MULTI, CAMS> pass.  Camera c owns the bin ids [bin_base, bin_base + its bins)
+// and the raster tiles [tile_base, tile_base + its tiles) of the run; the raster finds a tile's camera in this table, staged
+// in shared memory.
+struct RasterCamera {
+  uint8_t *rt;                 // linear device image, or nullptr: the CUDA array behind `surf`
+  cudaSurfaceObject_t surf;
+  const float *depth;          // the camera's scene depth buffer (device memory), or nullptr
+  uint32_t pitch, tile_base, bin_base, ntx, binsX, W, H;
+  uint32_t load;               // 1: blend under what the image holds; 0: the image starts cleared
+};
+struct DrawCameras {
+  RasterCamera cam[kRunObjects];
+  uint32_t count;
+};
+// The run's binning, in three steps around its pairs' sorts and view-calcs (a pair's emit must follow its view-calc before
+// the next sort or view-calc of the same asset overwrites order / rect / block_bits):
+//   launch_bin_list_begin: empties the list and zeroes `ghist`, the digit histograms the emits count into;
+//   launch_bin_emit_pair:  appends one pair's entries, keys offset by its camera's bin_base, values tagged with its slot;
+//   launch_bin_list_sort:  the stable sort of the run's list by bin id, over `bins` bins, with the histograms in `ghist`.
+// bin_sort_bits gives the digit plan the emits and the sort share.
+void bin_sort_bits(uint32_t bins, int *bits, int *passes);
+void launch_bin_list_begin(const BinScratch &bs, uint32_t *ghist, cudaStream_t s);
+void launch_bin_emit_pair(const uint32_t *order, const uint32_t *rect, const uint32_t *block_bits, uint32_t n, uint32_t binsX,
+                          uint32_t bin_base, uint32_t slot, bool clear_overflow, uint32_t bins, const BinScratch &bs, uint32_t *ghist,
+                          cudaStream_t s);
+cudaError_t launch_bin_list_sort(uint32_t bins, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted,
+                                 int *launches);
+// k_bin_ranges over the run's bins, k_tile_order over its raster tiles (history indexed by tile_base + tile), and the raster.
+// Every render target of the run has rt_format.
+void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, uint32_t bins, uint32_t tiles, uint32_t blend_mode,
+                           uint32_t rt_format, const BinScratch &bs, cudaStream_t s);
 // scene_depth: the W x H depth buffer the depth-tested objects are tested against (nullptr: none).  opt: tile partition,
 // band_packed, blend mode and GS_FLAG_LOAD_RT.  Images here are linear device memory (pointer, pitch) or, when the pointer is
 // null, a CUDA array behind a surface object.

@@ -21,6 +21,7 @@
 //               every splat (GS_BLEND_FP16_ROP) -- or kept in float32 (GS_BLEND_FP32).
 //   3. composite (S/GaussianComposite.shader:35-39).
 #include <cstdlib>
+#include <cstring>
 #include <type_traits>
 
 #include "gs_kernels.cuh"
@@ -48,14 +49,15 @@ __device__ __forceinline__ uint32_t entry_tile(uint32_t e, uint32_t r, const Par
 // APPEND (several objects into one list): the entries go behind the entry_count[2] already listed, and each value is tagged
 // `tag | splat id` (tag = the object's slot << kSlotShift).  clear_overflow: the overflow flag entry_count[1] is set from this
 // list's total; otherwise it is only ever set.
-template <bool APPEND>
+// CAMS (a camera run of gs_frame_cameras, with APPEND): each key is the bin id plus key_base, the camera's first bin in the run.
+template <bool APPEND, bool CAMS = false>
 __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ order, const uint32_t *__restrict__ rect,
                                                   const uint32_t *__restrict__ block_bits, uint32_t bits_words, uint32_t n, Partition part,
                                                   uint32_t tilesX, volatile uint32_t *status,
                                                   uint32_t *ticket, uint32_t capacity, uint32_t *__restrict__ keys,
                                                   uint32_t *__restrict__ vals, uint32_t *__restrict__ entry_count,
                                                   uint32_t *__restrict__ ghist, uint32_t digit_bits, bool two_pass, bool clear_overflow,
-                                                  uint32_t tag) {
+                                                  uint32_t tag, uint32_t key_base) {
   extern __shared__ uint32_t s_bits[];   // the view kernel's block bitmap (bits_words words), or nothing when it is too large to hold
   __shared__ uint32_t s_w[8];
   __shared__ uint32_t s_block, s_excl, s_base;
@@ -185,7 +187,7 @@ __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ o
       const uint32_t oid = __shfl_sync(0xffffffffu, it.x, lo);
       const uint32_t o = off + x;
       if (x < T && o < capacity) {
-        const uint32_t tile = entry_tile(x - opre, orc, part, tilesX);
+        const uint32_t tile = entry_tile(x - opre, orc, part, tilesX) + (CAMS ? key_base : 0u);
         keys[o] = tile;
         vals[o] = APPEND ? (tag | oid) : oid;
         atomicAdd(&s_dh[tile & dmask], 1u);
@@ -210,6 +212,56 @@ static void bin_sort_plan(uint32_t bins, int *bits, int *passes) {
   *passes = 2;
   *bits = bins <= 1024u ? 5 : bins <= 4096u ? 6 : bins <= 16384u ? 7 : 8;
 }
+void bin_sort_bits(uint32_t bins, int *bits, int *passes) { bin_sort_plan(bins, bits, passes); }
+
+// the sort by bin id of a list whose digit histograms are in sc.ghist; an odd number of passes leaves it in the sorter's
+// ping-pong buffers
+static cudaError_t sort_bin_list(int bits, int passes, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted) {
+  // the entry count lives on the device: a persistent grid sorts whatever it is (no capacity-sized grid or memset)
+  const cudaError_t e = launch_sort_pairs(bs.tile_keys, bs.tile_vals, bs.entry_count, bs.capacity, passes, bits, true, sc, s, nullptr,
+                                          nullptr, /*count_is_capacity=*/false);
+  if (e != cudaSuccess) return e;
+  if (passes & 1) { sorted->tile_keys = sc.alt_keys; sorted->tile_vals = sc.alt_vals; }
+  return cudaSuccess;
+}
+
+// the shared-memory copy of the view kernel's block bitmap (0 words: read through L1)
+static uint32_t bin_bits_words(uint32_t n) {
+  static int bits_global = -1;   // GS_WALK_BITS_GLOBAL=1 forces the large-asset path (bitmap read through L1) for tests
+  if (bits_global < 0) { const char *e = getenv("GS_WALK_BITS_GLOBAL"); bits_global = (e && e[0] == '1') ? 1 : 0; }
+  uint32_t words = (uint32_t)block_bits_words(n);
+  if (bits_global) words = 0;
+  if (words * 4u > 16u * 1024u) words = 0;   // beside the kernel's 28 KB of static shared memory only 20 KB of the default 48
+                                              // remain: a larger bitmap (> 33 M splats) is read through L1 instead
+  return words;
+}
+
+void launch_bin_list_begin(const BinScratch &bs, uint32_t *ghist, cudaStream_t s) {
+  cudaMemsetAsync(bs.entry_count + 2, 0, sizeof(uint32_t), s);   // the pairs append behind an empty list
+  cudaMemsetAsync(ghist, 0, 4 * 256 * sizeof(uint32_t), s);
+}
+
+void launch_bin_emit_pair(const uint32_t *order, const uint32_t *rect, const uint32_t *block_bits, uint32_t n, uint32_t binsX,
+                          uint32_t bin_base, uint32_t slot, bool clear_overflow, uint32_t bins, const BinScratch &bs, uint32_t *ghist,
+                          cudaStream_t s) {
+  int bits, passes;
+  bin_sort_plan(bins, &bits, &passes);
+  const uint32_t nblocks = (n + kBinBlock - 1) / kBinBlock, words = bin_bits_words(n);
+  cudaMemsetAsync(bs.block_sums, 0, ((size_t)nblocks + 1) * sizeof(uint32_t), s);   // [0] ticket, [1..] look-back status
+  k_bin_emit<true, true><<<nblocks, 256, words * 4u, s>>>(order, rect, block_bits, words, n, Partition{0, 0, 1, 0, 0, 0}, binsX,
+                                                          bs.block_sums + 1, bs.block_sums, bs.capacity, bs.tile_keys, bs.tile_vals,
+                                                          bs.entry_count, ghist, (uint32_t)bits, passes == 2, clear_overflow,
+                                                          slot << kSlotShift, bin_base);
+}
+
+cudaError_t launch_bin_list_sort(uint32_t bins, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted,
+                                 int *launches) {
+  int bits, passes;
+  bin_sort_plan(bins, &bits, &passes);
+  *sorted = bs;
+  *launches = passes;
+  return sort_bin_list(bits, passes, bs, sc, s, sorted);
+}
 
 cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, const DrawObjects &objs, bool clear_overflow,
                            const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted, int *launches) {
@@ -221,33 +273,22 @@ cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, co
   *launches = passes;
   if (run) cudaMemsetAsync(bs.entry_count + 2, 0, sizeof(uint32_t), s);   // the objects append behind an empty list
   cudaMemsetAsync(sc.ghist, 0, 4 * 256 * sizeof(uint32_t), s);
-  static int bits_global = -1;   // GS_WALK_BITS_GLOBAL=1 forces the large-asset path (bitmap read through L1) for tests
-  if (bits_global < 0) { const char *e = getenv("GS_WALK_BITS_GLOBAL"); bits_global = (e && e[0] == '1') ? 1 : 0; }
   for (uint32_t k = 0; k < objs.count; ++k) {
     const uint32_t n = objs.n[k], nblocks = (n + kBinBlock - 1) / kBinBlock;
     cudaMemsetAsync(bs.block_sums, 0, ((size_t)nblocks + 1) * sizeof(uint32_t), s);   // [0] ticket, [1..] look-back status
-    uint32_t words = (uint32_t)block_bits_words(n);
-    if (bits_global) words = 0;
-    if (words * 4u > 16u * 1024u) words = 0;   // beside the kernel's 28 KB of static shared memory only 20 KB of the default 48
-                                                // remain: a larger bitmap (> 33 M splats) is read through L1 instead
+    const uint32_t words = bin_bits_words(n);
     const bool clear = clear_overflow && k == 0;   // the later objects' totals include this one's: they can only add overflow
     if (run)
       k_bin_emit<true><<<nblocks, 256, words * 4u, s>>>(objs.order[k], objs.rect[k], objs.block_bits[k], words, n, part, fc.binsX,
                                                         bs.block_sums + 1, bs.block_sums, bs.capacity, bs.tile_keys, bs.tile_vals,
-                                                        bs.entry_count, sc.ghist, (uint32_t)bits, passes == 2, clear, k << kSlotShift);
+                                                        bs.entry_count, sc.ghist, (uint32_t)bits, passes == 2, clear, k << kSlotShift, 0u);
     else
       k_bin_emit<false><<<nblocks, 256, words * 4u, s>>>(objs.order[k], objs.rect[k], objs.block_bits[k], words, n, part, fc.binsX,
                                                          bs.block_sums + 1, bs.block_sums, bs.capacity, bs.tile_keys, bs.tile_vals,
-                                                         bs.entry_count, sc.ghist, (uint32_t)bits, passes == 2, clear, 0u);
+                                                         bs.entry_count, sc.ghist, (uint32_t)bits, passes == 2, clear, 0u, 0u);
     *launches += 2;   // look-back clear, bin_emit
   }
-  // the entry count lives on the device: a persistent grid sorts whatever it is (no capacity-sized grid or memset)
-  const cudaError_t e = launch_sort_pairs(bs.tile_keys, bs.tile_vals, bs.entry_count, bs.capacity, passes, bits, true, sc, s, nullptr,
-                                          nullptr, /*count_is_capacity=*/false);
-  if (e != cudaSuccess) return e;
-  // an odd number of passes leaves the sorted lists in the sorter's ping-pong buffers
-  if (passes & 1) { sorted->tile_keys = sc.alt_keys; sorted->tile_vals = sc.alt_vals; }
-  return cudaSuccess;
+  return sort_bin_list(bits, passes, bs, sc, s, sorted);
 }
 
 // ---- 2. raster ---------------------------------------------------------------------------------
@@ -374,13 +415,17 @@ __device__ __forceinline__ bool block_may_touch_quad(const float4 &A, float i2x,
 // separate instantiation so that the linear ones keep their code.
 // MULTI: the list holds the entries of several objects (one run of gs_frame_objects), each tagged with its slot in `objs`; the
 // records are gathered from that object's buffers, and the result is what drawing the objects one after the other leaves.
-template <bool FP16_ROP, int OUT_FMT, bool STATS, bool SEL = false, bool SURF = false, bool MULTI = false>
+// CAMS (with MULTI): a camera run of gs_frame_cameras.  The grid covers every camera's tiles; a tile finds its camera in `cams`
+// (staged in shared memory), which gives it the screen size, bins, image (pointer and pitch, or a surface when the pointer is
+// null), scene depth buffer and load flag that the other instantiations take from fc and the image arguments.  The camera's
+// bin ids start at its bin_base in bin_ranges; tile_cost is indexed by tile_base + the tile.
+template <bool FP16_ROP, int OUT_FMT, bool STATS, bool SEL = false, bool SURF = false, bool MULTI = false, bool CAMS = false>
 __global__ void __launch_bounds__(256)
 k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const uint2 *__restrict__ bin_ranges,
          const uint32_t *__restrict__ tile_vals, const uint32_t *__restrict__ tile_order, uint32_t *__restrict__ tile_cost, uint32_t ntx,
          uint8_t *__restrict__ rt, uint32_t pitch, cudaSurfaceObject_t surf, uint32_t band_packed, uint32_t load_rt,
          unsigned long long *stats, const float *__restrict__ zndc, const float *__restrict__ scene_depth,
-         std::conditional_t<MULTI, DrawObjects, NoRasterObjects> objs) {
+         std::conditional_t<MULTI, DrawObjects, NoRasterObjects> objs, std::conditional_t<CAMS, DrawCameras, NoRasterObjects> cams) {
   uint32_t st_batches = 0, st_culls = 0, st_cand = 0, st_eval = 0, st_blend = 0;   // GS_RASTER_STATS diagnostics (per warp)
   unsigned long long st_t0 = 0;
   if (STATS) asm volatile("mov.u64 %0, %globaltimer;" : "=l"(st_t0));
@@ -388,11 +433,29 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   // asynchronously while batch k is composited
   __shared__ __align__(128) float4 s_rec[2][3][256];  // plane 0: cx, cy, i1x, i1y   1: i2x, i2y, opacity, hx   2: r, g, b, hy
   __shared__ float s_z[SEL ? 2 : 1][SEL ? 256 : 1];   // quad depths of the staged batch (depth test only)
-  const bool depth_test = SEL && scene_depth != nullptr;
   // MULTI: the object table, staged where a slot can index it without local memory, and each staged entry's slot
   __shared__ const float4 *s_draw[MULTI ? kRunObjects : 1];
   __shared__ const float *s_zndc[MULTI ? kRunObjects : 1];
   __shared__ uint8_t s_slot[MULTI ? 2 : 1][MULTI ? 256 : 1];
+  __shared__ RasterCamera s_cam[CAMS ? kRunObjects : 1];
+  // CAMS: the tile's camera and its first tile / bin in the run
+  uint32_t lin = 0, tile_base = 0, bin_base = 0;
+  if constexpr (CAMS) {
+    if (threadIdx.x == 0) {
+#pragma unroll
+      for (uint32_t k = 0; k < kRunObjects; ++k) { s_draw[k] = objs.draw[k]; s_zndc[k] = objs.zndc[k]; s_cam[k] = cams.cam[k]; }
+    }
+    __syncthreads();
+    lin = __ldg(tile_order + blockIdx.x);
+    uint32_t c = 0;
+    for (uint32_t k = 1; k < cams.count; ++k) if (lin >= s_cam[k].tile_base) c = k;
+    const RasterCamera &cam = s_cam[c];
+    fc.screenW = (float)cam.W; fc.screenH = (float)cam.H; fc.binsX = cam.binsX;
+    ntx = cam.ntx; rt = cam.rt; pitch = cam.pitch; surf = cam.surf; scene_depth = cam.depth; load_rt = cam.load;
+    tile_base = cam.tile_base; bin_base = cam.bin_base;
+  }
+  const bool surf_io = SURF || (CAMS && rt == nullptr);
+  const bool depth_test = SEL && scene_depth != nullptr;
   // FP32 blending into an RGBA16F target: drawing the objects one after the other stores (rounds to half) each object's result
   // and the next object starts from it.  Rounding is idempotent, so rounding at the next object's first candidate is exact.
   constexpr bool kRoundAtObject = MULTI && !FP16_ROP && OUT_FMT == GS_PIX_RGBA16F;
@@ -403,22 +466,22 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   constexpr uint32_t R = kBin / kTile;   // raster tiles per bin edge
   // launch order != raster order: CTA i takes tile order[i] (k_tile_order: most expensive first, by last frame's cost),
   // so the expensive tiles start early instead of forming the tail
-  const uint32_t lin = __ldg(tile_order + blockIdx.x);   // tile id in the whole image: ty * ntx + tx
-  const uint32_t ty = lin / ntx;
-  const uint32_t tx = lin - ty * ntx, brow = ty / R;
+  if (!CAMS) lin = __ldg(tile_order + blockIdx.x);   // tile id in the whole image: ty * ntx + tx (CAMS: in the run)
+  const uint32_t ty = (lin - tile_base) / ntx;
+  const uint32_t tx = (lin - tile_base) - ty * ntx, brow = ty / R;
   if (ty * kTile >= (uint32_t)fc.screenH) { if (threadIdx.x == 0) tile_cost[lin] = 0; return; }
   __shared__ uint32_t s_cost;
   if (threadIdx.x == 0) s_cost = 0;
   if constexpr (MULTI) {
     depth_mask = objs.depth_mask;
-    if (threadIdx.x == 0) {
+    if (!CAMS && threadIdx.x == 0) {
 #pragma unroll
       for (uint32_t k = 0; k < kRunObjects; ++k) { s_draw[k] = objs.draw[k]; s_zndc[k] = objs.zndc[k]; }
     }
-    __syncthreads();
+    if (!CAMS) __syncthreads();
   }
   // [start,end) of this tile's bin in the bin-sorted entry list (k_bin_ranges); R*R tiles share one list
-  const uint2 range = __ldg(bin_ranges + brow * fc.binsX + (tx / R));
+  const uint2 range = __ldg(bin_ranges + bin_base + brow * fc.binsX + (tx / R));
   const uint32_t bx = tx * kTile + (warp & 1) * 8, by = ty * kTile + (warp >> 1) * 4;
   const uint32_t px = bx + (lane & 7), py = by + (lane >> 3);
   const float pxc = (float)px + 0.5f, pyc = (float)py + 0.5f;
@@ -437,12 +500,12 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
     const uint8_t *row = rt + (size_t)out_row * pitch;
     if (OUT_FMT == GS_PIX_RGBA16F) {
       uint2 v;
-      if (SURF) surf2Dread(&v, surf, (int)(px * 8u), (int)out_row);
+      if (surf_io) surf2Dread(&v, surf, (int)(px * 8u), (int)out_row);
       else v = reinterpret_cast<const uint2 *>(row)[px];
       d0 = f16lo(v.x); d1 = f16hi(v.x); d2 = f16lo(v.y); d3 = f16hi(v.y);
     } else {
       float4 v;
-      if (SURF) surf2Dread(&v, surf, (int)(px * 16u), (int)out_row);
+      if (surf_io) surf2Dread(&v, surf, (int)(px * 16u), (int)out_row);
       else v = reinterpret_cast<const float4 *>(row)[px];
       d0 = v.x; d1 = v.y; d2 = v.z; d3 = v.w;
     }
@@ -582,10 +645,10 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
       uint2 o;
       o.x = f32tof16(d0) | (f32tof16(d1) << 16);
       o.y = f32tof16(d2) | (f32tof16(d3) << 16);
-      if (SURF) surf2Dwrite(o, surf, (int)(px * 8u), (int)out_row);
+      if (surf_io) surf2Dwrite(o, surf, (int)(px * 8u), (int)out_row);
       else reinterpret_cast<uint2 *>(row)[px] = o;
     } else {
-      if (SURF) surf2Dwrite(make_float4(d0, d1, d2, d3), surf, (int)(px * 16u), (int)out_row);
+      if (surf_io) surf2Dwrite(make_float4(d0, d1, d2, d3), surf, (int)(px * 16u), (int)out_row);
       else reinterpret_cast<float4 *>(row)[px] = make_float4(d0, d1, d2, d3);
     }
   }
@@ -617,7 +680,7 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const Draw
   // a run's raster reads each object's records and quad depths from `objs`, one object's from the draw / zndc arguments
 #define GS_RASTER_ARGS(OBJS)                                                                                                     \
   <<<grid, 256, 0, s>>>(fc, part, objs.draw[0], ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, \
-                        packed, load, stats, objs.zndc[0], scene_depth, OBJS)
+                        packed, load, stats, objs.zndc[0], scene_depth, OBJS, NoRasterObjects{})
 #define GS_LAUNCH_RASTER(ROP, FMT, SURF)                                                                                        \
   do {                                                                                                                         \
     if (run && objs.extras) k_raster<ROP, FMT, false, true, SURF, true> GS_RASTER_ARGS(objs);                                   \
@@ -639,6 +702,33 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const Draw
 #undef GS_LAUNCH_RASTER_TARGET
 #undef GS_LAUNCH_RASTER
 #undef GS_RASTER_ARGS
+}
+
+void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, uint32_t bins, uint32_t tiles, uint32_t blend_mode,
+                           uint32_t rt_format, const BinScratch &bs, cudaStream_t s) {
+  const Partition whole{0, 0, 1, 0, 0, 0};
+  // without a partition a tile's id is its launch-order id: ntx = tiles puts all of them in row 0
+  k_tile_order<<<1, 1024, 0, s>>>(bs.tile_cost, tiles, tiles, whole, bs.tile_order);
+  uint2 *ranges = reinterpret_cast<uint2 *>(bs.bin_ranges);
+  k_bin_ranges<<<(bins + 7) / 8, 256, 0, s>>>(bs.tile_keys, bs.entry_count, bins, ranges);
+  FrameConsts fc;   // screen size and bins come from each tile's camera
+  memset(&fc, 0, sizeof(fc));
+  const bool rop = blend_mode == GS_BLEND_FP16_ROP;
+#define GS_RASTER_CAMS(ROP, FMT)                                                                                                \
+  do {                                                                                                                         \
+    if (objs.extras)                                                                                                           \
+      k_raster<ROP, FMT, false, true, false, true, true><<<tiles, 256, 0, s>>>(fc, whole, nullptr, ranges, bs.tile_vals,        \
+          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, 0, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);                      \
+    else                                                                                                                       \
+      k_raster<ROP, FMT, false, false, false, true, true><<<tiles, 256, 0, s>>>(fc, whole, nullptr, ranges, bs.tile_vals,       \
+          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, 0, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);                      \
+  } while (0)
+  if (rt_format == GS_PIX_RGBA16F) {
+    if (rop) GS_RASTER_CAMS(true, GS_PIX_RGBA16F); else GS_RASTER_CAMS(false, GS_PIX_RGBA16F);
+  } else {
+    if (rop) GS_RASTER_CAMS(true, GS_PIX_RGBA32F); else GS_RASTER_CAMS(false, GS_PIX_RGBA32F);
+  }
+#undef GS_RASTER_CAMS
 }
 
 uint32_t partition_own_bin_rows(const GsRenderOptions &opt, uint32_t binsY) { return make_partition(opt).own_rows_below(binsY); }

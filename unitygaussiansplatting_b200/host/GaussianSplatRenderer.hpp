@@ -120,6 +120,72 @@ class GaussianSplatRenderer {
     return renderers[0]->ok(gs_frame_objects(renderers[0]->m_Ctx, (uint32_t)renderers.size(), assets.data(), fps.data(), doSort.data(),
                                              &opt, rt, cameraTarget));
   }
+  // The camera loop of GaussianSplatRenderSystem (OnPreCullCamera, :187-211): SortAndRenderSplatsMulti for cams[c] into rts[c] /
+  // cameraTargets[c] (either may be nullptr, not both), one camera after the other.  Every renderer is gathered per camera
+  // (GatherSplatsForCamera, :73-105) and its frame counter advances once per camera (:120-122).  All renderers share one
+  // context.  When they also share their options (GS_FLAG_LOAD_RT aside) and none asks for GS_FLAG_ASYNC_READBACK, this is one
+  // gs_frame_cameras call; otherwise it is that loop, SortAndRenderSplatsMulti per camera, as the Python mirror does.  A
+  // renderer listed twice or a camera without any image returns false before any frame counter moves; what only the library
+  // checks (screen and image sizes) returns false after they moved, as SortAndRenderSplatsMulti does.
+  static bool SortAndRenderSplatsCameras(const std::vector<CameraState> &cams, const std::vector<GaussianSplatRenderer *> &renderers,
+                                         const std::vector<GsImage *> &rts, const std::vector<GsImage *> &cameraTargets) {
+    if (rts.size() != cams.size() || cameraTargets.size() != cams.size()) return false;
+    if (renderers.empty()) return true;
+    for (const GaussianSplatRenderer *r : renderers)   // checked before any renderer's frame counter moves
+      if (!r || !r->HasValidRenderSetup() || r->m_Ctx != renderers[0]->m_Ctx) return false;
+    {
+      std::vector<const GaussianSplatRenderer *> sorted(renderers.begin(), renderers.end());
+      std::sort(sorted.begin(), sorted.end());
+      if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) return false;
+    }
+    for (size_t c = 0; c < cams.size(); ++c)
+      if (!rts[c] && !cameraTargets[c]) return false;
+    auto same = [](const GsRenderOptions &a, const GsRenderOptions &b) {
+      return a.blend_mode == b.blend_mode && a.band_packed == b.band_packed && a.partition_index == b.partition_index &&
+             a.partition_count == b.partition_count && a.band_rows == b.band_rows && a.row_begin == b.row_begin && a.row_end == b.row_end &&
+             ((a.flags ^ b.flags) & ~(uint32_t)GS_FLAG_LOAD_RT) == 0 && !(a.flags & GS_FLAG_ASYNC_READBACK);
+    };
+    bool oneCall = true;
+    for (const GaussianSplatRenderer *r : renderers) oneCall = oneCall && same(r->options, renderers[0]->options);
+    if (!oneCall) {
+      for (size_t c = 0; c < cams.size(); ++c)
+        if (!SortAndRenderSplatsMulti(cams[c], renderers, rts[c], cameraTargets[c])) return false;
+      return true;
+    }
+    std::vector<uint32_t> counts;
+    std::vector<GsAsset *> assets;
+    std::vector<GsFrameParams> fps;
+    std::vector<int32_t> doSort;
+    std::vector<GsImage *> camRts, camTargets;
+    GaussianSplatRenderer *first = nullptr;
+    for (size_t c = 0; c < cams.size(); ++c) {
+      const CameraState &cam = cams[c];
+      auto depth = [&](const GaussianSplatRenderer *r) {   // camera-space z of the object's position, +z forward
+        const float *v = cam.worldToCameraMatrix.m, *p = r->localToWorldMatrix.m + 12;
+        return -(v[2] * p[0] + v[6] * p[1] + v[10] * p[2] + v[14]);
+      };
+      std::vector<GaussianSplatRenderer *> order = renderers;
+      std::stable_sort(order.begin(), order.end(), [&](const GaussianSplatRenderer *a, const GaussianSplatRenderer *b) {
+        if (a->m_RenderOrder != b->m_RenderOrder) return a->m_RenderOrder > b->m_RenderOrder;
+        return depth(a) < depth(b);
+      });
+      if (!first) first = order[0];
+      counts.push_back((uint32_t)order.size());
+      camRts.push_back(rts[c]);
+      camTargets.push_back(cameraTargets[c]);
+      for (GaussianSplatRenderer *r : order) {
+        assets.push_back(r->m_Asset);
+        fps.push_back(r->params(cam));
+        doSort.push_back((r->m_FrameCounter % (r->m_SortNthFrame > 0 ? r->m_SortNthFrame : 1)) == 0);   // :120-121
+        ++r->m_FrameCounter;
+      }
+    }
+    if (counts.empty()) return true;   // no camera
+    GsRenderOptions opt = first->options;
+    opt.flags &= ~(uint32_t)GS_FLAG_LOAD_RT;
+    return first->ok(gs_frame_cameras(first->m_Ctx, (uint32_t)counts.size(), counts.data(), assets.data(), fps.data(), doSort.data(), &opt,
+                                      camRts.data(), camTargets.data()));
+  }
   bool Sync() { return ok(gs_sync(m_Ctx)); }
   // EditExportData, R/GaussianSplatRenderer.cs:936-958: n x 62 floats (the .ply attribute record), cut splats marked by nor = 1
   bool EditExportData(float *dstRecords, bool bakeTransform = false) {

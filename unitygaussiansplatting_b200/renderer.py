@@ -11,6 +11,7 @@ the hot path; everything it does is a call into libgsplat_b200.so (there is no C
   composite DrawProcedural            (:206)   Composite(rt, target)         -> gs_composite
   SortAndRenderSplats(cam, cmb)       (:108)   SortAndRenderSplats(cam, ...) -> gs_frame
   (several objects of one camera)              SortAndRenderSplatsMulti(...) -> gs_frame_objects
+  camera loop, OnPreCullCamera        (:187)   SortAndRenderCameras(...)     -> gs_frame_cameras
   OnDisable / DisposeResourcesForAsset(:533)   Dispose()
 """
 from __future__ import annotations
@@ -434,6 +435,61 @@ def SortAndRenderSplatsMulti(renderers, cam: Camera, rt, camera_target=None):
     if camera_target is not None:
         active[0].Composite(rt, camera_target)
     return active
+
+
+def cameras_in_one_call(actives) -> bool:
+    """Whether gs_frame_cameras can draw these cameras (each a non-empty list of active renderers in draw order): every list
+    passes draws_in_one_call, all on one context with one blend mode, and nobody asks for asynchronous read-back."""
+    r0 = actives[0][0]
+    return all(draws_in_one_call(a) and a[0].context is r0.context and a[0].blend_mode == r0.blend_mode and not a[0].async_readback
+               for a in actives)
+
+
+def SortAndRenderCameras(renderers, cams, rts, camera_targets=None):
+    """The camera loop of GaussianSplatRenderSystem (R/GaussianSplatRenderer.cs:187-211): SortAndRenderSplatsMulti for each
+    camera in turn -- GatherSplatsForCamera per camera, each renderer's m_FrameCounter advanced once per camera that draws it
+    -- in one gs_frame_cameras call when cameras_in_one_call holds for the cameras that draw something, else camera by camera.
+    rts[c] / camera_targets[c] may be None (not both for a camera that draws).  Returns each camera's active renderers."""
+    camera_targets = camera_targets if camera_targets is not None else [None] * len(cams)
+    actives = [GatherSplatsForCamera(renderers, cam) for cam in cams]
+    drawn = [c for c, a in enumerate(actives) if a]
+    if not drawn:
+        return actives
+    if cameras_in_one_call([actives[c] for c in drawn]):
+        _frame_cameras([actives[c] for c in drawn], [cams[c] for c in drawn], [rts[c] for c in drawn],
+                       [camera_targets[c] for c in drawn])
+        return actives
+    for c in drawn:
+        SortAndRenderSplatsMulti(renderers, cams[c], rts[c], camera_targets[c])
+    return actives
+
+
+def _frame_cameras(actives, cams, rts, camera_targets):
+    n = sum(len(a) for a in actives)
+    fps = (N.GsFrameParams * n)()
+    assets = (C.c_void_p * n)()
+    do_sort = (C.c_int32 * n)()
+    counts = (C.c_uint32 * len(cams))(*[len(a) for a in actives])
+    keep = []
+    i = 0
+    for active, cam in zip(actives, cams):
+        for r in active:
+            do_sort[i] = 1 if (r.m_FrameCounter % max(1, int(r.m_SortNthFrame)) == 0) else 0
+            r.m_FrameCounter += 1
+            fps[i], k = make_frame_params(cam, r.localToWorldMatrix, r.m_SplatScale, r.m_OpacityScale, r.m_SHOrder, r.m_SHOnly,
+                                          r.m_Cutouts, r.m_DeletedBits, r.splatCount, r.m_SelectedBits, r.sceneDepth)
+            keep.append(k)
+            assets[i] = r._asset.value if isinstance(r._asset, C.c_void_p) else r._asset
+            i += 1
+    opt = actives[0][0]._options()
+    opt.flags &= ~N.GS_FLAG_LOAD_RT
+    images = [(_image(rt, cam.pixelWidth, cam.pixelHeight) if rt is not None else None,
+               _image(tg, cam.pixelWidth, cam.pixelHeight) if tg is not None else None) for cam, rt, tg in zip(cams, rts, camera_targets)]
+    a = (C.POINTER(N.GsImage) * len(cams))(*[C.pointer(x) if x is not None else C.POINTER(N.GsImage)() for x, _ in images])
+    b = (C.POINTER(N.GsImage) * len(cams))(*[C.pointer(y) if y is not None else C.POINTER(N.GsImage)() for _, y in images])
+    ctx = actives[0][0].context
+    N.check(ctx.handle, ctx._lib.gs_frame_cameras(ctx.handle, len(cams), counts, assets, fps, do_sort, C.byref(opt), a, b))
+    del keep
 
 
 def _frame_objects(active, cam: Camera, rt, camera_target):
