@@ -391,6 +391,27 @@ def test_large_camera_between_small_ones(g, ctx, ca):
         tw.dispose()
 
 
+def test_camera_of_seventeen_objects_between_small_ones(g, ctx, ca):
+    """The middle camera cannot join a run: it is drawn as two runs, the second loading the first's image, between two runs of
+    one small camera each."""
+    assets = [g.synthetic_asset(g.SCENE_CLUSTERED, 3000 + 250 * i, 0xCA3E1000 + i, ("Medium", "VeryHigh")[i % 2]) for i in range(17)]
+
+    def setup(i, r):
+        r.localToWorldMatrix = g_trs(position=(0.7 * (i % 6) - 1.75, 0.6 * (i // 6) - 0.6, 0.3 * (i % 2)), scale=(0.5, 0.5, 0.5))
+        r.m_SortNthFrame = (1, 2)[i % 2]
+
+    tw = Twins(g, ctx, assets, setup)
+    try:
+        for f, kind in enumerate(["host", "device", "array"]):
+            cams = [orbit(g, f, 97, 61), orbit(g, f, 320, 200, phase=0.3), orbit(g, f, 256, 256, phase=0.6)]
+            idx = tw.gathered(g, [[0, 1], list(range(17)), [2, 16]], cams)
+            assert len(idx[1]) == 17
+            assert compare(g, ctx, ca, tw, idx, cams, f % 2, np.float16, ["device", kind, "host"], [None, "device", None],
+                           "frame %d" % f) > 0
+    finally:
+        tw.dispose()
+
+
 def test_own_depth_buffer_per_camera(g, ctx, ca):
     import torch
     tw = Twins(g, ctx, _mixed_assets(g, 3), _setup)
@@ -484,6 +505,40 @@ def test_overflow_reported_then_next_call_fits(g):
         assert call_cameras(g, ctx, [[rs], [rs]], cams, 0, host, [None, None], check=False) == 0
         assert all(h.any() for h in host)
         assert ctx._lib.gs_sync(ctx.handle) == 0
+    finally:
+        rh.Dispose()
+        rs.Dispose()
+        ctx.close()
+
+
+@pytest.mark.parametrize("host", [False, True])
+def test_overflow_kept_across_a_growing_camera(g, host):
+    """A truncated run of two cameras, then a camera above 8160 px (129 bin rows, every splat in each) whose own list grows and
+    fits: the call still reports the truncation, and the next call that fits reports none."""
+    import torch
+    ctx = g.GaussianSplatContext(0)   # a fresh context: its bin list has the smallest capacity (4 Mi entries)
+    rng = np.random.default_rng(12)
+    n = 40000   # 8 n < 4 Mi; on the tall camera n x 129 bins > 4 Mi
+    pos = np.c_[rng.uniform(-0.05, 0.05, (n, 2)), rng.uniform(-0.05, 0.05, n)].astype(np.float32)
+    huge = g.create_asset(splat_records(pos, (20.0, 20.0, 20.0), 0.02), "VeryHigh")   # every splat covers every bin
+    small = g.synthetic_asset(g.SCENE_CLUSTERED, 6000, 0xCA3E0F31, "Medium")
+    rh, rs = g.GaussianSplatRenderer(huge, ctx), g.GaussianSplatRenderer(small, ctx)
+    try:
+        cams = [camera(g, 1024, 1024), camera(g, 1024, 1024, pos=(0.064, 0.5, -6.0)), camera(g, 64, 8200)]
+        if host:
+            rts = [np.zeros((c.pixelHeight, c.pixelWidth, 4), np.float16) for c in cams]
+        else:
+            rts = [torch.zeros((c.pixelHeight, c.pixelWidth, 4), dtype=torch.float16, device="cuda") for c in cams]
+        rc = call_cameras(g, ctx, [[rh], [rh], [rh]], cams, 0, rts, [None] * 3, check=False)
+        if host:
+            assert rc == OOM
+        else:
+            assert rc == 0 and ctx._lib.gs_sync(ctx.handle) == OOM
+        assert call_cameras(g, ctx, [[rs], [rs], [rh]], cams, 0, rts, [None] * 3, check=False) == 0
+        assert ctx._lib.gs_sync(ctx.handle) == 0
+        if host:
+            assert ctx.stage_times().tile_entries > 4 << 20, "the tall camera's list must outgrow 4 Mi entries"
+            assert all(r.any() for r in rts)
     finally:
         rh.Dispose()
         rs.Dispose()

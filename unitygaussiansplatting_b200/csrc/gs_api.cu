@@ -405,32 +405,14 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
   return GS_OK;
 }
 
-// raster-tile cost history (launch order); invalidated when the tile grid changes
-static int ensure_raster_tiles(GsContext *ctx, const FrameConsts &fc) {
-  // per-tile state is indexed by the tile's id in the whole image, whatever part of it this context composites
-  const uint32_t rtiles = (((uint32_t)fc.screenW + kTile - 1) / kTile) * fc.binsY * (kBin / kTile);
-  if (rtiles > ctx->raster_tiles_cap) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(ctx->bin.tile_cost); cudaFree(ctx->bin.tile_order);
-    ctx->bin.tile_cost = ctx->bin.tile_order = nullptr;
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.tile_cost, (size_t)rtiles * 4));
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.tile_order, (size_t)rtiles * 4));
-    ctx->raster_tiles_cap = rtiles;
-    ctx->raster_tiles_cur = 0;
-  }
-  if (rtiles != ctx->raster_tiles_cur) {
-    GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->bin.tile_cost, 0, (size_t)rtiles * 4, ctx->stream));
-    ctx->raster_tiles_cur = rtiles;
-  }
-  return GS_OK;
-}
-
-// The tile-cost history of a camera run of gs_frame_cameras, in *cost: one per camera layout ((raster tiles per row, rows) of
-// each camera of the run), kept in cams_tile_cost apart from the single-grid history above, so that the runs of one call and
-// the single-camera draws between calls do not reset each other's.  At most kCameraLayouts layouts are kept; one more starts
-// the cache afresh.  The launch-order scratch bin.tile_order is shared with the single-grid draws.
+// The raster-tile cost history (launch order) of a draw of `tiles` tiles, in *cost.  layout == nullptr: the single-grid history
+// of gs_frame, gs_render, the group path and the one-camera runs, indexed by the tile's id in the whole image and reset when
+// the tile count changes.  Otherwise a run of several cameras, whose layout ((raster tiles per row, rows) of each camera) keeps
+// its own history in cams_tile_cost, so that the runs of one call and the single-grid draws between calls do not reset each
+// other's.  At most kCameraLayouts layouts are kept; one more starts that cache afresh.  The launch-order scratch
+// bin.tile_order serves both.
 constexpr size_t kCameraLayouts = 16;
-static int camera_tile_history(GsContext *ctx, uint32_t tiles, const std::vector<uint32_t> &layout, uint32_t **cost) {
+static int tile_history(GsContext *ctx, uint32_t tiles, const std::vector<uint32_t> *layout, uint32_t **cost) {
   if (tiles > ctx->raster_tiles_cap) {
     cudaStreamSynchronize(ctx->stream);
     cudaFree(ctx->bin.tile_cost); cudaFree(ctx->bin.tile_order);
@@ -440,8 +422,16 @@ static int camera_tile_history(GsContext *ctx, uint32_t tiles, const std::vector
     ctx->raster_tiles_cap = tiles;
     ctx->raster_tiles_cur = 0;
   }
+  if (!layout) {
+    if (tiles != ctx->raster_tiles_cur) {
+      GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->bin.tile_cost, 0, (size_t)tiles * 4, ctx->stream));
+      ctx->raster_tiles_cur = tiles;
+    }
+    *cost = ctx->bin.tile_cost;
+    return GS_OK;
+  }
   for (size_t i = 0; i < ctx->cams_layouts.size(); ++i)
-    if (ctx->cams_layouts[i] == layout) { *cost = ctx->cams_tile_cost + ctx->cams_layout_base[i]; return GS_OK; }
+    if (ctx->cams_layouts[i] == *layout) { *cost = ctx->cams_tile_cost + ctx->cams_layout_base[i]; return GS_OK; }
   if (ctx->cams_layouts.size() >= kCameraLayouts) { ctx->cams_layouts.clear(); ctx->cams_layout_base.clear(); ctx->cams_cost_used = 0; }
   const size_t need = ctx->cams_cost_used + tiles;
   if (need > ctx->cams_cost_cap) {   // grown with the histories kept
@@ -458,61 +448,47 @@ static int camera_tile_history(GsContext *ctx, uint32_t tiles, const std::vector
     ctx->cams_cost_cap = cap;
   }
   GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->cams_tile_cost + ctx->cams_cost_used, 0, (size_t)tiles * 4, ctx->stream));
-  ctx->cams_layouts.push_back(layout);
+  ctx->cams_layouts.push_back(*layout);
   ctx->cams_layout_base.push_back(ctx->cams_cost_used);
   *cost = ctx->cams_tile_cost + ctx->cams_cost_used;
   ctx->cams_cost_used = need;
   return GS_OK;
 }
 
-int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *const *as, const GsFrameParams *fps,
-            uint32_t count, bool first, void *d_rt, uint32_t pitch, uint32_t fmt, cudaSurfaceObject_t surf, cudaEvent_t bin_done) {
+int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *as, const GsFrameParams *fp, bool first,
+            void *d_rt, uint32_t pitch, uint32_t fmt, cudaSurfaceObject_t surf, cudaEvent_t bin_done) {
   GsNvtxRange nvtx("GaussianSplat.Draw");
-  DrawObjects objs;
-  memset(&objs, 0, sizeof(objs));
-  objs.count = count;
-  const GsFrameParams *depth_fp = &fps[0];   // every object that binds a scene depth buffer binds this one
-  uint64_t total = 0;
-  for (uint32_t k = 0; k < count; ++k) {
-    const GsAsset *a = as[k];
-    const GsFrameParams &f = fps[k];
-    total += a->av.n;
-    objs.n[k] = a->av.n; objs.order[k] = a->order; objs.rect[k] = a->rect; objs.block_bits[k] = a->block_bits; objs.draw[k] = a->draw;
-    if (f.scene_depth) {
-      objs.zndc[k] = a->zndc;
-      objs.depth_mask |= 1u << k;
-      if (!depth_fp->scene_depth) depth_fp = &f;
-    }
-    objs.extras |= f.selected_bits != nullptr || f.scene_depth != nullptr;
-  }
-  const uint32_t n = (uint32_t)std::min<uint64_t>(total, 0xFFFFFFFFu);
+  const uint32_t n = as->av.n;
   int rc = ensure_bin_scratch(ctx, n, fc.binsX * fc.binsY, 0);
   if (rc) return rc;
-  if ((rc = ensure_raster_tiles(ctx, fc))) return rc;
+  uint32_t *tile_cost = nullptr;
+  const uint32_t rtiles = (((uint32_t)fc.screenW + kTile - 1) / kTile) * fc.binsY * (kBin / kTile);   // of the whole image
+  if ((rc = tile_history(ctx, rtiles, nullptr, &tile_cost))) return rc;
   const float *depth = nullptr;
-  if ((rc = bind_depth(ctx, depth_fp, &depth))) return rc;
+  if ((rc = bind_depth(ctx, fp, &depth))) return rc;
   BinScratch lists;
   int bin_launches = 0, more = 0;
-  GS_CUDA_TRY(ctx, launch_binning(fc, opt, objs, first, ctx->bin, ctx->sort, ctx->stream, &lists, &bin_launches));
+  GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order, as->rect, as->block_bits, n, first, ctx->bin, ctx->sort, ctx->stream, &lists,
+                                  &bin_launches));
   bool again = false;
   if ((rc = grow_bin_list(ctx, fc, n, &again))) return rc;
   if (again) {
     // the grown list fits: the flag this draw set is cleared again, unless an earlier draw of the call left its list truncated
-    // (every draw of a call has the same screen, so every one was checked here)
     const bool clear = first || !ctx->bin_overflow;
-    GS_CUDA_TRY(ctx, launch_binning(fc, opt, objs, clear, ctx->bin, ctx->sort, ctx->stream, &lists, &more));
+    GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order, as->rect, as->block_bits, n, clear, ctx->bin, ctx->sort, ctx->stream, &lists,
+                                    &more));
     bin_launches += more;
     ctx->bin_overflow = !clear;
   }
   rec(ctx, EV_BIN1);
   if (bin_done) cudaEventRecord(bin_done, ctx->stream);
-  launch_raster(fc, opt, objs, lists, d_rt, pitch, fmt, surf, ctx->stream, depth);
+  launch_raster(fc, opt, as->draw, fp->scene_depth ? as->zndc : nullptr, fp->selected_bits != nullptr || fp->scene_depth != nullptr,
+                lists, d_rt, pitch, fmt, surf, ctx->stream, depth);
   rec(ctx, EV_RASTER1);
-  ctx->launches += bin_launches + 3;  // per object look-back clear + bin_emit, 1-2 sort passes; bin_ranges, tile_order, raster
+  ctx->launches += bin_launches + 3;  // look-back clear + bin_emit, 1-2 sort passes; bin_ranges, tile_order, raster
   GS_CUDA_TRY(ctx, cudaGetLastError());
   return GS_OK;
 }
-
 
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch) {
   if (!im || !im->data) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image is null");
@@ -820,17 +796,17 @@ int gs_render(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRend
   if (fp->scene_depth && !as->zndc_valid) return fail(ctx, GS_ERR_NOT_READY, "a scene depth buffer needs the quad depths: run gs_calc_view with scene_depth set");
   for (int e = EV_BIN1; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
   rec(ctx, EV_VIEW1);
-  if (rt->memory == GS_MEM_DEVICE) return do_draw(ctx, fc, opt, &as, fp, 1, true, rt->data, pitch, rt->format);
+  if (rt->memory == GS_MEM_DEVICE) return do_draw(ctx, fc, opt, as, fp, true, rt->data, pitch, rt->format);
   if (rt->memory == GS_MEM_ARRAY) {
     CallSurfaces surfs(ctx);
     cudaSurfaceObject_t so = 0;
     if ((rc = surfs.make(rt, &so))) return rc;
-    return do_draw(ctx, fc, opt, &as, fp, 1, true, nullptr, 0, rt->format, so);
+    return do_draw(ctx, fc, opt, as, fp, true, nullptr, 0, rt->format, so);
   }
   const uint32_t tight = W * pix_bytes(rt->format);
   if ((rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)tight * H))) return rc;
   if ((rc = init_staging(ctx, opt, ctx->rt_scratch, tight, W, H, rt->format, rt, pitch))) return rc;
-  if ((rc = do_draw(ctx, fc, opt, &as, fp, 1, true, ctx->rt_scratch, tight, rt->format))) return rc;
+  if ((rc = do_draw(ctx, fc, opt, as, fp, true, ctx->rt_scratch, tight, rt->format))) return rc;
   GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, pitch, ctx->rt_scratch, tight, tight, H, cudaMemcpyDeviceToHost, ctx->stream));
   return check_bin_overflow(ctx);
 }
@@ -898,9 +874,10 @@ struct FrameImage {
   int slot = 0;
 };
 
-// what gs_frame and gs_frame_objects do between their view-calcs and their draw; rt (when given) has passed image_ok
+// what a frame does between its view-calcs and its draw; rt (when given) has passed image_ok.  staging (optional): where a
+// staging image goes instead of rt_scratch (one slice per camera of a run of several cameras)
 static int begin_frame_image(GsContext *ctx, CallSurfaces &surfs, const GsRenderOptions &opt, GsImage *rt, uint32_t rt_pitch,
-                             uint32_t rt_fmt, const GsImage *tgt, uint32_t W, uint32_t H, FrameImage *fi) {
+                             uint32_t rt_fmt, const GsImage *tgt, uint32_t W, uint32_t H, FrameImage *fi, void *staging = nullptr) {
   int rc = GS_OK;
   const bool rt_dev = rt && rt->memory == GS_MEM_DEVICE, rt_arr = rt && rt->memory == GS_MEM_ARRAY, rt_host = rt && rt->memory == GS_MEM_HOST;
   fi->async_rb = rt_host && !tgt && (opt.flags & GS_FLAG_ASYNC_READBACK) != 0;
@@ -920,8 +897,8 @@ static int begin_frame_image(GsContext *ctx, CallSurfaces &surfs, const GsRender
     if ((rc = init_staging(ctx, opt, fi->d_rt, fi->pitch, W, H, rt_fmt, rt, rt_pitch))) return rc;
   } else {
     fi->pitch = W * pix_bytes(rt_fmt);
-    if ((rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)fi->pitch * H))) return rc;
-    fi->d_rt = ctx->rt_scratch;
+    if (!staging && (rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)fi->pitch * H))) return rc;
+    fi->d_rt = staging ? staging : ctx->rt_scratch;
     if ((rc = init_staging(ctx, opt, fi->d_rt, fi->pitch, W, H, rt_fmt, rt, rt_pitch))) return rc;
   }
   return GS_OK;
@@ -955,12 +932,20 @@ static int end_frame_image(GsContext *ctx, CallSurfaces &surfs, GsImage *rt, uin
   return GS_OK;
 }
 
+// One camera of gs_frame_objects / gs_frame_cameras: its objects' arguments assets / fps / do_sort_flags [off, off + K), and
+// its images.
+struct CameraArgs {
+  uint32_t off, K, W, H, rt_pitch, rt_fmt;
+  std::vector<FrameConsts> fcs;
+  GsImage *rt, *tgt;
+  FrameImage fi;     // set up by the camera's first run
+};
+
 // What gs_frame_objects checks of one camera's arguments: the objects, the options (validated into *opt) and the images.
 // Out: the objects' uniforms, the screen size, and the render target's pitch and pixel format (RGBA16F without one).
-static int check_camera(GsContext *ctx, uint32_t K, GsAsset *const *assets, const GsFrameParams *fps, GsRenderOptions *opt,
-                        const GsImage *rt, const GsImage *tgt, std::vector<FrameConsts> *fcs, uint32_t *W, uint32_t *H,
-                        uint32_t *rt_pitch, uint32_t *rt_fmt) {
+static int check_camera(GsContext *ctx, GsAsset *const *assets, const GsFrameParams *fps, GsRenderOptions *opt, CameraArgs *a) {
   int rc = GS_OK;
+  const uint32_t K = a->K;
   for (uint32_t k = 0; k < K; ++k) {
     if (!assets[k]) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null asset");
     if ((rc = check_params(ctx, assets[k], &fps[k]))) return rc;
@@ -973,178 +958,269 @@ static int check_camera(GsContext *ctx, uint32_t K, GsAsset *const *assets, cons
     if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
       return fail(ctx, GS_ERR_INVALID_ARGUMENT, "an asset is listed for two objects (its draw order would be sorted twice)");
   }
-  if (!rt && !tgt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_frame_objects needs rt and/or camera_target");
+  if (!a->rt && !a->tgt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_frame_objects needs rt and/or camera_target");
   if (opt->flags & GS_FLAG_LOAD_RT) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "GS_FLAG_LOAD_RT is not accepted: the call clears the target once itself");
   if (opt->partition_count > 1 || opt->partition_index || opt->row_begin || opt->row_end || opt->band_packed)
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_frame_objects draws the whole screen: no partition, row range or band packing");
-  fcs->resize(K);
-  for (uint32_t k = 0; k < K; ++k) (*fcs)[k] = make_frame_consts(&fps[k]);
-  if ((rc = check_options(ctx, (*fcs)[0], *opt))) return rc;
-  *W = (uint32_t)fps[0].screen_w; *H = (uint32_t)fps[0].screen_h;
+  a->fcs.resize(K);
+  for (uint32_t k = 0; k < K; ++k) a->fcs[k] = make_frame_consts(&fps[k]);
+  if ((rc = check_options(ctx, a->fcs[0], *opt))) return rc;
+  a->W = (uint32_t)fps[0].screen_w; a->H = (uint32_t)fps[0].screen_h;
   uint32_t tgt_pitch = 0;
-  *rt_pitch = 0; *rt_fmt = GS_PIX_RGBA16F;
-  if (rt) { if ((rc = image_ok(ctx, rt, *W, *H, rt_pitch))) return rc; *rt_fmt = rt->format; }
-  if (tgt && (rc = image_ok(ctx, tgt, *W, *H, &tgt_pitch))) return rc;
+  a->rt_pitch = 0; a->rt_fmt = GS_PIX_RGBA16F;
+  if (a->rt) { if ((rc = image_ok(ctx, a->rt, a->W, a->H, &a->rt_pitch))) return rc; a->rt_fmt = a->rt->format; }
+  if (a->tgt && (rc = image_ok(ctx, a->tgt, a->W, a->H, &tgt_pitch))) return rc;
   return GS_OK;
 }
 
-// gs_frame_objects' work for one camera whose arguments have passed check_camera and whose frame inputs are reserved: per
-// object the sort and the view-calc, then the runs into the image *fi (set up here).  first: the first draw of its public call.
-static int draw_objects(GsContext *ctx, CallSurfaces &surfs, uint32_t K, GsAsset *const *assets, const GsFrameParams *fps,
-                        const int32_t *do_sort_flags, const std::vector<FrameConsts> &fcs, const GsRenderOptions &opt, GsImage *rt,
-                        uint32_t rt_pitch, uint32_t rt_fmt, const GsImage *tgt, uint32_t W, uint32_t H, bool first, FrameImage *fi) {
-  int rc = GS_OK;
-  for (uint32_t k = 0; k < K; ++k) {
-    if (do_sort_flags[k] && (rc = do_sort(ctx, assets[k], fcs[k]))) return rc;
-    if ((rc = do_view(ctx, assets[k], &fps[k], fcs[k], true, opt, ctx->stream))) return rc;
-  }
-  if ((rc = begin_frame_image(ctx, surfs, opt, rt, rt_pitch, rt_fmt, tgt, W, H, fi))) return rc;
-  // Runs: consecutive objects drawn by one bin list and one raster -- at most kRunObjects, each with fewer than 2^kSlotShift
-  // splats (the slot tag), binding at most one scene depth buffer.  An object of more splats, and the only object of a
-  // one-object call, is a run of one.  The first run starts from a cleared target, each later one blends under it.
-  for (uint32_t k = 0; k < K;) {
-    const GsFrameParams *depth_fp = &fps[k];
-    uint32_t e = k;
-    for (; e < K && e - k < kRunObjects && assets[e]->av.n <= kLocalIdMask; ++e) {
-      const GsFrameParams &f = fps[e];
-      if (!f.scene_depth) continue;
-      if (!depth_fp->scene_depth) depth_fp = &f;
-      else if (f.scene_depth != depth_fp->scene_depth || f.scene_depth_on_device != depth_fp->scene_depth_on_device) break;
-    }
-    e = std::max(e, k + 1);
-    GsRenderOptions o = opt;
-    if (k) o.flags |= GS_FLAG_LOAD_RT;
-    if ((rc = do_draw(ctx, fcs[k], o, assets + k, fps + k, e - k, first && k == 0, fi->d_rt, fi->pitch, rt_fmt, fi->surf))) return rc;
-    k = e;
-  }
-  return GS_OK;
-}
-
-// ---- gs_frame_cameras ---------------------------------------------------------------------------------
-// A camera run holds whole cameras of at most kMaxRunScreen px per axis, kRunObjects (camera, object) pairs and kMaxRunBins
-// bins in all (the largest bin space the bin sort's digit plans cover).
+// ---- runs ---------------------------------------------------------------------------------------------
+// A run (see DrawCameras) is a list of camera segments: the camera's pairs [k0, k0 + K), and load = 1 where an earlier run of
+// the call drew the camera's first pairs.  A run holds at most kRunObjects pairs, each object of fewer than 2^kSlotShift splats
+// (the slot tag), at most one scene depth buffer per camera, whole cameras of at most kMaxRunScreen px per axis when it holds
+// several, and at most kMaxRunBins bins (the largest bin space the bin sort's digit plans cover).
 constexpr uint32_t kMaxRunScreen = 8160, kMaxRunBins = 65536;
-
-struct CameraArgs {
-  uint32_t off, K, W, H, rt_pitch, rt_fmt;
-  std::vector<FrameConsts> fcs;
-  GsImage *rt, *tgt;
+struct Segment {
+  uint32_t cam, k0, K, load;
 };
+using Run = std::vector<Segment>;
 
 static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-// Draws the cameras cams[0, count) as one camera run (see DrawCameras): pair by pair the sort, the view-calc and the bin
-// emit, then one bin sort, one raster over every camera's tiles, and per camera the host read-back and the composite.
-static int draw_camera_run(GsContext *ctx, CallSurfaces &surfs, const CameraArgs *cams, uint32_t count, GsAsset *const *assets,
-                           const GsFrameParams *fps, const int32_t *do_sort_flags, const GsRenderOptions &opt, bool first) {
-  GsNvtxRange nvtx("GaussianSplat.DrawCameras");
-  const uint32_t rt_fmt = cams[0].rt_fmt;
+// The end of the longest run of the objects [k, K) that starts at k: at most kRunObjects objects, each of fewer than
+// 2^kSlotShift splats, binding at most one scene depth buffer.
+static uint32_t run_end(GsAsset *const *assets, const GsFrameParams *fps, uint32_t k, uint32_t K) {
+  const GsFrameParams *depth = nullptr;
+  uint32_t e = k;
+  for (; e < K && e - k < kRunObjects && assets[e]->av.n <= kLocalIdMask; ++e) {
+    const GsFrameParams &f = fps[e];
+    if (!f.scene_depth) continue;
+    if (!depth) depth = &f;
+    else if (f.scene_depth != depth->scene_depth || f.scene_depth_on_device != depth->scene_depth_on_device) break;
+  }
+  return e;
+}
+
+// The call's cameras as runs, in order.  Consecutive whole cameras share a run while each fits it, the run's totals hold, they
+// have one pixel format, and no camera's image is another's render target (two cameras rasterizing into one image at once
+// would race, where the loop draws one after the other).  A camera alone is split into runs of run_end, each later one
+// loading what the earlier ones drew.
+static std::vector<Run> form_runs(const std::vector<CameraArgs> &cams, GsAsset *const *assets, const GsFrameParams *fps) {
+  auto whole = [&](uint32_t c) {
+    const CameraArgs &a = cams[c];
+    return a.W <= kMaxRunScreen && a.H <= kMaxRunScreen && run_end(assets + a.off, fps + a.off, 0, a.K) == a.K;
+  };
+  auto joins = [&](uint32_t c0, uint32_t c, uint32_t run_pairs, uint32_t run_bins) {
+    const CameraArgs &a = cams[c];
+    if (run_pairs + a.K > kRunObjects || run_bins + a.fcs[0].binsX * a.fcs[0].binsY > kMaxRunBins || a.rt_fmt != cams[c0].rt_fmt) return false;
+    for (uint32_t j = c0; j < c; ++j) {
+      const void *rj = cams[j].rt ? cams[j].rt->data : nullptr, *tj = cams[j].tgt ? cams[j].tgt->data : nullptr;
+      if (a.rt && (a.rt->data == rj || a.rt->data == tj)) return false;
+      if (a.tgt && a.tgt->data == rj) return false;
+    }
+    return true;
+  };
+  std::vector<Run> runs;
+  const uint32_t count = (uint32_t)cams.size();
+  for (uint32_t c = 0; c < count;) {
+    uint32_t e = c, run_pairs = 0, run_bins = 0;
+    while (e < count && whole(e) && (e == c || joins(c, e, run_pairs, run_bins))) {
+      run_pairs += cams[e].K;
+      run_bins += cams[e].fcs[0].binsX * cams[e].fcs[0].binsY;
+      ++e;
+    }
+    if (e - c >= 2) {
+      runs.emplace_back();
+      for (uint32_t j = c; j < e; ++j) runs.back().push_back({j, 0, cams[j].K, 0});
+      c = e;
+      continue;
+    }
+    const CameraArgs &a = cams[c];
+    for (uint32_t k = 0; k < a.K;) {
+      const uint32_t ke = std::max(run_end(assets + a.off, fps + a.off, k, a.K), k + 1);
+      runs.push_back({{c, k, ke - k, k ? 1u : 0u}});
+      k = ke;
+    }
+    ++c;
+  }
+  return runs;
+}
+
+// Draws one run.  Pair by pair the sort and the view-calc; a pair's bin entries are emitted before a later pair of the run
+// sorts or view-calculates the same asset, and otherwise after the last view-calc.  A run of one pair is then drawn by
+// do_draw; a longer one by one bin sort and one MULTI raster over every camera's tiles.  A run whose only camera has more than
+// kRuleBins bins on either axis grows its bin list as do_draw does.  Each camera's image is set up by its first run (a camera of
+// a run of several stages a host image in the run's scratch, every other camera in rt_scratch) and read back / composited
+// after its last.  first: the first draw of its public call (do_draw).
+static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs> &cams, const Run &run, GsAsset *const *assets,
+                    const GsFrameParams *fps, const int32_t *do_sort_flags, const GsRenderOptions &opt, bool first) {
+  GsNvtxRange nvtx("GaussianSplat.DrawRun");
+  std::vector<uint32_t> pair_at, seg_of;   // each pair's argument index and segment, in draw order
+  for (uint32_t i = 0; i < run.size(); ++i)
+    for (uint32_t k = run[i].k0; k < run[i].k0 + run[i].K; ++k) { pair_at.push_back(cams[run[i].cam].off + k); seg_of.push_back(i); }
+  const uint32_t count = (uint32_t)pair_at.size();
+  const bool multi = count > 1, cams_run = run.size() > 1;
   DrawCameras dc;
   memset(&dc, 0, sizeof(dc));
-  dc.count = count;
+  dc.count = (uint32_t)run.size();
   std::vector<uint32_t> layout;
-  uint32_t tiles = 0, bins = 0, pairs = 0;
+  uint32_t tiles = 0, bins = 0;
   uint64_t total = 0;
   size_t bytes = 0;
-  std::vector<size_t> slab_at, stage_at(count, 0), depth_at(count, 0);
-  std::vector<const GsFrameParams *> depth_fp(count, nullptr);
-  for (uint32_t i = 0; i < count; ++i) {
-    const CameraArgs &c = cams[i];
-    RasterCamera &rc = dc.cam[i];
-    rc.W = c.W; rc.H = c.H;
-    rc.binsX = c.fcs[0].binsX;
-    rc.ntx = (c.W + kTile - 1) / kTile;
+  std::vector<size_t> slab_at(count, 0), depth_at(run.size(), 0), stage_at(run.size(), 0);
+  std::vector<const GsFrameParams *> depth_fp(run.size(), nullptr);
+  for (uint32_t i = 0, q = 0; i < run.size(); ++i) {
+    const CameraArgs &c = cams[run[i].cam];
+    RasterCamera &r = dc.cam[i];
+    r.W = c.W; r.H = c.H;
+    r.binsX = c.fcs[0].binsX;
+    r.ntx = (c.W + kTile - 1) / kTile;
+    r.load = run[i].load;
     const uint32_t rows = c.fcs[0].binsY * (kBin / kTile);
-    rc.tile_base = tiles; rc.bin_base = bins;
-    tiles += rc.ntx * rows;
-    bins += rc.binsX * c.fcs[0].binsY;
-    layout.push_back(rc.ntx); layout.push_back(rows);
-    for (uint32_t k = 0; k < c.K; ++k) {
-      const GsAsset *as = assets[c.off + k];
-      const GsFrameParams &f = fps[c.off + k];
+    r.tile_base = tiles; r.bin_base = bins;
+    tiles += r.ntx * rows;
+    bins += r.binsX * c.fcs[0].binsY;
+    layout.push_back(r.ntx); layout.push_back(rows);
+    for (uint32_t k = 0; k < run[i].K; ++k, ++q) {
+      const GsAsset *as = assets[pair_at[q]];
+      const GsFrameParams &f = fps[pair_at[q]];
       total += as->av.n;
       if (f.scene_depth && !depth_fp[i]) depth_fp[i] = &f;
       // every appearance of an asset but its last in the run draws from a record slab: a later view-calc overwrites its own
       bool later = false;
-      for (uint32_t j = i; j < count && !later; ++j)
-        for (uint32_t m = (j == i ? k + 1 : 0); m < cams[j].K; ++m) later |= assets[cams[j].off + m] == as;
-      slab_at.push_back(later ? bytes + 1 : 0);   // 0: the asset's own buffers (offsets are stored + 1)
+      for (uint32_t m = q + 1; m < count; ++m) later |= assets[pair_at[m]] == as;
+      slab_at[q] = later ? bytes + 1 : 0;   // 0: the asset's own buffers (offsets are stored + 1)
       if (later) bytes += align256((size_t)as->av.n * 48) + (f.scene_depth ? align256((size_t)as->av.n * 4 + 16) : 0);
-      ++pairs;
     }
-    if (!c.rt || c.rt->memory == GS_MEM_HOST) { stage_at[i] = bytes; bytes += align256((size_t)c.W * pix_bytes(rt_fmt) * c.H); }
-    if (depth_fp[i] && !depth_fp[i]->scene_depth_on_device) { depth_at[i] = bytes; bytes += align256((size_t)c.W * c.H * 4); }
+    if (multi && depth_fp[i] && !depth_fp[i]->scene_depth_on_device) { depth_at[i] = bytes; bytes += align256((size_t)c.W * c.H * 4); }
+    if (cams_run && (!c.rt || c.rt->memory == GS_MEM_HOST)) { stage_at[i] = bytes; bytes += align256((size_t)c.W * pix_bytes(c.rt_fmt) * c.H); }
   }
   int rc = GS_OK;
   if (bytes && (rc = grow(ctx, &ctx->cams_scratch, &ctx->cams_bytes, bytes))) return rc;
-  if (!ctx->cams_ghist) GS_CUDA_TRY(ctx, cudaMalloc(&ctx->cams_ghist, 4 * 256 * sizeof(uint32_t)));
-  if ((rc = ensure_bin_scratch(ctx, (uint32_t)std::min<uint64_t>(total, 0xFFFFFFFFu), bins, 0))) return rc;
-  uint32_t *tile_cost = nullptr;
-  if ((rc = camera_tile_history(ctx, tiles, layout, &tile_cost))) return rc;
   uint8_t *scratch = static_cast<uint8_t *>(ctx->cams_scratch);
-  for (uint32_t i = 0; i < count; ++i) {
-    const CameraArgs &c = cams[i];
-    RasterCamera &r = dc.cam[i];
-    if (!c.rt || c.rt->memory == GS_MEM_HOST) { r.rt = scratch + stage_at[i]; r.pitch = c.W * pix_bytes(rt_fmt); }
-    else if (c.rt->memory == GS_MEM_DEVICE) { r.rt = static_cast<uint8_t *>(c.rt->data); r.pitch = c.rt_pitch; }
-    else if ((rc = surfs.make(c.rt, &r.surf))) return rc;
-    if (depth_fp[i] && depth_fp[i]->scene_depth_on_device) r.depth = depth_fp[i]->scene_depth;
-    else if (depth_fp[i]) {
-      r.depth = reinterpret_cast<const float *>(scratch + depth_at[i]);
-      GS_CUDA_TRY(ctx, cudaMemcpyAsync(scratch + depth_at[i], depth_fp[i]->scene_depth, (size_t)c.W * c.H * 4, cudaMemcpyHostToDevice, ctx->stream));
+  const uint32_t n = (uint32_t)std::min<uint64_t>(total, 0xFFFFFFFFu);
+  uint32_t *tile_cost = nullptr;
+  if (multi) {
+    if (!ctx->cams_ghist) GS_CUDA_TRY(ctx, cudaMalloc(&ctx->cams_ghist, 4 * 256 * sizeof(uint32_t)));
+    if ((rc = ensure_bin_scratch(ctx, n, bins, 0))) return rc;
+    if ((rc = tile_history(ctx, tiles, cams_run ? &layout : nullptr, &tile_cost))) return rc;
+    for (uint32_t i = 0; i < run.size(); ++i) {
+      if (depth_fp[i] && depth_fp[i]->scene_depth_on_device) dc.cam[i].depth = depth_fp[i]->scene_depth;
+      else if (depth_fp[i]) {
+        dc.cam[i].depth = reinterpret_cast<const float *>(scratch + depth_at[i]);
+        GS_CUDA_TRY(ctx, cudaMemcpyAsync(scratch + depth_at[i], depth_fp[i]->scene_depth, (size_t)dc.cam[i].W * dc.cam[i].H * 4,
+                                         cudaMemcpyHostToDevice, ctx->stream));
+      }
     }
+    launch_bin_list_begin(ctx->bin, ctx->cams_ghist, ctx->stream);
   }
 
   DrawObjects objs;
   memset(&objs, 0, sizeof(objs));
-  objs.count = pairs;
-  launch_bin_list_begin(ctx->bin, ctx->cams_ghist, ctx->stream);
-  uint32_t p = 0;
-  for (uint32_t i = 0; i < count; ++i) {
-    const CameraArgs &c = cams[i];
-    for (uint32_t k = 0; k < c.K; ++k, ++p) {
-      GsAsset *as = assets[c.off + k];
-      const GsFrameParams &f = fps[c.off + k];
-      float4 *draw = nullptr;
-      float *zndc = nullptr;
-      if (slab_at[p]) {
-        draw = reinterpret_cast<float4 *>(scratch + slab_at[p] - 1);
-        zndc = reinterpret_cast<float *>(scratch + slab_at[p] - 1 + align256((size_t)as->av.n * 48));
-      }
-      if (do_sort_flags[c.off + k] && (rc = do_sort(ctx, as, c.fcs[k]))) return rc;
-      if ((rc = do_view(ctx, as, &f, c.fcs[k], true, opt, ctx->stream, draw, zndc))) return rc;
-      // emitted before the next sort or view-calc of this asset replaces its order, rectangles and block bits
-      launch_bin_emit_pair(as->order, as->rect, as->block_bits, as->av.n, dc.cam[i].binsX, dc.cam[i].bin_base, p, first && p == 0, bins,
+  objs.count = count;
+  uint32_t emitted = 0;   // the pairs [emitted, p) are view-calculated and not yet emitted
+  auto emit_to = [&](uint32_t end, bool clear) {
+    for (; emitted < end; ++emitted) {
+      const GsAsset *as = assets[pair_at[emitted]];
+      const RasterCamera &r = dc.cam[seg_of[emitted]];
+      launch_bin_emit_pair(as->order, as->rect, as->block_bits, as->av.n, r.binsX, r.bin_base, emitted, clear && emitted == 0, bins,
                            ctx->bin, ctx->cams_ghist, ctx->stream);
       ctx->launches += 2;   // look-back clear, bin_emit
-      objs.n[p] = as->av.n;
-      objs.draw[p] = draw ? draw : as->draw;
-      if (f.scene_depth) {
-        objs.zndc[p] = draw ? zndc : as->zndc;
-        objs.depth_mask |= 1u << p;
-      }
-      objs.extras |= f.selected_bits != nullptr || f.scene_depth != nullptr;
     }
+  };
+  for (uint32_t p = 0; p < count; ++p) {
+    GsAsset *as = assets[pair_at[p]];
+    const GsFrameParams &f = fps[pair_at[p]];
+    const CameraArgs &c = cams[run[seg_of[p]].cam];
+    for (uint32_t q = emitted; q < p; ++q)
+      if (assets[pair_at[q]] == as) { emit_to(p, first); break; }
+    float4 *draw = nullptr;
+    float *zndc = nullptr;
+    if (slab_at[p]) {
+      draw = reinterpret_cast<float4 *>(scratch + slab_at[p] - 1);
+      zndc = reinterpret_cast<float *>(scratch + slab_at[p] - 1 + align256((size_t)as->av.n * 48));
+    }
+    if (do_sort_flags[pair_at[p]] && (rc = do_sort(ctx, as, c.fcs[pair_at[p] - c.off]))) return rc;
+    if ((rc = do_view(ctx, as, &f, c.fcs[pair_at[p] - c.off], true, opt, ctx->stream, draw, zndc))) return rc;
+    objs.draw[p] = draw ? draw : as->draw;
+    if (f.scene_depth) {
+      objs.zndc[p] = draw ? zndc : as->zndc;
+      objs.depth_mask |= 1u << p;
+    }
+    objs.extras |= f.selected_bits != nullptr || f.scene_depth != nullptr;
   }
-  SortScratch sc = ctx->sort;
-  sc.ghist = ctx->cams_ghist;
-  BinScratch lists;
-  int sort_launches = 0;
-  GS_CUDA_TRY(ctx, launch_bin_list_sort(bins, ctx->bin, sc, ctx->stream, &lists, &sort_launches));
-  lists.tile_cost = tile_cost;
-  rec(ctx, EV_BIN1);
-  launch_raster_cameras(objs, dc, bins, tiles, opt.blend_mode, rt_fmt, lists, ctx->stream);
-  rec(ctx, EV_RASTER1);
-  ctx->launches += sort_launches + 3;   // bin sort passes; bin_ranges, tile_order, raster
-  GS_CUDA_TRY(ctx, cudaGetLastError());
-  for (uint32_t i = 0; i < count; ++i) {
-    const CameraArgs &c = cams[i];
-    const RasterCamera &r = dc.cam[i];
-    if (c.rt && c.rt->memory == GS_MEM_HOST)
-      GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(c.rt->data, c.rt_pitch, r.rt, r.pitch, (size_t)c.W * pix_bytes(rt_fmt), c.H, cudaMemcpyDeviceToHost, ctx->stream));
-    if (c.tgt && (rc = composite_impl(ctx, surfs, r.rt, r.pitch, r.surf, rt_fmt, c.tgt, c.W, c.H, ctx->stream))) return rc;
+  for (uint32_t i = 0; i < run.size(); ++i) {
+    CameraArgs &c = cams[run[i].cam];
+    if (!run[i].load && (rc = begin_frame_image(ctx, surfs, opt, c.rt, c.rt_pitch, c.rt_fmt, c.tgt, c.W, c.H, &c.fi,
+                                                cams_run ? scratch + stage_at[i] : nullptr)))
+      return rc;
+    dc.cam[i].rt = static_cast<uint8_t *>(c.fi.d_rt); dc.cam[i].pitch = c.fi.pitch; dc.cam[i].surf = c.fi.surf;
+  }
+  if (!multi) {
+    const CameraArgs &c = cams[run[0].cam];
+    GsRenderOptions o = opt;
+    if (run[0].load) o.flags |= GS_FLAG_LOAD_RT;
+    if ((rc = do_draw(ctx, c.fcs[run[0].k0], o, assets[pair_at[0]], &fps[pair_at[0]], first, c.fi.d_rt, c.fi.pitch, c.rt_fmt, c.fi.surf)))
+      return rc;
+  } else {
+    emit_to(count, first);
+    BinScratch lists;
+    int sort_launches = 0, more = 0;
+    GS_CUDA_TRY(ctx, launch_bin_list_sort(bins, ctx->bin, ctx->sort, ctx->cams_ghist, ctx->stream, &lists, &sort_launches));
+    bool again = false;
+    if (!cams_run && (rc = grow_bin_list(ctx, cams[run[0].cam].fcs[0], n, &again))) return rc;
+    if (again) {   // as in do_draw
+      const bool clear = first || !ctx->bin_overflow;
+      launch_bin_list_begin(ctx->bin, ctx->cams_ghist, ctx->stream);
+      emitted = 0;
+      emit_to(count, clear);
+      GS_CUDA_TRY(ctx, launch_bin_list_sort(bins, ctx->bin, ctx->sort, ctx->cams_ghist, ctx->stream, &lists, &more));
+      sort_launches += more;
+      ctx->bin_overflow = !clear;
+    }
+    lists.tile_cost = tile_cost;
+    rec(ctx, EV_BIN1);
+    launch_raster_cameras(objs, dc, bins, tiles, opt.blend_mode, cams[run[0].cam].rt_fmt, lists, ctx->stream);
+    rec(ctx, EV_RASTER1);
+    ctx->launches += sort_launches + 3;   // bin sort passes; bin_ranges, tile_order, raster
+    GS_CUDA_TRY(ctx, cudaGetLastError());
+  }
+  for (const Segment &sg : run) {
+    CameraArgs &c = cams[sg.cam];
+    if (sg.k0 + sg.K == c.K && (rc = end_frame_image(ctx, surfs, c.rt, c.rt_pitch, c.rt_fmt, c.tgt, c.W, c.H, c.fi, false))) return rc;
   }
   return GS_OK;
+}
+
+// The work of gs_frame_objects and gs_frame_cameras once every camera has passed check_camera: the runs in order, and the bin
+// list's overflow reported here when some image was read back to the host, else at gs_sync.
+static int draw_cameras(GsContext *ctx, std::vector<CameraArgs> &cams, GsAsset *const *assets, const GsFrameParams *fps,
+                        const int32_t *do_sort_flags, const GsRenderOptions &opt) {
+  int rc = GS_OK;
+  // the objects' cutouts / bits share the context's buffers: sized for all of them before the first view-calc is queued
+  const uint32_t pairs = cams.back().off + cams.back().K;
+  for (uint32_t p = 0; p < pairs; ++p)
+    if ((rc = reserve_frame_inputs(ctx, assets[p], &fps[p]))) return rc;
+  for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
+  CallSurfaces surfs(ctx);
+  const std::vector<Run> runs = form_runs(cams, assets, fps);
+  bool flag_read = true;   // ctx->bin_overflow is current: the last draw read the list back
+  for (size_t r = 0; r < runs.size(); ++r) {
+    const FrameConsts &fc = cams[runs[r][0].cam].fcs[0];
+    const bool grows = runs[r].size() == 1 && (fc.binsX > kRuleBins || fc.binsY > kRuleBins);
+    if (grows && r > 0 && !flag_read) {
+      // a grown list clears the overflow flag unless an earlier draw of the call was truncated (do_draw): read it first
+      uint32_t flag = 0;
+      GS_CUDA_TRY(ctx, cudaMemcpyAsync(&flag, ctx->bin.entry_count + 1, 4, cudaMemcpyDeviceToHost, ctx->stream));
+      GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+      ctx->bin_overflow = flag != 0;
+    }
+    flag_read = grows;
+    if ((rc = draw_run(ctx, surfs, cams, runs[r], assets, fps, do_sort_flags, opt, r == 0))) return rc;
+  }
+  bool host = false;
+  for (const CameraArgs &c : cams)
+    host |= (c.rt && c.rt->memory == GS_MEM_HOST && !c.fi.async_rb) || (c.tgt && c.tgt->memory == GS_MEM_HOST);
+  return host ? check_bin_overflow(ctx) : GS_OK;
 }
 }  // namespace gs
 
@@ -1171,29 +1247,20 @@ int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRende
   CallSurfaces surfs(ctx);
   FrameImage fi;
   if ((rc = begin_frame_image(ctx, surfs, opt, rt, rt_pitch, rt_fmt, tgt, W, H, &fi))) return rc;
-  if ((rc = do_draw(ctx, fc, opt, &as, fp, 1, true, fi.d_rt, fi.pitch, rt_fmt, fi.surf))) return rc;
+  if ((rc = do_draw(ctx, fc, opt, as, fp, true, fi.d_rt, fi.pitch, rt_fmt, fi.surf))) return rc;
   return end_frame_image(ctx, surfs, rt, rt_pitch, rt_fmt, tgt, W, H, fi);
 }
 
 int gs_frame_objects(GsContext *ctx, uint32_t object_count, GsAsset *const *assets, const GsFrameParams *fps, const int32_t *do_sort_flags,
                      const GsRenderOptions *opt_in, GsImage *rt, GsImage *tgt) {
   if (!ctx || !assets || !fps || !do_sort_flags) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null context / assets / fps / do_sort");
-  const uint32_t K = object_count;
-  if (K == 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "object_count is 0");
+  if (object_count == 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "object_count is 0");
   GsRenderOptions opt = opt_in ? *opt_in : default_opts();
-  std::vector<FrameConsts> fcs;
-  uint32_t W = 0, H = 0, rt_pitch = 0, rt_fmt = GS_PIX_RGBA16F;
-  int rc = check_camera(ctx, K, assets, fps, &opt, rt, tgt, &fcs, &W, &H, &rt_pitch, &rt_fmt);
+  std::vector<CameraArgs> cams(1);
+  cams[0].off = 0; cams[0].K = object_count; cams[0].rt = rt; cams[0].tgt = tgt;
+  const int rc = check_camera(ctx, assets, fps, &opt, &cams[0]);
   if (rc) return rc;
-  // the objects' cutouts / bits share the context's buffers: sized for all of them before the first view-calc is queued
-  for (uint32_t k = 0; k < K; ++k)
-    if ((rc = reserve_frame_inputs(ctx, assets[k], &fps[k]))) return rc;
-
-  for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
-  CallSurfaces surfs(ctx);
-  FrameImage fi;
-  if ((rc = draw_objects(ctx, surfs, K, assets, fps, do_sort_flags, fcs, opt, rt, rt_pitch, rt_fmt, tgt, W, H, true, &fi))) return rc;
-  return end_frame_image(ctx, surfs, rt, rt_pitch, rt_fmt, tgt, W, H, fi);
+  return draw_cameras(ctx, cams, assets, fps, do_sort_flags, opt);
 }
 
 int gs_frame_cameras(GsContext *ctx, uint32_t camera_count, const uint32_t *object_counts, GsAsset *const *assets, const GsFrameParams *fps,
@@ -1206,7 +1273,6 @@ int gs_frame_cameras(GsContext *ctx, uint32_t camera_count, const uint32_t *obje
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "GS_FLAG_ASYNC_READBACK is not accepted by gs_frame_cameras: its host images are read back before it returns");
   std::vector<CameraArgs> cams(camera_count);
   uint64_t pairs = 0;
-  int rc = GS_OK;
   for (uint32_t c = 0; c < camera_count; ++c) {
     CameraArgs &a = cams[c];
     if (object_counts[c] == 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "a camera has no objects (leave it out: the reference draws nothing for it)");
@@ -1214,68 +1280,10 @@ int gs_frame_cameras(GsContext *ctx, uint32_t camera_count, const uint32_t *obje
     pairs += a.K;
     if (pairs > 0xFFFFFFFFu) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "more than 2^32 - 1 objects in all");
     GsRenderOptions o = opt;
-    if ((rc = check_camera(ctx, a.K, assets + a.off, fps + a.off, &o, a.rt, a.tgt, &a.fcs, &a.W, &a.H, &a.rt_pitch, &a.rt_fmt))) return rc;
+    const int rc = check_camera(ctx, assets + a.off, fps + a.off, &o, &a);
+    if (rc) return rc;
   }
-  for (uint64_t p = 0; p < pairs; ++p)
-    if ((rc = reserve_frame_inputs(ctx, assets[p], &fps[p]))) return rc;
-
-  for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
-  CallSurfaces surfs(ctx);
-  bool host = false;
-  // May camera `c` join the run cams[c0, c)?  Its own limits, the run's totals, one pixel format, and no image shared with the
-  // run's render targets (two cameras rasterizing into one image at once would race, where the loop draws one after the other).
-  auto joins = [&](uint32_t c0, uint32_t c, uint32_t run_pairs, uint32_t run_bins) {
-    const CameraArgs &a = cams[c];
-    if (a.W > kMaxRunScreen || a.H > kMaxRunScreen || a.K > kRunObjects) return false;
-    const GsFrameParams *depth = nullptr;
-    for (uint32_t k = 0; k < a.K; ++k) {
-      const GsFrameParams &f = fps[a.off + k];
-      if (assets[a.off + k]->av.n > kLocalIdMask) return false;
-      if (!f.scene_depth) continue;
-      if (!depth) depth = &f;
-      else if (f.scene_depth != depth->scene_depth || f.scene_depth_on_device != depth->scene_depth_on_device) return false;
-    }
-    if (c == c0) return true;
-    if (run_pairs + a.K > kRunObjects || run_bins + a.fcs[0].binsX * a.fcs[0].binsY > kMaxRunBins || a.rt_fmt != cams[c0].rt_fmt) return false;
-    for (uint32_t j = c0; j < c; ++j) {
-      const void *rj = cams[j].rt ? cams[j].rt->data : nullptr, *tj = cams[j].tgt ? cams[j].tgt->data : nullptr;
-      if (a.rt && (a.rt->data == rj || a.rt->data == tj)) return false;
-      if (a.tgt && a.tgt->data == rj) return false;
-    }
-    return true;
-  };
-  for (uint32_t c = 0; c < camera_count;) {
-    uint32_t e = c, run_pairs = 0, run_bins = 0;
-    while (e < camera_count && joins(c, e, run_pairs, run_bins)) {
-      run_pairs += cams[e].K;
-      run_bins += cams[e].fcs[0].binsX * cams[e].fcs[0].binsY;
-      ++e;
-    }
-    for (uint32_t j = c; j < std::max(e, c + 1); ++j)
-      host |= (cams[j].rt && cams[j].rt->memory == GS_MEM_HOST) || (cams[j].tgt && cams[j].tgt->memory == GS_MEM_HOST);
-    if (e - c >= 2) {
-      if ((rc = draw_camera_run(ctx, surfs, &cams[c], e - c, assets, fps, do_sort_flags, opt, c == 0))) return rc;
-      c = e;
-      continue;
-    }
-    // a camera on its own: gs_frame_objects' work
-    CameraArgs &a = cams[c];
-    if (c > 0 && (a.fcs[0].binsX > kRuleBins || a.fcs[0].binsY > kRuleBins)) {
-      // a growing bin list clears the overflow flag unless an earlier draw of the call was truncated (do_draw): read it
-      uint32_t flag = 0;
-      GS_CUDA_TRY(ctx, cudaMemcpyAsync(&flag, ctx->bin.entry_count + 1, 4, cudaMemcpyDeviceToHost, ctx->stream));
-      GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-      ctx->bin_overflow = flag != 0;
-    }
-    FrameImage fi;
-    if ((rc = draw_objects(ctx, surfs, a.K, assets + a.off, fps + a.off, do_sort_flags + a.off, a.fcs, opt, a.rt, a.rt_pitch, a.rt_fmt, a.tgt,
-                           a.W, a.H, c == 0, &fi)))
-      return rc;
-    if ((rc = end_frame_image(ctx, surfs, a.rt, a.rt_pitch, a.rt_fmt, a.tgt, a.W, a.H, fi, false))) return rc;
-    ++c;
-  }
-  // overflow is reported as gs_frame_objects reports it: here when a host image was read back, else at gs_sync
-  return host ? check_bin_overflow(ctx) : GS_OK;
+  return draw_cameras(ctx, cams, assets, fps, do_sort_flags, opt);
 }
 
 int gs_unshuffle_bands(GsContext *ctx, const void *gathered, uint32_t parts, uint32_t band_rows, uint32_t rows_pp, uint32_t fmt,

@@ -872,7 +872,7 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
         opt.flags = k ? (uint32_t)GS_FLAG_LOAD_RT : 0u;
         rec(ctx, EV_VIEW1);
         if (timing) cudaEventRecord(mb.obj_tev[2 * k], ctx->stream);
-        if ((rc = do_draw(ctx, o.fc, opt, o.assets + i, o.fp, 1, k == 0, d_rt, pitch, fmt, 0, timing ? mb.obj_tev[2 * k + 1] : nullptr)))
+        if ((rc = do_draw(ctx, o.fc, opt, o.assets[i], o.fp, k == 0, d_rt, pitch, fmt, 0, timing ? mb.obj_tev[2 * k + 1] : nullptr)))
           return rc;
         ctx->launches += 1;   // k_row_costs: here for every object but the last (before the next one's raster overwrites the
                               // tile costs), on the transfer stream below for the last

@@ -119,13 +119,13 @@ int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cu
 // record slabs); the asset's draw state is then left as it was
 int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameConsts &fc, bool cull, const GsRenderOptions &opt,
             cudaStream_t stream, float4 *draw = nullptr, float *zndc = nullptr);
-// Bins and rasterizes the objects as[0, count), drawn with the uniforms fps[0, count), into a device image (d_rt == nullptr:
-// the CUDA array behind `surf`) on ctx->stream: one object with gs_frame's kernels, or several as one run of gs_frame_objects
-// (DrawObjects).  The scene depth buffer bound is that of the first object that has one.  `first`: the first draw of its
-// public call, whose bin list sets the overflow flag; a later draw of the call only ever sets it, so the call reports every
-// truncated list.  bin_done (optional) is recorded on ctx->stream when binning ends.
-int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *const *as, const GsFrameParams *fps, uint32_t count,
-            bool first, void *d_rt, uint32_t pitch, uint32_t fmt, cudaSurfaceObject_t surf = 0, cudaEvent_t bin_done = nullptr);
+// Bins and rasterizes one object `as`, drawn with the uniforms *fp, into a device image (d_rt == nullptr: the CUDA array behind
+// `surf`) on ctx->stream with gs_frame's kernels; its scene depth buffer is bound here.  A run of several objects or cameras is
+// gs_api.cu's draw_run.  `first`: the first draw of its public call, whose bin list sets the overflow flag; a later draw of
+// the call only ever sets it, so the call reports every truncated list.  bin_done (optional) is recorded on ctx->stream when
+// binning ends.
+int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *as, const GsFrameParams *fp, bool first,
+            void *d_rt, uint32_t pitch, uint32_t fmt, cudaSurfaceObject_t surf = 0, cudaEvent_t bin_done = nullptr);
 // The composite pass (gs_composite) of a linear device render target onto `tgt` (host, device or CUDA-array memory, already
 // validated as W x H), enqueued on `s`.  A host target is uploaded and read back, and the call waits for `s`.
 int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H,

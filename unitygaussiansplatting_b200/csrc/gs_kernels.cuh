@@ -180,64 +180,62 @@ struct BinScratch {
   uint32_t *tile_cost, *tile_order;   // per raster tile: last frame's cost, this frame's launch order
   uint32_t capacity;
 };
-// The splat objects one draw bins and rasterizes, in draw order.  A list of one is drawn by gs_frame's kernels, under any tile
-// partition.  A longer list is a run of gs_frame_objects: at most kRunObjects objects, each with fewer than 2^kSlotShift
-// splats, on the whole screen.  Their entries go into one list, object after object, each tagged (slot << kSlotShift) | splat
-// id; that list is sorted once by bin id and drawn by one k_raster<..., MULTI> pass, whose kernel parameter this is.
+// A run: several (camera, object) pairs, at most kRunObjects, drawn by one bin list, one bin sort and one k_raster<..., MULTI>
+// pass.  Each pair's object has fewer than 2^kSlotShift splats; its entries are tagged (slot << kSlotShift) | splat id, slot
+// being the pair's index in the run.  A single object is drawn by gs_frame's kernels instead (launch_binning, launch_raster).
 constexpr uint32_t kRunObjects = 16, kSlotShift = 28, kLocalIdMask = (1u << kSlotShift) - 1u;
+// What the MULTI raster reads of the run's pairs (a kernel parameter).
 struct DrawObjects {
   const float4 *draw[kRunObjects];   // raster records
-  const float *zndc[kRunObjects];    // quad depths, where the object is depth-tested
-  uint32_t depth_mask;               // bit k: object k is depth-tested against the draw's scene depth buffer
+  const float *zndc[kRunObjects];    // quad depths, where the pair is depth-tested
+  uint32_t depth_mask;               // bit k: pair k is depth-tested against its camera's scene depth buffer
   uint32_t count;
-  bool extras;                       // some object has a selection or is depth-tested: the raster's SEL instantiation
-  uint32_t n[kRunObjects];           // splats, and what binning reads of them
-  const uint32_t *order[kRunObjects], *rect[kRunObjects], *block_bits[kRunObjects];
+  bool extras;                       // some pair has a selection or is depth-tested: the raster's SEL instantiation
 };
 struct NoRasterObjects {};
-// The objects' (bin id, splat id) lists, sorted by bin id.  *sorted: the scratch view whose tile_keys / tile_vals hold them
+// One object's (bin id, splat id) list, sorted by bin id.  *sorted: the scratch view whose tile_keys / tile_vals hold it
 // (launch_raster's input).  clear_overflow: this is the first draw of its call, and its list sets the overflow flag
 // entry_count[1] from its own total; otherwise the flag is only ever set, so an earlier draw's truncation stays reported.
-cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, const DrawObjects &objs, bool clear_overflow,
-                           const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted, int *launches);
+cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, const uint32_t *order, const uint32_t *rect,
+                           const uint32_t *block_bits, uint32_t n, bool clear_overflow, const BinScratch &bs, const SortScratch &sc,
+                           cudaStream_t s, BinScratch *sorted, int *launches);
 
-// A camera run of gs_frame_cameras: consecutive cameras whose (camera, object) pairs, at most kRunObjects in all, share one
-// bin list, one bin sort and one k_raster<..., MULTI, CAMS> pass.  Camera c owns the bin ids [bin_base, bin_base + its bins)
-// and the raster tiles [tile_base, tile_base + its tiles) of the run; the raster finds a tile's camera in this table, staged
-// in shared memory.
+// The cameras of a run, in shared memory in the MULTI raster.  A run is a list of camera segments: camera c's pairs of the run
+// own the bin ids [bin_base, bin_base + its bins) and the raster tiles [tile_base, tile_base + its tiles).  A run of one camera
+// has bin_base = tile_base = 0.
 struct RasterCamera {
   uint8_t *rt;                 // linear device image, or nullptr: the CUDA array behind `surf`
   cudaSurfaceObject_t surf;
   const float *depth;          // the camera's scene depth buffer (device memory), or nullptr
   uint32_t pitch, tile_base, bin_base, ntx, binsX, W, H;
-  uint32_t load;               // 1: blend under what the image holds; 0: the image starts cleared
+  uint32_t load;               // 1: blend under what the image holds (the camera's earlier run drew it); 0: the image starts cleared
 };
 struct DrawCameras {
   RasterCamera cam[kRunObjects];
   uint32_t count;
 };
-// The run's binning, in three steps around its pairs' sorts and view-calcs (a pair's emit must follow its view-calc before
-// the next sort or view-calc of the same asset overwrites order / rect / block_bits):
+// The run's binning, in three steps around its pairs' sorts and view-calcs (a pair's emit must come before a later sort or
+// view-calc of the same asset overwrites order / rect / block_bits):
 //   launch_bin_list_begin: empties the list and zeroes `ghist`, the digit histograms the emits count into;
 //   launch_bin_emit_pair:  appends one pair's entries, keys offset by its camera's bin_base, values tagged with its slot;
-//   launch_bin_list_sort:  the stable sort of the run's list by bin id, over `bins` bins, with the histograms in `ghist`.
-// bin_sort_bits gives the digit plan the emits and the sort share.
-void bin_sort_bits(uint32_t bins, int *bits, int *passes);
+//   launch_bin_list_sort:  the stable sort of the list by bin id, over `bins` bins, with the histograms in `ghist`.
 void launch_bin_list_begin(const BinScratch &bs, uint32_t *ghist, cudaStream_t s);
 void launch_bin_emit_pair(const uint32_t *order, const uint32_t *rect, const uint32_t *block_bits, uint32_t n, uint32_t binsX,
                           uint32_t bin_base, uint32_t slot, bool clear_overflow, uint32_t bins, const BinScratch &bs, uint32_t *ghist,
                           cudaStream_t s);
-cudaError_t launch_bin_list_sort(uint32_t bins, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted,
+cudaError_t launch_bin_list_sort(uint32_t bins, const BinScratch &bs, SortScratch sc, uint32_t *ghist, cudaStream_t s, BinScratch *sorted,
                                  int *launches);
 // k_bin_ranges over the run's bins, k_tile_order over its raster tiles (history indexed by tile_base + tile), and the raster.
 // Every render target of the run has rt_format.
 void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, uint32_t bins, uint32_t tiles, uint32_t blend_mode,
                            uint32_t rt_format, const BinScratch &bs, cudaStream_t s);
-// scene_depth: the W x H depth buffer the depth-tested objects are tested against (nullptr: none).  opt: tile partition,
+// One object's raster: records `draw`, quad depths `zndc` (when depth-tested), `extras`: a selection or a scene depth buffer
+// (the SEL instantiation).  scene_depth: the W x H depth buffer it is tested against (nullptr: none).  opt: tile partition,
 // band_packed, blend mode and GS_FLAG_LOAD_RT.  Images here are linear device memory (pointer, pitch) or, when the pointer is
 // null, a CUDA array behind a surface object.
-void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const DrawObjects &objs, const BinScratch &bs, void *rt,
-                   uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s, const float *scene_depth);
+void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const float *zndc, bool extras,
+                   const BinScratch &bs, void *rt, uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s,
+                   const float *scene_depth);
 extern unsigned long long *g_raster_stats;   // diagnostics, see GS_RASTER_STATS
 uint32_t partition_own_bin_rows(const GsRenderOptions &opt, uint32_t binsY);
 uint32_t partition_own_tile_rows(const GsRenderOptions &opt, uint32_t binsY);

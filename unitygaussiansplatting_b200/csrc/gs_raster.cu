@@ -46,11 +46,10 @@ __device__ __forceinline__ uint32_t entry_tile(uint32_t e, uint32_t r, const Par
   return ty * tilesX + x0 + col;
 }
 
-// APPEND (several objects into one list): the entries go behind the entry_count[2] already listed, and each value is tagged
-// `tag | splat id` (tag = the object's slot << kSlotShift).  clear_overflow: the overflow flag entry_count[1] is set from this
-// list's total; otherwise it is only ever set.
-// CAMS (a camera run of gs_frame_cameras, with APPEND): each key is the bin id plus key_base, the camera's first bin in the run.
-template <bool APPEND, bool CAMS = false>
+// APPEND (one pair of a run, see DrawCameras): the entries go behind the entry_count[2] already listed, each key is the bin
+// id plus key_base (the camera's first bin in the run) and each value is tagged `tag | splat id` (tag = the pair's slot <<
+// kSlotShift).  clear_overflow: the overflow flag entry_count[1] is set from this list's total; otherwise it is only ever set.
+template <bool APPEND>
 __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ order, const uint32_t *__restrict__ rect,
                                                   const uint32_t *__restrict__ block_bits, uint32_t bits_words, uint32_t n, Partition part,
                                                   uint32_t tilesX, volatile uint32_t *status,
@@ -187,7 +186,7 @@ __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ o
       const uint32_t oid = __shfl_sync(0xffffffffu, it.x, lo);
       const uint32_t o = off + x;
       if (x < T && o < capacity) {
-        const uint32_t tile = entry_tile(x - opre, orc, part, tilesX) + (CAMS ? key_base : 0u);
+        const uint32_t tile = entry_tile(x - opre, orc, part, tilesX) + (APPEND ? key_base : 0u);
         keys[o] = tile;
         vals[o] = APPEND ? (tag | oid) : oid;
         atomicAdd(&s_dh[tile & dmask], 1u);
@@ -212,7 +211,6 @@ static void bin_sort_plan(uint32_t bins, int *bits, int *passes) {
   *passes = 2;
   *bits = bins <= 1024u ? 5 : bins <= 4096u ? 6 : bins <= 16384u ? 7 : 8;
 }
-void bin_sort_bits(uint32_t bins, int *bits, int *passes) { bin_sort_plan(bins, bits, passes); }
 
 // the sort by bin id of a list whose digit histograms are in sc.ghist; an odd number of passes leaves it in the sorter's
 // ping-pong buffers
@@ -241,54 +239,46 @@ void launch_bin_list_begin(const BinScratch &bs, uint32_t *ghist, cudaStream_t s
   cudaMemsetAsync(ghist, 0, 4 * 256 * sizeof(uint32_t), s);
 }
 
-void launch_bin_emit_pair(const uint32_t *order, const uint32_t *rect, const uint32_t *block_bits, uint32_t n, uint32_t binsX,
-                          uint32_t bin_base, uint32_t slot, bool clear_overflow, uint32_t bins, const BinScratch &bs, uint32_t *ghist,
-                          cudaStream_t s) {
+// the look-back clear and k_bin_emit of one object's entries, counted into ghist by the digit plan of `bins` bins
+template <bool APPEND>
+static void bin_emit(const uint32_t *order, const uint32_t *rect, const uint32_t *block_bits, uint32_t n, const Partition &part,
+                     uint32_t binsX, uint32_t bins, bool clear_overflow, uint32_t tag, uint32_t key_base, const BinScratch &bs,
+                     uint32_t *ghist, cudaStream_t s) {
   int bits, passes;
   bin_sort_plan(bins, &bits, &passes);
   const uint32_t nblocks = (n + kBinBlock - 1) / kBinBlock, words = bin_bits_words(n);
   cudaMemsetAsync(bs.block_sums, 0, ((size_t)nblocks + 1) * sizeof(uint32_t), s);   // [0] ticket, [1..] look-back status
-  k_bin_emit<true, true><<<nblocks, 256, words * 4u, s>>>(order, rect, block_bits, words, n, Partition{0, 0, 1, 0, 0, 0}, binsX,
-                                                          bs.block_sums + 1, bs.block_sums, bs.capacity, bs.tile_keys, bs.tile_vals,
-                                                          bs.entry_count, ghist, (uint32_t)bits, passes == 2, clear_overflow,
-                                                          slot << kSlotShift, bin_base);
+  k_bin_emit<APPEND><<<nblocks, 256, words * 4u, s>>>(order, rect, block_bits, words, n, part, binsX, bs.block_sums + 1, bs.block_sums,
+                                                      bs.capacity, bs.tile_keys, bs.tile_vals, bs.entry_count, ghist, (uint32_t)bits,
+                                                      passes == 2, clear_overflow, tag, key_base);
 }
 
-cudaError_t launch_bin_list_sort(uint32_t bins, const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted,
+void launch_bin_emit_pair(const uint32_t *order, const uint32_t *rect, const uint32_t *block_bits, uint32_t n, uint32_t binsX,
+                          uint32_t bin_base, uint32_t slot, bool clear_overflow, uint32_t bins, const BinScratch &bs, uint32_t *ghist,
+                          cudaStream_t s) {
+  bin_emit<true>(order, rect, block_bits, n, Partition{0, 0, 1, 0, 0, 0}, binsX, bins, clear_overflow, slot << kSlotShift, bin_base, bs,
+                 ghist, s);
+}
+
+cudaError_t launch_bin_list_sort(uint32_t bins, const BinScratch &bs, SortScratch sc, uint32_t *ghist, cudaStream_t s, BinScratch *sorted,
                                  int *launches) {
   int bits, passes;
   bin_sort_plan(bins, &bits, &passes);
   *sorted = bs;
   *launches = passes;
+  sc.ghist = ghist;
   return sort_bin_list(bits, passes, bs, sc, s, sorted);
 }
 
-cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, const DrawObjects &objs, bool clear_overflow,
-                           const BinScratch &bs, const SortScratch &sc, cudaStream_t s, BinScratch *sorted, int *launches) {
-  const Partition part = make_partition(opt);
-  const bool run = objs.count > 1;
-  *sorted = bs;
-  int bits, passes;
-  bin_sort_plan(fc.binsX * fc.binsY, &bits, &passes);
-  *launches = passes;
-  if (run) cudaMemsetAsync(bs.entry_count + 2, 0, sizeof(uint32_t), s);   // the objects append behind an empty list
+cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, const uint32_t *order, const uint32_t *rect,
+                           const uint32_t *block_bits, uint32_t n, bool clear_overflow, const BinScratch &bs, const SortScratch &sc,
+                           cudaStream_t s, BinScratch *sorted, int *launches) {
+  const uint32_t bins = fc.binsX * fc.binsY;
   cudaMemsetAsync(sc.ghist, 0, 4 * 256 * sizeof(uint32_t), s);
-  for (uint32_t k = 0; k < objs.count; ++k) {
-    const uint32_t n = objs.n[k], nblocks = (n + kBinBlock - 1) / kBinBlock;
-    cudaMemsetAsync(bs.block_sums, 0, ((size_t)nblocks + 1) * sizeof(uint32_t), s);   // [0] ticket, [1..] look-back status
-    const uint32_t words = bin_bits_words(n);
-    const bool clear = clear_overflow && k == 0;   // the later objects' totals include this one's: they can only add overflow
-    if (run)
-      k_bin_emit<true><<<nblocks, 256, words * 4u, s>>>(objs.order[k], objs.rect[k], objs.block_bits[k], words, n, part, fc.binsX,
-                                                        bs.block_sums + 1, bs.block_sums, bs.capacity, bs.tile_keys, bs.tile_vals,
-                                                        bs.entry_count, sc.ghist, (uint32_t)bits, passes == 2, clear, k << kSlotShift, 0u);
-    else
-      k_bin_emit<false><<<nblocks, 256, words * 4u, s>>>(objs.order[k], objs.rect[k], objs.block_bits[k], words, n, part, fc.binsX,
-                                                         bs.block_sums + 1, bs.block_sums, bs.capacity, bs.tile_keys, bs.tile_vals,
-                                                         bs.entry_count, sc.ghist, (uint32_t)bits, passes == 2, clear, 0u, 0u);
-    *launches += 2;   // look-back clear, bin_emit
-  }
-  return sort_bin_list(bits, passes, bs, sc, s, sorted);
+  bin_emit<false>(order, rect, block_bits, n, make_partition(opt), fc.binsX, bins, clear_overflow, 0u, 0u, bs, sc.ghist, s);
+  const cudaError_t e = launch_bin_list_sort(bins, bs, sc, sc.ghist, s, sorted, launches);
+  *launches += 2;   // look-back clear, bin_emit
+  return e;
 }
 
 // ---- 2. raster ---------------------------------------------------------------------------------
@@ -413,19 +403,19 @@ __device__ __forceinline__ bool block_may_touch_quad(const float4 &A, float i2x,
 // (reversed Z: quad depth >= stored depth), the per-splat quad depths being staged beside the records.
 // SURF: the target is a CUDA array (GS_MEM_ARRAY), read and written through the surface object `surf` instead of `rt`/`pitch`; a
 // separate instantiation so that the linear ones keep their code.
-// MULTI: the list holds the entries of several objects (one run of gs_frame_objects), each tagged with its slot in `objs`; the
-// records are gathered from that object's buffers, and the result is what drawing the objects one after the other leaves.
-// CAMS (with MULTI): a camera run of gs_frame_cameras.  The grid covers every camera's tiles; a tile finds its camera in `cams`
-// (staged in shared memory), which gives it the screen size, bins, image (pointer and pitch, or a surface when the pointer is
-// null), scene depth buffer and load flag that the other instantiations take from fc and the image arguments.  The camera's
-// bin ids start at its bin_base in bin_ranges; tile_cost is indexed by tile_base + the tile.
-template <bool FP16_ROP, int OUT_FMT, bool STATS, bool SEL = false, bool SURF = false, bool MULTI = false, bool CAMS = false>
-__global__ void __launch_bounds__(256)
+// MULTI: a run (DrawCameras) of several (camera, object) pairs.  The list holds every pair's entries, each tagged with its slot
+// in `objs`; the records are gathered from that pair's buffers, and each camera's result is what drawing its objects one after
+// the other leaves.  The grid covers every camera's tiles; a tile finds its camera c in `cams`, which gives it the screen size, bins, image (pointer and pitch, or a surface when the pointer is null), scene depth buffer and load
+// flag that the other instantiations take from fc and the image arguments.  The camera's bin ids start at its bin_base in
+// bin_ranges; tile_cost is indexed by tile_base + the tile.  SURF: some camera's image is a CUDA array.  MULTI with SEL is held
+// to 32 registers, 8 CTAs per SM, which its shared memory also fits (selected runs measured 20 % slower at 7).
+template <bool FP16_ROP, int OUT_FMT, bool STATS, bool SEL = false, bool SURF = false, bool MULTI = false>
+__global__ void __launch_bounds__(256, MULTI && SEL ? 8 : 0)
 k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const uint2 *__restrict__ bin_ranges,
          const uint32_t *__restrict__ tile_vals, const uint32_t *__restrict__ tile_order, uint32_t *__restrict__ tile_cost, uint32_t ntx,
          uint8_t *__restrict__ rt, uint32_t pitch, cudaSurfaceObject_t surf, uint32_t band_packed, uint32_t load_rt,
          unsigned long long *stats, const float *__restrict__ zndc, const float *__restrict__ scene_depth,
-         std::conditional_t<MULTI, DrawObjects, NoRasterObjects> objs, std::conditional_t<CAMS, DrawCameras, NoRasterObjects> cams) {
+         std::conditional_t<MULTI, DrawObjects, NoRasterObjects> objs, std::conditional_t<MULTI, DrawCameras, NoRasterObjects> cams) {
   uint32_t st_batches = 0, st_culls = 0, st_cand = 0, st_eval = 0, st_blend = 0;   // GS_RASTER_STATS diagnostics (per warp)
   unsigned long long st_t0 = 0;
   if (STATS) asm volatile("mov.u64 %0, %globaltimer;" : "=l"(st_t0));
@@ -437,24 +427,27 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   __shared__ const float4 *s_draw[MULTI ? kRunObjects : 1];
   __shared__ const float *s_zndc[MULTI ? kRunObjects : 1];
   __shared__ uint8_t s_slot[MULTI ? 2 : 1][MULTI ? 256 : 1];
-  __shared__ RasterCamera s_cam[CAMS ? kRunObjects : 1];
-  // CAMS: the tile's camera and its first tile / bin in the run
+  // MULTI: the tile's first tile / bin in the run, and its camera (found again where it is used, so that nothing of it is held
+  // in registers across the blend loop)
   uint32_t lin = 0, tile_base = 0, bin_base = 0;
-  if constexpr (CAMS) {
-    if (threadIdx.x == 0) {
-#pragma unroll
-      for (uint32_t k = 0; k < kRunObjects; ++k) { s_draw[k] = objs.draw[k]; s_zndc[k] = objs.zndc[k]; s_cam[k] = cams.cam[k]; }
-    }
+  auto camera = [&](const auto &cs) -> const RasterCamera & {   // (generic: instantiated only where MULTI calls it)
+    uint32_t c = 0;
+    for (uint32_t k = 1; k < cs.count; ++k) if (lin >= cs.cam[k].tile_base) c = k;
+    return cs.cam[c];
+  };
+  if constexpr (MULTI) {
+    if (threadIdx.x < objs.count) { s_draw[threadIdx.x] = objs.draw[threadIdx.x]; s_zndc[threadIdx.x] = objs.zndc[threadIdx.x]; }
     __syncthreads();
     lin = __ldg(tile_order + blockIdx.x);
-    uint32_t c = 0;
-    for (uint32_t k = 1; k < cams.count; ++k) if (lin >= s_cam[k].tile_base) c = k;
-    const RasterCamera &cam = s_cam[c];
+    const RasterCamera &cam = camera(cams);
     fc.screenW = (float)cam.W; fc.screenH = (float)cam.H; fc.binsX = cam.binsX;
-    ntx = cam.ntx; rt = cam.rt; pitch = cam.pitch; surf = cam.surf; scene_depth = cam.depth; load_rt = cam.load;
+    ntx = cam.ntx; scene_depth = cam.depth; load_rt = cam.load;
     tile_base = cam.tile_base; bin_base = cam.bin_base;
   }
-  const bool surf_io = SURF || (CAMS && rt == nullptr);
+  bool surf_io = SURF;
+  auto camera_image = [&]() {
+    if constexpr (MULTI) { const RasterCamera &cam = camera(cams); rt = cam.rt; pitch = cam.pitch; surf = cam.surf; surf_io = SURF && rt == nullptr; }
+  };
   const bool depth_test = SEL && scene_depth != nullptr;
   // FP32 blending into an RGBA16F target: drawing the objects one after the other stores (rounds to half) each object's result
   // and the next object starts from it.  Rounding is idempotent, so rounding at the next object's first candidate is exact.
@@ -466,20 +459,13 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   constexpr uint32_t R = kBin / kTile;   // raster tiles per bin edge
   // launch order != raster order: CTA i takes tile order[i] (k_tile_order: most expensive first, by last frame's cost),
   // so the expensive tiles start early instead of forming the tail
-  if (!CAMS) lin = __ldg(tile_order + blockIdx.x);   // tile id in the whole image: ty * ntx + tx (CAMS: in the run)
+  if (!MULTI) lin = __ldg(tile_order + blockIdx.x);   // tile id in the whole image: ty * ntx + tx (MULTI: in the run)
   const uint32_t ty = (lin - tile_base) / ntx;
   const uint32_t tx = (lin - tile_base) - ty * ntx, brow = ty / R;
   if (ty * kTile >= (uint32_t)fc.screenH) { if (threadIdx.x == 0) tile_cost[lin] = 0; return; }
   __shared__ uint32_t s_cost;
   if (threadIdx.x == 0) s_cost = 0;
-  if constexpr (MULTI) {
-    depth_mask = objs.depth_mask;
-    if (!CAMS && threadIdx.x == 0) {
-#pragma unroll
-      for (uint32_t k = 0; k < kRunObjects; ++k) { s_draw[k] = objs.draw[k]; s_zndc[k] = objs.zndc[k]; }
-    }
-    if (!CAMS) __syncthreads();
-  }
+  if constexpr (MULTI) depth_mask = objs.depth_mask;
   // [start,end) of this tile's bin in the bin-sorted entry list (k_bin_ranges); R*R tiles share one list
   const uint2 range = __ldg(bin_ranges + bin_base + brow * fc.binsX + (tx / R));
   const uint32_t bx = tx * kTile + (warp & 1) * 8, by = ty * kTile + (warp >> 1) * 4;
@@ -497,6 +483,7 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   if (load_rt && in_image) {
     // GS_FLAG_LOAD_RT: the target was cleared once and earlier renderers of this camera already drew into it
     // (R/GaussianSplatRenderer.cs:111-168 loops the active splat objects over ONE _GaussianSplatRT); blend under what is there
+    camera_image();
     const uint8_t *row = rt + (size_t)out_row * pitch;
     if (OUT_FMT == GS_PIX_RGBA16F) {
       uint2 v;
@@ -640,6 +627,7 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   }
 
   if (in_image) {
+    camera_image();
     uint8_t *row = rt + (size_t)out_row * pitch;
     if (OUT_FMT == GS_PIX_RGBA16F) {
       uint2 o;
@@ -656,15 +644,16 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
 
 unsigned long long *g_raster_stats = nullptr;
 
-void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const DrawObjects &objs, const BinScratch &bs, void *rt,
-                   uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s, const float *scene_depth) {
+void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const float *zndc, bool extras,
+                   const BinScratch &bs, void *rt, uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s,
+                   const float *scene_depth) {
   const Partition part = make_partition(opt);
   const uint32_t rows = part.own_tile_rows(fc.binsY);
   if (!rows || !fc.binsX) return;
   const uint32_t ntx = ((uint32_t)fc.screenW + kTile - 1) / kTile, ntiles = ntx * rows;
   const uint32_t grid = ntiles;
   k_tile_order<<<1, 1024, 0, s>>>(bs.tile_cost, ntiles, ntx, part, bs.tile_order);
-  const bool rop = opt.blend_mode == GS_BLEND_FP16_ROP, run = objs.count > 1;
+  const bool rop = opt.blend_mode == GS_BLEND_FP16_ROP;
   uint8_t *out = reinterpret_cast<uint8_t *>(rt);
   // GS_RASTER_STATS=1: per-frame work counters of a one-object draw (diagnostics; printed by tools/raster_stats.py through
   // gs_debug_raster_stats)
@@ -677,17 +666,14 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const Draw
   uint2 *ranges = reinterpret_cast<uint2 *>(bs.bin_ranges);
   const uint32_t packed = part.range ? 0u : opt.band_packed, load = (opt.flags & GS_FLAG_LOAD_RT) ? 1u : 0u;
   k_bin_ranges<<<(bins + 7) / 8, 256, 0, s>>>(bs.tile_keys, bs.entry_count, bins, ranges);
-  // a run's raster reads each object's records and quad depths from `objs`, one object's from the draw / zndc arguments
-#define GS_RASTER_ARGS(OBJS)                                                                                                     \
-  <<<grid, 256, 0, s>>>(fc, part, objs.draw[0], ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, \
-                        packed, load, stats, objs.zndc[0], scene_depth, OBJS, NoRasterObjects{})
+#define GS_RASTER_ARGS                                                                                                           \
+  <<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed,  \
+                        load, stats, zndc, scene_depth, NoRasterObjects{}, NoRasterObjects{})
 #define GS_LAUNCH_RASTER(ROP, FMT, SURF)                                                                                        \
   do {                                                                                                                         \
-    if (run && objs.extras) k_raster<ROP, FMT, false, true, SURF, true> GS_RASTER_ARGS(objs);                                   \
-    else if (run) k_raster<ROP, FMT, false, false, SURF, true> GS_RASTER_ARGS(objs);                                            \
-    else if (objs.extras) k_raster<ROP, FMT, false, true, SURF> GS_RASTER_ARGS(NoRasterObjects{});                              \
-    else if (stats) k_raster<ROP, FMT, true, false, SURF> GS_RASTER_ARGS(NoRasterObjects{});                                    \
-    else k_raster<ROP, FMT, false, false, SURF> GS_RASTER_ARGS(NoRasterObjects{});                                              \
+    if (extras) k_raster<ROP, FMT, false, true, SURF> GS_RASTER_ARGS;                                                          \
+    else if (stats) k_raster<ROP, FMT, true, false, SURF> GS_RASTER_ARGS;                                                      \
+    else k_raster<ROP, FMT, false, false, SURF> GS_RASTER_ARGS;                                                                \
   } while (0)
   // a null `rt` means the target is a CUDA array behind rt_surf
 #define GS_LAUNCH_RASTER_TARGET(ROP, FMT)                                                                                       \
@@ -714,20 +700,27 @@ void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, uin
   FrameConsts fc;   // screen size and bins come from each tile's camera
   memset(&fc, 0, sizeof(fc));
   const bool rop = blend_mode == GS_BLEND_FP16_ROP;
-#define GS_RASTER_CAMS(ROP, FMT)                                                                                                \
+  bool surf = false;
+  for (uint32_t i = 0; i < cams.count; ++i) surf |= cams.cam[i].rt == nullptr;
+#define GS_RASTER_CAMS(ROP, FMT, SURF)                                                                                          \
   do {                                                                                                                         \
     if (objs.extras)                                                                                                           \
-      k_raster<ROP, FMT, false, true, false, true, true><<<tiles, 256, 0, s>>>(fc, whole, nullptr, ranges, bs.tile_vals,        \
-          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, 0, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);                      \
+      k_raster<ROP, FMT, false, true, SURF, true><<<tiles, 256, 0, s>>>(fc, whole, nullptr, ranges, bs.tile_vals, bs.tile_order,  \
+          bs.tile_cost, 1u, nullptr, 0u, 0, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);                                     \
     else                                                                                                                       \
-      k_raster<ROP, FMT, false, false, false, true, true><<<tiles, 256, 0, s>>>(fc, whole, nullptr, ranges, bs.tile_vals,       \
-          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, 0, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);                      \
+      k_raster<ROP, FMT, false, false, SURF, true><<<tiles, 256, 0, s>>>(fc, whole, nullptr, ranges, bs.tile_vals, bs.tile_order, \
+          bs.tile_cost, 1u, nullptr, 0u, 0, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);                                     \
+  } while (0)
+#define GS_RASTER_CAMS_TARGET(ROP, FMT)                                                                                         \
+  do {                                                                                                                         \
+    if (surf) GS_RASTER_CAMS(ROP, FMT, true); else GS_RASTER_CAMS(ROP, FMT, false);                                            \
   } while (0)
   if (rt_format == GS_PIX_RGBA16F) {
-    if (rop) GS_RASTER_CAMS(true, GS_PIX_RGBA16F); else GS_RASTER_CAMS(false, GS_PIX_RGBA16F);
+    if (rop) GS_RASTER_CAMS_TARGET(true, GS_PIX_RGBA16F); else GS_RASTER_CAMS_TARGET(false, GS_PIX_RGBA16F);
   } else {
-    if (rop) GS_RASTER_CAMS(true, GS_PIX_RGBA32F); else GS_RASTER_CAMS(false, GS_PIX_RGBA32F);
+    if (rop) GS_RASTER_CAMS_TARGET(true, GS_PIX_RGBA32F); else GS_RASTER_CAMS_TARGET(false, GS_PIX_RGBA32F);
   }
+#undef GS_RASTER_CAMS_TARGET
 #undef GS_RASTER_CAMS
 }
 
