@@ -103,27 +103,10 @@ FrameConsts make_frame_consts(const GsFrameParams *fp) {
   return fc;
 }
 
-static int grow(GsContext *ctx, void **p, size_t *cur, size_t need) {
-  if (*cur >= need && *p) return GS_OK;
-  if (*p) { cudaStreamSynchronize(ctx->stream); cudaFree(*p); *p = nullptr; *cur = 0; }
-  GS_CUDA_TRY(ctx, cudaMalloc(p, need));
-  *cur = need;
-  return GS_OK;
-}
-
 int ensure_sort_scratch(GsContext *ctx, uint32_t capacity) {
-  if (capacity <= ctx->sort_capacity) return GS_OK;
-  cudaStreamSynchronize(ctx->stream);
-  cudaFree(ctx->sort.alt_keys); cudaFree(ctx->sort.alt_vals); cudaFree(ctx->sort.lookback);
-  ctx->sort.alt_keys = ctx->sort.alt_vals = ctx->sort.lookback = nullptr;
-  ctx->sort_capacity = 0;
-  GS_CUDA_TRY(ctx, cudaMalloc(&ctx->sort.alt_keys, (size_t)capacity * 4));
-  GS_CUDA_TRY(ctx, cudaMalloc(&ctx->sort.alt_vals, (size_t)capacity * 4));
-  ctx->lookback_words = sort_lookback_words(capacity, 4);
-  GS_CUDA_TRY(ctx, cudaMalloc(&ctx->sort.lookback, ctx->lookback_words * 4));
-  ctx->sort.max_tiles = (capacity + kSortTileItems - 1) / kSortTileItems;
-  ctx->sort.lookback_words = ctx->lookback_words;
-  ctx->sort_capacity = capacity;
+  GS_CUDA_TRY(ctx, ctx->sort_alt_keys.reserve(capacity, {ctx->stream}));
+  GS_CUDA_TRY(ctx, ctx->sort_alt_vals.reserve(capacity, {ctx->stream}));
+  GS_CUDA_TRY(ctx, ctx->sort_lookback.reserve(sort_lookback_words(capacity, 4), {ctx->stream}));
   return GS_OK;
 }
 
@@ -138,33 +121,14 @@ static int ensure_bin_scratch(GsContext *ctx, uint32_t n, uint32_t tiles, uint32
   if (want < (4u << 20)) want = 4u << 20;
   if (want > kBinListMax) want = kBinListMax;
   if (want < min_capacity) want = min_capacity;
-  if ((uint32_t)want > ctx->bin.capacity) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(ctx->bin.tile_keys); cudaFree(ctx->bin.tile_vals);
-    ctx->bin.tile_keys = ctx->bin.tile_vals = nullptr;
-    ctx->bin.capacity = 0;
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.tile_keys, want * 4));
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.tile_vals, want * 4));
-    ctx->bin.capacity = (uint32_t)want;
-  }
-  int rc = ensure_sort_scratch(ctx, ctx->bin.capacity > n ? ctx->bin.capacity : n);
+  GS_CUDA_TRY(ctx, ctx->bin_keys.reserve(want, {ctx->stream}));
+  GS_CUDA_TRY(ctx, ctx->bin_vals.reserve(want, {ctx->stream}));
+  const uint32_t capacity = bin_scratch(ctx).capacity;
+  int rc = ensure_sort_scratch(ctx, capacity > n ? capacity : n);
   if (rc) return rc;
   const uint32_t blocks = n / 1024 + 2 < 1024u ? 1024u : n / 1024 + 2;   // the binner's ticket + range totals (<= 593 words) fit too
-  if (blocks > ctx->bin_blocks_cap) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(ctx->bin.block_sums);
-    ctx->bin.block_sums = nullptr;
-    ctx->bin_blocks_cap = 0;
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.block_sums, (size_t)blocks * 4));
-    ctx->bin_blocks_cap = blocks;
-  }
-  if (tiles > ctx->tiles_cap) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(ctx->bin.bin_ranges);
-    ctx->bin.bin_ranges = nullptr;
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.bin_ranges, (size_t)tiles * 8));
-    ctx->tiles_cap = tiles;
-  }
+  GS_CUDA_TRY(ctx, ctx->bin_block_sums.reserve(blocks, {ctx->stream}));
+  GS_CUDA_TRY(ctx, ctx->bin_ranges.reserve(tiles, {ctx->stream}));
   return GS_OK;
 }
 
@@ -178,9 +142,9 @@ static int grow_bin_list(GsContext *ctx, const FrameConsts &fc, uint32_t n, bool
   if (fc.binsX <= kRuleBins && fc.binsY <= kRuleBins) return GS_OK;
   const uint32_t tiles = fc.binsX * fc.binsY;
   uint32_t ec[3] = {0, 0, 0};   // clamped count, overflow flag, total (of this run, for gs_frame_objects)
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ec, ctx->bin.entry_count, sizeof(ec), cudaMemcpyDeviceToHost, ctx->stream));
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ec, ctx->bin_entry_count.get(), sizeof(ec), cudaMemcpyDeviceToHost, ctx->stream));
   GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  if (ec[2] <= ctx->bin.capacity || ec[2] > kBinListMax) {
+  if (ec[2] <= bin_scratch(ctx).capacity || ec[2] > kBinListMax) {
     ctx->bin_overflow = ec[1] != 0;
     return GS_OK;
   }
@@ -279,44 +243,22 @@ class CallSurfaces {
   std::vector<cudaSurfaceObject_t> made_;
 };
 
-int reserve_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t busy) {
-  auto drain = [&]() {
-    cudaStreamSynchronize(ctx->stream);
-    if (busy) cudaStreamSynchronize(busy);
-  };
-  if (fp->cutouts && fp->cutout_count && fp->cutout_count > ctx->cutout_cap) {
-    drain();
-    cudaFree(ctx->d_cutouts);
-    ctx->d_cutouts = nullptr;
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->d_cutouts, sizeof(GsCutout) * fp->cutout_count));
-    ctx->cutout_cap = fp->cutout_count;
-  }
+int reserve_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, std::initializer_list<cudaStream_t> users) {
+  if (fp->cutouts && fp->cutout_count) GS_CUDA_TRY(ctx, ctx->d_cutouts.reserve(fp->cutout_count, users));
   const size_t words = ((size_t)as->av.n + 31) / 32;
-  if (fp->deleted_bits && words > ctx->deleted_words) {
-    drain();
-    cudaFree(ctx->d_deleted);
-    ctx->d_deleted = nullptr;
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->d_deleted, words * 4));
-    ctx->deleted_words = words;
-  }
-  if (fp->selected_bits && words > ctx->selected_words) {
-    drain();
-    cudaFree(ctx->d_selected);
-    ctx->d_selected = nullptr;
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->d_selected, words * 4));
-    ctx->selected_words = words;
-  }
+  if (fp->deleted_bits) GS_CUDA_TRY(ctx, ctx->d_deleted.reserve(words, users));
+  if (fp->selected_bits) GS_CUDA_TRY(ctx, ctx->d_selected.reserve(words, users));
   return GS_OK;
 }
 
 int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t stream) {
-  int rc = reserve_frame_inputs(ctx, as, fp);
+  int rc = reserve_frame_inputs(ctx, as, fp, {ctx->stream});
   if (rc) return rc;
   const size_t words = ((size_t)as->av.n + 31) / 32;
   if (fp->cutouts && fp->cutout_count)
-    GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_cutouts, fp->cutouts, sizeof(GsCutout) * fp->cutout_count, cudaMemcpyHostToDevice, stream));
-  if (fp->deleted_bits) GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_deleted, fp->deleted_bits, words * 4, cudaMemcpyHostToDevice, stream));
-  if (fp->selected_bits) GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_selected, fp->selected_bits, words * 4, cudaMemcpyHostToDevice, stream));
+    GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_cutouts.get(), fp->cutouts, sizeof(GsCutout) * fp->cutout_count, cudaMemcpyHostToDevice, stream));
+  if (fp->deleted_bits) GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_deleted.get(), fp->deleted_bits, words * 4, cudaMemcpyHostToDevice, stream));
+  if (fp->selected_bits) GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_selected.get(), fp->selected_bits, words * 4, cudaMemcpyHostToDevice, stream));
   return GS_OK;
 }
 
@@ -326,16 +268,10 @@ static int bind_depth(GsContext *ctx, const GsFrameParams *fp, const float **dep
   *depth = nullptr;
   if (!fp->scene_depth) return GS_OK;
   if (fp->scene_depth_on_device) { *depth = fp->scene_depth; return GS_OK; }
-  const size_t bytes = (size_t)(uint32_t)fp->screen_w * (uint32_t)fp->screen_h * sizeof(float);
-  if (bytes > ctx->depth_bytes) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(ctx->d_depth);
-    ctx->d_depth = nullptr; ctx->depth_bytes = 0;
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->d_depth, bytes));
-    ctx->depth_bytes = bytes;
-  }
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_depth, fp->scene_depth, bytes, cudaMemcpyHostToDevice, ctx->stream));
-  *depth = ctx->d_depth;
+  const size_t pixels = (size_t)(uint32_t)fp->screen_w * (uint32_t)fp->screen_h;
+  GS_CUDA_TRY(ctx, ctx->d_depth.reserve(pixels, {ctx->stream}));
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_depth.get(), fp->scene_depth, pixels * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  *depth = ctx->d_depth.get();
   return GS_OK;
 }
 
@@ -354,11 +290,11 @@ static int do_sort(GsContext *ctx, GsAsset *as, const FrameConsts &fc) {
   int rc = ensure_sort_scratch(ctx, as->av.n);
   if (rc) return rc;
   rec(ctx, EV_BEGIN);
-  GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->sort.ghist, 0, 4 * 256 * 4, ctx->stream));
-  launch_calc_distances(as->av, fc, as->key_table, ctx->sort.ghist, ctx->stream);
+  GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->sort_ghist.get(), 0, 4 * 256 * 4, ctx->stream));
+  launch_calc_distances(as->av, fc, as->key_table, ctx->sort_ghist.get(), ctx->stream);
   rec(ctx, EV_DIST);
   cudaEvent_t pe[5] = {ctx->ev[EV_SORT0], ctx->ev[EV_SORT1], ctx->ev[EV_SORT2], ctx->ev[EV_SORT3], ctx->ev[EV_SORT4]};
-  GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order, as->d_n, as->av.n, 4, 8, true, ctx->sort, ctx->stream, ctx->timing ? pe : nullptr,
+  GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order, as->d_n, as->av.n, 4, 8, true, sort_scratch(ctx), ctx->stream, ctx->timing ? pe : nullptr,
                                      as->key_table));
   if (ctx->timing) for (int e = EV_SORT0; e <= EV_SORT4; ++e) ctx->ev_valid[e] = true;
   ctx->launches += 1 + 4;
@@ -380,7 +316,7 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
   const bool own = stream == ctx->stream;   // the group path runs view-calc beside the sort on a second stream and times it itself
   if (own) rec(ctx, EV_VIEW0);
   if (draw) {   // a record slab: the asset's own records stay as they are
-    launch_calc_view(as->av, fc, ctx->d_cutouts, ctx->d_deleted, ctx->d_selected, as->view, as->rect, draw, as->block_bits,
+    launch_calc_view(as->av, fc, ctx->d_cutouts.get(), ctx->d_deleted.get(), ctx->d_selected.get(), as->view, as->rect, draw, as->block_bits,
                      fp->scene_depth ? zndc : nullptr, cull, make_partition(opt), stream);
     if (own) rec(ctx, EV_VIEW1);
     ctx->launches += 1;
@@ -389,7 +325,7 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
   }
   if (fp->scene_depth && !as->zndc) GS_CUDA_TRY(ctx, cudaMalloc(&as->zndc, (size_t)as->av.n * sizeof(float) + 16));
   as->zndc_valid = fp->scene_depth != nullptr;
-  launch_calc_view(as->av, fc, ctx->d_cutouts, ctx->d_deleted, ctx->d_selected, as->view, as->rect, as->draw, as->block_bits,
+  launch_calc_view(as->av, fc, ctx->d_cutouts.get(), ctx->d_deleted.get(), ctx->d_selected.get(), as->view, as->rect, as->draw, as->block_bits,
                    as->zndc_valid ? as->zndc : nullptr, cull, make_partition(opt), stream);
   if (own) rec(ctx, EV_VIEW1);
   ctx->launches += 1;
@@ -410,47 +346,36 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
 // the tile count changes.  Otherwise a run of several cameras, whose layout ((raster tiles per row, rows) of each camera) keeps
 // its own history in cams_tile_cost, so that the runs of one call and the single-grid draws between calls do not reset each
 // other's.  At most kCameraLayouts layouts are kept; one more starts that cache afresh.  The launch-order scratch
-// bin.tile_order serves both.
+// tile_order serves both.
 constexpr size_t kCameraLayouts = 16;
 static int tile_history(GsContext *ctx, uint32_t tiles, const std::vector<uint32_t> *layout, uint32_t **cost) {
-  if (tiles > ctx->raster_tiles_cap) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(ctx->bin.tile_cost); cudaFree(ctx->bin.tile_order);
-    ctx->bin.tile_cost = ctx->bin.tile_order = nullptr;
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.tile_cost, (size_t)tiles * 4));
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.tile_order, (size_t)tiles * 4));
-    ctx->raster_tiles_cap = tiles;
-    ctx->raster_tiles_cur = 0;
-  }
+  if (tiles > ctx->tile_cost.size()) ctx->raster_tiles_cur = 0;   // a new buffer holds no history
+  GS_CUDA_TRY(ctx, ctx->tile_cost.reserve(tiles, {ctx->stream}));
+  GS_CUDA_TRY(ctx, ctx->tile_order.reserve(tiles, {ctx->stream}));
   if (!layout) {
     if (tiles != ctx->raster_tiles_cur) {
-      GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->bin.tile_cost, 0, (size_t)tiles * 4, ctx->stream));
+      GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->tile_cost.get(), 0, (size_t)tiles * 4, ctx->stream));
       ctx->raster_tiles_cur = tiles;
     }
-    *cost = ctx->bin.tile_cost;
+    *cost = ctx->tile_cost.get();
     return GS_OK;
   }
   for (size_t i = 0; i < ctx->cams_layouts.size(); ++i)
-    if (ctx->cams_layouts[i] == *layout) { *cost = ctx->cams_tile_cost + ctx->cams_layout_base[i]; return GS_OK; }
+    if (ctx->cams_layouts[i] == *layout) { *cost = ctx->cams_tile_cost.get() + ctx->cams_layout_base[i]; return GS_OK; }
   if (ctx->cams_layouts.size() >= kCameraLayouts) { ctx->cams_layouts.clear(); ctx->cams_layout_base.clear(); ctx->cams_cost_used = 0; }
   const size_t need = ctx->cams_cost_used + tiles;
-  if (need > ctx->cams_cost_cap) {   // grown with the histories kept
-    uint32_t *grown = nullptr;
-    const size_t cap = std::max(need, 2 * ctx->cams_cost_cap);
-    GS_CUDA_TRY(ctx, cudaMalloc(&grown, cap * 4));
-    const cudaError_t e = ctx->cams_cost_used ? cudaMemcpyAsync(grown, ctx->cams_tile_cost, ctx->cams_cost_used * 4,
-                                                                cudaMemcpyDeviceToDevice, ctx->stream)
-                                              : cudaSuccess;
-    if (e != cudaSuccess) { cudaFree(grown); return fail_cuda(ctx, e, "cudaMemcpyAsync", __FILE__, __LINE__); }
+  if (need > ctx->cams_tile_cost.size()) {   // grown with the histories kept
+    Buffer<uint32_t> grown;
+    GS_CUDA_TRY(ctx, grown.reserve(std::max(need, 2 * ctx->cams_tile_cost.size()), {ctx->stream}));
+    if (ctx->cams_cost_used)
+      GS_CUDA_TRY(ctx, cudaMemcpyAsync(grown.get(), ctx->cams_tile_cost.get(), ctx->cams_cost_used * 4, cudaMemcpyDeviceToDevice, ctx->stream));
     cudaStreamSynchronize(ctx->stream);
-    cudaFree(ctx->cams_tile_cost);
-    ctx->cams_tile_cost = grown;
-    ctx->cams_cost_cap = cap;
+    std::swap(ctx->cams_tile_cost, grown);   // the old buffer is freed with `grown`
   }
-  GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->cams_tile_cost + ctx->cams_cost_used, 0, (size_t)tiles * 4, ctx->stream));
+  GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->cams_tile_cost.get() + ctx->cams_cost_used, 0, (size_t)tiles * 4, ctx->stream));
   ctx->cams_layouts.push_back(*layout);
   ctx->cams_layout_base.push_back(ctx->cams_cost_used);
-  *cost = ctx->cams_tile_cost + ctx->cams_cost_used;
+  *cost = ctx->cams_tile_cost.get() + ctx->cams_cost_used;
   ctx->cams_cost_used = need;
   return GS_OK;
 }
@@ -468,14 +393,14 @@ int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, G
   if ((rc = bind_depth(ctx, fp, &depth))) return rc;
   BinScratch lists;
   int bin_launches = 0, more = 0;
-  GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order, as->rect, as->block_bits, n, first, ctx->bin, ctx->sort, ctx->stream, &lists,
+  GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order, as->rect, as->block_bits, n, first, bin_scratch(ctx), sort_scratch(ctx), ctx->stream, &lists,
                                   &bin_launches));
   bool again = false;
   if ((rc = grow_bin_list(ctx, fc, n, &again))) return rc;
   if (again) {
     // the grown list fits: the flag this draw set is cleared again, unless an earlier draw of the call left its list truncated
     const bool clear = first || !ctx->bin_overflow;
-    GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order, as->rect, as->block_bits, n, clear, ctx->bin, ctx->sort, ctx->stream, &lists,
+    GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order, as->rect, as->block_bits, n, clear, bin_scratch(ctx), sort_scratch(ctx), ctx->stream, &lists,
                                     &more));
     bin_launches += more;
     ctx->bin_overflow = !clear;
@@ -566,7 +491,7 @@ cudaError_t asset_init_work(GsContext *ctx, GsAsset *as, uint32_t n, uint32_t po
 
 static int check_bin_overflow(GsContext *ctx) {
   uint32_t ec[2] = {0, 0};
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ec, ctx->bin.entry_count, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ec, ctx->bin_entry_count.get(), 8, cudaMemcpyDeviceToHost, ctx->stream));
   GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   ctx->times.tile_entries = ec[0];
   if (ec[1]) return fail(ctx, GS_ERR_OUT_OF_MEMORY, "tile-list capacity exceeded (splat footprints cover too many tiles)");
@@ -608,11 +533,11 @@ int gs_create(int cuda_device, void *stream_handle, GsContext **out) {
       ctx->own_stream = true;
     }
     for (int i = 0; i < EV_COUNT; ++i) GS_CUDA_TRY(ctx, cudaEventCreate(&ctx->ev[i]));
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->sort.ghist, 4 * 256 * 4));
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->sort.tickets, 4 * 4));
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->d_scalar, 16 * 4));
-    GS_CUDA_TRY(ctx, cudaMalloc(&ctx->bin.entry_count, 4 * 4));
-    GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->bin.entry_count, 0, 16, ctx->stream));
+    GS_CUDA_TRY(ctx, ctx->sort_ghist.reserve(4 * 256, {ctx->stream}));
+    GS_CUDA_TRY(ctx, ctx->sort_tickets.reserve(4, {ctx->stream}));
+    GS_CUDA_TRY(ctx, ctx->d_scalar.reserve(16, {ctx->stream}));
+    GS_CUDA_TRY(ctx, ctx->bin_entry_count.reserve(4, {ctx->stream}));
+    GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->bin_entry_count.get(), 0, 16, ctx->stream));
     return GS_OK;
   };
   const int rc = init();
@@ -629,14 +554,8 @@ void gs_destroy(GsContext *ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-  cudaFree(ctx->sort.alt_keys); cudaFree(ctx->sort.alt_vals); cudaFree(ctx->sort.lookback);
-  cudaFree(ctx->sort.ghist); cudaFree(ctx->sort.tickets); cudaFree(ctx->d_scalar);
-  cudaFree(ctx->bin.bin_ranges); cudaFree(ctx->bin.tile_cost); cudaFree(ctx->bin.tile_order); cudaFree(ctx->bin.block_sums); cudaFree(ctx->bin.entry_count); cudaFree(ctx->bin.tile_keys); cudaFree(ctx->bin.tile_vals);
-  cudaFree(ctx->rt_scratch); cudaFree(ctx->tgt_scratch); cudaFree(ctx->d_cutouts); cudaFree(ctx->d_deleted); cudaFree(ctx->d_selected); cudaFree(ctx->d_depth);
-  cudaFree(ctx->cams_ghist); cudaFree(ctx->cams_scratch); cudaFree(ctx->cams_tile_cost);
   if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
   for (int i = 0; i < 2; ++i) {
-    cudaFree(ctx->rt_async[i]);
     if (ctx->ev_rt_ready[i]) cudaEventDestroy(ctx->ev_rt_ready[i]);
     if (ctx->ev_copy_done[i]) cudaEventDestroy(ctx->ev_copy_done[i]);
   }
@@ -644,7 +563,7 @@ void gs_destroy(GsContext *ctx) {
   release_surfaces(ctx, true);   // waits for each batch's event (a group's transfer stream may still hold one)
   for (cudaEvent_t e : ctx->spare_events) cudaEventDestroy(e);
   if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
-  delete ctx;
+  delete ctx;   // frees the scratch buffers, on the context's device
 }
 
 int gs_sync(GsContext *ctx) {
@@ -682,7 +601,7 @@ int gs_get_stage_times(GsContext *ctx, GsStageTimes *out) {
   for (int e = EV_VIEW1; e < EV_COUNT; ++e) if (ctx->ev_valid[e]) last = e;
   t.total_ms = ev_ms(ctx, first, last);
   uint32_t ec[2] = {0, 0};
-  if (ctx->bin.entry_count) cudaMemcpy(ec, ctx->bin.entry_count, 8, cudaMemcpyDeviceToHost);
+  if (ctx->bin_entry_count.get()) cudaMemcpy(ec, ctx->bin_entry_count.get(), 8, cudaMemcpyDeviceToHost);
   t.tile_entries = ec[0];
   t.kernel_launches = ctx->launches;
   *out = t;
@@ -804,10 +723,10 @@ int gs_render(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRend
     return do_draw(ctx, fc, opt, as, fp, true, nullptr, 0, rt->format, so);
   }
   const uint32_t tight = W * pix_bytes(rt->format);
-  if ((rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)tight * H))) return rc;
-  if ((rc = init_staging(ctx, opt, ctx->rt_scratch, tight, W, H, rt->format, rt, pitch))) return rc;
-  if ((rc = do_draw(ctx, fc, opt, as, fp, true, ctx->rt_scratch, tight, rt->format))) return rc;
-  GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, pitch, ctx->rt_scratch, tight, tight, H, cudaMemcpyDeviceToHost, ctx->stream));
+  GS_CUDA_TRY(ctx, ctx->rt_scratch.reserve((size_t)tight * H, {ctx->stream}));
+  if ((rc = init_staging(ctx, opt, ctx->rt_scratch.get(), tight, W, H, rt->format, rt, pitch))) return rc;
+  if ((rc = do_draw(ctx, fc, opt, as, fp, true, ctx->rt_scratch.get(), tight, rt->format))) return rc;
+  GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, pitch, ctx->rt_scratch.get(), tight, tight, H, cudaMemcpyDeviceToHost, ctx->stream));
   return check_bin_overflow(ctx);
 }
 
@@ -827,10 +746,10 @@ static int composite_impl(GsContext *ctx, CallSurfaces &surfs, const void *d_rt,
     launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, nullptr, 0, so, tgt->format, W, H, s);
   } else {
     const uint32_t tight = W * pix_bytes(tgt->format);
-    if ((rc = grow(ctx, &ctx->tgt_scratch, &ctx->tgt_bytes, (size_t)tight * H))) return rc;
-    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->tgt_scratch, tight, tgt->data, tp, tight, H, cudaMemcpyHostToDevice, s));
-    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, ctx->tgt_scratch, tight, 0, tgt->format, W, H, s);
-    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(tgt->data, tp, ctx->tgt_scratch, tight, tight, H, cudaMemcpyDeviceToHost, s));
+    GS_CUDA_TRY(ctx, ctx->tgt_scratch.reserve((size_t)tight * H, {ctx->stream}));
+    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->tgt_scratch.get(), tight, tgt->data, tp, tight, H, cudaMemcpyHostToDevice, s));
+    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, ctx->tgt_scratch.get(), tight, 0, tgt->format, W, H, s);
+    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(tgt->data, tp, ctx->tgt_scratch.get(), tight, tight, H, cudaMemcpyDeviceToHost, s));
   }
   if (s == ctx->stream) rec(ctx, EV_COMP1);
   ctx->launches += 1;
@@ -856,9 +775,9 @@ int gs_composite(GsContext *ctx, const GsImage *rt, GsImage *tgt) {
     return composite_impl(ctx, surfs, nullptr, 0, so, rt->format, tgt, W, H, ctx->stream);
   }
   const uint32_t tight = W * pix_bytes(rt->format);
-  if ((rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)tight * H))) return rc;
-  GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->rt_scratch, tight, rt->data, rp, tight, H, cudaMemcpyHostToDevice, ctx->stream));
-  return composite_impl(ctx, surfs, ctx->rt_scratch, tight, 0, rt->format, tgt, W, H, ctx->stream);
+  GS_CUDA_TRY(ctx, ctx->rt_scratch.reserve((size_t)tight * H, {ctx->stream}));
+  GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->rt_scratch.get(), tight, rt->data, rp, tight, H, cudaMemcpyHostToDevice, ctx->stream));
+  return composite_impl(ctx, surfs, ctx->rt_scratch.get(), tight, 0, rt->format, tgt, W, H, ctx->stream);
 }
 
 }  // extern "C"
@@ -891,14 +810,13 @@ static int begin_frame_image(GsContext *ctx, CallSurfaces &surfs, const GsRender
     fi->pitch = W * pix_bytes(rt_fmt);
     // the staging image of two frames ago: its copy must have left the device before this frame's raster overwrites it
     if (ctx->copy_pending[slot]) GS_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy_done[slot], 0));
-    if (ctx->rt_async_bytes[slot] < (size_t)fi->pitch * H && ctx->copy_pending[slot]) GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->copy_stream));  // about to be freed
-    if ((rc = grow(ctx, &ctx->rt_async[slot], &ctx->rt_async_bytes[slot], (size_t)fi->pitch * H))) return rc;
-    fi->d_rt = ctx->rt_async[slot];
+    GS_CUDA_TRY(ctx, ctx->rt_async[slot].reserve((size_t)fi->pitch * H, {ctx->stream, ctx->copy_stream}));
+    fi->d_rt = ctx->rt_async[slot].get();
     if ((rc = init_staging(ctx, opt, fi->d_rt, fi->pitch, W, H, rt_fmt, rt, rt_pitch))) return rc;
   } else {
     fi->pitch = W * pix_bytes(rt_fmt);
-    if (!staging && (rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)fi->pitch * H))) return rc;
-    fi->d_rt = staging ? staging : ctx->rt_scratch;
+    if (!staging) GS_CUDA_TRY(ctx, ctx->rt_scratch.reserve((size_t)fi->pitch * H, {ctx->stream}));
+    fi->d_rt = staging ? staging : ctx->rt_scratch.get();
     if ((rc = init_staging(ctx, opt, fi->d_rt, fi->pitch, W, H, rt_fmt, rt, rt_pitch))) return rc;
   }
   return GS_OK;
@@ -1095,12 +1013,12 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
     if (cams_run && (!c.rt || c.rt->memory == GS_MEM_HOST)) { stage_at[i] = bytes; bytes += align256((size_t)c.W * pix_bytes(c.rt_fmt) * c.H); }
   }
   int rc = GS_OK;
-  if (bytes && (rc = grow(ctx, &ctx->cams_scratch, &ctx->cams_bytes, bytes))) return rc;
-  uint8_t *scratch = static_cast<uint8_t *>(ctx->cams_scratch);
+  GS_CUDA_TRY(ctx, ctx->cams_scratch.reserve(bytes, {ctx->stream}));
+  uint8_t *scratch = ctx->cams_scratch.get();
   const uint32_t n = (uint32_t)std::min<uint64_t>(total, 0xFFFFFFFFu);
   uint32_t *tile_cost = nullptr;
   if (multi) {
-    if (!ctx->cams_ghist) GS_CUDA_TRY(ctx, cudaMalloc(&ctx->cams_ghist, 4 * 256 * sizeof(uint32_t)));
+    GS_CUDA_TRY(ctx, ctx->cams_ghist.reserve(4 * 256, {ctx->stream}));
     if ((rc = ensure_bin_scratch(ctx, n, bins, 0))) return rc;
     if ((rc = tile_history(ctx, tiles, cams_run ? &layout : nullptr, &tile_cost))) return rc;
     for (uint32_t i = 0; i < run.size(); ++i) {
@@ -1111,7 +1029,7 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
                                          cudaMemcpyHostToDevice, ctx->stream));
       }
     }
-    launch_bin_list_begin(ctx->bin, ctx->cams_ghist, ctx->stream);
+    launch_bin_list_begin(bin_scratch(ctx), ctx->cams_ghist.get(), ctx->stream);
   }
 
   DrawObjects objs;
@@ -1123,7 +1041,7 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
       const GsAsset *as = assets[pair_at[emitted]];
       const RasterCamera &r = dc.cam[seg_of[emitted]];
       launch_bin_emit_pair(as->order, as->rect, as->block_bits, as->av.n, r.binsX, r.bin_base, emitted, clear && emitted == 0, bins,
-                           ctx->bin, ctx->cams_ghist, ctx->stream);
+                           bin_scratch(ctx), ctx->cams_ghist.get(), ctx->stream);
       ctx->launches += 2;   // look-back clear, bin_emit
     }
   };
@@ -1165,15 +1083,15 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
     emit_to(count, first);
     BinScratch lists;
     int sort_launches = 0, more = 0;
-    GS_CUDA_TRY(ctx, launch_bin_list_sort(bins, ctx->bin, ctx->sort, ctx->cams_ghist, ctx->stream, &lists, &sort_launches));
+    GS_CUDA_TRY(ctx, launch_bin_list_sort(bins, bin_scratch(ctx), sort_scratch(ctx), ctx->cams_ghist.get(), ctx->stream, &lists, &sort_launches));
     bool again = false;
     if (!cams_run && (rc = grow_bin_list(ctx, cams[run[0].cam].fcs[0], n, &again))) return rc;
     if (again) {   // as in do_draw
       const bool clear = first || !ctx->bin_overflow;
-      launch_bin_list_begin(ctx->bin, ctx->cams_ghist, ctx->stream);
+      launch_bin_list_begin(bin_scratch(ctx), ctx->cams_ghist.get(), ctx->stream);
       emitted = 0;
       emit_to(count, clear);
-      GS_CUDA_TRY(ctx, launch_bin_list_sort(bins, ctx->bin, ctx->sort, ctx->cams_ghist, ctx->stream, &lists, &more));
+      GS_CUDA_TRY(ctx, launch_bin_list_sort(bins, bin_scratch(ctx), sort_scratch(ctx), ctx->cams_ghist.get(), ctx->stream, &lists, &more));
       sort_launches += more;
       ctx->bin_overflow = !clear;
     }
@@ -1199,7 +1117,7 @@ static int draw_cameras(GsContext *ctx, std::vector<CameraArgs> &cams, GsAsset *
   // the objects' cutouts / bits share the context's buffers: sized for all of them before the first view-calc is queued
   const uint32_t pairs = cams.back().off + cams.back().K;
   for (uint32_t p = 0; p < pairs; ++p)
-    if ((rc = reserve_frame_inputs(ctx, assets[p], &fps[p]))) return rc;
+    if ((rc = reserve_frame_inputs(ctx, assets[p], &fps[p], {ctx->stream}))) return rc;
   for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
   CallSurfaces surfs(ctx);
   const std::vector<Run> runs = form_runs(cams, assets, fps);
@@ -1210,7 +1128,7 @@ static int draw_cameras(GsContext *ctx, std::vector<CameraArgs> &cams, GsAsset *
     if (grows && r > 0 && !flag_read) {
       // a grown list clears the overflow flag unless an earlier draw of the call was truncated (do_draw): read it first
       uint32_t flag = 0;
-      GS_CUDA_TRY(ctx, cudaMemcpyAsync(&flag, ctx->bin.entry_count + 1, 4, cudaMemcpyDeviceToHost, ctx->stream));
+      GS_CUDA_TRY(ctx, cudaMemcpyAsync(&flag, ctx->bin_entry_count.get() + 1, 4, cudaMemcpyDeviceToHost, ctx->stream));
       GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
       ctx->bin_overflow = flag != 0;
     }
@@ -1302,10 +1220,10 @@ int gs_unshuffle_bands(GsContext *ctx, const void *gathered, uint32_t parts, uin
     return GS_OK;
   }
   const uint32_t tight = W * pix_bytes(fmt);
-  if ((rc = grow(ctx, &ctx->rt_scratch, &ctx->rt_bytes, (size_t)tight * H))) return rc;
-  launch_unshuffle(gathered, parts, band_rows, rows_pp, fmt, ctx->rt_scratch, tight, W, H, ctx->stream);
+  GS_CUDA_TRY(ctx, ctx->rt_scratch.reserve((size_t)tight * H, {ctx->stream}));
+  launch_unshuffle(gathered, parts, band_rows, rows_pp, fmt, ctx->rt_scratch.get(), tight, W, H, ctx->stream);
   ctx->launches += 1;
-  GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(out->data, pitch, ctx->rt_scratch, tight, tight, H, cudaMemcpyDeviceToHost, ctx->stream));
+  GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(out->data, pitch, ctx->rt_scratch.get(), tight, tight, H, cudaMemcpyDeviceToHost, ctx->stream));
   GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return GS_OK;
 }
@@ -1317,11 +1235,11 @@ int gs_sort_pairs_device(GsContext *ctx, uint32_t *d_keys, uint32_t *d_payload, 
   if (count >= (1u << 30)) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "count must be < 2^30");
   int rc = ensure_sort_scratch(ctx, count);
   if (rc) return rc;
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_scalar, &count, 4, cudaMemcpyHostToDevice, ctx->stream));
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_scalar.get(), &count, 4, cudaMemcpyHostToDevice, ctx->stream));
   for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
   cudaEvent_t pe[5] = {ctx->ev[EV_SORT0], ctx->ev[EV_SORT1], ctx->ev[EV_SORT2], ctx->ev[EV_SORT3], ctx->ev[EV_SORT4]};
   rec(ctx, EV_BEGIN);
-  GS_CUDA_TRY(ctx, launch_sort_pairs(d_keys, d_payload, ctx->d_scalar, count, 4, 8, false, ctx->sort, ctx->stream, ctx->timing ? pe : nullptr));
+  GS_CUDA_TRY(ctx, launch_sort_pairs(d_keys, d_payload, ctx->d_scalar.get(), count, 4, 8, false, sort_scratch(ctx), ctx->stream, ctx->timing ? pe : nullptr));
   if (ctx->timing) for (int e = EV_SORT0; e <= EV_SORT4; ++e) ctx->ev_valid[e] = true;
   ctx->launches += 5;
   GS_CUDA_TRY(ctx, cudaGetLastError());
@@ -1375,7 +1293,7 @@ int gs_export_splats(GsContext *ctx, GsAsset *as, const GsCutout *cutouts, uint3
   float *d_out = nullptr;
   const size_t bytes = (size_t)as->av.n * 62 * sizeof(float);
   GS_CUDA_TRY(ctx, cudaMalloc(&d_out, bytes));
-  launch_export_data(as->av, cutout_count, ctx->d_cutouts, d_out, ctx->stream);
+  launch_export_data(as->av, cutout_count, ctx->d_cutouts.get(), d_out, ctx->stream);
   ctx->launches += 1;
   cudaError_t e = cudaMemcpyAsync(dst, d_out, bytes, cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);

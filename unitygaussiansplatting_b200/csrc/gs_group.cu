@@ -50,19 +50,16 @@ struct Member {
   cudaEvent_t ev_begin = nullptr, ev_view = nullptr, ev_info = nullptr, ev_cost[2] = {nullptr, nullptr};
   cudaEvent_t ev_produced = nullptr, ev_consumed = nullptr;   // emulated exchange
   cudaEvent_t tev[GT_COUNT]{};
-  uint32_t *d_info = nullptr, *d_slab_count = nullptr, *d_cmp_status = nullptr, *d_row_cost = nullptr;
-  uint32_t *d_gather = nullptr;   // staging of the order exchange: G slabs of `cap` ids each (the all-gather's buffer)
-  size_t gather_words = 0;
-  size_t cmp_words = 0;
-  uint32_t rows_cap = 0;
-  uint32_t *h_info = nullptr, *h_row_cost[2] = {nullptr, nullptr};   // pinned
-  uint32_t info_slots = 1;             // slab tables d_info / h_info hold: one per splat object of a call
-  uint32_t *d_ghist_more = nullptr;    // the distance kernel's digit histograms of objects 1.. of a call (object 0: the context's)
-  uint32_t ghist_more_slots = 0;
+  // scratch, freed by member_free on the member's device
+  struct Scratch {
+    Buffer<uint32_t> info, slab_count, cmp_status, row_cost;
+    Buffer<uint32_t, true> h_info, h_row_cost[2];   // pinned host copies of info / row_cost
+    Buffer<uint32_t> gather;       // staging of the order exchange: G slabs of `cap` ids each (the all-gather's buffer)
+    Buffer<uint32_t> ghist_more;   // the distance kernel's digit histograms of objects 1.. of a call (object 0: the context's)
+    Buffer<uint8_t> rt;            // the image, without a device render target
+  } buf;
   std::vector<cudaEvent_t> obj_tev;    // timing, per object of the last call: [2k] its draw begins, [2k + 1] its binning ends
   uint32_t obj_timed = 0;              // objects of the last call whose draw was timed here
-  void *rt_scratch = nullptr;
-  size_t rt_bytes = 0;
 };
 
 // One splat object of a gs_group_frame_objects call: its assets on the local members, its uniforms, and what the call derives
@@ -136,9 +133,9 @@ int member_init(Member &mb) {
   cudaEvent_t *evs[] = {&mb.ev_begin, &mb.ev_view, &mb.ev_info, &mb.ev_cost[0], &mb.ev_cost[1], &mb.ev_produced, &mb.ev_consumed, &mb.ev_raster, &mb.ev_image};
   for (cudaEvent_t *e : evs) GS_CUDA_TRY(ctx, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
   for (int i = 0; i < GT_COUNT; ++i) GS_CUDA_TRY(ctx, cudaEventCreate(&mb.tev[i]));
-  GS_CUDA_TRY(ctx, cudaMalloc(&mb.d_info, 2 * kMaxSlabs * 4));
-  GS_CUDA_TRY(ctx, cudaMalloc(&mb.d_slab_count, 16));
-  GS_CUDA_TRY(ctx, cudaMallocHost(&mb.h_info, 2 * kMaxSlabs * 4));
+  GS_CUDA_TRY(ctx, mb.buf.info.reserve(2 * kMaxSlabs, {ctx->stream}));
+  GS_CUDA_TRY(ctx, mb.buf.slab_count.reserve(4, {ctx->stream}));
+  GS_CUDA_TRY(ctx, mb.buf.h_info.reserve(2 * kMaxSlabs, {ctx->stream}));
   return GS_OK;
 }
 
@@ -152,24 +149,18 @@ void member_free(Member &mb) {
   for (cudaEvent_t e : evs) if (e) cudaEventDestroy(e);
   for (int i = 0; i < GT_COUNT; ++i) if (mb.tev[i]) cudaEventDestroy(mb.tev[i]);
   for (cudaEvent_t e : mb.obj_tev) cudaEventDestroy(e);
-  cudaFree(mb.d_ghist_more);
-  cudaFree(mb.d_info); cudaFree(mb.d_slab_count); cudaFree(mb.d_cmp_status); cudaFree(mb.d_row_cost); cudaFree(mb.rt_scratch); cudaFree(mb.d_gather);
-  cudaFreeHost(mb.h_info); cudaFreeHost(mb.h_row_cost[0]); cudaFreeHost(mb.h_row_cost[1]);
+  mb.buf = Member::Scratch();
   if (mb.comm && nccl_api().ok()) nccl_api().CommDestroy(mb.comm);
   if (mb.own_ctx) gs_destroy(mb.ctx);
   mb.ctx = nullptr;
 }
 
-int member_rows(Member &mb, uint32_t rows) {   // row-cost vectors for a screen of `rows` 16-pixel rows
-  if (rows <= mb.rows_cap) return GS_OK;
+// row-cost vectors for a screen of `rows` 16-pixel rows: the last call's k_row_costs and read-back use them on the transfer stream
+int member_rows(Member &mb, uint32_t rows) {
   GsContext *ctx = mb.ctx;
-  cudaStreamSynchronize(ctx->stream);
-  cudaFree(mb.d_row_cost); cudaFreeHost(mb.h_row_cost[0]); cudaFreeHost(mb.h_row_cost[1]);
-  mb.d_row_cost = nullptr; mb.h_row_cost[0] = mb.h_row_cost[1] = nullptr; mb.rows_cap = 0;
-  GS_CUDA_TRY(ctx, cudaMalloc(&mb.d_row_cost, (size_t)rows * 4));
-  GS_CUDA_TRY(ctx, cudaMallocHost(&mb.h_row_cost[0], (size_t)rows * 4));
-  GS_CUDA_TRY(ctx, cudaMallocHost(&mb.h_row_cost[1], (size_t)rows * 4));
-  mb.rows_cap = rows;
+  GS_CUDA_TRY(ctx, mb.buf.row_cost.reserve(rows, {ctx->stream, mb.xfer}));
+  GS_CUDA_TRY(ctx, mb.buf.h_row_cost[0].reserve(rows, {ctx->stream, mb.xfer}));
+  GS_CUDA_TRY(ctx, mb.buf.h_row_cost[1].reserve(rows, {ctx->stream, mb.xfer}));
   return GS_OK;
 }
 
@@ -179,36 +170,17 @@ int member_asset(Member &mb, GsAsset *as) {   // per-asset buffers only the grou
   if (!as->slab_mask) GS_CUDA_TRY(ctx, cudaMalloc(&as->slab_mask, ((size_t)(n + 1023) / 1024) * 128 + 64));
   if (!as->order_tmp) GS_CUDA_TRY(ctx, cudaMalloc(&as->order_tmp, (size_t)n * 4 + 16));
   if (!as->slab_group_bits) GS_CUDA_TRY(ctx, cudaMalloc(&as->slab_group_bits, group_bits_words(n) * 4 + 64));
-  const size_t words = compact_status_words(n);
-  if (words > mb.cmp_words) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(mb.d_cmp_status);
-    mb.d_cmp_status = nullptr; mb.cmp_words = 0;
-    GS_CUDA_TRY(ctx, cudaMalloc(&mb.d_cmp_status, words * 4));
-    mb.cmp_words = words;
-  }
+  GS_CUDA_TRY(ctx, mb.buf.cmp_status.reserve(compact_status_words(n), {ctx->stream}));
   return ensure_sort_scratch(ctx, n);
 }
 
 // per-object scratch of a call with `objects` splat objects: slab tables, digit histograms, timing events
 int member_objects(Member &mb, uint32_t objects, bool timing) {
   GsContext *ctx = mb.ctx;
-  const size_t table = 2 * kMaxSlabs * 4;
-  if (objects > mb.info_slots) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(mb.d_info); cudaFreeHost(mb.h_info);
-    mb.d_info = nullptr; mb.h_info = nullptr; mb.info_slots = 0;
-    GS_CUDA_TRY(ctx, cudaMalloc(&mb.d_info, objects * table));
-    GS_CUDA_TRY(ctx, cudaMallocHost(&mb.h_info, objects * table));
-    mb.info_slots = objects;
-  }
-  if (objects - 1 > mb.ghist_more_slots) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(mb.d_ghist_more);
-    mb.d_ghist_more = nullptr; mb.ghist_more_slots = 0;
-    GS_CUDA_TRY(ctx, cudaMalloc(&mb.d_ghist_more, (size_t)(objects - 1) * 4 * 256 * 4));
-    mb.ghist_more_slots = objects - 1;
-  }
+  const size_t table = 2 * kMaxSlabs;
+  GS_CUDA_TRY(ctx, mb.buf.info.reserve(objects * table, {ctx->stream}));
+  GS_CUDA_TRY(ctx, mb.buf.h_info.reserve(objects * table, {ctx->stream}));
+  GS_CUDA_TRY(ctx, mb.buf.ghist_more.reserve((size_t)(objects - 1) * 4 * 256, {ctx->stream}));
   while (timing && mb.obj_tev.size() < 2 * (size_t)objects) {
     cudaEvent_t e = nullptr;
     GS_CUDA_TRY(ctx, cudaEventCreate(&e));
@@ -436,7 +408,7 @@ int gs_group_row_costs(GsGroup *g, uint32_t *out, uint32_t rows) {
   const int slot = (int)((g->hist_frames - 1) & 1u);   // written by the last call, after its row exchange
   GS_CUDA_TRY(m0.ctx, cudaSetDevice(m0.ctx->device));
   GS_CUDA_TRY(m0.ctx, cudaEventSynchronize(m0.ev_cost[slot]));
-  memcpy(out, m0.h_row_cost[slot], (size_t)rows * 4);
+  memcpy(out, m0.buf.h_row_cost[slot].get(), (size_t)rows * 4);
   return GS_OK;
 }
 
@@ -635,7 +607,7 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
   else if (g->hist_frames >= 2) {
     Member &m0 = g->m[0];
     GS_CUDA_TRY(m0.ctx, cudaEventSynchronize(m0.ev_cost[slot]));   // written by call hist_frames - 2: long done
-    balance_rows(m0.h_row_cost[slot], rows, G, g->bounds);
+    balance_rows(m0.buf.h_row_cost[slot].get(), rows, G, g->bounds);
   } else {
     balance_rows(nullptr, rows, G, g->bounds);
   }
@@ -650,7 +622,7 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
     // the objects' cutouts / bits share the context's buffers: sized for all of them before the first view-calc is queued, so
     // the uploads (behind each other on the second stream) never reallocate under a view-calc that reads them
     for (GroupObject &o : obj)
-      if ((rc = member_asset(mb, o.assets[i])) || (rc = reserve_frame_inputs(ctx, o.assets[i], o.fp, mb.aux))) return rc;
+      if ((rc = member_asset(mb, o.assets[i])) || (rc = reserve_frame_inputs(ctx, o.assets[i], o.fp, {ctx->stream, mb.aux}))) return rc;
     for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
     GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_begin, ctx->stream));
     if (timing) cudaEventRecord(mb.tev[GT_BEGIN], ctx->stream);
@@ -663,8 +635,8 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
       GsAsset *as = o.assets[i];
       if (o.sort) {
         // each object has its own digit histograms and slab table: all distance kernels run before the one host wait
-        uint32_t *ghist = k ? mb.d_ghist_more + (size_t)(k - 1) * 4 * 256 : ctx->sort.ghist;
-        uint32_t *info = mb.d_info + (size_t)k * 2 * kMaxSlabs;
+        uint32_t *ghist = k ? mb.buf.ghist_more.get() + (size_t)(k - 1) * 4 * 256 : ctx->sort_ghist.get();
+        uint32_t *info = mb.buf.info.get() + (size_t)k * 2 * kMaxSlabs;
         SlabArgs sl;
         memset(&sl, 0, sizeof(sl));
         sl.count = G; sl.index = mb.rank; sl.order_prev = as->order; sl.mask = as->slab_mask; sl.group_bits = as->slab_group_bits; sl.info = info;
@@ -674,7 +646,7 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
         launch_calc_distances(as->av, o.fc, as->key_table, ghist, ctx->stream, &sl);
         ctx->launches += 1;
         if (G > 1) {
-          GS_CUDA_TRY(ctx, cudaMemcpyAsync(mb.h_info + (size_t)k * 2 * kMaxSlabs, info, 2 * kMaxSlabs * 4, cudaMemcpyDeviceToHost, ctx->stream));
+          GS_CUDA_TRY(ctx, cudaMemcpyAsync(mb.buf.h_info.get() + (size_t)k * 2 * kMaxSlabs, info, 2 * kMaxSlabs * 4, cudaMemcpyDeviceToHost, ctx->stream));
           GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_info, ctx->stream));
         }
       }
@@ -708,7 +680,7 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
     for (uint32_t k = 0; k < K; ++k) {
       GroupObject &o = obj[k];
       if (!o.sort) continue;
-      const uint32_t *info = mb.h_info + (size_t)k * 2 * kMaxSlabs;
+      const uint32_t *info = mb.buf.h_info.get() + (size_t)k * 2 * kMaxSlabs;
       uint32_t off[GS_GROUP_MAX_GPUS + 1];
       off[0] = 0;
       for (uint32_t c = 1; c < G; ++c) {
@@ -756,13 +728,9 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
     }
     for (size_t i = 0; i < L && need; ++i) {
       Member &mb = g->m[i];
-      if (need <= mb.gather_words) continue;
+      if (need <= mb.buf.gather.size()) continue;
       GS_CUDA_TRY(mb.ctx, cudaSetDevice(mb.ctx->device));
-      cudaStreamSynchronize(mb.ctx->stream);
-      cudaFree(mb.d_gather);
-      mb.d_gather = nullptr; mb.gather_words = 0;
-      GS_CUDA_TRY(mb.ctx, cudaMalloc(&mb.d_gather, words * 4));
-      mb.gather_words = words;
+      GS_CUDA_TRY(mb.ctx, mb.buf.gather.reserve(words, {mb.ctx->stream}));
     }
     for (uint32_t k = 0; k < K; ++k) {
       const GroupObject &o = obj[k];
@@ -780,18 +748,18 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
         GsContext *ctx = mb.ctx;
         GsAsset *as = o.assets[i];
         GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-        SortScratch sc = ctx->sort;   // this object's digit histograms (the rest of the scratch is used in stream order)
-        if (k) sc.ghist = mb.d_ghist_more + (size_t)(k - 1) * 4 * 256;
+        SortScratch sc = sort_scratch(ctx);   // this object's digit histograms (the rest of the scratch is used in stream order)
+        if (k) sc.ghist = mb.buf.ghist_more.get() + (size_t)(k - 1) * 4 * 256;
         const uint32_t cnt = o.slab_cnt[mb.rank], off = o.slab_off[mb.rank];
         if (G == 1) {
           GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order, as->d_n, N, 4, 8, true, sc, ctx->stream, nullptr, as->key_table));
           ctx->launches += 4;
         } else if (cnt) {
-          launch_compact_order(as->order, N, as->slab_mask, as->slab_group_bits, as->key_table, as->order_tmp, as->keys, mb.d_cmp_status, mb.d_slab_count,
-                               ctx->stream);
-          GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order_tmp, mb.d_slab_count, cnt, 4, 8, true, sc, ctx->stream, nullptr, nullptr,
+          launch_compact_order(as->order, N, as->slab_mask, as->slab_group_bits, as->key_table, as->order_tmp, as->keys, mb.buf.cmp_status.get(),
+                               mb.buf.slab_count.get(), ctx->stream);
+          GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order_tmp, mb.buf.slab_count.get(), cnt, 4, 8, true, sc, ctx->stream, nullptr, nullptr,
                                              true, as->keys + off,
-                                             use_p2p ? p2p_new + off : use_gather ? mb.d_gather + (size_t)mb.rank * cap : as->order + off));
+                                             use_p2p ? p2p_new + off : use_gather ? mb.buf.gather.get() + (size_t)mb.rank * cap : as->order + off));
           ctx->launches += 5;
         }
         if (use_p2p) {
@@ -818,14 +786,14 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
         if (use_p2p) {
           // delivered by k_push_slab / awaited by k_wait_slabs above
         } else if (use_gather) {
-          for (size_t i = 0; i < L; ++i) bufs[i] = reinterpret_cast<uint8_t *>(g->m[i].d_gather);
+          for (size_t i = 0; i < L; ++i) bufs[i] = reinterpret_cast<uint8_t *>(g->m[i].buf.gather.get());
           if ((rc = exchange_allgather(g, bufs.data(), (size_t)cap * 4, cnt))) return rc;
           for (size_t i = 0; i < L; ++i) {   // slot c's ids -> their place in the order: G device copies (a copy kernel that found
             Member &mb = g->m[i];            // each element's slab was measured slower than the copy engine)
             GS_CUDA_TRY(mb.ctx, cudaSetDevice(mb.ctx->device));
             for (uint32_t c = 0; c < G; ++c)
               if (o.slab_cnt[c])
-                GS_CUDA_TRY(mb.ctx, cudaMemcpyAsync(o.assets[i]->order + o.slab_off[c], mb.d_gather + (size_t)c * cap, (size_t)o.slab_cnt[c] * 4,
+                GS_CUDA_TRY(mb.ctx, cudaMemcpyAsync(o.assets[i]->order + o.slab_off[c], mb.buf.gather.get() + (size_t)c * cap, (size_t)o.slab_cnt[c] * 4,
                                                     cudaMemcpyDeviceToDevice, mb.ctx->stream));
           }
         } else {
@@ -845,18 +813,12 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
     GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     const uint32_t pitch = pitches[i];
     void *d_rt = dev_rt[i];
-    if (!d_rt) {
-      if (mb.rt_bytes < (size_t)pitch * H) {
-        cudaStreamSynchronize(ctx->stream);
-        cudaFree(mb.rt_scratch);
-        mb.rt_scratch = nullptr; mb.rt_bytes = 0;
-        GS_CUDA_TRY(ctx, cudaMalloc(&mb.rt_scratch, (size_t)pitch * H));
-        mb.rt_bytes = (size_t)pitch * H;
-      }
-      d_rt = mb.rt_scratch;
+    if (!d_rt) {   // read by the row exchange and the read-back on the transfer stream
+      GS_CUDA_TRY(ctx, mb.buf.rt.reserve((size_t)pitch * H, {ctx->stream, mb.xfer}));
+      d_rt = mb.buf.rt.get();
     }
     img[i] = reinterpret_cast<uint8_t *>(d_rt);
-    costs[i] = reinterpret_cast<uint8_t *>(mb.d_row_cost);
+    costs[i] = reinterpret_cast<uint8_t *>(mb.buf.row_cost.get());
     GsRenderOptions opt = base;
     opt.row_begin = g->bounds[mb.rank]; opt.row_end = g->bounds[mb.rank + 1];
     mb.obj_timed = 0;
@@ -876,7 +838,7 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
           return rc;
         ctx->launches += 1;   // k_row_costs: here for every object but the last (before the next one's raster overwrites the
                               // tile costs), on the transfer stream below for the last
-        if (k + 1 < K) launch_row_costs(ctx->bin.tile_cost, ntx, g->bounds[mb.rank], g->bounds[mb.rank + 1], mb.d_row_cost, ctx->stream, k > 0);
+        if (k + 1 < K) launch_row_costs(ctx->tile_cost.get(), ntx, g->bounds[mb.rank], g->bounds[mb.rank + 1], mb.buf.row_cost.get(), ctx->stream, k > 0);
       }
       mb.obj_timed = timing ? K : 0;
     } else if (timing) {
@@ -893,7 +855,7 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
     GS_CUDA_TRY(mb.ctx, cudaEventRecord(mb.ev_raster, mb.ctx->stream));
     GS_CUDA_TRY(mb.ctx, cudaStreamWaitEvent(mb.xfer, mb.ev_raster, 0));
     if (g->bounds[mb.rank + 1] > g->bounds[mb.rank] || G == 1)   // the measured cost of my rows, for the balancer two calls on
-      launch_row_costs(mb.ctx->bin.tile_cost, ntx, g->bounds[mb.rank], g->bounds[mb.rank + 1], mb.d_row_cost, mb.xfer, K > 1);
+      launch_row_costs(mb.ctx->tile_cost.get(), ntx, g->bounds[mb.rank], g->bounds[mb.rank + 1], mb.buf.row_cost.get(), mb.xfer, K > 1);
   }
   if (G > 1) {
     size_t off[GS_GROUP_MAX_GPUS], cnt[GS_GROUP_MAX_GPUS], coff[GS_GROUP_MAX_GPUS], ccnt[GS_GROUP_MAX_GPUS];
@@ -912,7 +874,7 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
     GsContext *ctx = mb.ctx;
     GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     if (timing) cudaEventRecord(mb.tev[GT_IMAGE], mb.xfer);
-    GS_CUDA_TRY(ctx, cudaMemcpyAsync(mb.h_row_cost[slot], mb.d_row_cost, (size_t)rows * 4, cudaMemcpyDeviceToHost, mb.xfer));
+    GS_CUDA_TRY(ctx, cudaMemcpyAsync(mb.buf.h_row_cost[slot].get(), mb.buf.row_cost.get(), (size_t)rows * 4, cudaMemcpyDeviceToHost, mb.xfer));
     GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_cost[slot], mb.xfer));
     GsImage *rt = rts ? rts[i] : nullptr;
     if (rt && rt->memory == GS_MEM_HOST) {

@@ -1,11 +1,13 @@
 // gs_internal.cuh -- what gs_api.cu (single GPU) and gs_group.cu (several GPUs) share behind the C ABI:
 // the context / asset objects and the per-stage drivers.
 #pragma once
+#include <algorithm>
 #include <string>
 #include <vector>
 
 #include <nvtx3/nvToolsExt.h>   // header-only; costs one predicted-not-taken branch per range when no tool is attached
 
+#include "gs_buffer.cuh"
 #include "gs_kernels.cuh"
 
 // Host-side ranges named as the reference's profiler markers (R/GaussianSplatRenderer.cs:20-22,287): an Nsight timeline of a
@@ -34,47 +36,38 @@ struct GsContext {
   GsStageTimes times{};
   cudaEvent_t ev[EV_COUNT]{};
   bool ev_valid[EV_COUNT]{};
-  // sort scratch
-  gs::SortScratch sort{};
-  uint32_t sort_capacity = 0;
-  size_t lookback_words = 0;
-  uint32_t *d_scalar = nullptr;  // small device scalars (standalone sorter count)
-  // bin scratch
-  gs::BinScratch bin{};
-  uint32_t bin_blocks_cap = 0, tiles_cap = 0, raster_tiles_cap = 0, raster_tiles_cur = 0;
+  // sort scratch (launchers take the view sort_scratch(ctx))
+  gs::Buffer<uint32_t> sort_alt_keys, sort_alt_vals;   // ping-pong buffers, as many elements as the largest sort so far
+  gs::Buffer<uint32_t> sort_ghist, sort_lookback, sort_tickets;
+  gs::Buffer<uint32_t> d_scalar;  // small device scalars (standalone sorter count)
+  // bin scratch (launchers take the view bin_scratch(ctx))
+  gs::Buffer<uint32_t> bin_keys, bin_vals, bin_block_sums, bin_entry_count;
+  gs::Buffer<uint2> bin_ranges;
+  gs::Buffer<uint32_t> tile_cost, tile_order;   // the single-grid raster-tile history, and the launch order of every draw
+  uint32_t raster_tiles_cur = 0;   // the tile count tile_cost's history was kept for
   bool bin_overflow = false;   // the bin list's overflow flag as the last read-back of a frame above kLargeFrameBins left it
   // gs_frame_cameras: the tile-cost histories of the camera layouts seen ((raster tiles per row, rows) per camera of a run,
   // each history at its base in cams_tile_cost), the digit histograms of a camera run's bin list (the depth sorts between its
-  // emits use sort.ghist), and one scratch buffer for a run's record slabs, staging images and host depth buffers
+  // emits use sort_ghist), and one scratch buffer for a run's record slabs, staging images and host depth buffers
   std::vector<std::vector<uint32_t>> cams_layouts;
   std::vector<size_t> cams_layout_base;
-  uint32_t *cams_tile_cost = nullptr;
-  size_t cams_cost_cap = 0, cams_cost_used = 0;
-  uint32_t *cams_ghist = nullptr;
-  void *cams_scratch = nullptr;
-  size_t cams_bytes = 0;
+  gs::Buffer<uint32_t> cams_tile_cost;
+  size_t cams_cost_used = 0;
+  gs::Buffer<uint32_t> cams_ghist;
+  gs::Buffer<uint8_t> cams_scratch;
   // image scratch
-  void *rt_scratch = nullptr;
-  size_t rt_bytes = 0;
-  void *tgt_scratch = nullptr;
-  size_t tgt_bytes = 0;
+  gs::Buffer<uint8_t> rt_scratch, tgt_scratch;
   // asynchronous read-back (GS_FLAG_ASYNC_READBACK): two device staging images, a copy stream, and the events that order
   // "raster k -> copy k" and "copy k -> raster k+2 may reuse the staging image"
   cudaStream_t copy_stream = nullptr;
-  void *rt_async[2] = {nullptr, nullptr};
-  size_t rt_async_bytes[2] = {0, 0};
+  gs::Buffer<uint8_t> rt_async[2];
   cudaEvent_t ev_rt_ready[2]{}, ev_copy_done[2]{};
   bool copy_pending[2] = {false, false};
   int rt_flip = 0;
   // per-frame optional inputs
-  GsCutout *d_cutouts = nullptr;
-  uint32_t cutout_cap = 0;
-  uint32_t *d_deleted = nullptr;
-  size_t deleted_words = 0;
-  uint32_t *d_selected = nullptr;
-  size_t selected_words = 0;
-  float *d_depth = nullptr;          // the frame's scene depth buffer when it was handed over in host memory
-  size_t depth_bytes = 0;
+  gs::Buffer<GsCutout> d_cutouts;
+  gs::Buffer<uint32_t> d_deleted, d_selected;
+  gs::Buffer<float> d_depth;   // the frame's scene depth buffer when it was handed over in host memory
   uint32_t launches = 0;
   uint64_t pack_stats[4] = {0, 0, 0, 0};   // gs_debug_pack_stats
   // surface objects of GS_MEM_ARRAY images, one per array per call: each batch is destroyed once `done` (recorded behind the
@@ -107,13 +100,24 @@ struct GsAsset {
 };
 
 namespace gs {
+// The launchers' views of the context's scratch.  The bin list's capacity is the smaller of its two buffers: after a failed
+// growth one of them may still hold the larger, older size.
+inline SortScratch sort_scratch(const GsContext *ctx) {
+  return {ctx->sort_alt_keys.get(), ctx->sort_alt_vals.get(), ctx->sort_ghist.get(), ctx->sort_lookback.get(), ctx->sort_tickets.get(),
+          ctx->sort_lookback.size()};
+}
+inline BinScratch bin_scratch(const GsContext *ctx) {
+  return {ctx->bin_block_sums.get(), ctx->bin_entry_count.get(), ctx->bin_keys.get(), ctx->bin_vals.get(),
+          reinterpret_cast<uint32_t *>(ctx->bin_ranges.get()), ctx->tile_cost.get(), ctx->tile_order.get(),
+          (uint32_t)std::min(ctx->bin_keys.size(), ctx->bin_vals.size())};
+}
 FrameConsts make_frame_consts(const GsFrameParams *fp);
 int check_params(GsContext *ctx, GsAsset *as, const GsFrameParams *fp);
 int check_options(GsContext *ctx, const FrameConsts &fc, GsRenderOptions &opt);
 int ensure_sort_scratch(GsContext *ctx, uint32_t capacity);
-// Grows the context's cutout / deleted / selected buffers to what fp needs for `as`; a buffer is only reallocated once
-// ctx->stream and `busy` (when given: another stream whose view-calc may still read it) have drained.  Uploads nothing.
-int reserve_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t busy = nullptr);
+// Grows the context's cutout / deleted / selected buffers to what fp needs for `as`; `users`: the streams whose view-calcs may
+// still read them (Buffer::reserve).  Uploads nothing.
+int reserve_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, std::initializer_list<cudaStream_t> users);
 int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t stream);
 // draw / zndc (optional): where the raster records and quad depths go instead of the asset's own buffers (gs_frame_cameras'
 // record slabs); the asset's draw state is then left as it was

@@ -144,9 +144,8 @@ void launch_calc_view(const AssetView &a, const FrameConsts &fc, const GsCutout 
 struct SortScratch {
   uint32_t *alt_keys, *alt_vals;  // ping-pong buffers, >= capacity elements each
   uint32_t *ghist;                // 4*256 digit counts (one row of 256 per pass; a single 9-bit pass uses the first 512)
-  uint32_t *lookback;             // max_tiles * 1024 status words: per tile, 4 passes x 256 digits or 1 pass x 512
+  uint32_t *lookback;             // 1024 status words per tile: 4 passes x 256 digits or 1 pass x 512
   uint32_t *tickets;              // passes counters
-  uint32_t max_tiles;             // capacity / kSortTileItems rounded up
   size_t lookback_words;          // size of `lookback`
 };
 constexpr uint32_t kSortTileItems = 8192;  // 512 threads x 16 keys

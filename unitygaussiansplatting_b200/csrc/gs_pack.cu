@@ -950,10 +950,10 @@ int gs_pack_asset(GsContext *ctx, const GsPackDesc *desc, GsPackedAsset *blobs_o
   k_morton<<<blocks_for(n, 256), 256, 0, st>>>(in, n, d_bounds, lo, hi, idx);
   int rc = ensure_sort_scratch(ctx, n);
   if (rc) return rc;
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_scalar, &n, 4, cudaMemcpyHostToDevice, st));
-  GS_CUDA_TRY(ctx, launch_sort_pairs(lo, idx, ctx->d_scalar, n, 4, 8, false, ctx->sort, st));
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_scalar.get(), &n, 4, cudaMemcpyHostToDevice, st));
+  GS_CUDA_TRY(ctx, launch_sort_pairs(lo, idx, ctx->d_scalar.get(), n, 4, 8, false, sort_scratch(ctx), st));
   k_gather_u32<<<blocks_for(n, 256), 256, 0, st>>>(hi, idx, n, lo);
-  GS_CUDA_TRY(ctx, launch_sort_pairs(lo, idx, ctx->d_scalar, n, 4, 8, false, ctx->sort, st));
+  GS_CUDA_TRY(ctx, launch_sort_pairs(lo, idx, ctx->d_scalar.get(), n, 4, 8, false, sort_scratch(ctx), st));
   ctx->launches += 5 + 2 * 5;
   GS_CUDA_TRY(ctx, cudaGetLastError());
   float *recs;
