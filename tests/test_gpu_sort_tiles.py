@@ -1,5 +1,6 @@
 """The sorter's 8192-pair tiles and the bin sort's plans at their boundaries: sizes around one and two tiles, and screens at
-both edges of every plan, from 32 bins (one 5-bit pass) to 16384 bins (two 7-bit passes, the largest screen)."""
+both edges of every plan from 32 bins (one 5-bit pass) to 16384 bins (two 7-bit passes).  The two 8-bit passes above 16384
+bins, up to 65536 on a 16384 x 16384 screen, are tested in test_gpu_large_screens.py and test_gpu_run_plans.py."""
 import numpy as np
 import pytest
 
@@ -21,7 +22,8 @@ def test_sort_pairs_around_tile_edges(ctx, n, kind):
 
 
 # (width, height): bins = ceil(W/64) * ceil(H/64); bin_sort_plan takes one pass up to 512 bins (5, 6, 7, 8, 9 bits at 32, 64,
-# 128, 256, 512), else two passes of 5, 6, 7 bits up to 1024, 4096, 16384 bins.  Each plan at its upper edge and one past it.
+# 128, 256, 512), else two passes of 5, 6, 7, 8 bits up to 1024, 4096, 16384, 65536 bins.  Each plan up to 7 bits at its upper
+# edge and one past it.
 PLAN_SCREENS = [
     ((512, 256), 32, 1, 5), ((704, 192), 33, 1, 6),
     ((512, 512), 64, 1, 6), ((832, 320), 65, 1, 7),
@@ -31,9 +33,9 @@ PLAN_SCREENS = [
     ((2048, 1088), 544, 2, 5), ((1728, 1216), 513, 2, 5),
     ((2048, 2048), 1024, 2, 5), ((2624, 1600), 1025, 2, 6),
     ((4096, 4096), 4096, 2, 6), ((5248, 3200), 4100, 2, 7),
-    ((8160, 8160), 16384, 2, 7),                                # the largest screen (check_params)
+    ((8160, 8160), 16384, 2, 7),                                # also the largest camera a camera run takes
 ]
-# the largest screen of each narrow digit width sorts enough entries that the persistent grid's CTAs take several tiles
+# the upper edge of each two-pass digit width sorts enough entries that the persistent grid's CTAs take several tiles
 MULTI_TILE = {(2048, 2048), (4096, 4096), (8160, 8160)}
 
 
