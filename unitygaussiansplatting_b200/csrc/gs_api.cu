@@ -290,12 +290,20 @@ static int do_sort(GsContext *ctx, GsAsset *as, const FrameConsts &fc) {
   int rc = ensure_sort_scratch(ctx, as->av.n);
   if (rc) return rc;
   rec(ctx, EV_BEGIN);
-  GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->sort_ghist.get(), 0, 4 * 256 * 4, ctx->stream));
-  launch_calc_distances(as->av, fc, as->key_table, ctx->sort_ghist.get(), ctx->stream);
+  // one clear for the whole sort: the digit histograms k_calc_distances counts into, the four passes' look-back rows and
+  // their tickets.  It releases before it waits, so that k_calc_distances computes the keys beside the previous call's
+  // last kernel and waits only to count them into the cleared histograms
+  const SortScratch sc = sort_scratch(ctx);
+  ClearSpans cl = {};
+  cl.ptr[0] = sc.ghist; cl.words[0] = 4 * 256;
+  cl.ptr[1] = sc.lookback; cl.words[1] = sort_lookback_words(as->av.n, 4);
+  cl.ptr[2] = sc.tickets; cl.words[2] = 4;
+  launch_clear(cl, ctx->stream, /*release_first=*/true);
+  launch_calc_distances(as->av, fc, as->key_table, sc.ghist, ctx->stream);
   rec(ctx, EV_DIST);
   cudaEvent_t pe[5] = {ctx->ev[EV_SORT0], ctx->ev[EV_SORT1], ctx->ev[EV_SORT2], ctx->ev[EV_SORT3], ctx->ev[EV_SORT4]};
-  GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order, as->d_n, as->av.n, 4, 8, true, sort_scratch(ctx), ctx->stream, ctx->timing ? pe : nullptr,
-                                     as->key_table));
+  GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order, as->d_n, as->av.n, 4, 8, true, sc, ctx->stream, ctx->timing ? pe : nullptr,
+                                     as->key_table, true, nullptr, nullptr, /*scratch_clear=*/true));
   if (ctx->timing) for (int e = EV_SORT0; e <= EV_SORT4; ++e) ctx->ev_valid[e] = true;
   ctx->launches += 1 + 4;
   GS_CUDA_TRY(ctx, cudaGetLastError());
@@ -309,7 +317,7 @@ static GsRenderOptions default_opts() {
 }
 
 int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameConsts &fc, bool cull, const GsRenderOptions &opt,
-            cudaStream_t stream, float4 *draw, float *zndc) {
+            cudaStream_t stream, float4 *draw, float *zndc, bool after_sort) {
   GsNvtxRange nvtx("GaussianSplat.CalcView");
   int rc = upload_frame_inputs(ctx, as, fp, stream);
   if (rc) return rc;
@@ -317,7 +325,7 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
   if (own) rec(ctx, EV_VIEW0);
   if (draw) {   // a record slab: the asset's own records stay as they are
     launch_calc_view(as->av, fc, ctx->d_cutouts.get(), ctx->d_deleted.get(), ctx->d_selected.get(), as->view, as->rect, draw, as->block_bits,
-                     fp->scene_depth ? zndc : nullptr, cull, make_partition(opt), stream);
+                     fp->scene_depth ? zndc : nullptr, cull, make_partition(opt), stream, after_sort);
     if (own) rec(ctx, EV_VIEW1);
     ctx->launches += 1;
     GS_CUDA_TRY(ctx, cudaGetLastError());
@@ -326,7 +334,7 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
   if (fp->scene_depth && !as->zndc) GS_CUDA_TRY(ctx, cudaMalloc(&as->zndc, (size_t)as->av.n * sizeof(float) + 16));
   as->zndc_valid = fp->scene_depth != nullptr;
   launch_calc_view(as->av, fc, ctx->d_cutouts.get(), ctx->d_deleted.get(), ctx->d_selected.get(), as->view, as->rect, as->draw, as->block_bits,
-                   as->zndc_valid ? as->zndc : nullptr, cull, make_partition(opt), stream);
+                   as->zndc_valid ? as->zndc : nullptr, cull, make_partition(opt), stream, after_sort);
   if (own) rec(ctx, EV_VIEW1);
   ctx->launches += 1;
   as->view_valid = !cull;
@@ -1057,8 +1065,9 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
       draw = reinterpret_cast<float4 *>(scratch + slab_at[p] - 1);
       zndc = reinterpret_cast<float *>(scratch + slab_at[p] - 1 + align256((size_t)as->av.n * 48));
     }
-    if (do_sort_flags[pair_at[p]] && (rc = do_sort(ctx, as, c.fcs[pair_at[p] - c.off]))) return rc;
-    if ((rc = do_view(ctx, as, &f, c.fcs[pair_at[p] - c.off], true, opt, ctx->stream, draw, zndc))) return rc;
+    const bool sorted = do_sort_flags[pair_at[p]] != 0;
+    if (sorted && (rc = do_sort(ctx, as, c.fcs[pair_at[p] - c.off]))) return rc;
+    if ((rc = do_view(ctx, as, &f, c.fcs[pair_at[p] - c.off], true, opt, ctx->stream, draw, zndc, sorted))) return rc;
     objs.draw[p] = draw ? draw : as->draw;
     if (f.scene_depth) {
       objs.zndc[p] = draw ? zndc : as->zndc;
@@ -1161,7 +1170,8 @@ int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRende
   if (rt) { if ((rc = image_ok(ctx, rt, W, H, &rt_pitch))) return rc; rt_fmt = rt->format; }
   for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
   if (do_sort_flag && (rc = do_sort(ctx, as, fc))) return rc;
-  if ((rc = do_view(ctx, as, fp, fc, true, opt, ctx->stream))) return rc;   // fused frame: colour of never-drawn splats is dead code
+  // fused frame: colour of never-drawn splats is dead code; after the sort, the view-calc runs beside its last pass
+  if ((rc = do_view(ctx, as, fp, fc, true, opt, ctx->stream, nullptr, nullptr, do_sort_flag != 0))) return rc;
   CallSurfaces surfs(ctx);
   FrameImage fi;
   if ((rc = begin_frame_image(ctx, surfs, opt, rt, rt_pitch, rt_fmt, tgt, W, H, &fi))) return rc;

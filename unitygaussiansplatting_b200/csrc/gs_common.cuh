@@ -101,6 +101,20 @@ __device__ __forceinline__ uint32_t lookback_exclusive(volatile uint32_t *status
   return excl;
 }
 
+// ---- launch chain (programmatic dependent launch) ------------------------------------------------
+// A kernel launched by chain_launch (gs_kernels.cuh) may be placed on the SMs while its predecessor on the stream still
+// drains.  chain_wait() blocks until the predecessor grid has completed and its writes are visible; chain_release() lets
+// the successor be placed once every CTA of this grid has released or exited.  Both are no-ops in an ordinary launch.
+// Rules every chained kernel keeps (DESIGN §5 "Launch chain"):
+//   * every CTA calls chain_wait() before it exits, on every path, so that a grid's completion implies its predecessor's;
+//   * chain_release() comes after chain_wait(), so that when a kernel starts, every node before its immediate predecessor has
+//     completed.  The exceptions release earlier only where the successor's pre-wait work is safe beside the releasing
+//     kernel and the node before it (k_tile_order and the early k_calc_view, whose successors wait first, and the depth
+//     sort's k_clear, whose successor k_calc_distances writes only key_table before its wait);
+//   * work before chain_wait() touches nothing the immediate predecessor reads or writes (listed beside each call).
+__device__ __forceinline__ void chain_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void chain_release() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
 // ---- small device helpers -------------------------------------------------------------
 __device__ __forceinline__ float f16lo(uint32_t v) { return __half2float(__ushort_as_half((unsigned short)(v & 0xffffu))); }
 __device__ __forceinline__ float f16hi(uint32_t v) { return __half2float(__ushort_as_half((unsigned short)(v >> 16))); }

@@ -120,9 +120,10 @@ int ensure_sort_scratch(GsContext *ctx, uint32_t capacity);
 int reserve_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, std::initializer_list<cudaStream_t> users);
 int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cudaStream_t stream);
 // draw / zndc (optional): where the raster records and quad depths go instead of the asset's own buffers (gs_frame_cameras'
-// record slabs); the asset's draw state is then left as it was
+// record slabs); the asset's draw state is then left as it was.  after_sort: the last thing on `stream` is do_sort of `as`
+// (launch_calc_view)
 int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameConsts &fc, bool cull, const GsRenderOptions &opt,
-            cudaStream_t stream, float4 *draw = nullptr, float *zndc = nullptr);
+            cudaStream_t stream, float4 *draw = nullptr, float *zndc = nullptr, bool after_sort = false);
 // Bins and rasterizes one object `as`, drawn with the uniforms *fp, into a device image (d_rt == nullptr: the CUDA array behind
 // `surf`) on ctx->stream with gs_frame's kernels; its scene depth buffer is bound here.  A run of several objects or cameras is
 // gs_api.cu's draw_run.  `first`: the first draw of its public call, whose bin list sets the overflow flag; a later draw of

@@ -1,5 +1,7 @@
 // gs_kernels.cuh -- declarations shared between the .cu translation units.
 #pragma once
+#include <utility>
+
 #include "gs_common.cuh"
 
 namespace gs {
@@ -117,6 +119,31 @@ __device__ __forceinline__ uint32_t rect_entries(uint32_t r, const Partition &p)
 
 
 // ---- launchers (each enqueues on `s`, returns nothing; errors surface via cudaGetLastError) ----
+// A launch in the frame's chain: the kernel may be placed while its predecessor on `s` drains (programmatic stream
+// serialization); it must keep the rules beside chain_wait() in gs_common.cuh.
+template <typename... KArgs, typename... Args>
+inline void chain_launch(void (*kern)(KArgs...), uint32_t grid, uint32_t block, size_t smem, cudaStream_t s, Args &&...args) {
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(block);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = s;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
+}
+// Zeroes up to kClearSpans word ranges in one chained kernel: the per-frame clears of scratch that the frame's kernels count
+// or tick into, without a memset node in the chain.  Spans with a null pointer or no words are skipped.
+constexpr int kClearSpans = 4;
+struct ClearSpans {
+  uint32_t *ptr[kClearSpans];
+  size_t words[kClearSpans];
+};
+// release_first: the successor is placed before the clear waits for its own predecessor (see k_calc_distances)
+void launch_clear(const ClearSpans &spans, cudaStream_t s, bool release_first = false);
 uint32_t sm_count();   // multiprocessors of the current device (queried once per device): sizes grid-stride and persistent grids
 void launch_set_indices(uint32_t *order, uint32_t n, cudaStream_t s);
 void launch_export_data(const AssetView &a, uint32_t cutoutCount, const GsCutout *cutouts, float *out, cudaStream_t s);  // gs_export.cu
@@ -138,7 +165,8 @@ inline size_t block_bits_words(uint32_t n) { return ((size_t)(n + 255) / 256 + 3
 inline size_t group_bits_words(uint32_t n) { return ((size_t)(n + 127) / 128 + 31) / 32 + 1; }
 void launch_calc_view(const AssetView &a, const FrameConsts &fc, const GsCutout *cutouts, const uint32_t *deleted, const uint32_t *selected, uint32_t *view,
                       uint32_t *rect, float4 *draw, uint32_t *block_bits, float *zndc /* per-splat quad depth, or nullptr */, bool cull_undrawable,
-                      const Partition &part, cudaStream_t s);
+                      const Partition &part, cudaStream_t s, bool after_sort = false);
+// (after_sort: the kernel before it on `s` is the depth sort of this asset, and the view-calc runs beside its last pass)
 
 // Radix sort (gs_sort.cu).  Scratch layout is owned by the caller (gs_api.cu).
 struct SortScratch {
@@ -160,9 +188,11 @@ extern uint32_t g_sort_phase_tiles;
 // passes * 2^bits words per 8192-pair tile.  An unsupported request launches nothing and returns cudaErrorInvalidValue.
 // After an even number of passes the result is back in keys/vals -- unless final_keys/final_vals name where the last pass
 // writes.  key_table != nullptr: the input keys are key_table[vals[i]] (gathered inside pass 0; `keys` is then output only).
+// scratch_clear (count_is_capacity only): the caller has zeroed the passes' look-back rows and the 4 tickets.
 cudaError_t launch_sort_pairs(uint32_t *keys, uint32_t *vals, const uint32_t *d_count, uint32_t capacity, int passes, int bits, bool hist_ready,
                        const SortScratch &sc, cudaStream_t s, cudaEvent_t *pass_events = nullptr, const uint32_t *key_table = nullptr,
-                       bool count_is_capacity = true, uint32_t *final_keys = nullptr, uint32_t *final_vals = nullptr);
+                       bool count_is_capacity = true, uint32_t *final_keys = nullptr, uint32_t *final_vals = nullptr,
+                       bool scratch_clear = false);
 // (out_ids, out_keys) = (id, key_table[id]) of the ids of order[0..n) whose mask bit is set, order kept; *count_out = how many.
 // group_bits (one bit per 128 ids, kept in shared memory) lets whole groups be skipped without reading their mask words.
 // status: compact_status_words(n) words of scratch.

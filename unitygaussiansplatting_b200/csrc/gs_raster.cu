@@ -60,6 +60,8 @@ __global__ void __launch_bounds__(256) k_bin_emit(const uint32_t *__restrict__ o
   extern __shared__ uint32_t s_bits[];   // the view kernel's block bitmap (bits_words words), or nothing when it is too large to hold
   __shared__ uint32_t s_w[8];
   __shared__ uint32_t s_block, s_excl, s_base;
+  chain_wait();   // nothing before the wait: the ticket, the list's length and block_bits / rect all come from predecessors
+  chain_release();
   if (APPEND && threadIdx.x == 0) {
     // read before this block publishes its status: the last block writes the new total only after every block has published
     s_base = *(volatile uint32_t *)(entry_count + 2);
@@ -235,22 +237,27 @@ static uint32_t bin_bits_words(uint32_t n) {
 }
 
 void launch_bin_list_begin(const BinScratch &bs, uint32_t *ghist, cudaStream_t s) {
-  cudaMemsetAsync(bs.entry_count + 2, 0, sizeof(uint32_t), s);   // the pairs append behind an empty list
-  cudaMemsetAsync(ghist, 0, 4 * 256 * sizeof(uint32_t), s);
+  ClearSpans cl = {};
+  cl.ptr[0] = bs.entry_count + 2; cl.words[0] = 1;   // the pairs append behind an empty list
+  cl.ptr[1] = ghist; cl.words[1] = 4 * 256;
+  launch_clear(cl, s);
 }
 
 // the look-back clear and k_bin_emit of one object's entries, counted into ghist by the digit plan of `bins` bins
 template <bool APPEND>
 static void bin_emit(const uint32_t *order, const uint32_t *rect, const uint32_t *block_bits, uint32_t n, const Partition &part,
                      uint32_t binsX, uint32_t bins, bool clear_overflow, uint32_t tag, uint32_t key_base, const BinScratch &bs,
-                     uint32_t *ghist, cudaStream_t s) {
+                     uint32_t *ghist, cudaStream_t s, uint32_t *clear_ghist = nullptr) {
   int bits, passes;
   bin_sort_plan(bins, &bits, &passes);
   const uint32_t nblocks = (n + kBinBlock - 1) / kBinBlock, words = bin_bits_words(n);
-  cudaMemsetAsync(bs.block_sums, 0, ((size_t)nblocks + 1) * sizeof(uint32_t), s);   // [0] ticket, [1..] look-back status
-  k_bin_emit<APPEND><<<nblocks, 256, words * 4u, s>>>(order, rect, block_bits, words, n, part, binsX, bs.block_sums + 1, bs.block_sums,
-                                                      bs.capacity, bs.tile_keys, bs.tile_vals, bs.entry_count, ghist, (uint32_t)bits,
-                                                      passes == 2, clear_overflow, tag, key_base);
+  ClearSpans cl = {};
+  cl.ptr[0] = bs.block_sums; cl.words[0] = (size_t)nblocks + 1;   // [0] ticket, [1..] look-back status
+  cl.ptr[1] = clear_ghist; cl.words[1] = 4 * 256;
+  launch_clear(cl, s);
+  chain_launch(k_bin_emit<APPEND>, nblocks, 256, words * 4u, s, order, rect, block_bits, words, n, part, binsX, bs.block_sums + 1,
+               bs.block_sums, bs.capacity, bs.tile_keys, bs.tile_vals, bs.entry_count, ghist, (uint32_t)bits, passes == 2, clear_overflow,
+               tag, key_base);
 }
 
 void launch_bin_emit_pair(const uint32_t *order, const uint32_t *rect, const uint32_t *block_bits, uint32_t n, uint32_t binsX,
@@ -274,8 +281,8 @@ cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, co
                            const uint32_t *block_bits, uint32_t n, bool clear_overflow, const BinScratch &bs, const SortScratch &sc,
                            cudaStream_t s, BinScratch *sorted, int *launches) {
   const uint32_t bins = fc.binsX * fc.binsY;
-  cudaMemsetAsync(sc.ghist, 0, 4 * 256 * sizeof(uint32_t), s);
-  bin_emit<false>(order, rect, block_bits, n, make_partition(opt), fc.binsX, bins, clear_overflow, 0u, 0u, bs, sc.ghist, s);
+  // the digit histograms are the depth sort's: cleared with the emit's look-back, after the view-calc (and so the sort) completed
+  bin_emit<false>(order, rect, block_bits, n, make_partition(opt), fc.binsX, bins, clear_overflow, 0u, 0u, bs, sc.ghist, s, sc.ghist);
   const cudaError_t e = launch_bin_list_sort(bins, bs, sc, sc.ghist, s, sorted, launches);
   *launches += 2;   // look-back clear, bin_emit
   return e;
@@ -317,6 +324,8 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 __global__ void __launch_bounds__(256) k_bin_ranges(const uint32_t *__restrict__ keys, const uint32_t *__restrict__ entry_count,
                                                     uint32_t bins, uint2 *__restrict__ ranges) {
   const uint32_t bin = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  chain_wait();   // the sorted list and its length come from the bin sort
+  chain_release();
   if (bin >= bins) return;
   const uint32_t m = __ldg(entry_count);
   const uint32_t a = lower_bound32(keys, m, bin, lane), b = lower_bound32(keys, m, bin + 1, lane);
@@ -331,6 +340,10 @@ __global__ void __launch_bounds__(1024) k_tile_order(const uint32_t *__restrict_
   // `order` receives the ids of OUR ntiles tiles (own tile row k = kth_own_tile_row(k)), most expensive first
   __shared__ uint32_t s_hist[64], s_base[64];
   __shared__ uint32_t s_any;
+  // The whole body runs before the wait, beside the bin sort: it reads only tile_cost, last written by an earlier frame's
+  // raster, and writes only tile_order, last read by that raster -- both completed before this frame's first kernel began.
+  // Releasing at once is safe because the successor (k_bin_ranges) waits before it does anything.
+  chain_release();
   if (threadIdx.x < 64) s_hist[threadIdx.x] = 0;
   if (threadIdx.x == 0) s_any = 0;
   __syncthreads();
@@ -354,12 +367,13 @@ __global__ void __launch_bounds__(1024) k_tile_order(const uint32_t *__restrict_
   __syncthreads();
   if (!s_any) {   // no history (first frame / new resolution): a stride permutation spreads spatial clusters
     for (uint32_t t = threadIdx.x; t < ntiles; t += 1024) order[t] = global_id((ntiles % 1031u) ? (uint32_t)(((uint64_t)t * 1031u) % ntiles) : t);
-    return;
+  } else {
+    for (uint32_t t = threadIdx.x; t < ntiles; t += 1024) {
+      const uint32_t gid = global_id(t);
+      order[atomicAdd(&s_base[63u - bucket(cost[gid])], 1u)] = gid;
+    }
   }
-  for (uint32_t t = threadIdx.x; t < ntiles; t += 1024) {
-    const uint32_t gid = global_id(t);
-    order[atomicAdd(&s_base[63u - bucket(cost[gid])], 1u)] = gid;
-  }
+  chain_wait();
 }
 
 // per raster-tile row: the sum of its tiles' costs (what the group path balances its row ranges with).  accumulate != 0 adds
@@ -418,6 +432,8 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
          std::conditional_t<MULTI, DrawObjects, NoRasterObjects> objs, std::conditional_t<MULTI, DrawCameras, NoRasterObjects> cams) {
   uint32_t st_batches = 0, st_culls = 0, st_cand = 0, st_eval = 0, st_blend = 0;   // GS_RASTER_STATS diagnostics (per warp)
   unsigned long long st_t0 = 0;
+  chain_wait();   // nothing before the wait: the bin ranges come from the predecessor
+  chain_release();
   if (STATS) asm volatile("mov.u64 %0, %globaltimer;" : "=l"(st_t0));
   // two staging buffers of 256 raster records (3 x float4 each, planar [buf][plane][entry]): batch k+1 lands
   // asynchronously while batch k is composited
@@ -652,7 +668,7 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const floa
   if (!rows || !fc.binsX) return;
   const uint32_t ntx = ((uint32_t)fc.screenW + kTile - 1) / kTile, ntiles = ntx * rows;
   const uint32_t grid = ntiles;
-  k_tile_order<<<1, 1024, 0, s>>>(bs.tile_cost, ntiles, ntx, part, bs.tile_order);
+  chain_launch(k_tile_order, 1, 1024, 0, s, bs.tile_cost, ntiles, ntx, part, bs.tile_order);
   const bool rop = opt.blend_mode == GS_BLEND_FP16_ROP;
   uint8_t *out = reinterpret_cast<uint8_t *>(rt);
   // GS_RASTER_STATS=1: per-frame work counters of a one-object draw (diagnostics; printed by tools/raster_stats.py through
@@ -665,15 +681,15 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const floa
   const uint32_t bins = fc.binsX * fc.binsY;
   uint2 *ranges = reinterpret_cast<uint2 *>(bs.bin_ranges);
   const uint32_t packed = part.range ? 0u : opt.band_packed, load = (opt.flags & GS_FLAG_LOAD_RT) ? 1u : 0u;
-  k_bin_ranges<<<(bins + 7) / 8, 256, 0, s>>>(bs.tile_keys, bs.entry_count, bins, ranges);
+  chain_launch(k_bin_ranges, (bins + 7) / 8, 256, 0, s, bs.tile_keys, bs.entry_count, bins, ranges);
 #define GS_RASTER_ARGS                                                                                                           \
-  <<<grid, 256, 0, s>>>(fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed,  \
-                        load, stats, zndc, scene_depth, NoRasterObjects{}, NoRasterObjects{})
+  grid, 256, 0, s, fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed,  \
+      load, stats, zndc, scene_depth, NoRasterObjects{}, NoRasterObjects{}
 #define GS_LAUNCH_RASTER(ROP, FMT, SURF)                                                                                        \
   do {                                                                                                                         \
-    if (extras) k_raster<ROP, FMT, false, true, SURF> GS_RASTER_ARGS;                                                          \
-    else if (stats) k_raster<ROP, FMT, true, false, SURF> GS_RASTER_ARGS;                                                      \
-    else k_raster<ROP, FMT, false, false, SURF> GS_RASTER_ARGS;                                                                \
+    if (extras) chain_launch(k_raster<ROP, FMT, false, true, SURF>, GS_RASTER_ARGS);                                           \
+    else if (stats) chain_launch(k_raster<ROP, FMT, true, false, SURF>, GS_RASTER_ARGS);                                       \
+    else chain_launch(k_raster<ROP, FMT, false, false, SURF>, GS_RASTER_ARGS);                                                 \
   } while (0)
   // a null `rt` means the target is a CUDA array behind rt_surf
 #define GS_LAUNCH_RASTER_TARGET(ROP, FMT)                                                                                       \
@@ -694,9 +710,9 @@ void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, uin
                            uint32_t rt_format, const BinScratch &bs, cudaStream_t s) {
   const Partition whole{0, 0, 1, 0, 0, 0};
   // without a partition a tile's id is its launch-order id: ntx = tiles puts all of them in row 0
-  k_tile_order<<<1, 1024, 0, s>>>(bs.tile_cost, tiles, tiles, whole, bs.tile_order);
+  chain_launch(k_tile_order, 1, 1024, 0, s, bs.tile_cost, tiles, tiles, whole, bs.tile_order);
   uint2 *ranges = reinterpret_cast<uint2 *>(bs.bin_ranges);
-  k_bin_ranges<<<(bins + 7) / 8, 256, 0, s>>>(bs.tile_keys, bs.entry_count, bins, ranges);
+  chain_launch(k_bin_ranges, (bins + 7) / 8, 256, 0, s, bs.tile_keys, bs.entry_count, bins, ranges);
   FrameConsts fc;   // screen size and bins come from each tile's camera
   memset(&fc, 0, sizeof(fc));
   const bool rop = blend_mode == GS_BLEND_FP16_ROP;
@@ -705,11 +721,11 @@ void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, uin
 #define GS_RASTER_CAMS(ROP, FMT, SURF)                                                                                          \
   do {                                                                                                                         \
     if (objs.extras)                                                                                                           \
-      k_raster<ROP, FMT, false, true, SURF, true><<<tiles, 256, 0, s>>>(fc, whole, nullptr, ranges, bs.tile_vals, bs.tile_order,  \
-          bs.tile_cost, 1u, nullptr, 0u, 0, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);                                     \
+      chain_launch(k_raster<ROP, FMT, false, true, SURF, true>, tiles, 256, 0, s, fc, whole, nullptr, ranges, bs.tile_vals,        \
+          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, 0, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);                       \
     else                                                                                                                       \
-      k_raster<ROP, FMT, false, false, SURF, true><<<tiles, 256, 0, s>>>(fc, whole, nullptr, ranges, bs.tile_vals, bs.tile_order, \
-          bs.tile_cost, 1u, nullptr, 0u, 0, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);                                     \
+      chain_launch(k_raster<ROP, FMT, false, false, SURF, true>, tiles, 256, 0, s, fc, whole, nullptr, ranges, bs.tile_vals,       \
+          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, 0, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);                       \
   } while (0)
 #define GS_RASTER_CAMS_TARGET(ROP, FMT)                                                                                         \
   do {                                                                                                                         \

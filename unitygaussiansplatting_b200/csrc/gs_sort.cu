@@ -151,6 +151,11 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
   __shared__ unsigned long long s_ph[3];
 
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  // nothing before the wait: the ticket, the count, the histograms and the keys may all come from the predecessor.  A
+  // persistent grid is at most as large as the SMs hold, so releasing at the start lets the launch order's kernel
+  // (k_tile_order) run its pre-wait body beside the bin sort
+  chain_wait();
+  chain_release();
   const uint32_t n = *d_count;
   const uint32_t num_tiles = (n + kTileItems - 1) / kTileItems;
   do {   // one tile per iteration (a single iteration unless PERSIST; every shared array written below was last read
@@ -331,9 +336,13 @@ k_onesweep(const uint32_t *__restrict__ src_k, const uint32_t *__restrict__ src_
 }
 
 // zero `per_item_words * ceil(count / items)` words, count read on the device: clears exactly the look-back rows a sort of a
-// device-sized list will use (instead of a capacity-sized cudaMemset)
+// device-sized list will use (instead of a capacity-sized cudaMemset), and the sort's `ticket_words` tickets
 __global__ void __launch_bounds__(256) k_zero_rows(uint32_t *__restrict__ buf, const uint32_t *__restrict__ d_count, uint32_t items,
-                                                   uint32_t words_per_row, uint32_t row_stride_words, uint32_t reps, uint32_t rep_stride_words) {
+                                                   uint32_t words_per_row, uint32_t row_stride_words, uint32_t reps, uint32_t rep_stride_words,
+                                                   uint32_t *__restrict__ tickets, uint32_t ticket_words) {
+  chain_wait();   // the count comes from the predecessor, and the rows may still be in use by an earlier sort's last pass
+  chain_release();
+  if (blockIdx.x == 0 && threadIdx.x < ticket_words) tickets[threadIdx.x] = 0u;
   const uint32_t rows = (*d_count + items - 1) / items;
   const size_t per_rep = (size_t)rows * words_per_row;
   for (size_t i = blockIdx.x * 256 + threadIdx.x; i < per_rep * reps; i += (size_t)gridDim.x * 256) {
@@ -341,6 +350,28 @@ __global__ void __launch_bounds__(256) k_zero_rows(uint32_t *__restrict__ buf, c
     const size_t j = i - (size_t)rep * per_rep;
     buf[(size_t)rep * rep_stride_words + (j / words_per_row) * row_stride_words + (j % words_per_row)] = 0u;
   }
+}
+
+__global__ void __launch_bounds__(256) k_clear(ClearSpans sp, uint32_t release_first) {
+  // release_first: the successor may be placed before this kernel waits (its pre-wait work is safe beside this kernel and
+  // the node before it: k_calc_distances after the depth sort's clear)
+  if (release_first) chain_release();
+  chain_wait();   // the spans may still be read or counted into by the predecessor
+  if (!release_first) chain_release();
+#pragma unroll
+  for (int k = 0; k < kClearSpans; ++k) {
+    uint32_t *p = sp.ptr[k];
+    const size_t words = p ? sp.words[k] : 0;
+    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < words; i += (size_t)gridDim.x * 256) p[i] = 0u;
+  }
+}
+
+void launch_clear(const ClearSpans &spans, cudaStream_t s, bool release_first) {
+  size_t most = 0;
+  for (int k = 0; k < kClearSpans; ++k) if (spans.ptr[k]) most = std::max(most, spans.words[k]);
+  if (!most) return;
+  const uint32_t grid = (uint32_t)std::min<size_t>((most + 1023) / 1024, sm_count() * 4u);   // 4 words per thread and span, at least
+  chain_launch(k_clear, grid, 256, 0, s, spans, release_first ? 1u : 0u);
 }
 
 // ---- ordered compaction of a draw order by a membership mask ------------------------------------------
@@ -474,7 +505,7 @@ static void launch_pass(uint32_t count_bound, bool persist, cudaStream_t s, cons
     }
     uint32_t grid = (uint32_t)(((uint64_t)count_bound + kSortTileItems - 1) / kSortTileItems);
     if (persist) grid = min(grid, sm_count() * 2u);   // the 2 CTAs per SM that __launch_bounds__ asks for
-    kern<<<grid, kSortThreads, smem, s>>>(sk, sv, dk, dv, d_count, shift, ghist, lookback, ticket, phases);
+    chain_launch(kern, grid, kSortThreads, smem, s, sk, sv, dk, dv, d_count, shift, ghist, lookback, ticket, phases);
   };
   if constexpr (BITS == 8) {   // the depth sort's digit width: the only one the phase diagnostics record
     if (phases) { if (gather) go(k_onesweep<BITS, true, false, true>); else go(k_onesweep<BITS, false, false, true>); return; }
@@ -488,7 +519,7 @@ static void launch_pass(uint32_t count_bound, bool persist, cudaStream_t s, cons
 
 cudaError_t launch_sort_pairs(uint32_t *keys, uint32_t *vals, const uint32_t *d_count, uint32_t capacity, int passes, int bits,
                               bool hist_ready, const SortScratch &sc, cudaStream_t s, cudaEvent_t *pass_events, const uint32_t *key_table,
-                              bool count_is_capacity, uint32_t *final_keys, uint32_t *final_vals) {
+                              bool count_is_capacity, uint32_t *final_keys, uint32_t *final_vals, bool scratch_clear) {
   if (capacity == 0) return cudaSuccess;
   const uint32_t tiles = (capacity + kSortTileItems - 1) / kSortTileItems;
   const uint32_t nb = 1u << bits;
@@ -497,15 +528,25 @@ cudaError_t launch_sort_pairs(uint32_t *keys, uint32_t *vals, const uint32_t *d_
   const bool shape_ok = passes >= 1 && passes <= 4 && bits >= 5 && (bits <= 8 || (bits == 9 && passes == 1));
   const bool hist_ok = hist_ready || (passes == 4 && bits == 8) || (passes <= 2 && bits <= 8);
   if (!shape_ok || !hist_ok || (size_t)tiles * nb * passes > sc.lookback_words) return cudaErrorInvalidValue;
-  // count_is_capacity: the host knows the exact count (depth sort, slab sort) -> exact grid, exact memset.  Otherwise the list
+  // count_is_capacity: the host knows the exact count (depth sort, slab sort) -> exact grid, exact clear.  Otherwise the list
   // length lives on the device only (the binner's entries): a persistent grid, and the look-back rows actually needed are
   // cleared by a kernel that reads the count.
+  // scratch_clear: the caller has already cleared the look-back rows and tickets (the depth sort clears them with its
+  // histograms, before k_calc_distances counts into those)
   const bool persist = !count_is_capacity;
-  if (persist) k_zero_rows<<<sm_count(), 256, 0, s>>>(sc.lookback, d_count, kSortTileItems, nb, nb, (uint32_t)passes, tiles * nb);
-  else cudaMemsetAsync(sc.lookback, 0, (size_t)tiles * nb * passes * sizeof(uint32_t), s);
-  cudaMemsetAsync(sc.tickets, 0, 4 * sizeof(uint32_t), s);
+  if (persist)
+    chain_launch(k_zero_rows, sm_count(), 256, 0, s, sc.lookback, d_count, (uint32_t)kSortTileItems, nb, nb, (uint32_t)passes, tiles * nb,
+                 sc.tickets, 4u);
+  {
+    ClearSpans cl = {};
+    if (!persist && !scratch_clear) {
+      cl.ptr[0] = sc.lookback; cl.words[0] = (size_t)tiles * nb * passes;
+      cl.ptr[1] = sc.tickets; cl.words[1] = 4;
+    }
+    if (!hist_ready) { cl.ptr[2] = sc.ghist; cl.words[2] = 4 * 256; }
+    launch_clear(cl, s);
+  }
   if (!hist_ready) {
-    cudaMemsetAsync(sc.ghist, 0, 4 * 256 * sizeof(uint32_t), s);
     const uint32_t grid = min(tiles, sm_count() * 8u);
     if (passes == 4) k_sort_hist<4, 8><<<grid, 256, 0, s>>>(keys, d_count, sc.ghist);
     else if (bits == 5) k_sort_hist<2, 5><<<grid, 256, 0, s>>>(keys, d_count, sc.ghist);

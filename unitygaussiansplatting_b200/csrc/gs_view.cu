@@ -58,6 +58,16 @@ __global__ void __launch_bounds__(256) k_calc_distances(AssetView a, float4 row,
   __shared__ uint32_t s_thr[MAXT + 1];
   __shared__ uint32_t s_ge[MAXT + 1];
   for (int i = threadIdx.x; i < 1024; i += 256) sh[i] = 0;
+  // Without slabs, everything but the flush into ghist runs before the wait: its predecessor is the k_clear that starts the
+  // depth sort, which releases at once, so this kernel can run beside the end of the previous frame's raster.  Pre-wait
+  // reads: the asset's position blobs and chunks, which no kernel writes.  Pre-wait writes: key_table, which only pass 0 of
+  // this asset's depth sort reads; the kernels still running are at most that k_clear and the node before it, never a
+  // depth sort's pass 0 (a sort ends with its last pass).  ghist is cleared by the k_clear, so it is counted into after the
+  // wait.  The slab variant (group path) reads last frame's order and writes the slab masks: it waits first.
+  if (MAXT) {
+    chain_wait();
+    chain_release();
+  }
   const uint32_t nthr = MAXT ? sl.count - 1 : 0;   // number of splitters
   if (MAXT) {
     if (threadIdx.x < nthr) {
@@ -184,6 +194,10 @@ __global__ void __launch_bounds__(256) k_calc_distances(AssetView a, float4 row,
     }
   }
   __syncthreads();
+  if (!MAXT) {
+    chain_wait();
+    chain_release();
+  }
   for (int i = threadIdx.x; i < 1024; i += 256) {
     uint32_t c = sh[i];
     if (c) atomicAdd(&ghist[i], c);
@@ -294,11 +308,21 @@ template <int SHFMT, bool CULL, bool BC7>
 __global__ void __launch_bounds__(256, (CULL && SHFMT == 3 && !BC7) ? 5 : 1)
 k_calc_view(AssetView a, FrameConsts fc, const GsCutout *__restrict__ cutouts, const uint32_t *__restrict__ deleted,
             const uint32_t *__restrict__ selected, uint32_t *__restrict__ view_out, uint32_t *__restrict__ rect_out, float4 *__restrict__ draw_out,
-            uint32_t *__restrict__ block_bits, float *__restrict__ zndc, Partition part) {
+            uint32_t *__restrict__ block_bits, float *__restrict__ zndc, Partition part, uint32_t early) {
   __shared__ __align__(16) uint32_t s_view[256 * 10];
   __shared__ __align__(16) Chunk s_chunk;
   const uint32_t idx = blockIdx.x * 256 + threadIdx.x;
   const bool chunked = blockIdx.x < a.chunkCount;
+  // early != 0: the host knows the predecessor is the depth sort of this asset (which reads and writes keys, order and the
+  // sort scratch only), so the whole body runs before the wait and overlaps the sort's last pass.  Pre-wait reads: the
+  // asset's blobs, fc, cutouts / deleted / selected (their uploads are copies, which complete before it starts); pre-wait writes: view_out,
+  // rect_out, draw_out, zndc and this CTA's bit of block_bits, which only the previous frame's binner and raster read, and
+  // those completed before the sort began.  Otherwise the kernel waits first: in a run, a view-calc may follow an emit that
+  // reads this asset's rect / block_bits.  The early kernel releases nothing itself (its successor is placed as it exits).
+  if (!early) {
+    chain_wait();
+    chain_release();
+  }
   if (chunked && threadIdx.x < 4)
     reinterpret_cast<uint4 *>(&s_chunk)[threadIdx.x] = __ldg(reinterpret_cast<const uint4 *>(a.chunks + blockIdx.x) + threadIdx.x);
   // the per-splat streams do not depend on the chunk header: start them before the barrier so the CTA pays one
@@ -359,7 +383,9 @@ k_calc_view(AssetView a, FrameConsts fc, const GsCutout *__restrict__ cutouts, c
     __syncthreads();
     if (s_cull) {
       if (idx < a.n) rect_out[idx] = kRectEmpty;
-      return;   // block_bits was zeroed before the launch: nothing to set
+      if (threadIdx.x == 0) atomicAnd(block_bits + (blockIdx.x >> 5), ~(1u << (blockIdx.x & 31u)));
+      if (early) chain_wait();
+      return;
     }
   }
 
@@ -626,15 +652,21 @@ k_calc_view(AssetView a, FrameConsts fc, const GsCutout *__restrict__ cutouts, c
     }
     rect_out[idx] = rect;
   }
-  {  // one BIT per 256-splat block: "some splat of this block has a bin rectangle" (zeroed before the launch, set here).  The
+  {  // one BIT per 256-splat block: "some splat of this block has a bin rectangle" (set or cleared here, by its CTA).  The
      // binner walks the draw order and gathers a splat's rectangle only when its block's bit is set; the bitmap (n/2048 bytes:
      // 3 KB for cfg2) sits in the binner's shared memory, so the per-entry test is a shared-memory read and the random
      // 4-byte gathers are paid for blocks with something to draw only (every other GPU's blocks drop out in a group).
     const int any = __syncthreads_or(rect != kRectEmpty);
-    if (threadIdx.x == 0 && any) atomicOr(block_bits + (blockIdx.x >> 5), 1u << (blockIdx.x & 31u));
+    if (threadIdx.x == 0) {
+      if (any) atomicOr(block_bits + (blockIdx.x >> 5), 1u << (blockIdx.x & 31u));
+      else atomicAnd(block_bits + (blockIdx.x >> 5), ~(1u << (blockIdx.x & 31u)));
+    }
   }
 
-  if (CULL) return;   // fused frame: the compositor reads the 48-byte draw records; _SplatViewData is not materialised
+  if (CULL) {
+    if (early) chain_wait();
+    return;
+  }   // fused frame: the compositor reads the 48-byte draw records; _SplatViewData is not materialised
   // ---- coalesced store of the CTA's 256 x 40-byte records ----
 #pragma unroll
   for (int k = 0; k < 10; ++k) s_view[threadIdx.x * 10 + k] = vw[k];
@@ -647,6 +679,7 @@ k_calc_view(AssetView a, FrameConsts fc, const GsCutout *__restrict__ cutouts, c
   for (uint32_t q = threadIdx.x; q * 4 + 3 < words; q += 256) dst[q] = src[q];
   // tail words when cnt*10 is not a multiple of 4 (only the last CTA)
   for (uint32_t wi = (words & ~3u) + threadIdx.x; wi < words; wi += 256) view_out[(uint64_t)first * 10 + wi] = s_view[wi];
+  if (early) chain_wait();
 }
 
 // ------------------------------------------------------------------------------------------
@@ -664,22 +697,25 @@ void launch_calc_distances(const AssetView &a, const FrameConsts &fc, uint32_t *
   const float4 row = make_float4(fc.sort_row[0], fc.sort_row[1], fc.sort_row[2], fc.sort_row[3]);
   SlabArgs none{};
   if (slabs && slabs->count > 1) cudaMemsetAsync(slabs->group_bits, 0, group_bits_words(a.n) * sizeof(uint32_t), s);
-  if (!slabs || slabs->count <= 1) k_calc_distances<0><<<grid, 256, 0, s>>>(a, row, key_table, ghist, none);
-  else if (slabs->count <= 2) k_calc_distances<1><<<grid, 256, 0, s>>>(a, row, key_table, ghist, *slabs);
-  else if (slabs->count <= 4) k_calc_distances<3><<<grid, 256, 0, s>>>(a, row, key_table, ghist, *slabs);
-  else if (slabs->count <= 8) k_calc_distances<7><<<grid, 256, 0, s>>>(a, row, key_table, ghist, *slabs);
-  else k_calc_distances<kMaxSlabs - 1><<<grid, 256, 0, s>>>(a, row, key_table, ghist, *slabs);
+  if (!slabs || slabs->count <= 1) chain_launch(k_calc_distances<0>, grid, 256, 0, s, a, row, key_table, ghist, none);
+  else if (slabs->count <= 2) chain_launch(k_calc_distances<1>, grid, 256, 0, s, a, row, key_table, ghist, *slabs);
+  else if (slabs->count <= 4) chain_launch(k_calc_distances<3>, grid, 256, 0, s, a, row, key_table, ghist, *slabs);
+  else if (slabs->count <= 8) chain_launch(k_calc_distances<7>, grid, 256, 0, s, a, row, key_table, ghist, *slabs);
+  else chain_launch(k_calc_distances<kMaxSlabs - 1>, grid, 256, 0, s, a, row, key_table, ghist, *slabs);
 }
 
 template <bool CULL>
 static void launch_calc_view_t(const AssetView &a, const FrameConsts &fc, const GsCutout *cutouts, const uint32_t *deleted, const uint32_t *selected, uint32_t *view,
-                               uint32_t *rect, float4 *draw, uint32_t *block_bits, float *zndc, const Partition &part, cudaStream_t s) {
-  const uint32_t grid = (a.n + 255) / 256;
+                               uint32_t *rect, float4 *draw, uint32_t *block_bits, float *zndc, const Partition &part, bool after_sort,
+                               cudaStream_t s) {
+  const uint32_t grid = (a.n + 255) / 256, early = after_sort ? 1u : 0u;
   // BC7 colour (VeryLow preset) is a separate instantiation: the block decode must not cost the other formats registers
 #define GS_VIEW(SH)                                                                                                        \
   do {                                                                                                                    \
-    if (a.colFmt == 3) k_calc_view<SH, CULL, true><<<grid, 256, 0, s>>>(a, fc, cutouts, deleted, selected, view, rect, draw, block_bits, zndc, part);  \
-    else k_calc_view<SH, CULL, false><<<grid, 256, 0, s>>>(a, fc, cutouts, deleted, selected, view, rect, draw, block_bits, zndc, part);               \
+    if (a.colFmt == 3)                                                                                                    \
+      chain_launch(k_calc_view<SH, CULL, true>, grid, 256, 0, s, a, fc, cutouts, deleted, selected, view, rect, draw, block_bits, zndc, part, early); \
+    else                                                                                                                  \
+      chain_launch(k_calc_view<SH, CULL, false>, grid, 256, 0, s, a, fc, cutouts, deleted, selected, view, rect, draw, block_bits, zndc, part, early); \
   } while (0)
   switch (a.shFmt) {
     case 0: GS_VIEW(0); break;
@@ -692,11 +728,12 @@ static void launch_calc_view_t(const AssetView &a, const FrameConsts &fc, const 
 }
 
 void launch_calc_view(const AssetView &a, const FrameConsts &fc, const GsCutout *cutouts, const uint32_t *deleted, const uint32_t *selected, uint32_t *view,
-                      uint32_t *rect, float4 *draw, uint32_t *block_bits, float *zndc, bool cull_undrawable, const Partition &part, cudaStream_t s) {
+                      uint32_t *rect, float4 *draw, uint32_t *block_bits, float *zndc, bool cull_undrawable, const Partition &part, cudaStream_t s,
+                      bool after_sort) {
   if (!a.n) return;
-  cudaMemsetAsync(block_bits, 0, block_bits_words(a.n) * sizeof(uint32_t), s);
-  if (cull_undrawable) launch_calc_view_t<true>(a, fc, cutouts, deleted, selected, view, rect, draw, block_bits, zndc, part, s);
-  else launch_calc_view_t<false>(a, fc, cutouts, deleted, selected, view, rect, draw, block_bits, zndc, part, s);
+  // no clear of block_bits: every CTA sets or clears its own bit
+  if (cull_undrawable) launch_calc_view_t<true>(a, fc, cutouts, deleted, selected, view, rect, draw, block_bits, zndc, part, after_sort, s);
+  else launch_calc_view_t<false>(a, fc, cutouts, deleted, selected, view, rect, draw, block_bits, zndc, part, after_sort, s);
 }
 
 }  // namespace gs
