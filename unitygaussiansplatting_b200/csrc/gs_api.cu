@@ -299,11 +299,11 @@ static int do_sort(GsContext *ctx, GsAsset *as, const FrameConsts &fc) {
   cl.ptr[1] = sc.lookback; cl.words[1] = sort_lookback_words(as->av.n, 4);
   cl.ptr[2] = sc.tickets; cl.words[2] = 4;
   launch_clear(cl, ctx->stream, /*release_first=*/true);
-  launch_calc_distances(as->av, fc, as->key_table, sc.ghist, ctx->stream);
+  launch_calc_distances(as->av, fc, as->key_table.get(), sc.ghist, ctx->stream);
   rec(ctx, EV_DIST);
   cudaEvent_t pe[5] = {ctx->ev[EV_SORT0], ctx->ev[EV_SORT1], ctx->ev[EV_SORT2], ctx->ev[EV_SORT3], ctx->ev[EV_SORT4]};
-  GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order, as->d_n, as->av.n, 4, 8, true, sc, ctx->stream, ctx->timing ? pe : nullptr,
-                                     as->key_table, true, nullptr, nullptr, /*scratch_clear=*/true));
+  GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys.get(), as->order.get(), as->d_n.get(), as->av.n, 4, 8, true, sc, ctx->stream,
+                                     ctx->timing ? pe : nullptr, as->key_table.get(), true, nullptr, nullptr, /*scratch_clear=*/true));
   if (ctx->timing) for (int e = EV_SORT0; e <= EV_SORT4; ++e) ctx->ev_valid[e] = true;
   ctx->launches += 1 + 4;
   GS_CUDA_TRY(ctx, cudaGetLastError());
@@ -324,17 +324,17 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
   const bool own = stream == ctx->stream;   // the group path runs view-calc beside the sort on a second stream and times it itself
   if (own) rec(ctx, EV_VIEW0);
   if (draw) {   // a record slab: the asset's own records stay as they are
-    launch_calc_view(as->av, fc, ctx->d_cutouts.get(), ctx->d_deleted.get(), ctx->d_selected.get(), as->view, as->rect, draw, as->block_bits,
-                     fp->scene_depth ? zndc : nullptr, cull, make_partition(opt), stream, after_sort);
+    launch_calc_view(as->av, fc, ctx->d_cutouts.get(), ctx->d_deleted.get(), ctx->d_selected.get(), as->view.get(), as->rect.get(), draw,
+                     as->block_bits.get(), fp->scene_depth ? zndc : nullptr, cull, make_partition(opt), stream, after_sort);
     if (own) rec(ctx, EV_VIEW1);
     ctx->launches += 1;
     GS_CUDA_TRY(ctx, cudaGetLastError());
     return GS_OK;
   }
-  if (fp->scene_depth && !as->zndc) GS_CUDA_TRY(ctx, cudaMalloc(&as->zndc, (size_t)as->av.n * sizeof(float) + 16));
+  if (fp->scene_depth) GS_CUDA_TRY(ctx, as->zndc.reserve((size_t)as->av.n + 4, {ctx->stream}));   // 16 bytes of slack
   as->zndc_valid = fp->scene_depth != nullptr;
-  launch_calc_view(as->av, fc, ctx->d_cutouts.get(), ctx->d_deleted.get(), ctx->d_selected.get(), as->view, as->rect, as->draw, as->block_bits,
-                   as->zndc_valid ? as->zndc : nullptr, cull, make_partition(opt), stream, after_sort);
+  launch_calc_view(as->av, fc, ctx->d_cutouts.get(), ctx->d_deleted.get(), ctx->d_selected.get(), as->view.get(), as->rect.get(), as->draw.get(),
+                   as->block_bits.get(), as->zndc_valid ? as->zndc.get() : nullptr, cull, make_partition(opt), stream, after_sort);
   if (own) rec(ctx, EV_VIEW1);
   ctx->launches += 1;
   as->view_valid = !cull;
@@ -401,21 +401,21 @@ int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, G
   if ((rc = bind_depth(ctx, fp, &depth))) return rc;
   BinScratch lists;
   int bin_launches = 0, more = 0;
-  GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order, as->rect, as->block_bits, n, first, bin_scratch(ctx), sort_scratch(ctx), ctx->stream, &lists,
-                                  &bin_launches));
+  GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order.get(), as->rect.get(), as->block_bits.get(), n, first, bin_scratch(ctx), sort_scratch(ctx),
+                                  ctx->stream, &lists, &bin_launches));
   bool again = false;
   if ((rc = grow_bin_list(ctx, fc, n, &again))) return rc;
   if (again) {
     // the grown list fits: the flag this draw set is cleared again, unless an earlier draw of the call left its list truncated
     const bool clear = first || !ctx->bin_overflow;
-    GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order, as->rect, as->block_bits, n, clear, bin_scratch(ctx), sort_scratch(ctx), ctx->stream, &lists,
-                                    &more));
+    GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order.get(), as->rect.get(), as->block_bits.get(), n, clear, bin_scratch(ctx), sort_scratch(ctx),
+                                    ctx->stream, &lists, &more));
     bin_launches += more;
     ctx->bin_overflow = !clear;
   }
   rec(ctx, EV_BIN1);
   if (bin_done) cudaEventRecord(bin_done, ctx->stream);
-  launch_raster(fc, opt, as->draw, fp->scene_depth ? as->zndc : nullptr, fp->selected_bits != nullptr || fp->scene_depth != nullptr,
+  launch_raster(fc, opt, as->draw.get(), fp->scene_depth ? as->zndc.get() : nullptr, fp->selected_bits != nullptr || fp->scene_depth != nullptr,
                 lists, d_rt, pitch, fmt, surf, ctx->stream, depth);
   rec(ctx, EV_RASTER1);
   ctx->launches += bin_launches + 3;  // look-back clear + bin_emit, 1-2 sort passes; bin_ranges, tile_order, raster
@@ -479,22 +479,24 @@ static int init_staging(GsContext *ctx, const GsRenderOptions &opt, void *d_rt, 
 
 cudaError_t asset_init_work(GsContext *ctx, GsAsset *as, uint32_t n, uint32_t pos_fmt, uint32_t scale_fmt, uint32_t sh_fmt,
                             uint32_t col_fmt, uint32_t chunk_count) {
+  const cudaStream_t s = ctx->stream;
   cudaError_t e = cudaSuccess;
-  if ((e = cudaMalloc(&as->order, (size_t)n * 4)) != cudaSuccess || (e = cudaMalloc(&as->keys, (size_t)n * 4)) != cudaSuccess ||
-      (e = cudaMalloc(&as->key_table, (size_t)n * 4)) != cudaSuccess || (e = cudaMalloc(&as->draw, (size_t)n * 48)) != cudaSuccess ||
-      (e = cudaMalloc(&as->view, (size_t)n * kViewStride + 16)) != cudaSuccess || (e = cudaMalloc(&as->rect, (size_t)n * 4)) != cudaSuccess ||
-      (e = cudaMalloc(&as->d_n, 4)) != cudaSuccess || (e = cudaMalloc(&as->block_bits, block_bits_words(n) * 4 + 64)) != cudaSuccess)
+  // view: 16 bytes of slack; block_bits: 64
+  if ((e = as->order.reserve(n, {s})) != cudaSuccess || (e = as->keys.reserve(n, {s})) != cudaSuccess ||
+      (e = as->key_table.reserve(n, {s})) != cudaSuccess || (e = as->draw.reserve((size_t)n * 3, {s})) != cudaSuccess ||
+      (e = as->view.reserve((size_t)n * kViewStride / 4 + 4, {s})) != cudaSuccess || (e = as->rect.reserve(n, {s})) != cudaSuccess ||
+      (e = as->d_n.reserve(1, {s})) != cudaSuccess || (e = as->block_bits.reserve(block_bits_words(n) + 16, {s})) != cudaSuccess)
     return e;
-  if ((e = cudaMemcpyAsync(as->d_n, &n, 4, cudaMemcpyHostToDevice, ctx->stream)) != cudaSuccess) return e;
+  if ((e = cudaMemcpyAsync(as->d_n.get(), &n, 4, cudaMemcpyHostToDevice, s)) != cudaSuccess) return e;
   as->av.n = n;
   as->av.posFmt = pos_fmt; as->av.scaleFmt = scale_fmt; as->av.shFmt = sh_fmt; as->av.colFmt = col_fmt;
   as->av.chunkCount = chunk_count;
-  as->av.pos = (const uint8_t *)as->d_pos; as->av.other = (const uint8_t *)as->d_other; as->av.sh = (const uint8_t *)as->d_sh;
-  as->av.color = (const uint8_t *)as->d_color; as->av.chunks = (const Chunk *)as->d_chunks;
-  launch_set_indices(as->order, as->av.n, ctx->stream);  // CSSetIndices
+  as->av.pos = as->d_pos.get(); as->av.other = as->d_other.get(); as->av.sh = as->d_sh.get();
+  as->av.color = as->d_color.get(); as->av.chunks = (const Chunk *)as->d_chunks.get();
+  launch_set_indices(as->order.get(), as->av.n, s);  // CSSetIndices
   ctx->launches += 1;
   // `n` is a stack value: the copy above must have left it before this returns
-  return cudaStreamSynchronize(ctx->stream);
+  return cudaStreamSynchronize(s);
 }
 
 static int check_bin_overflow(GsContext *ctx) {
@@ -642,23 +644,24 @@ int gs_asset_upload(GsContext *ctx, const GsAssetDesc *d, GsAsset **out) {
   GsAsset *as = new (std::nothrow) GsAsset();
   if (!as) return fail(ctx, GS_ERR_OUT_OF_MEMORY, "host allocation failed");
   as->ctx = ctx;
-  auto up = [&](void **dst, const void *src, uint64_t bytes, uint64_t min_bytes = 0) -> cudaError_t {
+  auto up = [&](gs::Buffer<uint8_t> &dst, const void *src, uint64_t bytes, uint64_t min_bytes = 0) -> cudaError_t {
     // +16 bytes of slack: the widest vector load of the last splat may read past a tightly sized blob
     const uint64_t alloc = (bytes > min_bytes ? bytes : min_bytes) + 16;
-    cudaError_t e = cudaMalloc(dst, alloc);
+    cudaError_t e = dst.reserve(alloc, {ctx->stream});
     if (e != cudaSuccess) return e;
-    e = cudaMemsetAsync((uint8_t *)*dst + bytes, 0, alloc - bytes, ctx->stream);
+    e = cudaMemsetAsync(dst.get() + bytes, 0, alloc - bytes, ctx->stream);
     if (e != cudaSuccess) return e;
-    return cudaMemcpyAsync(*dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
+    return cudaMemcpyAsync(dst.get(), src, bytes, cudaMemcpyHostToDevice, ctx->stream);
   };
   // a u16 palette index can name any of 65536 entries whatever the palette's nominal size: back all of them (zeros)
   const uint64_t sh_min = clustered ? 65536ull * 96ull : 0ull;
   cudaError_t e = cudaSuccess;
-  if ((e = up(&as->d_pos, d->pos, d->pos_bytes)) != cudaSuccess || (e = up(&as->d_other, d->other, d->other_bytes)) != cudaSuccess ||
-      (e = up(&as->d_sh, d->sh, d->sh_bytes, sh_min)) != cudaSuccess || (e = up(&as->d_color, d->color, d->color_bytes)) != cudaSuccess ||
-      (chunk_count && (e = up(&as->d_chunks, d->chunks, (uint64_t)chunk_count * 64)) != cudaSuccess) ||
+  if ((e = up(as->d_pos, d->pos, d->pos_bytes)) != cudaSuccess || (e = up(as->d_other, d->other, d->other_bytes)) != cudaSuccess ||
+      (e = up(as->d_sh, d->sh, d->sh_bytes, sh_min)) != cudaSuccess || (e = up(as->d_color, d->color, d->color_bytes)) != cudaSuccess ||
+      (chunk_count && (e = up(as->d_chunks, d->chunks, (uint64_t)chunk_count * 64)) != cudaSuccess) ||
       (e = asset_init_work(ctx, as, d->splat_count, d->pos_format, d->scale_format, d->sh_format, d->color_format, chunk_count)) != cudaSuccess) {
     gs_asset_destroy(as);
+    cudaGetLastError();   // a failed copy or launch leaves its error behind: the next call on the context must not report it
     return fail_cuda(ctx, e, "asset upload", __FILE__, __LINE__);
   }
   GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // host blobs are only borrowed for this call
@@ -669,14 +672,12 @@ int gs_asset_upload(GsContext *ctx, const GsAssetDesc *d, GsAsset **out) {
 void gs_asset_destroy(GsAsset *as) {
   if (!as) return;
   if (as->ctx) { cudaSetDevice(as->ctx->device); cudaStreamSynchronize(as->ctx->stream); }
-  cudaFree(as->d_pos); cudaFree(as->d_other); cudaFree(as->d_sh); cudaFree(as->d_color); cudaFree(as->d_chunks);
-  cudaFree(as->order); cudaFree(as->keys); cudaFree(as->key_table); cudaFree(as->draw); cudaFree(as->view); cudaFree(as->rect); cudaFree(as->d_n); cudaFree(as->block_bits); cudaFree(as->zndc); cudaFree(as->slab_mask); cudaFree(as->order_tmp); cudaFree(as->order_alt); cudaFree(as->slab_group_bits);
   delete as;
 }
 
 int gs_asset_reset_order(GsAsset *as) {
   if (!as) return fail(nullptr, GS_ERR_INVALID_ARGUMENT, "null asset");
-  launch_set_indices(as->order, as->av.n, as->ctx->stream);
+  launch_set_indices(as->order.get(), as->av.n, as->ctx->stream);
   as->ctx->launches += 1;
   GS_CUDA_TRY(as->ctx, cudaGetLastError());
   return GS_OK;
@@ -1048,7 +1049,7 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
     for (; emitted < end; ++emitted) {
       const GsAsset *as = assets[pair_at[emitted]];
       const RasterCamera &r = dc.cam[seg_of[emitted]];
-      launch_bin_emit_pair(as->order, as->rect, as->block_bits, as->av.n, r.binsX, r.bin_base, emitted, clear && emitted == 0, bins,
+      launch_bin_emit_pair(as->order.get(), as->rect.get(), as->block_bits.get(), as->av.n, r.binsX, r.bin_base, emitted, clear && emitted == 0, bins,
                            bin_scratch(ctx), ctx->cams_ghist.get(), ctx->stream);
       ctx->launches += 2;   // look-back clear, bin_emit
     }
@@ -1068,9 +1069,9 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
     const bool sorted = do_sort_flags[pair_at[p]] != 0;
     if (sorted && (rc = do_sort(ctx, as, c.fcs[pair_at[p] - c.off]))) return rc;
     if ((rc = do_view(ctx, as, &f, c.fcs[pair_at[p] - c.off], true, opt, ctx->stream, draw, zndc, sorted))) return rc;
-    objs.draw[p] = draw ? draw : as->draw;
+    objs.draw[p] = draw ? draw : as->draw.get();
     if (f.scene_depth) {
-      objs.zndc[p] = draw ? zndc : as->zndc;
+      objs.zndc[p] = draw ? zndc : as->zndc.get();
       objs.depth_mask |= 1u << p;
     }
     objs.extras |= f.selected_bits != nullptr || f.scene_depth != nullptr;
@@ -1259,21 +1260,17 @@ int gs_sort_pairs_device(GsContext *ctx, uint32_t *d_keys, uint32_t *d_payload, 
 int gs_sort_pairs_host(GsContext *ctx, uint32_t *keys, uint32_t *payload, uint32_t count) {
   if (!ctx || (count && (!keys || !payload))) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null argument");
   if (count == 0) return GS_OK;
-  uint32_t *dk = nullptr, *dv = nullptr;
-  GS_CUDA_TRY(ctx, cudaMalloc(&dk, (size_t)count * 4));
-  cudaError_t e = cudaMalloc(&dv, (size_t)count * 4);
-  if (e != cudaSuccess) { cudaFree(dk); return fail_cuda(ctx, e, "cudaMalloc", __FILE__, __LINE__); }
-  cudaMemcpyAsync(dk, keys, (size_t)count * 4, cudaMemcpyHostToDevice, ctx->stream);
-  cudaMemcpyAsync(dv, payload, (size_t)count * 4, cudaMemcpyHostToDevice, ctx->stream);
-  int rc = gs_sort_pairs_device(ctx, dk, dv, count);
-  if (rc == GS_OK) {
-    cudaMemcpyAsync(keys, dk, (size_t)count * 4, cudaMemcpyDeviceToHost, ctx->stream);
-    cudaMemcpyAsync(payload, dv, (size_t)count * 4, cudaMemcpyDeviceToHost, ctx->stream);
-    e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) rc = fail_cuda(ctx, e, "sort", __FILE__, __LINE__);
-  }
-  cudaFree(dk); cudaFree(dv);
-  return rc;
+  gs::Buffer<uint32_t> dk, dv;
+  GS_CUDA_TRY(ctx, dk.reserve(count, {ctx->stream}));
+  GS_CUDA_TRY(ctx, dv.reserve(count, {ctx->stream}));
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(dk.get(), keys, (size_t)count * 4, cudaMemcpyHostToDevice, ctx->stream));
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(dv.get(), payload, (size_t)count * 4, cudaMemcpyHostToDevice, ctx->stream));
+  int rc = gs_sort_pairs_device(ctx, dk.get(), dv.get(), count);
+  if (rc) return rc;
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(keys, dk.get(), (size_t)count * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(payload, dv.get(), (size_t)count * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return GS_OK;
 }
 
 // ---- test hooks -------------------------------------------------------------------------------------
@@ -1284,11 +1281,11 @@ static int readback(GsAsset *as, void *dst, const void *src, size_t bytes) {
   GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return GS_OK;
 }
-int gs_readback_order(GsAsset *as, uint32_t *dst) { return readback(as, dst, as ? as->order : nullptr, as ? (size_t)as->av.n * 4 : 0); }
-int gs_readback_keys(GsAsset *as, uint32_t *dst) { return readback(as, dst, as ? as->keys : nullptr, as ? (size_t)as->av.n * 4 : 0); }
+int gs_readback_order(GsAsset *as, uint32_t *dst) { return readback(as, dst, as ? as->order.get() : nullptr, as ? (size_t)as->av.n * 4 : 0); }
+int gs_readback_keys(GsAsset *as, uint32_t *dst) { return readback(as, dst, as ? as->keys.get() : nullptr, as ? (size_t)as->av.n * 4 : 0); }
 int gs_readback_view(GsAsset *as, void *dst) {
   if (as && !as->view_valid) return fail(as->ctx, GS_ERR_NOT_READY, "_SplatViewData is only materialised by gs_calc_view (gs_frame hands the draw its own records)");
-  return readback(as, dst, as ? as->view : nullptr, as ? (size_t)as->av.n * kViewStride : 0);
+  return readback(as, dst, as ? as->view.get() : nullptr, as ? (size_t)as->av.n * kViewStride : 0);
 }
 int gs_export_splats(GsContext *ctx, GsAsset *as, const GsCutout *cutouts, uint32_t cutout_count, uint32_t bake_transform, void *dst) {
   if (!ctx || !as || !dst || (cutout_count && !cutouts)) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null argument");
@@ -1300,21 +1297,19 @@ int gs_export_splats(GsContext *ctx, GsAsset *as, const GsCutout *cutouts, uint3
   fp.cutouts = cutouts; fp.cutout_count = cutout_count;
   int rc = upload_frame_inputs(ctx, as, &fp, ctx->stream);
   if (rc != GS_OK) return rc;
-  float *d_out = nullptr;
-  const size_t bytes = (size_t)as->av.n * 62 * sizeof(float);
-  GS_CUDA_TRY(ctx, cudaMalloc(&d_out, bytes));
-  launch_export_data(as->av, cutout_count, ctx->d_cutouts.get(), d_out, ctx->stream);
+  gs::Buffer<float> d_out;
+  const size_t floats = (size_t)as->av.n * 62;
+  GS_CUDA_TRY(ctx, d_out.reserve(floats, {ctx->stream}));
+  launch_export_data(as->av, cutout_count, ctx->d_cutouts.get(), d_out.get(), ctx->stream);
   ctx->launches += 1;
-  cudaError_t e = cudaMemcpyAsync(dst, d_out, bytes, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  cudaFree(d_out);
-  if (e != cudaSuccess) return fail_cuda(ctx, e, "gs_export_splats", __FILE__, __LINE__);
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(dst, d_out.get(), floats * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+  GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return GS_OK;
 }
 
 int gs_upload_order(GsAsset *as, const uint32_t *src) {
   if (!as || !src) return fail(as ? as->ctx : nullptr, GS_ERR_INVALID_ARGUMENT, "null argument");
-  GS_CUDA_TRY(as->ctx, cudaMemcpyAsync(as->order, src, (size_t)as->av.n * 4, cudaMemcpyHostToDevice, as->ctx->stream));
+  GS_CUDA_TRY(as->ctx, cudaMemcpyAsync(as->order.get(), src, (size_t)as->av.n * 4, cudaMemcpyHostToDevice, as->ctx->stream));
   GS_CUDA_TRY(as->ctx, cudaStreamSynchronize(as->ctx->stream));
   return GS_OK;
 }
@@ -1368,7 +1363,7 @@ int gs_debug_sort_phases(GsContext *ctx, uint64_t *out, uint32_t max_words, uint
 void *gs_context_stream(GsContext *ctx) { return ctx ? (void *)ctx->stream : nullptr; }
 void *gs_asset_device_ptr(GsAsset *as, int which) {
   if (!as) return nullptr;
-  return which == 0 ? (void *)as->order : which == 1 ? (void *)as->keys : which == 2 ? (void *)as->view : nullptr;
+  return which == 0 ? (void *)as->order.get() : which == 1 ? (void *)as->keys.get() : which == 2 ? (void *)as->view.get() : nullptr;
 }
 
 }  // extern "C"

@@ -27,6 +27,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <new>
+#include <utility>
 #include <vector>
 
 #include "gs_internal.cuh"
@@ -83,8 +84,9 @@ struct PeerLink {
   GsAsset *asset = nullptr;
   uint32_t *buf[2] = {nullptr, nullptr};                       // local: the asset's two order buffers, by fixed index
   uint32_t *peer_buf[2][GS_GROUP_MAX_GPUS] = {};               // the same two buffers of every rank (own rank: local)
-  uint32_t *flags = nullptr, *peer_flags[GS_GROUP_MAX_GPUS] = {};   // flags[c] = last sort frame whose slab rank c delivered here
-  uint32_t *d_done = nullptr;                                   // block counter of the push kernel
+  Buffer<uint32_t> flags;                                       // flags[c] = last sort frame whose slab rank c delivered here
+  uint32_t *peer_flags[GS_GROUP_MAX_GPUS] = {};                 // the flags of every rank (own rank: local)
+  Buffer<uint32_t> d_done;                                      // block counter of the push kernel
   void *opened[3 * GS_GROUP_MAX_GPUS] = {};
   int n_opened = 0;
   uint32_t sort_frames = 0;
@@ -167,9 +169,10 @@ int member_rows(Member &mb, uint32_t rows) {
 int member_asset(Member &mb, GsAsset *as) {   // per-asset buffers only the group path needs
   GsContext *ctx = mb.ctx;
   const uint32_t n = as->av.n;
-  if (!as->slab_mask) GS_CUDA_TRY(ctx, cudaMalloc(&as->slab_mask, ((size_t)(n + 1023) / 1024) * 128 + 64));
-  if (!as->order_tmp) GS_CUDA_TRY(ctx, cudaMalloc(&as->order_tmp, (size_t)n * 4 + 16));
-  if (!as->slab_group_bits) GS_CUDA_TRY(ctx, cudaMalloc(&as->slab_group_bits, group_bits_words(n) * 4 + 64));
+  // slack: 64 bytes on the bit masks, 16 on order_tmp
+  GS_CUDA_TRY(ctx, as->slab_mask.reserve(((size_t)(n + 1023) / 1024) * 32 + 16, {ctx->stream}));
+  GS_CUDA_TRY(ctx, as->order_tmp.reserve((size_t)n + 4, {ctx->stream}));
+  GS_CUDA_TRY(ctx, as->slab_group_bits.reserve(group_bits_words(n) + 16, {ctx->stream}));
   GS_CUDA_TRY(ctx, mb.buf.cmp_status.reserve(compact_status_words(n), {ctx->stream}));
   return ensure_sort_scratch(ctx, n);
 }
@@ -301,33 +304,34 @@ int peer_link_setup(GsGroup *g, GsAsset *as) {
   static_assert(sizeof(Pack) == 3 * 64 + 64, "pack layout");
   Pack mine;
   memset(&mine, 0, sizeof(mine));
-  bool ok = true;
-  if (!as->order_alt) ok = cudaMalloc(&as->order_alt, (size_t)n * 4 + 16) == cudaSuccess;
-  if (ok && !k.flags) ok = cudaMalloc(&k.flags, 64 * 4) == cudaSuccess && cudaMalloc(&k.d_done, 16) == cudaSuccess;
+  // order_alt: 16 bytes of slack.  An earlier link's exchanges may have left the n-element buffer that was the order in
+  // order_alt; it is kept, not reallocated, as a peer of that link may still map it
+  bool ok = (as->order_alt.get() || as->order_alt.reserve((size_t)n + 4, {ctx->stream}) == cudaSuccess) &&
+            k.flags.reserve(64, {ctx->stream}) == cudaSuccess && k.d_done.reserve(4, {ctx->stream}) == cudaSuccess;
   if (ok) {
-    cudaMemsetAsync(k.flags, 0, 64 * 4, ctx->stream);
-    cudaMemsetAsync(k.d_done, 0, 16, ctx->stream);
-    cudaMemsetAsync(as->order_alt, 0, (size_t)n * 4, ctx->stream);
-    ok = cudaIpcGetMemHandle(&mine.h[0], as->order) == cudaSuccess && cudaIpcGetMemHandle(&mine.h[1], as->order_alt) == cudaSuccess &&
-         cudaIpcGetMemHandle(&mine.h[2], k.flags) == cudaSuccess;
+    cudaMemsetAsync(k.flags.get(), 0, 64 * 4, ctx->stream);
+    cudaMemsetAsync(k.d_done.get(), 0, 16, ctx->stream);
+    cudaMemsetAsync(as->order_alt.get(), 0, (size_t)n * 4, ctx->stream);
+    ok = cudaIpcGetMemHandle(&mine.h[0], as->order.get()) == cudaSuccess && cudaIpcGetMemHandle(&mine.h[1], as->order_alt.get()) == cudaSuccess &&
+         cudaIpcGetMemHandle(&mine.h[2], k.flags.get()) == cudaSuccess;
   }
   cudaGetLastError();
   mine.ok = ok ? 1u : 0u;
-  Pack *d_all = nullptr;
+  Buffer<Pack> d_all;
   std::vector<Pack> all(G);
-  if (cudaMalloc(&d_all, sizeof(Pack) * G) != cudaSuccess) return fail(ctx, GS_ERR_OUT_OF_MEMORY, "peer link: device allocation failed");
-  cudaMemcpyAsync(d_all + mb.rank, &mine, sizeof(Pack), cudaMemcpyHostToDevice, ctx->stream);
-  ncclResult_t r = nc.AllGather(d_all + mb.rank, d_all, sizeof(Pack), ncclUint8, mb.comm, ctx->stream);
-  if (r != ncclSuccess) { cudaFree(d_all); return fail_nccl(ctx, r, "ncclAllGather(peer handles)"); }
-  cudaMemcpyAsync(all.data(), d_all, sizeof(Pack) * G, cudaMemcpyDeviceToHost, ctx->stream);
-  if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) { cudaFree(d_all); return fail(ctx, GS_ERR_CUDA, "peer link: handle exchange failed"); }
+  if (d_all.reserve(G, {ctx->stream}) != cudaSuccess) return fail(ctx, GS_ERR_OUT_OF_MEMORY, "peer link: device allocation failed");
+  cudaMemcpyAsync(d_all.get() + mb.rank, &mine, sizeof(Pack), cudaMemcpyHostToDevice, ctx->stream);
+  ncclResult_t r = nc.AllGather(d_all.get() + mb.rank, d_all.get(), sizeof(Pack), ncclUint8, mb.comm, ctx->stream);
+  if (r != ncclSuccess) return fail_nccl(ctx, r, "ncclAllGather(peer handles)");
+  cudaMemcpyAsync(all.data(), d_all.get(), sizeof(Pack) * G, cudaMemcpyDeviceToHost, ctx->stream);
+  if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) return fail(ctx, GS_ERR_CUDA, "peer link: handle exchange failed");
   bool everyone = true;
   for (uint32_t c = 0; c < G; ++c) everyone &= all[c].ok != 0;
   uint32_t opened_ok = everyone ? 1u : 0u;
   if (everyone) {
-    k.buf[0] = as->order; k.buf[1] = as->order_alt;
+    k.buf[0] = as->order.get(); k.buf[1] = as->order_alt.get();
     for (uint32_t c = 0; c < G && opened_ok; ++c) {
-      if (c == mb.rank) { k.peer_buf[0][c] = k.buf[0]; k.peer_buf[1][c] = k.buf[1]; k.peer_flags[c] = k.flags; continue; }
+      if (c == mb.rank) { k.peer_buf[0][c] = k.buf[0]; k.peer_buf[1][c] = k.buf[1]; k.peer_flags[c] = k.flags.get(); continue; }
       void *ptr[3] = {nullptr, nullptr, nullptr};
       for (int j = 0; j < 3 && opened_ok; ++j) {
         if (cudaIpcOpenMemHandle(&ptr[j], all[c].h[j], cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { opened_ok = 0; cudaGetLastError(); break; }
@@ -337,13 +341,12 @@ int peer_link_setup(GsGroup *g, GsAsset *as) {
     }
   }
   // second round: did everybody manage to map everybody?
-  uint32_t *d_ok = reinterpret_cast<uint32_t *>(d_all);
+  uint32_t *d_ok = reinterpret_cast<uint32_t *>(d_all.get());
   cudaMemcpyAsync(d_ok + mb.rank, &opened_ok, 4, cudaMemcpyHostToDevice, ctx->stream);
   r = nc.AllGather(d_ok + mb.rank, d_ok, 4, ncclUint8, mb.comm, ctx->stream);
   std::vector<uint32_t> oks(G, 0);
   if (r == ncclSuccess) cudaMemcpyAsync(oks.data(), d_ok, 4 * G, cudaMemcpyDeviceToHost, ctx->stream);
   const bool synced = cudaStreamSynchronize(ctx->stream) == cudaSuccess;
-  cudaFree(d_all);
   if (r != ncclSuccess || !synced) return fail(ctx, GS_ERR_CUDA, "peer link: confirmation exchange failed");
   bool all_ok = true;
   for (uint32_t c = 0; c < G; ++c) all_ok &= oks[c] != 0;
@@ -355,10 +358,7 @@ void peer_link_release(GsGroup *g) {
   PeerLink &k = g->link;
   if (!g->m.empty() && g->m[0].ctx) { cudaSetDevice(g->m[0].ctx->device); cudaStreamSynchronize(g->m[0].ctx->stream); }
   for (int i = 0; i < k.n_opened; ++i) if (k.opened[i]) cudaIpcCloseMemHandle(k.opened[i]);
-  k.n_opened = 0;
-  cudaFree(k.flags); cudaFree(k.d_done);
-  k.flags = k.d_done = nullptr;
-  k.ready = false;
+  k = PeerLink();
   cudaGetLastError();
 }
 
@@ -526,7 +526,7 @@ int gs_group_sync(GsGroup *g) {
     mb.image_pending = false;
     if (g->link.ready && rc == GS_OK) {   // a peer that never delivered its slab made k_wait_slabs give up: the frame is void
       uint32_t bad = 0;
-      e = cudaMemcpy(&bad, g->link.flags + g->size, 4, cudaMemcpyDeviceToHost);
+      e = cudaMemcpy(&bad, g->link.flags.get() + g->size, 4, cudaMemcpyDeviceToHost);
       if (e != cudaSuccess) rc = fail_cuda(mb.ctx, e, "cudaMemcpy(peer flags)", __FILE__, __LINE__);
       else if (bad) rc = fail(mb.ctx, GS_ERR_CUDA, "peer-to-peer order exchange timed out: a process of the group did not deliver its slab");
     }
@@ -639,11 +639,12 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
         uint32_t *info = mb.buf.info.get() + (size_t)k * 2 * kMaxSlabs;
         SlabArgs sl;
         memset(&sl, 0, sizeof(sl));
-        sl.count = G; sl.index = mb.rank; sl.order_prev = as->order; sl.mask = as->slab_mask; sl.group_bits = as->slab_group_bits; sl.info = info;
+        sl.count = G; sl.index = mb.rank; sl.order_prev = as->order.get(); sl.mask = as->slab_mask.get();
+        sl.group_bits = as->slab_group_bits.get(); sl.info = info;
         for (uint32_t j = 0; j + 1 < G; ++j) sl.qpos[j] = (uint32_t)(((uint64_t)o.n * (j + 1)) / G);
         GS_CUDA_TRY(ctx, cudaMemsetAsync(ghist, 0, 4 * 256 * 4, ctx->stream));
         GS_CUDA_TRY(ctx, cudaMemsetAsync(info, 0, 2 * kMaxSlabs * 4, ctx->stream));
-        launch_calc_distances(as->av, o.fc, as->key_table, ghist, ctx->stream, &sl);
+        launch_calc_distances(as->av, o.fc, as->key_table.get(), ghist, ctx->stream, &sl);
         ctx->launches += 1;
         if (G > 1) {
           GS_CUDA_TRY(ctx, cudaMemcpyAsync(mb.buf.h_info.get() + (size_t)k * 2 * kMaxSlabs, info, 2 * kMaxSlabs * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -740,7 +741,7 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
       uint32_t *p2p_new = nullptr;
       int p2p_idx = 0;
       if (use_p2p) {   // the two order buffers alternate: last frame's order is read, the other one is assembled
-        p2p_idx = o.assets[0]->order == g->link.buf[0] ? 1 : 0;
+        p2p_idx = o.assets[0]->order.get() == g->link.buf[0] ? 1 : 0;
         p2p_new = g->link.buf[p2p_idx];
       }
       for (size_t i = 0; i < L; ++i) {
@@ -752,14 +753,15 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
         if (k) sc.ghist = mb.buf.ghist_more.get() + (size_t)(k - 1) * 4 * 256;
         const uint32_t cnt = o.slab_cnt[mb.rank], off = o.slab_off[mb.rank];
         if (G == 1) {
-          GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order, as->d_n, N, 4, 8, true, sc, ctx->stream, nullptr, as->key_table));
+          GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys.get(), as->order.get(), as->d_n.get(), N, 4, 8, true, sc, ctx->stream, nullptr,
+                                             as->key_table.get()));
           ctx->launches += 4;
         } else if (cnt) {
-          launch_compact_order(as->order, N, as->slab_mask, as->slab_group_bits, as->key_table, as->order_tmp, as->keys, mb.buf.cmp_status.get(),
-                               mb.buf.slab_count.get(), ctx->stream);
-          GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys, as->order_tmp, mb.buf.slab_count.get(), cnt, 4, 8, true, sc, ctx->stream, nullptr, nullptr,
-                                             true, as->keys + off,
-                                             use_p2p ? p2p_new + off : use_gather ? mb.buf.gather.get() + (size_t)mb.rank * cap : as->order + off));
+          launch_compact_order(as->order.get(), N, as->slab_mask.get(), as->slab_group_bits.get(), as->key_table.get(), as->order_tmp.get(),
+                               as->keys.get(), mb.buf.cmp_status.get(), mb.buf.slab_count.get(), ctx->stream);
+          GS_CUDA_TRY(ctx, launch_sort_pairs(as->keys.get(), as->order_tmp.get(), mb.buf.slab_count.get(), cnt, 4, 8, true, sc, ctx->stream, nullptr,
+                                             nullptr, true, as->keys.get() + off,
+                                             use_p2p ? p2p_new + off : use_gather ? mb.buf.gather.get() + (size_t)mb.rank * cap : as->order.get() + off));
           ctx->launches += 5;
         }
         if (use_p2p) {
@@ -769,12 +771,12 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
           memset(&pa, 0, sizeof(pa));
           for (uint32_t c = 0; c < G; ++c)
             if (c != mb.rank) { pa.dst[pa.npeers] = lk.peer_buf[p2p_idx][c] + off; pa.flag[pa.npeers] = lk.peer_flags[c] + mb.rank; ++pa.npeers; }
-          k_push_slab<<<sm_count(), 512, 0, ctx->stream>>>(p2p_new + off, cnt, pa, tag, lk.d_done);
-          k_wait_slabs<<<1, 32, 0, ctx->stream>>>(lk.flags, G, mb.rank, tag);
+          k_push_slab<<<sm_count(), 512, 0, ctx->stream>>>(p2p_new + off, cnt, pa, tag, lk.d_done.get());
+          k_wait_slabs<<<1, 32, 0, ctx->stream>>>(lk.flags.get(), G, mb.rank, tag);
           ctx->launches += 2;
-          // from here on the assembled buffer IS the draw order; last frame's becomes the next frame's target
-          as->order_alt = as->order;
-          as->order = p2p_new;
+          // from here on the assembled buffer (p2p_new, the one that was not the order) IS the draw order; last frame's becomes
+          // the next frame's target
+          std::swap(as->order, as->order_alt);
         }
         GS_CUDA_TRY(ctx, cudaGetLastError());
         if (timing) cudaEventRecord(mb.tev[GT_SORT], ctx->stream);
@@ -793,11 +795,11 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
             GS_CUDA_TRY(mb.ctx, cudaSetDevice(mb.ctx->device));
             for (uint32_t c = 0; c < G; ++c)
               if (o.slab_cnt[c])
-                GS_CUDA_TRY(mb.ctx, cudaMemcpyAsync(o.assets[i]->order + o.slab_off[c], mb.buf.gather.get() + (size_t)c * cap, (size_t)o.slab_cnt[c] * 4,
+                GS_CUDA_TRY(mb.ctx, cudaMemcpyAsync(o.assets[i]->order.get() + o.slab_off[c], mb.buf.gather.get() + (size_t)c * cap, (size_t)o.slab_cnt[c] * 4,
                                                     cudaMemcpyDeviceToDevice, mb.ctx->stream));
           }
         } else {
-          for (size_t i = 0; i < L; ++i) bufs[i] = reinterpret_cast<uint8_t *>(o.assets[i]->order);
+          for (size_t i = 0; i < L; ++i) bufs[i] = reinterpret_cast<uint8_t *>(o.assets[i]->order.get());
           if ((rc = exchange_begin(g)) || (rc = exchange_add(g, bufs.data(), off, cnt)) || (rc = exchange_end(g))) return rc;
         }
       }

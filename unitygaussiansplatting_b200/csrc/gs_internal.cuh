@@ -80,19 +80,20 @@ struct GsContext {
   std::vector<cudaEvent_t> spare_events;
 };
 
+// Its buffers are freed by gs_asset_destroy, with the context's device current and its stream drained.
 struct GsAsset {
   GsContext *ctx = nullptr;
   gs::AssetView av{};
-  void *d_pos = nullptr, *d_other = nullptr, *d_sh = nullptr, *d_color = nullptr, *d_chunks = nullptr;
-  uint32_t *order = nullptr, *keys = nullptr, *key_table = nullptr, *view = nullptr, *rect = nullptr, *d_n = nullptr;
-  uint32_t *block_bits = nullptr;  // bit j: some splat of block j (256 splats) got a bin rectangle from the last view-calc
+  gs::Buffer<uint8_t> d_pos, d_other, d_sh, d_color, d_chunks;   // the blobs (av points into them), 16 bytes of slack each
+  gs::Buffer<uint32_t> order, keys, key_table, view, rect, d_n;
+  gs::Buffer<uint32_t> block_bits;  // bit j: some splat of block j (256 splats) got a bin rectangle from the last view-calc
   // group path only (allocated by gs_group_*): slab membership (bit per splat, byte per 128), compaction output / sort ping-pong payload
-  uint32_t *slab_mask = nullptr, *order_tmp = nullptr;
-  float *zndc = nullptr;           // per-splat quad depth clip.z / clip.w, written by view-calc when a scene depth buffer is bound
+  gs::Buffer<uint32_t> slab_mask, order_tmp;
+  gs::Buffer<float> zndc;           // per-splat quad depth clip.z / clip.w, written by view-calc when a scene depth buffer is bound
   bool zndc_valid = false;
-  uint32_t *order_alt = nullptr;   // peer-to-peer order exchange: `order` and `order_alt` alternate as last / new draw order
-  uint32_t *slab_group_bits = nullptr;
-  float4 *draw = nullptr;  // raster-ready 48-byte records of the drawable splats
+  gs::Buffer<uint32_t> order_alt;   // peer-to-peer order exchange: `order` and `order_alt` alternate as last / new draw order
+  gs::Buffer<uint32_t> slab_group_bits;
+  gs::Buffer<float4> draw;  // raster-ready 48-byte records of the drawable splats (3 float4 each)
   bool view_valid = false;   // the full 40-byte _SplatViewData buffer is current (gs_calc_view)
   bool draw_valid = false;   // draw records + bin rects are current (gs_calc_view or gs_frame)
   uint32_t draw_part[3] = {0, 0, 1};   // the tile partition those records were culled for (count <= 1: complete)

@@ -17,6 +17,7 @@
 #include <cmath>
 #include <cstring>
 #include <new>
+#include <utility>
 #include <vector>
 
 #include "gs_internal.cuh"
@@ -725,44 +726,24 @@ __global__ void __launch_bounds__(128) k_bc7(const float4 *__restrict__ image, u
 }
 
 // ---- host side ----------------------------------------------------------------------------------------------------------
-// device allocations of one call, released on every return path
-struct DevBufs {
-  std::vector<void *> ptrs;
-  ~DevBufs() { for (void *p : ptrs) cudaFree(p); }
-  template <class T>
-  cudaError_t alloc(T **p, size_t bytes) {
-    *p = nullptr;
-    void *q = nullptr;
-    cudaError_t e = cudaMalloc(&q, bytes ? bytes : 1);
-    if (e == cudaSuccess) { ptrs.push_back(q); *p = (T *)q; }
-    return e;
-  }
-  void release(void *p) {   // ownership moves to the caller
-    for (void *&q : ptrs) if (q == p) q = nullptr;
-  }
-};
 #define PK_TRY(expr) GS_CUDA_TRY(ctx, expr)
 #define PK_LAUNCHED() GS_CUDA_TRY(ctx, cudaGetLastError())
 
 inline uint32_t blocks_for(uint64_t items, uint32_t per) { return (uint32_t)((items + per - 1) / per); }
 
 // labels[p] (may be NULL) / best[p] (may be NULL) = nearest of the k means for each of the npts points
-int nearest(GsContext *ctx, DevBufs &bufs, const float *data, uint32_t stride, uint32_t dim, uint32_t npts, const float *means, uint32_t k,
-            int32_t *labels, float *best, float **scratch_v, uint32_t **scratch_i, uint32_t *scratch_cap) {
+// scratch_v / scratch_i: the per-split partial results, grown to the largest call (final labelling)
+int nearest(GsContext *ctx, const float *data, uint32_t stride, uint32_t dim, uint32_t npts, const float *means, uint32_t k,
+            int32_t *labels, float *best, Buffer<float> &scratch_v, Buffer<uint32_t> &scratch_i) {
   const uint32_t ptiles = blocks_for(npts, kNP), ctiles = blocks_for(k, kNC);
   const uint32_t want = std::max(1u, (sm_count() * 4u) / std::max(1u, ptiles));
   const uint32_t splits = std::min(ctiles, std::min(want, 64u));
   const size_t need = (size_t)splits * npts;
-  if (need > *scratch_cap) {   // grows once to the largest call (final labelling)
-    float *v;
-    uint32_t *ix;
-    PK_TRY(bufs.alloc(&v, need * 4));
-    PK_TRY(bufs.alloc(&ix, need * 4));
-    *scratch_v = v; *scratch_i = ix; *scratch_cap = (uint32_t)need;
-  }
+  PK_TRY(scratch_v.reserve(need, {ctx->stream}));
+  PK_TRY(scratch_i.reserve(need, {ctx->stream}));
   const size_t smem = ((size_t)dim * kNP + 8 * kNC) * sizeof(float);
-  k_nearest<<<dim3(ptiles, splits), 256, smem, ctx->stream>>>(data, stride, dim, npts, means, k, *scratch_v, *scratch_i);
-  k_nearest_combine<<<blocks_for(npts, 256), 256, 0, ctx->stream>>>(*scratch_v, *scratch_i, npts, splits, labels, best);
+  k_nearest<<<dim3(ptiles, splits), 256, smem, ctx->stream>>>(data, stride, dim, npts, means, k, scratch_v.get(), scratch_i.get());
+  k_nearest_combine<<<blocks_for(npts, 256), 256, 0, ctx->stream>>>(scratch_v.get(), scratch_i.get(), npts, splits, labels, best);
   ctx->launches += 2;
   PK_LAUNCHED();
   return GS_OK;
@@ -771,7 +752,6 @@ int nearest(GsContext *ctx, DevBufs &bufs, const float *data, uint32_t stride, u
 // gsa_kmeans on the device.  data: n rows of `dim` floats at `stride`; d_means k x dim, d_labels n (device).
 int kmeans_device(GsContext *ctx, const float *data, uint32_t stride, uint32_t dim, uint32_t n, uint32_t batch, float passes,
                   float *d_means, uint32_t k, int32_t *d_labels) {
-  DevBufs bufs;
   cudaStream_t st = ctx->stream;
   batch = std::min(n, batch);
   const uint32_t m = std::min(10u * k, n);   // initialize_centroids' batch
@@ -791,32 +771,31 @@ int kmeans_device(GsContext *ctx, const float *data, uint32_t stride, uint32_t d
   ctx->pack_stats[1] = iters;
   ctx->pack_stats[2] = 3ull * (k - 1);
 
-  uint32_t *d_idx, *d_mb, *ticket;
-  float *d_cb, *d_vb, *min_dist, *partial, *cur, *best, *counts, *bpts;
-  uint8_t *taken;
-  int32_t *blab;
+  Buffer<uint32_t> d_idx, d_mb, ticket;
+  Buffer<float> d_cb, d_vb, min_dist, partial, cur, best, counts, bpts, sv;
+  Buffer<uint8_t> taken;
+  Buffer<int32_t> blab;
+  Buffer<uint32_t> si;
   const uint32_t nb = blocks_for(m, kSumBatch);
-  PK_TRY(bufs.alloc(&d_idx, (size_t)m * 4));
-  PK_TRY(bufs.alloc(&d_cb, (size_t)m * dim * 4));
-  PK_TRY(bufs.alloc(&d_vb, (size_t)m * dim * 4));
-  PK_TRY(bufs.alloc(&min_dist, (size_t)m * 4));
-  PK_TRY(bufs.alloc(&best, (size_t)m * 4));
-  PK_TRY(bufs.alloc(&taken, m));
-  PK_TRY(bufs.alloc(&partial, (size_t)nb * 4));
-  PK_TRY(bufs.alloc(&ticket, 4));
-  PK_TRY(bufs.alloc(&cur, (size_t)k * dim * 4));
-  PK_TRY(bufs.alloc(&counts, (size_t)k * 4));
-  PK_TRY(bufs.alloc(&d_mb, std::max<size_t>(mb.size(), 1) * 4));
-  PK_TRY(bufs.alloc(&bpts, (size_t)batch * dim * 4));
-  PK_TRY(bufs.alloc(&blab, (size_t)batch * 4));
-  float *sv = nullptr;
-  uint32_t *si = nullptr, scap = 0;
-  PK_TRY(cudaMemcpyAsync(d_idx, cb.data(), (size_t)m * 4, cudaMemcpyHostToDevice, st));
-  k_gather_rows<<<blocks_for((uint64_t)m * dim, 256), 256, 0, st>>>(data, stride, dim, d_idx, m, d_cb);
+  PK_TRY(d_idx.reserve(m, {st}));
+  PK_TRY(d_cb.reserve((size_t)m * dim, {st}));
+  PK_TRY(d_vb.reserve((size_t)m * dim, {st}));
+  PK_TRY(min_dist.reserve(m, {st}));
+  PK_TRY(best.reserve(m, {st}));
+  PK_TRY(taken.reserve(m, {st}));
+  PK_TRY(partial.reserve(nb, {st}));
+  PK_TRY(ticket.reserve(1, {st}));
+  PK_TRY(cur.reserve((size_t)k * dim, {st}));
+  PK_TRY(counts.reserve(k, {st}));
+  PK_TRY(d_mb.reserve(std::max<size_t>(mb.size(), 1), {st}));
+  PK_TRY(bpts.reserve((size_t)batch * dim, {st}));
+  PK_TRY(blab.reserve(batch, {st}));
+  PK_TRY(cudaMemcpyAsync(d_idx.get(), cb.data(), (size_t)m * 4, cudaMemcpyHostToDevice, st));
+  k_gather_rows<<<blocks_for((uint64_t)m * dim, 256), 256, 0, st>>>(data, stride, dim, d_idx.get(), m, d_cb.get());
   PK_TRY(cudaStreamSynchronize(st));   // d_idx is reused for the validation batch
-  PK_TRY(cudaMemcpyAsync(d_idx, vb.data(), (size_t)m * 4, cudaMemcpyHostToDevice, st));
-  k_gather_rows<<<blocks_for((uint64_t)m * dim, 256), 256, 0, st>>>(data, stride, dim, d_idx, m, d_vb);
-  PK_TRY(cudaMemsetAsync(ticket, 0, 4, st));
+  PK_TRY(cudaMemcpyAsync(d_idx.get(), vb.data(), (size_t)m * 4, cudaMemcpyHostToDevice, st));
+  k_gather_rows<<<blocks_for((uint64_t)m * dim, 256), 256, 0, st>>>(data, stride, dim, d_idx.get(), m, d_vb.get());
+  PK_TRY(cudaMemsetAsync(ticket.get(), 0, 4, st));
   PK_TRY(cudaMemsetAsync(d_means, 0, (size_t)k * dim * 4, st));
   PK_LAUNCHED();
 
@@ -825,37 +804,38 @@ int kmeans_device(GsContext *ctx, const float *data, uint32_t stride, uint32_t d
   std::vector<float> hbest(m);
   float min_dist_sum = FLT_MAX;
   for (int a = 0; a < 3; ++a) {
-    PK_TRY(cudaMemsetAsync(taken, 0, m, st));
-    PK_TRY(cudaMemsetAsync(taken + point0[a], 1, 1, st));
-    PK_TRY(cudaMemcpyAsync(cur, d_cb + (size_t)point0[a] * dim, (size_t)dim * 4, cudaMemcpyDeviceToDevice, st));
+    PK_TRY(cudaMemsetAsync(taken.get(), 0, m, st));
+    PK_TRY(cudaMemsetAsync(taken.get() + point0[a], 1, 1, st));
+    PK_TRY(cudaMemcpyAsync(cur.get(), d_cb.get() + (size_t)point0[a] * dim, (size_t)dim * 4, cudaMemcpyDeviceToDevice, st));
     for (uint32_t rc = 1; rc < k; ++rc)
-      k_kpp_round<<<nb, kSumBatch, 0, st>>>(d_cb, dim, m, min_dist, taken, cur, rc, rc == 1, partial, ticket, rng_at[a]);
+      k_kpp_round<<<nb, kSumBatch, 0, st>>>(d_cb.get(), dim, m, min_dist.get(), taken.get(), cur.get(), rc, rc == 1, partial.get(), ticket.get(),
+                                            rng_at[a]);
     ctx->launches += k - 1;
     PK_LAUNCHED();
-    int rc = nearest(ctx, bufs, d_vb, dim, dim, m, cur, k, nullptr, best, &sv, &si, &scap);
+    int rc = nearest(ctx, d_vb.get(), dim, dim, m, cur.get(), k, nullptr, best.get(), sv, si);
     if (rc) return rc;
-    PK_TRY(cudaMemcpyAsync(hbest.data(), best, (size_t)m * 4, cudaMemcpyDeviceToHost, st));
+    PK_TRY(cudaMemcpyAsync(hbest.data(), best.get(), (size_t)m * 4, cudaMemcpyDeviceToHost, st));
     PK_TRY(cudaStreamSynchronize(st));
     float dist_sum = 0.0f;
     for (uint32_t i = 0; i < m; ++i) dist_sum += hbest[i];
     if (dist_sum < min_dist_sum) {
       min_dist_sum = dist_sum;
-      PK_TRY(cudaMemcpyAsync(d_means, cur, (size_t)k * dim * 4, cudaMemcpyDeviceToDevice, st));
+      PK_TRY(cudaMemcpyAsync(d_means, cur.get(), (size_t)k * dim * 4, cudaMemcpyDeviceToDevice, st));
     }
   }
   // mini-batch passes (K:29-136)
-  PK_TRY(cudaMemsetAsync(counts, 0, (size_t)k * 4, st));
-  if (iters) PK_TRY(cudaMemcpyAsync(d_mb, mb.data(), mb.size() * 4, cudaMemcpyHostToDevice, st));
+  PK_TRY(cudaMemsetAsync(counts.get(), 0, (size_t)k * 4, st));
+  if (iters) PK_TRY(cudaMemcpyAsync(d_mb.get(), mb.data(), mb.size() * 4, cudaMemcpyHostToDevice, st));
   for (uint32_t it = 0; it < iters; ++it) {
-    k_gather_rows<<<blocks_for((uint64_t)batch * dim, 256), 256, 0, st>>>(data, stride, dim, d_mb + (size_t)it * batch, batch, bpts);
-    int rc = nearest(ctx, bufs, bpts, dim, dim, batch, d_means, k, blab, nullptr, &sv, &si, &scap);
+    k_gather_rows<<<blocks_for((uint64_t)batch * dim, 256), 256, 0, st>>>(data, stride, dim, d_mb.get() + (size_t)it * batch, batch, bpts.get());
+    int rc = nearest(ctx, bpts.get(), dim, dim, batch, d_means, k, blab.get(), nullptr, sv, si);
     if (rc) return rc;
-    k_mb_update<<<blocks_for(batch, 128), 128, 0, st>>>(bpts, blab, batch, dim, d_means, counts);
+    k_mb_update<<<blocks_for(batch, 128), 128, 0, st>>>(bpts.get(), blab.get(), batch, dim, d_means, counts.get());
     ctx->launches += 2;
   }
   PK_LAUNCHED();
   // final labelling of every point
-  int rc = nearest(ctx, bufs, data, stride, dim, n, d_means, k, d_labels, nullptr, &sv, &si, &scap);
+  int rc = nearest(ctx, data, stride, dim, n, d_means, k, d_labels, nullptr, sv, si);
   if (rc) return rc;
   PK_TRY(cudaStreamSynchronize(st));   // the host vectors above are freed on return
   return GS_OK;
@@ -888,17 +868,16 @@ int gs_kmeans(GsContext *ctx, uint32_t dim, const float *data, uint32_t n, uint3
   if (dim < 1 || dim > kMaxKmeansDim || batch < 1 || !(passes >= 0.0001f) || k < 1 || n < k)
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_kmeans needs 1 <= dim <= 128, batch >= 1, passes >= 0.0001 and 1 <= k <= n");
   GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  DevBufs bufs;
-  float *d_data, *d_means;
-  int32_t *d_labels;
-  GS_CUDA_TRY(ctx, bufs.alloc(&d_data, (size_t)n * dim * 4));
-  GS_CUDA_TRY(ctx, bufs.alloc(&d_means, (size_t)k * dim * 4));
-  GS_CUDA_TRY(ctx, bufs.alloc(&d_labels, (size_t)n * 4));
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(d_data, data, (size_t)n * dim * 4, cudaMemcpyHostToDevice, ctx->stream));
-  int rc = kmeans_device(ctx, d_data, dim, dim, n, batch, passes, d_means, k, d_labels);
+  Buffer<float> d_data, d_means;
+  Buffer<int32_t> d_labels;
+  GS_CUDA_TRY(ctx, d_data.reserve((size_t)n * dim, {ctx->stream}));
+  GS_CUDA_TRY(ctx, d_means.reserve((size_t)k * dim, {ctx->stream}));
+  GS_CUDA_TRY(ctx, d_labels.reserve(n, {ctx->stream}));
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(d_data.get(), data, (size_t)n * dim * 4, cudaMemcpyHostToDevice, ctx->stream));
+  int rc = kmeans_device(ctx, d_data.get(), dim, dim, n, batch, passes, d_means.get(), k, d_labels.get());
   if (rc) return rc;
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(means_out, d_means, (size_t)k * dim * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(labels_out, d_labels, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(means_out, d_means.get(), (size_t)k * dim * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(labels_out, d_labels.get(), (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
   GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return GS_OK;
 }
@@ -923,119 +902,118 @@ int gs_pack_asset(GsContext *ctx, const GsPackDesc *desc, GsPackedAsset *blobs_o
   ctx->pack_stats[0] = ctx->pack_stats[1] = ctx->pack_stats[2] = 0;
   cudaStream_t st = ctx->stream;
   const bool chunked = sz.chunk_bytes != 0, clustered = shf > 3;
-  DevBufs bufs;
 
   // input
   const float *in = (const float *)desc->splats;
+  Buffer<float> d_in;
   if (desc->memory == GS_MEM_HOST) {
-    float *d_in;
-    GS_CUDA_TRY(ctx, bufs.alloc(&d_in, (size_t)n * sizeof(GsInputSplat)));
-    GS_CUDA_TRY(ctx, cudaMemcpyAsync(d_in, desc->splats, (size_t)n * sizeof(GsInputSplat), cudaMemcpyHostToDevice, st));
-    in = d_in;
+    GS_CUDA_TRY(ctx, d_in.reserve((size_t)n * kRecFloats, {st}));
+    GS_CUDA_TRY(ctx, cudaMemcpyAsync(d_in.get(), desc->splats, (size_t)n * sizeof(GsInputSplat), cudaMemcpyHostToDevice, st));
+    in = d_in.get();
   }
   // 1. bounds
   const uint32_t bgrid = std::min(blocks_for(n, 256), sm_count() * 4u);
-  float *part_v, *d_bounds;
-  uint32_t *part_i;
-  GS_CUDA_TRY(ctx, bufs.alloc(&part_v, (size_t)bgrid * 6 * 4));
-  GS_CUDA_TRY(ctx, bufs.alloc(&part_i, (size_t)bgrid * 6 * 4));
-  GS_CUDA_TRY(ctx, bufs.alloc(&d_bounds, 6 * 4));
-  k_bounds<<<bgrid, 256, 0, st>>>(in, n, part_v, part_i);
-  k_bounds_final<<<1, 256, 0, st>>>(part_v, part_i, bgrid, d_bounds);
+  Buffer<float> part_v, d_bounds;
+  Buffer<uint32_t> part_i;
+  GS_CUDA_TRY(ctx, part_v.reserve((size_t)bgrid * 6, {st}));
+  GS_CUDA_TRY(ctx, part_i.reserve((size_t)bgrid * 6, {st}));
+  GS_CUDA_TRY(ctx, d_bounds.reserve(6, {st}));
+  k_bounds<<<bgrid, 256, 0, st>>>(in, n, part_v.get(), part_i.get());
+  k_bounds_final<<<1, 256, 0, st>>>(part_v.get(), part_i.get(), bgrid, d_bounds.get());
   // 2. Morton order: (code, index) by two stable LSD sorts -- low word with the identity as payload, then the high word
-  uint32_t *lo, *hi, *idx;
-  GS_CUDA_TRY(ctx, bufs.alloc(&lo, (size_t)n * 4));
-  GS_CUDA_TRY(ctx, bufs.alloc(&hi, (size_t)n * 4));
-  GS_CUDA_TRY(ctx, bufs.alloc(&idx, (size_t)n * 4));
-  k_morton<<<blocks_for(n, 256), 256, 0, st>>>(in, n, d_bounds, lo, hi, idx);
+  Buffer<uint32_t> lo, hi, idx;
+  GS_CUDA_TRY(ctx, lo.reserve(n, {st}));
+  GS_CUDA_TRY(ctx, hi.reserve(n, {st}));
+  GS_CUDA_TRY(ctx, idx.reserve(n, {st}));
+  k_morton<<<blocks_for(n, 256), 256, 0, st>>>(in, n, d_bounds.get(), lo.get(), hi.get(), idx.get());
   int rc = ensure_sort_scratch(ctx, n);
   if (rc) return rc;
   GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_scalar.get(), &n, 4, cudaMemcpyHostToDevice, st));
-  GS_CUDA_TRY(ctx, launch_sort_pairs(lo, idx, ctx->d_scalar.get(), n, 4, 8, false, sort_scratch(ctx), st));
-  k_gather_u32<<<blocks_for(n, 256), 256, 0, st>>>(hi, idx, n, lo);
-  GS_CUDA_TRY(ctx, launch_sort_pairs(lo, idx, ctx->d_scalar.get(), n, 4, 8, false, sort_scratch(ctx), st));
+  GS_CUDA_TRY(ctx, launch_sort_pairs(lo.get(), idx.get(), ctx->d_scalar.get(), n, 4, 8, false, sort_scratch(ctx), st));
+  k_gather_u32<<<blocks_for(n, 256), 256, 0, st>>>(hi.get(), idx.get(), n, lo.get());
+  GS_CUDA_TRY(ctx, launch_sort_pairs(lo.get(), idx.get(), ctx->d_scalar.get(), n, 4, 8, false, sort_scratch(ctx), st));
   ctx->launches += 5 + 2 * 5;
   GS_CUDA_TRY(ctx, cudaGetLastError());
-  float *recs;
-  GS_CUDA_TRY(ctx, bufs.alloc(&recs, (size_t)n * sizeof(GsInputSplat)));
-  k_gather_rows<<<blocks_for((uint64_t)n * kRecFloats, 256), 256, 0, st>>>(in, kRecFloats, kRecFloats, idx, n, recs);
+  Buffer<float> recs;
+  GS_CUDA_TRY(ctx, recs.reserve((size_t)n * kRecFloats, {st}));
+  k_gather_rows<<<blocks_for((uint64_t)n * kRecFloats, 256), 256, 0, st>>>(in, kRecFloats, kRecFloats, idx.get(), n, recs.get());
   GS_CUDA_TRY(ctx, cudaGetLastError());
 
   // the blobs, in HBM; allocated like gs_asset_upload's (16 bytes of slack; a clustered palette backs all 65536 entries)
-  uint8_t *b_pos, *b_other, *b_color, *b_sh, *b_chunks = nullptr;
+  Buffer<uint8_t> b_pos, b_other, b_color, b_sh, b_chunks;
   const uint64_t sh_alloc = std::max<uint64_t>(sz.sh_bytes, clustered ? 65536ull * 96ull : 0ull) + 16;
-  GS_CUDA_TRY(ctx, bufs.alloc(&b_pos, sz.pos_bytes + 16));
-  GS_CUDA_TRY(ctx, bufs.alloc(&b_other, sz.other_bytes + 16));
-  GS_CUDA_TRY(ctx, bufs.alloc(&b_color, sz.color_bytes + 16));
-  GS_CUDA_TRY(ctx, bufs.alloc(&b_sh, sh_alloc));
-  if (chunked) GS_CUDA_TRY(ctx, bufs.alloc(&b_chunks, sz.chunk_bytes + 16));
-  GS_CUDA_TRY(ctx, cudaMemsetAsync(b_pos, 0, sz.pos_bytes + 16, st));
-  GS_CUDA_TRY(ctx, cudaMemsetAsync(b_other, 0, sz.other_bytes + 16, st));
-  GS_CUDA_TRY(ctx, cudaMemsetAsync(b_color, 0, sz.color_bytes + 16, st));
-  GS_CUDA_TRY(ctx, cudaMemsetAsync(b_sh, 0, sh_alloc, st));
-  if (chunked) GS_CUDA_TRY(ctx, cudaMemsetAsync(b_chunks, 0, sz.chunk_bytes + 16, st));
+  GS_CUDA_TRY(ctx, b_pos.reserve(sz.pos_bytes + 16, {st}));
+  GS_CUDA_TRY(ctx, b_other.reserve(sz.other_bytes + 16, {st}));
+  GS_CUDA_TRY(ctx, b_color.reserve(sz.color_bytes + 16, {st}));
+  GS_CUDA_TRY(ctx, b_sh.reserve(sh_alloc, {st}));
+  if (chunked) GS_CUDA_TRY(ctx, b_chunks.reserve(sz.chunk_bytes + 16, {st}));
+  GS_CUDA_TRY(ctx, cudaMemsetAsync(b_pos.get(), 0, sz.pos_bytes + 16, st));
+  GS_CUDA_TRY(ctx, cudaMemsetAsync(b_other.get(), 0, sz.other_bytes + 16, st));
+  GS_CUDA_TRY(ctx, cudaMemsetAsync(b_color.get(), 0, sz.color_bytes + 16, st));
+  GS_CUDA_TRY(ctx, cudaMemsetAsync(b_sh.get(), 0, sh_alloc, st));
+  if (chunked) GS_CUDA_TRY(ctx, cudaMemsetAsync(b_chunks.get(), 0, sz.chunk_bytes + 16, st));
 
   // 3. SH palette: k-means over the reordered, not yet normalised SH
-  int32_t *labels = nullptr;
+  Buffer<float> means;
+  Buffer<int32_t> labels;
   if (clustered) {
     static const float kPasses[5] = {0.3f, 0.4f, 0.5f, 0.8f, 1.2f};   // Cluster64k..4k, as gsa_create_asset
     const uint32_t k = sh_count(shf, n);
-    float *means;
-    GS_CUDA_TRY(ctx, bufs.alloc(&means, (size_t)k * 45 * 4));
-    GS_CUDA_TRY(ctx, bufs.alloc(&labels, (size_t)n * 4));
-    if ((rc = kmeans_device(ctx, recs + kOffSh, kRecFloats, 45, n, 2048, kPasses[shf - 4], means, k, labels))) return rc;
-    k_palette<<<blocks_for((uint64_t)k * 45, 256), 256, 0, st>>>(means, k, b_sh);
+    GS_CUDA_TRY(ctx, means.reserve((size_t)k * 45, {st}));
+    GS_CUDA_TRY(ctx, labels.reserve(n, {st}));
+    if ((rc = kmeans_device(ctx, recs.get() + kOffSh, kRecFloats, 45, n, 2048, kPasses[shf - 4], means.get(), k, labels.get()))) return rc;
+    k_palette<<<blocks_for((uint64_t)k * 45, 256), 256, 0, st>>>(means.get(), k, b_sh.get());
     GS_CUDA_TRY(ctx, cudaGetLastError());
   }
   // 4. chunks
+  Buffer<uint32_t> fix_idx, fix_count;
+  Buffer<float> fix_val;
   if (chunked) {
-    uint32_t *fix_idx, *fix_count;
-    float *fix_val;
-    GS_CUDA_TRY(ctx, bufs.alloc(&fix_idx, (size_t)n * 3 * 4));
-    GS_CUDA_TRY(ctx, bufs.alloc(&fix_val, (size_t)n * 3 * 4));
-    GS_CUDA_TRY(ctx, bufs.alloc(&fix_count, 4));
-    GS_CUDA_TRY(ctx, cudaMemsetAsync(fix_count, 0, 4, st));
-    k_pow_scales<<<blocks_for(n, 256), 256, 0, st>>>(recs, n, fix_idx, fix_val, fix_count);
+    GS_CUDA_TRY(ctx, fix_idx.reserve((size_t)n * 3, {st}));
+    GS_CUDA_TRY(ctx, fix_val.reserve((size_t)n * 3, {st}));
+    GS_CUDA_TRY(ctx, fix_count.reserve(1, {st}));
+    GS_CUDA_TRY(ctx, cudaMemsetAsync(fix_count.get(), 0, 4, st));
+    k_pow_scales<<<blocks_for(n, 256), 256, 0, st>>>(recs.get(), n, fix_idx.get(), fix_val.get(), fix_count.get());
     uint32_t count = 0;
-    GS_CUDA_TRY(ctx, cudaMemcpyAsync(&count, fix_count, 4, cudaMemcpyDeviceToHost, st));
+    GS_CUDA_TRY(ctx, cudaMemcpyAsync(&count, fix_count.get(), 4, cudaMemcpyDeviceToHost, st));
     GS_CUDA_TRY(ctx, cudaStreamSynchronize(st));
     ctx->pack_stats[0] = count;
     if (count) {   // the host's own pow for the values next to a rounding midpoint
       std::vector<float> v(count);
-      GS_CUDA_TRY(ctx, cudaMemcpyAsync(v.data(), fix_val, (size_t)count * 4, cudaMemcpyDeviceToHost, st));
+      GS_CUDA_TRY(ctx, cudaMemcpyAsync(v.data(), fix_val.get(), (size_t)count * 4, cudaMemcpyDeviceToHost, st));
       GS_CUDA_TRY(ctx, cudaStreamSynchronize(st));
       for (float &x : v) x = (float)std::pow((double)x, (double)(1.0f / 8.0f));
-      GS_CUDA_TRY(ctx, cudaMemcpyAsync(fix_val, v.data(), (size_t)count * 4, cudaMemcpyHostToDevice, st));
-      k_scatter_scales<<<blocks_for(count, 256), 256, 0, st>>>(recs, fix_idx, fix_val, count);
+      GS_CUDA_TRY(ctx, cudaMemcpyAsync(fix_val.get(), v.data(), (size_t)count * 4, cudaMemcpyHostToDevice, st));
+      k_scatter_scales<<<blocks_for(count, 256), 256, 0, st>>>(recs.get(), fix_idx.get(), fix_val.get(), count);
       GS_CUDA_TRY(ctx, cudaStreamSynchronize(st));   // `v` is freed at the end of this scope
     }
-    k_chunks<<<blocks_for(n, kChunkSize), kChunkSize, 0, st>>>(recs, n, (Chunk *)b_chunks);
+    k_chunks<<<blocks_for(n, kChunkSize), kChunkSize, 0, st>>>(recs.get(), n, (Chunk *)b_chunks.get());
     GS_CUDA_TRY(ctx, cudaGetLastError());
   }
   // 5. emit, 6. BC7
-  float4 *image = nullptr;
+  Buffer<float4> image;
   if (cf == GS_COL_BC7) {
     const size_t texels = (size_t)sz.tex_width * sz.tex_height;
-    GS_CUDA_TRY(ctx, bufs.alloc(&image, texels * 16));
-    GS_CUDA_TRY(ctx, cudaMemsetAsync(image, 0, texels * 16, st));
+    GS_CUDA_TRY(ctx, image.reserve(texels, {st}));
+    GS_CUDA_TRY(ctx, cudaMemsetAsync(image.get(), 0, texels * 16, st));
   }
-  EmitArgs ea{recs, n, pf, sf, cf, shf, b_pos, b_other, b_color, b_sh, image, labels};
+  EmitArgs ea{recs.get(), n, pf, sf, cf, shf, b_pos.get(), b_other.get(), b_color.get(), b_sh.get(), image.get(), labels.get()};
   k_emit<<<blocks_for(n, 256), 256, 0, st>>>(ea);
   if (cf == GS_COL_BC7) {
     const uint32_t bw = sz.tex_width / 4, nblocks = bw * (sz.tex_height / 4);
-    k_bc7<<<blocks_for(nblocks, 128), 128, 0, st>>>(image, bw, nblocks, b_color);
+    k_bc7<<<blocks_for(nblocks, 128), 128, 0, st>>>(image.get(), bw, nblocks, b_color.get());
   }
   GS_CUDA_TRY(ctx, cudaGetLastError());
 
   if (blobs_out) {
     const cudaMemcpyKind kind = blobs_out->memory == GS_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-    GS_CUDA_TRY(ctx, cudaMemcpyAsync(blobs_out->pos, b_pos, sz.pos_bytes, kind, st));
-    GS_CUDA_TRY(ctx, cudaMemcpyAsync(blobs_out->other, b_other, sz.other_bytes, kind, st));
-    GS_CUDA_TRY(ctx, cudaMemcpyAsync(blobs_out->color, b_color, sz.color_bytes, kind, st));
-    GS_CUDA_TRY(ctx, cudaMemcpyAsync(blobs_out->sh, b_sh, sz.sh_bytes, kind, st));
-    if (chunked) GS_CUDA_TRY(ctx, cudaMemcpyAsync(blobs_out->chunks, b_chunks, sz.chunk_bytes, kind, st));
+    GS_CUDA_TRY(ctx, cudaMemcpyAsync(blobs_out->pos, b_pos.get(), sz.pos_bytes, kind, st));
+    GS_CUDA_TRY(ctx, cudaMemcpyAsync(blobs_out->other, b_other.get(), sz.other_bytes, kind, st));
+    GS_CUDA_TRY(ctx, cudaMemcpyAsync(blobs_out->color, b_color.get(), sz.color_bytes, kind, st));
+    GS_CUDA_TRY(ctx, cudaMemcpyAsync(blobs_out->sh, b_sh.get(), sz.sh_bytes, kind, st));
+    if (chunked) GS_CUDA_TRY(ctx, cudaMemcpyAsync(blobs_out->chunks, b_chunks.get(), sz.chunk_bytes, kind, st));
     float hb[6];
-    GS_CUDA_TRY(ctx, cudaMemcpyAsync(hb, d_bounds, sizeof(hb), cudaMemcpyDeviceToHost, st));
+    GS_CUDA_TRY(ctx, cudaMemcpyAsync(hb, d_bounds.get(), sizeof(hb), cudaMemcpyDeviceToHost, st));
     GS_CUDA_TRY(ctx, cudaStreamSynchronize(st));
     memcpy(blobs_out->bounds_min, hb, 12);
     memcpy(blobs_out->bounds_max, hb + 3, 12);
@@ -1044,8 +1022,8 @@ int gs_pack_asset(GsContext *ctx, const GsPackDesc *desc, GsPackedAsset *blobs_o
     GsAsset *as = new (std::nothrow) GsAsset();
     if (!as) return fail(ctx, GS_ERR_OUT_OF_MEMORY, "host allocation failed");
     as->ctx = ctx;
-    as->d_pos = b_pos; as->d_other = b_other; as->d_color = b_color; as->d_sh = b_sh; as->d_chunks = b_chunks;
-    for (void *p : {(void *)b_pos, (void *)b_other, (void *)b_color, (void *)b_sh, (void *)b_chunks}) bufs.release(p);
+    as->d_pos = std::move(b_pos); as->d_other = std::move(b_other); as->d_color = std::move(b_color); as->d_sh = std::move(b_sh);
+    as->d_chunks = std::move(b_chunks);
     const cudaError_t e = asset_init_work(ctx, as, n, pf, sf, shf, cf, chunked ? (uint32_t)(sz.chunk_bytes / 64) : 0u);
     if (e != cudaSuccess) {
       gs_asset_destroy(as);
