@@ -132,12 +132,28 @@ typedef enum GsPixelFormat {
  * effect on an array render target (it applies to host images only). */
 typedef enum GsMemory { GS_MEM_HOST = 0, GS_MEM_DEVICE = 1, GS_MEM_ARRAY = 2 } GsMemory;
 
+/* GS_MEM_ARRAY_LAYER (images only): `data` points to a GsArrayLayer, a host descriptor borrowed for the call, that names one
+ * layer of a layered CUDA array -- e.g. one eye of an XR eye-texture array in single-pass-instanced mode, or one face of a
+ * cube map, imported with extent.depth = its layer count and flags cudaArrayLayered | cudaArraySurfaceLoadStore.  The layer is
+ * rendered into / composited onto in place through a layered surface; the array's other layers are not touched.  The rules of
+ * GS_MEM_ARRAY apply, except that:
+ *   - the array must have been created with cudaArrayLayered | cudaArraySurfaceLoadStore, with extent width x height, and
+ *     `layer` must be below its depth (its layer count); `reserved` must be 0 (else GS_ERR_INVALID_ARGUMENT).
+ * A layered array passed as GS_MEM_ARRAY is GS_ERR_INVALID_ARGUMENT, as is a 2-D array passed as GS_MEM_ARRAY_LAYER.
+ * Memory kind 3 is not defined (GS_ERR_INVALID_ARGUMENT). */
+#define GS_MEM_ARRAY_LAYER 4u
+typedef struct GsArrayLayer {
+  void *array;      /* a layered cudaArray_t (mip level 0) on the context's device */
+  uint32_t layer;   /* the layer drawn into, below the array's layer count */
+  uint32_t reserved;
+} GsArrayLayer;
+
 typedef struct GsImage {
-  void *data;                /* host pointer, device pointer, or cudaArray_t (GS_MEM_ARRAY) */
+  void *data;                /* host pointer, device pointer, cudaArray_t (GS_MEM_ARRAY) or GsArrayLayer * (GS_MEM_ARRAY_LAYER) */
   uint32_t width, height;
-  uint32_t row_pitch_bytes;  /* 0 = tightly packed (and always 0 for GS_MEM_ARRAY) */
+  uint32_t row_pitch_bytes;  /* 0 = tightly packed (and always 0 for GS_MEM_ARRAY / GS_MEM_ARRAY_LAYER) */
   uint32_t format;           /* GsPixelFormat */
-  uint32_t memory;           /* GsMemory: where `data` lives; a value above GS_MEM_ARRAY is GS_ERR_INVALID_ARGUMENT */
+  uint32_t memory;           /* GsMemory or GS_MEM_ARRAY_LAYER: where `data` lives; any other value is GS_ERR_INVALID_ARGUMENT */
 } GsImage;
 
 /* How the render-target blend is evaluated.

@@ -16,6 +16,7 @@ GS_OK = 0
 GS_ERR_NO_DEVICE = -6
 GS_PIX_RGBA16F, GS_PIX_RGBA32F = 0, 1
 GS_MEM_HOST, GS_MEM_DEVICE, GS_MEM_ARRAY = 0, 1, 2
+GS_MEM_ARRAY_LAYER = 4
 GS_BLEND_FP16_ROP, GS_BLEND_FP32 = 0, 1
 
 
@@ -51,6 +52,10 @@ class GsFrameParams(C.Structure):
         ("cutouts", C.c_void_p), ("deleted_bits", C.c_void_p), ("selected_bits", C.c_void_p),
         ("scene_depth", C.c_void_p), ("scene_depth_on_device", C.c_uint32), ("reserved1", C.c_uint32),
     ]
+
+
+class GsArrayLayer(C.Structure):
+    _fields_ = [("array", C.c_void_p), ("layer", C.c_uint32), ("reserved", C.c_uint32)]
 
 
 class GsImage(C.Structure):

@@ -177,7 +177,7 @@ static int ensure_async_readback(GsContext *ctx) {
 
 uint32_t pix_bytes(uint32_t fmt) { return fmt == GS_PIX_RGBA16F ? 8u : 16u; }
 
-// ---- GS_MEM_ARRAY images -----------------------------------------------------------------------------
+// ---- GS_MEM_ARRAY / GS_MEM_ARRAY_LAYER images -----------------------------------------------------------------------------
 // Destroys the held surface objects whose last use has completed; with `all`, every one, after waiting for its event.  The
 // event, not the context stream, is what guards a batch: the group path composites onto CUDA-array camera targets on a
 // member's transfer stream, which the context stream never waits for.
@@ -204,9 +204,10 @@ static void release_surfaces(GsContext *ctx, bool all) {
   held.resize(keep);
 }
 
-// The surface objects one call creates for its GS_MEM_ARRAY images.  When the call returns they are handed to the context behind
-// an event recorded on the stream that used them (the context's, unless another is named) after their last use.  They are never
-// cached by cudaArray_t value: a freed array's handle can be reused by the next allocation.
+// The surface objects one call creates for its CUDA-array images, one per array: the layers of one layered array share it.
+// When the call returns they are handed to the context behind an event recorded on the stream that used them (the context's,
+// unless another is named) after their last use.  They are never cached by cudaArray_t value beyond the call: a freed array's
+// handle can be reused by the next allocation.
 class CallSurfaces {
  public:
   explicit CallSurfaces(GsContext *ctx, cudaStream_t stream = nullptr) : ctx_(ctx), stream_(stream ? stream : ctx->stream) {}
@@ -225,15 +226,19 @@ class CallSurfaces {
     for (cudaSurfaceObject_t so : made_) cudaDestroySurfaceObject(so);
     if (ev) ctx_->spare_events.push_back(ev);
   }
-  // `im` has passed image_ok as a GS_MEM_ARRAY image
-  int make(const GsImage *im, cudaSurfaceObject_t *out) {
+  // `im` has passed image_ok as a GS_MEM_ARRAY or GS_MEM_ARRAY_LAYER image
+  int make(const GsImage *im, Surface *out) {
+    const cudaArray_t arr = image_array(im, &out->layer);
+    for (size_t i = 0; i < arrays_.size(); ++i)
+      if (arrays_[i] == arr) { out->obj = made_[i]; return GS_OK; }
     if (made_.empty()) release_surfaces(ctx_, false);
     cudaResourceDesc rd;
     memset(&rd, 0, sizeof(rd));
     rd.resType = cudaResourceTypeArray;
-    rd.res.array.array = static_cast<cudaArray_t>(im->data);
-    GS_CUDA_TRY(ctx_, cudaCreateSurfaceObject(out, &rd));
-    made_.push_back(*out);
+    rd.res.array.array = arr;
+    GS_CUDA_TRY(ctx_, cudaCreateSurfaceObject(&out->obj, &rd));
+    made_.push_back(out->obj);
+    arrays_.push_back(arr);
     return GS_OK;
   }
 
@@ -241,6 +246,7 @@ class CallSurfaces {
   GsContext *ctx_;
   cudaStream_t stream_;
   std::vector<cudaSurfaceObject_t> made_;
+  std::vector<cudaArray_t> arrays_;   // made_[i] is the surface of arrays_[i]
 };
 
 int reserve_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, std::initializer_list<cudaStream_t> users) {
@@ -389,7 +395,7 @@ static int tile_history(GsContext *ctx, uint32_t tiles, const std::vector<uint32
 }
 
 int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *as, const GsFrameParams *fp, bool first,
-            void *d_rt, uint32_t pitch, uint32_t fmt, cudaSurfaceObject_t surf, cudaEvent_t bin_done) {
+            void *d_rt, uint32_t pitch, uint32_t fmt, Surface surf, cudaEvent_t bin_done) {
   GsNvtxRange nvtx("GaussianSplat.Draw");
   const uint32_t n = as->av.n;
   int rc = ensure_bin_scratch(ctx, n, fc.binsX * fc.binsY, 0);
@@ -426,20 +432,31 @@ int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, G
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch) {
   if (!im || !im->data) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image is null");
   if (im->format > GS_PIX_RGBA32F) return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "unsupported pixel format");
-  if (im->memory > GS_MEM_ARRAY) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "unknown image memory kind");
+  if (im->memory > GS_MEM_ARRAY_LAYER || im->memory == 3)   // 3 is not a memory kind
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, "unknown image memory kind");
   if (im->width != W || im->height != H) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image size does not match screen size");
-  if (im->memory == GS_MEM_ARRAY) {   // a 2-D CUDA array: data is a cudaArray_t
+  if (is_array_image(im)) {   // a 2-D CUDA array (data is a cudaArray_t), or a layer of a layered one (data is a GsArrayLayer *)
     if (im->row_pitch_bytes) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "row_pitch_bytes must be 0 for a CUDA array image");
+    const bool layered = im->memory == GS_MEM_ARRAY_LAYER;
+    if (layered) {
+      const GsArrayLayer *d = static_cast<const GsArrayLayer *>(im->data);
+      if (!d->array || d->reserved) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "GsArrayLayer: array is null or reserved is not 0");
+    }
+    int32_t layer = -1;
     cudaChannelFormatDesc cd;
     cudaExtent ext;
     unsigned int flags = 0;
-    const cudaError_t e = cudaArrayGetInfo(&cd, &ext, &flags, static_cast<cudaArray_t>(im->data));
+    const cudaError_t e = cudaArrayGetInfo(&cd, &ext, &flags, image_array(im, &layer));
     if (e != cudaSuccess) { cudaGetLastError(); return fail(ctx, GS_ERR_INVALID_ARGUMENT, std::string("not a CUDA array: ") + cudaGetErrorString(e)); }
     const int bits = im->format == GS_PIX_RGBA16F ? 16 : 32;
     if (cd.f != cudaChannelFormatKindFloat || cd.x != bits || cd.y != bits || cd.z != bits || cd.w != bits)
       return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "the CUDA array's channel format does not match the image's pixel format");
-    if (ext.width != W || ext.height != H || ext.depth != 0)
+    if (!layered && (ext.width != W || ext.height != H || ext.depth != 0))
       return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array is not a 2-D array of the image's size");
+    if (layered && (ext.width != W || ext.height != H || !(flags & cudaArrayLayered)))
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array is not a layered array of the image's size");
+    if (layered && (uint32_t)layer >= ext.depth)
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the layer is not below the CUDA array's layer count");
     if (!(flags & cudaArraySurfaceLoadStore))
       return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array was not created with cudaArraySurfaceLoadStore");
     *pitch = 0;
@@ -718,16 +735,16 @@ int gs_render(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRend
       return fail(ctx, GS_ERR_NOT_READY, "the last gs_frame prepared draw records for another tile partition; run gs_calc_view");
   }
   const uint32_t H = opt.band_packed ? partition_own_bin_rows(opt, fc.binsY) * kBin : (uint32_t)fp->screen_h;
-  if (opt.band_packed && rt && rt->memory == GS_MEM_ARRAY)
+  if (opt.band_packed && rt && is_array_image(rt))
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "band_packed output is the send buffer of an all-gather: it must be linear memory, not a CUDA array");
   if ((rc = image_ok(ctx, rt, W, H, &pitch))) return rc;
   if (fp->scene_depth && !as->zndc_valid) return fail(ctx, GS_ERR_NOT_READY, "a scene depth buffer needs the quad depths: run gs_calc_view with scene_depth set");
   for (int e = EV_BIN1; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
   rec(ctx, EV_VIEW1);
   if (rt->memory == GS_MEM_DEVICE) return do_draw(ctx, fc, opt, as, fp, true, rt->data, pitch, rt->format);
-  if (rt->memory == GS_MEM_ARRAY) {
+  if (is_array_image(rt)) {
     CallSurfaces surfs(ctx);
-    cudaSurfaceObject_t so = 0;
+    Surface so;
     if ((rc = surfs.make(rt, &so))) return rc;
     return do_draw(ctx, fc, opt, as, fp, true, nullptr, 0, rt->format, so);
   }
@@ -739,25 +756,25 @@ int gs_render(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRend
   return check_bin_overflow(ctx);
 }
 
-// d_rt == nullptr: the render target is the CUDA array behind rt_surf.  Enqueued on `s`: the context's stream, or the group
+// d_rt == nullptr: the render target is the CUDA array (layer) behind rt_surf.  Enqueued on `s`: the context's stream, or the group
 // path's transfer stream (surfs must then hand its surfaces over on `s` as well).
-static int composite_impl(GsContext *ctx, CallSurfaces &surfs, const void *d_rt, uint32_t rt_pitch, cudaSurfaceObject_t rt_surf,
+static int composite_impl(GsContext *ctx, CallSurfaces &surfs, const void *d_rt, uint32_t rt_pitch, Surface rt_surf,
                           uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H, cudaStream_t s) {
   GsNvtxRange nvtx("GaussianSplat.Compose");
   uint32_t tp = 0;
   int rc = image_ok(ctx, tgt, W, H, &tp);
   if (rc) return rc;
   if (tgt->memory == GS_MEM_DEVICE) {
-    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, tgt->data, tp, 0, tgt->format, W, H, s);
-  } else if (tgt->memory == GS_MEM_ARRAY) {
-    cudaSurfaceObject_t so = 0;
+    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, tgt->data, tp, Surface{}, tgt->format, W, H, s);
+  } else if (is_array_image(tgt)) {
+    Surface so;
     if ((rc = surfs.make(tgt, &so))) return rc;
     launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, nullptr, 0, so, tgt->format, W, H, s);
   } else {
     const uint32_t tight = W * pix_bytes(tgt->format);
     GS_CUDA_TRY(ctx, ctx->tgt_scratch.reserve((size_t)tight * H, {ctx->stream}));
     GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->tgt_scratch.get(), tight, tgt->data, tp, tight, H, cudaMemcpyHostToDevice, s));
-    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, ctx->tgt_scratch.get(), tight, 0, tgt->format, W, H, s);
+    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, ctx->tgt_scratch.get(), tight, Surface{}, tgt->format, W, H, s);
     GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(tgt->data, tp, ctx->tgt_scratch.get(), tight, tight, H, cudaMemcpyDeviceToHost, s));
   }
   if (s == ctx->stream) rec(ctx, EV_COMP1);
@@ -777,16 +794,16 @@ int gs_composite(GsContext *ctx, const GsImage *rt, GsImage *tgt) {
   ctx->ev_valid[EV_COMP1] = false;
   rec(ctx, EV_RASTER1);
   CallSurfaces surfs(ctx);
-  if (rt->memory == GS_MEM_DEVICE) return composite_impl(ctx, surfs, rt->data, rp, 0, rt->format, tgt, W, H, ctx->stream);
-  if (rt->memory == GS_MEM_ARRAY) {
-    cudaSurfaceObject_t so = 0;
+  if (rt->memory == GS_MEM_DEVICE) return composite_impl(ctx, surfs, rt->data, rp, Surface{}, rt->format, tgt, W, H, ctx->stream);
+  if (is_array_image(rt)) {
+    Surface so;
     if ((rc = surfs.make(rt, &so))) return rc;
     return composite_impl(ctx, surfs, nullptr, 0, so, rt->format, tgt, W, H, ctx->stream);
   }
   const uint32_t tight = W * pix_bytes(rt->format);
   GS_CUDA_TRY(ctx, ctx->rt_scratch.reserve((size_t)tight * H, {ctx->stream}));
   GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->rt_scratch.get(), tight, rt->data, rp, tight, H, cudaMemcpyHostToDevice, ctx->stream));
-  return composite_impl(ctx, surfs, ctx->rt_scratch.get(), tight, 0, rt->format, tgt, W, H, ctx->stream);
+  return composite_impl(ctx, surfs, ctx->rt_scratch.get(), tight, Surface{}, rt->format, tgt, W, H, ctx->stream);
 }
 
 }  // extern "C"
@@ -795,9 +812,9 @@ namespace gs {
 // The device image a frame draws into: `rt` itself when it is device or array memory, else library scratch (or, with
 // GS_FLAG_ASYNC_READBACK, one of the two asynchronous staging images) that a host `rt` is read back from.
 struct FrameImage {
-  void *d_rt = nullptr;            // nullptr: the CUDA array behind `surf`
+  void *d_rt = nullptr;            // nullptr: the CUDA array (layer) behind `surf`
   uint32_t pitch = 0;
-  cudaSurfaceObject_t surf = 0;
+  Surface surf;
   bool async_rb = false;
   int slot = 0;
 };
@@ -807,7 +824,7 @@ struct FrameImage {
 static int begin_frame_image(GsContext *ctx, CallSurfaces &surfs, const GsRenderOptions &opt, GsImage *rt, uint32_t rt_pitch,
                              uint32_t rt_fmt, const GsImage *tgt, uint32_t W, uint32_t H, FrameImage *fi, void *staging = nullptr) {
   int rc = GS_OK;
-  const bool rt_dev = rt && rt->memory == GS_MEM_DEVICE, rt_arr = rt && rt->memory == GS_MEM_ARRAY, rt_host = rt && rt->memory == GS_MEM_HOST;
+  const bool rt_dev = rt && rt->memory == GS_MEM_DEVICE, rt_arr = rt && is_array_image(rt), rt_host = rt && rt->memory == GS_MEM_HOST;
   fi->async_rb = rt_host && !tgt && (opt.flags & GS_FLAG_ASYNC_READBACK) != 0;
   if (rt_dev) { fi->d_rt = rt->data; fi->pitch = rt_pitch; }
   else if (rt_arr) {   // rendered into in place, through a surface
@@ -927,6 +944,18 @@ static uint32_t run_end(GsAsset *const *assets, const GsFrameParams *fps, uint32
   return e;
 }
 
+// What makes two images of a call one image: the same pointer, or the same array and layer (GS_MEM_ARRAY_LAYER; the layers of
+// one array are separate images).
+static std::pair<const void *, int32_t> image_id(const GsImage *im) {
+  if (!im) return {nullptr, -1};
+  if (im->memory == GS_MEM_ARRAY_LAYER) {
+    int32_t layer = -1;
+    const cudaArray_t arr = image_array(im, &layer);
+    return {arr, layer};
+  }
+  return {im->data, -1};
+}
+
 // The call's cameras as runs, in order.  Consecutive whole cameras share a run while each fits it, the run's totals hold, they
 // have one pixel format, and no camera's image is another's render target (two cameras rasterizing into one image at once
 // would race, where the loop draws one after the other).  A camera alone is split into runs of run_end, each later one
@@ -940,9 +969,9 @@ static std::vector<Run> form_runs(const std::vector<CameraArgs> &cams, GsAsset *
     const CameraArgs &a = cams[c];
     if (run_pairs + a.K > kRunObjects || run_bins + a.fcs[0].binsX * a.fcs[0].binsY > kMaxRunBins || a.rt_fmt != cams[c0].rt_fmt) return false;
     for (uint32_t j = c0; j < c; ++j) {
-      const void *rj = cams[j].rt ? cams[j].rt->data : nullptr, *tj = cams[j].tgt ? cams[j].tgt->data : nullptr;
-      if (a.rt && (a.rt->data == rj || a.rt->data == tj)) return false;
-      if (a.tgt && a.tgt->data == rj) return false;
+      const auto rj = image_id(cams[j].rt), tj = image_id(cams[j].tgt), ra = image_id(a.rt), ta = image_id(a.tgt);
+      if (a.rt && (ra == rj || ra == tj)) return false;
+      if (a.tgt && ta == rj) return false;
     }
     return true;
   };
@@ -1166,7 +1195,7 @@ int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRende
   if ((rc = check_options(ctx, fc, opt))) return rc;
   const uint32_t H = opt.band_packed ? partition_own_bin_rows(opt, fc.binsY) * kBin : (uint32_t)fp->screen_h;
   if (opt.band_packed && tgt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "band_packed output cannot be composited before the gather");
-  if (opt.band_packed && rt && rt->memory == GS_MEM_ARRAY)
+  if (opt.band_packed && rt && is_array_image(rt))
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "band_packed output is the send buffer of an all-gather: it must be linear memory, not a CUDA array");
   if (rt) { if ((rc = image_ok(ctx, rt, W, H, &rt_pitch))) return rc; rt_fmt = rt->format; }
   for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
@@ -1218,7 +1247,7 @@ int gs_frame_cameras(GsContext *ctx, uint32_t camera_count, const uint32_t *obje
 int gs_unshuffle_bands(GsContext *ctx, const void *gathered, uint32_t parts, uint32_t band_rows, uint32_t rows_pp, uint32_t fmt,
                        GsImage *out) {
   if (!ctx || !gathered || !out || parts == 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null argument");
-  if (out->memory == GS_MEM_ARRAY) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_unshuffle_bands writes host or linear device memory, not a CUDA array");
+  if (is_array_image(out)) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_unshuffle_bands writes host or linear device memory, not a CUDA array");
   uint32_t pitch = 0;
   int rc = image_ok(ctx, out, out->width, out->height, &pitch);
   if (rc) return rc;
@@ -1372,6 +1401,6 @@ namespace gs {
 int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H,
                         cudaStream_t s) {
   CallSurfaces surfs(ctx, s);
-  return composite_impl(ctx, surfs, d_rt, rt_pitch, 0, rt_fmt, tgt, W, H, s);
+  return composite_impl(ctx, surfs, d_rt, rt_pitch, Surface{}, rt_fmt, tgt, W, H, s);
 }
 }  // namespace gs

@@ -836,7 +836,7 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
         opt.flags = k ? (uint32_t)GS_FLAG_LOAD_RT : 0u;
         rec(ctx, EV_VIEW1);
         if (timing) cudaEventRecord(mb.obj_tev[2 * k], ctx->stream);
-        if ((rc = do_draw(ctx, o.fc, opt, o.assets[i], o.fp, k == 0, d_rt, pitch, fmt, 0, timing ? mb.obj_tev[2 * k + 1] : nullptr)))
+        if ((rc = do_draw(ctx, o.fc, opt, o.assets[i], o.fp, k == 0, d_rt, pitch, fmt, Surface{}, timing ? mb.obj_tev[2 * k + 1] : nullptr)))
           return rc;
         ctx->launches += 1;   // k_row_costs: here for every object but the last (before the next one's raster overwrites the
                               // tile costs), on the transfer stream below for the last
@@ -886,6 +886,16 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
     } else if (rt && rt->memory == GS_MEM_ARRAY) {   // e.g. the display GPU's imported render texture: one copy of the assembled frame
       GS_CUDA_TRY(ctx, cudaMemcpy2DToArrayAsync(static_cast<cudaArray_t>(rt->data), 0, 0, img[i], pitches[i], (size_t)W * pix_bytes(fmt), H,
                                                 cudaMemcpyDeviceToDevice, mb.xfer));
+    } else if (rt && rt->memory == GS_MEM_ARRAY_LAYER) {   // e.g. one eye of an XR eye-texture array: the same copy, into its layer
+      int32_t layer = -1;
+      cudaMemcpy3DParms cp;
+      memset(&cp, 0, sizeof(cp));
+      cp.srcPtr = make_cudaPitchedPtr(img[i], pitches[i], W, H);
+      cp.dstArray = image_array(rt, &layer);
+      cp.dstPos = make_cudaPos(0, 0, (size_t)layer);
+      cp.extent = make_cudaExtent(W, H, 1);   // in texels: the destination is an array
+      cp.kind = cudaMemcpyDeviceToDevice;
+      GS_CUDA_TRY(ctx, cudaMemcpy3DAsync(&cp, mb.xfer));
     }
     // the composite pass onto this member's camera target, from the assembled image, still on the transfer stream (a host
     // camera target is uploaded, blended and read back before the call returns, as gs_composite does)

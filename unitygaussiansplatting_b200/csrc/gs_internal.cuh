@@ -70,7 +70,7 @@ struct GsContext {
   gs::Buffer<float> d_depth;   // the frame's scene depth buffer when it was handed over in host memory
   uint32_t launches = 0;
   uint64_t pack_stats[4] = {0, 0, 0, 0};   // gs_debug_pack_stats
-  // surface objects of GS_MEM_ARRAY images, one per array per call: each batch is destroyed once `done` (recorded behind the
+  // surface objects of GS_MEM_ARRAY / GS_MEM_ARRAY_LAYER images, one per array per call: each batch is destroyed once `done` (recorded behind the
   // call's last use on `stream`) has completed, or at gs_sync / gs_destroy
   struct HeldSurfaces {
     cudaEvent_t done;
@@ -131,12 +131,23 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
 // the call only ever sets it, so the call reports every truncated list.  bin_done (optional) is recorded on ctx->stream when
 // binning ends.
 int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *as, const GsFrameParams *fp, bool first,
-            void *d_rt, uint32_t pitch, uint32_t fmt, cudaSurfaceObject_t surf = 0, cudaEvent_t bin_done = nullptr);
+            void *d_rt, uint32_t pitch, uint32_t fmt, Surface surf = Surface{}, cudaEvent_t bin_done = nullptr);
 // The composite pass (gs_composite) of a linear device render target onto `tgt` (host, device or CUDA-array memory, already
 // validated as W x H), enqueued on `s`.  A host target is uploaded and read back, and the call waits for `s`.
 int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H,
                         cudaStream_t s);
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch);
+inline bool is_array_image(const GsImage *im) { return im->memory == GS_MEM_ARRAY || im->memory == GS_MEM_ARRAY_LAYER; }
+// The CUDA array of a GS_MEM_ARRAY / GS_MEM_ARRAY_LAYER image, and in *layer the layer it names (-1: a 2-D array)
+inline cudaArray_t image_array(const GsImage *im, int32_t *layer) {
+  if (im->memory == GS_MEM_ARRAY_LAYER) {
+    const GsArrayLayer *d = static_cast<const GsArrayLayer *>(im->data);
+    *layer = (int32_t)d->layer;
+    return static_cast<cudaArray_t>(d->array);
+  }
+  *layer = -1;
+  return static_cast<cudaArray_t>(im->data);
+}
 uint32_t pix_bytes(uint32_t fmt);
 // The per-asset work buffers (order, keys, view data, ...) of an asset whose blobs as->d_* are already in HBM, the format
 // fields of as->av, and CSSetIndices: what gs_asset_upload and gs_pack_asset share.

@@ -229,12 +229,19 @@ cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, co
                            const uint32_t *block_bits, uint32_t n, bool clear_overflow, const BinScratch &bs, const SortScratch &sc,
                            cudaStream_t s, BinScratch *sorted, int *launches);
 
+// The surface of a CUDA-array image: a 2-D array (GS_MEM_ARRAY, layer -1), read and written with surf2Dread / surf2Dwrite, or
+// one layer of a layered array (GS_MEM_ARRAY_LAYER), read and written with surf2DLayeredread / surf2DLayeredwrite.
+struct Surface {
+  cudaSurfaceObject_t obj = 0;
+  int32_t layer = -1;
+};
+
 // The cameras of a run, in shared memory in the MULTI raster.  A run is a list of camera segments: camera c's pairs of the run
 // own the bin ids [bin_base, bin_base + its bins) and the raster tiles [tile_base, tile_base + its tiles).  A run of one camera
 // has bin_base = tile_base = 0.
 struct RasterCamera {
   uint8_t *rt;                 // linear device image, or nullptr: the CUDA array behind `surf`
-  cudaSurfaceObject_t surf;
+  Surface surf;
   const float *depth;          // the camera's scene depth buffer (device memory), or nullptr
   uint32_t pitch, tile_base, bin_base, ntx, binsX, W, H;
   uint32_t load;               // 1: blend under what the image holds (the camera's earlier run drew it); 0: the image starts cleared
@@ -263,14 +270,14 @@ void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, uin
 // band_packed, blend mode and GS_FLAG_LOAD_RT.  Images here are linear device memory (pointer, pitch) or, when the pointer is
 // null, a CUDA array behind a surface object.
 void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const float *zndc, bool extras,
-                   const BinScratch &bs, void *rt, uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s,
+                   const BinScratch &bs, void *rt, uint32_t rt_pitch_bytes, uint32_t rt_format, Surface rt_surf, cudaStream_t s,
                    const float *scene_depth);
 extern unsigned long long *g_raster_stats;   // diagnostics, see GS_RASTER_STATS
 uint32_t partition_own_bin_rows(const GsRenderOptions &opt, uint32_t binsY);
 uint32_t partition_own_tile_rows(const GsRenderOptions &opt, uint32_t binsY);
 void launch_unshuffle(const void *gathered, uint32_t parts, uint32_t band, uint32_t rows_pp, uint32_t fmt, void *out, uint32_t pitch,
                       uint32_t W, uint32_t H, cudaStream_t s);
-void launch_composite(const void *rt, uint32_t rt_pitch, cudaSurfaceObject_t rt_surf, uint32_t rt_format, void *target, uint32_t tgt_pitch,
-                      cudaSurfaceObject_t tgt_surf, uint32_t tgt_format, uint32_t W, uint32_t H, cudaStream_t s);
+void launch_composite(const void *rt, uint32_t rt_pitch, Surface rt_surf, uint32_t rt_format, void *target, uint32_t tgt_pitch,
+                      Surface tgt_surf, uint32_t tgt_format, uint32_t W, uint32_t H, cudaStream_t s);
 
 }  // namespace gs

@@ -411,23 +411,37 @@ __device__ __forceinline__ bool block_may_touch_quad(const float4 &A, float i2x,
   return axis_ok(A.z, A.w) && axis_ok(i2x, i2y);
 }
 
+// A texel of a CUDA-array image at byte column x_bytes, row y: surf2D* on a 2-D array, surf2DLayered* on a layer of a layered one.
+// LAYERED false: the image is known to be a 2-D array, and only the 2-D call is compiled.
+template <bool LAYERED, class T>
+__device__ __forceinline__ void surf_load(T *v, const Surface &s, uint32_t x_bytes, uint32_t y) {
+  if (LAYERED && s.layer >= 0) surf2DLayeredread(v, s.obj, (int)x_bytes, (int)y, s.layer);
+  else surf2Dread(v, s.obj, (int)x_bytes, (int)y);
+}
+template <bool LAYERED, class T>
+__device__ __forceinline__ void surf_store(const T &v, const Surface &s, uint32_t x_bytes, uint32_t y) {
+  if (LAYERED && s.layer >= 0) surf2DLayeredwrite(v, s.obj, (int)x_bytes, (int)y, s.layer);
+  else surf2Dwrite(v, s.obj, (int)x_bytes, (int)y);
+}
+
 // SEL ("extras"): a separate instantiation for frames with an edit selection and / or a scene depth buffer bound, so that
 // ordinary frames pay nothing.  Selected splats (records with opacity -1) take the pixel shader's other branch
 // (S/RenderGaussianSplats.shader:87-101); with `scene_depth` every fragment is depth-tested like the pass's ZTest LEqual
 // (reversed Z: quad depth >= stored depth), the per-splat quad depths being staged beside the records.
-// SURF: the target is a CUDA array (GS_MEM_ARRAY), read and written through the surface object `surf` instead of `rt`/`pitch`; a
-// separate instantiation so that the linear ones keep their code.
+// SURF: the target is a CUDA array, read and written through `surf` instead of `rt`/`pitch`: 1, a 2-D array (GS_MEM_ARRAY);
+// 2, some target is one layer of a layered array (GS_MEM_ARRAY_LAYER; surf.layer picks the surface call at the load and the
+// store).  Separate instantiations, so that the linear and the 2-D array ones keep their code.
 // MULTI: a run (DrawCameras) of several (camera, object) pairs.  The list holds every pair's entries, each tagged with its slot
 // in `objs`; the records are gathered from that pair's buffers, and each camera's result is what drawing its objects one after
 // the other leaves.  The grid covers every camera's tiles; a tile finds its camera c in `cams`, which gives it the screen size, bins, image (pointer and pitch, or a surface when the pointer is null), scene depth buffer and load
 // flag that the other instantiations take from fc and the image arguments.  The camera's bin ids start at its bin_base in
 // bin_ranges; tile_cost is indexed by tile_base + the tile.  SURF: some camera's image is a CUDA array.  MULTI with SEL is held
 // to 32 registers, 8 CTAs per SM, which its shared memory also fits (selected runs measured 20 % slower at 7).
-template <bool FP16_ROP, int OUT_FMT, bool STATS, bool SEL = false, bool SURF = false, bool MULTI = false>
+template <bool FP16_ROP, int OUT_FMT, bool STATS, bool SEL = false, int SURF = 0, bool MULTI = false>
 __global__ void __launch_bounds__(256, MULTI && SEL ? 8 : 0)
 k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const uint2 *__restrict__ bin_ranges,
          const uint32_t *__restrict__ tile_vals, const uint32_t *__restrict__ tile_order, uint32_t *__restrict__ tile_cost, uint32_t ntx,
-         uint8_t *__restrict__ rt, uint32_t pitch, cudaSurfaceObject_t surf, uint32_t band_packed, uint32_t load_rt,
+         uint8_t *__restrict__ rt, uint32_t pitch, Surface surf, uint32_t band_packed, uint32_t load_rt,
          unsigned long long *stats, const float *__restrict__ zndc, const float *__restrict__ scene_depth,
          std::conditional_t<MULTI, DrawObjects, NoRasterObjects> objs, std::conditional_t<MULTI, DrawCameras, NoRasterObjects> cams) {
   uint32_t st_batches = 0, st_culls = 0, st_cand = 0, st_eval = 0, st_blend = 0;   // GS_RASTER_STATS diagnostics (per warp)
@@ -460,9 +474,9 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
     ntx = cam.ntx; scene_depth = cam.depth; load_rt = cam.load;
     tile_base = cam.tile_base; bin_base = cam.bin_base;
   }
-  bool surf_io = SURF;
+  bool surf_io = SURF != 0;
   auto camera_image = [&]() {
-    if constexpr (MULTI) { const RasterCamera &cam = camera(cams); rt = cam.rt; pitch = cam.pitch; surf = cam.surf; surf_io = SURF && rt == nullptr; }
+    if constexpr (MULTI) { const RasterCamera &cam = camera(cams); rt = cam.rt; pitch = cam.pitch; surf = cam.surf; surf_io = SURF != 0 && rt == nullptr; }
   };
   const bool depth_test = SEL && scene_depth != nullptr;
   // FP32 blending into an RGBA16F target: drawing the objects one after the other stores (rounds to half) each object's result
@@ -503,12 +517,12 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
     const uint8_t *row = rt + (size_t)out_row * pitch;
     if (OUT_FMT == GS_PIX_RGBA16F) {
       uint2 v;
-      if (surf_io) surf2Dread(&v, surf, (int)(px * 8u), (int)out_row);
+      if (surf_io) surf_load<SURF == 2>(&v, surf, px * 8u, out_row);
       else v = reinterpret_cast<const uint2 *>(row)[px];
       d0 = f16lo(v.x); d1 = f16hi(v.x); d2 = f16lo(v.y); d3 = f16hi(v.y);
     } else {
       float4 v;
-      if (surf_io) surf2Dread(&v, surf, (int)(px * 16u), (int)out_row);
+      if (surf_io) surf_load<SURF == 2>(&v, surf, px * 16u, out_row);
       else v = reinterpret_cast<const float4 *>(row)[px];
       d0 = v.x; d1 = v.y; d2 = v.z; d3 = v.w;
     }
@@ -649,10 +663,10 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
       uint2 o;
       o.x = f32tof16(d0) | (f32tof16(d1) << 16);
       o.y = f32tof16(d2) | (f32tof16(d3) << 16);
-      if (surf_io) surf2Dwrite(o, surf, (int)(px * 8u), (int)out_row);
+      if (surf_io) surf_store<SURF == 2>(o, surf, px * 8u, out_row);
       else reinterpret_cast<uint2 *>(row)[px] = o;
     } else {
-      if (surf_io) surf2Dwrite(make_float4(d0, d1, d2, d3), surf, (int)(px * 16u), (int)out_row);
+      if (surf_io) surf_store<SURF == 2>(make_float4(d0, d1, d2, d3), surf, px * 16u, out_row);
       else reinterpret_cast<float4 *>(row)[px] = make_float4(d0, d1, d2, d3);
     }
   }
@@ -661,7 +675,7 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
 unsigned long long *g_raster_stats = nullptr;
 
 void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const float *zndc, bool extras,
-                   const BinScratch &bs, void *rt, uint32_t rt_pitch_bytes, uint32_t rt_format, cudaSurfaceObject_t rt_surf, cudaStream_t s,
+                   const BinScratch &bs, void *rt, uint32_t rt_pitch_bytes, uint32_t rt_format, Surface rt_surf, cudaStream_t s,
                    const float *scene_depth) {
   const Partition part = make_partition(opt);
   const uint32_t rows = part.own_tile_rows(fc.binsY);
@@ -694,7 +708,9 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const floa
   // a null `rt` means the target is a CUDA array behind rt_surf
 #define GS_LAUNCH_RASTER_TARGET(ROP, FMT)                                                                                       \
   do {                                                                                                                         \
-    if (out) GS_LAUNCH_RASTER(ROP, FMT, false); else GS_LAUNCH_RASTER(ROP, FMT, true);                                          \
+    if (out) GS_LAUNCH_RASTER(ROP, FMT, 0);                                                                                    \
+    else if (rt_surf.layer < 0) GS_LAUNCH_RASTER(ROP, FMT, 1);                                                                 \
+    else GS_LAUNCH_RASTER(ROP, FMT, 2);                                                                                        \
   } while (0)
   if (rt_format == GS_PIX_RGBA16F) {
     if (rop) GS_LAUNCH_RASTER_TARGET(true, GS_PIX_RGBA16F); else GS_LAUNCH_RASTER_TARGET(false, GS_PIX_RGBA16F);
@@ -716,20 +732,21 @@ void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, uin
   FrameConsts fc;   // screen size and bins come from each tile's camera
   memset(&fc, 0, sizeof(fc));
   const bool rop = blend_mode == GS_BLEND_FP16_ROP;
-  bool surf = false;
-  for (uint32_t i = 0; i < cams.count; ++i) surf |= cams.cam[i].rt == nullptr;
+  int surf = 0;   // the SURF instantiation: 2 if some image is a layer of a layered array, else 1 if some is a 2-D array
+  for (uint32_t i = 0; i < cams.count; ++i)
+    if (!cams.cam[i].rt) surf = std::max(surf, cams.cam[i].surf.layer < 0 ? 1 : 2);
 #define GS_RASTER_CAMS(ROP, FMT, SURF)                                                                                          \
   do {                                                                                                                         \
     if (objs.extras)                                                                                                           \
       chain_launch(k_raster<ROP, FMT, false, true, SURF, true>, tiles, 256, 0, s, fc, whole, nullptr, ranges, bs.tile_vals,        \
-          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, 0, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);                       \
+          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, Surface{}, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);               \
     else                                                                                                                       \
       chain_launch(k_raster<ROP, FMT, false, false, SURF, true>, tiles, 256, 0, s, fc, whole, nullptr, ranges, bs.tile_vals,       \
-          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, 0, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);                       \
+          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, Surface{}, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);               \
   } while (0)
 #define GS_RASTER_CAMS_TARGET(ROP, FMT)                                                                                         \
   do {                                                                                                                         \
-    if (surf) GS_RASTER_CAMS(ROP, FMT, true); else GS_RASTER_CAMS(ROP, FMT, false);                                            \
+    if (surf == 2) GS_RASTER_CAMS(ROP, FMT, 2); else if (surf) GS_RASTER_CAMS(ROP, FMT, 1); else GS_RASTER_CAMS(ROP, FMT, 0);   \
   } while (0)
   if (rt_format == GS_PIX_RGBA16F) {
     if (rop) GS_RASTER_CAMS_TARGET(true, GS_PIX_RGBA16F); else GS_RASTER_CAMS_TARGET(false, GS_PIX_RGBA16F);
@@ -772,22 +789,22 @@ __device__ __forceinline__ float gamma_to_linear(float x) {  // UnityCG.cginc Ga
 }
 
 // one pixel of an RGBA16F / RGBA32F image: linear memory at (base, pitch), or, when base is null, a CUDA array behind `surf`
-__device__ __forceinline__ float4 load_px(const uint8_t *base, uint32_t pitch, cudaSurfaceObject_t surf, uint32_t fmt, uint32_t x, uint32_t y) {
+__device__ __forceinline__ float4 load_px(const uint8_t *base, uint32_t pitch, const Surface &surf, uint32_t fmt, uint32_t x, uint32_t y) {
   if (fmt == GS_PIX_RGBA16F) {
     uint2 v;
     if (base) v = reinterpret_cast<const uint2 *>(base + (size_t)y * pitch)[x];
-    else surf2Dread(&v, surf, (int)(x * 8u), (int)y);
+    else surf_load<true>(&v, surf, x * 8u, y);
     return make_float4(f16lo(v.x), f16hi(v.x), f16lo(v.y), f16hi(v.y));
   }
   float4 c;
   if (base) c = reinterpret_cast<const float4 *>(base + (size_t)y * pitch)[x];
-  else surf2Dread(&c, surf, (int)(x * 16u), (int)y);
+  else surf_load<true>(&c, surf, x * 16u, y);
   return c;
 }
 
-__global__ void __launch_bounds__(256) k_composite(const uint8_t *__restrict__ rt, uint32_t rt_pitch, cudaSurfaceObject_t rt_surf,
+__global__ void __launch_bounds__(256) k_composite(const uint8_t *__restrict__ rt, uint32_t rt_pitch, Surface rt_surf,
                                                    uint32_t rt_fmt, uint8_t *__restrict__ tgt, uint32_t tgt_pitch,
-                                                   cudaSurfaceObject_t tgt_surf, uint32_t tgt_fmt, uint32_t W, uint32_t H) {
+                                                   Surface tgt_surf, uint32_t tgt_fmt, uint32_t W, uint32_t H) {
   const uint32_t x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= W || y >= H) return;
   const float4 c = load_px(rt, rt_pitch, rt_surf, rt_fmt, x, y);
@@ -804,15 +821,15 @@ __global__ void __launch_bounds__(256) k_composite(const uint8_t *__restrict__ r
     v.x = f32tof16(o.x) | (f32tof16(o.y) << 16);
     v.y = f32tof16(o.z) | (f32tof16(o.w) << 16);
     if (tgt) reinterpret_cast<uint2 *>(tgt + (size_t)y * tgt_pitch)[x] = v;
-    else surf2Dwrite(v, tgt_surf, (int)(x * 8u), (int)y);
+    else surf_store<true>(v, tgt_surf, x * 8u, y);
   } else {
     if (tgt) reinterpret_cast<float4 *>(tgt + (size_t)y * tgt_pitch)[x] = o;
-    else surf2Dwrite(o, tgt_surf, (int)(x * 16u), (int)y);
+    else surf_store<true>(o, tgt_surf, x * 16u, y);
   }
 }
 
-void launch_composite(const void *rt, uint32_t rt_pitch, cudaSurfaceObject_t rt_surf, uint32_t rt_format, void *target, uint32_t tgt_pitch,
-                      cudaSurfaceObject_t tgt_surf, uint32_t tgt_format, uint32_t W, uint32_t H, cudaStream_t s) {
+void launch_composite(const void *rt, uint32_t rt_pitch, Surface rt_surf, uint32_t rt_format, void *target, uint32_t tgt_pitch,
+                      Surface tgt_surf, uint32_t tgt_format, uint32_t W, uint32_t H, cudaStream_t s) {
   if (!W || !H) return;
   dim3 grid((W + 31) / 32, (H + 7) / 8);
   k_composite<<<grid, 256, 0, s>>>(reinterpret_cast<const uint8_t *>(rt), rt_pitch, rt_surf, rt_format, reinterpret_cast<uint8_t *>(target),

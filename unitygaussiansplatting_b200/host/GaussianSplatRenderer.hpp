@@ -37,6 +37,15 @@ inline GsImage ArrayImage(void *array, uint32_t width, uint32_t height, uint32_t
   return im;
 }
 
+// An image that is one layer of a layered CUDA array (GS_MEM_ARRAY_LAYER), e.g. one eye of an XR eye-texture array or one face of
+// a cube map, created with cudaArrayLayered | cudaArraySurfaceLoadStore.  The image points to `desc`, which must outlive every
+// call the image is passed to.
+inline GsImage ArrayLayerImage(GsArrayLayer *desc, uint32_t width, uint32_t height, uint32_t format = GS_PIX_RGBA16F) {
+  GsImage im = ArrayImage(desc, width, height, format);
+  im.memory = GS_MEM_ARRAY_LAYER;
+  return im;
+}
+
 class GaussianSplatRenderer {
  public:
   // serialized knobs, :225-251

@@ -88,14 +88,22 @@ class GaussianSplatContext:
 class CudaArrayImage:
     """A 2-D CUDA array (cudaArray_t, e.g. an imported graphics render texture) of RGBA float16 or float32 texels, given to the
     library as an image (GS_MEM_ARRAY): it is rendered into / composited onto in place.  The host creates the array, with
-    cudaArraySurfaceLoadStore, and keeps it alive; the library never allocates or frees one."""
+    cudaArraySurfaceLoadStore, and keeps it alive; the library never allocates or frees one.
 
-    def __init__(self, handle: int, width: int, height: int, dtype=np.float16):
+    layer: the array is a layered one (cudaArrayLayered, e.g. an XR eye-texture array or a cube map) and the image is this
+    layer of it (GS_MEM_ARRAY_LAYER); the other layers are left as they are."""
+
+    def __init__(self, handle: int, width: int, height: int, dtype=np.float16, layer=None):
         self.handle = int(handle)
         self.width, self.height = int(width), int(height)
         self.dtype = np.dtype(dtype)
         if self.dtype not in (np.float16, np.float32):
             raise ValueError("CudaArrayImage dtype must be float16 or float32")
+        self.layer = None if layer is None else int(layer)
+        if self.layer is not None and not 0 <= self.layer < 2 ** 32:
+            raise ValueError("CudaArrayImage layer must be a non-negative 32-bit index")
+        # the descriptor a GS_MEM_ARRAY_LAYER image points to, alive as long as this object
+        self._layer_desc = None if self.layer is None else N.GsArrayLayer(self.handle, self.layer, 0)
 
     @property
     def shape(self):
@@ -110,7 +118,12 @@ def _image(arr, width: int, height: int) -> N.GsImage:
         if arr.shape != (height, width, 4):
             raise ValueError("CUDA array is %dx%d, the image must be %dx%d" % (arr.width, arr.height, width, height))
         im.format = N.GS_PIX_RGBA16F if arr.dtype == np.float16 else N.GS_PIX_RGBA32F
-        im.data, im.memory, im.row_pitch_bytes = arr.handle, N.GS_MEM_ARRAY, 0
+        if arr.layer is None:
+            im.data, im.memory = arr.handle, N.GS_MEM_ARRAY
+        else:
+            im.data, im.memory = C.addressof(arr._layer_desc), N.GS_MEM_ARRAY_LAYER
+            im._layer_desc = arr._layer_desc   # the descriptor lives as long as the image that points to it
+        im.row_pitch_bytes = 0
         return im
     if isinstance(arr, np.ndarray):
         if arr.shape != (height, width, 4) or not arr.flags.c_contiguous:
