@@ -2,9 +2,9 @@
 (cudaExternalMemoryGetMappedMipmappedArray / cudaGraphicsSubResourceGetMappedArray).  The library renders into and composites
 onto such an array in place, through surface objects.
 
-Arrays are made here with the CUDA runtime torch already loaded (a runtime cudaArray_t is a driver CUarray in the device's
-primary context, so the library's own runtime can use it).  Every GPU test compares the array result byte for byte with the
-same call on a torch device tensor: the linear path is pinned to the oracle elsewhere, so equality is the parity contract."""
+Arrays are made by cuda_arrays.Cudart, through the CUDA runtime torch already loaded.  Every GPU test compares the array result
+byte for byte with the same call on a torch device tensor: the linear path is pinned to the oracle elsewhere, so equality is the
+parity contract."""
 import ctypes as C
 import re
 import sys
@@ -13,15 +13,11 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from cuda_arrays import KIND_FLOAT, KIND_UNSIGNED, SURFACE_LOAD_STORE, Cudart
 from util import camera
 
 ROOT = Path(__file__).resolve().parents[1]
 GOLD = Path(__file__).parent / "golden"
-
-# cudaChannelFormatKind / cudaArray flags / cudaMemcpyKind (cuda_runtime_api.h)
-_KIND_UNSIGNED, _KIND_FLOAT = 1, 2
-_SURFACE_LOAD_STORE = 0x02
-_H2D, _D2H = 1, 2
 
 
 def test_header_and_python_agree_on_gs_mem_array():
@@ -34,53 +30,9 @@ def test_header_and_python_agree_on_gs_mem_array():
     assert N.GS_MEM_ARRAY == 2
 
 
-class _ChannelDesc(C.Structure):
-    _fields_ = [("x", C.c_int), ("y", C.c_int), ("z", C.c_int), ("w", C.c_int), ("f", C.c_int)]
-
-
-class _Cudart:
-    """cudaMallocArray / cudaMemcpy2D{To,From}Array / cudaFreeArray through the runtime torch loaded."""
-
-    def __init__(self):
-        import torch
-        torch.cuda.init()
-        self.lib = C.CDLL("libcudart.so.12")   # resolves to the copy torch already loaded (same soname)
-        self.lib.cudaMallocArray.argtypes = [C.POINTER(C.c_void_p), C.POINTER(_ChannelDesc), C.c_size_t, C.c_size_t, C.c_uint]
-        self.lib.cudaMemcpy2DToArray.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
-        self.lib.cudaMemcpy2DFromArray.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
-        self.lib.cudaFreeArray.argtypes = [C.c_void_p]
-        self.live = []
-
-    def _check(self, rc, what):
-        assert rc == 0, "%s failed with CUDA error %d" % (what, rc)
-
-    def array(self, width, height, bits=16, kind=_KIND_FLOAT, flags=_SURFACE_LOAD_STORE):
-        h = C.c_void_p()
-        desc = _ChannelDesc(bits, bits, bits, bits, kind)
-        self._check(self.lib.cudaMallocArray(C.byref(h), C.byref(desc), width, height, flags), "cudaMallocArray")
-        self.live.append(h.value)
-        return h.value
-
-    def upload(self, handle, host):
-        host = np.ascontiguousarray(host)
-        row = host.shape[1] * host.shape[2] * host.itemsize
-        self._check(self.lib.cudaMemcpy2DToArray(handle, 0, 0, host.ctypes.data, row, row, host.shape[0], _H2D), "cudaMemcpy2DToArray")
-
-    def download(self, handle, shape, dtype):
-        out = np.empty(shape, dtype)
-        row = shape[1] * shape[2] * out.itemsize
-        self._check(self.lib.cudaMemcpy2DFromArray(out.ctypes.data, row, handle, 0, 0, row, shape[0], _D2H), "cudaMemcpy2DFromArray")
-        return out
-
-    def free_all(self):
-        for h in self.live:
-            self.lib.cudaFreeArray(h)
-        self.live = []
-
-
 @pytest.fixture
 def rt_arrays(ctx):
-    ca = _Cudart()
+    ca = Cudart()
     yield ca
     ctx.sync()
     ca.free_all()
@@ -88,7 +40,7 @@ def rt_arrays(ctx):
 
 def _image_array(g, ca, w, h, dtype=np.float16, fill=None):
     """A CudaArrayImage of (h, w) RGBA texels, pre-filled with `fill` (default: random halves / floats)."""
-    handle = ca.array(w, h, 16 if dtype == np.float16 else 32)
+    handle = ca.array(w, h, dtype=dtype)
     if fill is None:
         fill = np.random.default_rng(w * 7919 + h).random((h, w, 4), np.float32).astype(dtype)
     ca.upload(handle, np.broadcast_to(np.asarray(fill, dtype), (h, w, 4)))
@@ -371,16 +323,14 @@ def test_array_rejections_leave_the_array_untouched(g, ctx, rt_arrays):
 
     pattern = np.random.default_rng(3).random((128, 128, 4), np.float32).astype(np.float16)
 
-    def filled(width=128, bits=16, kind=_KIND_FLOAT, flags=_SURFACE_LOAD_STORE, fill=pattern):
-        h = rt_arrays.array(width, 128, bits, kind, flags)
-        rt_arrays.upload(h, fill)
-        return h
+    def filled(width=128, kind=KIND_FLOAT, flags=SURFACE_LOAD_STORE, fill=pattern):
+        return rt_arrays.array(width, 128, dtype=fill.dtype, flags=flags, kind=kind, fill=fill)
 
     def unchanged(h, fill=pattern, width=128):
         return np.array_equal(rt_arrays.download(h, (128, width, 4), fill.dtype).view(np.uint8), fill.view(np.uint8))
 
     bytes8 = np.random.default_rng(4).integers(0, 256, (128, 128, 4), np.uint8)
-    h = filled(bits=8, kind=_KIND_UNSIGNED, fill=bytes8)                      # uint8 x 4
+    h = filled(kind=KIND_UNSIGNED, fill=bytes8)                               # uint8 x 4
     assert frame(h) == -4 and "channel format" in lib.gs_last_error(ctx.handle).decode()
     ctx.sync()
     assert unchanged(h, bytes8)

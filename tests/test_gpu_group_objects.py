@@ -154,13 +154,13 @@ def test_objects_device_array_and_async_host_images(g, ctx):
     """Member images of every kind in one group: a device tensor, a CUDA array, and pinned host images filled asynchronously
     (GS_FLAG_ASYNC_READBACK, two in rotation, completed by sync())."""
     import torch
-    from test_gpu_array_targets import _Cudart
+    from cuda_arrays import Cudart
     cams = _cams(g, 320, 200, 4)
     assets, knobs = _scene(g, 320, 200)
     want = _single(g, ctx, assets, knobs, cams)
     grp, objs = _group(assets, knobs, 3)
     grp.async_readback = True
-    rt = _Cudart()
+    rt = Cudart()
     from unitygaussiansplatting_b200.renderer import CudaArrayImage
     arr = CudaArrayImage(rt.array(320, 200), 320, 200)
     dev = torch.zeros((200, 320, 4), dtype=torch.float16, device="cuda")
@@ -181,7 +181,7 @@ def test_objects_camera_targets(g, ctx):
     """Members with a camera target end with the bytes single-GPU gs_composite leaves on the same initial target (device,
     CUDA array and host targets); a member without one, and every member's render target, is as without targets."""
     import torch
-    from test_gpu_array_targets import _Cudart
+    from cuda_arrays import Cudart
     from unitygaussiansplatting_b200.renderer import CudaArrayImage
     W, H = 320, 200
     cams = _cams(g, W, H, 3)
@@ -189,7 +189,7 @@ def test_objects_camera_targets(g, ctx):
     want = _single(g, ctx, assets, knobs, cams)
     rng = np.random.default_rng(9)
     grp, objs = _group(assets, knobs, 4)
-    cu = _Cudart()
+    cu = Cudart()
     comp = g.GaussianSplatRenderer(assets[2], ctx)   # gs_composite on one GPU, through a renderer's context
     try:
         for f, cam in enumerate(cams):
@@ -351,7 +351,7 @@ def test_member_context_sync_with_a_pending_array_camera_target(g, ctx):
     """gs_sync on a member's own context right after the call, before gs_group_sync, waits for the composite onto a CUDA-array
     camera target (on the member's transfer stream) before it releases that target's surface; the target ends right."""
     import torch
-    from test_gpu_array_targets import _Cudart
+    from cuda_arrays import Cudart
     from unitygaussiansplatting_b200.renderer import CudaArrayImage
     W, H = 320, 200
     cam = _cams(g, W, H, 1)[0]
@@ -364,7 +364,7 @@ def test_member_context_sync_with_a_pending_array_camera_target(g, ctx):
     ctx.sync()
     expect = expect.cpu().numpy()
     grp, objs = _group(assets, knobs, 2)
-    cu = _Cudart()
+    cu = Cudart()
     try:
         targets = [CudaArrayImage(cu.array(W, H), W, H) for _ in range(2)]
         for t in targets:

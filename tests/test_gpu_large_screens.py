@@ -129,16 +129,17 @@ def test_wide_screen_target_kinds_and_composite(g, O, ctx):
     """Host, device and CUDA-array render targets hold the oracle's frame; gs_composite of it onto host and CUDA-array camera
     targets leaves what the oracle's composite does."""
     import torch
-    from test_gpu_array_targets import _Cudart
+    from cuda_arrays import Cudart
     W, H = 16384, 512
     cam = camera(g, W, H)
     asset = _edge_scene(g, cam)
     fp, _keep = g.make_frame_params(cam)
     ref = O.frame(asset, fp, threads=O.max_threads())["rt"]
-    cu = _Cudart()
+    cu = Cudart()
     try:
         host = np.zeros((H, W, 4), np.float16)
         dev = torch.zeros((H, W, 4), dtype=torch.float16, device="cuda")
+        torch.cuda.synchronize()   # filled on torch's stream: before the context's stream draws into it
         arr = g.CudaArrayImage(cu.array(W, H), W, H)
         got = {}
         for name, target in (("host", host), ("device", dev), ("array", arr)):
@@ -180,6 +181,9 @@ def test_splat_inside_the_last_bin_is_drawn(g, O, ctx, edge, last_bin):
                                          0.9), "VeryHigh")
     r = g.GaussianSplatRenderer(asset, ctx)
     rt = torch.zeros((H, W, 4), dtype=torch.float16, device="cuda")
+    # the zero fill runs on torch's stream and the frame on the context's own: the fill must land first (the splat's bin is
+    # the last thing a 2 GiB fill writes, and the frame reaches it in well under a millisecond)
+    torch.cuda.synchronize()
     r.SortAndRenderSplats(cam, rt=rt)
     ctx.sync()
     torch.cuda.synchronize()

@@ -2,9 +2,9 @@
 mode, or a cube map, looks like once it is imported into CUDA.  The library renders into and composites onto the layer in place,
 through a layered surface, and leaves the array's other layers alone.
 
-Arrays are made here with cudaMalloc3DArray through the CUDA runtime torch already loaded, as test_gpu_array_targets.py makes its
-2-D arrays.  Every result is compared byte for byte with the same call on linear device memory (or, for the stereo run, with the
-camera loop it stands for), and every layer the call does not name is checked to still hold its sentinel."""
+Arrays are made by cuda_arrays.Cudart, as test_gpu_array_targets.py makes its 2-D arrays.  Every result is compared byte for
+byte with the same call on linear device memory (or, for the stereo run, with the camera loop it stands for), and every layer
+the call does not name is checked to still hold its sentinel."""
 import ctypes as C
 import re
 from pathlib import Path
@@ -12,14 +12,11 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from cuda_arrays import KIND_UNSIGNED, LAYERED, SURFACE_LOAD_STORE, Cudart
 from util import camera
 
 ROOT = Path(__file__).resolve().parents[1]
 
-# cudaChannelFormatKind / cudaArray flags / cudaMemcpyKind (cuda_runtime_api.h)
-_KIND_UNSIGNED, _KIND_FLOAT = 1, 2
-_LAYERED, _SURFACE_LOAD_STORE = 0x01, 0x02
-_H2D, _D2H = 1, 2
 INVALID, UNSUPPORTED = -1, -4
 SENTINEL = -3.25   # exact in half and float
 
@@ -46,74 +43,9 @@ def test_cuda_array_image_layer_argument(g):
         g.CudaArrayImage(0x1234, 8, 4, layer=-1)
 
 
-class _Dim3(C.Structure):
-    _fields_ = [("x", C.c_size_t), ("y", C.c_size_t), ("z", C.c_size_t)]   # cudaExtent and cudaPos
-
-
-class _PitchedPtr(C.Structure):
-    _fields_ = [("ptr", C.c_void_p), ("pitch", C.c_size_t), ("xsize", C.c_size_t), ("ysize", C.c_size_t)]
-
-
-class _Memcpy3DParms(C.Structure):
-    _fields_ = [("srcArray", C.c_void_p), ("srcPos", _Dim3), ("srcPtr", _PitchedPtr),
-                ("dstArray", C.c_void_p), ("dstPos", _Dim3), ("dstPtr", _PitchedPtr), ("extent", _Dim3), ("kind", C.c_int)]
-
-
-class _ChannelDesc(C.Structure):
-    _fields_ = [("x", C.c_int), ("y", C.c_int), ("z", C.c_int), ("w", C.c_int), ("f", C.c_int)]
-
-
-class _Cudart:
-    """cudaMalloc3DArray / cudaMemcpy3D / cudaFreeArray through the runtime torch loaded."""
-
-    def __init__(self):
-        import torch
-        torch.cuda.init()
-        self.lib = C.CDLL("libcudart.so.12")   # resolves to the copy torch already loaded (same soname)
-        self.lib.cudaMalloc3DArray.argtypes = [C.POINTER(C.c_void_p), C.POINTER(_ChannelDesc), _Dim3, C.c_uint]
-        self.lib.cudaMemcpy3D.argtypes = [C.POINTER(_Memcpy3DParms)]
-        self.lib.cudaFreeArray.argtypes = [C.c_void_p]
-        self.live = []
-
-    def array(self, w, h, depth, dtype=np.float16, flags=_LAYERED | _SURFACE_LOAD_STORE, kind=_KIND_FLOAT, fill=SENTINEL):
-        """A (depth, h, w) array of RGBA texels (depth 0: a 2-D array), every texel set to `fill`."""
-        dtype = np.dtype(dtype)
-        bits = 8 * dtype.itemsize
-        h_ = C.c_void_p()
-        rc = self.lib.cudaMalloc3DArray(C.byref(h_), C.byref(_ChannelDesc(bits, bits, bits, bits, kind)), _Dim3(w, h, depth), flags)
-        assert rc == 0, "cudaMalloc3DArray failed with CUDA error %d" % rc
-        self.live.append(h_.value)
-        self.upload(h_.value, np.broadcast_to(np.asarray(fill, dtype), (max(depth, 1), h, w, 4)))
-        return h_.value
-
-    def _copy(self, handle, host, kind):
-        p = _Memcpy3DParms()
-        pitched = _PitchedPtr(host.ctypes.data, host.shape[2] * 4 * host.itemsize, host.shape[2], host.shape[1])
-        if kind == _H2D:
-            p.srcPtr, p.dstArray = pitched, handle
-        else:
-            p.srcArray, p.dstPtr = handle, pitched
-        p.extent, p.kind = _Dim3(host.shape[2], host.shape[1], host.shape[0]), kind
-        rc = self.lib.cudaMemcpy3D(C.byref(p))
-        assert rc == 0, "cudaMemcpy3D failed with CUDA error %d" % rc
-
-    def upload(self, handle, host):
-        self._copy(handle, np.ascontiguousarray(host), _H2D)
-
-    def download(self, handle, shape, dtype):
-        out = np.empty(shape, dtype)   # (layers, h, w, 4)
-        self._copy(handle, out, _D2H)
-        return out
-
-    def free_all(self):
-        for h in self.live:
-            self.lib.cudaFreeArray(h)
-        self.live = []
-
-
 @pytest.fixture
 def ca(ctx):
-    c = _Cudart()
+    c = Cudart()
     yield c
     ctx.sync()
     c.free_all()
@@ -124,7 +56,7 @@ class Layered:
 
     def __init__(self, g, ca, w, h, depth, dtype=np.float16):
         self.g, self.ca, self.w, self.h, self.depth, self.dtype = g, ca, w, h, depth, np.dtype(dtype)
-        self.handle = ca.array(w, h, depth, dtype)
+        self.handle = ca.array(w, h, depth, dtype, fill=SENTINEL)
 
     def image(self, k):
         return self.g.CudaArrayImage(self.handle, self.w, self.h, self.dtype, layer=k)
@@ -311,7 +243,7 @@ def test_stereo_pair_on_layers_is_the_camera_loop(g, ctx, ca, same_layer):
 
         # the pair drawn by gs_frame_cameras into two separate 2-D arrays: the run it forms
         flat = renderers()
-        flat_rts = [ca.array(W, H, 0, flags=_SURFACE_LOAD_STORE, fill=0.0) for _ in eyes]
+        flat_rts = [ca.array(W, H, 0, flags=SURFACE_LOAD_STORE, fill=0.0) for _ in eyes]
         n0 = ctx.stage_times().kernel_launches
         g.SortAndRenderCameras(flat, eyes, [g.CudaArrayImage(h, W, H) for h in flat_rts],
                                [_tensor(bg) for _ in eyes])
@@ -416,11 +348,11 @@ def test_layer_refusals_write_nothing(g, ctx, ca):
         got = ca.download(h, (max(depth, 1), 128, 128, 4), dtype)
         return (got == np.asarray(fill, dtype)).all()
 
-    good = ca.array(128, 128, 2)
-    flat = ca.array(128, 128, 0, flags=_SURFACE_LOAD_STORE)                 # a 2-D array
-    no_surface = ca.array(128, 128, 2, flags=_LAYERED)                      # no cudaArraySurfaceLoadStore
-    wide = ca.array(128, 128, 2, np.float32)                                # 4 x 32-bit for an RGBA16F image
-    bytes8 = ca.array(128, 128, 2, np.uint8, kind=_KIND_UNSIGNED, fill=7)   # 4 x 8-bit
+    good = ca.array(128, 128, 2, fill=SENTINEL)
+    flat = ca.array(128, 128, 0, flags=SURFACE_LOAD_STORE, fill=SENTINEL)             # a 2-D array
+    no_surface = ca.array(128, 128, 2, flags=LAYERED, fill=SENTINEL)                  # no cudaArraySurfaceLoadStore
+    wide = ca.array(128, 128, 2, np.float32, fill=SENTINEL)                           # 4 x 32-bit for an RGBA16F image
+    bytes8 = ca.array(128, 128, 2, np.uint8, kind=KIND_UNSIGNED, fill=7)              # 4 x 8-bit
     cases = [
         (image(good, layer=2), INVALID, "layer"),                                     # layer == depth
         (image(good, layer=1 << 31), INVALID, "layer"),

@@ -251,6 +251,12 @@ def test_async_readback_equals_blocking(g, ctx):
     got.append(pins[0].numpy().copy())      # frame 4
     for k in range(5):
         assert np.array_equal(got[k].view(np.uint16), want[k].view(np.uint16)), "frame %d" % k
+    # gs_render ignores GS_FLAG_ASYNC_READBACK: its host target is read back before it returns.  The last frame redrawn
+    # staged, with no gs_sync, into a fresh pinned image (a copy into pageable memory would complete before returning anyway)
+    pinned = torch.zeros((300, 400, 4), dtype=torch.float16).pin_memory()
+    r.CalcViewData(cams[4])
+    r.DrawSplats(cams[4], pinned.numpy())
+    assert np.array_equal(pinned.numpy().view(np.uint16), want[4].view(np.uint16)), "staged redraw of frame 4"
     r.Dispose()
 
 

@@ -175,80 +175,6 @@ static int ensure_async_readback(GsContext *ctx) {
   return GS_OK;
 }
 
-uint32_t pix_bytes(uint32_t fmt) { return fmt == GS_PIX_RGBA16F ? 8u : 16u; }
-
-// ---- GS_MEM_ARRAY / GS_MEM_ARRAY_LAYER images -----------------------------------------------------------------------------
-// Destroys the held surface objects whose last use has completed; with `all`, every one, after waiting for its event.  The
-// event, not the context stream, is what guards a batch: the group path composites onto CUDA-array camera targets on a
-// member's transfer stream, which the context stream never waits for.
-static void release_surfaces(GsContext *ctx, bool all) {
-  auto &held = ctx->held_surfaces;
-  size_t keep = 0;
-  for (size_t i = 0; i < held.size(); ++i) {
-    bool done = all;
-    if (all) {
-      if (cudaEventSynchronize(held[i].done) != cudaSuccess) cudaGetLastError();   // failed: nothing will use the surfaces any more
-    } else {
-      const cudaError_t q = cudaEventQuery(held[i].done);
-      done = q != cudaErrorNotReady;   // completed, or failed: either way nothing will use the surfaces any more
-      if (!done && cudaPeekAtLastError() == cudaErrorNotReady) cudaGetLastError();
-    }
-    if (done) {
-      for (cudaSurfaceObject_t so : held[i].surfs) cudaDestroySurfaceObject(so);
-      ctx->spare_events.push_back(held[i].done);
-    } else {
-      if (keep != i) held[keep] = std::move(held[i]);
-      ++keep;
-    }
-  }
-  held.resize(keep);
-}
-
-// The surface objects one call creates for its CUDA-array images, one per array: the layers of one layered array share it.
-// When the call returns they are handed to the context behind an event recorded on the stream that used them (the context's,
-// unless another is named) after their last use.  They are never cached by cudaArray_t value beyond the call: a freed array's
-// handle can be reused by the next allocation.
-class CallSurfaces {
- public:
-  explicit CallSurfaces(GsContext *ctx, cudaStream_t stream = nullptr) : ctx_(ctx), stream_(stream ? stream : ctx->stream) {}
-  CallSurfaces(const CallSurfaces &) = delete;
-  CallSurfaces &operator=(const CallSurfaces &) = delete;
-  ~CallSurfaces() {
-    if (made_.empty()) return;
-    cudaEvent_t ev = nullptr;
-    if (!ctx_->spare_events.empty()) { ev = ctx_->spare_events.back(); ctx_->spare_events.pop_back(); }
-    else if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) ev = nullptr;
-    if (ev && cudaEventRecord(ev, stream_) == cudaSuccess) {
-      ctx_->held_surfaces.push_back({ev, std::move(made_)});
-      return;
-    }
-    cudaStreamSynchronize(stream_);   // no event to wait for: wait for the stream itself
-    for (cudaSurfaceObject_t so : made_) cudaDestroySurfaceObject(so);
-    if (ev) ctx_->spare_events.push_back(ev);
-  }
-  // `im` has passed image_ok as a GS_MEM_ARRAY or GS_MEM_ARRAY_LAYER image
-  int make(const GsImage *im, Surface *out) {
-    const cudaArray_t arr = image_array(im, &out->layer);
-    for (size_t i = 0; i < arrays_.size(); ++i)
-      if (arrays_[i] == arr) { out->obj = made_[i]; return GS_OK; }
-    if (made_.empty()) release_surfaces(ctx_, false);
-    cudaResourceDesc rd;
-    memset(&rd, 0, sizeof(rd));
-    rd.resType = cudaResourceTypeArray;
-    rd.res.array.array = arr;
-    GS_CUDA_TRY(ctx_, cudaCreateSurfaceObject(&out->obj, &rd));
-    made_.push_back(out->obj);
-    arrays_.push_back(arr);
-    return GS_OK;
-  }
-
- private:
-  GsContext *ctx_;
-  cudaStream_t stream_;
-  std::vector<cudaSurfaceObject_t> made_;
-  std::vector<cudaArray_t> arrays_;   // made_[i] is the surface of arrays_[i]
-};
-
 int reserve_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, std::initializer_list<cudaStream_t> users) {
   if (fp->cutouts && fp->cutout_count) GS_CUDA_TRY(ctx, ctx->d_cutouts.reserve(fp->cutout_count, users));
   const size_t words = ((size_t)as->av.n + 31) / 32;
@@ -429,45 +355,6 @@ int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, G
   return GS_OK;
 }
 
-int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch) {
-  if (!im || !im->data) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image is null");
-  if (im->format > GS_PIX_RGBA32F) return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "unsupported pixel format");
-  if (im->memory > GS_MEM_ARRAY_LAYER || im->memory == 3)   // 3 is not a memory kind
-    return fail(ctx, GS_ERR_INVALID_ARGUMENT, "unknown image memory kind");
-  if (im->width != W || im->height != H) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image size does not match screen size");
-  if (is_array_image(im)) {   // a 2-D CUDA array (data is a cudaArray_t), or a layer of a layered one (data is a GsArrayLayer *)
-    if (im->row_pitch_bytes) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "row_pitch_bytes must be 0 for a CUDA array image");
-    const bool layered = im->memory == GS_MEM_ARRAY_LAYER;
-    if (layered) {
-      const GsArrayLayer *d = static_cast<const GsArrayLayer *>(im->data);
-      if (!d->array || d->reserved) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "GsArrayLayer: array is null or reserved is not 0");
-    }
-    int32_t layer = -1;
-    cudaChannelFormatDesc cd;
-    cudaExtent ext;
-    unsigned int flags = 0;
-    const cudaError_t e = cudaArrayGetInfo(&cd, &ext, &flags, image_array(im, &layer));
-    if (e != cudaSuccess) { cudaGetLastError(); return fail(ctx, GS_ERR_INVALID_ARGUMENT, std::string("not a CUDA array: ") + cudaGetErrorString(e)); }
-    const int bits = im->format == GS_PIX_RGBA16F ? 16 : 32;
-    if (cd.f != cudaChannelFormatKindFloat || cd.x != bits || cd.y != bits || cd.z != bits || cd.w != bits)
-      return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "the CUDA array's channel format does not match the image's pixel format");
-    if (!layered && (ext.width != W || ext.height != H || ext.depth != 0))
-      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array is not a 2-D array of the image's size");
-    if (layered && (ext.width != W || ext.height != H || !(flags & cudaArrayLayered)))
-      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array is not a layered array of the image's size");
-    if (layered && (uint32_t)layer >= ext.depth)
-      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the layer is not below the CUDA array's layer count");
-    if (!(flags & cudaArraySurfaceLoadStore))
-      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array was not created with cudaArraySurfaceLoadStore");
-    *pitch = 0;
-    return GS_OK;
-  }
-  uint32_t p = im->row_pitch_bytes ? im->row_pitch_bytes : W * pix_bytes(im->format);
-  if (p < W * pix_bytes(im->format) || (p % pix_bytes(im->format)) != 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "bad row pitch");
-  *pitch = p;
-  return GS_OK;
-}
-
 // options shared by gs_render / gs_frame: validated copy
 int check_options(GsContext *ctx, const FrameConsts &fc, GsRenderOptions &opt) {
   if (opt.blend_mode > GS_BLEND_FP32) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "bad blend mode");
@@ -477,19 +364,6 @@ int check_options(GsContext *ctx, const FrameConsts &fc, GsRenderOptions &opt) {
     opt.band_packed = 0; opt.partition_count = 0; opt.partition_index = 0;
   } else {
     opt.row_begin = opt.row_end = 0;
-  }
-  return GS_OK;
-}
-
-// what the compositor starts from in a device staging image: the host image's content (GS_FLAG_LOAD_RT), or zeros where a
-// partition leaves rows untouched
-static int init_staging(GsContext *ctx, const GsRenderOptions &opt, void *d_rt, uint32_t d_pitch, uint32_t W, uint32_t H, uint32_t fmt,
-                        const GsImage *host_rt, uint32_t host_pitch) {
-  if (opt.flags & GS_FLAG_LOAD_RT) {
-    if (host_rt) GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(d_rt, d_pitch, host_rt->data, host_pitch, (size_t)W * pix_bytes(fmt), H, cudaMemcpyHostToDevice, ctx->stream));
-    else GS_CUDA_TRY(ctx, cudaMemsetAsync(d_rt, 0, (size_t)d_pitch * H, ctx->stream));
-  } else if (opt.partition_count > 1 || opt.row_end > opt.row_begin) {
-    GS_CUDA_TRY(ctx, cudaMemsetAsync(d_rt, 0, (size_t)d_pitch * H, ctx->stream));
   }
   return GS_OK;
 }
@@ -523,6 +397,83 @@ static int check_bin_overflow(GsContext *ctx) {
   ctx->times.tile_entries = ec[0];
   if (ec[1]) return fail(ctx, GS_ERR_OUT_OF_MEMORY, "tile-list capacity exceeded (splat footprints cover too many tiles)");
   return GS_OK;
+}
+
+// d_rt == nullptr: the render target is the CUDA array (layer) behind rt_surf.  Enqueued on `s`: the context's stream, or the group
+// path's transfer stream (surfs must then hand its surfaces over on `s` as well).
+static int composite_impl(GsContext *ctx, CallSurfaces &surfs, const void *d_rt, uint32_t rt_pitch, Surface rt_surf,
+                          uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H, cudaStream_t s) {
+  GsNvtxRange nvtx("GaussianSplat.Compose");
+  uint32_t tp = 0;
+  int rc = image_ok(ctx, tgt, W, H, &tp);
+  if (rc) return rc;
+  const bool host = tgt->memory == GS_MEM_HOST;
+  if (host) GS_CUDA_TRY(ctx, ctx->tgt_scratch.reserve((size_t)W * pix_bytes(tgt->format) * H, {ctx->stream}));
+  DeviceImage t;
+  if ((rc = bind_image(ctx, surfs, tgt, tp, tgt->format, W, H, ctx->tgt_scratch.get(), StagingFill::kUpload, s, &t))) return rc;
+  launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, t.d_rt, t.pitch, t.surf, tgt->format, W, H, s);
+  if (host && (rc = copy_to_image(ctx, tgt, tp, t.d_rt, t.pitch, W, H, s))) return rc;
+  if (s == ctx->stream) rec(ctx, EV_COMP1);
+  ctx->launches += 1;
+  GS_CUDA_TRY(ctx, cudaGetLastError());
+  if (host) GS_CUDA_TRY(ctx, cudaStreamSynchronize(s));
+  return GS_OK;
+}
+int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H,
+                        cudaStream_t s) {
+  CallSurfaces surfs(ctx, s);
+  return composite_impl(ctx, surfs, d_rt, rt_pitch, Surface{}, rt_fmt, tgt, W, H, s);
+}
+
+// The device image a frame draws into (DeviceImage): `rt` itself when it is device or array memory, else library scratch (or,
+// with GS_FLAG_ASYNC_READBACK, one of the two asynchronous staging images) that a host `rt` is read back from.
+struct FrameImage : DeviceImage {
+  bool async_rb = false;
+  int slot = 0;
+};
+
+// what a frame does between its view-calcs and its draw; rt (when given) has passed image_ok.  staging (optional): where a
+// staging image goes instead of rt_scratch (one slice per camera of a run of several cameras).  A staging image starts from
+// the host rt's content (GS_FLAG_LOAD_RT; zeros without an rt), or from zeros where a partition leaves rows untouched.
+static int begin_frame_image(GsContext *ctx, CallSurfaces &surfs, const GsRenderOptions &opt, GsImage *rt, uint32_t rt_pitch,
+                             uint32_t rt_fmt, const GsImage *tgt, uint32_t W, uint32_t H, FrameImage *fi, void *staging = nullptr) {
+  int rc = GS_OK;
+  const bool staged = !rt || rt->memory == GS_MEM_HOST;
+  const size_t bytes = (size_t)W * pix_bytes(rt_fmt) * H;
+  fi->async_rb = rt && staged && !tgt && (opt.flags & GS_FLAG_ASYNC_READBACK) != 0;
+  if (fi->async_rb) {
+    if ((rc = ensure_async_readback(ctx))) return rc;
+    const int slot = fi->slot = ctx->rt_flip;
+    ctx->rt_flip ^= 1;
+    // the staging image of two frames ago: its copy must have left the device before this frame's raster overwrites it
+    if (ctx->copy_pending[slot]) GS_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy_done[slot], 0));
+    GS_CUDA_TRY(ctx, ctx->rt_async[slot].reserve(bytes, {ctx->stream, ctx->copy_stream}));
+    staging = ctx->rt_async[slot].get();
+  } else if (staged && !staging) {
+    GS_CUDA_TRY(ctx, ctx->rt_scratch.reserve(bytes, {ctx->stream}));
+    staging = ctx->rt_scratch.get();
+  }
+  const StagingFill fill = (opt.flags & GS_FLAG_LOAD_RT) ? (rt ? StagingFill::kUpload : StagingFill::kZero)
+                           : (opt.partition_count > 1 || opt.row_end > opt.row_begin) ? StagingFill::kZero : StagingFill::kNone;
+  return bind_image(ctx, surfs, rt, rt_pitch, rt_fmt, W, H, staging, fill, ctx->stream, fi);
+}
+
+// what follows the draw: the read-back of a host `rt` (enqueued only, with GS_FLAG_ASYNC_READBACK) and the composite onto the
+// camera target.  The caller checks the bin list once, after its last draw.
+static int end_frame_image(GsContext *ctx, CallSurfaces &surfs, GsImage *rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W,
+                           uint32_t H, const FrameImage &fi) {
+  int rc = GS_OK;
+  if (fi.async_rb) {
+    const int slot = fi.slot;
+    GS_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_rt_ready[slot], ctx->stream));
+    GS_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_rt_ready[slot], 0));
+    if ((rc = copy_to_image(ctx, rt, rt_pitch, fi.d_rt, fi.pitch, W, H, ctx->copy_stream))) return rc;
+    GS_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_copy_done[slot], ctx->copy_stream));
+    ctx->copy_pending[slot] = true;
+    return GS_OK;   // completion and the bin-list check: gs_sync
+  }
+  if (rt && rt->memory == GS_MEM_HOST && (rc = copy_to_image(ctx, rt, rt_pitch, fi.d_rt, fi.pitch, W, H, ctx->stream))) return rc;
+  return tgt ? composite_impl(ctx, surfs, fi.d_rt, fi.pitch, fi.surf, rt_fmt, tgt, W, H, ctx->stream) : GS_OK;
 }
 
 }  // namespace gs
@@ -741,47 +692,14 @@ int gs_render(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRend
   if (fp->scene_depth && !as->zndc_valid) return fail(ctx, GS_ERR_NOT_READY, "a scene depth buffer needs the quad depths: run gs_calc_view with scene_depth set");
   for (int e = EV_BIN1; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
   rec(ctx, EV_VIEW1);
-  if (rt->memory == GS_MEM_DEVICE) return do_draw(ctx, fc, opt, as, fp, true, rt->data, pitch, rt->format);
-  if (is_array_image(rt)) {
-    CallSurfaces surfs(ctx);
-    Surface so;
-    if ((rc = surfs.make(rt, &so))) return rc;
-    return do_draw(ctx, fc, opt, as, fp, true, nullptr, 0, rt->format, so);
-  }
-  const uint32_t tight = W * pix_bytes(rt->format);
-  GS_CUDA_TRY(ctx, ctx->rt_scratch.reserve((size_t)tight * H, {ctx->stream}));
-  if ((rc = init_staging(ctx, opt, ctx->rt_scratch.get(), tight, W, H, rt->format, rt, pitch))) return rc;
-  if ((rc = do_draw(ctx, fc, opt, as, fp, true, ctx->rt_scratch.get(), tight, rt->format))) return rc;
-  GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, pitch, ctx->rt_scratch.get(), tight, tight, H, cudaMemcpyDeviceToHost, ctx->stream));
-  return check_bin_overflow(ctx);
-}
-
-// d_rt == nullptr: the render target is the CUDA array (layer) behind rt_surf.  Enqueued on `s`: the context's stream, or the group
-// path's transfer stream (surfs must then hand its surfaces over on `s` as well).
-static int composite_impl(GsContext *ctx, CallSurfaces &surfs, const void *d_rt, uint32_t rt_pitch, Surface rt_surf,
-                          uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H, cudaStream_t s) {
-  GsNvtxRange nvtx("GaussianSplat.Compose");
-  uint32_t tp = 0;
-  int rc = image_ok(ctx, tgt, W, H, &tp);
-  if (rc) return rc;
-  if (tgt->memory == GS_MEM_DEVICE) {
-    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, tgt->data, tp, Surface{}, tgt->format, W, H, s);
-  } else if (is_array_image(tgt)) {
-    Surface so;
-    if ((rc = surfs.make(tgt, &so))) return rc;
-    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, nullptr, 0, so, tgt->format, W, H, s);
-  } else {
-    const uint32_t tight = W * pix_bytes(tgt->format);
-    GS_CUDA_TRY(ctx, ctx->tgt_scratch.reserve((size_t)tight * H, {ctx->stream}));
-    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->tgt_scratch.get(), tight, tgt->data, tp, tight, H, cudaMemcpyHostToDevice, s));
-    launch_composite(d_rt, rt_pitch, rt_surf, rt_fmt, ctx->tgt_scratch.get(), tight, Surface{}, tgt->format, W, H, s);
-    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(tgt->data, tp, ctx->tgt_scratch.get(), tight, tight, H, cudaMemcpyDeviceToHost, s));
-  }
-  if (s == ctx->stream) rec(ctx, EV_COMP1);
-  ctx->launches += 1;
-  GS_CUDA_TRY(ctx, cudaGetLastError());
-  if (tgt->memory == GS_MEM_HOST) GS_CUDA_TRY(ctx, cudaStreamSynchronize(s));
-  return GS_OK;
+  opt.flags &= ~(uint32_t)GS_FLAG_ASYNC_READBACK;   // a host rt is read back before gs_render returns
+  CallSurfaces surfs(ctx);
+  FrameImage fi;
+  if ((rc = begin_frame_image(ctx, surfs, opt, rt, pitch, rt->format, nullptr, W, H, &fi))) return rc;
+  if ((rc = do_draw(ctx, fc, opt, as, fp, true, fi.d_rt, fi.pitch, rt->format, fi.surf)) ||
+      (rc = end_frame_image(ctx, surfs, rt, pitch, rt->format, nullptr, W, H, fi)))
+    return rc;
+  return rt->memory == GS_MEM_HOST ? check_bin_overflow(ctx) : GS_OK;
 }
 
 int gs_composite(GsContext *ctx, const GsImage *rt, GsImage *tgt) {
@@ -794,92 +712,19 @@ int gs_composite(GsContext *ctx, const GsImage *rt, GsImage *tgt) {
   ctx->ev_valid[EV_COMP1] = false;
   rec(ctx, EV_RASTER1);
   CallSurfaces surfs(ctx);
-  if (rt->memory == GS_MEM_DEVICE) return composite_impl(ctx, surfs, rt->data, rp, Surface{}, rt->format, tgt, W, H, ctx->stream);
-  if (is_array_image(rt)) {
-    Surface so;
-    if ((rc = surfs.make(rt, &so))) return rc;
-    return composite_impl(ctx, surfs, nullptr, 0, so, rt->format, tgt, W, H, ctx->stream);
-  }
-  const uint32_t tight = W * pix_bytes(rt->format);
-  GS_CUDA_TRY(ctx, ctx->rt_scratch.reserve((size_t)tight * H, {ctx->stream}));
-  GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->rt_scratch.get(), tight, rt->data, rp, tight, H, cudaMemcpyHostToDevice, ctx->stream));
-  return composite_impl(ctx, surfs, ctx->rt_scratch.get(), tight, Surface{}, rt->format, tgt, W, H, ctx->stream);
+  if (rt->memory == GS_MEM_HOST) GS_CUDA_TRY(ctx, ctx->rt_scratch.reserve((size_t)W * pix_bytes(rt->format) * H, {ctx->stream}));
+  DeviceImage r;
+  if ((rc = bind_image(ctx, surfs, rt, rp, rt->format, W, H, ctx->rt_scratch.get(), StagingFill::kUpload, ctx->stream, &r))) return rc;
+  return composite_impl(ctx, surfs, r.d_rt, r.pitch, r.surf, rt->format, tgt, W, H, ctx->stream);
 }
 
 }  // extern "C"
 
 namespace gs {
-// The device image a frame draws into: `rt` itself when it is device or array memory, else library scratch (or, with
-// GS_FLAG_ASYNC_READBACK, one of the two asynchronous staging images) that a host `rt` is read back from.
-struct FrameImage {
-  void *d_rt = nullptr;            // nullptr: the CUDA array (layer) behind `surf`
-  uint32_t pitch = 0;
-  Surface surf;
-  bool async_rb = false;
-  int slot = 0;
-};
-
-// what a frame does between its view-calcs and its draw; rt (when given) has passed image_ok.  staging (optional): where a
-// staging image goes instead of rt_scratch (one slice per camera of a run of several cameras)
-static int begin_frame_image(GsContext *ctx, CallSurfaces &surfs, const GsRenderOptions &opt, GsImage *rt, uint32_t rt_pitch,
-                             uint32_t rt_fmt, const GsImage *tgt, uint32_t W, uint32_t H, FrameImage *fi, void *staging = nullptr) {
-  int rc = GS_OK;
-  const bool rt_dev = rt && rt->memory == GS_MEM_DEVICE, rt_arr = rt && is_array_image(rt), rt_host = rt && rt->memory == GS_MEM_HOST;
-  fi->async_rb = rt_host && !tgt && (opt.flags & GS_FLAG_ASYNC_READBACK) != 0;
-  if (rt_dev) { fi->d_rt = rt->data; fi->pitch = rt_pitch; }
-  else if (rt_arr) {   // rendered into in place, through a surface
-    if ((rc = surfs.make(rt, &fi->surf))) return rc;
-  } else if (fi->async_rb) {
-    if ((rc = ensure_async_readback(ctx))) return rc;
-    const int slot = fi->slot = ctx->rt_flip;
-    ctx->rt_flip ^= 1;
-    fi->pitch = W * pix_bytes(rt_fmt);
-    // the staging image of two frames ago: its copy must have left the device before this frame's raster overwrites it
-    if (ctx->copy_pending[slot]) GS_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy_done[slot], 0));
-    GS_CUDA_TRY(ctx, ctx->rt_async[slot].reserve((size_t)fi->pitch * H, {ctx->stream, ctx->copy_stream}));
-    fi->d_rt = ctx->rt_async[slot].get();
-    if ((rc = init_staging(ctx, opt, fi->d_rt, fi->pitch, W, H, rt_fmt, rt, rt_pitch))) return rc;
-  } else {
-    fi->pitch = W * pix_bytes(rt_fmt);
-    if (!staging) GS_CUDA_TRY(ctx, ctx->rt_scratch.reserve((size_t)fi->pitch * H, {ctx->stream}));
-    fi->d_rt = staging ? staging : ctx->rt_scratch.get();
-    if ((rc = init_staging(ctx, opt, fi->d_rt, fi->pitch, W, H, rt_fmt, rt, rt_pitch))) return rc;
-  }
-  return GS_OK;
-}
-
-// what follows the draw: the read-back of a host `rt` (enqueued only, with GS_FLAG_ASYNC_READBACK), the composite onto the
-// camera target, and the bin-list check of a call that waits for the device anyway
-// (check_overflow false: the caller checks the bin list once, after its last draw)
-static int end_frame_image(GsContext *ctx, CallSurfaces &surfs, GsImage *rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W,
-                           uint32_t H, const FrameImage &fi, bool check_overflow = true) {
-  int rc = GS_OK;
-  const bool rt_host = rt && rt->memory == GS_MEM_HOST;
-  if (fi.async_rb) {
-    const int slot = fi.slot;
-    GS_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_rt_ready[slot], ctx->stream));
-    GS_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_rt_ready[slot], 0));
-    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, rt_pitch, fi.d_rt, fi.pitch, (size_t)W * pix_bytes(rt_fmt), H, cudaMemcpyDeviceToHost, ctx->copy_stream));
-    GS_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_copy_done[slot], ctx->copy_stream));
-    ctx->copy_pending[slot] = true;
-    return GS_OK;   // completion and the bin-list check: gs_sync
-  }
-  if (rt_host) {
-    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, rt_pitch, fi.d_rt, fi.pitch, (size_t)W * pix_bytes(rt_fmt), H, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  bool synced = false;
-  if (tgt) {
-    if ((rc = composite_impl(ctx, surfs, fi.d_rt, fi.pitch, fi.surf, rt_fmt, tgt, W, H, ctx->stream))) return rc;
-    synced = tgt->memory == GS_MEM_HOST;
-  }
-  if (check_overflow && (rt_host || synced)) return check_bin_overflow(ctx);
-  return GS_OK;
-}
-
 // One camera of gs_frame_objects / gs_frame_cameras: its objects' arguments assets / fps / do_sort_flags [off, off + K), and
 // its images.
 struct CameraArgs {
-  uint32_t off, K, W, H, rt_pitch, rt_fmt;
+  uint32_t off, K, W, H, rt_pitch = 0, rt_fmt = GS_PIX_RGBA16F;
   std::vector<FrameConsts> fcs;
   GsImage *rt, *tgt;
   FrameImage fi;     // set up by the camera's first run
@@ -911,7 +756,6 @@ static int check_camera(GsContext *ctx, GsAsset *const *assets, const GsFramePar
   if ((rc = check_options(ctx, a->fcs[0], *opt))) return rc;
   a->W = (uint32_t)fps[0].screen_w; a->H = (uint32_t)fps[0].screen_h;
   uint32_t tgt_pitch = 0;
-  a->rt_pitch = 0; a->rt_fmt = GS_PIX_RGBA16F;
   if (a->rt) { if ((rc = image_ok(ctx, a->rt, a->W, a->H, &a->rt_pitch))) return rc; a->rt_fmt = a->rt->format; }
   if (a->tgt && (rc = image_ok(ctx, a->tgt, a->W, a->H, &tgt_pitch))) return rc;
   return GS_OK;
@@ -942,18 +786,6 @@ static uint32_t run_end(GsAsset *const *assets, const GsFrameParams *fps, uint32
     else if (f.scene_depth != depth->scene_depth || f.scene_depth_on_device != depth->scene_depth_on_device) break;
   }
   return e;
-}
-
-// What makes two images of a call one image: the same pointer, or the same array and layer (GS_MEM_ARRAY_LAYER; the layers of
-// one array are separate images).
-static std::pair<const void *, int32_t> image_id(const GsImage *im) {
-  if (!im) return {nullptr, -1};
-  if (im->memory == GS_MEM_ARRAY_LAYER) {
-    int32_t layer = -1;
-    const cudaArray_t arr = image_array(im, &layer);
-    return {arr, layer};
-  }
-  return {im->data, -1};
 }
 
 // The call's cameras as runs, in order.  Consecutive whole cameras share a run while each fits it, the run's totals hold, they
@@ -1143,7 +975,7 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
   }
   for (const Segment &sg : run) {
     CameraArgs &c = cams[sg.cam];
-    if (sg.k0 + sg.K == c.K && (rc = end_frame_image(ctx, surfs, c.rt, c.rt_pitch, c.rt_fmt, c.tgt, c.W, c.H, c.fi, false))) return rc;
+    if (sg.k0 + sg.K == c.K && (rc = end_frame_image(ctx, surfs, c.rt, c.rt_pitch, c.rt_fmt, c.tgt, c.W, c.H, c.fi))) return rc;
   }
   return GS_OK;
 }
@@ -1188,25 +1020,19 @@ int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRende
   int rc = check_params(ctx, as, fp);
   if (rc) return rc;
   if (!rt && !tgt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_frame needs rt and/or camera_target");
-  const uint32_t W = (uint32_t)fp->screen_w;
   GsRenderOptions opt = opt_in ? *opt_in : default_opts();
-  uint32_t rt_pitch = 0, rt_fmt = GS_PIX_RGBA16F;
-  FrameConsts fc = make_frame_consts(fp);
-  if ((rc = check_options(ctx, fc, opt))) return rc;
-  const uint32_t H = opt.band_packed ? partition_own_bin_rows(opt, fc.binsY) * kBin : (uint32_t)fp->screen_h;
+  std::vector<CameraArgs> cams(1);
+  CameraArgs &a = cams[0];
+  a.off = 0; a.K = 1; a.rt = rt; a.tgt = tgt;
+  a.fcs.assign(1, make_frame_consts(fp));
+  if ((rc = check_options(ctx, a.fcs[0], opt))) return rc;
+  a.W = (uint32_t)fp->screen_w;
+  a.H = opt.band_packed ? partition_own_bin_rows(opt, a.fcs[0].binsY) * kBin : (uint32_t)fp->screen_h;
   if (opt.band_packed && tgt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "band_packed output cannot be composited before the gather");
   if (opt.band_packed && rt && is_array_image(rt))
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "band_packed output is the send buffer of an all-gather: it must be linear memory, not a CUDA array");
-  if (rt) { if ((rc = image_ok(ctx, rt, W, H, &rt_pitch))) return rc; rt_fmt = rt->format; }
-  for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
-  if (do_sort_flag && (rc = do_sort(ctx, as, fc))) return rc;
-  // fused frame: colour of never-drawn splats is dead code; after the sort, the view-calc runs beside its last pass
-  if ((rc = do_view(ctx, as, fp, fc, true, opt, ctx->stream, nullptr, nullptr, do_sort_flag != 0))) return rc;
-  CallSurfaces surfs(ctx);
-  FrameImage fi;
-  if ((rc = begin_frame_image(ctx, surfs, opt, rt, rt_pitch, rt_fmt, tgt, W, H, &fi))) return rc;
-  if ((rc = do_draw(ctx, fc, opt, as, fp, true, fi.d_rt, fi.pitch, rt_fmt, fi.surf))) return rc;
-  return end_frame_image(ctx, surfs, rt, rt_pitch, rt_fmt, tgt, W, H, fi);
+  if (rt) { if ((rc = image_ok(ctx, rt, a.W, a.H, &a.rt_pitch))) return rc; a.rt_fmt = rt->format; }
+  return draw_cameras(ctx, cams, &as, fp, &do_sort_flag, opt);
 }
 
 int gs_frame_objects(GsContext *ctx, uint32_t object_count, GsAsset *const *assets, const GsFrameParams *fps, const int32_t *do_sort_flags,
@@ -1253,18 +1079,16 @@ int gs_unshuffle_bands(GsContext *ctx, const void *gathered, uint32_t parts, uin
   if (rc) return rc;
   if (out->format != fmt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gathered and output pixel formats differ");
   const uint32_t W = out->width, H = out->height;
-  if (out->memory == GS_MEM_DEVICE) {
-    launch_unshuffle(gathered, parts, band_rows, rows_pp, fmt, out->data, pitch, W, H, ctx->stream);
-    ctx->launches += 1;
-    GS_CUDA_TRY(ctx, cudaGetLastError());
-    return GS_OK;
-  }
-  const uint32_t tight = W * pix_bytes(fmt);
-  GS_CUDA_TRY(ctx, ctx->rt_scratch.reserve((size_t)tight * H, {ctx->stream}));
-  launch_unshuffle(gathered, parts, band_rows, rows_pp, fmt, ctx->rt_scratch.get(), tight, W, H, ctx->stream);
+  const bool host = out->memory == GS_MEM_HOST;
+  if (host) GS_CUDA_TRY(ctx, ctx->rt_scratch.reserve((size_t)W * pix_bytes(fmt) * H, {ctx->stream}));
+  CallSurfaces surfs(ctx);
+  DeviceImage o;
+  if ((rc = bind_image(ctx, surfs, out, pitch, fmt, W, H, ctx->rt_scratch.get(), StagingFill::kNone, ctx->stream, &o))) return rc;
+  launch_unshuffle(gathered, parts, band_rows, rows_pp, fmt, o.d_rt, o.pitch, W, H, ctx->stream);
   ctx->launches += 1;
-  GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(out->data, pitch, ctx->rt_scratch.get(), tight, tight, H, cudaMemcpyDeviceToHost, ctx->stream));
-  GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  GS_CUDA_TRY(ctx, cudaGetLastError());
+  if (host && (rc = copy_to_image(ctx, out, pitch, o.d_rt, o.pitch, W, H, ctx->stream))) return rc;
+  if (host) GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return GS_OK;
 }
 
@@ -1396,11 +1220,3 @@ void *gs_asset_device_ptr(GsAsset *as, int which) {
 }
 
 }  // extern "C"
-
-namespace gs {
-int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H,
-                        cudaStream_t s) {
-  CallSurfaces surfs(ctx, s);
-  return composite_impl(ctx, surfs, d_rt, rt_pitch, Surface{}, rt_fmt, tgt, W, H, s);
-}
-}  // namespace gs

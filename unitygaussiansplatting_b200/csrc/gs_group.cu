@@ -572,17 +572,16 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
   if (base.blend_mode > GS_BLEND_FP32) return fail(g->m[0].ctx, GS_ERR_INVALID_ARGUMENT, "bad blend mode");
   uint32_t fmt = GS_PIX_RGBA16F;
   for (size_t i = 0; i < L; ++i) if (rts && rts[i]) { fmt = rts[i]->format; break; }
-  std::vector<uint32_t> pitches(L);
+  std::vector<uint32_t> pitches(L), rt_pitches(L, 0);   // of the image drawn into, and of rt itself
   std::vector<void *> dev_rt(L, nullptr);   // a device rt is composited into in place; other members use library scratch
   for (size_t i = 0; i < L; ++i) {
     GsContext *ctx = g->m[i].ctx;
     GsImage *rt = rts ? rts[i] : nullptr;
     pitches[i] = W * pix_bytes(fmt);
     if (rt) {
-      uint32_t p = 0;
-      if ((rc = image_ok(ctx, rt, W, H, &p))) return rc;
+      if ((rc = image_ok(ctx, rt, W, H, &rt_pitches[i]))) return rc;
       if (rt->format != fmt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "members' images differ in pixel format");
-      if (rt->memory == GS_MEM_DEVICE) { dev_rt[i] = rt->data; pitches[i] = p; }
+      if (rt->memory == GS_MEM_DEVICE) { dev_rt[i] = rt->data; pitches[i] = rt_pitches[i]; }
     }
     if (G > 1 && pitches[i] != pitches[0]) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "members' images differ in row pitch");
     GsImage *ct = cams ? cams[i] : nullptr;
@@ -879,24 +878,10 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
     GS_CUDA_TRY(ctx, cudaMemcpyAsync(mb.buf.h_row_cost[slot].get(), mb.buf.row_cost.get(), (size_t)rows * 4, cudaMemcpyDeviceToHost, mb.xfer));
     GS_CUDA_TRY(ctx, cudaEventRecord(mb.ev_cost[slot], mb.xfer));
     GsImage *rt = rts ? rts[i] : nullptr;
-    if (rt && rt->memory == GS_MEM_HOST) {
-      const uint32_t hp = rt->row_pitch_bytes ? rt->row_pitch_bytes : W * pix_bytes(fmt);
-      GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(rt->data, hp, img[i], pitches[i], (size_t)W * pix_bytes(fmt), H, cudaMemcpyDeviceToHost, mb.xfer));
-      host_out = true;
-    } else if (rt && rt->memory == GS_MEM_ARRAY) {   // e.g. the display GPU's imported render texture: one copy of the assembled frame
-      GS_CUDA_TRY(ctx, cudaMemcpy2DToArrayAsync(static_cast<cudaArray_t>(rt->data), 0, 0, img[i], pitches[i], (size_t)W * pix_bytes(fmt), H,
-                                                cudaMemcpyDeviceToDevice, mb.xfer));
-    } else if (rt && rt->memory == GS_MEM_ARRAY_LAYER) {   // e.g. one eye of an XR eye-texture array: the same copy, into its layer
-      int32_t layer = -1;
-      cudaMemcpy3DParms cp;
-      memset(&cp, 0, sizeof(cp));
-      cp.srcPtr = make_cudaPitchedPtr(img[i], pitches[i], W, H);
-      cp.dstArray = image_array(rt, &layer);
-      cp.dstPos = make_cudaPos(0, 0, (size_t)layer);
-      cp.extent = make_cudaExtent(W, H, 1);   // in texels: the destination is an array
-      cp.kind = cudaMemcpyDeviceToDevice;
-      GS_CUDA_TRY(ctx, cudaMemcpy3DAsync(&cp, mb.xfer));
-    }
+    // a host or CUDA-array rt (e.g. the display GPU's imported render texture, or one eye of an XR eye-texture array) gets one
+    // copy of the assembled frame
+    if (rt && !dev_rt[i] && (rc = copy_to_image(ctx, rt, rt_pitches[i], img[i], pitches[i], W, H, mb.xfer))) return rc;
+    host_out |= rt && rt->memory == GS_MEM_HOST;
     // the composite pass onto this member's camera target, from the assembled image, still on the transfer stream (a host
     // camera target is uploaded, blended and read back before the call returns, as gs_composite does)
     GsImage *ct = cams ? cams[i] : nullptr;

@@ -1,0 +1,124 @@
+// gs_image.cu -- how the library reaches the pixels of a GsImage in each memory kind: validation, the device view a kernel
+// draws into (the image itself, a surface of its CUDA array, or a staging image), and the copy of a linear device image into
+// an image of any kind.
+#include <cstring>
+#include <string>
+
+#include "gs_internal.cuh"
+
+namespace gs {
+
+uint32_t pix_bytes(uint32_t fmt) { return fmt == GS_PIX_RGBA16F ? 8u : 16u; }
+
+int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch) {
+  if (!im || !im->data) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image is null");
+  if (im->format > GS_PIX_RGBA32F) return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "unsupported pixel format");
+  if (im->memory > GS_MEM_ARRAY_LAYER || im->memory == 3)   // 3 is not a memory kind
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, "unknown image memory kind");
+  if (im->width != W || im->height != H) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image size does not match screen size");
+  if (is_array_image(im)) {   // a 2-D CUDA array (data is a cudaArray_t), or a layer of a layered one (data is a GsArrayLayer *)
+    if (im->row_pitch_bytes) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "row_pitch_bytes must be 0 for a CUDA array image");
+    const bool layered = im->memory == GS_MEM_ARRAY_LAYER;
+    if (layered) {
+      const GsArrayLayer *d = static_cast<const GsArrayLayer *>(im->data);
+      if (!d->array || d->reserved) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "GsArrayLayer: array is null or reserved is not 0");
+    }
+    int32_t layer = -1;
+    cudaChannelFormatDesc cd;
+    cudaExtent ext;
+    unsigned int flags = 0;
+    const cudaError_t e = cudaArrayGetInfo(&cd, &ext, &flags, image_array(im, &layer));
+    if (e != cudaSuccess) { cudaGetLastError(); return fail(ctx, GS_ERR_INVALID_ARGUMENT, std::string("not a CUDA array: ") + cudaGetErrorString(e)); }
+    const int bits = im->format == GS_PIX_RGBA16F ? 16 : 32;
+    if (cd.f != cudaChannelFormatKindFloat || cd.x != bits || cd.y != bits || cd.z != bits || cd.w != bits)
+      return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "the CUDA array's channel format does not match the image's pixel format");
+    if (!layered && (ext.width != W || ext.height != H || ext.depth != 0))
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array is not a 2-D array of the image's size");
+    if (layered && (ext.width != W || ext.height != H || !(flags & cudaArrayLayered)))
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array is not a layered array of the image's size");
+    if (layered && (uint32_t)layer >= ext.depth)
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the layer is not below the CUDA array's layer count");
+    if (!(flags & cudaArraySurfaceLoadStore))
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array was not created with cudaArraySurfaceLoadStore");
+    *pitch = 0;
+    return GS_OK;
+  }
+  uint32_t p = im->row_pitch_bytes ? im->row_pitch_bytes : W * pix_bytes(im->format);
+  if (p < W * pix_bytes(im->format) || (p % pix_bytes(im->format)) != 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "bad row pitch");
+  *pitch = p;
+  return GS_OK;
+}
+
+std::pair<const void *, int32_t> image_id(const GsImage *im) {
+  if (!im) return {nullptr, -1};
+  if (im->memory == GS_MEM_ARRAY_LAYER) {
+    int32_t layer = -1;
+    const cudaArray_t arr = image_array(im, &layer);
+    return {arr, layer};
+  }
+  return {im->data, -1};
+}
+
+// Destroys the held surface objects whose last use has completed; with `all`, every one, after waiting for its event.  The
+// event, not the context stream, is what guards a batch: the group path composites onto CUDA-array camera targets on a
+// member's transfer stream, which the context stream never waits for.
+void release_surfaces(GsContext *ctx, bool all) {
+  auto &held = ctx->held_surfaces;
+  size_t keep = 0;
+  for (size_t i = 0; i < held.size(); ++i) {
+    bool done = all;
+    if (all) {
+      if (cudaEventSynchronize(held[i].done) != cudaSuccess) cudaGetLastError();   // failed: nothing will use the surfaces any more
+    } else {
+      const cudaError_t q = cudaEventQuery(held[i].done);
+      done = q != cudaErrorNotReady;   // completed, or failed: either way nothing will use the surfaces any more
+      if (!done && cudaPeekAtLastError() == cudaErrorNotReady) cudaGetLastError();
+    }
+    if (done) {
+      for (cudaSurfaceObject_t so : held[i].surfs) cudaDestroySurfaceObject(so);
+      ctx->spare_events.push_back(held[i].done);
+    } else {
+      if (keep != i) held[keep] = std::move(held[i]);
+      ++keep;
+    }
+  }
+  held.resize(keep);
+}
+
+int bind_image(GsContext *ctx, CallSurfaces &surfs, const GsImage *im, uint32_t pitch, uint32_t fmt, uint32_t W, uint32_t H, void *staging,
+               StagingFill fill, cudaStream_t s, DeviceImage *out) {
+  *out = DeviceImage{};
+  if (im && im->memory == GS_MEM_DEVICE) { out->d_rt = im->data; out->pitch = pitch; return GS_OK; }
+  if (im && is_array_image(im)) return surfs.make(im, &out->surf);
+  out->d_rt = staging;
+  out->pitch = W * pix_bytes(fmt);
+  if (fill == StagingFill::kUpload)
+    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(staging, out->pitch, im->data, pitch, out->pitch, H, cudaMemcpyHostToDevice, s));
+  else if (fill == StagingFill::kZero)
+    GS_CUDA_TRY(ctx, cudaMemsetAsync(staging, 0, (size_t)out->pitch * H, s));
+  return GS_OK;
+}
+
+int copy_to_image(GsContext *ctx, const GsImage *im, uint32_t pitch, const void *src, uint32_t src_pitch, uint32_t W, uint32_t H,
+                  cudaStream_t s) {
+  const size_t row = (size_t)W * pix_bytes(im->format);
+  if (im->memory == GS_MEM_ARRAY) {
+    GS_CUDA_TRY(ctx, cudaMemcpy2DToArrayAsync(static_cast<cudaArray_t>(im->data), 0, 0, src, src_pitch, row, H, cudaMemcpyDeviceToDevice, s));
+  } else if (im->memory == GS_MEM_ARRAY_LAYER) {
+    int32_t layer = -1;
+    cudaMemcpy3DParms cp;
+    memset(&cp, 0, sizeof(cp));
+    cp.srcPtr = make_cudaPitchedPtr(const_cast<void *>(src), src_pitch, W, H);
+    cp.dstArray = image_array(im, &layer);
+    cp.dstPos = make_cudaPos(0, 0, (size_t)layer);
+    cp.extent = make_cudaExtent(W, H, 1);   // in texels: the destination is an array
+    cp.kind = cudaMemcpyDeviceToDevice;
+    GS_CUDA_TRY(ctx, cudaMemcpy3DAsync(&cp, s));
+  } else {
+    const cudaMemcpyKind kind = im->memory == GS_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+    GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(im->data, pitch, src, src_pitch, row, H, kind, s));
+  }
+  return GS_OK;
+}
+
+}  // namespace gs

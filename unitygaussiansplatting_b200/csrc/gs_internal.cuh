@@ -2,6 +2,7 @@
 // the context / asset objects and the per-stage drivers.
 #pragma once
 #include <algorithm>
+#include <cstring>
 #include <string>
 #include <vector>
 
@@ -136,7 +137,10 @@ int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, G
 // validated as W x H), enqueued on `s`.  A host target is uploaded and read back, and the call waits for `s`.
 int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H,
                         cudaStream_t s);
+
+// ---- images (gs_image.cu) -------------------------------------------------------------------------------------------------
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch);
+uint32_t pix_bytes(uint32_t fmt);
 inline bool is_array_image(const GsImage *im) { return im->memory == GS_MEM_ARRAY || im->memory == GS_MEM_ARRAY_LAYER; }
 // The CUDA array of a GS_MEM_ARRAY / GS_MEM_ARRAY_LAYER image, and in *layer the layer it names (-1: a 2-D array)
 inline cudaArray_t image_array(const GsImage *im, int32_t *layer) {
@@ -148,7 +152,74 @@ inline cudaArray_t image_array(const GsImage *im, int32_t *layer) {
   *layer = -1;
   return static_cast<cudaArray_t>(im->data);
 }
-uint32_t pix_bytes(uint32_t fmt);
+// What makes two images of a call one image: the same pointer, or the same array and layer (GS_MEM_ARRAY_LAYER; the layers of
+// one array are separate images).
+std::pair<const void *, int32_t> image_id(const GsImage *im);
+void release_surfaces(GsContext *ctx, bool all);
+
+// The surface objects one call creates for its CUDA-array images, one per array: the layers of one layered array share it.
+// When the call returns they are handed to the context behind an event recorded on the stream that used them (the context's,
+// unless another is named) after their last use.  They are never cached by cudaArray_t value beyond the call: a freed array's
+// handle can be reused by the next allocation.
+class CallSurfaces {
+ public:
+  explicit CallSurfaces(GsContext *ctx, cudaStream_t stream = nullptr) : ctx_(ctx), stream_(stream ? stream : ctx->stream) {}
+  CallSurfaces(const CallSurfaces &) = delete;
+  CallSurfaces &operator=(const CallSurfaces &) = delete;
+  ~CallSurfaces() {
+    if (made_.empty()) return;
+    cudaEvent_t ev = nullptr;
+    if (!ctx_->spare_events.empty()) { ev = ctx_->spare_events.back(); ctx_->spare_events.pop_back(); }
+    else if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) ev = nullptr;
+    if (ev && cudaEventRecord(ev, stream_) == cudaSuccess) {
+      ctx_->held_surfaces.push_back({ev, std::move(made_)});
+      return;
+    }
+    cudaStreamSynchronize(stream_);   // no event to wait for: wait for the stream itself
+    for (cudaSurfaceObject_t so : made_) cudaDestroySurfaceObject(so);
+    if (ev) ctx_->spare_events.push_back(ev);
+  }
+  // `im` has passed image_ok as a GS_MEM_ARRAY or GS_MEM_ARRAY_LAYER image
+  int make(const GsImage *im, Surface *out) {
+    const cudaArray_t arr = image_array(im, &out->layer);
+    for (size_t i = 0; i < arrays_.size(); ++i)
+      if (arrays_[i] == arr) { out->obj = made_[i]; return GS_OK; }
+    if (made_.empty()) release_surfaces(ctx_, false);
+    cudaResourceDesc rd;
+    memset(&rd, 0, sizeof(rd));
+    rd.resType = cudaResourceTypeArray;
+    rd.res.array.array = arr;
+    GS_CUDA_TRY(ctx_, cudaCreateSurfaceObject(&out->obj, &rd));
+    made_.push_back(out->obj);
+    arrays_.push_back(arr);
+    return GS_OK;
+  }
+
+ private:
+  GsContext *ctx_;
+  cudaStream_t stream_;
+  std::vector<cudaSurfaceObject_t> made_;
+  std::vector<cudaArray_t> arrays_;   // made_[i] is the surface of arrays_[i]
+};
+
+// The device view of an image a kernel reads and writes: linear memory at d_rt / pitch, or (d_rt == nullptr) the CUDA array
+// (layer) behind `surf`.
+struct DeviceImage {
+  void *d_rt = nullptr;
+  uint32_t pitch = 0;
+  Surface surf;
+};
+// What a staging image holds before the kernel runs: the host image's pixels, zeros, or whatever it held.
+enum class StagingFill { kUpload, kZero, kNone };
+// The device view of `im` (passed image_ok with `pitch`), on `s`: device memory is the image itself, a CUDA array (layer) a
+// surface made through `surfs`.  A host image, or none (im == nullptr, whose fill must not be kUpload), is the tight W x H
+// image of pixel format `fmt` at `staging`, which the caller has grown, filled as `fill` says.
+int bind_image(GsContext *ctx, CallSurfaces &surfs, const GsImage *im, uint32_t pitch, uint32_t fmt, uint32_t W, uint32_t H, void *staging,
+               StagingFill fill, cudaStream_t s, DeviceImage *out);
+// Copies W x H pixels of linear device memory (src / src_pitch) into `im` (passed image_ok with `pitch`), of any memory kind,
+// on `s`.
+int copy_to_image(GsContext *ctx, const GsImage *im, uint32_t pitch, const void *src, uint32_t src_pitch, uint32_t W, uint32_t H,
+                  cudaStream_t s);
 // The per-asset work buffers (order, keys, view data, ...) of an asset whose blobs as->d_* are already in HBM, the format
 // fields of as->av, and CSSetIndices: what gs_asset_upload and gs_pack_asset share.
 cudaError_t asset_init_work(GsContext *ctx, GsAsset *as, uint32_t n, uint32_t pos_fmt, uint32_t scale_fmt, uint32_t sh_fmt,
