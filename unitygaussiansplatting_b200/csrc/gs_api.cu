@@ -110,50 +110,6 @@ int ensure_sort_scratch(GsContext *ctx, uint32_t capacity) {
   return GS_OK;
 }
 
-// The bin list holds clamp(8 x splats, 4 Mi, kBinListMax) entries, a rule set for screens of at most kRuleBins bins per axis
-// (8160 px).  A splat's footprint in bins grows with the square of the screen size, so larger frames check their list after
-// binning and grow it (grow_bin_list).
-constexpr uint32_t kBinListMax = 768u << 20;
-constexpr uint32_t kRuleBins = 128;
-
-static int ensure_bin_scratch(GsContext *ctx, uint32_t n, uint32_t tiles, uint32_t min_capacity) {
-  uint64_t want = (uint64_t)n * 8;
-  if (want < (4u << 20)) want = 4u << 20;
-  if (want > kBinListMax) want = kBinListMax;
-  if (want < min_capacity) want = min_capacity;
-  GS_CUDA_TRY(ctx, ctx->bin_keys.reserve(want, {ctx->stream}));
-  GS_CUDA_TRY(ctx, ctx->bin_vals.reserve(want, {ctx->stream}));
-  const uint32_t capacity = bin_scratch(ctx).capacity;
-  int rc = ensure_sort_scratch(ctx, capacity > n ? capacity : n);
-  if (rc) return rc;
-  const uint32_t blocks = n / 1024 + 2 < 1024u ? 1024u : n / 1024 + 2;   // the binner's ticket + range totals (<= 593 words) fit too
-  GS_CUDA_TRY(ctx, ctx->bin_block_sums.reserve(blocks, {ctx->stream}));
-  GS_CUDA_TRY(ctx, ctx->bin_ranges.reserve(tiles, {ctx->stream}));
-  return GS_OK;
-}
-
-// Screens of more than kRuleBins bins on either axis only: the host waits for the binning just enqueued and reads
-// entry_count back.  A list that overflowed grows to its total plus a quarter (at most kBinListMax) and *again asks the
-// caller to bin once more from the same rectangles (the view-calc output still holds them).  The capacity stays, and the
-// headroom lets the next frames of a moving camera, whose counts drift, bin once instead of growing the list again and again.
-// A total above kBinListMax is left truncated and reported like any overflow, at gs_sync or at the host read-back.
-static int grow_bin_list(GsContext *ctx, const FrameConsts &fc, uint32_t n, bool *again) {
-  *again = false;
-  if (fc.binsX <= kRuleBins && fc.binsY <= kRuleBins) return GS_OK;
-  const uint32_t tiles = fc.binsX * fc.binsY;
-  uint32_t ec[3] = {0, 0, 0};   // clamped count, overflow flag, total (of this run, for gs_frame_objects)
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ec, ctx->bin_entry_count.get(), sizeof(ec), cudaMemcpyDeviceToHost, ctx->stream));
-  GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  if (ec[2] <= bin_scratch(ctx).capacity || ec[2] > kBinListMax) {
-    ctx->bin_overflow = ec[1] != 0;
-    return GS_OK;
-  }
-  const int rc = ensure_bin_scratch(ctx, n, tiles, (uint32_t)std::min<uint64_t>((uint64_t)ec[2] + ec[2] / 4, kBinListMax));
-  if (rc) return rc;
-  *again = true;
-  return GS_OK;
-}
-
 void rec(GsContext *ctx, int e) {
   if (ctx->timing) { cudaEventRecord(ctx->ev[e], ctx->stream); ctx->ev_valid[e] = true; }
 }
@@ -320,12 +276,12 @@ static int tile_history(GsContext *ctx, uint32_t tiles, const std::vector<uint32
   return GS_OK;
 }
 
-int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *as, const GsFrameParams *fp, bool first,
-            void *d_rt, uint32_t pitch, uint32_t fmt, Surface surf, cudaEvent_t bin_done) {
+int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *as, const GsFrameParams *fp, void *d_rt,
+            uint32_t pitch, uint32_t fmt, Surface surf, cudaEvent_t bin_done) {
   GsNvtxRange nvtx("GaussianSplat.Draw");
-  const uint32_t n = as->av.n;
-  int rc = ensure_bin_scratch(ctx, n, fc.binsX * fc.binsY, 0);
-  if (rc) return rc;
+  const uint32_t n = as->av.n, bins = fc.binsX * fc.binsY;
+  int rc = GS_OK;
+  if ((rc = ctx->bins.begin_draw(ctx, 1, fc)) || (rc = ctx->bins.reserve(ctx, n, bins))) return rc;
   uint32_t *tile_cost = nullptr;
   const uint32_t rtiles = (((uint32_t)fc.screenW + kTile - 1) / kTile) * fc.binsY * (kBin / kTile);   // of the whole image
   if ((rc = tile_history(ctx, rtiles, nullptr, &tile_cost))) return rc;
@@ -333,17 +289,14 @@ int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, G
   if ((rc = bind_depth(ctx, fp, &depth))) return rc;
   BinScratch lists;
   int bin_launches = 0, more = 0;
-  GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order.get(), as->rect.get(), as->block_bits.get(), n, first, bin_scratch(ctx), sort_scratch(ctx),
-                                  ctx->stream, &lists, &bin_launches));
-  bool again = false;
-  if ((rc = grow_bin_list(ctx, fc, n, &again))) return rc;
+  GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order.get(), as->rect.get(), as->block_bits.get(), n, ctx->bins.clears(), bin_scratch(ctx),
+                                  sort_scratch(ctx), ctx->stream, &lists, &bin_launches));
+  bool again = false, clear = false;
+  if ((rc = ctx->bins.end_draw(ctx, n, bins, &again, &clear))) return rc;
   if (again) {
-    // the grown list fits: the flag this draw set is cleared again, unless an earlier draw of the call left its list truncated
-    const bool clear = first || !ctx->bin_overflow;
     GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order.get(), as->rect.get(), as->block_bits.get(), n, clear, bin_scratch(ctx), sort_scratch(ctx),
                                     ctx->stream, &lists, &more));
     bin_launches += more;
-    ctx->bin_overflow = !clear;
   }
   rec(ctx, EV_BIN1);
   if (bin_done) cudaEventRecord(bin_done, ctx->stream);
@@ -388,15 +341,6 @@ cudaError_t asset_init_work(GsContext *ctx, GsAsset *as, uint32_t n, uint32_t po
   ctx->launches += 1;
   // `n` is a stack value: the copy above must have left it before this returns
   return cudaStreamSynchronize(s);
-}
-
-static int check_bin_overflow(GsContext *ctx) {
-  uint32_t ec[2] = {0, 0};
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ec, ctx->bin_entry_count.get(), 8, cudaMemcpyDeviceToHost, ctx->stream));
-  GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  ctx->times.tile_entries = ec[0];
-  if (ec[1]) return fail(ctx, GS_ERR_OUT_OF_MEMORY, "tile-list capacity exceeded (splat footprints cover too many tiles)");
-  return GS_OK;
 }
 
 // d_rt == nullptr: the render target is the CUDA array (layer) behind rt_surf.  Enqueued on `s`: the context's stream, or the group
@@ -514,8 +458,8 @@ int gs_create(int cuda_device, void *stream_handle, GsContext **out) {
     GS_CUDA_TRY(ctx, ctx->sort_ghist.reserve(4 * 256, {ctx->stream}));
     GS_CUDA_TRY(ctx, ctx->sort_tickets.reserve(4, {ctx->stream}));
     GS_CUDA_TRY(ctx, ctx->d_scalar.reserve(16, {ctx->stream}));
-    GS_CUDA_TRY(ctx, ctx->bin_entry_count.reserve(4, {ctx->stream}));
-    GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->bin_entry_count.get(), 0, 16, ctx->stream));
+    GS_CUDA_TRY(ctx, ctx->bins.entry_count.reserve(4, {ctx->stream}));
+    GS_CUDA_TRY(ctx, cudaMemsetAsync(ctx->bins.entry_count.get(), 0, 16, ctx->stream));
     return GS_OK;
   };
   const int rc = init();
@@ -548,7 +492,7 @@ int gs_sync(GsContext *ctx) {
   if (!ctx) return fail(nullptr, GS_ERR_INVALID_ARGUMENT, "null context");
   GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   // frames rendered into device images are not checked when they are enqueued: surface a truncated bin list here
-  const int rc = check_bin_overflow(ctx);
+  const int rc = ctx->bins.check(ctx);
   if (ctx->copy_stream) {   // asynchronous read-backs in flight complete here
     GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->copy_stream));
     ctx->copy_pending[0] = ctx->copy_pending[1] = false;
@@ -579,7 +523,7 @@ int gs_get_stage_times(GsContext *ctx, GsStageTimes *out) {
   for (int e = EV_VIEW1; e < EV_COUNT; ++e) if (ctx->ev_valid[e]) last = e;
   t.total_ms = ev_ms(ctx, first, last);
   uint32_t ec[2] = {0, 0};
-  if (ctx->bin_entry_count.get()) cudaMemcpy(ec, ctx->bin_entry_count.get(), 8, cudaMemcpyDeviceToHost);
+  ctx->bins.read(ctx, ec, 2);   // a failed read reports no entries
   t.tile_entries = ec[0];
   t.kernel_launches = ctx->launches;
   *out = t;
@@ -696,10 +640,11 @@ int gs_render(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRend
   CallSurfaces surfs(ctx);
   FrameImage fi;
   if ((rc = begin_frame_image(ctx, surfs, opt, rt, pitch, rt->format, nullptr, W, H, &fi))) return rc;
-  if ((rc = do_draw(ctx, fc, opt, as, fp, true, fi.d_rt, fi.pitch, rt->format, fi.surf)) ||
+  ctx->bins.begin_call();
+  if ((rc = do_draw(ctx, fc, opt, as, fp, fi.d_rt, fi.pitch, rt->format, fi.surf)) ||
       (rc = end_frame_image(ctx, surfs, rt, pitch, rt->format, nullptr, W, H, fi)))
     return rc;
-  return rt->memory == GS_MEM_HOST ? check_bin_overflow(ctx) : GS_OK;
+  return rt->memory == GS_MEM_HOST ? ctx->bins.check(ctx) : GS_OK;
 }
 
 int gs_composite(GsContext *ctx, const GsImage *rt, GsImage *tgt) {
@@ -835,13 +780,14 @@ static std::vector<Run> form_runs(const std::vector<CameraArgs> &cams, GsAsset *
 
 // Draws one run.  Pair by pair the sort and the view-calc; a pair's bin entries are emitted before a later pair of the run
 // sorts or view-calculates the same asset, and otherwise after the last view-calc.  A run of one pair is then drawn by
-// do_draw; a longer one by one bin sort and one MULTI raster over every camera's tiles.  A run whose only camera has more than
-// kRuleBins bins on either axis grows its bin list as do_draw does.  Each camera's image is set up by its first run (a camera of
-// a run of several stages a host image in the run's scratch, every other camera in rt_scratch) and read back / composited
-// after its last.  first: the first draw of its public call (do_draw).
+// do_draw; a longer one by one bin sort and one MULTI raster over every camera's tiles.  Each camera's image is set up by its
+// first run (a camera of a run of several stages a host image in the run's scratch, every other camera in rt_scratch) and read
+// back / composited after its last.
 static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs> &cams, const Run &run, GsAsset *const *assets,
-                    const GsFrameParams *fps, const int32_t *do_sort_flags, const GsRenderOptions &opt, bool first) {
+                    const GsFrameParams *fps, const int32_t *do_sort_flags, const GsRenderOptions &opt) {
   GsNvtxRange nvtx("GaussianSplat.DrawRun");
+  int rc = ctx->bins.begin_draw(ctx, (uint32_t)run.size(), cams[run[0].cam].fcs[0]);   // any wait: before the run's sorts
+  if (rc) return rc;
   std::vector<uint32_t> pair_at, seg_of;   // each pair's argument index and segment, in draw order
   for (uint32_t i = 0; i < run.size(); ++i)
     for (uint32_t k = run[i].k0; k < run[i].k0 + run[i].K; ++k) { pair_at.push_back(cams[run[i].cam].off + k); seg_of.push_back(i); }
@@ -882,14 +828,13 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
     if (multi && depth_fp[i] && !depth_fp[i]->scene_depth_on_device) { depth_at[i] = bytes; bytes += align256((size_t)c.W * c.H * 4); }
     if (cams_run && (!c.rt || c.rt->memory == GS_MEM_HOST)) { stage_at[i] = bytes; bytes += align256((size_t)c.W * pix_bytes(c.rt_fmt) * c.H); }
   }
-  int rc = GS_OK;
   GS_CUDA_TRY(ctx, ctx->cams_scratch.reserve(bytes, {ctx->stream}));
   uint8_t *scratch = ctx->cams_scratch.get();
   const uint32_t n = (uint32_t)std::min<uint64_t>(total, 0xFFFFFFFFu);
   uint32_t *tile_cost = nullptr;
   if (multi) {
     GS_CUDA_TRY(ctx, ctx->cams_ghist.reserve(4 * 256, {ctx->stream}));
-    if ((rc = ensure_bin_scratch(ctx, n, bins, 0))) return rc;
+    if ((rc = ctx->bins.reserve(ctx, n, bins))) return rc;
     if ((rc = tile_history(ctx, tiles, cams_run ? &layout : nullptr, &tile_cost))) return rc;
     for (uint32_t i = 0; i < run.size(); ++i) {
       if (depth_fp[i] && depth_fp[i]->scene_depth_on_device) dc.cam[i].depth = depth_fp[i]->scene_depth;
@@ -920,7 +865,7 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
     const GsFrameParams &f = fps[pair_at[p]];
     const CameraArgs &c = cams[run[seg_of[p]].cam];
     for (uint32_t q = emitted; q < p; ++q)
-      if (assets[pair_at[q]] == as) { emit_to(p, first); break; }
+      if (assets[pair_at[q]] == as) { emit_to(p, ctx->bins.clears()); break; }
     float4 *draw = nullptr;
     float *zndc = nullptr;
     if (slab_at[p]) {
@@ -948,23 +893,21 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
     const CameraArgs &c = cams[run[0].cam];
     GsRenderOptions o = opt;
     if (run[0].load) o.flags |= GS_FLAG_LOAD_RT;
-    if ((rc = do_draw(ctx, c.fcs[run[0].k0], o, assets[pair_at[0]], &fps[pair_at[0]], first, c.fi.d_rt, c.fi.pitch, c.rt_fmt, c.fi.surf)))
+    if ((rc = do_draw(ctx, c.fcs[run[0].k0], o, assets[pair_at[0]], &fps[pair_at[0]], c.fi.d_rt, c.fi.pitch, c.rt_fmt, c.fi.surf)))
       return rc;
   } else {
-    emit_to(count, first);
+    emit_to(count, ctx->bins.clears());
     BinScratch lists;
     int sort_launches = 0, more = 0;
     GS_CUDA_TRY(ctx, launch_bin_list_sort(bins, bin_scratch(ctx), sort_scratch(ctx), ctx->cams_ghist.get(), ctx->stream, &lists, &sort_launches));
-    bool again = false;
-    if (!cams_run && (rc = grow_bin_list(ctx, cams[run[0].cam].fcs[0], n, &again))) return rc;
-    if (again) {   // as in do_draw
-      const bool clear = first || !ctx->bin_overflow;
+    bool again = false, clear = false;
+    if ((rc = ctx->bins.end_draw(ctx, n, bins, &again, &clear))) return rc;
+    if (again) {
       launch_bin_list_begin(bin_scratch(ctx), ctx->cams_ghist.get(), ctx->stream);
       emitted = 0;
       emit_to(count, clear);
       GS_CUDA_TRY(ctx, launch_bin_list_sort(bins, bin_scratch(ctx), sort_scratch(ctx), ctx->cams_ghist.get(), ctx->stream, &lists, &more));
       sort_launches += more;
-      ctx->bin_overflow = !clear;
     }
     lists.tile_cost = tile_cost;
     rec(ctx, EV_BIN1);
@@ -991,25 +934,13 @@ static int draw_cameras(GsContext *ctx, std::vector<CameraArgs> &cams, GsAsset *
     if ((rc = reserve_frame_inputs(ctx, assets[p], &fps[p], {ctx->stream}))) return rc;
   for (int e = 0; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
   CallSurfaces surfs(ctx);
-  const std::vector<Run> runs = form_runs(cams, assets, fps);
-  bool flag_read = true;   // ctx->bin_overflow is current: the last draw read the list back
-  for (size_t r = 0; r < runs.size(); ++r) {
-    const FrameConsts &fc = cams[runs[r][0].cam].fcs[0];
-    const bool grows = runs[r].size() == 1 && (fc.binsX > kRuleBins || fc.binsY > kRuleBins);
-    if (grows && r > 0 && !flag_read) {
-      // a grown list clears the overflow flag unless an earlier draw of the call was truncated (do_draw): read it first
-      uint32_t flag = 0;
-      GS_CUDA_TRY(ctx, cudaMemcpyAsync(&flag, ctx->bin_entry_count.get() + 1, 4, cudaMemcpyDeviceToHost, ctx->stream));
-      GS_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-      ctx->bin_overflow = flag != 0;
-    }
-    flag_read = grows;
-    if ((rc = draw_run(ctx, surfs, cams, runs[r], assets, fps, do_sort_flags, opt, r == 0))) return rc;
-  }
+  ctx->bins.begin_call();
+  for (const Run &run : form_runs(cams, assets, fps))
+    if ((rc = draw_run(ctx, surfs, cams, run, assets, fps, do_sort_flags, opt))) return rc;
   bool host = false;
   for (const CameraArgs &c : cams)
     host |= (c.rt && c.rt->memory == GS_MEM_HOST && !c.fi.async_rb) || (c.tgt && c.tgt->memory == GS_MEM_HOST);
-  return host ? check_bin_overflow(ctx) : GS_OK;
+  return host ? ctx->bins.check(ctx) : GS_OK;
 }
 }  // namespace gs
 

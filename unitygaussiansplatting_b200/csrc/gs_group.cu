@@ -829,13 +829,14 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
       // the previous call's row exchange (transfer stream) may still be filling this image: composite only after it
       if (mb.image_pending) GS_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, mb.ev_image, 0));
       if (timing) cudaEventRecord(mb.tev[GT_VIEWWAIT], ctx->stream);
+      ctx->bins.begin_call();
       for (uint32_t k = 0; k < K; ++k) {
         GroupObject &o = obj[k];
         // object 0 starts from a cleared target, each later one blends under what the earlier ones left in my rows
         opt.flags = k ? (uint32_t)GS_FLAG_LOAD_RT : 0u;
         rec(ctx, EV_VIEW1);
         if (timing) cudaEventRecord(mb.obj_tev[2 * k], ctx->stream);
-        if ((rc = do_draw(ctx, o.fc, opt, o.assets[i], o.fp, k == 0, d_rt, pitch, fmt, Surface{}, timing ? mb.obj_tev[2 * k + 1] : nullptr)))
+        if ((rc = do_draw(ctx, o.fc, opt, o.assets[i], o.fp, d_rt, pitch, fmt, Surface{}, timing ? mb.obj_tev[2 * k + 1] : nullptr)))
           return rc;
         ctx->launches += 1;   // k_row_costs: here for every object but the last (before the next one's raster overwrites the
                               // tile costs), on the transfer stream below for the last

@@ -24,6 +24,49 @@ struct GsContext;
 namespace gs {
 int fail(GsContext *ctx, int code, const std::string &msg);
 int fail_cuda(GsContext *ctx, cudaError_t e, const char *expr, const char *file, int line);
+
+// The bin list (DESIGN §2, "Overflow across a call"), entry_count = [entries within the capacity, overflow flag, total]: its rules
+// inline, its buffers and CUDA calls in gs_bins.cu.  A call starts with begin_call; each draw is begin_draw, builds, end_draw.
+constexpr uint32_t kBinListMax = 768u << 20;
+constexpr uint32_t kRuleBins = 128;   // the capacity rule was set for screens of at most this many bins per axis (8160 px)
+class BinList {
+ public:
+  static uint32_t capacity_for(uint32_t splats) {
+    return (uint32_t)std::min<uint64_t>(std::max<uint64_t>((uint64_t)splats * 8, 4u << 20), kBinListMax);
+  }
+  void begin_call() { flag_ = kFirst; }
+  bool clears() const { return flag_ == kFirst; }   // the draw's first build
+  // One camera above kRuleBins bins on an axis reads back and may rebuild: it first reads the flag the last draw did not read.
+  int begin_draw(GsContext *ctx, uint32_t cameras, const FrameConsts &fc) {
+    reads_ = cameras == 1 && (fc.binsX > kRuleBins || fc.binsY > kRuleBins);
+    if (!reads_ || flag_ != kUnknown) return GS_OK;
+    uint32_t ec[2] = {0, 0};
+    GS_CUDA_TRY(ctx, read(ctx, ec, 2));
+    flag_ = ec[1] ? kSet : kClear;
+    return GS_OK;
+  }
+  // After the first build, an overflowed list grows to its total + 1/4, at most kBinListMax, and *again asks to rebuild it with
+  // *clear: the grown list fits, so only a truncated earlier draw of the call keeps the flag set.
+  int end_draw(GsContext *ctx, uint32_t n, uint32_t bins, bool *again, bool *clear) {
+    uint32_t ec[3] = {0, 0, 0};   // clamped count, overflow flag, total (of this run, for gs_frame_objects)
+    if (reads_) GS_CUDA_TRY(ctx, read(ctx, ec, 3));
+    *again = reads_ && ec[2] > capacity() && ec[2] <= kBinListMax;
+    *clear = flag_ != kSet;
+    if (!reads_) flag_ = kUnknown;
+    else flag_ = (*again ? *clear : ec[1] == 0) ? kClear : kSet;
+    return *again ? reserve(ctx, n, bins, (uint32_t)std::min<uint64_t>((uint64_t)ec[2] + ec[2] / 4, kBinListMax)) : GS_OK;
+  }
+  int reserve(GsContext *ctx, uint32_t n, uint32_t bins, uint32_t min_capacity = 0);   // with the bin sort's sort scratch
+  cudaError_t read(GsContext *ctx, uint32_t *ec, uint32_t words);   // entry_count[0, words), once the stream is done
+  uint32_t capacity() const;   // the smaller buffer: after a failed growth one of them may still hold the larger, older size
+  int check(GsContext *ctx);   // at a host sync point: ctx->times.tile_entries, and GS_ERR_OUT_OF_MEMORY for a truncated list
+  Buffer<uint32_t> keys, vals, block_sums, entry_count;   // launchers take the view bin_scratch(ctx)
+  Buffer<uint2> ranges;
+
+ private:
+  enum { kFirst, kClear, kSet, kUnknown } flag_ = kFirst;   // the flag as the host knows it (kFirst: the next build clears it)
+  bool reads_ = false;   // the current draw reads its list back
+};
 }  // namespace gs
 
 enum { EV_BEGIN = 0, EV_DIST, EV_SORT0, EV_SORT1, EV_SORT2, EV_SORT3, EV_SORT4, EV_VIEW0, EV_VIEW1, EV_BIN1, EV_RASTER1, EV_COMP1, EV_COUNT };
@@ -41,12 +84,9 @@ struct GsContext {
   gs::Buffer<uint32_t> sort_alt_keys, sort_alt_vals;   // ping-pong buffers, as many elements as the largest sort so far
   gs::Buffer<uint32_t> sort_ghist, sort_lookback, sort_tickets;
   gs::Buffer<uint32_t> d_scalar;  // small device scalars (standalone sorter count)
-  // bin scratch (launchers take the view bin_scratch(ctx))
-  gs::Buffer<uint32_t> bin_keys, bin_vals, bin_block_sums, bin_entry_count;
-  gs::Buffer<uint2> bin_ranges;
+  gs::BinList bins;
   gs::Buffer<uint32_t> tile_cost, tile_order;   // the single-grid raster-tile history, and the launch order of every draw
   uint32_t raster_tiles_cur = 0;   // the tile count tile_cost's history was kept for
-  bool bin_overflow = false;   // the bin list's overflow flag as the last read-back of a frame above kLargeFrameBins left it
   // gs_frame_cameras: the tile-cost histories of the camera layouts seen ((raster tiles per row, rows) per camera of a run,
   // each history at its base in cams_tile_cost), the digit histograms of a camera run's bin list (the depth sorts between its
   // emits use sort_ghist), and one scratch buffer for a run's record slabs, staging images and host depth buffers
@@ -102,16 +142,14 @@ struct GsAsset {
 };
 
 namespace gs {
-// The launchers' views of the context's scratch.  The bin list's capacity is the smaller of its two buffers: after a failed
-// growth one of them may still hold the larger, older size.
+// The launchers' views of the context's scratch.
 inline SortScratch sort_scratch(const GsContext *ctx) {
   return {ctx->sort_alt_keys.get(), ctx->sort_alt_vals.get(), ctx->sort_ghist.get(), ctx->sort_lookback.get(), ctx->sort_tickets.get(),
           ctx->sort_lookback.size()};
 }
 inline BinScratch bin_scratch(const GsContext *ctx) {
-  return {ctx->bin_block_sums.get(), ctx->bin_entry_count.get(), ctx->bin_keys.get(), ctx->bin_vals.get(),
-          reinterpret_cast<uint32_t *>(ctx->bin_ranges.get()), ctx->tile_cost.get(), ctx->tile_order.get(),
-          (uint32_t)std::min(ctx->bin_keys.size(), ctx->bin_vals.size())};
+  return {ctx->bins.block_sums.get(), ctx->bins.entry_count.get(), ctx->bins.keys.get(), ctx->bins.vals.get(),
+          reinterpret_cast<uint32_t *>(ctx->bins.ranges.get()), ctx->tile_cost.get(), ctx->tile_order.get(), ctx->bins.capacity()};
 }
 FrameConsts make_frame_consts(const GsFrameParams *fp);
 int check_params(GsContext *ctx, GsAsset *as, const GsFrameParams *fp);
@@ -128,11 +166,9 @@ int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameCon
             cudaStream_t stream, float4 *draw = nullptr, float *zndc = nullptr, bool after_sort = false);
 // Bins and rasterizes one object `as`, drawn with the uniforms *fp, into a device image (d_rt == nullptr: the CUDA array behind
 // `surf`) on ctx->stream with gs_frame's kernels; its scene depth buffer is bound here.  A run of several objects or cameras is
-// gs_api.cu's draw_run.  `first`: the first draw of its public call, whose bin list sets the overflow flag; a later draw of
-// the call only ever sets it, so the call reports every truncated list.  bin_done (optional) is recorded on ctx->stream when
-// binning ends.
-int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *as, const GsFrameParams *fp, bool first,
-            void *d_rt, uint32_t pitch, uint32_t fmt, Surface surf = Surface{}, cudaEvent_t bin_done = nullptr);
+// gs_api.cu's draw_run.  bin_done (optional) is recorded on ctx->stream when binning ends.
+int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *as, const GsFrameParams *fp, void *d_rt,
+            uint32_t pitch, uint32_t fmt, Surface surf = Surface{}, cudaEvent_t bin_done = nullptr);
 // The composite pass (gs_composite) of a linear device render target onto `tgt` (host, device or CUDA-array memory, already
 // validated as W x H), enqueued on `s`.  A host target is uploaded and read back, and the call waits for `s`.
 int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H,

@@ -223,8 +223,7 @@ struct DrawObjects {
 };
 struct NoRasterObjects {};
 // One object's (bin id, splat id) list, sorted by bin id.  *sorted: the scratch view whose tile_keys / tile_vals hold it
-// (launch_raster's input).  clear_overflow: this is the first draw of its call, and its list sets the overflow flag
-// entry_count[1] from its own total; otherwise the flag is only ever set, so an earlier draw's truncation stays reported.
+// (launch_raster's input).  clear_overflow: the list sets the flag entry_count[1], else only ever sets it (BinList decides).
 cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, const uint32_t *order, const uint32_t *rect,
                            const uint32_t *block_bits, uint32_t n, bool clear_overflow, const BinScratch &bs, const SortScratch &sc,
                            cudaStream_t s, BinScratch *sorted, int *launches);
