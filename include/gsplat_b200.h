@@ -109,7 +109,17 @@ typedef struct GsFrameParams {
                                      tightly packed, in mat_proj_gpu's convention (reversed Z: 1 = near plane), where LEqual is
                                      evaluated as "fragment depth >= stored depth"; every fragment of a splat has the depth
                                      clip.z / clip.w of its centre (the quad is flat).  NULL = no depth test. */
-  uint32_t scene_depth_on_device; /* 0: scene_depth is host memory (uploaded per frame), 1: device memory (used in place) */
+  uint32_t scene_depth_on_device; /* the GsMemory of scene_depth.  0 (GS_MEM_HOST): host memory, uploaded per frame.
+                                     GS_MEM_ARRAY (2): scene_depth is a cudaArray_t, a 2-D array of screen_w x screen_h (depth 0)
+                                     of one 32-bit float channel, created with cudaArraySurfaceLoadStore.  GS_MEM_ARRAY_LAYER (4):
+                                     scene_depth points to a borrowed GsArrayLayer naming one layer of a layered array of
+                                     screen_w x screen_h of one 32-bit float channel, created with cudaArrayLayered |
+                                     cudaArraySurfaceLoadStore (`layer` below its layer count, `reserved` 0) -- e.g. one eye of an XR
+                                     eye-depth array.  Texel (x, y) of the array (layer) is the depth of pixel (x, y), read in place.
+                                     Another channel format is GS_ERR_UNSUPPORTED_FORMAT; any other mismatch, a null array, or a
+                                     layered array passed as 2 (a 2-D one as 4) is GS_ERR_INVALID_ARGUMENT, refused before anything
+                                     is enqueued.  The group entry points (gs_group_*) refuse 2 and 4 (GS_ERR_INVALID_ARGUMENT).
+                                     Any other value: device memory, used in place. */
   uint32_t reserved1;
 } GsFrameParams;
 

@@ -150,19 +150,6 @@ int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cu
   return GS_OK;
 }
 
-// The scene depth buffer the splat pass is tested against (GsFrameParams.scene_depth), in *depth (nullptr: none): used in
-// place when it is device memory, uploaded on the context stream when it is host memory.
-static int bind_depth(GsContext *ctx, const GsFrameParams *fp, const float **depth) {
-  *depth = nullptr;
-  if (!fp->scene_depth) return GS_OK;
-  if (fp->scene_depth_on_device) { *depth = fp->scene_depth; return GS_OK; }
-  const size_t pixels = (size_t)(uint32_t)fp->screen_w * (uint32_t)fp->screen_h;
-  GS_CUDA_TRY(ctx, ctx->d_depth.reserve(pixels, {ctx->stream}));
-  GS_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_depth.get(), fp->scene_depth, pixels * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-  *depth = ctx->d_depth.get();
-  return GS_OK;
-}
-
 int check_params(GsContext *ctx, GsAsset *as, const GsFrameParams *fp) {
   if (!ctx || !as || !fp) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null context/asset/params");
   if (as->ctx != ctx) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "asset belongs to another context");
@@ -170,7 +157,7 @@ int check_params(GsContext *ctx, GsAsset *as, const GsFrameParams *fp) {
   if (!(fp->screen_w >= 1.0f) || !(fp->screen_h >= 1.0f) || fp->screen_w > 16384.0f || fp->screen_h > 16384.0f)
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "screen size must be in [1,16384] (8-bit indices of 64-pixel bins)");
   if (fp->sh_order > 3) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "sh_order must be 0..3");
-  return GS_OK;
+  return depth_ok(ctx, fp);
 }
 
 static int do_sort(GsContext *ctx, GsAsset *as, const FrameConsts &fc) {
@@ -276,8 +263,8 @@ static int tile_history(GsContext *ctx, uint32_t tiles, const std::vector<uint32
   return GS_OK;
 }
 
-int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *as, const GsFrameParams *fp, void *d_rt,
-            uint32_t pitch, uint32_t fmt, Surface surf, cudaEvent_t bin_done) {
+int do_draw(GsContext *ctx, CallSurfaces *surfs, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *as, const GsFrameParams *fp,
+            void *d_rt, uint32_t pitch, uint32_t fmt, Surface surf, cudaEvent_t bin_done) {
   GsNvtxRange nvtx("GaussianSplat.Draw");
   const uint32_t n = as->av.n, bins = fc.binsX * fc.binsY;
   int rc = GS_OK;
@@ -285,8 +272,9 @@ int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, G
   uint32_t *tile_cost = nullptr;
   const uint32_t rtiles = (((uint32_t)fc.screenW + kTile - 1) / kTile) * fc.binsY * (kBin / kTile);   // of the whole image
   if ((rc = tile_history(ctx, rtiles, nullptr, &tile_cost))) return rc;
-  const float *depth = nullptr;
-  if ((rc = bind_depth(ctx, fp, &depth))) return rc;
+  if (depth_on_host(fp)) GS_CUDA_TRY(ctx, ctx->d_depth.reserve((size_t)(uint32_t)fp->screen_w * (uint32_t)fp->screen_h, {ctx->stream}));
+  SceneDepth depth;
+  if ((rc = bind_depth(ctx, surfs, fp, ctx->d_depth.get(), ctx->stream, &depth))) return rc;
   BinScratch lists;
   int bin_launches = 0, more = 0;
   GS_CUDA_TRY(ctx, launch_binning(fc, opt, as->order.get(), as->rect.get(), as->block_bits.get(), n, ctx->bins.clears(), bin_scratch(ctx),
@@ -641,7 +629,7 @@ int gs_render(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRend
   FrameImage fi;
   if ((rc = begin_frame_image(ctx, surfs, opt, rt, pitch, rt->format, nullptr, W, H, &fi))) return rc;
   ctx->bins.begin_call();
-  if ((rc = do_draw(ctx, fc, opt, as, fp, fi.d_rt, fi.pitch, rt->format, fi.surf)) ||
+  if ((rc = do_draw(ctx, &surfs, fc, opt, as, fp, fi.d_rt, fi.pitch, rt->format, fi.surf)) ||
       (rc = end_frame_image(ctx, surfs, rt, pitch, rt->format, nullptr, W, H, fi)))
     return rc;
   return rt->memory == GS_MEM_HOST ? ctx->bins.check(ctx) : GS_OK;
@@ -728,7 +716,7 @@ static uint32_t run_end(GsAsset *const *assets, const GsFrameParams *fps, uint32
     const GsFrameParams &f = fps[e];
     if (!f.scene_depth) continue;
     if (!depth) depth = &f;
-    else if (f.scene_depth != depth->scene_depth || f.scene_depth_on_device != depth->scene_depth_on_device) break;
+    else if (depth_id(&f) != depth_id(depth)) break;
   }
   return e;
 }
@@ -795,6 +783,7 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
   const bool multi = count > 1, cams_run = run.size() > 1;
   DrawCameras dc;
   memset(&dc, 0, sizeof(dc));
+  DepthSurfaces depth_surfs{};
   dc.count = (uint32_t)run.size();
   std::vector<uint32_t> layout;
   uint32_t tiles = 0, bins = 0;
@@ -825,7 +814,7 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
       slab_at[q] = later ? bytes + 1 : 0;   // 0: the asset's own buffers (offsets are stored + 1)
       if (later) bytes += align256((size_t)as->av.n * 48) + (f.scene_depth ? align256((size_t)as->av.n * 4 + 16) : 0);
     }
-    if (multi && depth_fp[i] && !depth_fp[i]->scene_depth_on_device) { depth_at[i] = bytes; bytes += align256((size_t)c.W * c.H * 4); }
+    if (multi && depth_fp[i] && depth_on_host(depth_fp[i])) { depth_at[i] = bytes; bytes += align256((size_t)c.W * c.H * 4); }
     if (cams_run && (!c.rt || c.rt->memory == GS_MEM_HOST)) { stage_at[i] = bytes; bytes += align256((size_t)c.W * pix_bytes(c.rt_fmt) * c.H); }
   }
   GS_CUDA_TRY(ctx, ctx->cams_scratch.reserve(bytes, {ctx->stream}));
@@ -837,12 +826,11 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
     if ((rc = ctx->bins.reserve(ctx, n, bins))) return rc;
     if ((rc = tile_history(ctx, tiles, cams_run ? &layout : nullptr, &tile_cost))) return rc;
     for (uint32_t i = 0; i < run.size(); ++i) {
-      if (depth_fp[i] && depth_fp[i]->scene_depth_on_device) dc.cam[i].depth = depth_fp[i]->scene_depth;
-      else if (depth_fp[i]) {
-        dc.cam[i].depth = reinterpret_cast<const float *>(scratch + depth_at[i]);
-        GS_CUDA_TRY(ctx, cudaMemcpyAsync(scratch + depth_at[i], depth_fp[i]->scene_depth, (size_t)dc.cam[i].W * dc.cam[i].H * 4,
-                                         cudaMemcpyHostToDevice, ctx->stream));
-      }
+      SceneDepth d;
+      if (depth_fp[i] && (rc = bind_depth(ctx, &surfs, depth_fp[i], reinterpret_cast<float *>(scratch + depth_at[i]), ctx->stream, &d)))
+        return rc;
+      dc.cam[i].depth = d.ptr;
+      if (d.on_surface) { depth_surfs.surf[i] = d.surf; depth_surfs.on_surface |= 1u << i; }
     }
     launch_bin_list_begin(bin_scratch(ctx), ctx->cams_ghist.get(), ctx->stream);
   }
@@ -893,7 +881,7 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
     const CameraArgs &c = cams[run[0].cam];
     GsRenderOptions o = opt;
     if (run[0].load) o.flags |= GS_FLAG_LOAD_RT;
-    if ((rc = do_draw(ctx, c.fcs[run[0].k0], o, assets[pair_at[0]], &fps[pair_at[0]], c.fi.d_rt, c.fi.pitch, c.rt_fmt, c.fi.surf)))
+    if ((rc = do_draw(ctx, &surfs, c.fcs[run[0].k0], o, assets[pair_at[0]], &fps[pair_at[0]], c.fi.d_rt, c.fi.pitch, c.rt_fmt, c.fi.surf)))
       return rc;
   } else {
     emit_to(count, ctx->bins.clears());
@@ -911,7 +899,7 @@ static int draw_run(GsContext *ctx, CallSurfaces &surfs, std::vector<CameraArgs>
     }
     lists.tile_cost = tile_cost;
     rec(ctx, EV_BIN1);
-    launch_raster_cameras(objs, dc, bins, tiles, opt.blend_mode, cams[run[0].cam].rt_fmt, lists, ctx->stream);
+    launch_raster_cameras(objs, dc, depth_surfs, bins, tiles, opt.blend_mode, cams[run[0].cam].rt_fmt, lists, ctx->stream);
     rec(ctx, EV_RASTER1);
     ctx->launches += sort_launches + 3;   // bin sort passes; bin_ranges, tile_order, raster
     GS_CUDA_TRY(ctx, cudaGetLastError());

@@ -555,6 +555,8 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
     for (size_t i = 0; i < L; ++i) {
       GsAsset *as = o.assets[i];
       if (!as) return fail(g->m[i].ctx, GS_ERR_INVALID_ARGUMENT, "null asset");
+      if (depth_in_array(o.fp))   // the members share the frame parameters, and a CUDA array belongs to one device
+        return fail(g->m[i].ctx, GS_ERR_INVALID_ARGUMENT, "a group's scene depth buffer must be host or linear device memory, not a CUDA array");
       if ((rc = check_params(g->m[i].ctx, as, o.fp))) return rc;
       if (as->av.n != o.assets[0]->av.n) return fail(g->m[i].ctx, GS_ERR_INVALID_ARGUMENT, "members hold different assets");
       for (size_t j = 0; j < (size_t)k * L; ++j)
@@ -836,7 +838,7 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
         opt.flags = k ? (uint32_t)GS_FLAG_LOAD_RT : 0u;
         rec(ctx, EV_VIEW1);
         if (timing) cudaEventRecord(mb.obj_tev[2 * k], ctx->stream);
-        if ((rc = do_draw(ctx, o.fc, opt, o.assets[i], o.fp, d_rt, pitch, fmt, Surface{}, timing ? mb.obj_tev[2 * k + 1] : nullptr)))
+        if ((rc = do_draw(ctx, nullptr, o.fc, opt, o.assets[i], o.fp, d_rt, pitch, fmt, Surface{}, timing ? mb.obj_tev[2 * k + 1] : nullptr)))
           return rc;
         ctx->launches += 1;   // k_row_costs: here for every object but the last (before the next one's raster overwrites the
                               // tile costs), on the transfer stream below for the last

@@ -1,6 +1,6 @@
 // gs_image.cu -- how the library reaches the pixels of a GsImage in each memory kind: validation, the device view a kernel
 // draws into (the image itself, a surface of its CUDA array, or a staging image), and the copy of a linear device image into
-// an image of any kind.
+// an image of any kind.  The same for the scene depth buffer a draw is tested against.
 #include <cstring>
 #include <string>
 
@@ -10,6 +10,38 @@ namespace gs {
 
 uint32_t pix_bytes(uint32_t fmt) { return fmt == GS_PIX_RGBA16F ? 8u : 16u; }
 
+// The rules every CUDA array the library reads or writes keeps: `a` (a GS_MEM_ARRAY or GS_MEM_ARRAY_LAYER view: data and memory)
+// is a W x H 2-D array, or a layer below the layer count of a W x H layered one, made with cudaArraySurfaceLoadStore, whose
+// channels are `channels` x `bits`-bit float (else GS_ERR_UNSUPPORTED_FORMAT; everything else is GS_ERR_INVALID_ARGUMENT).
+// The messages start with `prefix`, and name the size `of` and the channels `format` expected.
+static int array_ok(GsContext *ctx, const GsImage &a, uint32_t W, uint32_t H, int channels, int bits, const char *prefix, const char *of,
+                    const char *format) {
+  const std::string p(prefix);
+  const bool layered = a.memory == GS_MEM_ARRAY_LAYER;
+  if (layered) {
+    const GsArrayLayer *d = static_cast<const GsArrayLayer *>(a.data);
+    if (!d->array || d->reserved) return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "GsArrayLayer: array is null or reserved is not 0");
+  }
+  int32_t layer = -1;
+  cudaChannelFormatDesc cd;
+  cudaExtent ext;
+  unsigned int flags = 0;
+  const cudaError_t e = cudaArrayGetInfo(&cd, &ext, &flags, image_array(&a, &layer));
+  if (e != cudaSuccess) { cudaGetLastError(); return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "not a CUDA array: " + cudaGetErrorString(e)); }
+  const int want[4] = {bits, channels > 1 ? bits : 0, channels > 2 ? bits : 0, channels > 3 ? bits : 0};
+  if (cd.f != cudaChannelFormatKindFloat || cd.x != want[0] || cd.y != want[1] || cd.z != want[2] || cd.w != want[3])
+    return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, p + "the CUDA array's channel format does not match " + format);
+  if (!layered && (ext.width != W || ext.height != H || ext.depth != 0))
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the CUDA array is not a 2-D array of " + of + " size");
+  if (layered && (ext.width != W || ext.height != H || !(flags & cudaArrayLayered)))
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the CUDA array is not a layered array of " + of + " size");
+  if (layered && (uint32_t)layer >= ext.depth)
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the layer is not below the CUDA array's layer count");
+  if (!(flags & cudaArraySurfaceLoadStore))
+    return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the CUDA array was not created with cudaArraySurfaceLoadStore");
+  return GS_OK;
+}
+
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch) {
   if (!im || !im->data) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image is null");
   if (im->format > GS_PIX_RGBA32F) return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "unsupported pixel format");
@@ -18,28 +50,9 @@ int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t
   if (im->width != W || im->height != H) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image size does not match screen size");
   if (is_array_image(im)) {   // a 2-D CUDA array (data is a cudaArray_t), or a layer of a layered one (data is a GsArrayLayer *)
     if (im->row_pitch_bytes) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "row_pitch_bytes must be 0 for a CUDA array image");
-    const bool layered = im->memory == GS_MEM_ARRAY_LAYER;
-    if (layered) {
-      const GsArrayLayer *d = static_cast<const GsArrayLayer *>(im->data);
-      if (!d->array || d->reserved) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "GsArrayLayer: array is null or reserved is not 0");
-    }
-    int32_t layer = -1;
-    cudaChannelFormatDesc cd;
-    cudaExtent ext;
-    unsigned int flags = 0;
-    const cudaError_t e = cudaArrayGetInfo(&cd, &ext, &flags, image_array(im, &layer));
-    if (e != cudaSuccess) { cudaGetLastError(); return fail(ctx, GS_ERR_INVALID_ARGUMENT, std::string("not a CUDA array: ") + cudaGetErrorString(e)); }
-    const int bits = im->format == GS_PIX_RGBA16F ? 16 : 32;
-    if (cd.f != cudaChannelFormatKindFloat || cd.x != bits || cd.y != bits || cd.z != bits || cd.w != bits)
-      return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "the CUDA array's channel format does not match the image's pixel format");
-    if (!layered && (ext.width != W || ext.height != H || ext.depth != 0))
-      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array is not a 2-D array of the image's size");
-    if (layered && (ext.width != W || ext.height != H || !(flags & cudaArrayLayered)))
-      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array is not a layered array of the image's size");
-    if (layered && (uint32_t)layer >= ext.depth)
-      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the layer is not below the CUDA array's layer count");
-    if (!(flags & cudaArraySurfaceLoadStore))
-      return fail(ctx, GS_ERR_INVALID_ARGUMENT, "the CUDA array was not created with cudaArraySurfaceLoadStore");
+    const int rc = array_ok(ctx, *im, W, H, 4, im->format == GS_PIX_RGBA16F ? 16 : 32, "", "the image's",
+                           "the image's pixel format");
+    if (rc) return rc;
     *pitch = 0;
     return GS_OK;
   }
@@ -118,6 +131,37 @@ int copy_to_image(GsContext *ctx, const GsImage *im, uint32_t pitch, const void 
     const cudaMemcpyKind kind = im->memory == GS_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
     GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(im->data, pitch, src, src_pitch, row, H, kind, s));
   }
+  return GS_OK;
+}
+
+int depth_ok(GsContext *ctx, const GsFrameParams *fp) {
+  if (!depth_in_array(fp)) return GS_OK;
+  return array_ok(ctx, depth_view(fp), (uint32_t)fp->screen_w, (uint32_t)fp->screen_h, 1, 32, "scene depth: ",
+                  "the screen's", "one 32-bit float channel");
+}
+
+std::tuple<const void *, int32_t, uint32_t> depth_id(const GsFrameParams *fp) {
+  if (!fp->scene_depth) return {nullptr, -1, 0};
+  if (fp->scene_depth_on_device == GS_MEM_ARRAY_LAYER) {
+    const GsArrayLayer *d = reinterpret_cast<const GsArrayLayer *>(fp->scene_depth);
+    return {d->array, (int32_t)d->layer, GS_MEM_ARRAY_LAYER};
+  }
+  return {fp->scene_depth, -1, fp->scene_depth_on_device};
+}
+
+int bind_depth(GsContext *ctx, CallSurfaces *surfs, const GsFrameParams *fp, float *staging, cudaStream_t s, SceneDepth *out) {
+  *out = SceneDepth{};
+  if (!fp->scene_depth) return GS_OK;
+  if (depth_in_array(fp)) {
+    if (!surfs) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "a scene depth buffer in a CUDA array needs the call's surfaces");
+    const GsImage a = depth_view(fp);
+    out->on_surface = true;
+    return surfs->make(&a, &out->surf);
+  }
+  if (!depth_on_host(fp)) { out->ptr = fp->scene_depth; return GS_OK; }
+  const size_t pixels = (size_t)(uint32_t)fp->screen_w * (uint32_t)fp->screen_h;
+  GS_CUDA_TRY(ctx, cudaMemcpyAsync(staging, fp->scene_depth, pixels * sizeof(float), cudaMemcpyHostToDevice, s));
+  out->ptr = staging;
   return GS_OK;
 }
 

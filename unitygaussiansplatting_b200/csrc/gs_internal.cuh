@@ -4,6 +4,7 @@
 #include <algorithm>
 #include <cstring>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include <nvtx3/nvToolsExt.h>   // header-only; costs one predicted-not-taken branch per range when no tool is attached
@@ -22,6 +23,7 @@ struct GsNvtxRange {
 
 struct GsContext;
 namespace gs {
+class CallSurfaces;
 int fail(GsContext *ctx, int code, const std::string &msg);
 int fail_cuda(GsContext *ctx, cudaError_t e, const char *expr, const char *file, int line);
 
@@ -165,10 +167,11 @@ int upload_frame_inputs(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, cu
 int do_view(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const FrameConsts &fc, bool cull, const GsRenderOptions &opt,
             cudaStream_t stream, float4 *draw = nullptr, float *zndc = nullptr, bool after_sort = false);
 // Bins and rasterizes one object `as`, drawn with the uniforms *fp, into a device image (d_rt == nullptr: the CUDA array behind
-// `surf`) on ctx->stream with gs_frame's kernels; its scene depth buffer is bound here.  A run of several objects or cameras is
-// gs_api.cu's draw_run.  bin_done (optional) is recorded on ctx->stream when binning ends.
-int do_draw(GsContext *ctx, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *as, const GsFrameParams *fp, void *d_rt,
-            uint32_t pitch, uint32_t fmt, Surface surf = Surface{}, cudaEvent_t bin_done = nullptr);
+// `surf`) on ctx->stream with gs_frame's kernels; its scene depth buffer is bound here, a CUDA array through `surfs` (nullptr:
+// the caller takes no CUDA-array depth).  A run of several objects or cameras is gs_api.cu's draw_run.  bin_done (optional) is
+// recorded on ctx->stream when binning ends.
+int do_draw(GsContext *ctx, CallSurfaces *surfs, const FrameConsts &fc, const GsRenderOptions &opt, GsAsset *as, const GsFrameParams *fp,
+            void *d_rt, uint32_t pitch, uint32_t fmt, Surface surf = Surface{}, cudaEvent_t bin_done = nullptr);
 // The composite pass (gs_composite) of a linear device render target onto `tgt` (host, device or CUDA-array memory, already
 // validated as W x H), enqueued on `s`.  A host target is uploaded and read back, and the call waits for `s`.
 int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H,
@@ -256,6 +259,31 @@ int bind_image(GsContext *ctx, CallSurfaces &surfs, const GsImage *im, uint32_t 
 // on `s`.
 int copy_to_image(GsContext *ctx, const GsImage *im, uint32_t pitch, const void *src, uint32_t src_pitch, uint32_t W, uint32_t H,
                   cudaStream_t s);
+
+// ---- the scene depth buffer (gs_image.cu) --------------------------------------------------------------------------------
+// GsFrameParams.scene_depth_on_device is the GsMemory of scene_depth: 0 host memory, GS_MEM_ARRAY a 2-D float32 CUDA array,
+// GS_MEM_ARRAY_LAYER a GsArrayLayer naming a layer of a layered one, any other value linear device memory.
+inline bool depth_on_host(const GsFrameParams *fp) { return fp->scene_depth && fp->scene_depth_on_device == GS_MEM_HOST; }
+inline bool depth_in_array(const GsFrameParams *fp) {
+  return fp->scene_depth && (fp->scene_depth_on_device == GS_MEM_ARRAY || fp->scene_depth_on_device == GS_MEM_ARRAY_LAYER);
+}
+// The array (layer) of a depth_in_array buffer as an image view (data and memory), as image_array and CallSurfaces take it.
+inline GsImage depth_view(const GsFrameParams *fp) {
+  GsImage a{};
+  a.data = const_cast<float *>(fp->scene_depth);
+  a.memory = fp->scene_depth_on_device;
+  return a;
+}
+// A CUDA-array depth buffer must be a screen_w x screen_h array (layer) of one 32-bit float channel made with
+// cudaArraySurfaceLoadStore: GS_ERR_UNSUPPORTED_FORMAT for another channel format, GS_ERR_INVALID_ARGUMENT for anything else.
+int depth_ok(GsContext *ctx, const GsFrameParams *fp);
+// What makes two objects' depth buffers one buffer: the same pointer and memory kind, or the same array and layer
+// (GS_MEM_ARRAY_LAYER: two descriptors of one layer are one buffer, the layers of one array are not).  (nullptr, ...): none.
+std::tuple<const void *, int32_t, uint32_t> depth_id(const GsFrameParams *fp);
+// The kernels' view of fp's depth buffer (passed depth_ok), on `s`: device memory in place, a CUDA array (layer) through a
+// surface made by `surfs` (nullptr: none may be made, and a CUDA array is GS_ERR_INVALID_ARGUMENT), or a host buffer uploaded
+// into `staging`, W x H floats that the caller has grown.
+int bind_depth(GsContext *ctx, CallSurfaces *surfs, const GsFrameParams *fp, float *staging, cudaStream_t s, SceneDepth *out);
 // The per-asset work buffers (order, keys, view data, ...) of an asset whose blobs as->d_* are already in HBM, the format
 // fields of as->av, and CSSetIndices: what gs_asset_upload and gs_pack_asset share.
 cudaError_t asset_init_work(GsContext *ctx, GsAsset *as, uint32_t n, uint32_t pos_fmt, uint32_t scale_fmt, uint32_t sh_fmt,

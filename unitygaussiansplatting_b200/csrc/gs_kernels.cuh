@@ -234,6 +234,15 @@ struct Surface {
   cudaSurfaceObject_t obj = 0;
   int32_t layer = -1;
 };
+// The scene depth buffer a draw is tested against, W x H float32 texels, texel (x, y) the depth of pixel (x, y): linear device
+// memory at `ptr` (rows tightly packed), or, with `on_surface`, a one-channel float32 CUDA array (layer) behind `surf`.  Neither:
+// no depth test.
+struct SceneDepth {
+  const float *ptr = nullptr;
+  Surface surf;
+  bool on_surface = false;
+  __host__ __device__ bool bound() const { return ptr != nullptr || on_surface; }
+};
 
 // The cameras of a run, in shared memory in the MULTI raster.  A run is a list of camera segments: camera c's pairs of the run
 // own the bin ids [bin_base, bin_base + its bins) and the raster tiles [tile_base, tile_base + its tiles).  A run of one camera
@@ -241,13 +250,20 @@ struct Surface {
 struct RasterCamera {
   uint8_t *rt;                 // linear device image, or nullptr: the CUDA array behind `surf`
   Surface surf;
-  const float *depth;          // the camera's scene depth buffer (device memory), or nullptr
+  const float *depth;          // the camera's scene depth buffer in linear device memory, or nullptr (see DepthSurfaces)
   uint32_t pitch, tile_base, bin_base, ntx, binsX, W, H;
   uint32_t load;               // 1: blend under what the image holds (the camera's earlier run drew it); 0: the image starts cleared
 };
 struct DrawCameras {
   RasterCamera cam[kRunObjects];
   uint32_t count;
+};
+// The run's scene depth buffers that are CUDA arrays (layers): with bit c of on_surface, camera c's depth is the array behind
+// surf[c] rather than cam[c].depth.  A parameter of the MULTI raster's SEL instantiations only, after the camera table, so that
+// the others keep their parameter layout and code.
+struct DepthSurfaces {
+  Surface surf[kRunObjects];
+  uint32_t on_surface;
 };
 // The run's binning, in three steps around its pairs' sorts and view-calcs (a pair's emit must come before a later sort or
 // view-calc of the same asset overwrites order / rect / block_bits):
@@ -262,15 +278,15 @@ cudaError_t launch_bin_list_sort(uint32_t bins, const BinScratch &bs, SortScratc
                                  int *launches);
 // k_bin_ranges over the run's bins, k_tile_order over its raster tiles (history indexed by tile_base + tile), and the raster.
 // Every render target of the run has rt_format.
-void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, uint32_t bins, uint32_t tiles, uint32_t blend_mode,
-                           uint32_t rt_format, const BinScratch &bs, cudaStream_t s);
+void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, const DepthSurfaces &depth_surfs, uint32_t bins,
+                           uint32_t tiles, uint32_t blend_mode, uint32_t rt_format, const BinScratch &bs, cudaStream_t s);
 // One object's raster: records `draw`, quad depths `zndc` (when depth-tested), `extras`: a selection or a scene depth buffer
-// (the SEL instantiation).  scene_depth: the W x H depth buffer it is tested against (nullptr: none).  opt: tile partition,
+// (the SEL instantiation).  scene_depth: the W x H depth buffer it is tested against (none: no test).  opt: tile partition,
 // band_packed, blend mode and GS_FLAG_LOAD_RT.  Images here are linear device memory (pointer, pitch) or, when the pointer is
 // null, a CUDA array behind a surface object.
 void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const float *zndc, bool extras,
                    const BinScratch &bs, void *rt, uint32_t rt_pitch_bytes, uint32_t rt_format, Surface rt_surf, cudaStream_t s,
-                   const float *scene_depth);
+                   const SceneDepth &scene_depth);
 extern unsigned long long *g_raster_stats;   // diagnostics, see GS_RASTER_STATS
 uint32_t partition_own_bin_rows(const GsRenderOptions &opt, uint32_t binsY);
 uint32_t partition_own_tile_rows(const GsRenderOptions &opt, uint32_t binsY);

@@ -427,7 +427,9 @@ __device__ __forceinline__ void surf_store(const T &v, const Surface &s, uint32_
 // SEL ("extras"): a separate instantiation for frames with an edit selection and / or a scene depth buffer bound, so that
 // ordinary frames pay nothing.  Selected splats (records with opacity -1) take the pixel shader's other branch
 // (S/RenderGaussianSplats.shader:87-101); with `scene_depth` every fragment is depth-tested like the pass's ZTest LEqual
-// (reversed Z: quad depth >= stored depth), the per-splat quad depths being staged beside the records.
+// (reversed Z: quad depth >= stored depth), the per-splat quad depths being staged beside the records.  The scene depth is read
+// once per pixel, from linear memory or a CUDA array (layer), by a branch that is uniform over the grid.  The other
+// instantiations take an unused null pointer in its place.
 // SURF: the target is a CUDA array, read and written through `surf` instead of `rt`/`pitch`: 1, a 2-D array (GS_MEM_ARRAY);
 // 2, some target is one layer of a layered array (GS_MEM_ARRAY_LAYER; surf.layer picks the surface call at the load and the
 // store).  Separate instantiations, so that the linear and the 2-D array ones keep their code.
@@ -442,8 +444,9 @@ __global__ void __launch_bounds__(256, MULTI && SEL ? 8 : 0)
 k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const uint2 *__restrict__ bin_ranges,
          const uint32_t *__restrict__ tile_vals, const uint32_t *__restrict__ tile_order, uint32_t *__restrict__ tile_cost, uint32_t ntx,
          uint8_t *__restrict__ rt, uint32_t pitch, Surface surf, uint32_t band_packed, uint32_t load_rt,
-         unsigned long long *stats, const float *__restrict__ zndc, const float *__restrict__ scene_depth,
-         std::conditional_t<MULTI, DrawObjects, NoRasterObjects> objs, std::conditional_t<MULTI, DrawCameras, NoRasterObjects> cams) {
+         unsigned long long *stats, const float *__restrict__ zndc, std::conditional_t<SEL, SceneDepth, const float *> scene_depth,
+         std::conditional_t<MULTI, DrawObjects, NoRasterObjects> objs, std::conditional_t<MULTI, DrawCameras, NoRasterObjects> cams,
+         std::conditional_t<MULTI && SEL, DepthSurfaces, NoRasterObjects> depth_surfs) {
   uint32_t st_batches = 0, st_culls = 0, st_cand = 0, st_eval = 0, st_blend = 0;   // GS_RASTER_STATS diagnostics (per warp)
   unsigned long long st_t0 = 0;
   chain_wait();   // nothing before the wait: the bin ranges come from the predecessor
@@ -460,25 +463,28 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   // MULTI: the tile's first tile / bin in the run, and its camera (found again where it is used, so that nothing of it is held
   // in registers across the blend loop)
   uint32_t lin = 0, tile_base = 0, bin_base = 0;
-  auto camera = [&](const auto &cs) -> const RasterCamera & {   // (generic: instantiated only where MULTI calls it)
+  auto camera_index = [&](const auto &cs) -> uint32_t {   // (generic: instantiated only where MULTI calls it)
     uint32_t c = 0;
     for (uint32_t k = 1; k < cs.count; ++k) if (lin >= cs.cam[k].tile_base) c = k;
-    return cs.cam[c];
+    return c;
   };
+  auto camera = [&](const auto &cs) -> const RasterCamera & { return cs.cam[camera_index(cs)]; };
+  bool depth_test = false;   // MULTI: the tile's camera's
+  if constexpr (SEL) depth_test = scene_depth.bound();
   if constexpr (MULTI) {
     if (threadIdx.x < objs.count) { s_draw[threadIdx.x] = objs.draw[threadIdx.x]; s_zndc[threadIdx.x] = objs.zndc[threadIdx.x]; }
     __syncthreads();
     lin = __ldg(tile_order + blockIdx.x);
     const RasterCamera &cam = camera(cams);
     fc.screenW = (float)cam.W; fc.screenH = (float)cam.H; fc.binsX = cam.binsX;
-    ntx = cam.ntx; scene_depth = cam.depth; load_rt = cam.load;
+    ntx = cam.ntx; load_rt = cam.load;
+    if constexpr (SEL) depth_test = cam.depth != nullptr || ((depth_surfs.on_surface >> camera_index(cams)) & 1u);   // the buffer itself is found again at its one load
     tile_base = cam.tile_base; bin_base = cam.bin_base;
   }
   bool surf_io = SURF != 0;
   auto camera_image = [&]() {
     if constexpr (MULTI) { const RasterCamera &cam = camera(cams); rt = cam.rt; pitch = cam.pitch; surf = cam.surf; surf_io = SURF != 0 && rt == nullptr; }
   };
-  const bool depth_test = SEL && scene_depth != nullptr;
   // FP32 blending into an RGBA16F target: drawing the objects one after the other stores (rounds to half) each object's result
   // and the next object starts from it.  Rounding is idempotent, so rounding at the next object's first candidate is exact.
   constexpr bool kRoundAtObject = MULTI && !FP16_ROP && OUT_FMT == GS_PIX_RGBA16F;
@@ -507,7 +513,20 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   float d0 = 0.f, d1 = 0.f, d2 = 0.f, d3 = 0.f;  // ClearRenderTarget(0,0,0,0), R/GaussianSplatRenderer.cs:196
   // the scene's depth at this pixel (depth target bound at R/GaussianSplatRenderer.cs:195; ZTest LEqual, ZWrite Off)
   float zscene = 0.0f;
-  if (SEL && depth_test && in_image) zscene = __ldg(scene_depth + (size_t)py * (uint32_t)fc.screenW + px);
+  if constexpr (SEL) {
+    if (depth_test && in_image) {
+      const size_t at = (size_t)py * (uint32_t)fc.screenW + px;
+      if constexpr (MULTI) {
+        const uint32_t c = camera_index(cams);
+        if ((depth_surfs.on_surface >> c) & 1u) surf_load<true>(&zscene, depth_surfs.surf[c], px * 4u, py);
+        else zscene = __ldg(cams.cam[c].depth + at);
+      } else if (scene_depth.on_surface) {
+        surf_load<true>(&zscene, scene_depth.surf, px * 4u, py);
+      } else {
+        zscene = __ldg(scene_depth.ptr + at);
+      }
+    }
+  }
   // where this pixel lives in the target (band-packed: own bin row k of an interleaved partition -> rows [64k, 64k+64))
   const uint32_t out_row = band_packed ? part.own_rows_below(brow) * kBin + (py - brow * kBin) : py;
   if (load_rt && in_image) {
@@ -676,7 +695,7 @@ unsigned long long *g_raster_stats = nullptr;
 
 void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const float4 *draw, const float *zndc, bool extras,
                    const BinScratch &bs, void *rt, uint32_t rt_pitch_bytes, uint32_t rt_format, Surface rt_surf, cudaStream_t s,
-                   const float *scene_depth) {
+                   const SceneDepth &scene_depth) {
   const Partition part = make_partition(opt);
   const uint32_t rows = part.own_tile_rows(fc.binsY);
   if (!rows || !fc.binsX) return;
@@ -696,14 +715,14 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const floa
   uint2 *ranges = reinterpret_cast<uint2 *>(bs.bin_ranges);
   const uint32_t packed = part.range ? 0u : opt.band_packed, load = (opt.flags & GS_FLAG_LOAD_RT) ? 1u : 0u;
   chain_launch(k_bin_ranges, (bins + 7) / 8, 256, 0, s, bs.tile_keys, bs.entry_count, bins, ranges);
-#define GS_RASTER_ARGS                                                                                                           \
+#define GS_RASTER_ARGS(DEPTH)                                                                                                    \
   grid, 256, 0, s, fc, part, draw, ranges, bs.tile_vals, bs.tile_order, bs.tile_cost, ntx, out, rt_pitch_bytes, rt_surf, packed,  \
-      load, stats, zndc, scene_depth, NoRasterObjects{}, NoRasterObjects{}
+      load, stats, zndc, DEPTH, NoRasterObjects{}, NoRasterObjects{}, NoRasterObjects{}
 #define GS_LAUNCH_RASTER(ROP, FMT, SURF)                                                                                        \
   do {                                                                                                                         \
-    if (extras) chain_launch(k_raster<ROP, FMT, false, true, SURF>, GS_RASTER_ARGS);                                           \
-    else if (stats) chain_launch(k_raster<ROP, FMT, true, false, SURF>, GS_RASTER_ARGS);                                       \
-    else chain_launch(k_raster<ROP, FMT, false, false, SURF>, GS_RASTER_ARGS);                                                 \
+    if (extras) chain_launch(k_raster<ROP, FMT, false, true, SURF>, GS_RASTER_ARGS(scene_depth));                              \
+    else if (stats) chain_launch(k_raster<ROP, FMT, true, false, SURF>, GS_RASTER_ARGS(nullptr));                              \
+    else chain_launch(k_raster<ROP, FMT, false, false, SURF>, GS_RASTER_ARGS(nullptr));                                        \
   } while (0)
   // a null `rt` means the target is a CUDA array behind rt_surf
 #define GS_LAUNCH_RASTER_TARGET(ROP, FMT)                                                                                       \
@@ -722,8 +741,8 @@ void launch_raster(const FrameConsts &fc, const GsRenderOptions &opt, const floa
 #undef GS_RASTER_ARGS
 }
 
-void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, uint32_t bins, uint32_t tiles, uint32_t blend_mode,
-                           uint32_t rt_format, const BinScratch &bs, cudaStream_t s) {
+void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, const DepthSurfaces &depth_surfs, uint32_t bins,
+                           uint32_t tiles, uint32_t blend_mode, uint32_t rt_format, const BinScratch &bs, cudaStream_t s) {
   const Partition whole{0, 0, 1, 0, 0, 0};
   // without a partition a tile's id is its launch-order id: ntx = tiles puts all of them in row 0
   chain_launch(k_tile_order, 1, 1024, 0, s, bs.tile_cost, tiles, tiles, whole, bs.tile_order);
@@ -739,10 +758,11 @@ void launch_raster_cameras(const DrawObjects &objs, const DrawCameras &cams, uin
   do {                                                                                                                         \
     if (objs.extras)                                                                                                           \
       chain_launch(k_raster<ROP, FMT, false, true, SURF, true>, tiles, 256, 0, s, fc, whole, nullptr, ranges, bs.tile_vals,        \
-          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, Surface{}, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);               \
+          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, Surface{}, 0u, 0u, nullptr, nullptr, SceneDepth{}, objs, cams, depth_surfs);  \
     else                                                                                                                       \
       chain_launch(k_raster<ROP, FMT, false, false, SURF, true>, tiles, 256, 0, s, fc, whole, nullptr, ranges, bs.tile_vals,       \
-          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, Surface{}, 0u, 0u, nullptr, nullptr, nullptr, objs, cams);               \
+          bs.tile_order, bs.tile_cost, 1u, nullptr, 0u, Surface{}, 0u, 0u, nullptr, nullptr, nullptr, objs, cams,                 \
+          NoRasterObjects{});                                                                                                  \
   } while (0)
 #define GS_RASTER_CAMS_TARGET(ROP, FMT)                                                                                         \
   do {                                                                                                                         \

@@ -57,6 +57,17 @@ class GaussianSplatRenderer {
   Matrix4x4 localToWorldMatrix{{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}};
   Matrix4x4 worldToLocalMatrix{{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}};
   std::vector<GsCutout> m_Cutouts;
+  // The camera's depth buffer the splats are depth-tested against (GsFrameParams.scene_depth), width x height float32 in
+  // reversed Z, or nullptr.  sceneDepthMemory is its GsMemory (scene_depth_on_device): GS_MEM_HOST, GS_MEM_DEVICE, GS_MEM_ARRAY
+  // (sceneDepth is a cudaArray_t of one float32 channel) or GS_MEM_ARRAY_LAYER (SetSceneDepthLayer).
+  const float *sceneDepth = nullptr;
+  uint32_t sceneDepthMemory = GS_MEM_HOST;
+  // The depth is one layer of a layered float32 CUDA array (e.g. one eye of an XR eye-depth array); `desc` must outlive every
+  // frame drawn with it.
+  void SetSceneDepthLayer(const GsArrayLayer *desc) {
+    sceneDepth = reinterpret_cast<const float *>(desc);
+    sceneDepthMemory = GS_MEM_ARRAY_LAYER;
+  }
   GsRenderOptions options{};
 
   ~GaussianSplatRenderer() { OnDisable(); }
@@ -221,6 +232,8 @@ class GaussianSplatRenderer {
     fp.sh_only = m_SHOnly ? 1u : 0u;
     fp.cutouts = m_Cutouts.empty() ? nullptr : m_Cutouts.data();
     fp.cutout_count = (uint32_t)m_Cutouts.size();
+    fp.scene_depth = sceneDepth;
+    fp.scene_depth_on_device = sceneDepthMemory;
     return fp;
   }
   bool ok(int rc) const {

@@ -110,6 +110,28 @@ class CudaArrayImage:
         return (self.height, self.width, 4)
 
 
+class CudaArrayDepth:
+    """A scene depth buffer in a CUDA array (cudaArray_t, e.g. a camera's depth copied into an imported R32 float texture): a
+    2-D array of one float32 channel (GS_MEM_ARRAY), or with `layer` that layer of a layered one (GS_MEM_ARRAY_LAYER, e.g. one
+    eye of an XR eye-depth array).  Texel (x, y) is the depth of pixel (x, y), reversed Z as for a depth tensor.  The array must
+    have been created with cudaArraySurfaceLoadStore (and cudaArrayLayered for a layer); the host keeps it alive."""
+
+    def __init__(self, handle: int, width: int, height: int, layer=None):
+        self.handle = int(handle)
+        self.width, self.height = int(width), int(height)
+        if self.width < 1 or self.height < 1:
+            raise ValueError("CudaArrayDepth width and height must be positive")
+        self.layer = None if layer is None else int(layer)
+        if self.layer is not None and not 0 <= self.layer < 2 ** 32:
+            raise ValueError("CudaArrayDepth layer must be a non-negative 32-bit index")
+        # the descriptor a GS_MEM_ARRAY_LAYER depth buffer points to, alive as long as this object
+        self._layer_desc = None if self.layer is None else N.GsArrayLayer(self.handle, self.layer, 0)
+
+    @property
+    def shape(self):
+        return (self.height, self.width)
+
+
 def _image(arr, width: int, height: int) -> N.GsImage:
     """numpy (host) array or torch CUDA tensor of shape (H, W, 4), float16/float32, or a CudaArrayImage -> GsImage."""
     im = N.GsImage()
@@ -242,8 +264,17 @@ def make_frame_params(cam: Camera, localToWorld=None, splat_scale=1.0, opacity_s
         assert bits.size >= (splat_count + 31) // 32
         fp.selected_bits = bits.ctypes.data
         keep.append(bits)
-    if scene_depth is not None:    # (H, W) float32: numpy host array or torch CUDA tensor
-        if isinstance(scene_depth, np.ndarray):
+    if scene_depth is not None:    # (H, W) float32: numpy host array, torch CUDA tensor or CudaArrayDepth
+        if isinstance(scene_depth, CudaArrayDepth):
+            if scene_depth.shape != (cam.pixelHeight, cam.pixelWidth):
+                raise ValueError("the depth CUDA array is %dx%d, the screen %dx%d" % (scene_depth.width, scene_depth.height,
+                                                                                   cam.pixelWidth, cam.pixelHeight))
+            if scene_depth.layer is None:
+                fp.scene_depth, fp.scene_depth_on_device = scene_depth.handle, N.GS_MEM_ARRAY
+            else:
+                fp.scene_depth, fp.scene_depth_on_device = C.addressof(scene_depth._layer_desc), N.GS_MEM_ARRAY_LAYER
+            depth = scene_depth   # keeps its layer descriptor alive with the frame params
+        elif isinstance(scene_depth, np.ndarray):
             depth = np.ascontiguousarray(scene_depth, np.float32)
             assert depth.shape == (cam.pixelHeight, cam.pixelWidth)
             fp.scene_depth, fp.scene_depth_on_device = depth.ctypes.data, 0
@@ -290,7 +321,8 @@ class GaussianSplatRenderer:
         self.m_Cutouts = []          # list of (4x4 matrix, type_and_flags)
         self.m_DeletedBits = None    # np.uint32[ceil(N/32)] or None
         self.m_SelectedBits = None   # np.uint32[ceil(N/32)] or None (m_GpuEditSelected, R/GaussianSplatRenderer.cs:496)
-        self.sceneDepth = None       # (H, W) float32 camera depth buffer (reversed Z) the splats are depth-tested against, or None
+        self.sceneDepth = None       # (H, W) float32 camera depth buffer (reversed Z) the splats are depth-tested against (numpy,
+                                     # torch CUDA tensor or CudaArrayDepth), or None
         self.blend_mode = N.GS_BLEND_FP16_ROP
         self.partition = (0, 0, 1)   # index, count, band_rows
         self.band_packed = False
