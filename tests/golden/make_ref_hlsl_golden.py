@@ -37,6 +37,9 @@ VIEW_QUALITIES = ("Medium", "VeryHigh", "High", "Low", "custom-f16sh", "custom-n
 VIEW_SAMPLE = 512
 KEY_QUALITIES = ("Medium", "VeryHigh", "custom-norm6pos-f16sh", "custom-f32pos-bc7-f16sh")   # + Norm6, chunked Float32 positions
 KEY_N, KEY_SAMPLE = 30000, 4096
+# "pose-<name>": the camera pose <name> of tests/util.py POSES (or "near", the near-plane scene) in place of the default camera
+VIEW_POSES = ("pose-inside-back", "pose-xr-left", "pose-mirrored", "pose-near")
+KEY_POSES = ("pose-inside-back",)
 EXPORT_N, EXPORT_SAMPLE = 3000, 128
 DRAW_W, DRAW_H = 200, 150
 
@@ -60,11 +63,25 @@ def sample_ids(n=N, k=SAMPLE, seed=SAMPLE_SEED):
     return np.sort(np.random.default_rng(seed).choice(n, k, replace=False)).astype(np.uint32)
 
 
+def pose_camera(g, pose):
+    from util import POSES, near_plane_camera
+    return near_plane_camera(g) if pose == "near" else POSES[pose](g)
+
+
 def view_case(quality):
-    """(asset, (fp, keep)): object transform, splat / opacity scale, a cutout box and deleted bits on a clustered scene."""
+    """(asset, (fp, keep)): object transform, splat / opacity scale, a cutout box and deleted bits on a clustered scene.
+    "pose-<name>": the Medium scene seen from that camera pose; "pose-near": the near-plane scene under an identity transform,
+    so that its view depths stay the exact ones it was built with."""
     import unitygaussiansplatting_b200 as g
-    from util import camera, case_asset, format_case, palette_backed
-    if quality in ("custom-f16sh", "custom-norm6pos"):     # Float16 SH; Norm6 positions with Norm16 scale
+    from util import camera, case_asset, format_case, near_plane_scene, palette_backed
+    cam = camera(g, 320, 240)
+    if quality.startswith("pose-"):
+        cam = pose_camera(g, quality[len("pose-"):])
+    if quality == "pose-near":
+        asset = near_plane_scene(g, cam)
+    elif quality.startswith("pose-"):
+        asset = g.synthetic_asset(g.SCENE_CLUSTERED, N, 0x5EED0091, "Medium")
+    elif quality in ("custom-f16sh", "custom-norm6pos"):     # Float16 SH; Norm6 positions with Norm16 scale
         fmts = {"custom-f16sh": (g.VectorFormat.Norm16, g.VectorFormat.Norm6, g.ColorFormat.Float16x4, g.SHFormat.Float16),
                 "custom-norm6pos": (g.VectorFormat.Norm6, g.VectorFormat.Norm16, g.ColorFormat.Float32x4, g.SHFormat.Norm11)}[quality]
         asset = g.create_asset(g.generate_input_splats(g.SCENE_CLUSTERED, N, 0x5EED0091), formats=fmts)
@@ -76,17 +93,23 @@ def view_case(quality):
     T = np.eye(4, dtype=np.float32)
     T[:3, :3] = np.array([[0.8, -0.6, 0.0], [0.6, 0.8, 0.0], [0.0, 0.0, 1.0]], np.float32) * 1.1
     T[:3, 3] = (0.3, -0.1, 0.2)
+    if quality == "pose-near":
+        T = np.eye(4, dtype=np.float32)
     box = np.diag([1 / 9.0, 1 / 9.0, 1 / 9.0, 1.0]).astype(np.float32)
     deleted = np.zeros((N + 31) // 32, np.uint32)
     deleted[3] = 0xF0F0F0F0
-    return asset, g.make_frame_params(camera(g, 320, 240), localToWorld=T, splat_scale=0.9, opacity_scale=1.3, sh_order=3,
-                                      cutouts=[(box, 1)], deleted_bits=deleted, splat_count=N)
+    return asset, g.make_frame_params(cam, localToWorld=T, splat_scale=0.9, opacity_scale=1.3, sh_order=3,
+                                      cutouts=[(box, 1)], deleted_bits=deleted, splat_count=asset.splatCount)
 
 
 def key_case(quality):
-    """(asset, (fp, keep), order): CSCalcDistances through a random permutation."""
+    """(asset, (fp, keep), order): CSCalcDistances through a random permutation ("pose-<name>": the Medium scene from that pose)."""
     import unitygaussiansplatting_b200 as g
     from util import camera, case_asset, format_case
+    if quality.startswith("pose-"):
+        asset = g.synthetic_asset(g.SCENE_CLUSTERED, KEY_N, 0x5EED0092, "Medium")
+        order = np.random.default_rng(1).permutation(KEY_N).astype(np.uint32)
+        return asset, g.make_frame_params(pose_camera(g, quality[len("pose-"):])), order
     if quality.startswith("custom-"):
         asset = case_asset(g, format_case(quality[len("custom-"):]), KEY_N, 0x5EED0092)
     else:
@@ -138,9 +161,9 @@ def rotation_quats():
     return np.array(out, np.float32)
 
 
-CASES = (["gpu_" + q.lower() for q in QUALITIES] + ["view_" + q.lower() for q in VIEW_QUALITIES] +
-         ["keys_" + q.lower() for q in KEY_QUALITIES] + ["export", "draw", "draw_selected", "rotation"])
-_NAMES = {q.lower(): q for q in VIEW_QUALITIES + KEY_QUALITIES}
+CASES = (["gpu_" + q.lower() for q in QUALITIES] + ["view_" + q.lower() for q in VIEW_QUALITIES + VIEW_POSES] +
+         ["keys_" + q.lower() for q in KEY_QUALITIES + KEY_POSES] + ["export", "draw", "draw_selected", "rotation"])
+_NAMES = {q.lower(): q for q in VIEW_QUALITIES + KEY_QUALITIES + VIEW_POSES + KEY_POSES}
 
 
 def compute(name):
@@ -153,7 +176,7 @@ def compute(name):
                 "keys": O.ref_calc_distances(asset, fp, np.arange(N, dtype=np.uint32)), "asset_sha256": digest}
     if kind == "view":
         asset, (fp, _keep) = view_case(_NAMES[q])
-        return {"idx": np.arange(N, dtype=np.uint32), "view": O.ref_calc_view(asset, fp), "asset_sha256": asset_digest(asset)}
+        return {"idx": np.arange(asset.splatCount, dtype=np.uint32), "view": O.ref_calc_view(asset, fp), "asset_sha256": asset_digest(asset)}
     if kind == "keys":
         asset, (fp, _keep), order = key_case(_NAMES[q])
         # CSCalcDistances reads positions only, and the compiled reference refuses a BC7 asset as a whole: call it Norm8x4
@@ -198,7 +221,7 @@ def stored(name):
     d = compute(name)
     kind = name.partition("_")[0]
     k = {"gpu": SAMPLE, "view": VIEW_SAMPLE, "keys": KEY_SAMPLE, "export": EXPORT_SAMPLE}.get(kind)
-    if k is None:
+    if k is None or k >= len(d["idx"]):
         return d
     idx = sample_ids(len(d["idx"]), k, SAMPLE_SEED if kind == "gpu" else SAMPLE_SEED + 1)
     return {key: (v if key == "asset_sha256" else v[idx]) for key, v in d.items()}

@@ -35,7 +35,7 @@ def _same_asset(asset, want):
     assert np.array_equal(M.asset_digest(asset), want["asset_sha256"]), "the scene is no longer the one the reference output is for"
 
 
-@pytest.mark.parametrize("quality", M.VIEW_QUALITIES)
+@pytest.mark.parametrize("quality", M.VIEW_QUALITIES + M.VIEW_POSES)
 def test_view_data_matches_the_reference_shader_code(O, quality):
     asset, (fp, _keep) = M.view_case(quality)
     want = M.reference("view_" + quality.lower())
@@ -58,7 +58,7 @@ def test_view_data_matches_the_reference_shader_code(O, quality):
     assert np.percentile(rel, 50) < 1e-6 and np.percentile(rel, 99) < 2e-5 and rel.max() < 2e-3
 
 
-@pytest.mark.parametrize("quality", M.KEY_QUALITIES)
+@pytest.mark.parametrize("quality", M.KEY_QUALITIES + M.KEY_POSES)
 def test_sort_keys_match_the_reference_shader_code(O, quality):
     asset, (fp, _keep), order = M.key_case(quality)
     want = M.reference("keys_" + quality.lower())

@@ -4,10 +4,150 @@ from collections import namedtuple
 
 import numpy as np
 
+from unitygaussiansplatting_b200.camera import Camera
+
 
 def camera(g, width=256, height=256, fov=39.09651, pos=(0.0, 0.5, -6.0), forward=(0.0, 0.0, 1.0)):
     return g.Camera(position=np.array(pos, np.float64), rotation=g.look_rotation(forward), fieldOfView=fov, pixelWidth=width,
                     pixelHeight=height)
+
+
+@dataclasses.dataclass
+class ProjCamera(Camera):
+    """A Camera whose projectionMatrix is a given OpenGL-style 4x4 (`proj`) instead of the symmetric perspective of
+    fieldOfView / aspect.  make_frame_params, SortAndRenderCameras and the group calls all read cam.gpuProjectionMatrix(True),
+    so the matrix reaches every entry point unchanged."""
+    proj: np.ndarray = None
+
+    @property
+    def projectionMatrix(self) -> np.ndarray:
+        return np.asarray(self.proj, np.float32)
+
+
+def with_projection(cam, proj):
+    """`cam` (pose, clip planes, screen) with the OpenGL-style projection `proj`."""
+    fields = {f.name: getattr(cam, f.name) for f in dataclasses.fields(Camera)}
+    return ProjCamera(**fields, proj=np.asarray(proj, np.float64))
+
+
+def off_axis(cam, l, r, b, t):
+    """glFrustum from the near-plane extents (l, r, b, t) at cam.nearClipPlane: an XR eye's projection (P[0,2], P[1,2] != 0)."""
+    n, f = cam.nearClipPlane, cam.farClipPlane
+    P = np.array([[2 * n / (r - l), 0, (r + l) / (r - l), 0], [0, 2 * n / (t - b), (t + b) / (t - b), 0],
+                  [0, 0, -(f + n) / (f - n), -2 * f * n / (f - n)], [0, 0, -1, 0]], np.float64)
+    return with_projection(cam, P)
+
+
+def oblique(cam, plane):
+    """Camera.CalculateObliqueMatrix: the near plane of cam's projection replaced by `plane` (a, b, c, d), a camera-space
+    plane with the camera on its negative side, as a planar-reflection camera uses it (Lengyel's construction)."""
+    P = np.asarray(cam.projectionMatrix, np.float64)
+    c = np.asarray(plane, np.float64)
+    q = np.linalg.inv(P) @ np.array([np.sign(c[0]), np.sign(c[1]), 1.0, 1.0])
+    c = c * (2.0 / (c @ q))
+    P = P.copy()
+    P[2] = c - P[3]
+    return with_projection(cam, P)
+
+
+def mirrored(cam):
+    """P diag(-1, 1, 1, 1): a mirror camera's projection (x flipped, so p00 < 0)."""
+    return with_projection(cam, np.asarray(cam.projectionMatrix, np.float64) @ np.diag([-1.0, 1.0, 1.0, 1.0]))
+
+
+def orthographic(cam, half_height):
+    """glOrtho of `half_height` world units up and down (and the screen's aspect across) between cam's clip planes: clip.w
+    is 1 everywhere, so no splat is behind the camera and only the view depth tells the chunk cull where the camera plane is."""
+    n, f, hw = cam.nearClipPlane, cam.farClipPlane, half_height * cam.aspect
+    return with_projection(cam, [[1 / hw, 0, 0, 0], [0, 1 / half_height, 0, 0], [0, 0, -2 / (f - n), -(f + n) / (f - n)], [0, 0, 0, 1]])
+
+
+def rolled(cam, deg):
+    """`cam` turned by `deg` degrees about its own view axis."""
+    a = np.radians(deg)
+    rz = np.array([[np.cos(a), -np.sin(a), 0], [np.sin(a), np.cos(a), 0], [0, 0, 1]], np.float64)
+    return dataclasses.replace(cam, rotation=np.asarray(cam.rotation, np.float64) @ rz)
+
+
+# Camera poses XR and walk-through users render, at screens the oracle draws quickly (tests/test_gpu_camera_poses.py).
+# The clustered scene has its clusters in [-8, 8] x [-2, 3] x [-8, 8] and a shell of splats at radius 8..30, so every "inside"
+# pose is among the splats; `inside-near` looks at the cluster next to it.
+XR_EYE = (-1.4, 0.9, -1.2, 1.1)        # near-plane extents / n of the left eye; the right eye is its mirror image
+
+
+def xr_eye(g, eye, width=256, height=256, pos=(0.3, 0.4, -1.0), forward=(0.2, -0.1, 1.0), ipd=0.064):
+    """The left (eye 0) or right (eye 1) eye of a head at `pos`: an off-axis frustum about 97 degrees across each way."""
+    l, r, b, t = XR_EYE
+    if eye:
+        l, r = -r, -l
+    head = camera(g, width, height, pos=pos, forward=forward)
+    right = np.asarray(head.rotation, np.float64)[:, 0]
+    c = dataclasses.replace(head, position=np.asarray(pos, np.float64) + (eye - 0.5) * ipd * right)
+    n = c.nearClipPlane
+    return off_axis(c, l * n, r * n, b * n, t * n)
+
+
+def _poses():
+    def inside(forward, pos=(0.0, 0.5, 0.0), width=256, height=256, fov=90.0):
+        return lambda g: camera(g, width, height, fov=fov, pos=pos, forward=forward)
+
+    return {
+        "inside-z": inside((0.0, 0.0, 1.0)),
+        "inside-back": inside((0.0, 0.0, -1.0)),
+        "inside-near": inside((0.45, -0.35, 0.8), pos=(-1.3, 0.4, 1.6)),
+        "xr-left": lambda g: xr_eye(g, 0),
+        "xr-right": lambda g: xr_eye(g, 1),
+        "roll-30": lambda g: rolled(camera(g, 320, 240, pos=(0.4, 0.8, -5.0), forward=(-0.1, -0.1, 1.0)), 30.0),
+        "roll-90": lambda g: rolled(camera(g, 320, 240, pos=(0.4, 0.8, -5.0), forward=(-0.1, -0.1, 1.0)), 90.0),
+        "roll-180": lambda g: rolled(camera(g, 320, 240, pos=(0.4, 0.8, -5.0), forward=(-0.1, -0.1, 1.0)), 180.0),
+        "fov-110": lambda g: camera(g, 320, 240, fov=110.0, pos=(0.0, 0.5, -3.0)),
+        "fov-3": lambda g: camera(g, 320, 240, fov=3.0, pos=(0.0, 0.5, -20.0), forward=(0.05, 0.0, 1.0)),
+        "portrait": lambda g: camera(g, 240, 320, fov=60.0, pos=(0.5, 0.5, -4.0)),
+        "strip-wide": lambda g: camera(g, 1024, 64, fov=12.0, pos=(0.0, 0.5, -6.0)),
+        "strip-tall": lambda g: camera(g, 64, 1024, fov=90.0, pos=(0.0, 0.5, -6.0)),
+        "mirrored": lambda g: mirrored(camera(g, 320, 240, fov=60.0, pos=(0.6, 0.7, -4.5), forward=(-0.15, -0.05, 1.0))),
+        "ortho-inside": lambda g: orthographic(camera(g, 256, 256, pos=(0.0, 0.5, 0.0), forward=(1.0, 0.0, 0.2)), 1.0),
+        "oblique": lambda g: oblique(camera(g, 320, 240, fov=60.0, pos=(0.0, 1.5, -5.0), forward=(0.0, -0.2, 1.0)),
+                                     (0.0, 0.35, -0.94, -2.5)),
+    }
+
+
+POSES = _poses()
+
+# The near-plane scene: splats at view depths NEAR_DEPTHS whose centres lie NEAR_OFFSETS pixels outside each edge of the
+# screen -- across the 11,880 px far_off reach of a clamped quad (quad_reach of an unbounded footprint), the 4096 px axis
+# clamp, and the 1e7 px no-raster cut-off of splat_footprint.
+NEAR_DEPTHS = (1e-3, -1e-3, 1e-6, -1e-6, 0.0)
+NEAR_OFFSETS = (-20.0, 40.0, 3900.0, 4300.0, 11000.0, 12500.0, 9.8e6, 1.03e7)
+NEAR_SCALES = (0.002, 0.03, 0.4)
+
+
+def near_plane_camera(g):
+    """An XR left eye at the origin looking along +z: its view matrix is diag(1, 1, -1, 1), so view depth is world z exactly."""
+    return xr_eye(g, 0, 256, 256, pos=(0.0, 0.0, 0.0), forward=(0.0, 0.0, 1.0), ipd=0.0)
+
+
+def near_plane_scene(g, cam):
+    """VeryHigh asset of the near-plane scene seen by `cam` (near_plane_camera)."""
+    P = cam.gpuProjectionMatrix(True).astype(np.float64)
+    W, H = cam.pixelWidth, cam.pixelHeight
+    rng = np.random.default_rng(11)
+    pos, scale = [], []
+    for d in NEAR_DEPTHS:
+        a = abs(d) if d else 1e-3
+        for o in NEAR_OFFSETS:
+            for edge in range(4):
+                for s in NEAR_SCALES:
+                    t = rng.uniform(0.2, 0.8)
+                    px, py = ((-o, t * H), (W + o, t * H), (t * W, -o), (t * W, H + o))[edge]
+                    ndx, ndy = 2 * px / W - 1, 1 - 2 * py / H
+                    # clip = P (x, y, -a, 1): clip.w = a, clip.x = P00 x - P02 a, clip.y = P11 y - P12 a
+                    pos.append(((ndx + P[0, 2]) * a / P[0, 0], (ndy + P[1, 2]) * a / P[1, 1], d))
+                    scale.append((s, s * rng.uniform(0.05, 1.0), s * rng.uniform(0.05, 1.0)))
+    n = len(pos)
+    rec = splat_records(np.array(pos), np.array(scale), rng.uniform(0.3, 1.0, n), dc=rng.uniform(0, 1, (n, 3)),
+                        quat=rng.standard_normal((n, 4)))
+    return g.create_asset(rec, "VeryHigh")
 
 
 def lattice_camera(g, width=256, height=256):
