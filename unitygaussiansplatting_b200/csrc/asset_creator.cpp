@@ -6,9 +6,13 @@
 // over one contiguous record array, not a translation of the Burst job structs.
 //
 // Third-party arithmetic that is not in /root/reference: Unity.Mathematics 1.2.6
-// (package/package.json:3) math.f32tof16 / math.pow.  f32tof16 is restated below from its
-// published source (truncate the low 12 mantissa bits, add half, shift; i.e. round half
-// up on bit 12); pow(float,float) is System.Math.Pow in double, narrowed to float.
+// (package/package.json:3) math.f32tof16 / math.pow / math.min / math.max / math.saturate.
+// f32tof16 is restated below from its published source (truncate the low 12 mantissa bits,
+// add half, shift; i.e. round half up on bit 12); pow(float,float) is System.Math.Pow in
+// double, narrowed to float; min / max return their second operand unless the first wins
+// strictly or the second is NaN, so saturate(NaN) = max(0, min(1, NaN)) = 1.
+// oracle/refcs/ compiles the reference's own C# against these semantics and
+// tests/test_reference_cs.py compares this file's bytes with it.
 #include "../../include/gsplat_asset.h"
 
 #include <algorithm>
@@ -71,7 +75,11 @@ inline uint32_t unity_f32tof16(float x) {
   return h | ((ux & ~msk) >> 16);
 }
 
-inline float saturate(float v) { return v < 0.0f ? 0.0f : (v > 1.0f ? 1.0f : v); }
+// Unity.Mathematics math.min / max / saturate (see file header): of two equal values (+0 / -0) the second is kept, a NaN
+// second operand is ignored.  Every min / max fold of the importer (bounds, chunk ranges) goes through these.
+inline float unity_min(float x, float y) { return (std::isnan(y) || x < y) ? x : y; }
+inline float unity_max(float x, float y) { return (std::isnan(y) || x > y) ? x : y; }
+inline float saturate(float v) { return unity_max(0.0f, unity_min(1.0f, v)); }   // clamp(v, 0, 1); NaN -> 1
 
 // R/GaussianUtils.cs:25-30
 inline float square_centered01(float x) {
@@ -309,8 +317,8 @@ int gsa_create_asset(GsaInputSplat *splats, uint32_t n, uint32_t pf, uint32_t sf
   float bmin[3] = {INFINITY, INFINITY, INFINITY}, bmax[3] = {-INFINITY, -INFINITY, -INFINITY};
   for (uint32_t i = 0; i < n; ++i)
     for (int k = 0; k < 3; ++k) {
-      bmin[k] = std::min(bmin[k], splats[i].pos[k]);
-      bmax[k] = std::max(bmax[k], splats[i].pos[k]);
+      bmin[k] = unity_min(bmin[k], splats[i].pos[k]);
+      bmax[k] = unity_max(bmax[k], splats[i].pos[k]);
     }
   if (bounds_out) { std::memcpy(bounds_out, bmin, 12); std::memcpy(bounds_out + 3, bmax, 12); }
 
@@ -374,21 +382,21 @@ int gsa_create_asset(GsaInputSplat *splats, uint32_t n, uint32_t pf, uint32_t sf
         s.opacity = square_centered01(s.opacity);
         float col[4] = {s.dc0[0], s.dc0[1], s.dc0[2], s.opacity};
         for (int k = 0; k < 3; ++k) {
-          mnp[k] = std::min(mnp[k], s.pos[k]); mxp[k] = std::max(mxp[k], s.pos[k]);
-          mns[k] = std::min(mns[k], s.scale[k]); mxs[k] = std::max(mxs[k], s.scale[k]);
+          mnp[k] = unity_min(mnp[k], s.pos[k]); mxp[k] = unity_max(mxp[k], s.pos[k]);
+          mns[k] = unity_min(mns[k], s.scale[k]); mxs[k] = unity_max(mxs[k], s.scale[k]);
         }
-        for (int k = 0; k < 4; ++k) { mnc[k] = std::min(mnc[k], col[k]); mxc[k] = std::max(mxc[k], col[k]); }
+        for (int k = 0; k < 4; ++k) { mnc[k] = unity_min(mnc[k], col[k]); mxc[k] = unity_max(mxc[k], col[k]); }
         for (int j = 0; j < 15; ++j)
           for (int k = 0; k < 3; ++k) {
-            mnh[k] = std::min(mnh[k], s.sh[j * 3 + k]); mxh[k] = std::max(mxh[k], s.sh[j * 3 + k]);
+            mnh[k] = unity_min(mnh[k], s.sh[j * 3 + k]); mxh[k] = unity_max(mxh[k], s.sh[j * 3 + k]);
           }
       }
       for (int k = 0; k < 3; ++k) {
-        mxp[k] = std::max(mxp[k], mnp[k] + 1.0e-5f);
-        mxs[k] = std::max(mxs[k], mns[k] + 1.0e-5f);
-        mxh[k] = std::max(mxh[k], mnh[k] + 1.0e-5f);
+        mxp[k] = unity_max(mxp[k], mnp[k] + 1.0e-5f);
+        mxs[k] = unity_max(mxs[k], mns[k] + 1.0e-5f);
+        mxh[k] = unity_max(mxh[k], mnh[k] + 1.0e-5f);
       }
-      for (int k = 0; k < 4; ++k) mxc[k] = std::max(mxc[k], mnc[k] + 1.0e-5f);
+      for (int k = 0; k < 4; ++k) mxc[k] = unity_max(mxc[k], mnc[k] + 1.0e-5f);
       ChunkInfo info;
       info.posX[0] = mnp[0]; info.posX[1] = mxp[0];
       info.posY[0] = mnp[1]; info.posY[1] = mxp[1];
@@ -643,8 +651,9 @@ static int ply_read_impl(const char *path, GsaInputSplat *out, uint32_t capacity
     std::memcpy(&s, d, sizeof(s));
     // LinearizeData (:207-232): rot_0..3 = (w,x,y,z) -> normalise -> (x,y,z,w) -> smallest-three
     float q[4] = {s.rot[0], s.rot[1], s.rot[2], s.rot[3]};
-    const float len = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-    const float qn[4] = {q[1] / len, q[2] / len, q[3] / len, q[0] / len};  // math.normalize(wxyz).yzwx
+    // math.normalize(wxyz).yzwx: rsqrt(dot(q, q)) * q, a multiply by the reciprocal length, not a divide
+    const float rlen = 1.0f / std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+    const float qn[4] = {rlen * q[1], rlen * q[2], rlen * q[3], rlen * q[0]};
     pack_smallest3(qn, s.rot);
     for (int k = 0; k < 3; ++k) s.scale[k] = std::fabs(std::exp(s.scale[k]));      // LinearScale
     for (int k = 0; k < 3; ++k) s.dc0[k] = s.dc0[k] * 0.2820948f + 0.5f;           // SH0ToColor

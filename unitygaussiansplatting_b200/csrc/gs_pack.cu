@@ -81,15 +81,21 @@ __device__ __forceinline__ uint32_t d_pcg_hash(uint32_t input) {
   return (word >> 22) ^ word;
 }
 
-// ---- ordered reductions: the result of a sequential std::min / std::max fold -------------------------------------------
-// b replaces a when it is strictly smaller (larger), or equal and earlier.  NaN never enters a reduction (see take()).
+// ---- ordered reductions: the result of a sequential Unity.Mathematics math.min / math.max fold ------------------------
+// `acc = math.min(acc, x)` keeps acc only when acc < x strictly (or x is NaN): of equal values (+0 / -0) the LATER one wins.
+// So b replaces a when it is strictly smaller (larger), or equal and later.  NaN never enters a reduction (see take()).
+template <bool MAX>
+__device__ __forceinline__ bool fold_better(float bv, uint32_t bi, float av, uint32_t ai) {
+  return (MAX ? (av < bv) : (bv < av)) || (bv == av && bi > ai);
+}
+// k-means' nearest mean: strictly smaller, or equal and earlier (the first of equal distances wins)
 template <bool MAX>
 __device__ __forceinline__ bool better(float bv, uint32_t bi, float av, uint32_t ai) {
   return (MAX ? (av < bv) : (bv < av)) || (bv == av && bi < ai);
 }
 template <bool MAX>
 __device__ __forceinline__ void take(float &v, uint32_t &i, float x, uint32_t xi) {   // one step of the fold
-  if (MAX ? (v < x) : (x < v)) { v = x; i = xi; }
+  if (!isnan(x) && (MAX ? !(v > x) : !(v < x))) { v = x; i = xi; }
 }
 template <bool MAX>
 __device__ __forceinline__ void warp_reduce(float &v, uint32_t &i) {
@@ -97,7 +103,7 @@ __device__ __forceinline__ void warp_reduce(float &v, uint32_t &i) {
   for (int o = 16; o; o >>= 1) {
     const float ov = __shfl_xor_sync(0xffffffffu, v, o);
     const uint32_t oi = __shfl_xor_sync(0xffffffffu, i, o);
-    if (better<MAX>(ov, oi, v, i)) { v = ov; i = oi; }
+    if (fold_better<MAX>(ov, oi, v, i)) { v = ov; i = oi; }
   }
 }
 // block of 256 threads; every thread gets the result.  `sv` / `si`: 8 entries of shared scratch
@@ -110,7 +116,7 @@ __device__ void block_reduce(float &v, uint32_t &i, float *sv, uint32_t *si) {
   __syncthreads();
   v = sv[0]; i = si[0];
   for (int k = 1; k < (int)(blockDim.x >> 5); ++k)
-    if (better<MAX>(sv[k], si[k], v, i)) { v = sv[k]; i = si[k]; }
+    if (fold_better<MAX>(sv[k], si[k], v, i)) { v = sv[k]; i = si[k]; }
 }
 
 // ---- 1. bounds (E/...:361-385) ---------------------------------------------------------------------------------------------
@@ -145,7 +151,7 @@ __global__ void __launch_bounds__(256) k_bounds_final(const float *part_v, const
     for (uint32_t p = threadIdx.x; p < parts; p += blockDim.x) {
       const float pv = part_v[p * 6 + q];
       const uint32_t pi = part_i[p * 6 + q];
-      if (q < 3 ? better<false>(pv, pi, v, i) : better<true>(pv, pi, v, i)) { v = pv; i = pi; }
+      if (q < 3 ? fold_better<false>(pv, pi, v, i) : fold_better<true>(pv, pi, v, i)) { v = pv; i = pi; }
     }
     if (q < 3) block_reduce<false>(v, i, sv, si); else block_reduce<true>(v, i, sv, si);
     if (threadIdx.x == 0) bounds[q] = v;
@@ -470,7 +476,11 @@ __device__ __forceinline__ float square_centered01(float x) {
   x *= x * sgn;
   return x * 2.0f + 0.5f;
 }
-__device__ __forceinline__ float maxf_host(float a, float b) { return (a < b) ? b : a; }   // std::max(a, b)
+__device__ __forceinline__ float unity_max(float x, float y) { return (isnan(y) || x > y) ? x : y; }   // math.max(x, y)
+
+// a / b as an x86 host computes it: a chunk whose range is 0 (|min| >= 256, where min + 1e-5 rounds back to min) divides
+// 0 by 0, and the NaN that writes into Float32 / Float16 blobs is x86's default NaN 0xFFC00000, not the GPU's 0x7FFFFFFF
+__device__ __forceinline__ float host_div(float a, float b) { const float q = a / b; return isnan(q) ? __uint_as_float(0xFFC00000u) : q; }
 
 // One CTA per 256 splats: min/max of position, scale^(1/8), colour (dc0, square_centered01(opacity)) and the 15 SH
 // coefficients per channel, ChunkInfo, then every value normalised to its chunk range.
@@ -502,7 +512,7 @@ __global__ void __launch_bounds__(256) k_chunks(float *rec, uint32_t n, Chunk *c
     }
     block_reduce<false>(mn, imn, sv, si);
     block_reduce<true>(mx, imx, sv, si);
-    if (t == 0) { s_mn[q] = mn; s_mx[q] = maxf_host(mx, mn + 1.0e-5f); }
+    if (t == 0) { s_mn[q] = mn; s_mx[q] = unity_max(mx, mn + 1.0e-5f); }
   }
   __syncthreads();
   if (t == 0) {
@@ -524,20 +534,21 @@ __global__ void __launch_bounds__(256) k_chunks(float *rec, uint32_t n, Chunk *c
   }
   if (!live) return;
   for (int k = 0; k < 3; ++k) {
-    s[k] = (s[k] - s_mn[k]) / (s_mx[k] - s_mn[k]);
-    s[kOffScale + k] = (s[kOffScale + k] - s_mn[3 + k]) / (s_mx[3 + k] - s_mn[3 + k]);
-    s[kOffDc0 + k] = (s[kOffDc0 + k] - s_mn[6 + k]) / (s_mx[6 + k] - s_mn[6 + k]);
+    s[k] = host_div(s[k] - s_mn[k], s_mx[k] - s_mn[k]);
+    s[kOffScale + k] = host_div(s[kOffScale + k] - s_mn[3 + k], s_mx[3 + k] - s_mn[3 + k]);
+    s[kOffDc0 + k] = host_div(s[kOffDc0 + k] - s_mn[6 + k], s_mx[6 + k] - s_mn[6 + k]);
   }
-  s[kOffOpacity] = (s[kOffOpacity] - s_mn[9]) / (s_mx[9] - s_mn[9]);
+  s[kOffOpacity] = host_div(s[kOffOpacity] - s_mn[9], s_mx[9] - s_mn[9]);
   for (int j = 0; j < 15; ++j)
-    for (int k = 0; k < 3; ++k) s[kOffSh + j * 3 + k] = (s[kOffSh + j * 3 + k] - s_mn[10 + k]) / (s_mx[10 + k] - s_mn[10 + k]);
+    for (int k = 0; k < 3; ++k) s[kOffSh + j * 3 + k] = host_div(s[kOffSh + j * 3 + k] - s_mn[10 + k], s_mx[10 + k] - s_mn[10 + k]);
 }
 
 // ---- 5. emit (E/...:705-1066) ---------------------------------------------------------------------------------------------
 // Every record stride of `other` is even but not always a multiple of 4: all stores are 16-bit.
 __device__ __forceinline__ void put16(uint8_t *p, uint32_t v) { *(uint16_t *)p = (uint16_t)v; }
 __device__ __forceinline__ void put32(uint8_t *p, uint32_t v) { put16(p, v & 0xffffu); put16(p + 2, v >> 16); }
-__device__ __forceinline__ float sat(float v) { return v < 0.0f ? 0.0f : (v > 1.0f ? 1.0f : v); }
+// math.saturate = max(0, min(1, v)) with math.min / max: NaN -> 1 (a chunk whose range is 0 / 0)
+__device__ __forceinline__ float sat(float v) { const float m = (isnan(v) || 1.0f < v) ? 1.0f : v; return (0.0f > m) ? 0.0f : m; }
 __device__ __forceinline__ uint32_t enc_norm11(const float *v) {
   return (uint32_t)(v[0] * 2047.5f) | ((uint32_t)(v[1] * 1023.5f) << 11) | ((uint32_t)(v[2] * 2047.5f) << 21);
 }
