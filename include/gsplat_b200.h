@@ -118,8 +118,13 @@ typedef struct GsFrameParams {
                                      eye-depth array.  Texel (x, y) of the array (layer) is the depth of pixel (x, y), read in place.
                                      Another channel format is GS_ERR_UNSUPPORTED_FORMAT; any other mismatch, a null array, or a
                                      layered array passed as 2 (a 2-D one as 4) is GS_ERR_INVALID_ARGUMENT, refused before anything
-                                     is enqueued.  The group entry points (gs_group_*) refuse 2 and 4 (GS_ERR_INVALID_ARGUMENT).
-                                     Any other value: device memory, used in place. */
+                                     is enqueued.  GS_MEM_ARRAY_RECT (5): scene_depth points to a borrowed GsArrayRect over a
+                                     2-D or layered array of one 32-bit float channel made with cudaArraySurfaceLoadStore; the
+                                     rectangle is screen_w x screen_h at (x, y) and must lie inside the array, and texel
+                                     (x + px, y + py) of the layer is the depth of pixel (px, py) -- e.g. the camera's depth in
+                                     an HDRP RTHandle allocated larger than the camera.  The group entry points (gs_group_*)
+                                     refuse 2, 4 and 5 (GS_ERR_INVALID_ARGUMENT).
+                                     Any other value (1, 3, 6, ...): device memory, used in place. */
   uint32_t reserved1;
 } GsFrameParams;
 
@@ -158,12 +163,36 @@ typedef struct GsArrayLayer {
   uint32_t reserved;
 } GsArrayLayer;
 
+/* GS_MEM_ARRAY_RECT (images only): `data` points to a GsArrayRect, a host descriptor borrowed for the call, that names a
+ * width x height rectangle of a 2-D CUDA array or of one layer of a layered one.  Pixel (px, py) of the image is texel
+ * (x + px, y + py) of the layer; the texels outside the rectangle, and the other layers, are not touched.  Two uses:
+ *   - a render target larger than the camera: HDRP allocates its RTHandles at the largest size any camera has needed, and each
+ *     camera draws into the rectangle at the texture's origin, at its (dynamically scaled) pixel size: GsArrayRect{array, 0, 0, 0,
+ *     0} with that size as the image's width x height and as screen_w x screen_h;
+ *   - several views in one texture (split screen, impostor or probe atlases, the quilt of a light-field display): one
+ *     rectangle per camera of gs_frame_cameras, which draws disjoint rectangles of one array in one camera run.
+ * Whether the array is 2-D or layered is read from it (cudaArrayGetInfo).  The rules of GS_MEM_ARRAY apply (channel format,
+ * cudaArraySurfaceLoadStore, row_pitch_bytes 0, not accepted as band_packed or gs_unshuffle_bands output), except for the
+ * extent: the rectangle must lie inside the array.  GS_ERR_INVALID_ARGUMENT, before anything is enqueued: a null array,
+ * `reserved` not 0, a nonzero `layer` of a 2-D array, a layer not below a layered array's layer count, a 3-D array that is not
+ * layered, a rectangle that does not lie inside the array.  A camera's rt and camera target must not overlap (the library
+ * does not check this, as for whole arrays).  Memory kinds 3 and above 5 are not defined (GS_ERR_INVALID_ARGUMENT). */
+#define GS_MEM_ARRAY_RECT 5u
+typedef struct GsArrayRect {
+  void *array;       /* a 2-D or layered cudaArray_t (mip level 0) on the context's device */
+  uint32_t layer;    /* 0 for a 2-D array; below the layer count of a layered one */
+  uint32_t x, y;     /* texel of the array that holds pixel (0, 0) of the image */
+  uint32_t reserved; /* 0 */
+} GsArrayRect;       /* 24 bytes */
+
 typedef struct GsImage {
-  void *data;                /* host pointer, device pointer, cudaArray_t (GS_MEM_ARRAY) or GsArrayLayer * (GS_MEM_ARRAY_LAYER) */
+  void *data;                /* host pointer, device pointer, cudaArray_t (GS_MEM_ARRAY), GsArrayLayer * (GS_MEM_ARRAY_LAYER) or
+                                GsArrayRect * (GS_MEM_ARRAY_RECT) */
   uint32_t width, height;
-  uint32_t row_pitch_bytes;  /* 0 = tightly packed (and always 0 for GS_MEM_ARRAY / GS_MEM_ARRAY_LAYER) */
+  uint32_t row_pitch_bytes;  /* 0 = tightly packed (and always 0 for the CUDA-array kinds 2, 4 and 5) */
   uint32_t format;           /* GsPixelFormat */
-  uint32_t memory;           /* GsMemory or GS_MEM_ARRAY_LAYER: where `data` lives; any other value is GS_ERR_INVALID_ARGUMENT */
+  uint32_t memory;           /* GsMemory, GS_MEM_ARRAY_LAYER or GS_MEM_ARRAY_RECT: where `data` lives; any other value is
+                                GS_ERR_INVALID_ARGUMENT */
 } GsImage;
 
 /* How the render-target blend is evaluated.
@@ -287,7 +316,7 @@ GS_API int gs_frame(GsContext *ctx, GsAsset *asset, const GsFrameParams *fp,
  * Per object, in order, on the context stream: the sort (when do_sort[k]) and the view-calc, as gs_frame.  Then consecutive
  * objects are drawn together as one run: their bin-list entries go into one list, object after object, which is sorted once
  * by bin id and drawn by one raster pass.  A run holds at most 16 objects, each with fewer than 2^28 splats, binding at most
- * one scene depth buffer (the same scene_depth pointer and memory); a new run starts where one of these would break, and
+ * one scene depth buffer (the same scene_depth pointer and memory; for CUDA arrays the same array, layer and rectangle); a new run starts where one of these would break, and
  * blends under what the earlier runs drew.  Any object count is accepted.  A run of one object (with one object: the whole
  * call) does the device work of gs_frame.  The bin-list capacity of a run is clamp(8 x its summed splat count, 4 Mi, 768 Mi)
  * entries; a run that needs more reports GS_ERR_OUT_OF_MEMORY as gs_frame does (at gs_sync when nothing is read back to the
@@ -326,7 +355,9 @@ GS_API int gs_frame_objects(GsContext *ctx, uint32_t object_count, GsAsset *cons
  * the run draws again are kept in a context scratch slab until the raster.  A run holds at most 16 (camera, object) pairs,
  * each object under 2^28 splats, cameras of at most 8160 px per axis and 65536 64-pixel bins in all, at most one scene depth
  * buffer per camera, and one render-target pixel format (RGBA16F for a camera without rt).  A camera whose rt or camera
- * target is the render target of an earlier camera of the run starts a new run.  A camera that breaks a limit of its own (a
+ * target is the render target of an earlier camera of the run starts a new run; for CUDA arrays "is" means the same array
+ * and layer with overlapping rectangles (a whole array or layer overlaps every rectangle of it), so cameras drawing into
+ * disjoint GS_MEM_ARRAY_RECT tiles of one array share a run.  A camera that breaks a limit of its own (a
  * larger screen, more objects or splats, two depth buffers), and a camera that ends up alone in its run, is drawn by
  * gs_frame_objects' own work, large screens' bin-list growth included.  A run's bin-list capacity is
  * clamp(8 x its summed splats over all pairs, 4 Mi, 768 Mi) entries; overflow is reported as gs_frame_objects reports it

@@ -32,12 +32,21 @@ namespace GaussianSplatting.Runtime
             public GaussianSplatNative.GsImage rt, camera_target;
         }
 
+        // include/gsplat_b200.h: a rectangle of a 2-D CUDA array or of one layer of a layered one (GS_MEM_ARRAY_RECT = 5), 24 bytes
+        [StructLayout(LayoutKind.Sequential)]
+        internal struct GsArrayRect
+        {
+            public IntPtr array;
+            public uint layer, x, y, reserved;
+        }
+
         [DllImport("gsplat_b200")] static extern IntPtr gs_unity_get_render_event_func();
         [DllImport("gsplat_b200")] static extern uint gs_unity_frame_event_size();
 
         const int kEventFrame = 1;                                  // GS_UNITY_EVENT_FRAME
         internal const int kInFlight = 3;                                   // command buffers may execute up to 2 frames late
         NativeArray<GsUnityFrameEvent> m_Events;                    // persistent => stable address, no GC pinning needed
+        NativeArray<GsArrayRect> m_Rects;                           // each slot's rt rectangle (RecordRect), borrowed until its event has run
         // The reference binds _SplatCutouts / _SplatDeletedBits / _SplatSelectedBits on every CalcViewData (SetAssetDataOnCS,
         // R/GaussianSplatRenderer.cs:485-509).  The native frame takes them as HOST arrays borrowed until the event has run,
         // so every in-flight slot owns its copies.  The bit arrays live in GraphicsBuffers in the reference (edited by compute
@@ -53,11 +62,13 @@ namespace GaussianSplatting.Runtime
             if (gs_unity_frame_event_size() != (uint)UnsafeUtility.SizeOf<GsUnityFrameEvent>())
                 throw new InvalidOperationException("GsUnityFrameEvent layout mismatch between C# and libgsplat_b200");
             m_Events = new NativeArray<GsUnityFrameEvent>(kInFlight, Allocator.Persistent);
+            m_Rects = new NativeArray<GsArrayRect>(kInFlight, Allocator.Persistent);
         }
 
         public void Dispose()
         {
             if (m_Events.IsCreated) m_Events.Dispose();
+            if (m_Rects.IsCreated) m_Rects.Dispose();
             for (int i = 0; i < kInFlight; ++i)
             {
                 if (m_Cutouts[i].IsCreated) m_Cutouts[i].Dispose();
@@ -104,6 +115,21 @@ namespace GaussianSplatting.Runtime
             ++gs.m_FrameCounter;
             cmb.IssuePluginEventAndData(s_EventFunc, kEventFrame, (IntPtr)ev);
             m_Next = (m_Next + 1) % kInFlight;
+        }
+
+        /// As Record, into the rtWidth x rtHeight rectangle at the origin of a larger texture: HDRP's _GaussianSplatRT is an
+        /// RTHandle allocated at the largest size any camera has needed (INTEGRATION.md section 3, "HDRP"), and the camera draws
+        /// into its scaled pixel size at texel (0, 0).  `rtArray` is that texture's import, redone when the RTHandle grows.
+        public void RecordRect(CommandBuffer cmb, GaussianSplatRenderer gs, Camera cam, IntPtr ctx, IntPtr asset, IntPtr rtArray,
+                               int rtWidth, int rtHeight, NativeArray<uint> hostDeletedBits = default, NativeArray<uint> hostSelectedBits = default)
+        {
+            int slot = m_Next;
+            var rect = (GsArrayRect*)m_Rects.GetUnsafePtr() + slot;
+            *rect = new GsArrayRect { array = rtArray, layer = 0, x = 0, y = 0, reserved = 0 };
+            Record(cmb, gs, cam, ctx, asset, rtArray, rtWidth, rtHeight, hostDeletedBits, hostSelectedBits);
+            var ev = (GsUnityFrameEvent*)m_Events.GetUnsafePtr() + slot;
+            ev->rt.data = rect;
+            ev->rt.memory = 5;   // GS_MEM_ARRAY_RECT; the event has been recorded, but it reads its payload only when it runs
         }
 
         /// The renderer's uniforms for in-flight slot `slot`.  The cutouts and bits they point to are this object's copies for

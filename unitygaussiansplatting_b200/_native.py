@@ -17,6 +17,7 @@ GS_ERR_NO_DEVICE = -6
 GS_PIX_RGBA16F, GS_PIX_RGBA32F = 0, 1
 GS_MEM_HOST, GS_MEM_DEVICE, GS_MEM_ARRAY = 0, 1, 2
 GS_MEM_ARRAY_LAYER = 4
+GS_MEM_ARRAY_RECT = 5
 GS_BLEND_FP16_ROP, GS_BLEND_FP32 = 0, 1
 
 
@@ -56,6 +57,10 @@ class GsFrameParams(C.Structure):
 
 class GsArrayLayer(C.Structure):
     _fields_ = [("array", C.c_void_p), ("layer", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class GsArrayRect(C.Structure):
+    _fields_ = [("array", C.c_void_p), ("layer", C.c_uint32), ("x", C.c_uint32), ("y", C.c_uint32), ("reserved", C.c_uint32)]
 
 
 class GsImage(C.Structure):

@@ -722,9 +722,9 @@ static uint32_t run_end(GsAsset *const *assets, const GsFrameParams *fps, uint32
 }
 
 // The call's cameras as runs, in order.  Consecutive whole cameras share a run while each fits it, the run's totals hold, they
-// have one pixel format, and no camera's image is another's render target (two cameras rasterizing into one image at once
-// would race, where the loop draws one after the other).  A camera alone is split into runs of run_end, each later one
-// loading what the earlier ones drew.
+// have one pixel format, and no camera's image shares pixels with another's render target (two cameras rasterizing into one
+// image at once would race, where the loop draws one after the other; disjoint rectangles of one array do not).  A camera
+// alone is split into runs of run_end, each later one loading what the earlier ones drew.
 static std::vector<Run> form_runs(const std::vector<CameraArgs> &cams, GsAsset *const *assets, const GsFrameParams *fps) {
   auto whole = [&](uint32_t c) {
     const CameraArgs &a = cams[c];
@@ -733,11 +733,8 @@ static std::vector<Run> form_runs(const std::vector<CameraArgs> &cams, GsAsset *
   auto joins = [&](uint32_t c0, uint32_t c, uint32_t run_pairs, uint32_t run_bins) {
     const CameraArgs &a = cams[c];
     if (run_pairs + a.K > kRunObjects || run_bins + a.fcs[0].binsX * a.fcs[0].binsY > kMaxRunBins || a.rt_fmt != cams[c0].rt_fmt) return false;
-    for (uint32_t j = c0; j < c; ++j) {
-      const auto rj = image_id(cams[j].rt), tj = image_id(cams[j].tgt), ra = image_id(a.rt), ta = image_id(a.tgt);
-      if (a.rt && (ra == rj || ra == tj)) return false;
-      if (a.tgt && ta == rj) return false;
-    }
+    for (uint32_t j = c0; j < c; ++j)
+      if (images_overlap(a.rt, cams[j].rt) || images_overlap(a.rt, cams[j].tgt) || images_overlap(a.tgt, cams[j].rt)) return false;
     return true;
   };
   std::vector<Run> runs;

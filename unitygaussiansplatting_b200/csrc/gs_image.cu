@@ -10,45 +10,71 @@ namespace gs {
 
 uint32_t pix_bytes(uint32_t fmt) { return fmt == GS_PIX_RGBA16F ? 8u : 16u; }
 
-// The rules every CUDA array the library reads or writes keeps: `a` (a GS_MEM_ARRAY or GS_MEM_ARRAY_LAYER view: data and memory)
-// is a W x H 2-D array, or a layer below the layer count of a W x H layered one, made with cudaArraySurfaceLoadStore, whose
-// channels are `channels` x `bits`-bit float (else GS_ERR_UNSUPPORTED_FORMAT; everything else is GS_ERR_INVALID_ARGUMENT).
-// The messages start with `prefix`, and name the size `of` and the channels `format` expected.
+// The rules every CUDA array the library reads or writes keeps: `a` (a GS_MEM_ARRAY, GS_MEM_ARRAY_LAYER or GS_MEM_ARRAY_RECT view:
+// data and memory) is a W x H 2-D array, a layer below the layer count of a W x H layered one, or a W x H rectangle inside a
+// 2-D array or inside a layer of a layered one, made with cudaArraySurfaceLoadStore, whose channels are `channels` x
+// `bits`-bit float (else GS_ERR_UNSUPPORTED_FORMAT; everything else is GS_ERR_INVALID_ARGUMENT).  The messages start with
+// `prefix`, and name the size `of` and the channels `format` expected.
 static int array_ok(GsContext *ctx, const GsImage &a, uint32_t W, uint32_t H, int channels, int bits, const char *prefix, const char *of,
                     const char *format) {
   const std::string p(prefix);
-  const bool layered = a.memory == GS_MEM_ARRAY_LAYER;
+  const bool layered = a.memory == GS_MEM_ARRAY_LAYER, rect = a.memory == GS_MEM_ARRAY_RECT;
   if (layered) {
     const GsArrayLayer *d = static_cast<const GsArrayLayer *>(a.data);
     if (!d->array || d->reserved) return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "GsArrayLayer: array is null or reserved is not 0");
   }
+  if (rect) {
+    const GsArrayRect *d = static_cast<const GsArrayRect *>(a.data);
+    if (!d->array || d->reserved) return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "GsArrayRect: array is null or reserved is not 0");
+  }
   int32_t layer = -1;
+  uint32_t x = 0, y = 0;
   cudaChannelFormatDesc cd;
   cudaExtent ext;
   unsigned int flags = 0;
-  const cudaError_t e = cudaArrayGetInfo(&cd, &ext, &flags, image_array(&a, &layer));
+  const cudaError_t e = cudaArrayGetInfo(&cd, &ext, &flags, image_array(&a, &layer, &x, &y));
   if (e != cudaSuccess) { cudaGetLastError(); return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "not a CUDA array: " + cudaGetErrorString(e)); }
   const int want[4] = {bits, channels > 1 ? bits : 0, channels > 2 ? bits : 0, channels > 3 ? bits : 0};
   if (cd.f != cudaChannelFormatKindFloat || cd.x != want[0] || cd.y != want[1] || cd.z != want[2] || cd.w != want[3])
     return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, p + "the CUDA array's channel format does not match " + format);
-  if (!layered && (ext.width != W || ext.height != H || ext.depth != 0))
-    return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the CUDA array is not a 2-D array of " + of + " size");
-  if (layered && (ext.width != W || ext.height != H || !(flags & cudaArrayLayered)))
-    return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the CUDA array is not a layered array of " + of + " size");
-  if (layered && (uint32_t)layer >= ext.depth)
-    return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the layer is not below the CUDA array's layer count");
+  if (rect) {
+    const bool is_layered = (flags & cudaArrayLayered) != 0;
+    if (!is_layered && ext.depth != 0)
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the CUDA array is a 3-D array, not a 2-D or layered one");
+    if (!is_layered && layer != 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the layer of a 2-D CUDA array must be 0");
+    if (is_layered && (uint32_t)layer >= ext.depth)
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the layer is not below the CUDA array's layer count");
+    if ((uint64_t)x + W > ext.width || (uint64_t)y + H > ext.height)   // 64-bit: a huge origin must not wrap around
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the rectangle of " + of + " size does not lie inside the CUDA array");
+  } else {
+    if (!layered && (ext.width != W || ext.height != H || ext.depth != 0))
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the CUDA array is not a 2-D array of " + of + " size");
+    if (layered && (ext.width != W || ext.height != H || !(flags & cudaArrayLayered)))
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the CUDA array is not a layered array of " + of + " size");
+    if (layered && (uint32_t)layer >= ext.depth)
+      return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the layer is not below the CUDA array's layer count");
+  }
   if (!(flags & cudaArraySurfaceLoadStore))
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "the CUDA array was not created with cudaArraySurfaceLoadStore");
   return GS_OK;
 }
 
+bool array_layered(cudaArray_t arr) {
+  cudaChannelFormatDesc cd;
+  cudaExtent ext;
+  unsigned int flags = 0;
+  if (cudaArrayGetInfo(&cd, &ext, &flags, arr) != cudaSuccess) { cudaGetLastError(); return false; }
+  return (flags & cudaArrayLayered) != 0;
+}
+
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch) {
   if (!im || !im->data) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image is null");
   if (im->format > GS_PIX_RGBA32F) return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "unsupported pixel format");
-  if (im->memory > GS_MEM_ARRAY_LAYER || im->memory == 3)   // 3 is not a memory kind
+  if (im->memory > GS_MEM_ARRAY_RECT || im->memory == 3)   // 3 is not a memory kind
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "unknown image memory kind");
   if (im->width != W || im->height != H) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image size does not match screen size");
-  if (is_array_image(im)) {   // a 2-D CUDA array (data is a cudaArray_t), or a layer of a layered one (data is a GsArrayLayer *)
+  if (is_array_image(im)) {   // a 2-D CUDA array (data is a cudaArray_t), a layer of a layered one (a GsArrayLayer *) or a
+                              // rectangle of either (a GsArrayRect *)
     if (im->row_pitch_bytes) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "row_pitch_bytes must be 0 for a CUDA array image");
     const int rc = array_ok(ctx, *im, W, H, 4, im->format == GS_PIX_RGBA16F ? 16 : 32, "", "the image's",
                            "the image's pixel format");
@@ -62,14 +88,17 @@ int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t
   return GS_OK;
 }
 
-std::pair<const void *, int32_t> image_id(const GsImage *im) {
-  if (!im) return {nullptr, -1};
-  if (im->memory == GS_MEM_ARRAY_LAYER) {
-    int32_t layer = -1;
-    const cudaArray_t arr = image_array(im, &layer);
-    return {arr, layer};
-  }
-  return {im->data, -1};
+bool images_overlap(const GsImage *a, const GsImage *b) {
+  if (!a || !b || is_array_image(a) != is_array_image(b)) return false;
+  if (!is_array_image(a)) return a->data == b->data;
+  int32_t la = -1, lb = -1;
+  uint32_t ax = 0, ay = 0, bx = 0, by = 0;
+  const cudaArray_t arr_a = image_array(a, &la, &ax, &ay), arr_b = image_array(b, &lb, &bx, &by);
+  // a whole 2-D array (layer -1) and a rectangle of it (layer 0) are one layer
+  if (arr_a != arr_b || std::max(la, 0) != std::max(lb, 0)) return false;
+  if (a->memory != GS_MEM_ARRAY_RECT || b->memory != GS_MEM_ARRAY_RECT) return true;
+  return (uint64_t)ax < (uint64_t)bx + b->width && (uint64_t)bx < (uint64_t)ax + a->width &&
+         (uint64_t)ay < (uint64_t)by + b->height && (uint64_t)by < (uint64_t)ay + a->height;
 }
 
 // Destroys the held surface objects whose last use has completed; with `all`, every one, after waiting for its event.  The
@@ -115,18 +144,23 @@ int bind_image(GsContext *ctx, CallSurfaces &surfs, const GsImage *im, uint32_t 
 int copy_to_image(GsContext *ctx, const GsImage *im, uint32_t pitch, const void *src, uint32_t src_pitch, uint32_t W, uint32_t H,
                   cudaStream_t s) {
   const size_t row = (size_t)W * pix_bytes(im->format);
-  if (im->memory == GS_MEM_ARRAY) {
-    GS_CUDA_TRY(ctx, cudaMemcpy2DToArrayAsync(static_cast<cudaArray_t>(im->data), 0, 0, src, src_pitch, row, H, cudaMemcpyDeviceToDevice, s));
-  } else if (im->memory == GS_MEM_ARRAY_LAYER) {
+  if (is_array_image(im)) {
     int32_t layer = -1;
-    cudaMemcpy3DParms cp;
-    memset(&cp, 0, sizeof(cp));
-    cp.srcPtr = make_cudaPitchedPtr(const_cast<void *>(src), src_pitch, W, H);
-    cp.dstArray = image_array(im, &layer);
-    cp.dstPos = make_cudaPos(0, 0, (size_t)layer);
-    cp.extent = make_cudaExtent(W, H, 1);   // in texels: the destination is an array
-    cp.kind = cudaMemcpyDeviceToDevice;
-    GS_CUDA_TRY(ctx, cudaMemcpy3DAsync(&cp, s));
+    uint32_t x = 0, y = 0;
+    const cudaArray_t arr = image_array(im, &layer, &x, &y);
+    if (im->memory == GS_MEM_ARRAY || (im->memory == GS_MEM_ARRAY_RECT && !array_layered(arr))) {
+      // wOffset is in bytes
+      GS_CUDA_TRY(ctx, cudaMemcpy2DToArrayAsync(arr, (size_t)x * pix_bytes(im->format), y, src, src_pitch, row, H, cudaMemcpyDeviceToDevice, s));
+    } else {
+      cudaMemcpy3DParms cp;
+      memset(&cp, 0, sizeof(cp));
+      cp.srcPtr = make_cudaPitchedPtr(const_cast<void *>(src), src_pitch, W, H);
+      cp.dstArray = arr;
+      cp.dstPos = make_cudaPos(x, y, (size_t)(uint32_t)layer);   // in texels: the destination is an array
+      cp.extent = make_cudaExtent(W, H, 1);
+      cp.kind = cudaMemcpyDeviceToDevice;
+      GS_CUDA_TRY(ctx, cudaMemcpy3DAsync(&cp, s));
+    }
   } else {
     const cudaMemcpyKind kind = im->memory == GS_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
     GS_CUDA_TRY(ctx, cudaMemcpy2DAsync(im->data, pitch, src, src_pitch, row, H, kind, s));
@@ -140,13 +174,17 @@ int depth_ok(GsContext *ctx, const GsFrameParams *fp) {
                   "the screen's", "one 32-bit float channel");
 }
 
-std::tuple<const void *, int32_t, uint32_t> depth_id(const GsFrameParams *fp) {
-  if (!fp->scene_depth) return {nullptr, -1, 0};
+std::tuple<const void *, int32_t, uint32_t, uint32_t, uint32_t> depth_id(const GsFrameParams *fp) {
+  if (!fp->scene_depth) return {nullptr, -1, 0, 0, 0};
   if (fp->scene_depth_on_device == GS_MEM_ARRAY_LAYER) {
     const GsArrayLayer *d = reinterpret_cast<const GsArrayLayer *>(fp->scene_depth);
-    return {d->array, (int32_t)d->layer, GS_MEM_ARRAY_LAYER};
+    return {d->array, (int32_t)d->layer, GS_MEM_ARRAY_LAYER, 0, 0};
   }
-  return {fp->scene_depth, -1, fp->scene_depth_on_device};
+  if (fp->scene_depth_on_device == GS_MEM_ARRAY_RECT) {
+    const GsArrayRect *d = reinterpret_cast<const GsArrayRect *>(fp->scene_depth);
+    return {d->array, (int32_t)d->layer, GS_MEM_ARRAY_RECT, d->x, d->y};
+  }
+  return {fp->scene_depth, -1, fp->scene_depth_on_device, 0, 0};
 }
 
 int bind_depth(GsContext *ctx, CallSurfaces *surfs, const GsFrameParams *fp, float *staging, cudaStream_t s, SceneDepth *out) {

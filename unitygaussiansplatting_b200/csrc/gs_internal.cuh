@@ -180,24 +180,40 @@ int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uin
 // ---- images (gs_image.cu) -------------------------------------------------------------------------------------------------
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch);
 uint32_t pix_bytes(uint32_t fmt);
-inline bool is_array_image(const GsImage *im) { return im->memory == GS_MEM_ARRAY || im->memory == GS_MEM_ARRAY_LAYER; }
-// The CUDA array of a GS_MEM_ARRAY / GS_MEM_ARRAY_LAYER image, and in *layer the layer it names (-1: a 2-D array)
-inline cudaArray_t image_array(const GsImage *im, int32_t *layer) {
+inline bool is_array_image(const GsImage *im) {
+  return im->memory == GS_MEM_ARRAY || im->memory == GS_MEM_ARRAY_LAYER || im->memory == GS_MEM_ARRAY_RECT;
+}
+// The CUDA array of a GS_MEM_ARRAY / GS_MEM_ARRAY_LAYER / GS_MEM_ARRAY_RECT image, in *layer the layer it names (-1: a whole
+// 2-D array; a GS_MEM_ARRAY_RECT image names its descriptor's layer, 0 on a 2-D array), and in *x / *y (optional) the texel
+// that holds its pixel (0, 0).
+inline cudaArray_t image_array(const GsImage *im, int32_t *layer, uint32_t *x = nullptr, uint32_t *y = nullptr) {
+  uint32_t ox = 0, oy = 0;
+  cudaArray_t arr = static_cast<cudaArray_t>(im->data);
+  *layer = -1;
   if (im->memory == GS_MEM_ARRAY_LAYER) {
     const GsArrayLayer *d = static_cast<const GsArrayLayer *>(im->data);
     *layer = (int32_t)d->layer;
-    return static_cast<cudaArray_t>(d->array);
+    arr = static_cast<cudaArray_t>(d->array);
+  } else if (im->memory == GS_MEM_ARRAY_RECT) {
+    const GsArrayRect *d = static_cast<const GsArrayRect *>(im->data);
+    *layer = (int32_t)d->layer;
+    ox = d->x; oy = d->y;
+    arr = static_cast<cudaArray_t>(d->array);
   }
-  *layer = -1;
-  return static_cast<cudaArray_t>(im->data);
+  if (x) *x = ox;
+  if (y) *y = oy;
+  return arr;
 }
-// What makes two images of a call one image: the same pointer, or the same array and layer (GS_MEM_ARRAY_LAYER; the layers of
-// one array are separate images).
-std::pair<const void *, int32_t> image_id(const GsImage *im);
+// Whether `arr` (a valid CUDA array) is a layered one, as cudaArrayGetInfo reports it.
+bool array_layered(cudaArray_t arr);
+// Whether two images of a call share pixels: linear images by pointer; CUDA-array images when they name the same array and
+// layer and their rectangles intersect (a whole array or layer intersects every rectangle of it; the layers of one array are
+// separate images).  A null image shares nothing.
+bool images_overlap(const GsImage *a, const GsImage *b);
 void release_surfaces(GsContext *ctx, bool all);
 
-// The surface objects one call creates for its CUDA-array images, one per array: the layers of one layered array share it.
-// When the call returns they are handed to the context behind an event recorded on the stream that used them (the context's,
+// The surface objects one call creates for its CUDA-array images, one per array: the layers and rectangles of one array share
+// it, and each image's Surface carries its own layer and origin.  When the call returns they are handed to the context behind an event recorded on the stream that used them (the context's,
 // unless another is named) after their last use.  They are never cached by cudaArray_t value beyond the call: a freed array's
 // handle can be reused by the next allocation.
 class CallSurfaces {
@@ -218,19 +234,25 @@ class CallSurfaces {
     for (cudaSurfaceObject_t so : made_) cudaDestroySurfaceObject(so);
     if (ev) ctx_->spare_events.push_back(ev);
   }
-  // `im` has passed image_ok as a GS_MEM_ARRAY or GS_MEM_ARRAY_LAYER image
+  // `im` has passed image_ok as a GS_MEM_ARRAY, GS_MEM_ARRAY_LAYER or GS_MEM_ARRAY_RECT image
   int make(const GsImage *im, Surface *out) {
-    const cudaArray_t arr = image_array(im, &out->layer);
-    for (size_t i = 0; i < arrays_.size(); ++i)
-      if (arrays_[i] == arr) { out->obj = made_[i]; return GS_OK; }
-    if (made_.empty()) release_surfaces(ctx_, false);
-    cudaResourceDesc rd;
-    memset(&rd, 0, sizeof(rd));
-    rd.resType = cudaResourceTypeArray;
-    rd.res.array.array = arr;
-    GS_CUDA_TRY(ctx_, cudaCreateSurfaceObject(&out->obj, &rd));
-    made_.push_back(out->obj);
-    arrays_.push_back(arr);
+    const cudaArray_t arr = image_array(im, &out->layer, &out->x, &out->y);
+    size_t i = 0;
+    while (i < arrays_.size() && arrays_[i] != arr) ++i;
+    if (i == arrays_.size()) {
+      if (made_.empty()) release_surfaces(ctx_, false);
+      cudaResourceDesc rd;
+      memset(&rd, 0, sizeof(rd));
+      rd.resType = cudaResourceTypeArray;
+      rd.res.array.array = arr;
+      cudaSurfaceObject_t so = 0;
+      GS_CUDA_TRY(ctx_, cudaCreateSurfaceObject(&so, &rd));
+      made_.push_back(so);
+      arrays_.push_back(arr);
+      layered_.push_back(im->memory == GS_MEM_ARRAY_LAYER || (im->memory == GS_MEM_ARRAY_RECT && array_layered(arr)));
+    }
+    out->obj = made_[i];
+    if (!layered_[i]) out->layer = -1;   // a rectangle of a 2-D array is drawn with the 2-D surface calls
     return GS_OK;
   }
 
@@ -239,6 +261,7 @@ class CallSurfaces {
   cudaStream_t stream_;
   std::vector<cudaSurfaceObject_t> made_;
   std::vector<cudaArray_t> arrays_;   // made_[i] is the surface of arrays_[i]
+  std::vector<bool> layered_;         // arrays_[i] is a layered array
 };
 
 // The device view of an image a kernel reads and writes: linear memory at d_rt / pitch, or (d_rt == nullptr) the CUDA array
@@ -262,24 +285,29 @@ int copy_to_image(GsContext *ctx, const GsImage *im, uint32_t pitch, const void 
 
 // ---- the scene depth buffer (gs_image.cu) --------------------------------------------------------------------------------
 // GsFrameParams.scene_depth_on_device is the GsMemory of scene_depth: 0 host memory, GS_MEM_ARRAY a 2-D float32 CUDA array,
-// GS_MEM_ARRAY_LAYER a GsArrayLayer naming a layer of a layered one, any other value linear device memory.
+// GS_MEM_ARRAY_LAYER a GsArrayLayer naming a layer of a layered one, GS_MEM_ARRAY_RECT a GsArrayRect naming a rectangle of
+// either, any other value linear device memory.
 inline bool depth_on_host(const GsFrameParams *fp) { return fp->scene_depth && fp->scene_depth_on_device == GS_MEM_HOST; }
 inline bool depth_in_array(const GsFrameParams *fp) {
-  return fp->scene_depth && (fp->scene_depth_on_device == GS_MEM_ARRAY || fp->scene_depth_on_device == GS_MEM_ARRAY_LAYER);
+  return fp->scene_depth && (fp->scene_depth_on_device == GS_MEM_ARRAY || fp->scene_depth_on_device == GS_MEM_ARRAY_LAYER ||
+                             fp->scene_depth_on_device == GS_MEM_ARRAY_RECT);
 }
-// The array (layer) of a depth_in_array buffer as an image view (data and memory), as image_array and CallSurfaces take it.
+// The array (layer, rectangle) of a depth_in_array buffer as an image view (data and memory), as image_array and CallSurfaces
+// take it.
 inline GsImage depth_view(const GsFrameParams *fp) {
   GsImage a{};
   a.data = const_cast<float *>(fp->scene_depth);
   a.memory = fp->scene_depth_on_device;
   return a;
 }
-// A CUDA-array depth buffer must be a screen_w x screen_h array (layer) of one 32-bit float channel made with
-// cudaArraySurfaceLoadStore: GS_ERR_UNSUPPORTED_FORMAT for another channel format, GS_ERR_INVALID_ARGUMENT for anything else.
+// A CUDA-array depth buffer must be a screen_w x screen_h array (layer), or a rectangle of that size inside one, of one 32-bit
+// float channel made with cudaArraySurfaceLoadStore: GS_ERR_UNSUPPORTED_FORMAT for another channel format,
+// GS_ERR_INVALID_ARGUMENT for anything else.
 int depth_ok(GsContext *ctx, const GsFrameParams *fp);
-// What makes two objects' depth buffers one buffer: the same pointer and memory kind, or the same array and layer
-// (GS_MEM_ARRAY_LAYER: two descriptors of one layer are one buffer, the layers of one array are not).  (nullptr, ...): none.
-std::tuple<const void *, int32_t, uint32_t> depth_id(const GsFrameParams *fp);
+// What makes two objects' depth buffers one buffer: the same pointer and memory kind, or the same array, layer and origin
+// (GS_MEM_ARRAY_LAYER / GS_MEM_ARRAY_RECT: two descriptors of one layer and rectangle are one buffer, the layers of one array
+// and its other rectangles are not).  (nullptr, ...): none.
+std::tuple<const void *, int32_t, uint32_t, uint32_t, uint32_t> depth_id(const GsFrameParams *fp);
 // The kernels' view of fp's depth buffer (passed depth_ok), on `s`: device memory in place, a CUDA array (layer) through a
 // surface made by `surfs` (nullptr: none may be made, and a CUDA array is GS_ERR_INVALID_ARGUMENT), or a host buffer uploaded
 // into `staging`, W x H floats that the caller has grown.

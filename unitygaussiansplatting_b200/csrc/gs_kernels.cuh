@@ -229,10 +229,12 @@ cudaError_t launch_binning(const FrameConsts &fc, const GsRenderOptions &opt, co
                            cudaStream_t s, BinScratch *sorted, int *launches);
 
 // The surface of a CUDA-array image: a 2-D array (GS_MEM_ARRAY, layer -1), read and written with surf2Dread / surf2Dwrite, or
-// one layer of a layered array (GS_MEM_ARRAY_LAYER), read and written with surf2DLayeredread / surf2DLayeredwrite.
+// one layer of a layered array (GS_MEM_ARRAY_LAYER), read and written with surf2DLayeredread / surf2DLayeredwrite.  Pixel
+// (px, py) of the image is texel (x + px, y + py): the rectangle's origin of a GS_MEM_ARRAY_RECT image, 0 for a whole array.
 struct Surface {
   cudaSurfaceObject_t obj = 0;
   int32_t layer = -1;
+  uint32_t x = 0, y = 0;
 };
 // The scene depth buffer a draw is tested against, W x H float32 texels, texel (x, y) the depth of pixel (x, y): linear device
 // memory at `ptr` (rows tightly packed), or, with `on_surface`, a one-channel float32 CUDA array (layer) behind `surf`.  Neither:

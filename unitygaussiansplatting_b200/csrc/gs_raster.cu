@@ -411,15 +411,20 @@ __device__ __forceinline__ bool block_may_touch_quad(const float4 &A, float i2x,
   return axis_ok(A.z, A.w) && axis_ok(i2x, i2y);
 }
 
-// A texel of a CUDA-array image at byte column x_bytes, row y: surf2D* on a 2-D array, surf2DLayered* on a layer of a layered one.
-// LAYERED false: the image is known to be a 2-D array, and only the 2-D call is compiled.
+// The texel of a CUDA-array image that holds the pixel at byte column x_bytes (a multiple of sizeof(T), the texel size), row y:
+// offset by the surface's origin, through surf2D* on a 2-D array, surf2DLayered* on a layer of a layered one.  LAYERED false:
+// the image is known to be a 2-D array, and only the 2-D call is compiled.
 template <bool LAYERED, class T>
 __device__ __forceinline__ void surf_load(T *v, const Surface &s, uint32_t x_bytes, uint32_t y) {
+  x_bytes += s.x * (uint32_t)sizeof(T);
+  y += s.y;
   if (LAYERED && s.layer >= 0) surf2DLayeredread(v, s.obj, (int)x_bytes, (int)y, s.layer);
   else surf2Dread(v, s.obj, (int)x_bytes, (int)y);
 }
 template <bool LAYERED, class T>
 __device__ __forceinline__ void surf_store(const T &v, const Surface &s, uint32_t x_bytes, uint32_t y) {
+  x_bytes += s.x * (uint32_t)sizeof(T);
+  y += s.y;
   if (LAYERED && s.layer >= 0) surf2DLayeredwrite(v, s.obj, (int)x_bytes, (int)y, s.layer);
   else surf2Dwrite(v, s.obj, (int)x_bytes, (int)y);
 }
@@ -438,9 +443,10 @@ __device__ __forceinline__ void surf_store(const T &v, const Surface &s, uint32_
 // the other leaves.  The grid covers every camera's tiles; a tile finds its camera c in `cams`, which gives it the screen size, bins, image (pointer and pitch, or a surface when the pointer is null), scene depth buffer and load
 // flag that the other instantiations take from fc and the image arguments.  The camera's bin ids start at its bin_base in
 // bin_ranges; tile_cost is indexed by tile_base + the tile.  SURF: some camera's image is a CUDA array.  MULTI with SEL is held
-// to 32 registers, 8 CTAs per SM, which its shared memory also fits (selected runs measured 20 % slower at 7).
+// to 32 registers, 8 CTAs per SM, which its shared memory also fits (selected runs measured 20 % slower at 7); so is SEL into a
+// layer (SURF 2), which the rectangle origin of its surface accesses would otherwise take to 38 registers, 6 CTAs per SM.
 template <bool FP16_ROP, int OUT_FMT, bool STATS, bool SEL = false, int SURF = 0, bool MULTI = false>
-__global__ void __launch_bounds__(256, MULTI && SEL ? 8 : 0)
+__global__ void __launch_bounds__(256, SEL && (MULTI || SURF == 2) ? 8 : 0)
 k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const uint2 *__restrict__ bin_ranges,
          const uint32_t *__restrict__ tile_vals, const uint32_t *__restrict__ tile_order, uint32_t *__restrict__ tile_cost, uint32_t ntx,
          uint8_t *__restrict__ rt, uint32_t pitch, Surface surf, uint32_t band_packed, uint32_t load_rt,

@@ -46,6 +46,16 @@ inline GsImage ArrayLayerImage(GsArrayLayer *desc, uint32_t width, uint32_t heig
   return im;
 }
 
+// An image that is a width x height rectangle of a 2-D CUDA array or of one layer of a layered one (GS_MEM_ARRAY_RECT): pixel
+// (px, py) is texel (desc->x + px, desc->y + py).  E.g. a camera's part of an HDRP render target allocated larger than the camera
+// (desc = {array, 0, 0, 0, 0}, width x height the camera's scaled pixel size), or one view's tile of an atlas.  The image points
+// to `desc`, which must outlive every call the image is passed to.
+inline GsImage ArrayRectImage(GsArrayRect *desc, uint32_t width, uint32_t height, uint32_t format = GS_PIX_RGBA16F) {
+  GsImage im = ArrayImage(desc, width, height, format);
+  im.memory = GS_MEM_ARRAY_RECT;
+  return im;
+}
+
 class GaussianSplatRenderer {
  public:
   // serialized knobs, :225-251
@@ -59,7 +69,8 @@ class GaussianSplatRenderer {
   std::vector<GsCutout> m_Cutouts;
   // The camera's depth buffer the splats are depth-tested against (GsFrameParams.scene_depth), width x height float32 in
   // reversed Z, or nullptr.  sceneDepthMemory is its GsMemory (scene_depth_on_device): GS_MEM_HOST, GS_MEM_DEVICE, GS_MEM_ARRAY
-  // (sceneDepth is a cudaArray_t of one float32 channel) or GS_MEM_ARRAY_LAYER (SetSceneDepthLayer).
+  // (sceneDepth is a cudaArray_t of one float32 channel), GS_MEM_ARRAY_LAYER (SetSceneDepthLayer) or GS_MEM_ARRAY_RECT
+  // (SetSceneDepthRect).
   const float *sceneDepth = nullptr;
   uint32_t sceneDepthMemory = GS_MEM_HOST;
   // The depth is one layer of a layered float32 CUDA array (e.g. one eye of an XR eye-depth array); `desc` must outlive every
@@ -67,6 +78,12 @@ class GaussianSplatRenderer {
   void SetSceneDepthLayer(const GsArrayLayer *desc) {
     sceneDepth = reinterpret_cast<const float *>(desc);
     sceneDepthMemory = GS_MEM_ARRAY_LAYER;
+  }
+  // The depth is the width x height rectangle at (desc->x, desc->y) of a 2-D or layered float32 CUDA array (e.g. the camera's
+  // part of an HDRP depth texture allocated larger than the camera); `desc` must outlive every frame drawn with it.
+  void SetSceneDepthRect(const GsArrayRect *desc) {
+    sceneDepth = reinterpret_cast<const float *>(desc);
+    sceneDepthMemory = GS_MEM_ARRAY_RECT;
   }
   GsRenderOptions options{};
 

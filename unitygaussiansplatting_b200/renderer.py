@@ -85,25 +85,51 @@ class GaussianSplatContext:
             pass
 
 
+def _array_descriptor(what, handle, layer, origin):
+    """The GsArrayLayer / GsArrayRect a CUDA-array image or depth buffer points to (None for a whole 2-D array), and its memory
+    kind.  origin (x, y): the texel of the array that holds pixel (0, 0), a GS_MEM_ARRAY_RECT rectangle."""
+    if layer is not None:
+        layer = int(layer)
+        if not 0 <= layer < 2 ** 32:
+            raise ValueError("%s layer must be a non-negative 32-bit index" % what)
+    if origin is None:
+        if layer is None:
+            return None, N.GS_MEM_ARRAY
+        return N.GsArrayLayer(handle, layer, 0), N.GS_MEM_ARRAY_LAYER
+    try:
+        x, y = origin
+    except (TypeError, ValueError):
+        raise ValueError("%s origin must be a pair (x, y)" % what) from None
+    return N.GsArrayRect(handle, layer or 0, _index32(what, "origin", x), _index32(what, "origin", y), 0), N.GS_MEM_ARRAY_RECT
+
+
+def _index32(what, name, v):
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 0 <= int(v) < 2 ** 32:
+        raise ValueError("%s %s must hold non-negative 32-bit integers" % (what, name))
+    return int(v)
+
+
 class CudaArrayImage:
     """A 2-D CUDA array (cudaArray_t, e.g. an imported graphics render texture) of RGBA float16 or float32 texels, given to the
     library as an image (GS_MEM_ARRAY): it is rendered into / composited onto in place.  The host creates the array, with
     cudaArraySurfaceLoadStore, and keeps it alive; the library never allocates or frees one.
 
     layer: the array is a layered one (cudaArrayLayered, e.g. an XR eye-texture array or a cube map) and the image is this
-    layer of it (GS_MEM_ARRAY_LAYER); the other layers are left as they are."""
+    layer of it (GS_MEM_ARRAY_LAYER); the other layers are left as they are.
+    origin (x, y): the image is the width x height rectangle at texel (x, y) of the array (of its `layer` when it is layered;
+    GS_MEM_ARRAY_RECT), e.g. a camera's part of a larger HDRP render target, or one view's tile of an atlas.  The texels outside
+    the rectangle are left as they are."""
 
-    def __init__(self, handle: int, width: int, height: int, dtype=np.float16, layer=None):
+    def __init__(self, handle: int, width: int, height: int, dtype=np.float16, layer=None, origin=None):
         self.handle = int(handle)
         self.width, self.height = int(width), int(height)
         self.dtype = np.dtype(dtype)
         if self.dtype not in (np.float16, np.float32):
             raise ValueError("CudaArrayImage dtype must be float16 or float32")
+        # the descriptor a GS_MEM_ARRAY_LAYER / GS_MEM_ARRAY_RECT image points to, alive as long as this object
+        self._layer_desc, self.memory = _array_descriptor("CudaArrayImage", self.handle, layer, origin)
         self.layer = None if layer is None else int(layer)
-        if self.layer is not None and not 0 <= self.layer < 2 ** 32:
-            raise ValueError("CudaArrayImage layer must be a non-negative 32-bit index")
-        # the descriptor a GS_MEM_ARRAY_LAYER image points to, alive as long as this object
-        self._layer_desc = None if self.layer is None else N.GsArrayLayer(self.handle, self.layer, 0)
+        self.origin = None if origin is None else (int(origin[0]), int(origin[1]))
 
     @property
     def shape(self):
@@ -113,19 +139,20 @@ class CudaArrayImage:
 class CudaArrayDepth:
     """A scene depth buffer in a CUDA array (cudaArray_t, e.g. a camera's depth copied into an imported R32 float texture): a
     2-D array of one float32 channel (GS_MEM_ARRAY), or with `layer` that layer of a layered one (GS_MEM_ARRAY_LAYER, e.g. one
-    eye of an XR eye-depth array).  Texel (x, y) is the depth of pixel (x, y), reversed Z as for a depth tensor.  The array must
-    have been created with cudaArraySurfaceLoadStore (and cudaArrayLayered for a layer); the host keeps it alive."""
+    eye of an XR eye-depth array), or with `origin` (x, y) the width x height rectangle at that texel of either
+    (GS_MEM_ARRAY_RECT, e.g. the camera's part of a larger HDRP depth texture).  Texel (x + px, y + py) is the depth of pixel
+    (px, py), reversed Z as for a depth tensor.  The array must have been created with cudaArraySurfaceLoadStore (and
+    cudaArrayLayered for a layer); the host keeps it alive."""
 
-    def __init__(self, handle: int, width: int, height: int, layer=None):
+    def __init__(self, handle: int, width: int, height: int, layer=None, origin=None):
         self.handle = int(handle)
         self.width, self.height = int(width), int(height)
         if self.width < 1 or self.height < 1:
             raise ValueError("CudaArrayDepth width and height must be positive")
+        # the descriptor a GS_MEM_ARRAY_LAYER / GS_MEM_ARRAY_RECT depth buffer points to, alive as long as this object
+        self._layer_desc, self.memory = _array_descriptor("CudaArrayDepth", self.handle, layer, origin)
         self.layer = None if layer is None else int(layer)
-        if self.layer is not None and not 0 <= self.layer < 2 ** 32:
-            raise ValueError("CudaArrayDepth layer must be a non-negative 32-bit index")
-        # the descriptor a GS_MEM_ARRAY_LAYER depth buffer points to, alive as long as this object
-        self._layer_desc = None if self.layer is None else N.GsArrayLayer(self.handle, self.layer, 0)
+        self.origin = None if origin is None else (int(origin[0]), int(origin[1]))
 
     @property
     def shape(self):
@@ -140,10 +167,10 @@ def _image(arr, width: int, height: int) -> N.GsImage:
         if arr.shape != (height, width, 4):
             raise ValueError("CUDA array is %dx%d, the image must be %dx%d" % (arr.width, arr.height, width, height))
         im.format = N.GS_PIX_RGBA16F if arr.dtype == np.float16 else N.GS_PIX_RGBA32F
-        if arr.layer is None:
+        if arr._layer_desc is None:
             im.data, im.memory = arr.handle, N.GS_MEM_ARRAY
         else:
-            im.data, im.memory = C.addressof(arr._layer_desc), N.GS_MEM_ARRAY_LAYER
+            im.data, im.memory = C.addressof(arr._layer_desc), arr.memory
             im._layer_desc = arr._layer_desc   # the descriptor lives as long as the image that points to it
         im.row_pitch_bytes = 0
         return im
@@ -269,11 +296,11 @@ def make_frame_params(cam: Camera, localToWorld=None, splat_scale=1.0, opacity_s
             if scene_depth.shape != (cam.pixelHeight, cam.pixelWidth):
                 raise ValueError("the depth CUDA array is %dx%d, the screen %dx%d" % (scene_depth.width, scene_depth.height,
                                                                                    cam.pixelWidth, cam.pixelHeight))
-            if scene_depth.layer is None:
+            if scene_depth._layer_desc is None:
                 fp.scene_depth, fp.scene_depth_on_device = scene_depth.handle, N.GS_MEM_ARRAY
             else:
-                fp.scene_depth, fp.scene_depth_on_device = C.addressof(scene_depth._layer_desc), N.GS_MEM_ARRAY_LAYER
-            depth = scene_depth   # keeps its layer descriptor alive with the frame params
+                fp.scene_depth, fp.scene_depth_on_device = C.addressof(scene_depth._layer_desc), scene_depth.memory
+            depth = scene_depth   # keeps its layer / rectangle descriptor alive with the frame params
         elif isinstance(scene_depth, np.ndarray):
             depth = np.ascontiguousarray(scene_depth, np.float32)
             assert depth.shape == (cam.pixelHeight, cam.pixelWidth)
