@@ -128,9 +128,28 @@ typedef struct GsFrameParams {
   uint32_t reserved1;
 } GsFrameParams;
 
+/* GS_PIX_B10G11R11_UFLOAT: one 32-bit texel per pixel, no alpha: R in bits 0-10 and G in bits 11-21 (unsigned float11), B in
+ * bits 22-31 (unsigned float10) -- Unity's B10G11R11_UFloatPack32, VK_FORMAT_B10G11R11_UFLOAT_PACK32,
+ * DXGI_FORMAT_R11G11B10_FLOAT: the HDR colour buffer of URP and HDRP cameras.  It is accepted as a CAMERA TARGET, in every
+ * memory kind: gs_composite's camera_target, the camera targets of gs_frame, gs_frame_objects and gs_frame_cameras,
+ * gs_group_frame_objects' camera_targets (and so the camera_target of GsUnityFrameEvent / GsUnityFrameObjectsEvent).  A CUDA
+ * array holding it has ONE 32-bit cudaChannelFormatKindUnsigned channel (cudaCreateChannelDesc<unsigned int>()); any other
+ * channel format is GS_ERR_UNSUPPORTED_FORMAT, as a uint32 array is for an RGBA16F / RGBA32F image.  It is refused with
+ * GS_ERR_UNSUPPORTED_FORMAT, before anything is enqueued, as any render target (rt, rts[], a group's rts), as gs_composite's
+ * rt, as band_packed output and as gs_unshuffle_bands' out.
+ * The composite onto it decodes the texel, blends r, g and b exactly as onto an RGBA16F / RGBA32F target, drops alpha and
+ * encodes; a pixel whose source alpha is not > 0 keeps its bits.  Each channel has 5 exponent bits (bias 15) and 6 (float11)
+ * or 5 (float10) mantissa bits:
+ *   decode  exact: exponent 0 is mantissa * 2^-14 / 2^m (denormals), exponent 31 is +Inf with mantissa 0, else NaN;
+ *   encode  NaN -> all ones (0x7FF / 0x3FF); any value <= 0, -0 and -Inf included -> 0; +Inf -> 0x7C0 / 0x3E0; anything else
+ *           rounds to nearest, ties to even, over the whole value set including denormals, and overflows to +Inf as IEEE
+ *           rounding does: float11 x >= 65280 (largest finite 65024), float10 x >= 65024 (largest finite 64512).
+ * This follows the format definitions of the Vulkan and D3D11 specifications, and rounds as the RGBA16F path's
+ * float -> half conversion does; whether a given GPU's blend unit rounds this format the same way is not known here. */
 typedef enum GsPixelFormat {
   GS_PIX_RGBA16F = 0,   /* _GaussianSplatRT: R16G16B16A16_SFloat (R/GaussianSplatRenderer.cs:194) */
-  GS_PIX_RGBA32F = 1
+  GS_PIX_RGBA32F = 1,
+  GS_PIX_B10G11R11_UFLOAT = 2   /* camera targets only (above) */
 } GsPixelFormat;
 
 /* GS_MEM_ARRAY (images only, not GsPackDesc / GsPackedAsset): `data` is a cudaArray_t -- a 2-D CUDA array (mip level 0) on the
@@ -139,8 +158,8 @@ typedef enum GsPixelFormat {
  * cudaGraphicsSubResourceGetMappedArray.  The library reads and writes it in place through surface objects, so:
  *   - the array must have been created with cudaArraySurfaceLoadStore (for an imported image: ask for that flag in
  *     cudaExternalMemoryMipmappedArrayDesc.flags);
- *   - its channel format must be the image's: 4 x 16-bit float for GS_PIX_RGBA16F, 4 x 32-bit float for GS_PIX_RGBA32F
- *     (else GS_ERR_UNSUPPORTED_FORMAT);
+ *   - its channel format must be the image's: 4 x 16-bit float for GS_PIX_RGBA16F, 4 x 32-bit float for GS_PIX_RGBA32F,
+ *     1 x 32-bit unsigned for GS_PIX_B10G11R11_UFLOAT (else GS_ERR_UNSUPPORTED_FORMAT);
  *   - its extent must be width x height with depth 0, and row_pitch_bytes must be 0 (else GS_ERR_INVALID_ARGUMENT).
  * The import itself and the graphics API's semaphores stay with the host: wait / signal them on gs_context_stream(ctx).
  * Not accepted (GS_ERR_INVALID_ARGUMENT): band_packed output and gs_unshuffle_bands output.  GS_FLAG_ASYNC_READBACK has no

@@ -271,4 +271,33 @@ namespace GaussianSplatting.Runtime
             m_Next = (m_Next + 1) % kInFlight;
         }
     }
+    /// The camera's colour buffer as a camera target (GsImage) of an event, e.g. GsUnityFrameEvent.camera_target with
+    /// has_camera_target = 1: URP's HDR camera colour (m_HDRColorBufferPrecision 32-bit, no alpha) and HDRP's
+    /// ctx.cameraColorBuffer (colorBufferFormat R11G11B10) are GraphicsFormat.B10G11R11_UFloatPack32, which the library
+    /// composites onto in place as GS_PIX_B10G11R11_UFLOAT (2); the built-in pipeline's ARGBHalf is GS_PIX_RGBA16F (0).
+    /// `colorArray` is the buffer imported as a CUDA array: for B10G11R11 with ONE 32-bit unsigned channel
+    /// (cudaCreateChannelDesc<unsigned int>(), INTEGRATION.md section 3).  Not compiled here, like the rest of this file.
+    internal static class GaussianSplatCameraTarget
+    {
+        public static uint PixelFormat(UnityEngine.Experimental.Rendering.GraphicsFormat f)
+        {
+            switch (f)
+            {
+                case UnityEngine.Experimental.Rendering.GraphicsFormat.R16G16B16A16_SFloat: return 0;   // GS_PIX_RGBA16F
+                case UnityEngine.Experimental.Rendering.GraphicsFormat.R32G32B32A32_SFloat: return 1;   // GS_PIX_RGBA32F
+                case UnityEngine.Experimental.Rendering.GraphicsFormat.B10G11R11_UFloatPack32: return 2; // GS_PIX_B10G11R11_UFLOAT
+                default: throw new NotSupportedException("camera colour format " + f + " is not a supported camera target");
+            }
+        }
+
+        public static unsafe GaussianSplatNative.GsImage Image(IntPtr colorArray, int width, int height,
+                                                               UnityEngine.Experimental.Rendering.GraphicsFormat f)
+        {
+            return new GaussianSplatNative.GsImage
+            {
+                data = (void*)colorArray, width = (uint)width, height = (uint)height,
+                row_pitch_bytes = 0, format = PixelFormat(f), memory = 2 /* GS_MEM_ARRAY */
+            };
+        }
+    }
 }

@@ -337,7 +337,7 @@ static int composite_impl(GsContext *ctx, CallSurfaces &surfs, const void *d_rt,
                           uint32_t rt_fmt, GsImage *tgt, uint32_t W, uint32_t H, cudaStream_t s) {
   GsNvtxRange nvtx("GaussianSplat.Compose");
   uint32_t tp = 0;
-  int rc = image_ok(ctx, tgt, W, H, &tp);
+  int rc = image_ok(ctx, tgt, W, H, ImageRole::kCameraTarget, &tp);
   if (rc) return rc;
   const bool host = tgt->memory == GS_MEM_HOST;
   if (host) GS_CUDA_TRY(ctx, ctx->tgt_scratch.reserve((size_t)W * pix_bytes(tgt->format) * H, {ctx->stream}));
@@ -620,7 +620,7 @@ int gs_render(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRend
   const uint32_t H = opt.band_packed ? partition_own_bin_rows(opt, fc.binsY) * kBin : (uint32_t)fp->screen_h;
   if (opt.band_packed && rt && is_array_image(rt))
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "band_packed output is the send buffer of an all-gather: it must be linear memory, not a CUDA array");
-  if ((rc = image_ok(ctx, rt, W, H, &pitch))) return rc;
+  if ((rc = image_ok(ctx, rt, W, H, ImageRole::kRenderTarget, &pitch))) return rc;
   if (fp->scene_depth && !as->zndc_valid) return fail(ctx, GS_ERR_NOT_READY, "a scene depth buffer needs the quad depths: run gs_calc_view with scene_depth set");
   for (int e = EV_BIN1; e < EV_COUNT; ++e) ctx->ev_valid[e] = false;
   rec(ctx, EV_VIEW1);
@@ -639,7 +639,7 @@ int gs_composite(GsContext *ctx, const GsImage *rt, GsImage *tgt) {
   if (!ctx || !rt || !tgt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null argument");
   GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));   // array images are inspected and bound on the context's device
   uint32_t rp = 0;
-  int rc = image_ok(ctx, rt, rt->width, rt->height, &rp);
+  int rc = image_ok(ctx, rt, rt->width, rt->height, ImageRole::kRenderTarget, &rp);
   if (rc) return rc;
   const uint32_t W = rt->width, H = rt->height;
   ctx->ev_valid[EV_COMP1] = false;
@@ -689,8 +689,8 @@ static int check_camera(GsContext *ctx, GsAsset *const *assets, const GsFramePar
   if ((rc = check_options(ctx, a->fcs[0], *opt))) return rc;
   a->W = (uint32_t)fps[0].screen_w; a->H = (uint32_t)fps[0].screen_h;
   uint32_t tgt_pitch = 0;
-  if (a->rt) { if ((rc = image_ok(ctx, a->rt, a->W, a->H, &a->rt_pitch))) return rc; a->rt_fmt = a->rt->format; }
-  if (a->tgt && (rc = image_ok(ctx, a->tgt, a->W, a->H, &tgt_pitch))) return rc;
+  if (a->rt) { if ((rc = image_ok(ctx, a->rt, a->W, a->H, ImageRole::kRenderTarget, &a->rt_pitch))) return rc; a->rt_fmt = a->rt->format; }
+  if (a->tgt && (rc = image_ok(ctx, a->tgt, a->W, a->H, ImageRole::kCameraTarget, &tgt_pitch))) return rc;
   return GS_OK;
 }
 
@@ -947,7 +947,7 @@ int gs_frame(GsContext *ctx, GsAsset *as, const GsFrameParams *fp, const GsRende
   if (opt.band_packed && tgt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "band_packed output cannot be composited before the gather");
   if (opt.band_packed && rt && is_array_image(rt))
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "band_packed output is the send buffer of an all-gather: it must be linear memory, not a CUDA array");
-  if (rt) { if ((rc = image_ok(ctx, rt, a.W, a.H, &a.rt_pitch))) return rc; a.rt_fmt = rt->format; }
+  if (rt) { if ((rc = image_ok(ctx, rt, a.W, a.H, ImageRole::kRenderTarget, &a.rt_pitch))) return rc; a.rt_fmt = rt->format; }
   return draw_cameras(ctx, cams, &as, fp, &do_sort_flag, opt);
 }
 
@@ -991,7 +991,7 @@ int gs_unshuffle_bands(GsContext *ctx, const void *gathered, uint32_t parts, uin
   if (!ctx || !gathered || !out || parts == 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null argument");
   if (is_array_image(out)) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gs_unshuffle_bands writes host or linear device memory, not a CUDA array");
   uint32_t pitch = 0;
-  int rc = image_ok(ctx, out, out->width, out->height, &pitch);
+  int rc = image_ok(ctx, out, out->width, out->height, ImageRole::kRenderTarget, &pitch);
   if (rc) return rc;
   if (out->format != fmt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "gathered and output pixel formats differ");
   const uint32_t W = out->width, H = out->height;

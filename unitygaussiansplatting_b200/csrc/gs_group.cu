@@ -581,14 +581,14 @@ static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsF
     GsImage *rt = rts ? rts[i] : nullptr;
     pitches[i] = W * pix_bytes(fmt);
     if (rt) {
-      if ((rc = image_ok(ctx, rt, W, H, &rt_pitches[i]))) return rc;
+      if ((rc = image_ok(ctx, rt, W, H, ImageRole::kRenderTarget, &rt_pitches[i]))) return rc;
       if (rt->format != fmt) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "members' images differ in pixel format");
       if (rt->memory == GS_MEM_DEVICE) { dev_rt[i] = rt->data; pitches[i] = rt_pitches[i]; }
     }
     if (G > 1 && pitches[i] != pitches[0]) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "members' images differ in row pitch");
     GsImage *ct = cams ? cams[i] : nullptr;
     uint32_t tp = 0;
-    if (ct && (rc = image_ok(ctx, ct, W, H, &tp))) return rc;
+    if (ct && (rc = image_ok(ctx, ct, W, H, ImageRole::kCameraTarget, &tp))) return rc;
   }
   const FrameConsts fc0 = make_frame_consts(obj[0].fp);
   for (uint32_t k = 0; k < K; ++k) obj[k].fc = k ? make_frame_consts(obj[k].fp) : fc0;

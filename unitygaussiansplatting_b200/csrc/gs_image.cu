@@ -8,15 +8,15 @@
 
 namespace gs {
 
-uint32_t pix_bytes(uint32_t fmt) { return fmt == GS_PIX_RGBA16F ? 8u : 16u; }
+uint32_t pix_bytes(uint32_t fmt) { return fmt == GS_PIX_RGBA16F ? 8u : fmt == GS_PIX_B10G11R11_UFLOAT ? 4u : 16u; }
 
 // The rules every CUDA array the library reads or writes keeps: `a` (a GS_MEM_ARRAY, GS_MEM_ARRAY_LAYER or GS_MEM_ARRAY_RECT view:
 // data and memory) is a W x H 2-D array, a layer below the layer count of a W x H layered one, or a W x H rectangle inside a
 // 2-D array or inside a layer of a layered one, made with cudaArraySurfaceLoadStore, whose channels are `channels` x
-// `bits`-bit float (else GS_ERR_UNSUPPORTED_FORMAT; everything else is GS_ERR_INVALID_ARGUMENT).  The messages start with
-// `prefix`, and name the size `of` and the channels `format` expected.
-static int array_ok(GsContext *ctx, const GsImage &a, uint32_t W, uint32_t H, int channels, int bits, const char *prefix, const char *of,
-                    const char *format) {
+// `bits`-bit of kind `kind` (else GS_ERR_UNSUPPORTED_FORMAT; everything else is GS_ERR_INVALID_ARGUMENT).  The messages start
+// with `prefix`, and name the size `of` and the channels `format` expected.
+static int array_ok(GsContext *ctx, const GsImage &a, uint32_t W, uint32_t H, cudaChannelFormatKind kind, int channels, int bits,
+                    const char *prefix, const char *of, const char *format) {
   const std::string p(prefix);
   const bool layered = a.memory == GS_MEM_ARRAY_LAYER, rect = a.memory == GS_MEM_ARRAY_RECT;
   if (layered) {
@@ -35,7 +35,7 @@ static int array_ok(GsContext *ctx, const GsImage &a, uint32_t W, uint32_t H, in
   const cudaError_t e = cudaArrayGetInfo(&cd, &ext, &flags, image_array(&a, &layer, &x, &y));
   if (e != cudaSuccess) { cudaGetLastError(); return fail(ctx, GS_ERR_INVALID_ARGUMENT, p + "not a CUDA array: " + cudaGetErrorString(e)); }
   const int want[4] = {bits, channels > 1 ? bits : 0, channels > 2 ? bits : 0, channels > 3 ? bits : 0};
-  if (cd.f != cudaChannelFormatKindFloat || cd.x != want[0] || cd.y != want[1] || cd.z != want[2] || cd.w != want[3])
+  if (cd.f != kind || cd.x != want[0] || cd.y != want[1] || cd.z != want[2] || cd.w != want[3])
     return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, p + "the CUDA array's channel format does not match " + format);
   if (rect) {
     const bool is_layered = (flags & cudaArrayLayered) != 0;
@@ -67,17 +67,21 @@ bool array_layered(cudaArray_t arr) {
   return (flags & cudaArrayLayered) != 0;
 }
 
-int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, uint32_t *pitch) {
+int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, ImageRole role, uint32_t *pitch) {
   if (!im || !im->data) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image is null");
-  if (im->format > GS_PIX_RGBA32F) return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "unsupported pixel format");
+  const bool packed = im->format == GS_PIX_B10G11R11_UFLOAT;
+  if (im->format > GS_PIX_B10G11R11_UFLOAT) return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "unsupported pixel format");
+  if (packed && role != ImageRole::kCameraTarget)
+    return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "GS_PIX_B10G11R11_UFLOAT is a camera-target format, not a render-target one");
   if (im->memory > GS_MEM_ARRAY_RECT || im->memory == 3)   // 3 is not a memory kind
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "unknown image memory kind");
   if (im->width != W || im->height != H) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image size does not match screen size");
   if (is_array_image(im)) {   // a 2-D CUDA array (data is a cudaArray_t), a layer of a layered one (a GsArrayLayer *) or a
                               // rectangle of either (a GsArrayRect *)
     if (im->row_pitch_bytes) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "row_pitch_bytes must be 0 for a CUDA array image");
-    const int rc = array_ok(ctx, *im, W, H, 4, im->format == GS_PIX_RGBA16F ? 16 : 32, "", "the image's",
-                           "the image's pixel format");
+    const int rc = packed ? array_ok(ctx, *im, W, H, cudaChannelFormatKindUnsigned, 1, 32, "", "the image's", "one 32-bit unsigned channel")
+                          : array_ok(ctx, *im, W, H, cudaChannelFormatKindFloat, 4, im->format == GS_PIX_RGBA16F ? 16 : 32, "",
+                                     "the image's", "the image's pixel format");
     if (rc) return rc;
     *pitch = 0;
     return GS_OK;
@@ -170,7 +174,7 @@ int copy_to_image(GsContext *ctx, const GsImage *im, uint32_t pitch, const void 
 
 int depth_ok(GsContext *ctx, const GsFrameParams *fp) {
   if (!depth_in_array(fp)) return GS_OK;
-  return array_ok(ctx, depth_view(fp), (uint32_t)fp->screen_w, (uint32_t)fp->screen_h, 1, 32, "scene depth: ",
+  return array_ok(ctx, depth_view(fp), (uint32_t)fp->screen_w, (uint32_t)fp->screen_h, cudaChannelFormatKindFloat, 1, 32, "scene depth: ",
                   "the screen's", "one 32-bit float channel");
 }
 

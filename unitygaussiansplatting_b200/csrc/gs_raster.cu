@@ -25,6 +25,7 @@
 #include <type_traits>
 
 #include "gs_kernels.cuh"
+#include "gs_packed_float.cuh"
 
 namespace gs {
 
@@ -810,6 +811,7 @@ void launch_unshuffle(const void *gathered, uint32_t parts, uint32_t band, uint3
 }
 
 // ---- 3. composite (S/GaussianComposite.shader:35-39, Blend SrcAlpha OneMinusSrcAlpha :11) ------
+// The camera target is RGBA16F, RGBA32F or B10G11R11_UFLOAT; the render target is never the packed format.
 __device__ __forceinline__ float gamma_to_linear(float x) {  // UnityCG.cginc GammaToLinearSpace (not vendored)
   return x * fmaf(x, fmaf(x, 0.305306011f, 0.682171111f), 0.012522878f);
 }
@@ -828,21 +830,36 @@ __device__ __forceinline__ float4 load_px(const uint8_t *base, uint32_t pitch, c
   return c;
 }
 
+// TGT_FMT: the camera target's pixel format, a template parameter so that the RGBA16F and RGBA32F instantiations carry no code
+// of the packed one (a uniform run-time branch cost the RGBA16F composite 3 % at 1920 x 1080 on an H100).
+template <uint32_t TGT_FMT>
 __global__ void __launch_bounds__(256) k_composite(const uint8_t *__restrict__ rt, uint32_t rt_pitch, Surface rt_surf,
                                                    uint32_t rt_fmt, uint8_t *__restrict__ tgt, uint32_t tgt_pitch,
-                                                   Surface tgt_surf, uint32_t tgt_fmt, uint32_t W, uint32_t H) {
+                                                   Surface tgt_surf, uint32_t W, uint32_t H) {
   const uint32_t x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= W || y >= H) return;
   const float4 c = load_px(rt, rt_pitch, rt_surf, rt_fmt, x, y);
   if (!(c.w > 0.0f)) return;  // SrcAlpha == 0 leaves the target untouched
-  const float4 d = load_px(tgt, tgt_pitch, tgt_surf, tgt_fmt, x, y);
+  float4 d = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  if constexpr (TGT_FMT == GS_PIX_B10G11R11_UFLOAT) {   // a camera target only: no alpha, one 32-bit texel
+    uint32_t v;
+    if (tgt) v = reinterpret_cast<const uint32_t *>(tgt + (size_t)y * tgt_pitch)[x];
+    else surf_load<true>(&v, tgt_surf, x * 4u, y);
+    unpack_b10g11r11(v, &d.x, &d.y, &d.z);
+  } else {
+    d = load_px(tgt, tgt_pitch, tgt_surf, TGT_FMT, x, y);
+  }
   const float a = c.w, om = 1.0f - a;
   float4 o;
   o.x = fmaf(gamma_to_linear(__fdiv_rn(c.x, a)), a, d.x * om);
   o.y = fmaf(gamma_to_linear(__fdiv_rn(c.y, a)), a, d.y * om);
   o.z = fmaf(gamma_to_linear(__fdiv_rn(c.z, a)), a, d.z * om);
   o.w = fmaf(a, a, d.w * om);
-  if (tgt_fmt == GS_PIX_RGBA16F) {
+  if constexpr (TGT_FMT == GS_PIX_B10G11R11_UFLOAT) {
+    const uint32_t v = pack_b10g11r11(o.x, o.y, o.z);
+    if (tgt) reinterpret_cast<uint32_t *>(tgt + (size_t)y * tgt_pitch)[x] = v;
+    else surf_store<true>(v, tgt_surf, x * 4u, y);
+  } else if constexpr (TGT_FMT == GS_PIX_RGBA16F) {
     uint2 v;
     v.x = f32tof16(o.x) | (f32tof16(o.y) << 16);
     v.y = f32tof16(o.z) | (f32tof16(o.w) << 16);
@@ -858,8 +875,14 @@ void launch_composite(const void *rt, uint32_t rt_pitch, Surface rt_surf, uint32
                       Surface tgt_surf, uint32_t tgt_format, uint32_t W, uint32_t H, cudaStream_t s) {
   if (!W || !H) return;
   dim3 grid((W + 31) / 32, (H + 7) / 8);
-  k_composite<<<grid, 256, 0, s>>>(reinterpret_cast<const uint8_t *>(rt), rt_pitch, rt_surf, rt_format, reinterpret_cast<uint8_t *>(target),
-                                   tgt_pitch, tgt_surf, tgt_format, W, H);
+  const uint8_t *r = reinterpret_cast<const uint8_t *>(rt);
+  uint8_t *t = reinterpret_cast<uint8_t *>(target);
+  if (tgt_format == GS_PIX_B10G11R11_UFLOAT)
+    k_composite<GS_PIX_B10G11R11_UFLOAT><<<grid, 256, 0, s>>>(r, rt_pitch, rt_surf, rt_format, t, tgt_pitch, tgt_surf, W, H);
+  else if (tgt_format == GS_PIX_RGBA16F)
+    k_composite<GS_PIX_RGBA16F><<<grid, 256, 0, s>>>(r, rt_pitch, rt_surf, rt_format, t, tgt_pitch, tgt_surf, W, H);
+  else
+    k_composite<GS_PIX_RGBA32F><<<grid, 256, 0, s>>>(r, rt_pitch, rt_surf, rt_format, t, tgt_pitch, tgt_surf, W, H);
 }
 
 }  // namespace gs

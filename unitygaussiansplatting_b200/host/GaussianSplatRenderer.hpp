@@ -56,6 +56,22 @@ inline GsImage ArrayRectImage(GsArrayRect *desc, uint32_t width, uint32_t height
   return im;
 }
 
+// A camera target of packed B10G11R11_UFLOAT texels (GS_PIX_B10G11R11_UFLOAT: the HDR colour buffer of URP and HDRP cameras,
+// accepted as a camera target only) in host or device memory (`memory`): one uint32 per pixel, rows `row_pitch_bytes` apart
+// (0: tightly packed).  Such a colour buffer imported as a CUDA array (one 32-bit unsigned channel) is ArrayImage /
+// ArrayLayerImage / ArrayRectImage with format GS_PIX_B10G11R11_UFLOAT.
+inline GsImage PackedCameraTarget(void *data, uint32_t width, uint32_t height, uint32_t memory, uint32_t row_pitch_bytes = 0) {
+  GsImage im;
+  std::memset(&im, 0, sizeof(im));
+  im.data = data;
+  im.width = width;
+  im.height = height;
+  im.row_pitch_bytes = row_pitch_bytes;
+  im.format = GS_PIX_B10G11R11_UFLOAT;
+  im.memory = memory;
+  return im;
+}
+
 class GaussianSplatRenderer {
  public:
   // serialized knobs, :225-251

@@ -111,7 +111,8 @@ def _index32(what, name, v):
 
 class CudaArrayImage:
     """A 2-D CUDA array (cudaArray_t, e.g. an imported graphics render texture) of RGBA float16 or float32 texels, given to the
-    library as an image (GS_MEM_ARRAY): it is rendered into / composited onto in place.  The host creates the array, with
+    library as an image (GS_MEM_ARRAY): it is rendered into / composited onto in place.  dtype uint32: an array of one 32-bit
+    unsigned channel holding GS_PIX_B10G11R11_UFLOAT texels (a URP / HDRP camera colour buffer), a camera target only.  The host creates the array, with
     cudaArraySurfaceLoadStore, and keeps it alive; the library never allocates or frees one.
 
     layer: the array is a layered one (cudaArrayLayered, e.g. an XR eye-texture array or a cube map) and the image is this
@@ -124,8 +125,8 @@ class CudaArrayImage:
         self.handle = int(handle)
         self.width, self.height = int(width), int(height)
         self.dtype = np.dtype(dtype)
-        if self.dtype not in (np.float16, np.float32):
-            raise ValueError("CudaArrayImage dtype must be float16 or float32")
+        if self.dtype not in (np.float16, np.float32, np.uint32):
+            raise ValueError("CudaArrayImage dtype must be float16, float32 or uint32")
         # the descriptor a GS_MEM_ARRAY_LAYER / GS_MEM_ARRAY_RECT image points to, alive as long as this object
         self._layer_desc, self.memory = _array_descriptor("CudaArrayImage", self.handle, layer, origin)
         self.layer = None if layer is None else int(layer)
@@ -133,7 +134,7 @@ class CudaArrayImage:
 
     @property
     def shape(self):
-        return (self.height, self.width, 4)
+        return (self.height, self.width) if self.dtype == np.uint32 else (self.height, self.width, 4)
 
 
 class CudaArrayDepth:
@@ -160,13 +161,14 @@ class CudaArrayDepth:
 
 
 def _image(arr, width: int, height: int) -> N.GsImage:
-    """numpy (host) array or torch CUDA tensor of shape (H, W, 4), float16/float32, or a CudaArrayImage -> GsImage."""
+    """numpy (host) array or torch CUDA tensor of shape (H, W, 4), float16/float32, or (H, W) uint32 (int32 for a tensor) of
+    packed GS_PIX_B10G11R11_UFLOAT texels, or a CudaArrayImage -> GsImage."""
     im = N.GsImage()
     im.width, im.height = width, height
     if isinstance(arr, CudaArrayImage):
-        if arr.shape != (height, width, 4):
+        if arr.shape[:2] != (height, width):
             raise ValueError("CUDA array is %dx%d, the image must be %dx%d" % (arr.width, arr.height, width, height))
-        im.format = N.GS_PIX_RGBA16F if arr.dtype == np.float16 else N.GS_PIX_RGBA32F
+        im.format = {np.float16: N.GS_PIX_RGBA16F, np.float32: N.GS_PIX_RGBA32F, np.uint32: N.GS_PIX_B10G11R11_UFLOAT}[arr.dtype.type]
         if arr._layer_desc is None:
             im.data, im.memory = arr.handle, N.GS_MEM_ARRAY
         else:
@@ -175,18 +177,31 @@ def _image(arr, width: int, height: int) -> N.GsImage:
         im.row_pitch_bytes = 0
         return im
     if isinstance(arr, np.ndarray):
-        if arr.shape != (height, width, 4) or not arr.flags.c_contiguous:
-            raise ValueError("image must be C-contiguous (H, W, 4)")
-        if arr.dtype == np.float16:
-            im.format = N.GS_PIX_RGBA16F
-        elif arr.dtype == np.float32:
-            im.format = N.GS_PIX_RGBA32F
+        if arr.dtype == np.uint32:
+            if arr.shape != (height, width) or not arr.flags.c_contiguous:
+                raise ValueError("a packed image must be C-contiguous (H, W) uint32")
+            im.format = N.GS_PIX_B10G11R11_UFLOAT
         else:
-            raise ValueError("image dtype must be float16 or float32")
+            if arr.shape != (height, width, 4) or not arr.flags.c_contiguous:
+                raise ValueError("image must be C-contiguous (H, W, 4)")
+            if arr.dtype == np.float16:
+                im.format = N.GS_PIX_RGBA16F
+            elif arr.dtype == np.float32:
+                im.format = N.GS_PIX_RGBA32F
+            else:
+                raise ValueError("image dtype must be float16, float32 or (packed) uint32")
         im.data, im.memory = arr.ctypes.data, N.GS_MEM_HOST
         im.row_pitch_bytes = arr.strides[0]
         return im
     # torch tensor (duck-typed so torch stays optional)
+    if str(arr.dtype) in ("torch.int32", "torch.uint32"):
+        if tuple(arr.shape) != (height, width) or not arr.is_contiguous():
+            raise ValueError("a packed image must be contiguous (H, W)")
+        im.format = N.GS_PIX_B10G11R11_UFLOAT
+        im.data = arr.data_ptr()
+        im.memory = N.GS_MEM_DEVICE if arr.is_cuda else N.GS_MEM_HOST
+        im.row_pitch_bytes = width * 4
+        return im
     if tuple(arr.shape) != (height, width, 4) or not arr.is_contiguous():
         raise ValueError("image must be contiguous (H, W, 4)")
     es = arr.element_size()
@@ -195,6 +210,48 @@ def _image(arr, width: int, height: int) -> N.GsImage:
     im.memory = N.GS_MEM_DEVICE if arr.is_cuda else N.GS_MEM_HOST
     im.row_pitch_bytes = width * 4 * es
     return im
+
+
+def _to_ufloat(x: np.ndarray, m: int) -> np.ndarray:
+    """float32 -> unsigned float of 5 exponent bits (bias 15) and m mantissa bits, as include/gsplat_b200.h states it."""
+    u = np.ascontiguousarray(x, np.float32).view(np.uint32).astype(np.int64)
+    inf = 31 << m
+    e = (u >> 23) - 127
+    mant = u & 0x7FFFFF
+    sub = e < -14   # a denormal code (its value below 2^-14)
+    shift = np.where(sub, 23 - m + np.clip(-14 - e, 0, 40), 23 - m)
+    mant = np.where(sub, mant | 0x800000, mant)
+    h = np.where(sub, 0, np.clip(e + 15, 0, 64) << m) + (mant >> np.minimum(shift, 40))
+    rem = mant & ((np.int64(1) << shift) - 1)
+    half = np.int64(1) << (shift - 1)
+    h = h + ((rem > half) | ((rem == half) & ((h & 1) == 1)))
+    h = np.where((e < -15 - m), 0, np.minimum(h, inf))
+    h = np.where(u == 0x7F800000, inf, h)
+    h = np.where((u >> 31) == 1, 0, h)
+    h = np.where((u & 0x7FFFFFFF) > 0x7F800000, inf | ((1 << m) - 1), h)
+    return h.astype(np.uint32)
+
+
+def _from_ufloat(c: np.ndarray, m: int) -> np.ndarray:
+    c = np.asarray(c, np.uint32)
+    e, mant = (c >> m) & 31, c & ((1 << m) - 1)
+    normal = (((e + 112) << 23) | (mant << (23 - m))).astype(np.uint32).view(np.float32)
+    special = np.where(mant != 0, np.uint32(0x7FC00000) | (mant << (23 - m)), np.uint32(0x7F800000)).astype(np.uint32).view(np.float32)
+    denormal = mant.astype(np.float32) * np.float32(2.0 ** (-14 - m))
+    return np.where(e == 0, denormal, np.where(e == 31, special, normal))
+
+
+def pack_b10g11r11(rgb) -> np.ndarray:
+    """(..., 3) float32 linear colours -> (...) uint32 GS_PIX_B10G11R11_UFLOAT texels (R bits 0-10, G 11-21, B 22-31), rounded as
+    the library's composite rounds them."""
+    rgb = np.asarray(rgb, np.float32)
+    return _to_ufloat(rgb[..., 0], 6) | (_to_ufloat(rgb[..., 1], 6) << 11) | (_to_ufloat(rgb[..., 2], 5) << 22)
+
+
+def unpack_b10g11r11(texels) -> np.ndarray:
+    """(...) uint32 GS_PIX_B10G11R11_UFLOAT texels -> (..., 3) float32, exactly."""
+    t = np.asarray(texels, np.uint32)
+    return np.stack([_from_ufloat(t & 0x7FF, 6), _from_ufloat((t >> 11) & 0x7FF, 6), _from_ufloat(t >> 22, 5)], axis=-1)
 
 
 _EYE4 = np.eye(4, dtype=np.float32)
