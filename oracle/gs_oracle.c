@@ -549,6 +549,9 @@ void gso_calc_view(const GsoAsset *a, const GsoFrame *f, GsoView *view, int thre
 
 /* ------------------------------------------------------------------ draw + blend */
 static inline float round_h(float v) { return gso_f16tof32(gso_f32tof16(v)); }
+/* A blend that yields NaN (a NaN or inf in the loaded target, or inf * 0) stores the GPU's canonical NaN 0x7FFFFFFF whatever the
+   operands' payloads: float arithmetic returns it, and the fp16 ROP's half NaN 0x7FFF widens to it. */
+static inline float canonical_nan(float v) { return v == v ? v : as_f32(0x7fffffffu); }
 
 /* band t covers rows [H*t/bands, H*(t+1)/bands): the band of row y is the largest t with H*t/bands <= y */
 static inline int band_of_row(int32_t y, int bands, uint32_t H) {
@@ -571,12 +574,12 @@ void gso_render(const GsoView *view, const uint32_t *order, uint32_t n, uint32_t
 
 void gso_render_sel(const GsoView *view, const uint32_t *order, uint32_t n, uint32_t W, uint32_t H, uint32_t blend_mode,
                     float *rt, int threads, const uint32_t *selected_bits) {
-  gso_render_ex(view, order, n, W, H, blend_mode, rt, threads, selected_bits, NULL);
+  gso_render_ex(view, order, n, W, H, blend_mode, rt, threads, selected_bits, NULL, 0);
 }
 
 void gso_render_ex(const GsoView *view, const uint32_t *order, uint32_t n, uint32_t W, uint32_t H, uint32_t blend_mode,
-                   float *rt, int threads, const uint32_t *selected_bits, const float *scene_depth) {
-  memset(rt, 0, (size_t)W * H * 16); /* ClearRenderTarget(0,0,0,0), R/GaussianSplatRenderer.cs:196 */
+                   float *rt, int threads, const uint32_t *selected_bits, const float *scene_depth, int load) {
+  if (!load) memset(rt, 0, (size_t)W * H * 16); /* ClearRenderTarget(0,0,0,0), R/GaussianSplatRenderer.cs:196 */
   if (threads < 1) threads = 1;
   const float fW = (float)W, fH = (float)H;
   DrawRec *recs = (DrawRec *)malloc((size_t)(n ? n : 1) * sizeof(DrawRec));
@@ -675,7 +678,7 @@ void gso_render_ex(const GsoView *view, const uint32_t *order, uint32_t n, uint3
           float r0 = fmaf(pr * alpha, om, d[0]), r1 = fmaf(pg * alpha, om, d[1]), r2 = fmaf(pb * alpha, om, d[2]),
                 r3 = fmaf(alpha, om, d[3]);
           if (blend_mode == 0) { r0 = round_h(r0); r1 = round_h(r1); r2 = round_h(r2); r3 = round_h(r3); }
-          d[0] = r0; d[1] = r1; d[2] = r2; d[3] = r3;
+          d[0] = canonical_nan(r0); d[1] = canonical_nan(r1); d[2] = canonical_nan(r2); d[3] = canonical_nan(r3);
         }
       }
     }

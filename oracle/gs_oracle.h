@@ -126,9 +126,12 @@ GSO_API void gso_render_sel(const GsoView *view, const uint32_t *order, uint32_t
 /* ... and with the scene's depth buffer bound (R/GaussianSplatRenderer.cs:195 binds the current depth target; the pass keeps
  * ShaderLab's default ZTest LEqual, ZWrite Off, S/RenderGaussianSplats.shader:8-12).  A splat's quad is flat: every fragment
  * has the depth clip.z / clip.w of the centre.  `scene_depth` is W x H float32 in the GPU projection's convention (reversed Z:
- * 1 = near), under which LEqual is evaluated as "fragment depth >= stored depth".  NULL = no test. */
+ * 1 = near), under which LEqual is evaluated as "fragment depth >= stored depth".  NULL = no test.  load != 0: the draw starts
+ * from rt as given instead of clearing it (GS_FLAG_LOAD_RT: a target earlier draws or the host filled); a pixel no fragment
+ * blends into keeps its bits, and a blend that yields NaN stores the GPU's canonical NaN 0x7FFFFFFF (in either blend mode). */
 GSO_API void gso_render_ex(const GsoView *view, const uint32_t *order, uint32_t n, uint32_t width, uint32_t height,
-                        uint32_t blend_mode, float *rt, int threads, const uint32_t *selected_bits, const float *scene_depth);
+                        uint32_t blend_mode, float *rt, int threads, const uint32_t *selected_bits, const float *scene_depth,
+                        int load);
 
 /* ---- GaussianComposite.shader:35-39, Blend SrcAlpha OneMinusSrcAlpha (:11).
  *      target: W*H*4 floats, read-modify-write; target_fp16 != 0 rounds the result to half. ---- */

@@ -69,7 +69,8 @@ def lib():
         L.gso_render_sel.restype = None
         L.gso_render_sel.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_int, C.c_void_p]
         L.gso_render_ex.restype = None
-        L.gso_render_ex.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        L.gso_render_ex.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                   C.c_int]
         L.gso_composite.restype, L.gso_composite.argtypes = None, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_int]
         L.gso_max_threads.restype, L.gso_max_threads.argtypes = C.c_int, []
         L.gso_export_data.restype, L.gso_export_data.argtypes = None, [C.POINTER(GsoAsset), C.POINTER(GsoFrame), C.c_void_p, C.c_int]
@@ -154,16 +155,25 @@ def export_data(asset, fp=None, threads: int = 1) -> np.ndarray:
 
 
 def render(view: np.ndarray, order: np.ndarray, width: int, height: int, blend_mode: int = 0, threads: int = 1,
-           selected_bits=None, scene_depth=None) -> np.ndarray:
+           selected_bits=None, scene_depth=None, init=None) -> np.ndarray:
+    """The draw into a cleared target, or with `init` ((H, W, 4) float32, e.g. an RGBA16F image widened exactly) onto that
+    content: GS_FLAG_LOAD_RT."""
     view = np.ascontiguousarray(view, np.uint32)
     order = np.ascontiguousarray(order, np.uint32)
-    rt = np.zeros((height, width, 4), np.float32)
+    if init is None:
+        rt = np.zeros((height, width, 4), np.float32)
+    else:
+        assert init.shape == (height, width, 4) and init.dtype == np.float32
+        rt = np.array(init, np.float32, order="C")   # a copy: every bit of it, NaN payloads included
+    depth = None
     if scene_depth is not None:
         depth = np.ascontiguousarray(scene_depth, np.float32)
         assert depth.shape == (height, width)
+    if depth is not None or init is not None:
         bits = None if selected_bits is None else np.ascontiguousarray(selected_bits, np.uint32)
         lib().gso_render_ex(view.ctypes.data, order.ctypes.data, order.size, width, height, blend_mode, rt.ctypes.data, threads,
-                            bits.ctypes.data if bits is not None else None, depth.ctypes.data)
+                            bits.ctypes.data if bits is not None else None, depth.ctypes.data if depth is not None else None,
+                            0 if init is None else 1)
     elif selected_bits is None:
         lib().gso_render(view.ctypes.data, order.ctypes.data, order.size, width, height, blend_mode, rt.ctypes.data, threads)
     else:
@@ -180,8 +190,9 @@ def composite(rt: np.ndarray, target: np.ndarray, target_fp16: bool = False) -> 
     return out
 
 
-def frame(asset, fp, prev_order=None, width=None, height=None, blend_mode: int = 0, threads: int = 1):
-    """Whole path: distances -> stable sort -> view -> draw.  Returns dict of every intermediate."""
+def frame(asset, fp, prev_order=None, width=None, height=None, blend_mode: int = 0, threads: int = 1, init=None):
+    """Whole path: distances -> stable sort -> view -> draw (onto `init`, as render takes it).  Returns dict of every
+    intermediate."""
     n = asset.splatCount
     order = np.arange(n, dtype=np.uint32) if prev_order is None else np.ascontiguousarray(prev_order, np.uint32).copy()
     keys = calc_distances(asset, fp, order, threads)
@@ -194,7 +205,7 @@ def frame(asset, fp, prev_order=None, width=None, height=None, blend_mode: int =
     if getattr(fp, "scene_depth", None):
         assert not fp.scene_depth_on_device, "the oracle reads host memory"
         depth = np.ctypeslib.as_array(C.cast(fp.scene_depth, C.POINTER(C.c_float)), shape=(H, W))
-    rt = render(view, order, W, H, blend_mode, threads, bits, depth)
+    rt = render(view, order, W, H, blend_mode, threads, bits, depth, init)
     return {"keys": keys, "order": order, "view": view, "rt": rt}
 
 

@@ -518,6 +518,10 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
   const bool in_image = px < (uint32_t)fc.screenW && py < (uint32_t)fc.screenH;
 
   float d0 = 0.f, d1 = 0.f, d2 = 0.f, d3 = 0.f;  // ClearRenderTarget(0,0,0,0), R/GaussianSplatRenderer.cs:196
+  // whether any splat blended into this pixel: under GS_FLAG_LOAD_RT a pixel nothing blends into is not written, so it keeps
+  // the words it was loaded with (the ROP writes only where a fragment blends; the half -> float -> half round trip would
+  // replace a NaN's payload with the canonical NaN)
+  bool blended = false;
   // the scene's depth at this pixel (depth target bound at R/GaussianSplatRenderer.cs:195; ZTest LEqual, ZWrite Off)
   float zscene = 0.0f;
   if constexpr (SEL) {
@@ -657,6 +661,7 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
             n0 = lo.x; n1 = lo.y; n2 = hi.x; n3 = hi.y;
           }
           d0 = n0; d1 = n1; d2 = n2; d3 = n3;
+          blended = true;
         }
       }
     }
@@ -682,7 +687,7 @@ k_raster(FrameConsts fc, Partition part, const float4 *__restrict__ draw, const 
     }
   }
 
-  if (in_image) {
+  if (in_image && (blended || !load_rt)) {
     camera_image();
     uint8_t *row = rt + (size_t)out_row * pitch;
     if (OUT_FMT == GS_PIX_RGBA16F) {
