@@ -2,7 +2,7 @@
 (cudaExternalMemoryGetMappedMipmappedArray / cudaGraphicsSubResourceGetMappedArray).  The library renders into and composites
 onto such an array in place, through surface objects.
 
-Arrays are made by cuda_arrays.Cudart, through the CUDA runtime torch already loaded.  Every GPU test compares the array result
+Arrays are made by images.Cudart, through the CUDA runtime torch already loaded.  Every GPU test compares the array result
 byte for byte with the same call on a torch device tensor: the linear path is pinned to the oracle elsewhere, so equality is the
 parity contract."""
 import ctypes as C
@@ -13,7 +13,7 @@ from pathlib import Path
 import numpy as np
 import pytest
 
-from cuda_arrays import KIND_FLOAT, KIND_UNSIGNED, SURFACE_LOAD_STORE, Cudart
+from images import KIND_FLOAT, KIND_UNSIGNED, SURFACE_LOAD_STORE, Image, bits, ca, to_device, to_host  # noqa: F401
 from util import camera
 
 ROOT = Path(__file__).resolve().parents[1]
@@ -30,45 +30,9 @@ def test_header_and_python_agree_on_gs_mem_array():
     assert N.GS_MEM_ARRAY == 2
 
 
-@pytest.fixture
-def rt_arrays(ctx):
-    ca = Cudart()
-    yield ca
-    ctx.sync()
-    ca.free_all()
-
-
-def _image_array(g, ca, w, h, dtype=np.float16, fill=None):
-    """A CudaArrayImage of (h, w) RGBA texels, pre-filled with `fill` (default: random halves / floats)."""
-    handle = ca.array(w, h, dtype=dtype)
-    if fill is None:
-        fill = np.random.default_rng(w * 7919 + h).random((h, w, 4), np.float32).astype(dtype)
-    ca.upload(handle, np.broadcast_to(np.asarray(fill, dtype), (h, w, 4)))
-    return g.CudaArrayImage(handle, w, h, dtype)
-
-
-def _read(ctx, ca, im):
-    ctx.sync()   # the library's stream does not synchronise with the legacy default stream the copy runs on
-    return ca.download(im.handle, im.shape, im.dtype)
-
-
-def _tensor(h, w, dtype=np.float16, fill=None):
-    import torch
-    t = torch.zeros((h, w, 4), dtype=torch.float16 if dtype == np.float16 else torch.float32, device="cuda")
-    if fill is not None:
-        t.copy_(torch.from_numpy(np.array(np.broadcast_to(np.asarray(fill, dtype), (h, w, 4)))))
-    return t
-
-
-def _host(ctx, t):
-    import torch
-    ctx.sync()
-    torch.cuda.synchronize()
-    return t.cpu().numpy()
-
-
-def _bits(a):
-    return a.view(np.uint16) if a.dtype == np.float16 else a.view(np.uint32)
+def _noise(w, h, dtype=np.float16):
+    """Random halves / floats: content every pixel of a render target must overwrite."""
+    return np.random.default_rng(w * 7919 + h).random((h, w, 4), np.float32).astype(dtype)
 
 
 def _lattice_case(g):
@@ -81,7 +45,7 @@ def _lattice_case(g):
 # ---- 1, 2: gs_frame into an array --------------------------------------------------------------------------------------------
 @pytest.mark.gpu
 @pytest.mark.parametrize("scene", ["lattice_1k_medium_256x256", "clustered_333x211"])
-def test_frame_into_rgba16f_array_equals_tensor(g, O, ctx, rt_arrays, scene):
+def test_frame_into_rgba16f_array_equals_tensor(g, O, ctx, ca, scene):
     if scene.startswith("lattice"):
         asset, cam, sh = _lattice_case(g)
     else:
@@ -89,15 +53,15 @@ def test_frame_into_rgba16f_array_equals_tensor(g, O, ctx, rt_arrays, scene):
     h, w = cam.pixelHeight, cam.pixelWidth
     r = g.GaussianSplatRenderer(asset, ctx)
     r.m_SHOrder = sh
-    t = _tensor(h, w)
+    t = to_device(np.zeros((h, w, 4), np.float16))
     r.SortAndRenderSplats(cam, rt=t)
-    want = _host(ctx, t)
+    want = to_host(ctx, t)
     r.ResetOrder()
-    im = _image_array(g, rt_arrays, w, h)     # random content: every pixel must be overwritten
-    r.SortAndRenderSplats(cam, rt=im)
-    got = _read(ctx, rt_arrays, im)
+    im = Image(g, ca, "array", _noise(w, h))     # random content: every pixel must be overwritten
+    r.SortAndRenderSplats(cam, rt=im.image)
+    got = im.read(ctx)
     assert want.any()
-    assert np.array_equal(_bits(got), _bits(want))
+    assert np.array_equal(bits(got), bits(want))
     if scene.startswith("lattice"):   # and straight against the oracle
         fp, _keep = g.make_frame_params(cam, sh_order=sh)
         ref = O.frame(asset, fp, threads=O.max_threads())
@@ -106,25 +70,25 @@ def test_frame_into_rgba16f_array_equals_tensor(g, O, ctx, rt_arrays, scene):
 
 
 @pytest.mark.gpu
-def test_frame_into_rgba32f_array_fp32_blend_equals_tensor(g, ctx, rt_arrays):
+def test_frame_into_rgba32f_array_fp32_blend_equals_tensor(g, ctx, ca):
     asset = g.synthetic_asset(g.SCENE_CLUSTERED, 30000, 0x5EED00A2, "Medium")
     cam = camera(g, 333, 211)
     r = g.GaussianSplatRenderer(asset, ctx)
     r.blend_mode = 1
-    t = _tensor(211, 333, np.float32)
+    t = to_device(np.zeros((211, 333, 4), np.float32))
     r.SortAndRenderSplats(cam, rt=t)
-    want = _host(ctx, t)
+    want = to_host(ctx, t)
     r.ResetOrder()
-    im = _image_array(g, rt_arrays, 333, 211, np.float32)
-    r.SortAndRenderSplats(cam, rt=im)
-    got = _read(ctx, rt_arrays, im)
-    assert want.any() and np.array_equal(_bits(got), _bits(want))
+    im = Image(g, ca, "array", _noise(333, 211, np.float32))
+    r.SortAndRenderSplats(cam, rt=im.image)
+    got = im.read(ctx)
+    assert want.any() and np.array_equal(bits(got), bits(want))
     r.Dispose()
 
 
 # ---- 3: GS_FLAG_LOAD_RT ------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_two_renderers_share_one_array_render_target(g, ctx, rt_arrays):
+def test_two_renderers_share_one_array_render_target(g, ctx, ca):
     a = g.synthetic_asset(g.SCENE_CLUSTERED, 30000, 0x5EED0091, "Medium")
     b = g.synthetic_asset(g.SCENE_CLUSTERED, 20000, 0x5EED0092, "VeryHigh")
     cam = camera(g, 400, 300)
@@ -137,20 +101,20 @@ def test_two_renderers_share_one_array_render_target(g, ctx, rt_arrays):
         assert active == [rb, ra]
         return ra, rb
 
-    t = _tensor(300, 400)
+    t = to_device(np.zeros((300, 400, 4), np.float16))
     keep = draw(t)
-    want = _host(ctx, t)
-    im = _image_array(g, rt_arrays, 400, 300)
-    keep += draw(im)
-    got = _read(ctx, rt_arrays, im)
-    assert want.any() and np.array_equal(_bits(got), _bits(want))
+    want = to_host(ctx, t)
+    im = Image(g, ca, "array", _noise(400, 300))
+    keep += draw(im.image)
+    got = im.read(ctx)
+    assert want.any() and np.array_equal(bits(got), bits(want))
     for r in keep:
         r.Dispose()
 
 
 # ---- 4: the extras variant (selection + scene depth) ---------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_selection_and_scene_depth_into_array(g, ctx, rt_arrays):
+def test_selection_and_scene_depth_into_array(g, ctx, ca):
     asset = g.synthetic_asset(g.SCENE_CLUSTERED, 40000, 0x5EED00A4, "Medium")
     n = asset.splatCount
     sel = np.zeros((n + 31) // 32, np.uint32)
@@ -163,97 +127,97 @@ def test_selection_and_scene_depth_into_array(g, ctx, rt_arrays):
     depth[:, :240] = np.float32(clip[2] / clip[3])
     r = g.GaussianSplatRenderer(asset, ctx)
     r.m_SelectedBits, r.sceneDepth = sel, depth
-    t = _tensor(300, 400)
+    t = to_device(np.zeros((300, 400, 4), np.float16))
     r.SortAndRenderSplats(cam, rt=t)
-    want = _host(ctx, t)
+    want = to_host(ctx, t)
     r.ResetOrder()
-    im = _image_array(g, rt_arrays, 400, 300)
-    r.SortAndRenderSplats(cam, rt=im)
-    got = _read(ctx, rt_arrays, im)
-    assert want.any() and np.array_equal(_bits(got), _bits(want))
+    im = Image(g, ca, "array", _noise(400, 300))
+    r.SortAndRenderSplats(cam, rt=im.image)
+    got = im.read(ctx)
+    assert want.any() and np.array_equal(bits(got), bits(want))
     r.Dispose()
 
 
 # ---- 5: staged calls -------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_staged_render_into_array_equals_fused_frame(g, ctx, rt_arrays):
+def test_staged_render_into_array_equals_fused_frame(g, ctx, ca):
     asset = g.synthetic_asset(g.SCENE_CLUSTERED, 30000, 0x5EED0006, "Medium")
     cam = camera(g, 300, 200)
     a, b = g.GaussianSplatRenderer(asset, ctx), g.GaussianSplatRenderer(asset, ctx)
-    t = _tensor(200, 300)
+    t = to_device(np.zeros((200, 300, 4), np.float16))
     a.SortAndRenderSplats(cam, rt=t)
-    want = _host(ctx, t)
-    im = _image_array(g, rt_arrays, 300, 200)
-    b.SortPoints(cam); b.CalcViewData(cam); b.DrawSplats(cam, im)
-    got = _read(ctx, rt_arrays, im)
-    assert want.any() and np.array_equal(_bits(got), _bits(want))
+    want = to_host(ctx, t)
+    im = Image(g, ca, "array", _noise(300, 200))
+    b.SortPoints(cam); b.CalcViewData(cam); b.DrawSplats(cam, im.image)
+    got = im.read(ctx)
+    assert want.any() and np.array_equal(bits(got), bits(want))
     a.Dispose(); b.Dispose()
 
 
 # ---- 6: composite --------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
 @pytest.mark.parametrize("tgt_dtype", [np.float16, np.float32])
-def test_composite_all_four_target_kinds(g, ctx, rt_arrays, tgt_dtype):
+def test_composite_all_four_target_kinds(g, ctx, ca, tgt_dtype):
     asset = g.synthetic_asset(g.SCENE_CLUSTERED, 20000, 0x5EED0002, "Medium")
     cam = camera(g, 320, 200)
     r = g.GaussianSplatRenderer(asset, ctx)
-    rt_t = _tensor(200, 320)
+    rt_t = to_device(np.zeros((200, 320, 4), np.float16))
     r.SortAndRenderSplats(cam, rt=rt_t)
-    rt_np = _host(ctx, rt_t)
+    rt_np = to_host(ctx, rt_t)
     assert (rt_np[..., 3] == 0).any() and (rt_np[..., 3] > 0).any()   # both sides of the SrcAlpha == 0 early-out occur
-    rt_a = _image_array(g, rt_arrays, 320, 200, fill=rt_np)
+    rt_a = Image(g, ca, "array", rt_np).image
     bg = np.random.default_rng(11).random((200, 320, 4), np.float32).astype(np.float16).astype(tgt_dtype)
     want = None
     for src in (rt_t, rt_a):
         for kind in ("tensor", "array"):
-            tgt = _tensor(200, 320, tgt_dtype, fill=bg) if kind == "tensor" else _image_array(g, rt_arrays, 320, 200, tgt_dtype, fill=bg)
-            r.Composite(src, tgt)
-            got = _host(ctx, tgt) if kind == "tensor" else _read(ctx, rt_arrays, tgt)
+            tgt = Image(g, ca, "device" if kind == "tensor" else "array", bg)
+            r.Composite(src, tgt.image)
+            got = tgt.read(ctx)
             if want is None:
                 want = got
                 untouched = rt_np[..., 3] == 0
-                assert np.array_equal(_bits(got)[untouched], _bits(bg)[untouched]) and not np.array_equal(got, bg)
-            assert np.array_equal(_bits(got), _bits(want)), "rt %s, target %s" % ("tensor" if src is rt_t else "array", kind)
+                assert np.array_equal(bits(got)[untouched], bits(bg)[untouched]) and not np.array_equal(got, bg)
+            assert np.array_equal(bits(got), bits(want)), "rt %s, target %s" % ("tensor" if src is rt_t else "array", kind)
     # gs_frame with an array camera target, with the render target in library scratch and with an array render target
     for with_rt in (False, True):
         r.ResetOrder(); r.m_FrameCounter = 0
-        tgt = _image_array(g, rt_arrays, 320, 200, tgt_dtype, fill=bg)
-        rt = _image_array(g, rt_arrays, 320, 200) if with_rt else None
-        r.SortAndRenderSplats(cam, rt=rt, camera_target=tgt)
-        assert np.array_equal(_bits(_read(ctx, rt_arrays, tgt)), _bits(want)), "gs_frame, rt %s" % ("array" if with_rt else "scratch")
+        tgt = Image(g, ca, "array", bg)
+        rt = Image(g, ca, "array", _noise(320, 200)) if with_rt else None
+        r.SortAndRenderSplats(cam, rt=rt and rt.image, camera_target=tgt.image)
+        assert np.array_equal(bits(tgt.read(ctx)), bits(want)), "gs_frame, rt %s" % ("array" if with_rt else "scratch")
         if with_rt:
-            assert np.array_equal(_bits(_read(ctx, rt_arrays, rt)), _bits(rt_np))
+            assert np.array_equal(bits(rt.read(ctx)), bits(rt_np))
     r.Dispose()
 
 
 # ---- 7: row ranges ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_row_range_into_array_keeps_other_rows(g, ctx, rt_arrays):
+def test_row_range_into_array_keeps_other_rows(g, ctx, ca):
     asset = g.synthetic_asset(g.SCENE_CLUSTERED, 30000, 0x5EED00A7, "Medium")
     cam = camera(g, 333, 211)
     r = g.GaussianSplatRenderer(asset, ctx)
-    full_t = _tensor(211, 333)
+    full_t = to_device(np.zeros((211, 333, 4), np.float16))
     r.SortAndRenderSplats(cam, rt=full_t)
-    full = _host(ctx, full_t)
+    full = to_host(ctx, full_t)
     sentinel = np.float16(-7.5)
     r.rows = (3, 11)                          # 16-pixel rows 3..10: pixel rows [48, 176)
     r.ResetOrder(); r.m_FrameCounter = 0
-    t = _tensor(211, 333, fill=sentinel)
+    t = to_device(np.full((211, 333, 4), sentinel))
     r.SortAndRenderSplats(cam, rt=t)
-    want = _host(ctx, t)
+    want = to_host(ctx, t)
     r.ResetOrder(); r.m_FrameCounter = 0
-    im = _image_array(g, rt_arrays, 333, 211, fill=sentinel)
-    r.SortAndRenderSplats(cam, rt=im)
-    got = _read(ctx, rt_arrays, im)
-    assert np.array_equal(_bits(got), _bits(want))
-    assert np.array_equal(_bits(got[48:176]), _bits(full[48:176])) and full[48:176].any()
+    im = Image(g, ca, "array", np.full((211, 333, 4), sentinel))
+    r.SortAndRenderSplats(cam, rt=im.image)
+    got = im.read(ctx)
+    assert np.array_equal(bits(got), bits(want))
+    assert np.array_equal(bits(got[48:176]), bits(full[48:176])) and full[48:176].any()
     assert (got[:48] == sentinel).all() and (got[176:] == sentinel).all()
     r.Dispose()
 
 
 # ---- 8: the Unity render-thread event ------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_unity_event_with_array_rt_equals_direct_frame(g, ctx, rt_arrays):
+def test_unity_event_with_array_rt_equals_direct_frame(g, ctx, ca):
     from unitygaussiansplatting_b200 import _native as N
     asset = g.synthetic_asset(g.SCENE_CLUSTERED, 20000, 0x5EED0051, "Medium")
     cam = camera(g, 200, 150)
@@ -261,7 +225,7 @@ def test_unity_event_with_array_rt_equals_direct_frame(g, ctx, rt_arrays):
     direct = np.zeros((150, 200, 4), np.float16)
     r.SortAndRenderSplats(cam, rt=direct)
     r.ResetOrder()
-    im = _image_array(g, rt_arrays, 200, 150)
+    im = Image(g, ca, "array", _noise(200, 150))
     fp, _keep = g.make_frame_params(cam, r.localToWorldMatrix, r.m_SplatScale, r.m_OpacityScale, r.m_SHOrder, r.m_SHOnly)
     ev = N.GsUnityFrameEvent()
     ev.ctx, ev.asset = C.cast(ctx.handle, C.c_void_p).value, C.cast(r._asset, C.c_void_p).value
@@ -269,22 +233,22 @@ def test_unity_event_with_array_rt_equals_direct_frame(g, ctx, rt_arrays):
     ev.options.blend_mode = 0
     ev.do_sort, ev.status = 1, -5
     ev.has_rt, ev.has_camera_target = 1, 0
-    ev.rt.data, ev.rt.width, ev.rt.height = im.handle, 200, 150
+    ev.rt.data, ev.rt.width, ev.rt.height = im.image.handle, 200, 150
     ev.rt.row_pitch_bytes, ev.rt.format, ev.rt.memory = 0, N.GS_PIX_RGBA16F, N.GS_MEM_ARRAY
     fn = N.native().gs_unity_get_render_event_func()
     fn(N.GS_UNITY_EVENT_FRAME, C.addressof(ev))
     assert ev.status == 0
     fn(N.GS_UNITY_EVENT_SYNC, C.addressof(ev))
     assert ev.status == 0
-    got = _read(ctx, rt_arrays, im)
-    assert direct.any() and np.array_equal(_bits(got), _bits(direct))
+    got = im.read(ctx)
+    assert direct.any() and np.array_equal(bits(got), bits(direct))
     r.Dispose()
 
 
 # ---- 9: groups -----------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
 @pytest.mark.parametrize("members", [2, 3])
-def test_emulated_group_with_array_members_equals_one_gpu(g, ctx, rt_arrays, members):
+def test_emulated_group_with_array_members_equals_one_gpu(g, ctx, ca, members):
     from unitygaussiansplatting_b200.multigpu import GaussianSplatGroup
     asset = g.synthetic_asset(g.SCENE_CLUSTERED, 40000, 0x5EED00A9, "Medium")
     cam = camera(g, 400, 300)
@@ -293,20 +257,20 @@ def test_emulated_group_with_array_members_equals_one_gpu(g, ctx, rt_arrays, mem
     r.SortAndRenderSplats(cam, rt=want)
     r.Dispose()
     grp = GaussianSplatGroup.create(asset, [0] * members, emulate=True)
-    arrays = [_image_array(g, rt_arrays, 400, 300) for _ in range(members - 1)]   # rts[0] (and rts[1] for 3 members)
+    arrays = [Image(g, ca, "array", _noise(400, 300)) for _ in range(members - 1)]   # rts[0] (and rts[1] for 3 members)
     rest = [np.zeros_like(want)]
-    grp.SortAndRenderSplats(cam, rts=arrays + rest)
+    grp.SortAndRenderSplats(cam, rts=[im.image for im in arrays] + rest)
     grp.sync()
     assert want.any()
     for im in arrays:
-        assert np.array_equal(_bits(_read(ctx, rt_arrays, im)), _bits(want))
-    assert np.array_equal(_bits(rest[0]), _bits(want))
+        assert np.array_equal(bits(im.read(ctx)), bits(want))
+    assert np.array_equal(bits(rest[0]), bits(want))
     grp.close()
 
 
 # ---- 10: rejections ------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_array_rejections_leave_the_array_untouched(g, ctx, rt_arrays):
+def test_array_rejections_leave_the_array_untouched(g, ctx, ca):
     import torch
     from unitygaussiansplatting_b200 import _native as N
     lib = N.native()
@@ -324,10 +288,10 @@ def test_array_rejections_leave_the_array_untouched(g, ctx, rt_arrays):
     pattern = np.random.default_rng(3).random((128, 128, 4), np.float32).astype(np.float16)
 
     def filled(width=128, kind=KIND_FLOAT, flags=SURFACE_LOAD_STORE, fill=pattern):
-        return rt_arrays.array(width, 128, dtype=fill.dtype, flags=flags, kind=kind, fill=fill)
+        return ca.array(width, 128, dtype=fill.dtype, flags=flags, kind=kind, fill=fill)
 
-    def unchanged(h, fill=pattern, width=128):
-        return np.array_equal(rt_arrays.download(h, (128, width, 4), fill.dtype).view(np.uint8), fill.view(np.uint8))
+    def unchanged(h, fill=pattern):
+        return np.array_equal(ca.download(h).view(np.uint8), fill.view(np.uint8))
 
     bytes8 = np.random.default_rng(4).integers(0, 256, (128, 128, 4), np.uint8)
     h = filled(kind=KIND_UNSIGNED, fill=bytes8)                               # uint8 x 4
@@ -338,9 +302,9 @@ def test_array_rejections_leave_the_array_untouched(g, ctx, rt_arrays):
     h = filled(width=129, fill=wide)                                           # 129 x 128 for a 128 x 128 image
     assert frame(h) == -1
     ctx.sync()
-    assert unchanged(h, wide, 129)
-    h = filled(flags=0)                                                        # no cudaArraySurfaceLoadStore
-    assert frame(h) == -1 and "cudaArraySurfaceLoadStore" in lib.gs_last_error(ctx.handle).decode()
+    assert unchanged(h, wide)
+    no_surface = filled(flags=0)                                               # no cudaArraySurfaceLoadStore
+    assert frame(no_surface) == -1 and "cudaArraySurfaceLoadStore" in lib.gs_last_error(ctx.handle).decode()
     good = filled()
     assert frame(good, pitch=128 * 8) == -1                                    # non-zero pitch
     assert frame(good, memory=3) == -1                                         # unknown memory kind
@@ -353,7 +317,7 @@ def test_array_rejections_leave_the_array_untouched(g, ctx, rt_arrays):
     im = N.GsImage(good, 128, 128, 0, N.GS_PIX_RGBA16F, N.GS_MEM_ARRAY)
     assert lib.gs_unshuffle_bands(ctx.handle, C.c_void_p(gathered.data_ptr()), 2, 1, 64, N.GS_PIX_RGBA16F, C.byref(im)) == -1
     ctx.sync()
-    assert unchanged(good) and unchanged(rt_arrays.live[2])
+    assert unchanged(good) and unchanged(no_surface)
     # and the same array, correctly described, is accepted
     assert frame(good) == 0
     ctx.sync()

@@ -13,7 +13,7 @@ import dataclasses
 import numpy as np
 import pytest
 
-from cuda_arrays import Cudart
+from images import SharedArray, bits, ca, to_device, to_host  # noqa: F401
 from util import POSES, near_plane_camera, near_plane_scene, splat_records, xr_eye
 
 pytestmark = pytest.mark.gpu
@@ -25,31 +25,6 @@ QUALITIES = ("Medium", "VeryHigh")     # chunked: the chunk-box cull decides fir
 @pytest.fixture(scope="module")
 def assets(g):
     return {q: g.synthetic_asset(g.SCENE_CLUSTERED, N, SEED, q) for q in QUALITIES}
-
-
-@pytest.fixture
-def ca(ctx):
-    c = Cudart()
-    yield c
-    ctx.sync()
-    c.free_all()
-
-
-def _bits(a):
-    a = np.ascontiguousarray(a)
-    return a.view(np.uint16) if a.dtype == np.float16 else a.view(np.uint32)
-
-
-def _tensor(host):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(host)).cuda()
-
-
-def _host(ctx, t):
-    import torch
-    ctx.sync()
-    torch.cuda.synchronize()
-    return t.cpu().numpy()
 
 
 def frame_vs_oracle(g, O, ctx, asset, cam, blend=0, selected=None, depth=None, localToWorld=None):
@@ -92,7 +67,7 @@ def _compare(g, O, ctx, r, asset, cam, blend, selected, depth):
     assert bad.size == 0, "SplatViewData differs for %d splats, first %s" % (bad.size, bad[:5])
     rt2 = np.zeros_like(rt)
     r.DrawSplats(cam, rt2)
-    assert np.array_equal(_bits(rt2), _bits(rt)), "the staged draw differs from the fused frame"
+    assert np.array_equal(bits(rt2), bits(rt)), "the staged draw differs from the fused frame"
     return ref, entries
 
 
@@ -193,7 +168,6 @@ def test_pose_is_bit_exact(g, O, ctx, assets, pose, quality):
 
 # ---- 2. XR eyes: a stereo camera run into two layers, and per-eye depth layers ------------------------------------------------
 def test_xr_stereo_run_on_layers_is_the_eye_loop(g, ctx, assets, ca):
-    from test_gpu_layered_targets import Layered
     W = H = 256
     eyes = [xr_eye(g, e, W, H) for e in range(2)]
     mats = [np.eye(4, dtype=np.float32), g.trs(position=(-0.6, 0.1, 0.4)).astype(np.float32)]
@@ -207,19 +181,16 @@ def test_xr_stereo_run_on_layers_is_the_eye_loop(g, ctx, assets, ca):
     loop = renderers()
     want = []
     for cam in eyes:
-        rt = _tensor(np.zeros((H, W, 4), np.float16))
+        rt = to_device(np.zeros((H, W, 4), np.float16))
         assert len(g.SortAndRenderSplatsMulti(loop, cam, rt)) == 2
-        want.append(_host(ctx, rt))
+        want.append(to_host(ctx, rt))
     want_orders = [r.readback_order() for r in loop]
     assert all(x.any() for x in want) and not np.array_equal(want[0], want[1])
     call = renderers()
-    A = Layered(g, ca, W, H, 3)
-    actives = g.SortAndRenderCameras(call, eyes, [A.image(0), A.image(1)])
+    A = SharedArray(g, ca, W, H, 3)
+    actives = g.SortAndRenderCameras(call, eyes, [A.view(layer=0), A.view(layer=1)])
     assert g.renderer.cameras_in_one_call(actives)
-    ctx.sync()
-    got = A.read()
-    for e in range(2):
-        assert np.array_equal(_bits(got[e]), _bits(want[e])), "eye %d differs" % e
+    A.check(ctx, [(e, 0, 0, want[e]) for e in range(2)], "eyes")
     for r, o in zip(call, want_orders):
         assert np.array_equal(r.readback_order(), o)
     for r in loop + call:
@@ -227,12 +198,11 @@ def test_xr_stereo_run_on_layers_is_the_eye_loop(g, ctx, assets, ca):
 
 
 def test_xr_eyes_with_depth_layers_equal_the_oracle(g, O, ctx, assets, ca):
-    from test_gpu_depth_arrays import depth_array
     W = H = 256
     asset = assets["Medium"]
     eyes = [xr_eye(g, e, W, H) for e in range(2)]
     depths = [wall(eyes[0], 2.5), np.ascontiguousarray(wall(eyes[1], 2.5)[:, ::-1])]
-    da = depth_array(ca, W, H, 2, np.stack(depths))
+    da = ca.array(W, H, 2, np.float32, 1, fill=np.stack(depths))
     for e, cam in enumerate(eyes):
         r = g.GaussianSplatRenderer(asset, ctx)
         r.sceneDepth = g.CudaArrayDepth(da, W, H, layer=e)
@@ -275,7 +245,7 @@ def test_emulated_group_at_pose_equals_one_gpu(g, ctx, assets, pose):
             rts = [np.zeros_like(rt) for _ in range(3)]
             grp.SortAndRenderSplats(cam, rts=rts)
             for i in range(3):
-                assert np.array_equal(_bits(rts[i]), _bits(rt)), "%s member %d" % (q, i)
+                assert np.array_equal(bits(rts[i]), bits(rt)), "%s member %d" % (q, i)
         finally:
             grp.close()
 

@@ -4,31 +4,12 @@ splat with an inf colour reaches them.  The oracle has none of these shortcuts: 
 import numpy as np
 import pytest
 
-from util import camera, splat_records, world_at_pixel, pixels_per_unit, view_fields
+from util import CAP_ENTRIES, CAP_H, CAP_SPLATS, CAP_W, bin_row_splats, camera, splat_records, world_at_pixel, pixels_per_unit, view_fields
 
 pytestmark = pytest.mark.gpu
 
 
 # ---- the bin list at its capacity ---------------------------------------------------------------------------------------
-CAP_W, CAP_H = 4096, 2048         # 64 x 32 bins: two 6-bit sort passes
-CAP_ENTRIES = 4 << 20             # clamp(8 N, 4 Mi, 768 Mi) for N < 512 Ki
-CAP_SPLATS = CAP_ENTRIES // 64    # one full bin row (64 entries) each
-
-
-def _bin_row_splats(cam, n, seed):
-    """n wide, flat splats: each one's visible part spans the whole screen width and 5 rows inside one 64-pixel bin row, so
-    it emits exactly 64 (bin, splat) entries while the oracle visits only about 4096 x 9 pixels of it."""
-    rng = np.random.default_rng(seed)
-    i = np.arange(n)
-    depth = 5.0 + 3.0 * rng.random(n)
-    cy = 64.0 * (i % (CAP_H // 64)) + 20.0 + (i // (CAP_H // 64)) % 25
-    pos = world_at_pixel(cam, CAP_W / 2, cy, depth)
-    ppu = pixels_per_unit(cam, depth)[:, None]
-    scale = np.array([0.3 * CAP_W, 0.01, 0.01]) / ppu      # axis1 ~ 0.42 W: the quad reaches 0.85 W beyond the centre
-    dc = rng.random((n, 3)) * 2.0 - 0.5
-    return splat_records(pos, scale, 0.05 + 0.3 * rng.random(n), dc)
-
-
 def _cap_frame(g, ctx, r, cam, rt=None):
     if rt is None:
         rt = np.zeros((CAP_H, CAP_W, 4), np.float16)
@@ -44,7 +25,7 @@ def test_bin_list_exact_capacity_overflow_and_recovery(g, O):
     renderers = []   # disposed before the context is closed, also when an assertion fails
     try:
         cam = camera(g, CAP_W, CAP_H)
-        rec = _bin_row_splats(cam, CAP_SPLATS + 1, 0xCA9)
+        rec = bin_row_splats(cam, CAP_SPLATS + 1, 0xCA9)
         T = O.max_threads()
 
         # exact capacity

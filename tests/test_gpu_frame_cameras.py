@@ -2,261 +2,17 @@
 stands for -- gs_frame_objects per camera.  Every comparison is bit for bit, on every render target, every camera target and
 every asset's persistent draw order and sorted keys.  The loop and the call each own a copy of every asset, on one context;
 an asset appears in several cameras, so its draw order chains from camera to camera."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
+from frame_loops import CAM_SIZES, Twins, call_cameras, compare, g_trs, loop_cameras, mixed_assets, mixed_setup, orbit
+from images import ca  # noqa: F401
 from util import camera, splat_records
 
 pytestmark = pytest.mark.gpu
 
 INVALID, OOM = -1, -3
-
-
-class _Cudart:
-    """CUDA arrays (GS_MEM_ARRAY images) through the runtime torch loaded."""
-
-    class _Desc(C.Structure):
-        _fields_ = [("x", C.c_int), ("y", C.c_int), ("z", C.c_int), ("w", C.c_int), ("f", C.c_int)]
-
-    def __init__(self):
-        import torch
-        torch.cuda.init()
-        self.lib = C.CDLL("libcudart.so.12")
-        self.lib.cudaMallocArray.argtypes = [C.POINTER(C.c_void_p), C.POINTER(self._Desc), C.c_size_t, C.c_size_t, C.c_uint]
-        self.lib.cudaMemcpy2DToArray.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
-        self.lib.cudaMemcpy2DFromArray.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
-        self.lib.cudaFreeArray.argtypes = [C.c_void_p]
-        self.live = []
-
-    def array(self, g, host):
-        h = C.c_void_p()
-        bits = 8 * host.itemsize
-        assert self.lib.cudaMallocArray(C.byref(h), C.byref(self._Desc(bits, bits, bits, bits, 2)), host.shape[1], host.shape[0], 2) == 0
-        self.live.append(h.value)
-        row = host.shape[1] * 4 * host.itemsize
-        assert self.lib.cudaMemcpy2DToArray(h.value, 0, 0, host.ctypes.data, row, row, host.shape[0], 1) == 0
-        return g.CudaArrayImage(h.value, host.shape[1], host.shape[0], host.dtype)
-
-    def read(self, im):
-        out = np.empty(im.shape, im.dtype)
-        row = im.width * 4 * out.itemsize
-        assert self.lib.cudaMemcpy2DFromArray(out.ctypes.data, row, im.handle, 0, 0, row, im.height, 2) == 0
-        return out
-
-    def free_all(self):
-        for h in self.live:
-            self.lib.cudaFreeArray(h)
-        self.live = []
-
-
-@pytest.fixture
-def ca(ctx):
-    c = _Cudart()
-    yield c
-    ctx.sync()
-    c.free_all()
-
-
-def _make(kind, host, g, ca):
-    import torch
-    if kind is None:
-        return None
-    if kind == "host":
-        return host.copy()
-    if kind == "device":
-        return torch.from_numpy(host.copy()).cuda()
-    return ca.array(g, np.ascontiguousarray(host))
-
-
-def _read(im, ca):
-    if im is None:
-        return None
-    if isinstance(im, np.ndarray):
-        return im.copy()
-    if hasattr(im, "handle"):
-        return ca.read(im)
-    return im.cpu().numpy()
-
-
-def _bits(a):
-    return None if a is None else a.view(np.uint16 if a.dtype == np.float16 else np.uint32)
-
-
-def _opt(N, blend, flags=0):
-    o = N.GsRenderOptions()
-    o.blend_mode, o.flags = blend, flags
-    return o
-
-
-def _next_sort(r):
-    s = 1 if r.m_FrameCounter % max(1, int(r.m_SortNthFrame)) == 0 else 0
-    r.m_FrameCounter += 1
-    return s
-
-
-def _params(g, r, cam, extra=None):
-    kw = dict(localToWorld=r.localToWorldMatrix, splat_scale=r.m_SplatScale, opacity_scale=r.m_OpacityScale, sh_order=r.m_SHOrder,
-              sh_only=r.m_SHOnly, cutouts=r.m_Cutouts, deleted_bits=r.m_DeletedBits, splat_count=r.splatCount,
-              selected_bits=r.m_SelectedBits, scene_depth=r.sceneDepth)
-    kw.update(extra or {})
-    return g.make_frame_params(cam, **kw)
-
-
-def _args(g, per_cam, cams, extras):
-    """Camera-major (assets, fps, do_sort) of per_cam[c] = renderers of camera c; extras[c][k]: make_frame_params overrides."""
-    from unitygaussiansplatting_b200 import _native as N
-    n = sum(len(rs) for rs in per_cam)
-    fps, assets, ds, keep = (N.GsFrameParams * n)(), (C.c_void_p * n)(), (C.c_int32 * n)(), []
-    i = 0
-    for c, (rs, cam) in enumerate(zip(per_cam, cams)):
-        for k, r in enumerate(rs):
-            fp, kp = _params(g, r, cam, extras[c][k] if extras else None)
-            fps[i], assets[i], ds[i] = fp, r._asset.value, _next_sort(r)
-            r.sorted_once = getattr(r, "sorted_once", False) or bool(ds[i])
-            keep.append(kp)
-            i += 1
-    return fps, assets, ds, keep
-
-
-def loop_cameras(g, ctx, per_cam, cams, blend, rts, tgts, extras=None):
-    """The definition: gs_frame_objects per camera."""
-    from unitygaussiansplatting_b200 import _native as N
-    from unitygaussiansplatting_b200.renderer import _image
-    lib = N.native()
-    fps, assets, ds, keep = _args(g, per_cam, cams, extras)
-    off = 0
-    for c, cam in enumerate(cams):
-        W, H = cam.pixelWidth, cam.pixelHeight
-        a = _image(rts[c], W, H) if rts[c] is not None else None
-        b = _image(tgts[c], W, H) if tgts[c] is not None else None
-        k = len(per_cam[c])
-        P = C.POINTER(N.GsFrameParams)
-        rc = lib.gs_frame_objects(ctx.handle, k, C.cast(C.byref(assets, off * C.sizeof(C.c_void_p)), C.POINTER(C.c_void_p)),
-                                  C.cast(C.byref(fps, off * C.sizeof(N.GsFrameParams)), P),
-                                  C.cast(C.byref(ds, off * 4), C.POINTER(C.c_int32)), C.byref(_opt(N, blend)),
-                                  C.byref(a) if a is not None else None, C.byref(b) if b is not None else None)
-        N.check(ctx.handle, rc)
-        off += k
-    del keep
-
-
-def call_cameras(g, ctx, per_cam, cams, blend, rts, tgts, extras=None, flags=0, check=True, counts=None, patch=None):
-    from unitygaussiansplatting_b200 import _native as N
-    from unitygaussiansplatting_b200.renderer import _image
-    lib = N.native()
-    fps, assets, ds, keep = _args(g, per_cam, cams, extras)
-    ims = []
-    for c, cam in enumerate(cams):
-        W, H = cam.pixelWidth, cam.pixelHeight
-        ims.append((_image(rts[c], W, H) if rts[c] is not None else None, _image(tgts[c], W, H) if tgts[c] is not None else None))
-    if patch:
-        patch(ims)
-    PI = C.POINTER(N.GsImage)
-    a = (PI * len(cams))(*[C.pointer(x) if x is not None else PI() for x, _ in ims])
-    b = (PI * len(cams))(*[C.pointer(y) if y is not None else PI() for _, y in ims])
-    counts = counts if counts is not None else [len(rs) for rs in per_cam]
-    cnt = (C.c_uint32 * len(cams))(*counts)
-    rc = lib.gs_frame_cameras(ctx.handle, len(cams), cnt, assets, fps, ds, C.byref(_opt(N, blend, flags)), a, b)
-    del keep
-    if check:
-        N.check(ctx.handle, rc)
-    return rc
-
-
-def orbit(g, f, W, H, radius=6.0, phase=0.0):
-    t = 0.35 * f + phase
-    pos = np.array([radius * np.sin(t), 0.6, -radius * np.cos(t)])
-    return camera(g, W, H, pos=tuple(pos), forward=tuple(-pos / np.linalg.norm(pos)))
-
-
-class Twins:
-    """Every asset twice on one context: `loop` draws with loop_cameras, `call` with gs_frame_cameras."""
-
-    def __init__(self, g, ctx, assets, setup=None):
-        self.loop = [g.GaussianSplatRenderer(a, ctx) for a in assets]
-        self.call = [g.GaussianSplatRenderer(a, ctx) for a in assets]
-        for i, (p, q) in enumerate(zip(self.loop, self.call)):
-            if setup:
-                setup(i, p)
-                setup(i, q)
-
-    def pick(self, idx_per_cam):
-        return [[self.loop[i] for i in ix] for ix in idx_per_cam], [[self.call[i] for i in ix] for ix in idx_per_cam]
-
-    def gathered(self, g, subsets, cams):
-        """GatherSplatsForCamera order of each camera's subset of the assets."""
-        out = []
-        for ix, cam in zip(subsets, cams):
-            rs = g.GatherSplatsForCamera([self.loop[i] for i in ix], cam)
-            out.append([self.loop.index(r) for r in rs])
-        return out
-
-    def check_state(self):
-        for p, q in zip(self.loop, self.call):
-            assert np.array_equal(p.readback_order(), q.readback_order()), "draw order"
-            assert getattr(p, "sorted_once", False) == getattr(q, "sorted_once", False)
-            if getattr(p, "sorted_once", False):   # the keys buffer of an asset never sorted holds whatever its allocation held
-                assert np.array_equal(p.readback_keys(), q.readback_keys()), "sorted keys"
-
-    def dispose(self):
-        for r in self.loop + self.call:
-            r.Dispose()
-
-
-def compare(g, ctx, ca, tw, idx_per_cam, cams, blend, dtype, rt_kinds, tgt_kinds, what, extras=None):
-    lo, hi = tw.pick(idx_per_cam)
-    loop_rts, call_rts, loop_tgts, call_tgts = [], [], [], []
-    for c, cam in enumerate(cams):
-        W, H = cam.pixelWidth, cam.pixelHeight
-        dt = dtype[c] if isinstance(dtype, (list, tuple)) else dtype
-        tgt0 = (np.random.default_rng(W * 7 + H + c).random((H, W, 4), np.float32) * 0.5).astype(dt)
-        rk, tk = rt_kinds[c], tgt_kinds[c]
-        loop_rts.append(_make(rk, np.zeros((H, W, 4), dt), g, ca))
-        call_rts.append(_make(rk, np.full((H, W, 4), 7, dt), g, ca))   # the call clears each target itself
-        loop_tgts.append(_make(tk, tgt0, g, ca))
-        call_tgts.append(_make(tk, tgt0, g, ca))
-    loop_cameras(g, ctx, lo, cams, blend, loop_rts, loop_tgts, extras)
-    call_cameras(g, ctx, hi, cams, blend, call_rts, call_tgts, extras)
-    ctx.sync()
-    drawn = 0
-    for c in range(len(cams)):
-        want_rt, want_tgt = _read(loop_rts[c], ca), _read(loop_tgts[c], ca)
-        if want_rt is not None:
-            drawn += int(want_rt.any())
-            assert np.array_equal(_bits(_read(call_rts[c], ca)), _bits(want_rt)), "%s: camera %d render target" % (what, c)
-        if want_tgt is not None:
-            assert np.array_equal(_bits(_read(call_tgts[c], ca)), _bits(want_tgt)), "%s: camera %d camera target" % (what, c)
-    tw.check_state()
-    return drawn
-
-
-QUALITIES = ["Medium", "VeryHigh", "Low", "VeryLow", "Medium", "VeryHigh", "Medium", "VeryHigh"]
-SIZES = [6000, 7000, 20000, 9000, 10000, 5000, 4000, 3000]
-CAM_SIZES = [(320, 200), (256, 256), (97, 61), (200, 320), (64, 48)]
 KINDS = ["host", "device", "array", None]
-
-
-def _mixed_assets(g, n):
-    return [g.synthetic_asset(g.SCENE_CLUSTERED, SIZES[i], 0xCA3E0F00 + i, QUALITIES[i]) for i in range(n)]
-
-
-def _setup(i, r):
-    s = -1.0 if i == 1 else 1.0
-    r.localToWorldMatrix = g_trs(position=(1.4 * i - 2.0, 0.2 * i, 0.8 * (i % 2)), scale=(0.8 * s, 0.8, 0.8))
-    r.m_SHOrder = (3, 1, 0, 2, 3, 1)[i % 6]
-    r.m_SortNthFrame = (1, 2, 1, 3, 1, 2)[i % 6]
-    if i == 0:
-        r.m_Cutouts = [(np.diag([1 / 0.8, 1 / 0.8, 1 / 0.8, 1.0]).astype(np.float32), 1 | 0x100)]
-    if i == 2:
-        bits = np.random.default_rng(i).integers(0, 2 ** 32, (r.splatCount + 31) // 32, dtype=np.uint64).astype(np.uint32)
-        r.m_DeletedBits = bits & np.uint32(0x11111111)
-
-
-def g_trs(**kw):
-    import unitygaussiansplatting_b200 as pkg
-    return pkg.trs(**kw).astype(np.float32)
 
 
 # ---- 1. equal to the loop -------------------------------------------------------------------------------------------------
@@ -264,7 +20,7 @@ def g_trs(**kw):
 @pytest.mark.parametrize("blend", [0, 1])
 @pytest.mark.parametrize("dtype", [np.float16, np.float32])
 def test_cameras_equal_the_loop(g, ctx, ca, ncam, blend, dtype):
-    tw = Twins(g, ctx, _mixed_assets(g, 5), _setup)
+    tw = Twins(g, ctx, mixed_assets(g, 5), mixed_setup)
     try:
         for f in range(3):
             cams = [orbit(g, f, *CAM_SIZES[c], phase=0.9 * c) for c in range(ncam)]
@@ -279,13 +35,13 @@ def test_cameras_equal_the_loop(g, ctx, ca, ncam, blend, dtype):
 
 def test_python_mirror_matches_the_loop(g, ctx):
     """SortAndRenderCameras takes the one call; its twin draws camera by camera with SortAndRenderSplatsMulti."""
-    assets = _mixed_assets(g, 4)
+    assets = mixed_assets(g, 4)
     a = [g.GaussianSplatRenderer(x, ctx) for x in assets]
     b = [g.GaussianSplatRenderer(x, ctx) for x in assets]
     try:
         for i in range(4):
-            _setup(i, a[i])
-            _setup(i, b[i])
+            mixed_setup(i, a[i])
+            mixed_setup(i, b[i])
         for f in range(3):
             cams = [orbit(g, f, *CAM_SIZES[c], phase=0.7 * c) for c in range(3)]
             ra = [np.zeros((c.pixelHeight, c.pixelWidth, 4), np.float16) for c in cams]
@@ -349,7 +105,7 @@ def test_order_chaining(g, ctx, ca):
 # ---- 3. run boundaries ----------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("counts", [[6, 6, 2, 2, 1], [4, 4, 4, 3, 2]])
 def test_seventeen_pairs_make_two_runs(g, ctx, ca, counts):
-    tw = Twins(g, ctx, _mixed_assets(g, 6), _setup)
+    tw = Twins(g, ctx, mixed_assets(g, 6), mixed_setup)
     try:
         for f in range(2):
             cams = [orbit(g, f, *CAM_SIZES[c], phase=0.5 * c) for c in range(len(counts))]
@@ -369,7 +125,7 @@ def test_seventeen_pairs_make_two_runs(g, ctx, ca, counts):
 def test_two_camera_runs_in_one_call(g, ctx, ca, counts, dtypes):
     """The second run's first emit keeps the overflow flag of the first, the run scratch is laid out again, and each run's camera
     layout keeps its own tile-cost history over the frames."""
-    tw = Twins(g, ctx, _mixed_assets(g, 8), _setup)
+    tw = Twins(g, ctx, mixed_assets(g, 8), mixed_setup)
     try:
         for f in range(3):
             cams = [orbit(g, f, *CAM_SIZES[c], phase=0.5 * c) for c in range(len(counts))]
@@ -382,7 +138,7 @@ def test_two_camera_runs_in_one_call(g, ctx, ca, counts, dtypes):
 
 
 def test_large_camera_between_small_ones(g, ctx, ca):
-    tw = Twins(g, ctx, _mixed_assets(g, 3), _setup)
+    tw = Twins(g, ctx, mixed_assets(g, 3), mixed_setup)
     try:
         cams = [orbit(g, 1, 97, 61), orbit(g, 1, 8200, 64, phase=0.2), orbit(g, 1, 256, 256, phase=0.4)]
         idx = tw.gathered(g, [[0, 1], [1, 2], [2, 0]], cams)
@@ -414,7 +170,7 @@ def test_camera_of_seventeen_objects_between_small_ones(g, ctx, ca):
 
 def test_own_depth_buffer_per_camera(g, ctx, ca):
     import torch
-    tw = Twins(g, ctx, _mixed_assets(g, 3), _setup)
+    tw = Twins(g, ctx, mixed_assets(g, 3), mixed_setup)
     try:
         cams = [orbit(g, 0, 320, 200), orbit(g, 0, 256, 256, phase=0.6)]
         d0 = np.full((200, 320), 0.02, np.float32)
@@ -431,7 +187,7 @@ def test_own_depth_buffer_per_camera(g, ctx, ca):
 
 
 def test_selection_on_one_camera(g, ctx, ca):
-    tw = Twins(g, ctx, _mixed_assets(g, 2), _setup)
+    tw = Twins(g, ctx, mixed_assets(g, 2), mixed_setup)
     try:
         cams = [orbit(g, 2, 320, 200), orbit(g, 2, 97, 61, phase=0.3)]
         idx = tw.gathered(g, [[0, 1], [0, 1]], cams)
@@ -443,7 +199,7 @@ def test_selection_on_one_camera(g, ctx, ca):
 
 
 def test_camera_with_everything_off_screen(g, ctx, ca):
-    tw = Twins(g, ctx, _mixed_assets(g, 2), _setup)
+    tw = Twins(g, ctx, mixed_assets(g, 2), mixed_setup)
     try:
         away = camera(g, 128, 96, pos=(0.0, 0.5, -60.0), forward=(0.0, 0.0, -1.0))
         cams = [orbit(g, 0, 320, 200), away, orbit(g, 1, 97, 61)]
@@ -548,7 +304,7 @@ def test_overflow_kept_across_a_growing_camera(g, host):
 # ---- 6. refused inputs ----------------------------------------------------------------------------------------------------
 def test_refused_inputs_write_nothing(g, ctx, ca):
     from unitygaussiansplatting_b200 import _native as N
-    tw = Twins(g, ctx, _mixed_assets(g, 2), _setup)
+    tw = Twins(g, ctx, mixed_assets(g, 2), mixed_setup)
     try:
         cams = [orbit(g, 0, 320, 200), orbit(g, 0, 97, 61, phase=0.5)]
         rs = tw.call
@@ -587,7 +343,7 @@ def test_refused_inputs_write_nothing(g, ctx, ca):
 # ---- 7. one camera --------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("nobj", [1, 3])
 def test_one_camera_is_frame_objects(g, ctx, ca, nobj):
-    tw = Twins(g, ctx, _mixed_assets(g, 3), _setup)
+    tw = Twins(g, ctx, mixed_assets(g, 3), mixed_setup)
     try:
         ctx.set_timing(True)
         cam = orbit(g, 2, 320, 200)

@@ -1,191 +1,23 @@
 """gs_frame_objects: several splat objects of one camera drawn by one call on one GPU, against the per-object loop it stands
 for -- gs_frame per object (GS_FLAG_LOAD_RT from the second on), then gs_composite.  Every comparison is bit for bit, on the
-render target, the camera target and every object's persistent draw order, over several orbit frames (so the orders evolve
-and the objects' draw order changes).  The loop and the call each own a copy of every object, on the same context."""
+render target, the camera target and every object's persistent draw order and sorted keys, over several orbit frames (so the
+orders evolve and the objects' draw order changes).  The loop and the call each own a copy of every object, on the same
+context (frame_loops.Twins)."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
-from util import camera, splat_records, world_at_pixel, pixels_per_unit
+from frame_loops import Twins, call_frame, compare_frame, frame_args, loop_frame, mixed_assets, next_sort, orbit
+from images import ca  # noqa: F401
+from util import CAP_ENTRIES, CAP_H, CAP_SPLATS, CAP_W, bin_row_splats, camera, pixels_per_unit, splat_records, world_at_pixel
 
 pytestmark = pytest.mark.gpu
 
 INVALID, OOM = -1, -3
 
 
-class _Cudart:
-    """CUDA arrays (GS_MEM_ARRAY images) through the runtime torch loaded."""
-
-    class _Desc(C.Structure):
-        _fields_ = [("x", C.c_int), ("y", C.c_int), ("z", C.c_int), ("w", C.c_int), ("f", C.c_int)]
-
-    def __init__(self):
-        import torch
-        torch.cuda.init()
-        self.lib = C.CDLL("libcudart.so.12")
-        self.lib.cudaMallocArray.argtypes = [C.POINTER(C.c_void_p), C.POINTER(self._Desc), C.c_size_t, C.c_size_t, C.c_uint]
-        self.lib.cudaMemcpy2DToArray.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
-        self.lib.cudaMemcpy2DFromArray.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
-        self.lib.cudaFreeArray.argtypes = [C.c_void_p]
-        self.live = []
-
-    def array(self, g, host):
-        h = C.c_void_p()
-        bits = 8 * host.itemsize
-        assert self.lib.cudaMallocArray(C.byref(h), C.byref(self._Desc(bits, bits, bits, bits, 2)), host.shape[1], host.shape[0], 2) == 0
-        self.live.append(h.value)
-        row = host.shape[1] * 4 * host.itemsize
-        assert self.lib.cudaMemcpy2DToArray(h.value, 0, 0, host.ctypes.data, row, row, host.shape[0], 1) == 0
-        return g.CudaArrayImage(h.value, host.shape[1], host.shape[0], host.dtype)
-
-    def read(self, im):
-        out = np.empty(im.shape, im.dtype)
-        row = im.width * 4 * out.itemsize
-        assert self.lib.cudaMemcpy2DFromArray(out.ctypes.data, row, im.handle, 0, 0, row, im.height, 2) == 0
-        return out
-
-    def free_all(self):
-        for h in self.live:
-            self.lib.cudaFreeArray(h)
-        self.live = []
-
-
-@pytest.fixture
-def ca(ctx):
-    c = _Cudart()
-    yield c
-    ctx.sync()
-    c.free_all()
-
-
-def _make(kind, host, g, ca):
-    """The same starting image in host, device or CUDA-array memory (None: no image)."""
-    import torch
-    if kind is None:
-        return None
-    if kind == "host":
-        return host.copy()
-    if kind == "device":
-        return torch.from_numpy(host.copy()).cuda()
-    return ca.array(g, np.ascontiguousarray(host))
-
-
-def _read(im, ca):
-    if im is None:
-        return None
-    if isinstance(im, np.ndarray):
-        return im.copy()
-    if hasattr(im, "handle"):
-        return ca.read(im)
-    return im.cpu().numpy()
-
-
-def _bits(a):
-    return None if a is None else a.view(np.uint16 if a.dtype == np.float16 else np.uint32)
-
-
-def _opt(N, blend, flags=0):
-    o = N.GsRenderOptions()
-    o.blend_mode, o.flags = blend, flags
-    return o
-
-
-def _next_sort(r):
-    s = 1 if r.m_FrameCounter % max(1, int(r.m_SortNthFrame)) == 0 else 0
-    r.m_FrameCounter += 1
-    return s
-
-
-def loop_frame(g, ctx, rs, cam, blend, rt, tgt):
-    """The definition: gs_frame per object, GS_FLAG_LOAD_RT from the second on, then gs_composite."""
-    from unitygaussiansplatting_b200 import _native as N
-    from unitygaussiansplatting_b200.renderer import _image
-    lib = N.native()
-    W, H = cam.pixelWidth, cam.pixelHeight
-    a = _image(rt, W, H)
-    b = _image(tgt, W, H) if tgt is not None else None
-    for k, r in enumerate(rs):
-        fp, opt = r.frame_params(cam), _opt(N, blend, N.GS_FLAG_LOAD_RT if k else 0)
-        N.check(ctx.handle, lib.gs_frame(ctx.handle, r._asset, C.byref(fp), C.byref(opt), _next_sort(r), C.byref(a), None))
-    if b is not None:
-        N.check(ctx.handle, lib.gs_composite(ctx.handle, C.byref(a), C.byref(b)))
-
-
-def call_frame(g, ctx, rs, cam, blend, rt, tgt, flags=0, check=True):
-    from unitygaussiansplatting_b200 import _native as N
-    from unitygaussiansplatting_b200.renderer import _image
-    lib = N.native()
-    W, H = cam.pixelWidth, cam.pixelHeight
-    k = len(rs)
-    fps, assets, ds = (N.GsFrameParams * k)(), (C.c_void_p * k)(), (C.c_int32 * k)()
-    for i, r in enumerate(rs):
-        fps[i], assets[i], ds[i] = r.frame_params(cam), r._asset.value, _next_sort(r)
-    a = _image(rt, W, H) if rt is not None else None
-    b = _image(tgt, W, H) if tgt is not None else None
-    opt = _opt(N, blend, flags)
-    rc = lib.gs_frame_objects(ctx.handle, k, assets, fps, ds, C.byref(opt), C.byref(a) if a is not None else None,
-                              C.byref(b) if b is not None else None)
-    if check:
-        N.check(ctx.handle, rc)
-    return rc
-
-
-def orbit(g, f, W=320, H=200, radius=6.0):
-    t = 0.35 * f
-    pos = np.array([radius * np.sin(t), 0.6, -radius * np.cos(t)])
-    return camera(g, W, H, pos=tuple(pos), forward=tuple(-pos / np.linalg.norm(pos)))
-
-
-class Twins:
-    """Every object twice on one context: `loop` draws with loop_frame, `call` with gs_frame_objects."""
-
-    def __init__(self, g, ctx, assets, setup):
-        self.loop = [g.GaussianSplatRenderer(a, ctx) for a in assets]
-        self.call = [g.GaussianSplatRenderer(a, ctx) for a in assets]
-        for i, (p, q) in enumerate(zip(self.loop, self.call)):
-            setup(i, p)
-            setup(i, q)
-
-    def ordered(self, g, cam):
-        """GatherSplatsForCamera order, the same for both copies."""
-        idx = [self.loop.index(r) for r in g.GatherSplatsForCamera(self.loop, cam)]
-        return [self.loop[i] for i in idx], [self.call[i] for i in idx]
-
-    def check_orders(self):
-        for p, q in zip(self.loop, self.call):
-            assert np.array_equal(p.readback_order(), q.readback_order())
-
-    def dispose(self):
-        for r in self.loop + self.call:
-            r.Dispose()
-
-
-def _compare_frame(g, ctx, ca, tw, cam, blend, dtype, rt_kind, tgt_kind, what):
-    W, H = cam.pixelWidth, cam.pixelHeight
-    rng = np.random.default_rng(W + H)
-    tgt0 = (rng.random((H, W, 4), np.float32) * 0.5).astype(dtype)
-    lo, hi = tw.ordered(g, cam)
-    # without an rt the call draws into RGBA16F library scratch, as gs_frame does
-    loop_rt = _make(rt_kind or "device", np.zeros((H, W, 4), dtype if rt_kind else np.float16), g, ca)
-    loop_tgt, call_tgt = _make(tgt_kind, tgt0, g, ca), _make(tgt_kind, tgt0, g, ca)
-    call_rt = _make(rt_kind, np.full((H, W, 4), 7, dtype), g, ca)   # the call clears the target itself
-    loop_frame(g, ctx, lo, cam, blend, loop_rt, loop_tgt)
-    call_frame(g, ctx, hi, cam, blend, call_rt, call_tgt)
-    ctx.sync()
-    want_rt, want_tgt = _read(loop_rt, ca), _read(loop_tgt, ca)
-    assert want_rt.any(), what
-    if call_rt is not None:
-        assert np.array_equal(_bits(_read(call_rt, ca)), _bits(want_rt)), what + ": render target"
-    if call_tgt is not None:
-        assert np.array_equal(_bits(_read(call_tgt, ca)), _bits(want_tgt)), what + ": camera target"
-    tw.check_orders()
-    return want_rt
-
-
 # ---- 1. mixed scenes ------------------------------------------------------------------------------------------------------
-QUALITIES = ["Medium", "VeryHigh", "Low", "VeryLow", "Medium"]
-SIZES = [6000, 7000, 20000, 9000, 10000]    # Low clusters SH into 16k entries: it needs more splats than that
 RT_KINDS = ["host", "device", "array", None]
 TGT_KINDS = [None, "host", "device", "array"]
 
@@ -194,7 +26,7 @@ TGT_KINDS = [None, "host", "device", "array"]
 @pytest.mark.parametrize("blend", [0, 1])
 @pytest.mark.parametrize("dtype", [np.float16, np.float32])
 def test_mixed_scenes_equal_the_loop(g, ctx, ca, K, blend, dtype):
-    assets = [g.synthetic_asset(g.SCENE_CLUSTERED, SIZES[i], 0x5EED0F00 + i, QUALITIES[i]) for i in range(K)]
+    assets = mixed_assets(g, K, 0x5EED0F00)
 
     def setup(i, r):
         s = -1.0 if i == 1 else 1.0    # object 1 is mirrored
@@ -212,7 +44,7 @@ def test_mixed_scenes_equal_the_loop(g, ctx, ca, K, blend, dtype):
         for f in range(4):
             rt_kind = RT_KINDS[f]
             tgt_kind = TGT_KINDS[(f + K) % 4] if rt_kind is not None else "device"
-            _compare_frame(g, ctx, ca, tw, orbit(g, f), blend, dtype, rt_kind, tgt_kind,
+            compare_frame(g, ctx, ca, tw, orbit(g, f), blend, dtype, rt_kind, tgt_kind,
                            "frame %d (rt %s, target %s)" % (f, rt_kind, tgt_kind))
     finally:
         tw.dispose()
@@ -236,7 +68,7 @@ def test_async_readback_equals_the_loop(g, ctx):
         call_frame(g, ctx, hi, cam, 0, pin.numpy(), None, flags=1)
         ctx.sync()
         assert want.any() and np.array_equal(pin.numpy().view(np.uint16), want.view(np.uint16))
-        tw.check_orders()
+        tw.check_state()
     finally:
         tw.dispose()
 
@@ -290,7 +122,7 @@ def test_selection_and_depth_in_one_run(g, ctx, ca, blend):
     tw = Twins(g, ctx, assets, setup)
     try:
         for f in range(3):
-            _compare_frame(g, ctx, ca, tw, orbit(g, f), blend, np.float16, "device", "host", "frame %d" % f)
+            compare_frame(g, ctx, ca, tw, orbit(g, f), blend, np.float16, "device", "host", "frame %d" % f)
     finally:
         tw.dispose()
 
@@ -310,8 +142,8 @@ def test_fp32_blend_into_half_rounds_at_each_object(g, ctx, ca):
     assets = [g.create_asset(rec0, "VeryHigh"), g.create_asset(rec1, "VeryHigh")]
     tw = Twins(g, ctx, assets, lambda i, r: None)
     try:
-        half = _compare_frame(g, ctx, ca, tw, cam, 1, np.float16, "host", None, "RGBA16F")
-        full = _compare_frame(g, ctx, ca, tw, cam, 1, np.float32, "host", None, "RGBA32F")
+        half = compare_frame(g, ctx, ca, tw, cam, 1, np.float16, "host", None, "RGBA16F")
+        full = compare_frame(g, ctx, ca, tw, cam, 1, np.float32, "host", None, "RGBA32F")
         differs = (full.astype(np.float16).view(np.uint16) != half.view(np.uint16)).any(-1)
         assert differs.sum() > 20, "the float result rounded once must differ where object 0's alpha rounds to 1"
         assert (half[..., 3] == 1.0).sum() > 20 and ((full[..., 3] < 1.0) & (half[..., 3] == 1.0)).any()
@@ -338,7 +170,7 @@ def test_saturated_pixels_ignore_an_inf_colour_in_a_later_object(g, ctx, ca, ble
 
     tw = Twins(g, ctx, assets, setup)
     try:
-        got = _compare_frame(g, ctx, ca, tw, cam, blend, np.float32 if blend else np.float16, "device", None, "saturation")
+        got = compare_frame(g, ctx, ca, tw, cam, blend, np.float32 if blend else np.float16, "device", None, "saturation")
         got = got.astype(np.float32)
         assert (got[..., 3] == 1.0).sum() > 100 and np.isposinf(got[..., :3]).any() and not np.isnan(got).any()
     finally:
@@ -355,7 +187,7 @@ def test_eighteen_objects_two_runs(g, ctx, ca):
     tw = Twins(g, ctx, assets, setup)
     try:
         for f in range(2):
-            _compare_frame(g, ctx, ca, tw, orbit(g, f), f, np.float16, "host", "device", "frame %d" % f)
+            compare_frame(g, ctx, ca, tw, orbit(g, f), f, np.float16, "host", "device", "frame %d" % f)
     finally:
         tw.dispose()
 
@@ -381,7 +213,7 @@ def test_two_depth_buffers_empty_and_offscreen_objects(g, ctx, ca):
     tw = Twins(g, ctx, assets, setup)
     try:
         for f in range(3):
-            _compare_frame(g, ctx, ca, tw, orbit(g, f), f % 2, np.float16, "array", "host" if f else None, "frame %d" % f)
+            compare_frame(g, ctx, ca, tw, orbit(g, f), f % 2, np.float16, "array", "host" if f else None, "frame %d" % f)
     finally:
         tw.dispose()
 
@@ -390,17 +222,16 @@ def test_two_depth_buffers_empty_and_offscreen_objects(g, ctx, ca):
 def test_summed_entries_over_capacity_and_recovery(g):
     """The construction of test_bin_list_exact_capacity_overflow_and_recovery split across two objects: 65,537 splats of 64
     entries each overflow the 4 Mi list by one splat; deleting one splat makes the next call fit exactly."""
-    import test_gpu_cull_edges as ce
     ctx = g.GaussianSplatContext(0)
     tw = None
     try:
-        cam = camera(g, ce.CAP_W, ce.CAP_H)
-        rec = ce._bin_row_splats(cam, ce.CAP_SPLATS + 1, 0xCA9)
-        half = ce.CAP_SPLATS // 2
+        cam = camera(g, CAP_W, CAP_H)
+        rec = bin_row_splats(cam, CAP_SPLATS + 1, 0xCA9)
+        half = CAP_SPLATS // 2
         assets = [g.create_asset(rec[:half].copy(), "VeryHigh"), g.create_asset(rec[half:].copy(), "VeryHigh")]
         tw = Twins(g, ctx, assets, lambda i, r: None)
         lo, hi = tw.ordered(g, cam)
-        rt = np.zeros((ce.CAP_H, ce.CAP_W, 4), np.float16)
+        rt = np.zeros((CAP_H, CAP_W, 4), np.float16)
         assert call_frame(g, ctx, hi, cam, 0, rt, None, check=False) == OOM
         from unitygaussiansplatting_b200 import _native as N
         assert "tile-list capacity exceeded" in N.native().gs_last_error(ctx.handle).decode()
@@ -413,7 +244,7 @@ def test_summed_entries_over_capacity_and_recovery(g):
         loop_frame(g, ctx, lo, cam, 0, want, None)
         got = np.zeros_like(rt)
         call_frame(g, ctx, hi, cam, 0, got, None)
-        assert ctx.stage_times().tile_entries == ce.CAP_ENTRIES
+        assert ctx.stage_times().tile_entries == CAP_ENTRIES
         assert got.any() and np.array_equal(got.view(np.uint16), want.view(np.uint16))
     finally:
         if tw:
@@ -485,7 +316,7 @@ def test_one_object_is_gs_frame(g, ctx, ca):
         n2 = ctx.stage_times().kernel_launches
         assert a.any() and np.array_equal(a.view(np.uint16), b.view(np.uint16))
         assert n2 - n1 == n1 - n0
-        tw.check_orders()
+        tw.check_state()
     finally:
         tw.dispose()
 
@@ -498,15 +329,10 @@ def test_unity_frame_objects_event_equals_a_direct_call(g, ctx):
     try:
         cam = orbit(g, 1)
         W, H = cam.pixelWidth, cam.pixelHeight
-        _lo, hi = tw.ordered(g, cam)
         direct = np.zeros((H, W, 4), np.float16)
         call_frame(g, ctx, tw.loop, cam, 0, direct, None)
-        k = len(hi)
-        fps, assets_arr, ds = (N.GsFrameParams * k)(), (C.c_void_p * k)(), (C.c_int32 * k)()
-        keep = []
-        for i, r in enumerate(tw.call):
-            fps[i], assets_arr[i], ds[i] = r.frame_params(cam), r._asset.value, _next_sort(r)
-            keep.append(r._keep)
+        k = len(tw.call)
+        assets_arr, fps, ds, keep = frame_args(g, [(cam, r, r.sceneDepth) for r in tw.call], sort=next_sort)
         via = np.zeros_like(direct)
         ev = N.GsUnityFrameObjectsEvent()
         ev.ctx, ev.object_count = C.cast(ctx.handle, C.c_void_p).value, k
@@ -519,7 +345,7 @@ def test_unity_frame_objects_event_equals_a_direct_call(g, ctx):
         assert ev.status == 0
         ctx.sync()
         assert direct.any() and np.array_equal(via.view(np.uint16), direct.view(np.uint16))
-        tw.check_orders()
+        tw.check_state()
         ev.object_count = 0
         fn(N.GS_UNITY_EVENT_FRAME_OBJECTS, C.addressof(ev))
         assert ev.status == INVALID

@@ -7,7 +7,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from util import camera
+from util import CAP_H, CAP_SPLATS, CAP_W, bin_row_splats, camera
 
 pytestmark = pytest.mark.gpu
 
@@ -154,7 +154,7 @@ def test_objects_device_array_and_async_host_images(g, ctx):
     """Member images of every kind in one group: a device tensor, a CUDA array, and pinned host images filled asynchronously
     (GS_FLAG_ASYNC_READBACK, two in rotation, completed by sync())."""
     import torch
-    from cuda_arrays import Cudart
+    from images import Cudart
     cams = _cams(g, 320, 200, 4)
     assets, knobs = _scene(g, 320, 200)
     want = _single(g, ctx, assets, knobs, cams)
@@ -170,7 +170,7 @@ def test_objects_device_array_and_async_host_images(g, ctx):
             grp.SortAndRenderSplatsMulti(objs, cam, rts=[dev, arr, pins[f & 1].numpy()])
             grp.sync()
             torch.cuda.synchronize()
-            for got in (dev.cpu().numpy(), rt.download(arr.handle, (200, 320, 4), np.float16), pins[f & 1].numpy()):
+            for got in (dev.cpu().numpy(), rt.download(arr.handle), pins[f & 1].numpy()):
                 assert np.array_equal(got.view(np.uint16), want[f][2].view(np.uint16)), "frame %d" % f
     finally:
         grp.close()
@@ -181,7 +181,7 @@ def test_objects_camera_targets(g, ctx):
     """Members with a camera target end with the bytes single-GPU gs_composite leaves on the same initial target (device,
     CUDA array and host targets); a member without one, and every member's render target, is as without targets."""
     import torch
-    from cuda_arrays import Cudart
+    from images import Cudart
     from unitygaussiansplatting_b200.renderer import CudaArrayImage
     W, H = 320, 200
     cams = _cams(g, W, H, 3)
@@ -209,7 +209,7 @@ def test_objects_camera_targets(g, ctx):
             torch.cuda.synchronize()
             for i in range(4):
                 assert np.array_equal(rts[i].view(np.uint16), want[f][2].view(np.uint16)), "frame %d member %d: render target" % (f, i)
-            for name, got in (("device", dev_t.cpu().numpy()), ("array", cu.download(arr_t.handle, (H, W, 4), np.float16)), ("host", host_t)):
+            for name, got in (("device", dev_t.cpu().numpy()), ("array", cu.download(arr_t.handle)), ("host", host_t)):
                 assert np.array_equal(got.view(np.uint16), expect.view(np.uint16)), "frame %d: %s camera target differs from gs_composite" % (f, name)
     finally:
         comp.Dispose()
@@ -351,7 +351,7 @@ def test_member_context_sync_with_a_pending_array_camera_target(g, ctx):
     """gs_sync on a member's own context right after the call, before gs_group_sync, waits for the composite onto a CUDA-array
     camera target (on the member's transfer stream) before it releases that target's surface; the target ends right."""
     import torch
-    from cuda_arrays import Cudart
+    from images import Cudart
     from unitygaussiansplatting_b200.renderer import CudaArrayImage
     W, H = 320, 200
     cam = _cams(g, W, H, 1)[0]
@@ -375,7 +375,7 @@ def test_member_context_sync_with_a_pending_array_camera_target(g, ctx):
         grp.sync()
         torch.cuda.synchronize()
         for i, t in enumerate(targets):
-            assert np.array_equal(cu.download(t.handle, (H, W, 4), np.float16).view(np.uint16), expect.view(np.uint16)), "member %d" % i
+            assert np.array_equal(cu.download(t.handle).view(np.uint16), expect.view(np.uint16)), "member %d" % i
     finally:
         comp.Dispose()
         grp.close()
@@ -389,12 +389,11 @@ def test_truncated_list_of_an_earlier_object_is_reported(g, ctx, image):
     fits: the call still reports GS_ERR_OUT_OF_MEMORY, when it returns with a host image and at gs_group_sync with a device
     image.  Deleting the splat that no longer fits makes the next call succeed and equal the per-object gs_frame loop."""
     import torch
-    import test_gpu_cull_edges as ce
-    from test_gpu_frame_objects import loop_frame
-    W, H = ce.CAP_W, ce.CAP_H
+    from frame_loops import loop_frame
+    W, H = CAP_W, CAP_H
     cam = camera(g, W, H)
-    assets = [g.create_asset(ce._bin_row_splats(cam, ce.CAP_SPLATS + 1, 0xCA9), "VeryHigh"),
-              g.create_asset(ce._bin_row_splats(cam, 1000, 0xCAA), "VeryHigh")]
+    assets = [g.create_asset(bin_row_splats(cam, CAP_SPLATS + 1, 0xCA9), "VeryHigh"),
+              g.create_asset(bin_row_splats(cam, 1000, 0xCAA), "VeryHigh")]
     grp, objs = _group(assets, [{}, {}], 1)
     rs = []
     try:

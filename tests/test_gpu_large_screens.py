@@ -129,7 +129,7 @@ def test_wide_screen_target_kinds_and_composite(g, O, ctx):
     """Host, device and CUDA-array render targets hold the oracle's frame; gs_composite of it onto host and CUDA-array camera
     targets leaves what the oracle's composite does."""
     import torch
-    from cuda_arrays import Cudart
+    from images import Cudart
     W, H = 16384, 512
     cam = camera(g, W, H)
     asset = _edge_scene(g, cam)
@@ -147,7 +147,7 @@ def test_wide_screen_target_kinds_and_composite(g, O, ctx):
             r.SortAndRenderSplats(cam, rt=target)
             ctx.sync()
             torch.cuda.synchronize()
-            got[name] = host if name == "host" else dev.cpu().numpy() if name == "device" else cu.download(arr.handle, (H, W, 4), np.float16)
+            got[name] = host if name == "host" else dev.cpu().numpy() if name == "device" else cu.download(arr.handle)
             assert np.array_equal(got[name].astype(np.float32), ref), "%s render target differs from the oracle" % name
             r.Dispose()
         init = np.random.default_rng(11).random((H, W, 4)).astype(np.float16)
@@ -159,7 +159,7 @@ def test_wide_screen_target_kinds_and_composite(g, O, ctx):
         cu.upload(arr_t.handle, init)
         comp.Composite(dev, arr_t)
         ctx.sync()
-        for name, t in (("host", host_t), ("array", cu.download(arr_t.handle, (H, W, 4), np.float16))):
+        for name, t in (("host", host_t), ("array", cu.download(arr_t.handle))):
             assert not np.array_equal(t, init) and np.array_equal(t.astype(np.float32), want), "%s camera target differs" % name
         comp.Dispose()
     finally:

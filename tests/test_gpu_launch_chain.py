@@ -8,47 +8,40 @@ it may change a bit.  Each case below is one where a kernel's early work could m
 import numpy as np
 import pytest
 
-import test_gpu_frame_cameras as FC
-import test_gpu_frame_objects as FO
+from frame_loops import CAM_SIZES, Twins, compare, compare_frame, mixed_assets, mixed_setup, orbit
+from images import ca  # noqa: F401
 from util import camera
 
 pytestmark = pytest.mark.gpu
 
 
 def _sort_every_frame(i, r):
-    FC._setup(i, r)
+    mixed_setup(i, r)
     r.m_SortNthFrame = 1
 
 
 @pytest.mark.parametrize("blend", [0, 1])
-def test_camera_run_sorts_and_views_an_asset_it_has_binned(g, ctx, blend):
+def test_camera_run_sorts_and_views_an_asset_it_has_binned(g, ctx, ca, blend):
     """Every camera draws the same two assets, so each later pair's sort and view-calc follows the bin emit of the same asset
     for an earlier camera; every pair is sorted, so every view-calc runs beside the sort's last pass."""
-    ca = FC._Cudart()
-    tw = FC.Twins(g, ctx, FC._mixed_assets(g, 3), _sort_every_frame)
+    tw = Twins(g, ctx, mixed_assets(g, 3), _sort_every_frame)
     try:
         for f in range(3):
-            cams = [FC.orbit(g, f, *FC.CAM_SIZES[c], phase=0.7 * c) for c in range(3)]
+            cams = [orbit(g, f, *CAM_SIZES[c], phase=0.7 * c) for c in range(3)]
             idx = tw.gathered(g, [[0, 1], [0, 1], [1, 0]], cams)
-            assert FC.compare(g, ctx, ca, tw, idx, cams, blend, np.float16, ["device"] * 3, [None] * 3, "frame %d" % f) > 0
+            assert compare(g, ctx, ca, tw, idx, cams, blend, np.float16, ["device"] * 3, [None] * 3, "frame %d" % f) > 0
     finally:
-        ctx.sync()
-        ca.free_all()
         tw.dispose()
 
 
 @pytest.mark.parametrize("blend", [0, 1])
-def test_object_run_sorted_every_frame_equals_the_loop(g, ctx, blend):
-    ca = FO._Cudart()
-    assets = FC._mixed_assets(g, 4)
-    tw = FO.Twins(g, ctx, assets, _sort_every_frame)
+def test_object_run_sorted_every_frame_equals_the_loop(g, ctx, ca, blend):
+    tw = Twins(g, ctx, mixed_assets(g, 4), _sort_every_frame)
     try:
         for f in range(3):
-            cam = FO.orbit(g, f)
-            FO._compare_frame(g, ctx, ca, tw, cam, blend, np.float16, "device", "device", "frame %d" % f)
+            cam = orbit(g, f)
+            compare_frame(g, ctx, ca, tw, cam, blend, np.float16, "device", "device", "frame %d" % f)
     finally:
-        ctx.sync()
-        ca.free_all()
         tw.dispose()
 
 
@@ -68,7 +61,7 @@ def test_two_screen_sizes_back_to_back(g, ctx):
     try:
         for f in range(6):
             W, H = sizes[f % 2]
-            cam = FO.orbit(g, f, W, H)
+            cam = orbit(g, f, W, H)
             want_rt, want_order = _frame(alone[(W, H)], cam)
             rt, order = _frame(alt, cam)
             assert want_rt.any()
@@ -108,7 +101,7 @@ def test_emulated_group_of_two_equals_one_gpu(g, ctx):
     grp = GaussianSplatGroup.create(asset, [0, 0], emulate=True)
     try:
         for f in range(4):
-            cam = FO.orbit(g, f)
+            cam = orbit(g, f)
             rt, order = _frame(r, cam)
             rts = [np.zeros_like(rt) for _ in range(2)]
             grp.SortAndRenderSplats(cam, rts=rts)

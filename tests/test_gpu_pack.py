@@ -17,7 +17,7 @@ def P(g):
     return pack
 
 
-def _host(g, splats, quality="Medium", formats=None):
+def _host_pack(g, splats, quality="Medium", formats=None):
     return g.create_asset(splats.copy(), quality, formats)
 
 
@@ -39,7 +39,7 @@ def _check(g, ctx, splats, quality="Medium", formats=None):
     before = splats.copy()
     gpu = g.pack_asset(splats, quality, formats, context=ctx)
     assert np.array_equal(splats.view(np.uint32), before.view(np.uint32)), "pack_asset modified its input"
-    _same(gpu, _host(g, splats, quality, formats))
+    _same(gpu, _host_pack(g, splats, quality, formats))
     return gpu
 
 
@@ -146,7 +146,7 @@ def test_nan_input_gives_well_formed_asset(g, ctx):
     s[17, 9:20] = np.inf
     s[300, 55] = np.nan
     a = g.pack_asset(s, "Medium", context=ctx)
-    h = _host(g, s)
+    h = _host_pack(g, s)
     for name in ("posData", "otherData", "colorData", "shData", "chunkData"):
         assert getattr(a, name).nbytes == getattr(h, name).nbytes
 
@@ -181,7 +181,7 @@ def test_device_asset_renders_like_uploaded(g, ctx, quality):
     t_before = t.clone()
     packed, r_dev = g.pack_asset(t, quality, context=ctx, keep_on_device=True)
     assert torch.equal(t, t_before), "pack_asset modified its input tensor"
-    host = _host(g, s, quality)
+    host = _host_pack(g, s, quality)
     _same(packed, host)
     r_up = g.GaussianSplatRenderer(host, ctx)
     for step in range(6):

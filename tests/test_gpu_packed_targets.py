@@ -13,21 +13,14 @@ import numpy as np
 import pytest
 
 import packed_oracle as P
-from cuda_arrays import D2H, H2D, KIND_FLOAT, KIND_UNSIGNED, LAYERED, SURFACE_LOAD_STORE, Cudart, _ChannelDesc, _Dim3, _Memcpy3DParms, _PitchedPtr
+from frame_loops import frame_args
+from images import KIND_FLOAT, SharedArray, ca, launches, to_device, to_host  # noqa: F401
 from util import camera
 
 ROOT = Path(__file__).resolve().parents[1]
 UNSUPPORTED = -4
 PACKED = 2
 W, H = 200, 120   # not a multiple of 16 on either axis
-
-
-@pytest.fixture
-def ca(ctx):
-    c = Cudart()
-    yield c
-    ctx.sync()
-    c.free_all()
 
 
 def codes(shape, seed):
@@ -41,81 +34,9 @@ def codes(shape, seed):
     return t
 
 
-def packed_array(ca, w, h, layers=0, kind=KIND_UNSIGNED, bits=32, fill=None):
-    """A (layers, h, w) CUDA array of one `bits`-bit channel of `kind` (layers 0: a 2-D array), made with
-    cudaArraySurfaceLoadStore; fill: its uint32 texels."""
-    flags = SURFACE_LOAD_STORE | (LAYERED if layers else 0)
-    h_ = C.c_void_p()
-    rc = ca.lib.cudaMalloc3DArray(C.byref(h_), C.byref(_ChannelDesc(bits, 0, 0, 0, kind)), _Dim3(w, h, layers), flags)
-    assert rc == 0, "cudaMalloc3DArray failed with CUDA error %d" % rc
-    ca.live.append(h_.value)
-    if fill is not None:
-        _copy(ca, h_.value, np.ascontiguousarray(fill, np.uint32), H2D)
-    return h_.value
-
-
-def _copy(ca, handle, host, kind):
-    host = host.reshape((-1,) + host.shape[-2:])
-    p = _Memcpy3DParms()
-    pitched = _PitchedPtr(host.ctypes.data, host.shape[2] * 4, host.shape[2], host.shape[1])
-    if kind == H2D:
-        p.srcPtr, p.dstArray = pitched, handle
-    else:
-        p.srcArray, p.dstPtr = handle, pitched
-    p.extent, p.kind = _Dim3(host.shape[2], host.shape[1], host.shape[0]), kind
-    assert ca.lib.cudaMemcpy3D(C.byref(p)) == 0
-
-
-class PArr:
-    """A packed camera-target array whose every texel starts as a random code."""
-
-    def __init__(self, g, ca, w, h, layers=0, seed=1):
-        self.g, self.ca, self.w, self.h, self.layers = g, ca, w, h, layers
-        self.start = codes((max(layers, 1), h, w), seed)
-        self.handle = packed_array(ca, w, h, layers, fill=self.start)
-
-    def image(self, x=None, y=None, w=W, h=H, layer=None):
-        origin = None if x is None else (x, y)
-        return self.g.CudaArrayImage(self.handle, w, h, np.uint32, layer=layer, origin=origin)
-
-    def part(self, layer, x, y, w=W, h=H):
-        return self.start[layer or 0, y:y + h, x:x + w].copy()
-
-    def read(self):
-        out = np.empty((max(self.layers, 1), self.h, self.w), np.uint32)
-        _copy(self.ca, self.handle, out, D2H)
-        return out
-
-    def check(self, ctx, regions, what):
-        """regions: [(layer, x, y, want)]: each rectangle equals `want`; every other texel holds its starting code."""
-        ctx.sync()
-        got = self.read()
-        expect = self.start.copy()
-        for layer, x, y, want in regions:
-            expect[layer or 0, y:y + want.shape[0], x:x + want.shape[1]] = want
-        assert np.array_equal(got, expect), "%s: %d texels differ" % (what, int((got != expect).sum()))
-
-
-def _tensor(host):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(host)).cuda()
-
-
-def _packed_tensor(host):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(host).view(np.int32)).cuda()
-
-
-def _host(ctx, t):
-    import torch
-    ctx.sync()
-    torch.cuda.synchronize()
-    out = t.cpu().numpy()
-    return out.view(np.uint32) if out.dtype == np.int32 else out
-
-
-def launches(ctx):
-    return ctx.stage_times().kernel_launches
+def packed(g, ca, w, h, layers=0, seed=1):
+    """A packed camera-target array (layers 0: a 2-D array) whose every texel starts as a random code."""
+    return SharedArray(g, ca, w, h, layers, np.uint32, "packed", codes((max(layers, 1), h, w), seed))
 
 
 def _assets(g):
@@ -144,9 +65,9 @@ def test_composite_equals_the_oracle(g, ctx, ca, dtype, blend):
     cam = camera(g, W, H)
     r = g.GaussianSplatRenderer(asset, ctx)
     r.blend_mode = blend
-    t = _tensor(np.zeros((H, W, 4), dtype))
+    t = to_device(np.zeros((H, W, 4), dtype))
     r.SortAndRenderSplats(cam, rt=t)
-    rt = _host(ctx, t)
+    rt = to_host(ctx, t)
     covered = rt[..., 3] > 0
     assert covered.any() and not covered.all()
     start = codes((H, W), 3)
@@ -156,15 +77,14 @@ def test_composite_equals_the_oracle(g, ctx, ca, dtype, blend):
     host = start.copy()
     r.Composite(rt, host)                      # host rt, host target
     assert np.array_equal(host, want), "host target"
-    dev = _packed_tensor(start)
+    dev = to_device(start)
     r.Composite(t, dev)                        # device rt, device target
-    assert np.array_equal(_host(ctx, dev), want), "device target"
+    assert np.array_equal(to_host(ctx, dev), want), "device target"
     for what, layers, layer, x, y, aw, ah in (("2-D array", 0, None, None, None, W, H), ("layer", 3, 1, None, None, W, H),
                                                 ("rectangle", 0, None, 37, 19, 301, 157), ("rectangle of a layer", 3, 2, 101, 37, 301, 157)):
-        A = PArr(g, ca, aw, ah, layers, seed=11)
-        A.start[layer or 0, (y or 0):(y or 0) + H, (x or 0):(x or 0) + W] = start
-        _copy(ca, A.handle, A.start, H2D)
-        r.Composite(t, A.image(x, y, layer=layer))
+        A = packed(g, ca, aw, ah, layers, seed=11)
+        A.fill(layer, x or 0, y or 0, start)
+        r.Composite(t, A.view(layer, None if x is None else (x, y), (W, H)))
         A.check(ctx, [(layer, x or 0, y or 0, want)], what)
     r.Dispose()
 
@@ -199,38 +119,37 @@ def test_frame_and_frame_objects_equal_draw_then_composite(g, ctx, ca):
     try:
         for name, fn in (("gs_frame", frame), ("gs_frame_objects", objects)):
             # the definition: the draw into rt, then gs_composite onto the packed target
-            t = _tensor(np.zeros((H, W, 4), np.float16))
+            t = to_device(np.zeros((H, W, 4), np.float16))
             fn(t, None)
-            want_rt = _host(ctx, t)
-            tg = _packed_tensor(start)
+            want_rt = to_host(ctx, t)
+            tg = to_device(start)
             r.Composite(t, tg)
-            want = _host(ctx, tg)
+            want = to_host(ctx, tg)
             assert not np.array_equal(want, start)
             # RGBA16F camera targets: the launch count the packed ones must match
-            n16 = counted(fn, _tensor(np.zeros((H, W, 4), np.float16)), _tensor(np.zeros((H, W, 4), np.float16)))
-            n16_alone = counted(fn, None, _tensor(np.zeros((H, W, 4), np.float16)))
+            n16 = counted(fn, to_device(np.zeros((H, W, 4), np.float16)), to_device(np.zeros((H, W, 4), np.float16)))
+            n16_alone = counted(fn, None, to_device(np.zeros((H, W, 4), np.float16)))
             for kind in ("host", "device", "2-D array", "layer", "rectangle"):
                 what = "%s onto a %s target" % (name, kind)
                 for with_rt in (True, False):
-                    t = _tensor(np.zeros((H, W, 4), np.float16)) if with_rt else None
+                    t = to_device(np.zeros((H, W, 4), np.float16)) if with_rt else None
                     if kind == "host":
                         tg = start.copy()
                         fn(t, tg)
                         assert np.array_equal(tg, want), what
                     elif kind == "device":
-                        tg = _packed_tensor(start)
+                        tg = to_device(start)
                         assert counted(fn, t, tg) == (n16 if with_rt else n16_alone), what
-                        assert np.array_equal(_host(ctx, tg), want), what
+                        assert np.array_equal(to_host(ctx, tg), want), what
                     else:
                         layers, layer, x, y, aw, ah = {"2-D array": (0, None, None, None, W, H), "layer": (2, 1, None, None, W, H),
                                                        "rectangle": (2, 1, 37, 19, 301, 157)}[kind]
-                        A = PArr(g, ca, aw, ah, layers, seed=12)
-                        A.start[layer or 0, (y or 0):(y or 0) + H, (x or 0):(x or 0) + W] = start
-                        _copy(ca, A.handle, A.start, H2D)
-                        assert counted(fn, t, A.image(x, y, layer=layer)) == (n16 if with_rt else n16_alone), what
+                        A = packed(g, ca, aw, ah, layers, seed=12)
+                        A.fill(layer, x or 0, y or 0, start)
+                        assert counted(fn, t, A.view(layer, None if x is None else (x, y), (W, H))) == (n16 if with_rt else n16_alone), what
                         A.check(ctx, [(layer, x or 0, y or 0, want)], what)
                     if with_rt:
-                        assert np.array_equal(_host(ctx, t).view(np.uint16), want_rt.view(np.uint16)), what + ": rt"
+                        assert np.array_equal(to_host(ctx, t).view(np.uint16), want_rt.view(np.uint16)), what + ": rt"
     finally:
         ctx.set_timing(False)
     for x in (r, ra, rb):
@@ -256,44 +175,44 @@ def test_frame_cameras_with_mixed_targets_is_one_run(g, ctx, ca):
     try:
         # the definition: the camera loop, into rts, then gs_composite onto each camera's target
         loop = renderers()
-        A = PArr(g, ca, 260, 200, 0, seed=21)
-        rts = [_tensor(np.zeros((h, w, 4), np.float16)) for (_, _, w, h) in TILES]
+        A = packed(g, ca, 260, 200, 0, seed=21)
+        rts = [to_device(np.zeros((h, w, 4), np.float16)) for (_, _, w, h) in TILES]
         n0 = launches(ctx)
         for c, cam in enumerate(cams):
             g.SortAndRenderSplatsMulti(loop, cam, rts[c])
         n_loop = launches(ctx) - n0
-        want_rt = [_host(ctx, t) for t in rts]
-        tg0 = _tensor(bg)
+        want_rt = [to_host(ctx, t) for t in rts]
+        tg0 = to_device(bg)
         loop[0].Composite(rts[0], tg0)
-        want0 = _host(ctx, tg0)
+        want0 = to_host(ctx, tg0)
         want_tiles = []
         for c in (1, 2):
             x, y, w, h = TILES[c]
-            t = _packed_tensor(A.part(None, x, y, w, h))
+            t = to_device(A.start[0, y:y + h, x:x + w])
             loop[0].Composite(rts[c], t)
-            want_tiles.append(_host(ctx, t))
+            want_tiles.append(to_host(ctx, t))
         want_order = [r.readback_order() for r in loop]
 
         # the same call onto RGBA16F targets: tiles of one RGBA16F array
         sep = renderers()
         h16 = ca.array(260, 200, 0, np.float16, fill=0.25)
         n0 = launches(ctx)
-        actives = g.SortAndRenderCameras(sep, cams, [_tensor(np.zeros((h, w, 4), np.float16)) for (_, _, w, h) in TILES],
-                                         [_tensor(bg)] + [g.CudaArrayImage(h16, w, h, np.float16, origin=(x, y)) for (x, y, w, h) in TILES[1:]])
+        actives = g.SortAndRenderCameras(sep, cams, [to_device(np.zeros((h, w, 4), np.float16)) for (_, _, w, h) in TILES],
+                                         [to_device(bg)] + [g.CudaArrayImage(h16, w, h, np.float16, origin=(x, y)) for (x, y, w, h) in TILES[1:]])
         n16 = launches(ctx) - n0
         assert g.renderer.cameras_in_one_call(actives)
         assert n16 < n_loop + 3, "the cameras were not drawn as one run"   # + the loop's three composites, made apart above
 
         call = renderers()
-        rts = [_tensor(np.zeros((h, w, 4), np.float16)) for (_, _, w, h) in TILES]
-        tg0 = _tensor(bg)
+        rts = [to_device(np.zeros((h, w, 4), np.float16)) for (_, _, w, h) in TILES]
+        tg0 = to_device(bg)
         n0 = launches(ctx)
-        g.SortAndRenderCameras(call, cams, rts, [tg0] + [A.image(x, y, w, h) for (x, y, w, h) in TILES[1:]])
+        g.SortAndRenderCameras(call, cams, rts, [tg0] + [A.view(origin=(x, y), size=(w, h)) for (x, y, w, h) in TILES[1:]])
         n_call = launches(ctx) - n0
         assert n_call == n16, (n_call, n16)
         for c in range(3):
-            assert np.array_equal(_host(ctx, rts[c]).view(np.uint16), want_rt[c].view(np.uint16)), "camera %d rt" % c
-        assert np.array_equal(_host(ctx, tg0).view(np.uint16), want0.view(np.uint16))
+            assert np.array_equal(to_host(ctx, rts[c]).view(np.uint16), want_rt[c].view(np.uint16)), "camera %d rt" % c
+        assert np.array_equal(to_host(ctx, tg0).view(np.uint16), want0.view(np.uint16))
         A.check(ctx, [(None, x, y, want) for (x, y, _, _), want in zip(TILES[1:], want_tiles)], "packed tiles")
         for r, o in zip(call, want_order):
             assert np.array_equal(r.readback_order(), o)
@@ -316,14 +235,13 @@ def test_unity_events_with_a_packed_array_target(g, ctx, ca):
 
     # GS_UNITY_EVENT_FRAME against gs_frame
     r.ResetOrder()
-    tg = _packed_tensor(start)
+    tg = to_device(start)
     r.SortAndRenderSplats(cam, camera_target=tg)
-    want = _host(ctx, tg)
+    want = to_host(ctx, tg)
     fp, _keep = g.make_frame_params(cam, r.localToWorldMatrix, r.m_SplatScale, r.m_OpacityScale, r.m_SHOrder, r.m_SHOnly)
-    A = PArr(g, ca, 301, 157, 0, seed=31)
-    A.start[0, 19:19 + H, 37:37 + W] = start
-    _copy(ca, A.handle, A.start, H2D)
-    tg_im = _image(A.image(37, 19), W, H)
+    A = packed(g, ca, 301, 157, 0, seed=31)
+    A.fill(None, 37, 19, start)
+    tg_im = _image(A.view(origin=(37, 19), size=(W, H)), W, H)
     ev = N.GsUnityFrameEvent()
     ev.ctx, ev.asset = C.cast(ctx.handle, C.c_void_p).value, C.cast(r._asset, C.c_void_p).value
     C.memmove(C.byref(ev.params), C.byref(fp), C.sizeof(fp))
@@ -340,25 +258,21 @@ def test_unity_events_with_a_packed_array_target(g, ctx, ca):
     # GS_UNITY_EVENT_FRAME_OBJECTS against gs_frame_objects
     rs = [g.GaussianSplatRenderer(x, ctx) for x in (a, b)]
     rs[1].localToWorldMatrix = g.trs(position=(1.5, 0.0, 3.0)).astype(np.float32)
-    tg = _packed_tensor(start)
+    tg = to_device(start)
     active = g.SortAndRenderSplatsMulti(rs, cam, None, tg)
-    want = _host(ctx, tg)
+    want = to_host(ctx, tg)
     k = len(active)
-    fps = (N.GsFrameParams * k)()
-    for i, x in enumerate(active):
-        fps[i] = x.frame_params(cam)   # x keeps the host buffers it points to
+    for x in active:
         x.ResetOrder()
-    assets_arr = (C.c_void_p * k)(*[C.cast(x._asset, C.c_void_p).value for x in active])
-    ds = (C.c_int32 * k)(*([1] * k))
-    B = PArr(g, ca, W, H, 3, seed=32)
-    B.start[2] = start
-    _copy(ca, B.handle, B.start, H2D)
+    assets_arr, fps, ds, keep = frame_args(g, [(cam, x, x.sceneDepth) for x in active])
+    B = packed(g, ca, W, H, 3, seed=32)
+    B.fill(2, 0, 0, start)
     ev = N.GsUnityFrameObjectsEvent()
     ev.ctx, ev.object_count = C.cast(ctx.handle, C.c_void_p).value, k
     ev.assets, ev.fps, ev.do_sort = C.addressof(assets_arr), C.addressof(fps), C.addressof(ds)
     ev.options.blend_mode = active[0].blend_mode
     ev.status, ev.has_rt, ev.has_camera_target = -5, 0, 1
-    tg_im = _image(B.image(layer=2), W, H)
+    tg_im = _image(B.view(layer=2), W, H)
     ev.camera_target = tg_im
     fn(N.GS_UNITY_EVENT_FRAME_OBJECTS, C.addressof(ev))
     assert ev.status == 0
@@ -378,9 +292,9 @@ def test_emulated_group_onto_packed_targets_equals_one_gpu(g, ctx, ca):
     rs = [g.GaussianSplatRenderer(a, ctx) for a in assets]
     for r, m in zip(rs, mats):
         r.localToWorldMatrix = m
-    rt, tg = _tensor(np.zeros((H, W, 4), np.float16)), _packed_tensor(start)
+    rt, tg = to_device(np.zeros((H, W, 4), np.float16)), to_device(start)
     g.SortAndRenderSplatsMulti(rs, cam, rt, tg)
-    want_rt, want = _host(ctx, rt), _host(ctx, tg)
+    want_rt, want = to_host(ctx, rt), to_host(ctx, tg)
     for r in rs:
         r.Dispose()
 
@@ -389,16 +303,15 @@ def test_emulated_group_onto_packed_targets_equals_one_gpu(g, ctx, ca):
     for o, m in zip(objs, mats):
         o.localToWorldMatrix = m
     # member 0 composites onto a device tensor, member 1 onto a rectangle of a packed array, member 2 onto host memory
-    A = PArr(g, ca, 301, 157, 0, seed=41)
-    A.start[0, 19:19 + H, 37:37 + W] = start
-    _copy(ca, A.handle, A.start, H2D)
-    dev, host = _packed_tensor(start), start.copy()
-    rts = [_tensor(np.zeros((H, W, 4), np.float16)) for _ in range(3)]
-    grp.SortAndRenderSplatsMulti(objs, cam, rts=rts, camera_targets=[dev, A.image(37, 19), host])
+    A = packed(g, ca, 301, 157, 0, seed=41)
+    A.fill(None, 37, 19, start)
+    dev, host = to_device(start), start.copy()
+    rts = [to_device(np.zeros((H, W, 4), np.float16)) for _ in range(3)]
+    grp.SortAndRenderSplatsMulti(objs, cam, rts=rts, camera_targets=[dev, A.view(origin=(37, 19), size=(W, H)), host])
     grp.sync()
     for t in rts:
-        assert np.array_equal(_host(ctx, t).view(np.uint16), want_rt.view(np.uint16))
-    assert np.array_equal(_host(ctx, dev), want)
+        assert np.array_equal(to_host(ctx, t).view(np.uint16), want_rt.view(np.uint16))
+    assert np.array_equal(to_host(ctx, dev), want)
     A.check(ctx, [(None, 37, 19, want)], "member 1")
     assert np.array_equal(host, want)
     grp.close()
@@ -417,8 +330,8 @@ def test_packed_refusals_write_nothing(g, ctx, ca):
     r.ResetOrder()
     r.CalcViewData(cam)   # gs_render's precondition, so that only the image can refuse it
     start = codes((H, W), 51)
-    rt16 = _tensor(np.random.default_rng(2).random((H, W, 4), np.float32).astype(np.float16))
-    rt16_host = _host(ctx, rt16)
+    rt16 = to_device(np.random.default_rng(2).random((H, W, 4), np.float32).astype(np.float16))
+    rt16_host = to_host(ctx, rt16)
 
     def refused(code, call, images):
         before = [im.copy() for im in images]
@@ -436,8 +349,8 @@ def test_packed_refusals_write_nothing(g, ctx, ca):
     tg = start.copy()
     refused(UNSUPPORTED, lambda: r.SortAndRenderSplats(cam, rt=host, camera_target=tg), [host, tg])
     refused(UNSUPPORTED, lambda: g.SortAndRenderSplatsMulti([r], cam, host, tg), [host, tg])
-    A = PArr(g, ca, W, H, 0, seed=52)
-    refused(UNSUPPORTED, lambda: r.SortAndRenderSplats(cam, rt=A.image()), [])
+    A = packed(g, ca, W, H, 0, seed=52)
+    refused(UNSUPPORTED, lambda: r.SortAndRenderSplats(cam, rt=A.view()), [])
     A.check(ctx, [], "a packed array as rt")
     refused(UNSUPPORTED, lambda: r.Composite(host, tg), [host, tg])
     # band_packed output
@@ -450,17 +363,17 @@ def test_packed_refusals_write_nothing(g, ctx, ca):
     # gs_unshuffle_bands into a packed image
     out = start.copy()
     im = _image(out, W, H)
-    gathered = _tensor(np.zeros((2, 64, W), np.uint32).view(np.int32))
+    gathered = to_device(np.zeros((2, 64, W), np.uint32))
     assert lib.gs_unshuffle_bands(ctx.handle, C.c_void_p(gathered.data_ptr()), 2, 1, 64, PACKED, C.byref(im)) == UNSUPPORTED
     assert np.array_equal(out, start)
     # a packed target array with a float channel, and an RGBA16F target given a uint32 array
-    fa = packed_array(ca, W, H, 0, kind=KIND_FLOAT)
+    fa = ca.array(W, H, 0, np.uint32, 1, kind=KIND_FLOAT)
     refused(UNSUPPORTED, lambda: r.Composite(rt16, g.CudaArrayImage(fa, W, H, np.uint32)), [])
-    ua = PArr(g, ca, W, H, 0, seed=53)
+    ua = packed(g, ca, W, H, 0, seed=53)
     refused(UNSUPPORTED, lambda: r.Composite(rt16, g.CudaArrayImage(ua.handle, W, H, np.float16)), [])
     refused(UNSUPPORTED, lambda: g.SortAndRenderSplatsMulti([r], cam, None, g.CudaArrayImage(fa, W, H, np.uint32)), [])
     ua.check(ctx, [], "a uint32 array as an RGBA16F target")
-    assert np.array_equal(_host(ctx, rt16).view(np.uint16), rt16_host.view(np.uint16))
+    assert np.array_equal(to_host(ctx, rt16).view(np.uint16), rt16_host.view(np.uint16))
     r.Dispose()
 
     # a group's render targets

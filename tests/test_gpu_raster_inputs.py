@@ -15,39 +15,13 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from cuda_arrays import Cudart
-from test_gpu_depth_arrays import _fps, _frame_cameras, depth_array
+from frame_loops import call_cameras, frame_args
+from images import Image, bits, ca, to_device, to_host  # noqa: F401
 from util import camera, splat_records, view_fields, world_at_pixel
 
 W, H = 320, 240
 RECT = (W + 61, H + 37, 37, 19)   # array width, height, and the rectangle's origin: non-zero in both axes
-SENTINEL = -3.25                  # exact in half and float
 CANON16 = 0x7FFF                  # the half NaN a GPU conversion or blend produces
-
-
-@pytest.fixture
-def ca(ctx):
-    c = Cudart()
-    yield c
-    ctx.sync()
-    c.free_all()
-
-
-def _tensor(host):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(host)).cuda()
-
-
-def _host(ctx, t):
-    import torch
-    ctx.sync()
-    torch.cuda.synchronize()
-    return t.cpu().numpy()
-
-
-def _words(a):
-    a = np.ascontiguousarray(a)
-    return a.view(np.uint16) if a.dtype == np.float16 else a.view(np.uint32)
 
 
 def _u32f(words):
@@ -154,18 +128,9 @@ def with_specials(field, seed):
 
 # ---- depth buffers in every memory kind -----------------------------------------------------------------------------------
 def depth_kinds(g, ca, field):
-    aw, ah, x, y = RECT
-    layers = np.ones((3, H, W), np.float32)
-    layers[1] = field
-    big = np.ones((ah, aw), np.float32)
-    big[y:y + H, x:x + W] = field
-    return {
-        "host": np.ascontiguousarray(field),
-        "device": _tensor(field),
-        "array": g.CudaArrayDepth(depth_array(ca, W, H, 0, field), W, H),
-        "layer": g.CudaArrayDepth(depth_array(ca, W, H, 3, layers), W, H, layer=1),
-        "rect": g.CudaArrayDepth(depth_array(ca, aw, ah, 0, big), W, H, origin=(x, y)),
-    }
+    """The field as a depth buffer of every memory kind; the other texels of a layered or larger array hold 1.0."""
+    return {kind: Image(g, ca, kind, field, "depth", start=1.0, layers=3, layer=1, rect=RECT).image
+            for kind in ("host", "device", "array", "layer", "rect")}
 
 
 def oracle_draw(O, g, asset, cam, field, staged, sel=None, blend=0, init=None):
@@ -185,7 +150,7 @@ def gpu_draw(r, cam, rt, staged):
         r.SortAndRenderSplats(cam, rt=rt)
 
 
-def _half_words(rt):
+def _halfbits(rt):
     """The oracle's float image narrowed to RGBA16F words (its fp16-ROP values are halves already); NaN is the canonical half."""
     with np.errstate(over="ignore", invalid="ignore"):
         w = rt.astype(np.float16).view(np.uint16)
@@ -222,14 +187,14 @@ def test_scene_depth_ties_every_path_and_memory_kind(g, O, ctx, ca):
         kinds = depth_kinds(g, ca, field)
         for staged in (False, True):
             for selected in (None, sel):
-                want = _half_words(oracle_draw(O, g, asset, cam, field, staged, selected))
-                assert not np.array_equal(want, _half_words(oracle_draw(O, g, asset, cam, None, staged, selected))), fname
+                want = _halfbits(oracle_draw(O, g, asset, cam, field, staged, selected))
+                assert not np.array_equal(want, _halfbits(oracle_draw(O, g, asset, cam, None, staged, selected))), fname
                 r.m_SelectedBits = selected
                 for kname, d in kinds.items():
                     r.sceneDepth = d
-                    t = _tensor(np.zeros((H, W, 4), np.float16))
+                    t = to_device(np.zeros((H, W, 4), np.float16))
                     gpu_draw(r, cam, t, staged)
-                    got = _words(_host(ctx, t))
+                    got = bits(to_host(ctx, t))
                     bad = np.argwhere((got != want).any(-1))
                     assert bad.size == 0, "%s, %s depth, %s, selection %s: %d pixels differ, first at (y, x) = %s" % (
                         fname, kname, "gs_calc_view + gs_render" if staged else "gs_frame", selected is not None, len(bad), bad[:3].tolist())
@@ -247,15 +212,15 @@ def test_scene_depth_ties_per_camera_and_per_object(g, O, ctx, ca):
     sep = separated_scene(g, cams[0])
     fields = [voronoi_field(O, g, sep, cams[c], 11 + c)[0] for c in range(2)]
     r = g.GaussianSplatRenderer(sep, ctx)
-    want = [_half_words(oracle_draw(O, g, sep, cams[c], fields[c], False)) for c in range(2)]
+    want = [_halfbits(oracle_draw(O, g, sep, cams[c], fields[c], False)) for c in range(2)]
     assert not np.array_equal(want[0], want[1])
-    stack = depth_array(ca, W, H, 2, np.stack(fields))
-    for dname, ds in (("device", [_tensor(f) for f in fields]), ("layer", [g.CudaArrayDepth(stack, W, H, layer=c) for c in range(2)])):
+    stack = ca.array(W, H, 2, np.float32, 1, fill=np.stack(fields))
+    for dname, ds in (("device", [to_device(f) for f in fields]), ("layer", [g.CudaArrayDepth(stack, W, H, layer=c) for c in range(2)])):
         r.ResetOrder()
-        rts = [_tensor(np.zeros((H, W, 4), np.float16)) for _ in range(2)]
-        assert _frame_cameras(g, ctx, [(cams[c], ds[c]) for c in range(2)], [r], rts) == 0
+        rts = [to_device(np.zeros((H, W, 4), np.float16)) for _ in range(2)]
+        assert call_cameras(g, ctx, [[r], [r]], cams, 0, rts, [None, None], [[{"scene_depth": d}] for d in ds], check=False) == 0
         for c in range(2):
-            assert np.array_equal(_words(_host(ctx, rts[c])), want[c]), "gs_frame_cameras, %s depth, camera %d" % (dname, c)
+            assert np.array_equal(bits(to_host(ctx, rts[c])), want[c]), "gs_frame_cameras, %s depth, camera %d" % (dname, c)
 
     # two objects, one depth-tested: drawing them one after the other onto one target
     cam = cams[0]
@@ -265,15 +230,15 @@ def test_scene_depth_ties_per_camera_and_per_object(g, O, ctx, ca):
     dfield = with_specials(stamped, 9)
     for objs in ([(r, sep, fields[0]), (rd, dense, None)], [(rd, dense, dfield), (r, sep, None)]):
         first = oracle_draw(O, g, objs[0][1], cam, objs[0][2], False)
-        expect = _half_words(oracle_draw(O, g, objs[1][1], cam, objs[1][2], False, init=first))
-        fps, assets, do_sort, keep = _fps(g, [(cam, x, None if f is None else _tensor(f)) for x, _, f in objs])
+        expect = _halfbits(oracle_draw(O, g, objs[1][1], cam, objs[1][2], False, init=first))
+        assets, fps, do_sort, keep = frame_args(g, [(cam, x, None if f is None else to_device(f)) for x, _, f in objs])
         for x, _, _ in objs:
             x.ResetOrder()
-        t = _tensor(np.zeros((H, W, 4), np.float16))
+        t = to_device(np.zeros((H, W, 4), np.float16))
         im = _image(t, W, H)
         opt = N.GsRenderOptions()
         assert ctx._lib.gs_frame_objects(ctx.handle, 2, assets, fps, do_sort, C.byref(opt), C.byref(im), None) == 0
-        assert np.array_equal(_words(_host(ctx, t)), expect), "gs_frame_objects, depth on object %d" % (0 if objs[0][2] is not None else 1)
+        assert np.array_equal(bits(to_host(ctx, t)), expect), "gs_frame_objects, depth on object %d" % (0 if objs[0][2] is not None else 1)
 
     # an emulated group of two on a host depth buffer: every member receives the whole frame
     grp = GaussianSplatGroup.create(dense, [0, 0], emulate=True)
@@ -282,9 +247,9 @@ def test_scene_depth_ties_per_camera_and_per_object(g, O, ctx, ca):
         rts = [np.zeros((H, W, 4), np.float16) for _ in range(2)]
         grp.SortAndRenderSplats(cam, rts=rts)
         grp.sync()
-        want_g = _half_words(oracle_draw(O, g, dense, cam, dfield, False))
+        want_g = _halfbits(oracle_draw(O, g, dense, cam, dfield, False))
         for i, x in enumerate(rts):
-            assert np.array_equal(_words(x), want_g), "group member %d" % i
+            assert np.array_equal(bits(x), want_g), "group member %d" % i
     finally:
         grp.close()
     r.Dispose()
@@ -369,67 +334,23 @@ def loaded_content(O, g, asset, cam, dtype):
     words[y, x] = nans[(np.arange(y.size)[:, None] + np.arange(4)) % nans.size]
     if dtype == np.float16:   # widened exactly, NaN payloads included
         wide = words.view(np.float16).astype(np.float32)
-        assert np.array_equal(_half_words(wide)[~np.isnan(wide)], words[~np.isnan(wide)])
+        assert np.array_equal(_halfbits(wide)[~np.isnan(wide)], words[~np.isnan(wide)])
     else:
         wide = words.view(np.float32)
     return words, np.ascontiguousarray(wide), fam
 
 
-def expected_words(rt, init, words, dtype):
+def expectedbits(rt, init, words, dtype):
     """The oracle's draw onto `init` as `dtype` words: what it left bit for bit unchanged is the loaded word, the rest narrowed."""
     if dtype == np.float32:
         return rt.view(np.uint32)
     same = rt.view(np.uint32) == init.view(np.uint32)
-    return np.where(same, words, _half_words(rt))
+    return np.where(same, words, _halfbits(rt))
 
 
-class LoadedTarget:
-    """A render target of one memory kind holding `words`; read() returns them after the draw, checking what lies outside."""
-
-    def __init__(self, g, ca, kind, words, dtype):
-        self.kind, self.ca, self.dtype = kind, ca, np.dtype(dtype)
-        sent = np.full((H, W, 4), SENTINEL, dtype)
-        if kind == "host":
-            self.host = words.view(dtype).copy()
-            self.image = self.host
-        elif kind == "device":
-            self.t = _tensor(words.view(dtype))
-            self.image = self.t
-        elif kind == "array":
-            self.handle = ca.array(W, H, 0, dtype)
-            ca.upload(self.handle, words.view(dtype))
-            self.image = g.CudaArrayImage(self.handle, W, H, dtype)
-        elif kind == "layer":
-            self.handle = ca.array(W, H, 2, dtype)
-            ca.upload(self.handle, np.stack([sent, words.view(dtype)]))
-            self.image = g.CudaArrayImage(self.handle, W, H, dtype, layer=1)
-        else:
-            aw, ah, x, y = RECT
-            big = np.full((ah, aw, 4), SENTINEL, dtype)
-            big[y:y + H, x:x + W] = words.view(dtype)
-            self.handle = ca.array(aw, ah, 0, dtype)
-            ca.upload(self.handle, big)
-            self.image = g.CudaArrayImage(self.handle, W, H, dtype, origin=(x, y))
-
-    def read(self, ctx):
-        ctx.sync()
-        sent = _words(np.full(1, SENTINEL, self.dtype))[0]
-        if self.kind == "host":
-            return _words(self.host)
-        if self.kind == "device":
-            return _words(_host(ctx, self.t))
-        if self.kind == "array":
-            return _words(self.ca.download(self.handle, (H, W, 4), self.dtype))
-        if self.kind == "layer":
-            both = _words(self.ca.download(self.handle, (2, H, W, 4), self.dtype))
-            assert (both[0] == sent).all(), "layer 0 of the target was touched"
-            return both[1]
-        aw, ah, x, y = RECT
-        big = _words(self.ca.download(self.handle, (ah, aw, 4), self.dtype))
-        outside = np.ones((ah, aw), bool)
-        outside[y:y + H, x:x + W] = False
-        assert (big[outside] == sent).all(), "a texel outside the rectangle was touched"
-        return big[y:y + H, x:x + W]
+def loaded_target(g, ca, kind, words, dtype):
+    """A render target of one memory kind holding `words`; in a layer or a rectangle, every other texel holds a sentinel."""
+    return Image(g, ca, kind, words.view(dtype), layers=2, layer=1, rect=RECT)
 
 
 def _check(got, want, init_words, what):
@@ -461,7 +382,7 @@ def test_loaded_target_content(g, O, ctx, ca, dtype, blend):
         for extras in (False, True):
             selected, depth = (sel, field) if extras else (None, None)
             rt = oracle_draw(O, g, asset, cam, depth, staged, selected, blend, init)
-            want = expected_words(rt, init, words, dtype)
+            want = expectedbits(rt, init, words, dtype)
             # preconditions: every family is in the image, the reached ones where splats blend, and some pixels are untouched
             untouched = (rt.view(np.uint32) == init.view(np.uint32)).all(-1)
             for name, m in fam.items():
@@ -473,11 +394,11 @@ def test_loaded_target_content(g, O, ctx, ca, dtype, blend):
                              "alpha 1 - 2^-11"):
                     assert (~untouched[fam[name]]).mean() > 0.5, name + " is mostly not blended into"
             r.m_SelectedBits = selected
-            r.sceneDepth = None if depth is None else _tensor(depth)
+            r.sceneDepth = None if depth is None else to_device(depth)
             for kind in ("host", "device", "array", "layer", "rect"):
-                t = LoadedTarget(g, ca, kind, words, dtype)
+                t = loaded_target(g, ca, kind, words, dtype)
                 gpu_draw(r, cam, t.image, staged)
-                _check(t.read(ctx), want, words, "%s target, %s, %s" % (kind, "gs_calc_view + gs_render" if staged else "gs_frame",
+                _check(bits(t.read(ctx)), want, words, "%s target, %s, %s" % (kind, "gs_calc_view + gs_render" if staged else "gs_frame",
                                                                         "selection + depth" if extras else "plain"))
     r.Dispose()
 
@@ -488,7 +409,7 @@ def test_partitioned_draw_keeps_unowned_rows(g, O, ctx):
     cam = camera(g, W, H)
     asset = loaded_scene(g, cam)
     words, init, _fam = loaded_content(O, g, asset, cam, np.float16)
-    want = expected_words(oracle_draw(O, g, asset, cam, None, False, init=init), init, words, np.float16)
+    want = expectedbits(oracle_draw(O, g, asset, cam, None, False, init=init), init, words, np.float16)
     r = g.GaussianSplatRenderer(asset, ctx)
     r.load_rt = True
     for index in (0, 1):
@@ -497,7 +418,7 @@ def test_partitioned_draw_keeps_unowned_rows(g, O, ctx):
         assert not np.array_equal(expect, want) and not np.array_equal(expect, words)
         r.partition = (index, 2, 1)
         for kind in ("host", "device"):
-            t = LoadedTarget(g, None, kind, words, np.float16)
+            t = loaded_target(g, None, kind, words, np.float16)
             gpu_draw(r, cam, t.image, False)
-            _check(t.read(ctx), expect, words, "partition %d of 2, %s target" % (index, kind))
+            _check(bits(t.read(ctx)), expect, words, "partition %d of 2, %s target" % (index, kind))
     r.Dispose()

@@ -14,10 +14,9 @@ from pathlib import Path
 import numpy as np
 import pytest
 
-from test_gpu_frame_cameras import Twins, _Cudart, call_cameras, compare, loop_cameras, orbit
-from test_gpu_frame_objects import Twins as ObjectTwins, _compare_frame
-from test_gpu_sort_tiles import PLAN_SCREENS, _plan_scene
-from util import camera, pixels_per_unit, splat_records, world_at_pixel
+from frame_loops import Twins, call_cameras, compare, compare_frame, loop_cameras, orbit
+from images import ca, launches  # noqa: F401
+from util import PLAN_SCREENS, camera, pixels_per_unit, plan_scene, splat_records, world_at_pixel
 
 ROOT = Path(__file__).resolve().parents[1]
 CSRC = ROOT / "unitygaussiansplatting_b200" / "csrc"
@@ -129,14 +128,6 @@ def test_run_table():
 
 
 # ---- on the GPU ------------------------------------------------------------------------------------------------------------
-@pytest.fixture
-def ca(ctx):
-    c = _Cudart()
-    yield c
-    ctx.sync()
-    c.free_all()
-
-
 def _cameras(g, sizes):
     """One camera per size, each 0.25 units right of the one before: no two cameras of a run see the same picture."""
     return [camera(g, w, h, pos=(0.25 * c, 0.5, -6.0)) for c, (w, h) in enumerate(sizes)]
@@ -148,33 +139,29 @@ def _loop_and_call_passes(name):
     return sum(bin_sort_plan(_bins(s))[0] for s in sizes) + sum(r[2] for r in runs)
 
 
-def _launches(ctx):
-    return ctx.stage_times().kernel_launches
-
-
 @gpu
 @pytest.mark.parametrize("names", [("512", "528"), ("stereo",), ("1024", "1056"), ("4096", "4160"), ("16384", "16512")],
                          ids=lambda n: "-".join(n))
 def test_camera_runs_at_plan_edges(g, ctx, ca, names):
     """Both sides of each plan edge equal the loop, every camera drawing its own scene with splats in its bottom-right bin;
     the launch counts differ by the bin-sort passes the table states (the 512-bin run takes one launch fewer than the 528)."""
-    launches = {}
+    per_set = {}
     for name in names:
         sizes, _runs = RUNS[name]
         cams = _cameras(g, sizes)
-        tw = Twins(g, ctx, [_plan_scene(g, cam, 0) for cam in cams])
+        tw = Twins(g, ctx, [plan_scene(g, cam, 0) for cam in cams])
         try:
-            n0 = _launches(ctx)
+            n0 = launches(ctx)
             drawn = compare(g, ctx, ca, tw, [[0], [1]], cams, 0, np.float16, ["device", "host"], [None, "device"], name)
-            launches[name] = _launches(ctx) - n0
+            per_set[name] = launches(ctx) - n0
             assert drawn == 2, name
         finally:
             tw.dispose()
     if len(names) == 2:
         a, b = names
-        assert launches[b] - launches[a] == _loop_and_call_passes(b) - _loop_and_call_passes(a), launches
+        assert per_set[b] - per_set[a] == _loop_and_call_passes(b) - _loop_and_call_passes(a), per_set
     if names == ("512", "528"):
-        assert launches["528"] - launches["512"] == 1
+        assert per_set["528"] - per_set["512"] == 1
 
 
 @gpu
@@ -183,16 +170,16 @@ def test_run_of_65536_bins_and_the_camera_past_it(g, ctx, ca):
     equal the loop, and the fifth camera costs the call what it costs the loop."""
     sizes, _runs = RUNS["65536+1"]
     cams = _cameras(g, sizes)
-    tw = Twins(g, ctx, [_plan_scene(g, cam, 0) for cam in cams[:4]])
+    tw = Twins(g, ctx, [plan_scene(g, cam, 0) for cam in cams[:4]])
     try:
-        n0 = _launches(ctx)
+        n0 = launches(ctx)
         assert compare(g, ctx, ca, tw, [[0], [1], [2], [3]], cams[:4], 0, np.float16, ["device"] * 4, [None] * 4, "65536") == 4
-        n1 = _launches(ctx)
+        n1 = launches(ctx)
         assert compare(g, ctx, ca, tw, [[0], [1], [2], [3], [0]], cams, 0, np.float16, ["device"] * 5, [None] * 5, "65536+1") == 5
-        n2 = _launches(ctx)
+        n2 = launches(ctx)
         small = np.zeros((64, 64, 4), np.float16)
         loop_cameras(g, ctx, [[tw.loop[0]]], cams[4:], 0, [small], [None])
-        alone = _launches(ctx) - n2
+        alone = launches(ctx) - n2
         # the loop draws the fifth camera once more, and the call draws it as a run of one camera, as the loop does
         assert (n2 - n1) - (n1 - n0) == 2 * alone, (n1 - n0, n2 - n1, alone)
     finally:
@@ -252,7 +239,7 @@ def test_appended_lists_of_several_tiles_per_cta(g, ctx, name):
     ctx = g.GaussianSplatContext(0)   # a fresh context (not the session's): its list has the smallest capacity
     sizes, _runs = RUNS[name]
     cams = _cameras(g, sizes)
-    tw = Twins(g, ctx, [_plan_scene(g, cam, 11 * grid_pairs // 20) for cam in cams])
+    tw = Twins(g, ctx, [plan_scene(g, cam, 11 * grid_pairs // 20) for cam in cams])
     try:
         compare(g, ctx, None, tw, [[0], [1]], cams, 0, np.float16, ["host", "host"], [None, None], name)
         entries = ctx.stage_times().tile_entries
@@ -274,16 +261,16 @@ def test_object_runs_at_plan_edges(g, ctx, ca, size, bins, blend, rt_kind, tgt_k
     object (GS_FLAG_LOAD_RT from the second) plus gs_composite."""
     assert _bins(size) == bins
     cam = camera(g, *size)
-    assets = [_plan_scene(g, cam, 0), g.synthetic_asset(g.SCENE_CLUSTERED, 12000, 0x5EED1150, "VeryHigh"),
+    assets = [plan_scene(g, cam, 0), g.synthetic_asset(g.SCENE_CLUSTERED, 12000, 0x5EED1150, "VeryHigh"),
               g.synthetic_asset(g.SCENE_CLUSTERED, 6000, 0x5EED1151, "Medium")]
 
     def setup(i, r):
         if i:
             r.localToWorldMatrix = g.trs(position=(1.2 * i - 1.8, 0.2, 1.0 * i - 0.5), scale=(0.7, 0.7, 0.7)).astype(np.float32)
 
-    tw = ObjectTwins(g, ctx, assets, setup)
+    tw = Twins(g, ctx, assets, setup)
     try:
-        _compare_frame(g, ctx, ca, tw, cam, blend, np.float16, rt_kind, tgt_kind, "%d bins" % bins)
+        compare_frame(g, ctx, ca, tw, cam, blend, np.float16, rt_kind, tgt_kind, "%d bins" % bins)
     finally:
         tw.dispose()
 
@@ -296,7 +283,7 @@ def test_stereo_run_raster_variants(g, ctx, ca, variant):
     CUDA array beside a tensor, and RGBA32F."""
     import torch
     cams = [camera(g, 1920, 1080), camera(g, 1920, 1080, pos=(0.064, 0.5, -6.0))]
-    assets = [_plan_scene(g, cams[0], 0), g.synthetic_asset(g.SCENE_CLUSTERED, 12000, 0x5EED1160, "VeryHigh"),
+    assets = [plan_scene(g, cams[0], 0), g.synthetic_asset(g.SCENE_CLUSTERED, 12000, 0x5EED1160, "VeryHigh"),
               g.synthetic_asset(g.SCENE_CLUSTERED, 8000, 0x5EED1161, "Medium")]
 
     def setup(i, r):

@@ -10,7 +10,7 @@ from util import camera, one_splat
 W, H = 96, 72
 
 
-def _bits(a):
+def _f32_bits(a):
     return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
@@ -35,10 +35,10 @@ def test_zero_init_is_the_cleared_draw(g, O, scene):
     for blend in (0, 1):
         want = O.render(view, order, W, H, blend)
         assert want[..., 3].any()
-        assert np.array_equal(_bits(O.render(view, order, W, H, blend, init=zeros)), _bits(want))
+        assert np.array_equal(_f32_bits(O.render(view, order, W, H, blend, init=zeros)), _f32_bits(want))
         want_d = O.render(view, order, W, H, blend, scene_depth=depth)
-        assert np.array_equal(_bits(O.render(view, order, W, H, blend, scene_depth=depth, init=zeros)), _bits(want_d))
-        assert np.array_equal(_bits(O.frame(asset, fp, blend_mode=blend, init=zeros)["rt"]), _bits(O.frame(asset, fp, blend_mode=blend)["rt"]))
+        assert np.array_equal(_f32_bits(O.render(view, order, W, H, blend, scene_depth=depth, init=zeros)), _f32_bits(want_d))
+        assert np.array_equal(_f32_bits(O.frame(asset, fp, blend_mode=blend, init=zeros)["rt"]), _f32_bits(O.frame(asset, fp, blend_mode=blend)["rt"]))
 
 
 def test_loaded_content_follows_the_blend_loop(g, O, scene):
@@ -92,19 +92,19 @@ def test_loaded_content_follows_the_blend_loop(g, O, scene):
         want = fused if blend else fused.astype(np.float16).astype(np.float32)
         want = np.where(np.isnan(want), np.uint32(canonical).view(np.float32), want)
         want = np.where(blendable[..., None], want, init)
-        assert np.array_equal(_bits(got), _bits(want)), blend
+        assert np.array_equal(_f32_bits(got), _f32_bits(want)), blend
         # spot checks of what the families promise
         for name in ("alpha 1", "alpha 1, inf colour", "alpha 1, NaN colour"):
             py, px = where[name]
-            assert np.array_equal(_bits(got[py, px]), _bits(init[py, px])), name
+            assert np.array_equal(_f32_bits(got[py, px]), _f32_bits(init[py, px])), name
         py, px = where["alpha 1.5"]
         assert (got[py, px, 3] < 1.5).all()            # om < 0: alpha above 1 keeps blending, downwards
         py, px = where["alpha -0.25"]
         assert (got[py, px, 3] > -0.25).all()
         py, px = where["alpha NaN"]
-        assert (_bits(got[py, px]) == np.uint32(canonical)).all()
+        assert (_f32_bits(got[py, px]) == np.uint32(canonical)).all()
         py, px = where["inf colour"]
         assert (got[py, px, 0] == np.inf).all() and (got[py, px, 1] == -np.inf).all()
         py, px = where["NaN colour"]
-        assert (_bits(got[py, px, 0]) == np.uint32(canonical)).all() and np.isfinite(got[py, px, 1:]).all()
-        assert np.array_equal(_bits(got[~reached]), _bits(init[~reached]))
+        assert (_f32_bits(got[py, px, 0]) == np.uint32(canonical)).all() and np.isfinite(got[py, px, 1:]).all()
+        assert np.array_equal(_f32_bits(got[~reached]), _f32_bits(init[~reached]))

@@ -58,7 +58,7 @@ def _dec(L, m):
     return L.gso_uf11_to_f32 if m == M11 else L.gso_uf10_to_f32
 
 
-def _bits(a):
+def _f32_bits(a):
     return np.asarray(a, np.float32).view(np.uint32)
 
 
@@ -69,9 +69,9 @@ def test_decode_every_code(L, m):
     want = np_decode(codes, m)
     nan = np.isnan(want)
     assert nan.sum() == (1 << m) - 1 and np.isnan(got[nan]).all()
-    assert np.array_equal(_bits(got[~nan]), _bits(want[~nan]))
+    assert np.array_equal(_f32_bits(got[~nan]), _f32_bits(want[~nan]))
     # the quiet NaN keeps the mantissa, so that the device and the oracle agree bit for bit
-    assert np.array_equal(_bits(got[nan]), (0x7FC00000 | ((codes[nan] & ((1 << m) - 1)) << (23 - m))).astype(np.uint32))
+    assert np.array_equal(_f32_bits(got[nan]), (0x7FC00000 | ((codes[nan] & ((1 << m) - 1)) << (23 - m))).astype(np.uint32))
     # round trip of every non-NaN code
     assert all(_enc(L, m)(float(v)) == c for c, v in zip(codes[~nan], want[~nan]))
 
@@ -152,7 +152,7 @@ def test_python_codec_matches_the_oracle(L):
     codes = rng.integers(0, 2 ** 32, 5000, dtype=np.uint64).astype(np.uint32)
     back = unpack_b10g11r11(codes)
     want = np.array([[L.gso_uf11_to_f32(int(c)), L.gso_uf11_to_f32(int(c) >> 11), L.gso_uf10_to_f32(int(c) >> 22)] for c in codes], np.float32)
-    assert np.array_equal(_bits(back), _bits(want))
+    assert np.array_equal(_f32_bits(back), _f32_bits(want))
 
 
 def test_header_constant_and_image_mapping():

@@ -14,21 +14,10 @@ from pathlib import Path
 import numpy as np
 import pytest
 
-from util import view_fields
+from util import screen_cov, unsortable, view_fields
 
 sys.path.insert(0, str(Path(__file__).parent / "golden"))
 import make_ref_hlsl_golden as M  # noqa: E402
-
-
-def _unsortable(keys):
-    k = keys.astype(np.uint32)
-    u = np.where(k & 0x80000000, k ^ np.uint32(0x80000000), ~k).astype(np.uint32)
-    return u.view(np.float32)
-
-
-def _cov(v):
-    a1, a2 = v["axis1"].astype(np.float64), v["axis2"].astype(np.float64)
-    return 0.5 * (a1[:, :, None] * a1[:, None, :] + a2[:, :, None] * a2[:, None, :])
 
 
 def _same_asset(asset, want):
@@ -53,7 +42,7 @@ def test_view_data_matches_the_reference_shader_code(O, quality):
         assert (d == 0).mean() > 0.9
     assert np.array_equal(ref["a"][vis], ora["a"][vis])
     # the two screen axes, through the covariance they encode (eigenvectors of near-circular footprints are ill-defined)
-    cr, co = _cov(ref)[vis], _cov(ora)[vis]
+    cr, co = screen_cov(ref)[vis], screen_cov(ora)[vis]
     rel = np.abs(cr - co).reshape(-1, 4).max(1) / (co[:, 0, 0] + co[:, 1, 1])
     assert np.percentile(rel, 50) < 1e-6 and np.percentile(rel, 99) < 2e-5 and rel.max() < 2e-3
 
@@ -64,7 +53,7 @@ def test_sort_keys_match_the_reference_shader_code(O, quality):
     want = M.reference("keys_" + quality.lower())
     _same_asset(asset, want)
     kr, ko = want["keys"], O.calc_distances(asset, fp, order)[want["idx"]]
-    zr, zo = _unsortable(kr), _unsortable(ko)
+    zr, zo = unsortable(kr), unsortable(ko)
     assert np.abs(zr - zo).max() <= 4e-6 and (kr == ko).mean() > 0.5     # view-space depth of +-36: a couple of ulp
     assert np.array_equal(np.argsort(kr, kind="stable")[:100], np.argsort(ko, kind="stable")[:100]) or (kr == ko).mean() < 1.0
 

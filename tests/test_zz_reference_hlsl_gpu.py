@@ -9,8 +9,7 @@ from pathlib import Path
 import numpy as np
 import pytest
 
-from test_reference_hlsl import _cov, _unsortable
-from util import view_fields
+from util import screen_cov, unsortable, view_fields
 
 GOLD = Path(__file__).parent / "golden"
 sys.path.insert(0, str(GOLD))
@@ -37,7 +36,7 @@ def test_cuda_view_data_and_keys_match_the_reference_shader_code(g, ctx, quality
         d = np.abs(ref[ch][vis] - got[ch][vis])
         assert (d <= np.maximum(np.abs(got[ch][vis]), 2.0 ** -14) * 2.0 ** -9).all(), ch
     assert np.array_equal(ref["a"][vis], got["a"][vis])
-    cr, cg = _cov(ref)[vis], _cov(got)[vis]
+    cr, cg = screen_cov(ref)[vis], screen_cov(got)[vis]
     rel = np.abs(cr - cg).reshape(-1, 4).max(1) / (cg[:, 0, 0] + cg[:, 1, 1])
     assert np.percentile(rel, 50) < 1e-6 and np.percentile(rel, 99) < 2e-5 and rel.max() < 2e-3
     # sorted keys: the reference's key of the splat at each sorted position is the same depth to a couple of ulp, and the
@@ -45,7 +44,7 @@ def test_cuda_view_data_and_keys_match_the_reference_shader_code(g, ctx, quality
     pos = np.empty(len(order), np.int64)
     pos[order] = np.arange(len(order))
     at = pos[idx]
-    assert np.abs(_unsortable(want["keys"]) - _unsortable(keys[at])).max() <= 4e-6
+    assert np.abs(unsortable(want["keys"]) - unsortable(keys[at])).max() <= 4e-6
     ranked = want["keys"][np.argsort(at)]
-    assert (np.diff(_unsortable(ranked).astype(np.float64)) >= -8e-6).all()
+    assert (np.diff(unsortable(ranked).astype(np.float64)) >= -8e-6).all()
     r.Dispose()

@@ -224,6 +224,78 @@ def view_fields(view):
             "a": h(col[:, 1])}
 
 
+
+def unsortable(keys):
+    """The float32 view depths the sortable uint32 distance keys encode."""
+    k = keys.astype(np.uint32)
+    u = np.where(k & 0x80000000, k ^ np.uint32(0x80000000), ~k).astype(np.uint32)
+    return u.view(np.float32)
+
+
+def screen_cov(v):
+    """The 2-D screen covariance 0.5 (axis1 axis1^T + axis2 axis2^T) of view_fields' axes, in float64."""
+    a1, a2 = v["axis1"].astype(np.float64), v["axis2"].astype(np.float64)
+    return 0.5 * (a1[:, :, None] * a1[:, None, :] + a2[:, :, None] * a2[:, None, :])
+
+
+# ---- the bin list at its capacity ---------------------------------------------------------------------------------------
+CAP_W, CAP_H = 4096, 2048         # 64 x 32 bins: two 6-bit sort passes
+CAP_ENTRIES = 4 << 20             # clamp(8 N, 4 Mi, 768 Mi) for N < 512 Ki
+CAP_SPLATS = CAP_ENTRIES // 64    # one full bin row (64 entries) each
+
+
+def bin_row_splats(cam, n, seed):
+    """n wide, flat splats: each one's visible part spans the whole screen width and 5 rows inside one 64-pixel bin row, so
+    it emits exactly 64 (bin, splat) entries while the oracle visits only about 4096 x 9 pixels of it."""
+    rng = np.random.default_rng(seed)
+    i = np.arange(n)
+    depth = 5.0 + 3.0 * rng.random(n)
+    cy = 64.0 * (i % (CAP_H // 64)) + 20.0 + (i // (CAP_H // 64)) % 25
+    pos = world_at_pixel(cam, CAP_W / 2, cy, depth)
+    ppu = pixels_per_unit(cam, depth)[:, None]
+    scale = np.array([0.3 * CAP_W, 0.01, 0.01]) / ppu      # axis1 ~ 0.42 W: the quad reaches 0.85 W beyond the centre
+    dc = rng.random((n, 3)) * 2.0 - 0.5
+    return splat_records(pos, scale, 0.05 + 0.3 * rng.random(n), dc)
+
+
+# ---- the bin sort's plans at their edges --------------------------------------------------------------------------------
+# (width, height): bins = ceil(W/64) * ceil(H/64); bin_sort_plan takes one pass up to 512 bins (5, 6, 7, 8, 9 bits at 32, 64,
+# 128, 256, 512), else two passes of 5, 6, 7, 8 bits up to 1024, 4096, 16384, 65536 bins.  Each plan up to 7 bits at its upper
+# edge and one past it.
+PLAN_SCREENS = [
+    ((512, 256), 32, 1, 5), ((704, 192), 33, 1, 6),
+    ((512, 512), 64, 1, 6), ((832, 320), 65, 1, 7),
+    ((1024, 512), 128, 1, 7), ((2752, 192), 129, 1, 8),
+    ((1024, 1024), 256, 1, 8), ((2752, 384), 258, 1, 9),        # 257 bins is prime: it would need a 16448-pixel row
+    ((1920, 1080), 510, 1, 9), ((2048, 1024), 512, 1, 9),
+    ((2048, 1088), 544, 2, 5), ((1728, 1216), 513, 2, 5),
+    ((2048, 2048), 1024, 2, 5), ((2624, 1600), 1025, 2, 6),
+    ((4096, 4096), 4096, 2, 6), ((5248, 3200), 4100, 2, 7),
+    ((8160, 8160), 16384, 2, 7),                                # also the largest camera a camera run takes
+]
+
+
+def plan_scene(g, cam, entries):
+    """The clustered scene, a few small splats in the bottom-right bin (where a digit one bit too narrow mis-sorts), and,
+    when `entries` is set, wide flat splats across the whole screen on the bin-row boundaries: 2 x binsX entries each,
+    as many as give about `entries`."""
+    W, H = cam.pixelWidth, cam.pixelHeight
+    base = g.generate_input_splats(g.SCENE_CLUSTERED, 60000, 0x5EED0002)
+    ppu = pixels_per_unit(cam, 6.0)
+    corner = splat_records(world_at_pixel(cam, [W - 20.5, W - 6.0, W - 40.2], [H - 18.3, H - 40.0, H - 5.5], 6.0),
+                           np.array([3.0, 2.0, 2.5]) / ppu, 0.9, (0.2, 0.9, 0.4))
+    parts = [base, corner]
+    if entries:
+        bins_x, bins_y = -(-W // 64), -(-H // 64)
+        n = -(-entries // (2 * bins_x))
+        rng = np.random.default_rng(W * H)
+        depth = 5.0 + 3.0 * rng.random(n)
+        cy = 64.0 * (1 + np.arange(n) % (bins_y - 1))
+        scale = np.array([0.3 * W, 0.01, 0.01]) / pixels_per_unit(cam, depth)[:, None]
+        parts.append(splat_records(world_at_pixel(cam, W / 2, cy, depth), scale, 0.1 + 0.3 * rng.random(n), rng.random((n, 3))))
+    return g.create_asset(np.ascontiguousarray(np.concatenate(parts)), "Medium")
+
+
 # ---- asset format combinations no preset uses ------------------------------------------------------------------------------
 # The importer's Custom quality lets a user pick any (position, scale, colour, SH) format.  One list of combinations, chosen so
 # that between them they reach every decode path of the view, distance and export kernels (tests/test_format_cases.py checks
