@@ -585,8 +585,11 @@ GS_API int gs_debug_sort_phases(GsContext *ctx, uint64_t *out, uint32_t max_word
 typedef enum GsUnityEvent {
   GS_UNITY_EVENT_FRAME = 1,   /* gs_frame(ctx, asset, &params, &options, do_sort, has_rt ? &rt : NULL, has_camera_target ? &camera_target : NULL) */
   GS_UNITY_EVENT_SYNC = 2,    /* gs_sync(ctx) */
-  GS_UNITY_EVENT_FRAME_OBJECTS = 3   /* data is a GsUnityFrameObjectsEvent: gs_frame_objects(ctx, object_count, assets, fps,
+  GS_UNITY_EVENT_FRAME_OBJECTS = 3,  /* data is a GsUnityFrameObjectsEvent: gs_frame_objects(ctx, object_count, assets, fps,
                                         do_sort, &options, has_rt ? &rt : NULL, has_camera_target ? &camera_target : NULL) */
+  GS_UNITY_EVENT_FRAME_CAMERAS = 4,  /* data is a GsUnityFrameCamerasEvent: gs_frame_cameras (below) */
+  GS_UNITY_EVENT_GROUP_FRAME_OBJECTS = 5,   /* data is a GsUnityGroupFrameObjectsEvent: gs_group_frame_objects (below) */
+  GS_UNITY_EVENT_GROUP_SYNC = 6      /* data is a GsUnityGroupSyncEvent: gs_group_sync(group) */
 } GsUnityEvent;
 
 typedef struct GsUnityFrameEvent {
@@ -614,10 +617,74 @@ typedef struct GsUnityFrameObjectsEvent {
   GsImage rt, camera_target;
 } GsUnityFrameObjectsEvent;
 
+/* The payloads of events 4-6 pass images BY VALUE, in arrays of GsImage: an image whose `data` is NULL is "none" (a NULL rt or
+ * camera target of the direct call), and a NULL array pointer is the direct call's NULL array.  A managed GsImage[] is then
+ * pinned once, and no payload holds a pointer to pointers.  Every array a payload points to, and every GsArrayLayer /
+ * GsArrayRect descriptor an image's `data` (or a GsFrameParams' scene_depth) points to, is borrowed: the managed side keeps
+ * it pinned (with the payload itself) until the command buffer has executed.  The library never writes them.
+ * Each event runs its entry point on the render thread and stores the GsStatus in `status`, which the managed side sets to
+ * GS_ERR_NOT_READY when it records the event; the library leaves it alone until the event runs.  An error is reported in
+ * `status` and through gs_last_error of the context named below, with the entry point's own code and text; the callback never
+ * throws and never aborts.  The device work of an event is the direct call's, launch for launch.  Unity's render thread may
+ * have another CUDA device current: the entry points make their contexts' devices current themselves, and the callback makes
+ * no CUDA call of its own, so an event leaves current the device the direct call leaves.  The `reserved` words are 0. */
+
+/* GS_UNITY_EVENT_FRAME_CAMERAS: gs_frame_cameras(ctx, camera_count, object_counts, assets, fps, do_sort, &options, rts',
+ * camera_targets') where rts'[c] = &rts[c] (NULL where rts[c].data is NULL), likewise camera_targets' -- e.g. the two eyes
+ * of a single-pass-instanced XR eye-texture array drawn into layers 0 and 1 as one camera run (GS_MEM_ARRAY_LAYER), or the
+ * tiles of an atlas or light-field quilt (GS_MEM_ARRAY_RECT).  At most GS_UNITY_EVENT_MAX_CAMERAS cameras per event: more is
+ * GS_ERR_INVALID_ARGUMENT with nothing enqueued (the callback does not allocate; a host with more views issues one event per
+ * GS_UNITY_EVENT_MAX_CAMERAS cameras, whose result is the same, as gs_frame_cameras is defined as its camera loop).  Errors:
+ * gs_last_error(ctx). */
+#define GS_UNITY_EVENT_MAX_CAMERAS 64u
+typedef struct GsUnityFrameCamerasEvent {
+  GsContext *ctx;
+  uint32_t camera_count, reserved0;
+  const uint32_t *object_counts;   /* [camera_count] */
+  GsAsset *const *assets;          /* [sum of object_counts], camera-major as in gs_frame_cameras */
+  const GsFrameParams *fps;        /* [sum of object_counts] */
+  const int32_t *do_sort;          /* [sum of object_counts] */
+  GsRenderOptions options;
+  const GsImage *rts;              /* [camera_count], by value */
+  const GsImage *camera_targets;   /* [camera_count], by value */
+  int32_t status;                  /* out: GsStatus of the call (GS_ERR_NOT_READY until the event has run) */
+  uint32_t reserved1[3];
+} GsUnityFrameCamerasEvent;        /* 112 bytes */
+
+/* GS_UNITY_EVENT_GROUP_FRAME_OBJECTS: gs_group_frame_objects(group, object_count, assets, fps, do_sort, &options, rts',
+ * camera_targets'), images as above, one per LOCAL member (gs_group_local_count).  The event is collective, as the call is.
+ * It holds Unity's render thread where the call blocks: once for all objects' slab tables when the group has several GPUs and
+ * an object sorts (see gs_group_frame_objects), and until the transfer streams are done when an image is in host memory and
+ * GS_FLAG_ASYNC_READBACK is not set.
+ * Errors: gs_last_error of the group's member-0 context (gs_group_context(group, 0)), whichever member the direct call named. */
+typedef struct GsUnityGroupFrameObjectsEvent {
+  GsGroup *group;
+  uint32_t object_count, reserved0;
+  GsAsset *const *assets;          /* [object_count][local_count], as in gs_group_frame_objects */
+  const GsFrameParams *fps;        /* [object_count] */
+  const int32_t *do_sort;          /* [object_count] */
+  GsRenderOptions options;
+  const GsImage *rts;              /* [local_count], by value */
+  const GsImage *camera_targets;   /* [local_count], by value */
+  int32_t status;                  /* out: GsStatus of the call (GS_ERR_NOT_READY until the event has run) */
+  uint32_t reserved1[3];
+} GsUnityGroupFrameObjectsEvent;   /* 104 bytes */
+
+/* GS_UNITY_EVENT_GROUP_SYNC: gs_group_sync(group); blocks the render thread until every member's streams are done.  Errors:
+ * gs_last_error of the member-0 context. */
+typedef struct GsUnityGroupSyncEvent {
+  GsGroup *group;
+  int32_t status;                  /* out: GsStatus of the call (GS_ERR_NOT_READY until the event has run) */
+  uint32_t reserved;
+} GsUnityGroupSyncEvent;           /* 16 bytes */
+
 typedef void (*GsUnityRenderEventAndDataFunc)(int event_id, void *data);
 GS_API GsUnityRenderEventAndDataFunc gs_unity_get_render_event_func(void);
 GS_API uint32_t gs_unity_frame_event_size(void);   /* sizeof(GsUnityFrameEvent), for the managed side's layout check */
 GS_API uint32_t gs_unity_frame_objects_event_size(void);   /* sizeof(GsUnityFrameObjectsEvent) */
+GS_API uint32_t gs_unity_frame_cameras_event_size(void);   /* sizeof(GsUnityFrameCamerasEvent) */
+GS_API uint32_t gs_unity_group_frame_objects_event_size(void);   /* sizeof(GsUnityGroupFrameObjectsEvent) */
+GS_API uint32_t gs_unity_group_sync_event_size(void);   /* sizeof(GsUnityGroupSyncEvent) */
 
 /* ---- device-pointer access for zero-copy hosts (torch / CUDA-Vulkan interop) ----- */
 GS_API void *gs_context_stream(GsContext *ctx);

@@ -103,7 +103,26 @@ class GsUnityFrameObjectsEvent(C.Structure):   # the payload of GS_UNITY_EVENT_F
                 ("rt", GsImage), ("camera_target", GsImage)]
 
 
+class GsUnityFrameCamerasEvent(C.Structure):   # the payload of GS_UNITY_EVENT_FRAME_CAMERAS; images by value
+    _fields_ = [("ctx", C.c_void_p), ("camera_count", C.c_uint32), ("reserved0", C.c_uint32), ("object_counts", C.c_void_p),
+                ("assets", C.c_void_p), ("fps", C.c_void_p), ("do_sort", C.c_void_p), ("options", GsRenderOptions),
+                ("rts", C.c_void_p), ("camera_targets", C.c_void_p), ("status", C.c_int32), ("reserved1", C.c_uint32 * 3)]
+
+
+class GsUnityGroupFrameObjectsEvent(C.Structure):   # the payload of GS_UNITY_EVENT_GROUP_FRAME_OBJECTS; images by value
+    _fields_ = [("group", C.c_void_p), ("object_count", C.c_uint32), ("reserved0", C.c_uint32), ("assets", C.c_void_p),
+                ("fps", C.c_void_p), ("do_sort", C.c_void_p), ("options", GsRenderOptions), ("rts", C.c_void_p),
+                ("camera_targets", C.c_void_p), ("status", C.c_int32), ("reserved1", C.c_uint32 * 3)]
+
+
+class GsUnityGroupSyncEvent(C.Structure):   # the payload of GS_UNITY_EVENT_GROUP_SYNC
+    _fields_ = [("group", C.c_void_p), ("status", C.c_int32), ("reserved", C.c_uint32)]
+
+
 GS_UNITY_EVENT_FRAME, GS_UNITY_EVENT_SYNC, GS_UNITY_EVENT_FRAME_OBJECTS = 1, 2, 3
+GS_UNITY_EVENT_FRAME_CAMERAS, GS_UNITY_EVENT_GROUP_FRAME_OBJECTS, GS_UNITY_EVENT_GROUP_SYNC = 4, 5, 6
+GS_UNITY_EVENT_MAX_CAMERAS = 64
+GS_ERR_NOT_READY = -5
 GsUnityRenderEventAndDataFunc = C.CFUNCTYPE(None, C.c_int, C.c_void_p)
 
 
@@ -184,6 +203,9 @@ NATIVE_SYMBOLS = {
     "gs_unity_get_render_event_func": (GsUnityRenderEventAndDataFunc, []),
     "gs_unity_frame_event_size": (C.c_uint32, []),
     "gs_unity_frame_objects_event_size": (C.c_uint32, []),
+    "gs_unity_frame_cameras_event_size": (C.c_uint32, []),
+    "gs_unity_group_frame_objects_event_size": (C.c_uint32, []),
+    "gs_unity_group_sync_event_size": (C.c_uint32, []),
     "gs_export_splats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     "gs_debug_raster_stats": (C.c_int, [C.c_void_p, C.c_void_p]),
     "gs_debug_sort_phases": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]),
@@ -224,6 +246,15 @@ def _bind(lib, table):
     return lib
 
 
+# the render-thread payloads and the size functions the managed side checks its layouts against
+UNITY_PAYLOADS = {
+    "gs_unity_frame_event_size": GsUnityFrameEvent,
+    "gs_unity_frame_objects_event_size": GsUnityFrameObjectsEvent,
+    "gs_unity_frame_cameras_event_size": GsUnityFrameCamerasEvent,
+    "gs_unity_group_frame_objects_event_size": GsUnityGroupFrameObjectsEvent,
+    "gs_unity_group_sync_event_size": GsUnityGroupSyncEvent,
+}
+
 _native = None
 _asset = None
 
@@ -234,7 +265,12 @@ def native():
     if _native is None:
         if not NATIVE_LIB.exists():
             raise GsError(-100, "CUDA extension %s is missing; run `python -c 'import __graft_entry__ as g; g.build()'`" % NATIVE_LIB)
-        _native = _bind(C.CDLL(str(NATIVE_LIB)), NATIVE_SYMBOLS)
+        lib = _bind(C.CDLL(str(NATIVE_LIB)), NATIVE_SYMBOLS)
+        for size_fn, payload in UNITY_PAYLOADS.items():   # a payload of another layout would be read as garbage
+            if getattr(lib, size_fn)() != C.sizeof(payload):
+                raise GsError(-100, "%s: the library's payload is %d bytes, the binding's %d" % (payload.__name__, getattr(lib, size_fn)(),
+                                                                                             C.sizeof(payload)))
+        _native = lib
     return _native
 
 
@@ -245,6 +281,22 @@ def asset_lib():
             raise GsError(-100, "asset packer %s is missing; run the build first" % ASSET_LIB)
         _asset = _bind(C.CDLL(str(ASSET_LIB)), ASSET_SYMBOLS)
     return _asset
+
+
+def unity_event(event_id: int, payload) -> int:
+    """Runs a render-thread event on this thread, as Unity's render thread runs what CommandBuffer.IssuePluginEventAndData
+    recorded: the callback of gs_unity_get_render_event_func on the payload.  Returns the payload's status."""
+    native().gs_unity_get_render_event_func()(event_id, C.addressof(payload))
+    return payload.status
+
+
+def image_array(images):
+    """A GsImage[] of the images by value, as the payloads of events 4-6 take them (None: an image with NULL data)."""
+    arr = (GsImage * len(images))()
+    for i, im in enumerate(images):
+        if im is not None:
+            arr[i] = im
+    return arr
 
 
 def check(ctx, rc: int):

@@ -986,6 +986,21 @@ int gs_frame_cameras(GsContext *ctx, uint32_t camera_count, const uint32_t *obje
   return draw_cameras(ctx, cams, assets, fps, do_sort_flags, opt);
 }
 
+// GS_UNITY_EVENT_FRAME_CAMERAS: the payload's by-value images as the GsImage * arrays gs_frame_cameras takes, on the stack
+static void unity_frame_cameras_event(GsUnityFrameCamerasEvent *ev) {
+  if (ev->camera_count > GS_UNITY_EVENT_MAX_CAMERAS) {
+    ev->status = fail(ev->ctx, GS_ERR_INVALID_ARGUMENT, "more than GS_UNITY_EVENT_MAX_CAMERAS cameras in one event: issue one event per 64 cameras");
+    return;
+  }
+  GsImage *rts[GS_UNITY_EVENT_MAX_CAMERAS], *tgts[GS_UNITY_EVENT_MAX_CAMERAS];
+  for (uint32_t c = 0; c < ev->camera_count; ++c) {
+    rts[c] = ev->rts && ev->rts[c].data ? const_cast<GsImage *>(&ev->rts[c]) : nullptr;
+    tgts[c] = ev->camera_targets && ev->camera_targets[c].data ? const_cast<GsImage *>(&ev->camera_targets[c]) : nullptr;
+  }
+  ev->status = gs_frame_cameras(ev->ctx, ev->camera_count, ev->object_counts, ev->assets, ev->fps, ev->do_sort, &ev->options,
+                                ev->rts ? rts : nullptr, ev->camera_targets ? tgts : nullptr);
+}
+
 int gs_unshuffle_bands(GsContext *ctx, const void *gathered, uint32_t parts, uint32_t band_rows, uint32_t rows_pp, uint32_t fmt,
                        GsImage *out) {
   if (!ctx || !gathered || !out || parts == 0) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "null argument");
@@ -1083,14 +1098,21 @@ int gs_upload_order(GsAsset *as, const uint32_t *src) {
   return GS_OK;
 }
 
-// ---- Unity render-thread entry: IssuePluginEventAndData -> gs_frame / gs_sync ----
+// ---- Unity render-thread entry: IssuePluginEventAndData -> gs_frame / gs_sync / gs_frame_objects / gs_frame_cameras / the
+// group calls (gs_group.cu) ----
 static void gs_unity_on_render_event(int event_id, void *data) {
   if (!data) return;
-  if (event_id == GS_UNITY_EVENT_FRAME_OBJECTS) {
-    GsUnityFrameObjectsEvent *ev = static_cast<GsUnityFrameObjectsEvent *>(data);
-    ev->status = gs_frame_objects(ev->ctx, ev->object_count, ev->assets, ev->fps, ev->do_sort, &ev->options, ev->has_rt ? &ev->rt : nullptr,
-                                  ev->has_camera_target ? &ev->camera_target : nullptr);
-    return;
+  switch (event_id) {
+    case GS_UNITY_EVENT_FRAME_OBJECTS: {
+      GsUnityFrameObjectsEvent *ev = static_cast<GsUnityFrameObjectsEvent *>(data);
+      ev->status = gs_frame_objects(ev->ctx, ev->object_count, ev->assets, ev->fps, ev->do_sort, &ev->options, ev->has_rt ? &ev->rt : nullptr,
+                                    ev->has_camera_target ? &ev->camera_target : nullptr);
+      return;
+    }
+    case GS_UNITY_EVENT_FRAME_CAMERAS: unity_frame_cameras_event(static_cast<GsUnityFrameCamerasEvent *>(data)); return;
+    case GS_UNITY_EVENT_GROUP_FRAME_OBJECTS: unity_group_frame_objects_event(static_cast<GsUnityGroupFrameObjectsEvent *>(data)); return;
+    case GS_UNITY_EVENT_GROUP_SYNC: unity_group_sync_event(static_cast<GsUnityGroupSyncEvent *>(data)); return;
+    default: break;
   }
   GsUnityFrameEvent *ev = static_cast<GsUnityFrameEvent *>(data);
   switch (event_id) {
@@ -1108,6 +1130,9 @@ static void gs_unity_on_render_event(int event_id, void *data) {
 GsUnityRenderEventAndDataFunc gs_unity_get_render_event_func(void) { return gs_unity_on_render_event; }
 uint32_t gs_unity_frame_event_size(void) { return (uint32_t)sizeof(GsUnityFrameEvent); }
 uint32_t gs_unity_frame_objects_event_size(void) { return (uint32_t)sizeof(GsUnityFrameObjectsEvent); }
+uint32_t gs_unity_frame_cameras_event_size(void) { return (uint32_t)sizeof(GsUnityFrameCamerasEvent); }
+uint32_t gs_unity_group_frame_objects_event_size(void) { return (uint32_t)sizeof(GsUnityGroupFrameObjectsEvent); }
+uint32_t gs_unity_group_sync_event_size(void) { return (uint32_t)sizeof(GsUnityGroupSyncEvent); }
 
 int gs_debug_raster_stats(GsContext *ctx, uint64_t out[8]) {
   if (!ctx || !out) return GS_ERR_INVALID_ARGUMENT;

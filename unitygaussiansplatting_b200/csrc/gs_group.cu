@@ -536,6 +536,20 @@ int gs_group_sync(GsGroup *g) {
   return rc;
 }
 
+}  // extern "C"
+
+namespace gs {
+// An event's status, its text also on member 0's context: the managed side reads gs_last_error there, whichever member failed.
+static int event_status(GsGroup *g, int rc) {
+  if (rc != GS_OK && g && !g->m.empty()) fail(g->m[0].ctx, rc, std::string(gs_last_error(nullptr)));
+  return rc;
+}
+
+void unity_group_sync_event(GsUnityGroupSyncEvent *ev) { ev->status = event_status(ev->group, gs_group_sync(ev->group)); }
+}  // namespace gs
+
+extern "C" {
+
 // One camera's frame of K splat objects on the group (gs_group_frame_objects; gs_group_frame is K = 1).  assets: [K][local
 // count].  strict: the new entry point's rules (GS_FLAG_LOAD_RT is refused); gs_group_frame ignores the flag, as it always has.
 static int group_frame(GsGroup *g, uint32_t K, GsAsset *const *assets, const GsFrameParams *fps, const int32_t *do_sort,
@@ -919,6 +933,24 @@ int gs_group_frame_objects(GsGroup *g, uint32_t object_count, GsAsset *const *as
   if (!assets || !fps || !do_sort) return fail(g->m[0].ctx, GS_ERR_INVALID_ARGUMENT, "null argument");
   return group_frame(g, object_count, assets, fps, do_sort, opt, rts, camera_targets, true);
 }
+
+}  // extern "C"
+
+namespace gs {
+// GS_UNITY_EVENT_GROUP_FRAME_OBJECTS: the payload's by-value images as the GsImage * arrays gs_group_frame_objects takes
+void unity_group_frame_objects_event(GsUnityGroupFrameObjectsEvent *ev) {
+  GsGroup *g = ev->group;
+  GsImage *rts[GS_GROUP_MAX_GPUS], *cams[GS_GROUP_MAX_GPUS];
+  for (size_t i = 0; g && i < g->m.size(); ++i) {
+    rts[i] = ev->rts && ev->rts[i].data ? const_cast<GsImage *>(&ev->rts[i]) : nullptr;
+    cams[i] = ev->camera_targets && ev->camera_targets[i].data ? const_cast<GsImage *>(&ev->camera_targets[i]) : nullptr;
+  }
+  ev->status = event_status(g, gs_group_frame_objects(g, ev->object_count, ev->assets, ev->fps, ev->do_sort, &ev->options,
+                                                      ev->rts ? rts : nullptr, ev->camera_targets ? cams : nullptr));
+}
+}  // namespace gs
+
+extern "C" {
 
 int gs_group_get_stats(GsGroup *g, GsGroupStats *out) {
   if (!g || !out) return fail(nullptr, GS_ERR_INVALID_ARGUMENT, "null argument");

@@ -320,6 +320,10 @@ int bind_depth(GsContext *ctx, CallSurfaces *surfs, const GsFrameParams *fp, flo
 cudaError_t asset_init_work(GsContext *ctx, GsAsset *as, uint32_t n, uint32_t pos_fmt, uint32_t scale_fmt, uint32_t sh_fmt,
                             uint32_t col_fmt, uint32_t chunk_count);
 void rec(GsContext *ctx, int e);
+// The render-thread events of the group calls (gs_group.cu), which gs_api.cu's event callback dispatches to: each runs its
+// entry point on the payload and stores the GsStatus in the payload's `status`.
+void unity_group_frame_objects_event(GsUnityGroupFrameObjectsEvent *ev);
+void unity_group_sync_event(GsUnityGroupSyncEvent *ev);
 void launch_row_costs(const uint32_t *cost, uint32_t ntx, uint32_t t0, uint32_t t1, uint32_t *row_cost, cudaStream_t s,
                       bool accumulate = false);   // gs_raster.cu
 }  // namespace gs

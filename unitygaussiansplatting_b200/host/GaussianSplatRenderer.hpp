@@ -72,6 +72,28 @@ inline GsImage PackedCameraTarget(void *data, uint32_t width, uint32_t height, u
   return im;
 }
 
+// The payload of GS_UNITY_EVENT_FRAME_CAMERAS (GaussianSplatRenderer::FillFrameCamerasEvent) and the arrays it points to.
+// `event` points into this object: keep it alive and unmoved until the event has run, and with it the renderers (their
+// cutouts), the host images and the GsArrayLayer / GsArrayRect descriptors the images point to.
+struct UnityFrameCamerasEvent {
+  GsUnityFrameCamerasEvent event{};
+  std::vector<uint32_t> counts;
+  std::vector<GsAsset *> assets;
+  std::vector<GsFrameParams> fps;
+  std::vector<int32_t> doSort;
+  std::vector<GsImage> rts, cameraTargets;   // by value; data == nullptr: none
+};
+
+// The payload of GS_UNITY_EVENT_GROUP_FRAME_OBJECTS (GaussianSplatRendererGroup::FillFrameObjectsEvent) and its arrays, under
+// the same rule.
+struct UnityGroupFrameObjectsEvent {
+  GsUnityGroupFrameObjectsEvent event{};
+  std::vector<GsAsset *> assets;
+  std::vector<GsFrameParams> fps;
+  std::vector<int32_t> doSort;
+  std::vector<GsImage> rts, cameraTargets;   // by value, one per local member; data == nullptr: none
+};
+
 class GaussianSplatRenderer {
  public:
   // serialized knobs, :225-251
@@ -182,6 +204,71 @@ class GaussianSplatRenderer {
   // checks (screen and image sizes) returns false after they moved, as SortAndRenderSplatsMulti does.
   static bool SortAndRenderSplatsCameras(const std::vector<CameraState> &cams, const std::vector<GaussianSplatRenderer *> &renderers,
                                          const std::vector<GsImage *> &rts, const std::vector<GsImage *> &cameraTargets) {
+    bool oneCall = false;
+    if (!CheckCameras(cams, renderers, rts, cameraTargets, &oneCall)) return false;
+    if (renderers.empty()) return true;
+    if (!oneCall) {
+      for (size_t c = 0; c < cams.size(); ++c)
+        if (!SortAndRenderSplatsMulti(cams[c], renderers, rts[c], cameraTargets[c])) return false;
+      return true;
+    }
+    std::vector<uint32_t> counts;
+    std::vector<GsAsset *> assets;
+    std::vector<GsFrameParams> fps;
+    std::vector<int32_t> doSort;
+    GaussianSplatRenderer *first = GatherCameras(cams, renderers, counts, assets, fps, doSort);
+    if (!first) return true;   // no camera
+    GsRenderOptions opt = first->options;
+    opt.flags &= ~(uint32_t)GS_FLAG_LOAD_RT;
+    return first->ok(gs_frame_cameras(first->m_Ctx, (uint32_t)counts.size(), counts.data(), assets.data(), fps.data(), doSort.data(), &opt,
+                                      rts.data(), cameraTargets.data()));
+  }
+  // The render-thread event of SortAndRenderSplatsCameras' one call: fills *out with the payload of
+  // GS_UNITY_EVENT_FRAME_CAMERAS (status GS_ERR_NOT_READY) for CommandBuffer.IssuePluginEventAndData, with the same checks,
+  // GatherSplatsForCamera order and frame-counter steps, and the images copied by value.  Returns false, with no frame counter
+  // moved, where SortAndRenderSplatsCameras would return false before drawing, where it would draw nothing (no renderer or no
+  // camera), and where the renderers' options make it a loop of calls, which no one event carries.
+  static bool FillFrameCamerasEvent(const std::vector<CameraState> &cams, const std::vector<GaussianSplatRenderer *> &renderers,
+                                    const std::vector<GsImage *> &rts, const std::vector<GsImage *> &cameraTargets, UnityFrameCamerasEvent *out) {
+    bool oneCall = false;
+    if (!out || !CheckCameras(cams, renderers, rts, cameraTargets, &oneCall) || !oneCall || renderers.empty() || cams.empty()) return false;
+    GaussianSplatRenderer *first = GatherCameras(cams, renderers, out->counts, out->assets, out->fps, out->doSort);
+    out->rts.assign(cams.size(), GsImage{});
+    out->cameraTargets.assign(cams.size(), GsImage{});
+    for (size_t c = 0; c < cams.size(); ++c) {
+      if (rts[c]) out->rts[c] = *rts[c];
+      if (cameraTargets[c]) out->cameraTargets[c] = *cameraTargets[c];
+    }
+    GsUnityFrameCamerasEvent &ev = out->event;
+    std::memset(&ev, 0, sizeof(ev));
+    ev.ctx = first->m_Ctx;
+    ev.camera_count = (uint32_t)out->counts.size();
+    ev.object_counts = out->counts.data();
+    ev.assets = out->assets.data();
+    ev.fps = out->fps.data();
+    ev.do_sort = out->doSort.data();
+    ev.options = first->options;
+    ev.options.flags &= ~(uint32_t)GS_FLAG_LOAD_RT;
+    ev.rts = out->rts.data();
+    ev.camera_targets = out->cameraTargets.data();
+    ev.status = GS_ERR_NOT_READY;
+    return true;
+  }
+  bool Sync() { return ok(gs_sync(m_Ctx)); }
+  // EditExportData, R/GaussianSplatRenderer.cs:936-958: n x 62 floats (the .ply attribute record), cut splats marked by nor = 1
+  bool EditExportData(float *dstRecords, bool bakeTransform = false) {
+    return ok(gs_export_splats(m_Ctx, m_Asset, m_Cutouts.empty() ? nullptr : m_Cutouts.data(), (uint32_t)m_Cutouts.size(), bakeTransform ? 1u : 0u,
+                               dstRecords));
+  }
+  GsContext *context() const { return m_Ctx; }
+  GsAsset *asset() const { return m_Asset; }
+
+ private:
+  // What SortAndRenderSplatsCameras checks before any frame counter moves.  *oneCall: the renderers share their options
+  // (GS_FLAG_LOAD_RT aside) and none asks for GS_FLAG_ASYNC_READBACK, so that one gs_frame_cameras call draws every camera.
+  static bool CheckCameras(const std::vector<CameraState> &cams, const std::vector<GaussianSplatRenderer *> &renderers,
+                           const std::vector<GsImage *> &rts, const std::vector<GsImage *> &cameraTargets, bool *oneCall) {
+    *oneCall = true;
     if (rts.size() != cams.size() || cameraTargets.size() != cams.size()) return false;
     if (renderers.empty()) return true;
     for (const GaussianSplatRenderer *r : renderers)   // checked before any renderer's frame counter moves
@@ -198,18 +285,16 @@ class GaussianSplatRenderer {
              a.partition_count == b.partition_count && a.band_rows == b.band_rows && a.row_begin == b.row_begin && a.row_end == b.row_end &&
              ((a.flags ^ b.flags) & ~(uint32_t)GS_FLAG_LOAD_RT) == 0 && !(a.flags & GS_FLAG_ASYNC_READBACK);
     };
-    bool oneCall = true;
-    for (const GaussianSplatRenderer *r : renderers) oneCall = oneCall && same(r->options, renderers[0]->options);
-    if (!oneCall) {
-      for (size_t c = 0; c < cams.size(); ++c)
-        if (!SortAndRenderSplatsMulti(cams[c], renderers, rts[c], cameraTargets[c])) return false;
-      return true;
-    }
-    std::vector<uint32_t> counts;
-    std::vector<GsAsset *> assets;
-    std::vector<GsFrameParams> fps;
-    std::vector<int32_t> doSort;
-    std::vector<GsImage *> camRts, camTargets;
+    for (const GaussianSplatRenderer *r : renderers) *oneCall = *oneCall && same(r->options, renderers[0]->options);
+    return true;
+  }
+  // gs_frame_cameras' per-object arguments: every camera's renderers in GatherSplatsForCamera order (:73-105), camera after
+  // camera, each renderer's frame counter advanced once per camera (:120-122).  Returns the first renderer drawn (nullptr: no
+  // camera).
+  static GaussianSplatRenderer *GatherCameras(const std::vector<CameraState> &cams, const std::vector<GaussianSplatRenderer *> &renderers,
+                                              std::vector<uint32_t> &counts, std::vector<GsAsset *> &assets, std::vector<GsFrameParams> &fps,
+                                              std::vector<int32_t> &doSort) {
+    counts.clear(); assets.clear(); fps.clear(); doSort.clear();
     GaussianSplatRenderer *first = nullptr;
     for (size_t c = 0; c < cams.size(); ++c) {
       const CameraState &cam = cams[c];
@@ -224,8 +309,6 @@ class GaussianSplatRenderer {
       });
       if (!first) first = order[0];
       counts.push_back((uint32_t)order.size());
-      camRts.push_back(rts[c]);
-      camTargets.push_back(cameraTargets[c]);
       for (GaussianSplatRenderer *r : order) {
         assets.push_back(r->m_Asset);
         fps.push_back(r->params(cam));
@@ -233,22 +316,8 @@ class GaussianSplatRenderer {
         ++r->m_FrameCounter;
       }
     }
-    if (counts.empty()) return true;   // no camera
-    GsRenderOptions opt = first->options;
-    opt.flags &= ~(uint32_t)GS_FLAG_LOAD_RT;
-    return first->ok(gs_frame_cameras(first->m_Ctx, (uint32_t)counts.size(), counts.data(), assets.data(), fps.data(), doSort.data(), &opt,
-                                      camRts.data(), camTargets.data()));
+    return first;
   }
-  bool Sync() { return ok(gs_sync(m_Ctx)); }
-  // EditExportData, R/GaussianSplatRenderer.cs:936-958: n x 62 floats (the .ply attribute record), cut splats marked by nor = 1
-  bool EditExportData(float *dstRecords, bool bakeTransform = false) {
-    return ok(gs_export_splats(m_Ctx, m_Asset, m_Cutouts.empty() ? nullptr : m_Cutouts.data(), (uint32_t)m_Cutouts.size(), bakeTransform ? 1u : 0u,
-                               dstRecords));
-  }
-  GsContext *context() const { return m_Ctx; }
-  GsAsset *asset() const { return m_Asset; }
-
- private:
   GsFrameParams params(const CameraState &cam) const {  // CalcViewData / SortPoints uniform binding, :586-606,:617-631
     GsFrameParams fp;
     std::memset(&fp, 0, sizeof(fp));
@@ -367,11 +436,61 @@ class GaussianSplatRendererGroup : public GaussianSplatGroupObject {
   // GatherSplatsForCamera order (:73-105) into one target, then composited onto cameraTargets[i] (may be nullptr / hold nullptrs).
   bool SortAndRenderSplatsMulti(const CameraState &cam, std::vector<GaussianSplatGroupObject *> objects, GsImage *const *rts,
                                 GsImage *const *cameraTargets = nullptr) {
+    if (objects.empty()) return true;   // no active splat object: OnPreCullCamera draws nothing
+    std::vector<GsAsset *> assets;
+    std::vector<GsFrameParams> fps;
+    std::vector<int32_t> doSort;
+    if (!GatherObjects(cam, std::move(objects), assets, fps, doSort)) return false;
+    return ok(gs_group_frame_objects(m_Group, (uint32_t)fps.size(), assets.data(), fps.data(), doSort.data(), &options, rts, cameraTargets));
+  }
+  // The render-thread event of SortAndRenderSplatsMulti: fills *out with the payload of GS_UNITY_EVENT_GROUP_FRAME_OBJECTS
+  // (status GS_ERR_NOT_READY) with the same checks, GatherSplatsForCamera order and frame-counter steps; rts / cameraTargets
+  // (each may be nullptr or hold nullptrs) are copied by value, one image per local member.  Returns false, with no frame
+  // counter moved, where SortAndRenderSplatsMulti would return false before drawing, or draw nothing (no object).
+  bool FillFrameObjectsEvent(const CameraState &cam, std::vector<GaussianSplatGroupObject *> objects, GsImage *const *rts,
+                             GsImage *const *cameraTargets, UnityGroupFrameObjectsEvent *out) {
+    if (!out || objects.empty() || !GatherObjects(cam, std::move(objects), out->assets, out->fps, out->doSort)) return false;
+    const size_t L = m_Assets.size();
+    out->rts.assign(L, GsImage{});
+    out->cameraTargets.assign(L, GsImage{});
+    for (size_t i = 0; i < L; ++i) {
+      if (rts && rts[i]) out->rts[i] = *rts[i];
+      if (cameraTargets && cameraTargets[i]) out->cameraTargets[i] = *cameraTargets[i];
+    }
+    GsUnityGroupFrameObjectsEvent &ev = out->event;
+    std::memset(&ev, 0, sizeof(ev));
+    ev.group = m_Group;
+    ev.object_count = (uint32_t)out->fps.size();
+    ev.assets = out->assets.data();
+    ev.fps = out->fps.data();
+    ev.do_sort = out->doSort.data();
+    ev.options = options;
+    ev.rts = rts ? out->rts.data() : nullptr;
+    ev.camera_targets = cameraTargets ? out->cameraTargets.data() : nullptr;
+    ev.status = GS_ERR_NOT_READY;
+    return true;
+  }
+  // The payload of GS_UNITY_EVENT_GROUP_SYNC (Sync on the render thread).
+  GsUnityGroupSyncEvent SyncEvent() const {
+    GsUnityGroupSyncEvent ev;
+    std::memset(&ev, 0, sizeof(ev));
+    ev.group = m_Group;
+    ev.status = GS_ERR_NOT_READY;
+    return ev;
+  }
+  bool Sync() { return ok(gs_group_sync(m_Group)); }
+  GsGroup *group() const { return m_Group; }
+  GsAsset *asset(size_t i) const { return m_Assets[i]; }
+
+ private:
+  // gs_group_frame_objects' per-object arguments: `objects` in GatherSplatsForCamera order (:73-105), frame counters advanced.
+  // False, with none moved, for a null object or one uploaded to another number of members.
+  bool GatherObjects(const CameraState &cam, std::vector<GaussianSplatGroupObject *> objects, std::vector<GsAsset *> &assets,
+                     std::vector<GsFrameParams> &fps, std::vector<int32_t> &doSort) const {
     auto depth = [&](const GaussianSplatGroupObject *o) {   // camera-space z of the object's position, +z forward
       const float *v = cam.worldToCameraMatrix.m, *p = o->localToWorldMatrix.m + 12;
       return -(v[2] * p[0] + v[6] * p[1] + v[10] * p[2] + v[14]);
     };
-    if (objects.empty()) return true;   // no active splat object: OnPreCullCamera draws nothing
     const size_t L = m_Assets.size();
     for (const GaussianSplatGroupObject *o : objects)   // checked before any object's frame counter moves
       if (!o || o->m_Assets.size() != L) return false;
@@ -379,21 +498,14 @@ class GaussianSplatRendererGroup : public GaussianSplatGroupObject {
       if (a->m_RenderOrder != b->m_RenderOrder) return a->m_RenderOrder > b->m_RenderOrder;
       return depth(a) < depth(b);
     });
-    std::vector<GsAsset *> assets;
-    std::vector<GsFrameParams> fps;
-    std::vector<int32_t> doSort;
+    assets.clear(); fps.clear(); doSort.clear();
     for (GaussianSplatGroupObject *o : objects) {
       assets.insert(assets.end(), o->m_Assets.begin(), o->m_Assets.end());
       fps.push_back(o->params(cam));
       doSort.push_back(o->nextDoSort());
     }
-    return ok(gs_group_frame_objects(m_Group, (uint32_t)objects.size(), assets.data(), fps.data(), doSort.data(), &options, rts, cameraTargets));
+    return true;
   }
-  bool Sync() { return ok(gs_group_sync(m_Group)); }
-  GsGroup *group() const { return m_Group; }
-  GsAsset *asset(size_t i) const { return m_Assets[i]; }
-
- private:
   bool ok(int rc) const {
     if (rc == GS_OK) return true;
     std::fprintf(stderr, "GaussianSplatRendererGroup: %s (%d)\n", gs_last_error(m_Group ? gs_group_context(m_Group, 0) : nullptr), rc);

@@ -194,12 +194,14 @@ class GaussianSplatGroup:
         ptrs = self._images(rts, cam, ims)
         N.check(self.contexts[0].handle, self._lib.gs_group_frame(self.handle, self._assets, C.byref(fp), C.byref(opt), do_sort, ptrs))
 
-    def SortAndRenderSplatsMulti(self, objects, cam, rts=None, camera_targets=None):
+    def SortAndRenderSplatsMulti(self, objects, cam, rts=None, camera_targets=None, via_event=False):
         """One camera's frame with several splat objects (the group itself and / or add_object's objects): ordered by
         GatherSplatsForCamera, the first drawn into a cleared target and each later one under it, one row exchange, then the
         composite onto every given camera target (gs_group_frame_objects).  rts / camera_targets: one image per LOCAL member
         or None, as in SortAndRenderSplats.  Returns the objects in the order they were drawn.  With no objects nothing is
-        drawn or composited, as OnPreCullCamera returns early when the camera has no active splat object."""
+        drawn or composited, as OnPreCullCamera returns early when the camera has no active splat object.
+        via_event: the call goes through the render-thread event GS_UNITY_EVENT_GROUP_FRAME_OBJECTS, run on this thread (what
+        the tests compare the two with)."""
         from .renderer import GatherSplatsForCamera
         objects = list(objects)
         for k, o in enumerate(objects):   # checked before any object's frame counter moves
@@ -226,7 +228,14 @@ class GaussianSplatGroup:
         ptrs, cptrs = self._images(rts, cam, ims), self._images(camera_targets, cam, ims)
         for o in active:   # the uniforms and images were accepted: now the frame counts (:120-121)
             o.m_FrameCounter += 1
-        N.check(self.contexts[0].handle, self._lib.gs_group_frame_objects(self.handle, K, assets, fps, do_sort, C.byref(opt), ptrs, cptrs))
+        if via_event:
+            a, b = (N.image_array([p.contents if p else None for p in pp]) for pp in (ptrs, cptrs))
+            ev = N.GsUnityGroupFrameObjectsEvent(group=self.handle.value, object_count=K, assets=C.addressof(assets), fps=C.addressof(fps),
+                                                 do_sort=C.addressof(do_sort), options=opt, rts=C.addressof(a), camera_targets=C.addressof(b),
+                                                 status=N.GS_ERR_NOT_READY)
+            N.check(self.contexts[0].handle, N.unity_event(N.GS_UNITY_EVENT_GROUP_FRAME_OBJECTS, ev))
+        else:
+            N.check(self.contexts[0].handle, self._lib.gs_group_frame_objects(self.handle, K, assets, fps, do_sort, C.byref(opt), ptrs, cptrs))
         return active
 
     def _group(self):
@@ -251,8 +260,13 @@ class GaussianSplatGroup:
                     ptrs[i] = C.pointer(im)
         return ptrs
 
-    def sync(self):
-        N.check(self.contexts[0].handle, self._lib.gs_group_sync(self.handle))
+    def sync(self, via_event=False):
+        """gs_group_sync; via_event: through the render-thread event GS_UNITY_EVENT_GROUP_SYNC, run on this thread."""
+        if via_event:
+            ev = N.GsUnityGroupSyncEvent(group=self.handle.value, status=N.GS_ERR_NOT_READY)
+            N.check(self.contexts[0].handle, N.unity_event(N.GS_UNITY_EVENT_GROUP_SYNC, ev))
+        else:
+            N.check(self.contexts[0].handle, self._lib.gs_group_sync(self.handle))
 
     def row_costs(self, rows: int):
         """gs_group_row_costs: the per-row costs the last call measured, summed over its objects (what the row split two calls

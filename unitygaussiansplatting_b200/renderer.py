@@ -12,6 +12,7 @@ the hot path; everything it does is a call into libgsplat_b200.so (there is no C
   SortAndRenderSplats(cam, cmb)       (:108)   SortAndRenderSplats(cam, ...) -> gs_frame
   (several objects of one camera)              SortAndRenderSplatsMulti(...) -> gs_frame_objects
   camera loop, OnPreCullCamera        (:187)   SortAndRenderCameras(...)     -> gs_frame_cameras
+                                               (via_event=True: GS_UNITY_EVENT_FRAME_CAMERAS, the render-thread event)
   OnDisable / DisposeResourcesForAsset(:533)   Dispose()
 """
 from __future__ import annotations
@@ -574,19 +575,24 @@ def cameras_in_one_call(actives) -> bool:
                for a in actives)
 
 
-def SortAndRenderCameras(renderers, cams, rts, camera_targets=None):
+def SortAndRenderCameras(renderers, cams, rts, camera_targets=None, via_event=False):
     """The camera loop of GaussianSplatRenderSystem (R/GaussianSplatRenderer.cs:187-211): SortAndRenderSplatsMulti for each
     camera in turn -- GatherSplatsForCamera per camera, each renderer's m_FrameCounter advanced once per camera that draws it
     -- in one gs_frame_cameras call when cameras_in_one_call holds for the cameras that draw something, else camera by camera.
-    rts[c] / camera_targets[c] may be None (not both for a camera that draws).  Returns each camera's active renderers."""
+    rts[c] / camera_targets[c] may be None (not both for a camera that draws).  Returns each camera's active renderers.
+    via_event: the one call goes through the render-thread event GS_UNITY_EVENT_FRAME_CAMERAS, run on this thread, instead of
+    gs_frame_cameras (what the tests compare the two with); the cameras must then pass cameras_in_one_call."""
     camera_targets = camera_targets if camera_targets is not None else [None] * len(cams)
     actives = [GatherSplatsForCamera(renderers, cam) for cam in cams]
     drawn = [c for c, a in enumerate(actives) if a]
     if not drawn:
         return actives
-    if cameras_in_one_call([actives[c] for c in drawn]):
-        _frame_cameras([actives[c] for c in drawn], [cams[c] for c in drawn], [rts[c] for c in drawn],
-                       [camera_targets[c] for c in drawn])
+    one_call = cameras_in_one_call([actives[c] for c in drawn])
+    if via_event and not one_call:
+        raise ValueError("the render-thread event draws the cameras in one call: they must pass cameras_in_one_call")
+    if one_call:
+        (_frame_cameras_event if via_event else _frame_cameras)([actives[c] for c in drawn], [cams[c] for c in drawn],
+                                                                [rts[c] for c in drawn], [camera_targets[c] for c in drawn])
         return actives
     for c in drawn:
         SortAndRenderSplatsMulti(renderers, cams[c], rts[c], camera_targets[c])
@@ -594,6 +600,28 @@ def SortAndRenderCameras(renderers, cams, rts, camera_targets=None):
 
 
 def _frame_cameras(actives, cams, rts, camera_targets):
+    ctx, counts, assets, fps, do_sort, opt, images, keep = _camera_call(actives, cams, rts, camera_targets)
+    a = (C.POINTER(N.GsImage) * len(cams))(*[C.pointer(x) if x is not None else C.POINTER(N.GsImage)() for x, _ in images])
+    b = (C.POINTER(N.GsImage) * len(cams))(*[C.pointer(y) if y is not None else C.POINTER(N.GsImage)() for _, y in images])
+    N.check(ctx.handle, ctx._lib.gs_frame_cameras(ctx.handle, len(cams), counts, assets, fps, do_sort, C.byref(opt), a, b))
+    del keep
+
+
+def _frame_cameras_event(actives, cams, rts, camera_targets):
+    """_frame_cameras through the payload a CommandBuffer would carry (GsUnityFrameCamerasEvent, images by value)."""
+    ctx, counts, assets, fps, do_sort, opt, images, keep = _camera_call(actives, cams, rts, camera_targets)
+    a, b = N.image_array([x for x, _ in images]), N.image_array([y for _, y in images])
+    ev = N.GsUnityFrameCamerasEvent(ctx=ctx.handle.value, camera_count=len(cams), object_counts=C.addressof(counts),
+                                    assets=C.addressof(assets), fps=C.addressof(fps), do_sort=C.addressof(do_sort), options=opt,
+                                    rts=C.addressof(a), camera_targets=C.addressof(b), status=N.GS_ERR_NOT_READY)
+    N.check(ctx.handle, N.unity_event(N.GS_UNITY_EVENT_FRAME_CAMERAS, ev))
+    del keep
+
+
+def _camera_call(actives, cams, rts, camera_targets):
+    """gs_frame_cameras' arguments for the cameras' active renderers: (context, object counts, assets, frame parameters,
+    do_sort, options, [(rt image, camera target image)], keep), keep holding what they point to.  Each renderer's frame counter
+    advances once per camera."""
     n = sum(len(a) for a in actives)
     fps = (N.GsFrameParams * n)()
     assets = (C.c_void_p * n)()
@@ -614,11 +642,7 @@ def _frame_cameras(actives, cams, rts, camera_targets):
     opt.flags &= ~N.GS_FLAG_LOAD_RT
     images = [(_image(rt, cam.pixelWidth, cam.pixelHeight) if rt is not None else None,
                _image(tg, cam.pixelWidth, cam.pixelHeight) if tg is not None else None) for cam, rt, tg in zip(cams, rts, camera_targets)]
-    a = (C.POINTER(N.GsImage) * len(cams))(*[C.pointer(x) if x is not None else C.POINTER(N.GsImage)() for x, _ in images])
-    b = (C.POINTER(N.GsImage) * len(cams))(*[C.pointer(y) if y is not None else C.POINTER(N.GsImage)() for _, y in images])
-    ctx = actives[0][0].context
-    N.check(ctx.handle, ctx._lib.gs_frame_cameras(ctx.handle, len(cams), counts, assets, fps, do_sort, C.byref(opt), a, b))
-    del keep
+    return actives[0][0].context, counts, assets, fps, do_sort, opt, images, keep
 
 
 def _frame_objects(active, cam: Camera, rt, camera_target):
