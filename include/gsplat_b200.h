@@ -145,11 +145,33 @@ typedef struct GsFrameParams {
  *           rounds to nearest, ties to even, over the whole value set including denormals, and overflows to +Inf as IEEE
  *           rounding does: float11 x >= 65280 (largest finite 65024), float10 x >= 65024 (largest finite 64512).
  * This follows the format definitions of the Vulkan and D3D11 specifications, and rounds as the RGBA16F path's
- * float -> half conversion does; whether a given GPU's blend unit rounds this format the same way is not known here. */
+ * float -> half conversion does; whether a given GPU's blend unit rounds this format the same way is not known here.
+ *
+ * GS_PIX_R8G8B8A8_SRGB: four bytes per pixel in memory order R, G, B, A; R, G and B sRGB-encoded, A linear UNorm -- Unity's
+ * R8G8B8A8_SRGB, VK_FORMAT_R8G8B8A8_SRGB, DXGI_FORMAT_R8G8B8A8_UNORM_SRGB: the colour buffer of an LDR camera (HDR off) in a
+ * linear-colour-space project, and the render texture the reference's GaussianSplatValidator renders into.  Like
+ * GS_PIX_B10G11R11_UFLOAT it is accepted as a CAMERA TARGET only, in every memory kind, by the same entry points (and so by the
+ * camera targets of every GsUnity*Event), and refused with GS_ERR_UNSUPPORTED_FORMAT, before anything is enqueued, wherever
+ * GS_PIX_B10G11R11_UFLOAT is.  A CUDA array holding it has FOUR 8-bit cudaChannelFormatKindUnsigned channels
+ * (cudaCreateChannelDesc<uchar4>()); any other channel format is GS_ERR_UNSUPPORTED_FORMAT.  A pitched linear image follows the
+ * pitch rules with a 4-byte texel.
+ * The composite onto it decodes the texel, blends r, g, b and a exactly as onto an RGBA32F target (alpha included:
+ * o.a = fma(a, a, d.a * (1 - a))) and encodes; a pixel whose source alpha is not > 0 keeps its bytes.  The codec is exact:
+ *   decode  RGB: code c -> the float32 nearest the IEC 61966-2-1 EOTF at v = c / 255, the exact value of v / 12.92 for
+ *           v <= 0.04045, else ((v + 0.055) / 1.055)^2.4 (a 256-entry table);  A: code a -> the float32 nearest a / 255;
+ *   encode  RGB: NaN and x <= 0 (-0 and -Inf included) -> 0; x >= 1 (+Inf included) -> 255; any other x -> the number of j in
+ *           1..255 with 255 OETF(x) >= j - 0.5, evaluated exactly, where OETF(x) = 12.92 x for x <= 0.0031308, else
+ *           1.055 x^(1/2.4) - 0.055: round to nearest in the encoded domain.  Equivalently x is compared with 255 float32
+ *           thresholds T_j, the smallest float32 with 255 OETF(T_j) >= j - 0.5.  The OETF falls by 2.9e-8 at its junction, but
+ *           no decision boundary lies in that step, so the code is monotone in x;
+ *           A: NaN -> 0; else clamp to [0, 1] and round 255 x to nearest (the only representable tie, x = 0.5, gives 128).
+ * Whether a given GPU's blend unit rounds this format the same way is not known here: D3D and Vulkan allow some tolerance in
+ * the sRGB conversion. */
 typedef enum GsPixelFormat {
   GS_PIX_RGBA16F = 0,   /* _GaussianSplatRT: R16G16B16A16_SFloat (R/GaussianSplatRenderer.cs:194) */
   GS_PIX_RGBA32F = 1,
-  GS_PIX_B10G11R11_UFLOAT = 2   /* camera targets only (above) */
+  GS_PIX_B10G11R11_UFLOAT = 2,   /* camera targets only (above) */
+  GS_PIX_R8G8B8A8_SRGB = 3       /* camera targets only (above) */
 } GsPixelFormat;
 
 /* GS_MEM_ARRAY (images only, not GsPackDesc / GsPackedAsset): `data` is a cudaArray_t -- a 2-D CUDA array (mip level 0) on the
@@ -159,7 +181,8 @@ typedef enum GsPixelFormat {
  *   - the array must have been created with cudaArraySurfaceLoadStore (for an imported image: ask for that flag in
  *     cudaExternalMemoryMipmappedArrayDesc.flags);
  *   - its channel format must be the image's: 4 x 16-bit float for GS_PIX_RGBA16F, 4 x 32-bit float for GS_PIX_RGBA32F,
- *     1 x 32-bit unsigned for GS_PIX_B10G11R11_UFLOAT (else GS_ERR_UNSUPPORTED_FORMAT);
+ *     1 x 32-bit unsigned for GS_PIX_B10G11R11_UFLOAT, 4 x 8-bit unsigned for GS_PIX_R8G8B8A8_SRGB
+ *     (else GS_ERR_UNSUPPORTED_FORMAT);
  *   - its extent must be width x height with depth 0, and row_pitch_bytes must be 0 (else GS_ERR_INVALID_ARGUMENT).
  * The import itself and the graphics API's semaphores stay with the host: wait / signal them on gs_context_stream(ctx).
  * Not accepted (GS_ERR_INVALID_ARGUMENT): band_packed output and gs_unshuffle_bands output.  GS_FLAG_ASYNC_READBACK has no

@@ -274,9 +274,12 @@ namespace GaussianSplatting.Runtime
     /// The camera's colour buffer as a camera target (GsImage) of an event, e.g. GsUnityFrameEvent.camera_target with
     /// has_camera_target = 1: URP's HDR camera colour (m_HDRColorBufferPrecision 32-bit, no alpha) and HDRP's
     /// ctx.cameraColorBuffer (colorBufferFormat R11G11B10) are GraphicsFormat.B10G11R11_UFloatPack32, which the library
-    /// composites onto in place as GS_PIX_B10G11R11_UFLOAT (2); the built-in pipeline's ARGBHalf is GS_PIX_RGBA16F (0).
+    /// composites onto in place as GS_PIX_B10G11R11_UFLOAT (2); the built-in pipeline's ARGBHalf is GS_PIX_RGBA16F (0).  An
+    /// LDR camera (HDR off) in a linear-colour-space project, and the validator's RenderTexture, draw into
+    /// GraphicsFormat.R8G8B8A8_SRGB, which is GS_PIX_R8G8B8A8_SRGB (3).
     /// `colorArray` is the buffer imported as a CUDA array: for B10G11R11 with ONE 32-bit unsigned channel
-    /// (cudaCreateChannelDesc<unsigned int>(), INTEGRATION.md section 3).  Not compiled here, like the rest of this file.
+    /// (cudaCreateChannelDesc<unsigned int>()), for R8G8B8A8_SRGB with FOUR 8-bit unsigned channels
+    /// (cudaCreateChannelDesc<uchar4>(); INTEGRATION.md section 3).  Not compiled here, like the rest of this file.
     internal static class GaussianSplatCameraTarget
     {
         public static uint PixelFormat(UnityEngine.Experimental.Rendering.GraphicsFormat f)
@@ -286,6 +289,7 @@ namespace GaussianSplatting.Runtime
                 case UnityEngine.Experimental.Rendering.GraphicsFormat.R16G16B16A16_SFloat: return 0;   // GS_PIX_RGBA16F
                 case UnityEngine.Experimental.Rendering.GraphicsFormat.R32G32B32A32_SFloat: return 1;   // GS_PIX_RGBA32F
                 case UnityEngine.Experimental.Rendering.GraphicsFormat.B10G11R11_UFloatPack32: return 2; // GS_PIX_B10G11R11_UFLOAT
+                case UnityEngine.Experimental.Rendering.GraphicsFormat.R8G8B8A8_SRGB: return 3;          // GS_PIX_R8G8B8A8_SRGB
                 default: throw new NotSupportedException("camera colour format " + f + " is not a supported camera target");
             }
         }

@@ -5,10 +5,11 @@ from .asset import (ColorFormat, GaussianSplatAsset, SHFormat, VectorFormat, QUA
                     SCENE_UNIFORM, create_asset, generate_input_splats, load_asset, read_ply, read_spz, save_asset, synthetic_asset, write_ply)
 from .camera import Camera, look_rotation, trs, quat_to_mat
 from .renderer import (CudaArrayDepth, CudaArrayImage, GaussianSplatContext, GaussianSplatRenderer, GatherSplatsForCamera, SortAndRenderCameras,
-                       SortAndRenderSplatsMulti, make_frame_params, pack_b10g11r11, unpack_b10g11r11)
+                       SortAndRenderSplatsMulti, make_frame_params, pack_b10g11r11, unpack_b10g11r11,
+                       encode_srgb8, decode_srgb8)
 from .pack import pack_asset
 from ._native import GsError
 
 __all__ = ["ColorFormat", "GaussianSplatAsset", "SHFormat", "VectorFormat", "QUALITY", "SCENE_CLUSTERED", "SCENE_LATTICE",
            "SCENE_UNIFORM", "create_asset", "generate_input_splats", "read_ply", "read_spz", "write_ply", "save_asset", "load_asset", "synthetic_asset", "Camera", "look_rotation", "trs",
-           "quat_to_mat", "CudaArrayDepth", "CudaArrayImage", "GaussianSplatContext", "GaussianSplatRenderer", "GatherSplatsForCamera", "SortAndRenderCameras", "SortAndRenderSplatsMulti", "make_frame_params", "pack_b10g11r11", "unpack_b10g11r11", "pack_asset", "GsError"]
+           "quat_to_mat", "CudaArrayDepth", "CudaArrayImage", "GaussianSplatContext", "GaussianSplatRenderer", "GatherSplatsForCamera", "SortAndRenderCameras", "SortAndRenderSplatsMulti", "make_frame_params", "pack_b10g11r11", "unpack_b10g11r11", "encode_srgb8", "decode_srgb8", "pack_asset", "GsError"]

@@ -16,6 +16,7 @@ GS_OK = 0
 GS_ERR_NO_DEVICE = -6
 GS_PIX_RGBA16F, GS_PIX_RGBA32F = 0, 1
 GS_PIX_B10G11R11_UFLOAT = 2   # camera targets only: one uint32 texel per pixel, no alpha
+GS_PIX_R8G8B8A8_SRGB = 3      # camera targets only: four bytes per pixel, RGB sRGB-encoded, alpha linear
 GS_MEM_HOST, GS_MEM_DEVICE, GS_MEM_ARRAY = 0, 1, 2
 GS_MEM_ARRAY_LAYER = 4
 GS_MEM_ARRAY_RECT = 5

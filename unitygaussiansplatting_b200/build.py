@@ -24,7 +24,7 @@ NATIVE_LIB = PKG / "libgsplat_b200.so"
 ASSET_LIB = PKG / "libgsplat_asset.so"
 
 CU_SOURCES = ["gs_api.cu", "gs_group.cu", "gs_image.cu", "gs_bins.cu", "gs_view.cu", "gs_sort.cu", "gs_raster.cu", "gs_export.cu", "gs_pack.cu"]
-CU_HEADERS = ["gs_buffer.cuh", "gs_common.cuh", "gs_kernels.cuh", "gs_internal.cuh", "gs_nccl.h", "gs_bc7.cuh", "gs_packed_float.cuh", "bc7_tables.h", "../../include/gsplat_b200.h"]
+CU_HEADERS = ["gs_buffer.cuh", "gs_common.cuh", "gs_kernels.cuh", "gs_internal.cuh", "gs_nccl.h", "gs_bc7.cuh", "gs_packed_float.cuh", "gs_srgb8.cuh", "gs_srgb8_tables.h", "bc7_tables.h", "../../include/gsplat_b200.h"]
 
 
 def _host_cxx() -> str:

@@ -8,7 +8,9 @@
 
 namespace gs {
 
-uint32_t pix_bytes(uint32_t fmt) { return fmt == GS_PIX_RGBA16F ? 8u : fmt == GS_PIX_B10G11R11_UFLOAT ? 4u : 16u; }
+uint32_t pix_bytes(uint32_t fmt) {
+  return fmt == GS_PIX_RGBA16F ? 8u : (fmt == GS_PIX_B10G11R11_UFLOAT || fmt == GS_PIX_R8G8B8A8_SRGB) ? 4u : 16u;
+}
 
 // The rules every CUDA array the library reads or writes keeps: `a` (a GS_MEM_ARRAY, GS_MEM_ARRAY_LAYER or GS_MEM_ARRAY_RECT view:
 // data and memory) is a W x H 2-D array, a layer below the layer count of a W x H layered one, or a W x H rectangle inside a
@@ -69,10 +71,12 @@ bool array_layered(cudaArray_t arr) {
 
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, ImageRole role, uint32_t *pitch) {
   if (!im || !im->data) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image is null");
-  const bool packed = im->format == GS_PIX_B10G11R11_UFLOAT;
-  if (im->format > GS_PIX_B10G11R11_UFLOAT) return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "unsupported pixel format");
+  const bool packed = im->format == GS_PIX_B10G11R11_UFLOAT, srgb8 = im->format == GS_PIX_R8G8B8A8_SRGB;
+  if (im->format > GS_PIX_R8G8B8A8_SRGB) return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "unsupported pixel format");
   if (packed && role != ImageRole::kCameraTarget)
     return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "GS_PIX_B10G11R11_UFLOAT is a camera-target format, not a render-target one");
+  if (srgb8 && role != ImageRole::kCameraTarget)
+    return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "GS_PIX_R8G8B8A8_SRGB is a camera-target format, not a render-target one");
   if (im->memory > GS_MEM_ARRAY_RECT || im->memory == 3)   // 3 is not a memory kind
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "unknown image memory kind");
   if (im->width != W || im->height != H) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "image size does not match screen size");
@@ -80,8 +84,9 @@ int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, ImageRol
                               // rectangle of either (a GsArrayRect *)
     if (im->row_pitch_bytes) return fail(ctx, GS_ERR_INVALID_ARGUMENT, "row_pitch_bytes must be 0 for a CUDA array image");
     const int rc = packed ? array_ok(ctx, *im, W, H, cudaChannelFormatKindUnsigned, 1, 32, "", "the image's", "one 32-bit unsigned channel")
-                          : array_ok(ctx, *im, W, H, cudaChannelFormatKindFloat, 4, im->format == GS_PIX_RGBA16F ? 16 : 32, "",
-                                     "the image's", "the image's pixel format");
+                   : srgb8  ? array_ok(ctx, *im, W, H, cudaChannelFormatKindUnsigned, 4, 8, "", "the image's", "four 8-bit unsigned channels")
+                            : array_ok(ctx, *im, W, H, cudaChannelFormatKindFloat, 4, im->format == GS_PIX_RGBA16F ? 16 : 32, "",
+                                       "the image's", "the image's pixel format");
     if (rc) return rc;
     *pitch = 0;
     return GS_OK;

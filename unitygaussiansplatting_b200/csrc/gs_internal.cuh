@@ -179,7 +179,7 @@ int composite_device_rt(GsContext *ctx, const void *d_rt, uint32_t rt_pitch, uin
 
 // ---- images (gs_image.cu) -------------------------------------------------------------------------------------------------
 // What an image is to the call: a render target (also gs_composite's source, band_packed and gs_unshuffle_bands output), which
-// is RGBA16F or RGBA32F, or a camera target, which may also be GS_PIX_B10G11R11_UFLOAT.
+// is RGBA16F or RGBA32F, or a camera target, which may also be GS_PIX_B10G11R11_UFLOAT or GS_PIX_R8G8B8A8_SRGB.
 enum class ImageRole { kRenderTarget, kCameraTarget };
 int image_ok(GsContext *ctx, const GsImage *im, uint32_t W, uint32_t H, ImageRole role, uint32_t *pitch);
 uint32_t pix_bytes(uint32_t fmt);

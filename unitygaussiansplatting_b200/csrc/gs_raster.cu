@@ -26,6 +26,7 @@
 
 #include "gs_kernels.cuh"
 #include "gs_packed_float.cuh"
+#include "gs_srgb8.cuh"
 
 namespace gs {
 
@@ -816,7 +817,7 @@ void launch_unshuffle(const void *gathered, uint32_t parts, uint32_t band, uint3
 }
 
 // ---- 3. composite (S/GaussianComposite.shader:35-39, Blend SrcAlpha OneMinusSrcAlpha :11) ------
-// The camera target is RGBA16F, RGBA32F or B10G11R11_UFLOAT; the render target is never the packed format.
+// The camera target is RGBA16F, RGBA32F, B10G11R11_UFLOAT or R8G8B8A8_SRGB; the render target is never one of the last two.
 __device__ __forceinline__ float gamma_to_linear(float x) {  // UnityCG.cginc GammaToLinearSpace (not vendored)
   return x * fmaf(x, fmaf(x, 0.305306011f, 0.682171111f), 0.012522878f);
 }
@@ -836,7 +837,7 @@ __device__ __forceinline__ float4 load_px(const uint8_t *base, uint32_t pitch, c
 }
 
 // TGT_FMT: the camera target's pixel format, a template parameter so that the RGBA16F and RGBA32F instantiations carry no code
-// of the packed one (a uniform run-time branch cost the RGBA16F composite 3 % at 1920 x 1080 on an H100).
+// of the packed and sRGB ones (a uniform run-time branch cost the RGBA16F composite 3 % at 1920 x 1080 on an H100).
 template <uint32_t TGT_FMT>
 __global__ void __launch_bounds__(256) k_composite(const uint8_t *__restrict__ rt, uint32_t rt_pitch, Surface rt_surf,
                                                    uint32_t rt_fmt, uint8_t *__restrict__ tgt, uint32_t tgt_pitch,
@@ -851,6 +852,11 @@ __global__ void __launch_bounds__(256) k_composite(const uint8_t *__restrict__ r
     if (tgt) v = reinterpret_cast<const uint32_t *>(tgt + (size_t)y * tgt_pitch)[x];
     else surf_load<true>(&v, tgt_surf, x * 4u, y);
     unpack_b10g11r11(v, &d.x, &d.y, &d.z);
+  } else if constexpr (TGT_FMT == GS_PIX_R8G8B8A8_SRGB) {   // a camera target only: four bytes, RGB sRGB-encoded
+    uint32_t v;
+    if (tgt) v = reinterpret_cast<const uint32_t *>(tgt + (size_t)y * tgt_pitch)[x];
+    else surf_load<true>(&v, tgt_surf, x * 4u, y);
+    unpack_srgb8(v, &d.x, &d.y, &d.z, &d.w);
   } else {
     d = load_px(tgt, tgt_pitch, tgt_surf, TGT_FMT, x, y);
   }
@@ -862,6 +868,10 @@ __global__ void __launch_bounds__(256) k_composite(const uint8_t *__restrict__ r
   o.w = fmaf(a, a, d.w * om);
   if constexpr (TGT_FMT == GS_PIX_B10G11R11_UFLOAT) {
     const uint32_t v = pack_b10g11r11(o.x, o.y, o.z);
+    if (tgt) reinterpret_cast<uint32_t *>(tgt + (size_t)y * tgt_pitch)[x] = v;
+    else surf_store<true>(v, tgt_surf, x * 4u, y);
+  } else if constexpr (TGT_FMT == GS_PIX_R8G8B8A8_SRGB) {
+    const uint32_t v = pack_srgb8(o.x, o.y, o.z, o.w);
     if (tgt) reinterpret_cast<uint32_t *>(tgt + (size_t)y * tgt_pitch)[x] = v;
     else surf_store<true>(v, tgt_surf, x * 4u, y);
   } else if constexpr (TGT_FMT == GS_PIX_RGBA16F) {
@@ -884,6 +894,8 @@ void launch_composite(const void *rt, uint32_t rt_pitch, Surface rt_surf, uint32
   uint8_t *t = reinterpret_cast<uint8_t *>(target);
   if (tgt_format == GS_PIX_B10G11R11_UFLOAT)
     k_composite<GS_PIX_B10G11R11_UFLOAT><<<grid, 256, 0, s>>>(r, rt_pitch, rt_surf, rt_format, t, tgt_pitch, tgt_surf, W, H);
+  else if (tgt_format == GS_PIX_R8G8B8A8_SRGB)
+    k_composite<GS_PIX_R8G8B8A8_SRGB><<<grid, 256, 0, s>>>(r, rt_pitch, rt_surf, rt_format, t, tgt_pitch, tgt_surf, W, H);
   else if (tgt_format == GS_PIX_RGBA16F)
     k_composite<GS_PIX_RGBA16F><<<grid, 256, 0, s>>>(r, rt_pitch, rt_surf, rt_format, t, tgt_pitch, tgt_surf, W, H);
   else

@@ -72,6 +72,16 @@ inline GsImage PackedCameraTarget(void *data, uint32_t width, uint32_t height, u
   return im;
 }
 
+// A camera target of R8G8B8A8_SRGB texels (GS_PIX_R8G8B8A8_SRGB: the colour buffer of an LDR camera in a linear-colour-space
+// project, accepted as a camera target only) in host or device memory (`memory`): four bytes R, G, B, A per pixel, rows
+// `row_pitch_bytes` apart (0: tightly packed).  Such a colour buffer imported as a CUDA array (four 8-bit unsigned channels) is
+// ArrayImage / ArrayLayerImage / ArrayRectImage with format GS_PIX_R8G8B8A8_SRGB.
+inline GsImage Srgb8CameraTarget(void *data, uint32_t width, uint32_t height, uint32_t memory, uint32_t row_pitch_bytes = 0) {
+  GsImage im = PackedCameraTarget(data, width, height, memory, row_pitch_bytes);
+  im.format = GS_PIX_R8G8B8A8_SRGB;
+  return im;
+}
+
 // The payload of GS_UNITY_EVENT_FRAME_CAMERAS (GaussianSplatRenderer::FillFrameCamerasEvent) and the arrays it points to.
 // `event` points into this object: keep it alive and unmoved until the event has run, and with it the renderers (their
 // cutouts), the host images and the GsArrayLayer / GsArrayRect descriptors the images point to.

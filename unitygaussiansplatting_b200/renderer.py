@@ -113,8 +113,10 @@ def _index32(what, name, v):
 class CudaArrayImage:
     """A 2-D CUDA array (cudaArray_t, e.g. an imported graphics render texture) of RGBA float16 or float32 texels, given to the
     library as an image (GS_MEM_ARRAY): it is rendered into / composited onto in place.  dtype uint32: an array of one 32-bit
-    unsigned channel holding GS_PIX_B10G11R11_UFLOAT texels (a URP / HDRP camera colour buffer), a camera target only.  The host creates the array, with
-    cudaArraySurfaceLoadStore, and keeps it alive; the library never allocates or frees one.
+    unsigned channel holding GS_PIX_B10G11R11_UFLOAT texels (a URP / HDRP camera colour buffer), a camera target only.  dtype
+    uint8: an array of four 8-bit unsigned channels holding GS_PIX_R8G8B8A8_SRGB texels (an LDR camera's colour buffer), a
+    camera target only.  The host creates the array, with cudaArraySurfaceLoadStore, and keeps it alive; the library never
+    allocates or frees one.
 
     layer: the array is a layered one (cudaArrayLayered, e.g. an XR eye-texture array or a cube map) and the image is this
     layer of it (GS_MEM_ARRAY_LAYER); the other layers are left as they are.
@@ -126,8 +128,8 @@ class CudaArrayImage:
         self.handle = int(handle)
         self.width, self.height = int(width), int(height)
         self.dtype = np.dtype(dtype)
-        if self.dtype not in (np.float16, np.float32, np.uint32):
-            raise ValueError("CudaArrayImage dtype must be float16, float32 or uint32")
+        if self.dtype not in (np.float16, np.float32, np.uint32, np.uint8):
+            raise ValueError("CudaArrayImage dtype must be float16, float32, uint32 or uint8")
         # the descriptor a GS_MEM_ARRAY_LAYER / GS_MEM_ARRAY_RECT image points to, alive as long as this object
         self._layer_desc, self.memory = _array_descriptor("CudaArrayImage", self.handle, layer, origin)
         self.layer = None if layer is None else int(layer)
@@ -162,14 +164,15 @@ class CudaArrayDepth:
 
 
 def _image(arr, width: int, height: int) -> N.GsImage:
-    """numpy (host) array or torch CUDA tensor of shape (H, W, 4), float16/float32, or (H, W) uint32 (int32 for a tensor) of
-    packed GS_PIX_B10G11R11_UFLOAT texels, or a CudaArrayImage -> GsImage."""
+    """numpy (host) array or torch CUDA tensor of shape (H, W, 4), float16/float32 or uint8 (GS_PIX_R8G8B8A8_SRGB texels), or
+    (H, W) uint32 (int32 for a tensor) of packed GS_PIX_B10G11R11_UFLOAT texels, or a CudaArrayImage -> GsImage."""
     im = N.GsImage()
     im.width, im.height = width, height
     if isinstance(arr, CudaArrayImage):
         if arr.shape[:2] != (height, width):
             raise ValueError("CUDA array is %dx%d, the image must be %dx%d" % (arr.width, arr.height, width, height))
-        im.format = {np.float16: N.GS_PIX_RGBA16F, np.float32: N.GS_PIX_RGBA32F, np.uint32: N.GS_PIX_B10G11R11_UFLOAT}[arr.dtype.type]
+        im.format = {np.float16: N.GS_PIX_RGBA16F, np.float32: N.GS_PIX_RGBA32F, np.uint32: N.GS_PIX_B10G11R11_UFLOAT,
+                     np.uint8: N.GS_PIX_R8G8B8A8_SRGB}[arr.dtype.type]
         if arr._layer_desc is None:
             im.data, im.memory = arr.handle, N.GS_MEM_ARRAY
         else:
@@ -189,8 +192,10 @@ def _image(arr, width: int, height: int) -> N.GsImage:
                 im.format = N.GS_PIX_RGBA16F
             elif arr.dtype == np.float32:
                 im.format = N.GS_PIX_RGBA32F
+            elif arr.dtype == np.uint8:
+                im.format = N.GS_PIX_R8G8B8A8_SRGB
             else:
-                raise ValueError("image dtype must be float16, float32 or (packed) uint32")
+                raise ValueError("image dtype must be float16, float32, uint8 (sRGB) or (packed) uint32")
         im.data, im.memory = arr.ctypes.data, N.GS_MEM_HOST
         im.row_pitch_bytes = arr.strides[0]
         return im
@@ -206,7 +211,7 @@ def _image(arr, width: int, height: int) -> N.GsImage:
     if tuple(arr.shape) != (height, width, 4) or not arr.is_contiguous():
         raise ValueError("image must be contiguous (H, W, 4)")
     es = arr.element_size()
-    im.format = N.GS_PIX_RGBA16F if es == 2 else N.GS_PIX_RGBA32F
+    im.format = N.GS_PIX_R8G8B8A8_SRGB if str(arr.dtype) == "torch.uint8" else N.GS_PIX_RGBA16F if es == 2 else N.GS_PIX_RGBA32F
     im.data = arr.data_ptr()
     im.memory = N.GS_MEM_DEVICE if arr.is_cuda else N.GS_MEM_HOST
     im.row_pitch_bytes = width * 4 * es
@@ -253,6 +258,38 @@ def unpack_b10g11r11(texels) -> np.ndarray:
     """(...) uint32 GS_PIX_B10G11R11_UFLOAT texels -> (..., 3) float32, exactly."""
     t = np.asarray(texels, np.uint32)
     return np.stack([_from_ufloat(t & 0x7FF, 6), _from_ufloat((t >> 11) & 0x7FF, 6), _from_ufloat(t >> 22, 5)], axis=-1)
+
+
+def _srgb_oetf(x: np.ndarray) -> np.ndarray:
+    with np.errstate(invalid="ignore"):
+        return np.where(x <= 0.0031308, 12.92 * x, 1.055 * np.power(np.maximum(x, 0.0), 1.0 / 2.4) - 0.055)
+
+
+def encode_srgb8(linear_rgba) -> np.ndarray:
+    """(..., 4) float32 linear RGBA -> (..., 4) uint8 GS_PIX_R8G8B8A8_SRGB texels, rounded as the library's composite rounds
+    them (include/gsplat_b200.h): RGB sRGB-encoded to the nearest code in the encoded domain, NaN and x <= 0 to 0, x >= 1 to 255;
+    alpha clamped to [0, 1] and 255 a rounded to nearest, NaN to 0.  Evaluated in float64, whose error lies far below the
+    distance of any float32 from a decision boundary."""
+    with np.errstate(invalid="ignore"):   # signalling NaNs among arbitrary bit patterns
+        x = np.asarray(linear_rgba, np.float32).astype(np.float64)
+    bad = ~(x > 0)   # NaN and x <= 0
+    xc = np.where(bad, 0.0, np.minimum(x, 1.0))
+    rgb = np.floor(255.0 * _srgb_oetf(xc[..., :3]) + 0.5)
+    a = np.floor(255.0 * xc[..., 3:] + 0.5)   # exact: a float32 times 255 fits in float64
+    out = np.clip(np.concatenate([rgb, a], -1), 0, 255)
+    out = np.where(bad, 0, np.where(x >= 1.0, 255, out))
+    return out.astype(np.uint8)
+
+
+_V8 = np.arange(256, dtype=np.float64) / 255.0
+_SRGB8_DECODE = np.where(_V8 <= 0.04045, _V8 / 12.92, ((_V8 + 0.055) / 1.055) ** 2.4).astype(np.float32)
+
+
+def decode_srgb8(texels) -> np.ndarray:
+    """(..., 4) uint8 GS_PIX_R8G8B8A8_SRGB texels -> (..., 4) float32 linear RGBA: RGB through the float32 nearest the sRGB EOTF
+    at c / 255, alpha the float32 nearest a / 255."""
+    t = np.asarray(texels, np.uint8)
+    return np.concatenate([_SRGB8_DECODE[t[..., :3]], (t[..., 3:].astype(np.float32) / np.float32(255.0)).astype(np.float32)], -1)
 
 
 _EYE4 = np.eye(4, dtype=np.float32)
