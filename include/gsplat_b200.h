@@ -301,7 +301,18 @@ GS_API const char *gs_version(void);
 /* CreateResourcesForAsset + InitSortBuffers + CSSetIndices,
  * R/GaussianSplatRenderer.cs:373-445, S/SplatUtilities.compute:59-67 */
 GS_API int gs_asset_upload(GsContext *ctx, const GsAssetDesc *desc, GsAsset **out);
-/* DisposeResourcesForAsset / OnDisable, R/GaussianSplatRenderer.cs:533-577 */
+/* A further renderer of an uploaded asset: CreateResourcesForAsset (R/GaussianSplatRenderer.cs:373-445) for a
+ * GaussianSplatRenderer whose m_Asset another renderer already has on this context.  *out behaves in every call exactly like an
+ * asset gs_asset_upload made on source's context from the same GsAssetDesc, and starts as a fresh upload does: draw order
+ * reset (CSSetIndices), no view data.  It shares source's five blobs in HBM (nothing is copied or allocated for them) and owns
+ * its own per-renderer state: draw order, keys, view data, bin rectangles, draw records, quad depths and group buffers.
+ * source may itself be an instance; the blobs are freed when the last asset holding them is destroyed, in any order.  A source
+ * and its instances are distinct assets: one call may list several of them, and an instance of a group member's asset is that
+ * member's asset in gs_group_frame / gs_group_frame_objects.  GS_ERR_INVALID_ARGUMENT for a NULL source or out;
+ * GS_ERR_OUT_OF_MEMORY with *out NULL when the per-renderer buffers cannot be allocated.  Blocks. */
+GS_API int gs_asset_instance(const GsAsset *source, GsAsset **out);
+/* DisposeResourcesForAsset / OnDisable, R/GaussianSplatRenderer.cs:533-577.  An asset shared with instances keeps its blobs
+ * alive for them. */
 GS_API void gs_asset_destroy(GsAsset *asset);
 /* CSSetIndices: order[i] = i (S/SplatUtilities.compute:59-67) */
 GS_API int gs_asset_reset_order(GsAsset *asset);
@@ -711,7 +722,9 @@ GS_API uint32_t gs_unity_group_sync_event_size(void);   /* sizeof(GsUnityGroupSy
 
 /* ---- device-pointer access for zero-copy hosts (torch / CUDA-Vulkan interop) ----- */
 GS_API void *gs_context_stream(GsContext *ctx);
-GS_API void *gs_asset_device_ptr(GsAsset *asset, int which); /* 0 order, 1 keys, 2 view */
+/* 0 order, 1 keys, 2 view (the asset's own); 3 pos, 4 other, 5 sh, 6 color, 7 chunks (NULL when the asset has none): the
+ * blobs, the same pointers for an asset and its instances (gs_asset_instance).  Any other `which`: NULL. */
+GS_API void *gs_asset_device_ptr(GsAsset *asset, int which);
 
 #ifdef __cplusplus
 }

@@ -164,6 +164,7 @@ NATIVE_SYMBOLS = {
     "gs_get_stage_times": (C.c_int, [C.c_void_p, C.POINTER(GsStageTimes)]),
     "gs_version": (C.c_char_p, []),
     "gs_asset_upload": (C.c_int, [C.c_void_p, C.POINTER(GsAssetDesc), C.POINTER(C.c_void_p)]),
+    "gs_asset_instance": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "gs_asset_destroy": (None, [C.c_void_p]),
     "gs_asset_reset_order": (C.c_int, [C.c_void_p]),
     "gs_asset_splat_count": (C.c_uint32, [C.c_void_p]),

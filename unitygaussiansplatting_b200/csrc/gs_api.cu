@@ -323,8 +323,9 @@ cudaError_t asset_init_work(GsContext *ctx, GsAsset *as, uint32_t n, uint32_t po
   as->av.n = n;
   as->av.posFmt = pos_fmt; as->av.scaleFmt = scale_fmt; as->av.shFmt = sh_fmt; as->av.colFmt = col_fmt;
   as->av.chunkCount = chunk_count;
-  as->av.pos = as->d_pos.get(); as->av.other = as->d_other.get(); as->av.sh = as->d_sh.get();
-  as->av.color = as->d_color.get(); as->av.chunks = (const Chunk *)as->d_chunks.get();
+  const GsBlobs &b = *as->blobs;
+  as->av.pos = b.pos.get(); as->av.other = b.other.get(); as->av.sh = b.sh.get();
+  as->av.color = b.color.get(); as->av.chunks = (const Chunk *)b.chunks.get();
   launch_set_indices(as->order.get(), as->av.n, s);  // CSSetIndices
   ctx->launches += 1;
   // `n` is a stack value: the copy above must have left it before this returns
@@ -542,8 +543,13 @@ int gs_asset_upload(GsContext *ctx, const GsAssetDesc *d, GsAsset **out) {
   const uint32_t chunk_count = (d->chunks && d->chunk_bytes) ? (uint32_t)(d->chunk_bytes / 64) : 0;
   GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   GsAsset *as = new (std::nothrow) GsAsset();
-  if (!as) return fail(ctx, GS_ERR_OUT_OF_MEMORY, "host allocation failed");
+  if (as) as->blobs = new (std::nothrow) GsBlobs();
+  if (!as || !as->blobs) {
+    delete as;
+    return fail(ctx, GS_ERR_OUT_OF_MEMORY, "host allocation failed");
+  }
   as->ctx = ctx;
+  GsBlobs &b = *as->blobs;
   auto up = [&](gs::Buffer<uint8_t> &dst, const void *src, uint64_t bytes, uint64_t min_bytes = 0) -> cudaError_t {
     // +16 bytes of slack: the widest vector load of the last splat may read past a tightly sized blob
     const uint64_t alloc = (bytes > min_bytes ? bytes : min_bytes) + 16;
@@ -556,9 +562,9 @@ int gs_asset_upload(GsContext *ctx, const GsAssetDesc *d, GsAsset **out) {
   // a u16 palette index can name any of 65536 entries whatever the palette's nominal size: back all of them (zeros)
   const uint64_t sh_min = clustered ? 65536ull * 96ull : 0ull;
   cudaError_t e = cudaSuccess;
-  if ((e = up(as->d_pos, d->pos, d->pos_bytes)) != cudaSuccess || (e = up(as->d_other, d->other, d->other_bytes)) != cudaSuccess ||
-      (e = up(as->d_sh, d->sh, d->sh_bytes, sh_min)) != cudaSuccess || (e = up(as->d_color, d->color, d->color_bytes)) != cudaSuccess ||
-      (chunk_count && (e = up(as->d_chunks, d->chunks, (uint64_t)chunk_count * 64)) != cudaSuccess) ||
+  if ((e = up(b.pos, d->pos, d->pos_bytes)) != cudaSuccess || (e = up(b.other, d->other, d->other_bytes)) != cudaSuccess ||
+      (e = up(b.sh, d->sh, d->sh_bytes, sh_min)) != cudaSuccess || (e = up(b.color, d->color, d->color_bytes)) != cudaSuccess ||
+      (chunk_count && (e = up(b.chunks, d->chunks, (uint64_t)chunk_count * 64)) != cudaSuccess) ||
       (e = asset_init_work(ctx, as, d->splat_count, d->pos_format, d->scale_format, d->sh_format, d->color_format, chunk_count)) != cudaSuccess) {
     gs_asset_destroy(as);
     cudaGetLastError();   // a failed copy or launch leaves its error behind: the next call on the context must not report it
@@ -573,6 +579,27 @@ void gs_asset_destroy(GsAsset *as) {
   if (!as) return;
   if (as->ctx) { cudaSetDevice(as->ctx->device); cudaStreamSynchronize(as->ctx->stream); }
   delete as;
+}
+
+int gs_asset_instance(const GsAsset *source, GsAsset **out) {
+  if (out) *out = nullptr;
+  if (!source || !out) return fail(source ? source->ctx : nullptr, GS_ERR_INVALID_ARGUMENT, "null argument");
+  GsContext *ctx = source->ctx;
+  GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  GsAsset *as = new (std::nothrow) GsAsset();
+  if (!as) return fail(ctx, GS_ERR_OUT_OF_MEMORY, "host allocation failed");
+  as->ctx = ctx;
+  as->blobs = source->blobs;
+  as->blobs->refs.fetch_add(1);
+  const AssetView &sv = source->av;
+  const cudaError_t e = asset_init_work(ctx, as, sv.n, sv.posFmt, sv.scaleFmt, sv.shFmt, sv.colFmt, sv.chunkCount);
+  if (e != cudaSuccess) {
+    gs_asset_destroy(as);   // gives its reference back: the source's blobs stay
+    cudaGetLastError();
+    return fail_cuda(ctx, e, "asset instance", __FILE__, __LINE__);
+  }
+  *out = as;
+  return GS_OK;
 }
 
 int gs_asset_reset_order(GsAsset *as) {
@@ -1157,7 +1184,18 @@ int gs_debug_sort_phases(GsContext *ctx, uint64_t *out, uint32_t max_words, uint
 void *gs_context_stream(GsContext *ctx) { return ctx ? (void *)ctx->stream : nullptr; }
 void *gs_asset_device_ptr(GsAsset *as, int which) {
   if (!as) return nullptr;
-  return which == 0 ? (void *)as->order.get() : which == 1 ? (void *)as->keys.get() : which == 2 ? (void *)as->view.get() : nullptr;
+  const GsBlobs &b = *as->blobs;
+  switch (which) {
+    case 0: return as->order.get();
+    case 1: return as->keys.get();
+    case 2: return as->view.get();
+    case 3: return b.pos.get();
+    case 4: return b.other.get();
+    case 5: return b.sh.get();
+    case 6: return b.color.get();
+    case 7: return b.chunks.get();
+    default: return nullptr;
+  }
 }
 
 }  // extern "C"

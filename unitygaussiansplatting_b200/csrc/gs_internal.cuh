@@ -2,6 +2,7 @@
 // the context / asset objects and the per-stage drivers.
 #pragma once
 #include <algorithm>
+#include <atomic>
 #include <cstring>
 #include <string>
 #include <tuple>
@@ -123,11 +124,19 @@ struct GsContext {
   std::vector<cudaEvent_t> spare_events;
 };
 
-// Its buffers are freed by gs_asset_destroy, with the context's device current and its stream drained.
+// The five blobs of an asset in HBM, 16 bytes of slack each.  Nothing writes them after gs_asset_upload / gs_pack_asset, so an
+// asset and its instances (gs_asset_instance), all on one context, hold one GsBlobs; the last of them to be destroyed frees it.
+struct GsBlobs {
+  gs::Buffer<uint8_t> pos, other, sh, color, chunks;
+  std::atomic<uint32_t> refs{1};   // the assets holding it
+};
+
+// Its buffers are freed by gs_asset_destroy, with the context's device current and its stream drained; so is its GsBlobs when
+// no other asset holds it.
 struct GsAsset {
   GsContext *ctx = nullptr;
   gs::AssetView av{};
-  gs::Buffer<uint8_t> d_pos, d_other, d_sh, d_color, d_chunks;   // the blobs (av points into them), 16 bytes of slack each
+  GsBlobs *blobs = nullptr;   // av points into them
   gs::Buffer<uint32_t> order, keys, key_table, view, rect, d_n;
   gs::Buffer<uint32_t> block_bits;  // bit j: some splat of block j (256 splats) got a bin rectangle from the last view-calc
   // group path only (allocated by gs_group_*): slab membership (bit per splat, byte per 128), compaction output / sort ping-pong payload
@@ -141,6 +150,13 @@ struct GsAsset {
   bool draw_valid = false;   // draw records + bin rects are current (gs_calc_view or gs_frame)
   uint32_t draw_part[3] = {0, 0, 1};   // the tile partition those records were culled for (count <= 1: complete)
   uint32_t view_w = 0, view_h = 0;
+
+  GsAsset() = default;
+  GsAsset(const GsAsset &) = delete;
+  GsAsset &operator=(const GsAsset &) = delete;
+  ~GsAsset() {
+    if (blobs && blobs->refs.fetch_sub(1) == 1) delete blobs;
+  }
 };
 
 namespace gs {
@@ -315,8 +331,8 @@ std::tuple<const void *, int32_t, uint32_t, uint32_t, uint32_t> depth_id(const G
 // surface made by `surfs` (nullptr: none may be made, and a CUDA array is GS_ERR_INVALID_ARGUMENT), or a host buffer uploaded
 // into `staging`, W x H floats that the caller has grown.
 int bind_depth(GsContext *ctx, CallSurfaces *surfs, const GsFrameParams *fp, float *staging, cudaStream_t s, SceneDepth *out);
-// The per-asset work buffers (order, keys, view data, ...) of an asset whose blobs as->d_* are already in HBM, the format
-// fields of as->av, and CSSetIndices: what gs_asset_upload and gs_pack_asset share.
+// The per-asset work buffers (order, keys, view data, ...) of an asset whose blobs as->blobs are already in HBM, the format
+// fields of as->av, and CSSetIndices: what gs_asset_upload, gs_pack_asset and gs_asset_instance share.
 cudaError_t asset_init_work(GsContext *ctx, GsAsset *as, uint32_t n, uint32_t pos_fmt, uint32_t scale_fmt, uint32_t sh_fmt,
                             uint32_t col_fmt, uint32_t chunk_count);
 void rec(GsContext *ctx, int e);

@@ -1031,10 +1031,15 @@ int gs_pack_asset(GsContext *ctx, const GsPackDesc *desc, GsPackedAsset *blobs_o
   }
   if (asset_out) {
     GsAsset *as = new (std::nothrow) GsAsset();
-    if (!as) return fail(ctx, GS_ERR_OUT_OF_MEMORY, "host allocation failed");
+    if (as) as->blobs = new (std::nothrow) GsBlobs();
+    if (!as || !as->blobs) {
+      delete as;
+      return fail(ctx, GS_ERR_OUT_OF_MEMORY, "host allocation failed");
+    }
     as->ctx = ctx;
-    as->d_pos = std::move(b_pos); as->d_other = std::move(b_other); as->d_color = std::move(b_color); as->d_sh = std::move(b_sh);
-    as->d_chunks = std::move(b_chunks);
+    GsBlobs &b = *as->blobs;
+    b.pos = std::move(b_pos); b.other = std::move(b_other); b.color = std::move(b_color); b.sh = std::move(b_sh);
+    b.chunks = std::move(b_chunks);
     const cudaError_t e = asset_init_work(ctx, as, n, pf, sf, shf, cf, chunked ? (uint32_t)(sz.chunk_bytes / 64) : 0u);
     if (e != cudaSuccess) {
       gs_asset_destroy(as);

@@ -156,6 +156,17 @@ class GaussianSplatRenderer {
     m_FrameCounter = 0;
     return true;
   }
+  // OnEnable of a renderer whose m_Asset `source` (enabled) already has: an instance of its asset (gs_asset_instance) on
+  // source's context -- the blobs stay one copy in HBM, the draw order is this renderer's own.  The blobs outlive whichever
+  // renderer is disabled first; the context must outlive this renderer, as for OnEnable(asset, sharedContext).
+  bool CreateInstanceOf(const GaussianSplatRenderer &source) {
+    OnDisable();
+    if (!source.HasValidRenderSetup()) return false;
+    m_Ctx = source.m_Ctx;
+    if (!ok(gs_asset_instance(source.m_Asset, &m_Asset))) return false;
+    m_FrameCounter = 0;
+    return true;
+  }
   void OnDisable() {  // :533-577
     if (m_Asset) gs_asset_destroy(m_Asset);
     if (m_Ctx && m_OwnsCtx) gs_destroy(m_Ctx);
@@ -433,6 +444,22 @@ class GaussianSplatRendererGroup : public GaussianSplatGroupObject {
     GaussianSplatGroupObject *o = new GaussianSplatGroupObject();
     o->m_Assets.assign(gs_group_local_count(m_Group), nullptr);
     if (!m_Group || !ok(gs_group_asset_upload(m_Group, &asset, o->m_Assets.data()))) { delete o; return nullptr; }
+    m_Objects.push_back(o);
+    return o;
+  }
+  // Another splat object drawing the asset of `source` (this group or one of its objects): on every member an instance of
+  // source's asset (gs_asset_instance), sharing its blobs in HBM.  Owned by the group, nullptr on failure.
+  GaussianSplatGroupObject *AddInstance(const GaussianSplatGroupObject &source) {
+    if (!m_Group || source.m_Assets.size() != m_Assets.size()) return nullptr;
+    GaussianSplatGroupObject *o = new GaussianSplatGroupObject();
+    o->m_Assets.assign(m_Assets.size(), nullptr);
+    for (size_t i = 0; i < m_Assets.size(); ++i) {
+      if (!ok(gs_asset_instance(source.m_Assets[i], &o->m_Assets[i]))) {
+        for (GsAsset *a : o->m_Assets) if (a) gs_asset_destroy(a);
+        delete o;
+        return nullptr;
+      }
+    }
     m_Objects.push_back(o);
     return o;
   }

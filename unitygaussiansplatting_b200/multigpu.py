@@ -182,6 +182,16 @@ class GaussianSplatGroup:
         self._objects.append(o)
         return o
 
+    def add_instance(self, source) -> "GaussianSplatGroupObject":
+        """Another splat object drawing the asset of `source` (this group or one of its objects): on every member an instance of
+        source's asset (gs_asset_instance), which shares its blobs in HBM and keeps its own draw order.  Behaves like
+        add_object(source.m_Asset); freed by the group's close()."""
+        if source._group() is not self:
+            raise ValueError("the source belongs to another group")
+        o = GaussianSplatGroupObject(self, source.m_Asset, share=source)
+        self._objects.append(o)
+        return o
+
     def SortAndRenderSplats(self, cam, rts=None, fp=None):
         """rts: one image per LOCAL member (numpy host array, torch CUDA tensor, CudaArrayImage, or None); each receives the
         whole frame."""
@@ -317,12 +327,15 @@ class GaussianSplatGroupObject:
     """A further splat object on a GaussianSplatGroup (GaussianSplatGroup.add_object): the renderer's knobs and the object's
     asset on every local member.  Its assets are freed by the group's close()."""
 
-    def __init__(self, group: GaussianSplatGroup, asset):
+    def __init__(self, group: GaussianSplatGroup, asset, share=None):
         import weakref
         self._group = weakref.ref(group)
         self._lib = group._lib
         self.m_Asset = asset
-        self._assets = _upload(group._lib, group.handle, asset, group.local_count)
+        if share is None:
+            self._assets = _upload(group._lib, group.handle, asset, group.local_count)
+        else:   # `share`: the group or an object of it whose asset this object instances (add_instance)
+            self._assets = _instance(group._lib, share._assets)
         _init_knobs(self)
 
     @property
@@ -344,6 +357,20 @@ def _upload(lib, handle, asset, local_count):
     d = asset.desc()
     assets = (C.c_void_p * local_count)()
     N.check(None, lib.gs_group_asset_upload(handle, C.byref(d), assets))
+    return assets
+
+
+def _instance(lib, sources):
+    """gs_asset_instance of every member's asset; on a failure the instances made so far are destroyed."""
+    assets = (C.c_void_p * len(sources))()
+    for i, src in enumerate(sources):
+        h = C.c_void_p()
+        rc = lib.gs_asset_instance(src, C.byref(h))
+        if rc != N.GS_OK:
+            for j in range(i):
+                lib.gs_asset_destroy(assets[j])
+            N.check(None, rc)
+        assets[i] = h.value
     return assets
 
 

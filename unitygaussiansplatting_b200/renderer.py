@@ -5,6 +5,7 @@ the hot path; everything it does is a call into libgsplat_b200.so (there is no C
   C#                                          here
   ------------------------------------------  ------------------------------------------------
   OnEnable -> CreateResourcesForAsset (:373)   GaussianSplatRenderer(asset)  -> gs_asset_upload
+  (a further renderer of the same asset)       renderer.Instance()           -> gs_asset_instance
   SortPoints(cmd, cam, matrix)        (:612)   SortPoints(cam)               -> gs_sort
   CalcViewData(cmb, cam)              (:579)   CalcViewData(cam)             -> gs_calc_view
   cmb.DrawProcedural(matSplats)       (:165)   DrawSplats(cam, rt)           -> gs_render
@@ -424,6 +425,14 @@ class GaussianSplatRenderer:
         self._init_state(asset, context)
         self._asset = handle
         return self
+
+    def Instance(self) -> "GaussianSplatRenderer":
+        """A further renderer of this renderer's asset on its context (gs_asset_instance): the blobs in HBM are shared, not
+        uploaded again; the new renderer has its own draw order, view data and knobs (at their defaults) and its own Dispose().
+        It behaves exactly like GaussianSplatRenderer(self.m_Asset, self.context), and outlives this renderer if need be."""
+        h = C.c_void_p()
+        N.check(self.context.handle, self._lib.gs_asset_instance(self._asset, C.byref(h)))
+        return GaussianSplatRenderer.from_device_asset(self.m_Asset, h, self.context)
 
     def _init_state(self, asset: GaussianSplatAsset, context: Optional[GaussianSplatContext]):
         self.context = context or GaussianSplatContext(0)
