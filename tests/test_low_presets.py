@@ -67,6 +67,21 @@ def test_bc7_encoder_round_trip(g, O):
     assert enc(weird)[0] & 0x7F == 0x40
 
 
+def test_bc7_encoder_bytes_match_fixture(g):
+    """tests/golden/bc7_encode_blocks.npz (tests/golden/make_bc7_encode_golden.py): 2,560 blocks -- random, noisy ramps,
+    constant, two-colour, out of range, NaN / Inf -- and the 16 bytes the encoder wrote for each.  The GPU packer runs the
+    same encoder (csrc/gs_asset_format.h), so this pins both."""
+    from unitygaussiansplatting_b200 import _native as N
+    L = N.asset_lib()
+    d = np.load(ROOT / "tests" / "golden" / "bc7_encode_blocks.npz")
+    rgba = np.ascontiguousarray(d["rgba"], np.float32)
+    out = np.zeros((len(rgba), 16), np.uint8)
+    for i in range(len(rgba)):
+        L.gsa_bc7_encode_block(rgba[i].ctypes.data, out[i].ctypes.data)
+    bad = np.nonzero((out != d["encoded"]).any(axis=1))[0]
+    assert bad.size == 0, "BC7 encoder output differs for blocks %s" % bad[:8]
+
+
 # ---- k-means: a scalar restatement of E/Utils/KMeansClustering.cs in numpy float32, for a case small enough for Python ----
 F = np.float32
 

@@ -24,7 +24,7 @@ NATIVE_LIB = PKG / "libgsplat_b200.so"
 ASSET_LIB = PKG / "libgsplat_asset.so"
 
 CU_SOURCES = ["gs_api.cu", "gs_group.cu", "gs_image.cu", "gs_bins.cu", "gs_view.cu", "gs_sort.cu", "gs_raster.cu", "gs_export.cu", "gs_pack.cu"]
-CU_HEADERS = ["gs_buffer.cuh", "gs_common.cuh", "gs_kernels.cuh", "gs_internal.cuh", "gs_nccl.h", "gs_bc7.cuh", "gs_packed_float.cuh", "gs_srgb8.cuh", "gs_srgb8_tables.h", "bc7_tables.h", "../../include/gsplat_b200.h"]
+CU_HEADERS = ["gs_asset_format.h", "gs_buffer.cuh", "gs_common.cuh", "gs_kernels.cuh", "gs_internal.cuh", "gs_nccl.h", "gs_bc7.cuh", "gs_packed_float.cuh", "gs_srgb8.cuh", "gs_srgb8_tables.h", "bc7_tables.h", "../../include/gsplat_b200.h"]
 
 
 def _host_cxx() -> str:
@@ -100,7 +100,7 @@ def build_native(force: bool = False, verbose: bool = False) -> Path:
 
 def build_asset(force: bool = False) -> Path:
     srcs = [CSRC / "asset_creator.cpp", CSRC / "asset_cluster_bc7.cpp", CSRC / "asset_export.cpp"]
-    if force or _stale(ASSET_LIB, [*srcs, ROOT / "include" / "gsplat_asset.h"]):
+    if force or _stale(ASSET_LIB, [*srcs, CSRC / "gs_asset_format.h", ROOT / "include" / "gsplat_asset.h"]):
         # -mavx2: the k-means distance loops evaluate 16 candidate means side by side (no FMA: -ffp-contract=off)
         _run([_host_cxx(), "-O3", "-mavx2", "-std=c++17", "-fopenmp", "-fPIC", "-shared", "-ffp-contract=off", "-fvisibility=hidden",
               "-o", str(ASSET_LIB), *map(str, srcs), "-lz"])

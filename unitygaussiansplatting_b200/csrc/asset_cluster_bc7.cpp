@@ -7,9 +7,12 @@
 //     distances are evaluated side by side (each lane keeps the scalar operation order, so results equal the scalar ones).
 //   * BC7 colour: the reference calls Unity's closed-source texture compressor (E/GaussianSplatAssetCreator.cs:901-912),
 //     which cannot be reproduced; any conformant BC7 stream decodes the same way on the GPU, so this packer emits mode-6
-//     blocks (one subset, 7.7.7.7 endpoints + p-bits, 4-bit indices) from a bounding-box fit.  Lossy, NOT bit-identical
+//     blocks (one subset, 7.7.7.7 endpoints + p-bits, 4-bit indices) from a principal-axis fit.  Lossy, NOT bit-identical
 //     to Unity's encoder; the decode side (gs_bc7.cuh / oracle) handles all eight modes.
+// The pcg stream, the batch draw, the squared distance and the BC7 block encoder are gs_asset_format.h, shared with the
+// GPU packer (gs_pack.cu).
 #include "../../include/gsplat_asset.h"
+#include "gs_asset_format.h"
 
 #include <algorithm>
 #include <cmath>
@@ -56,39 +59,7 @@ int usable_threads() { static const int t = usable_threads_uncached(); return t;
 // keeps the fork/join and barrier cost below the work (each loop is 1-5 ms of arithmetic)
 inline int small_team(int threads) { return std::min(threads, 16); }
 
-inline uint32_t as_u32(float f) { uint32_t u; std::memcpy(&u, &f, 4); return u; }
-inline float as_f32(uint32_t u) { float f; std::memcpy(&f, &u, 4); return f; }
-
-// K:571-593
-inline uint32_t pcg_hash(uint32_t input) {
-  uint32_t state = input * 747796405u + 2891336453u;
-  uint32_t word = ((state >> ((state >> 28) + 4u)) ^ state) * 277803737u;
-  return (word >> 22) ^ word;
-}
-inline float pcg_hash_float(uint32_t input, float up_to) {
-  uint32_t val = pcg_hash(input);
-  float f = as_f32(0x3f800000u | (val >> 9)) - 1.0f;
-  return f * up_to;
-}
-inline uint32_t pcg_random(uint32_t &rng_state) {
-  uint32_t state = rng_state;
-  rng_state = rng_state * 747796405u + 2891336453u;
-  uint32_t word = ((state >> ((state >> 28) + 4u)) ^ state) * 277803737u;
-  return (word >> 22) ^ word;
-}
-
-// DistanceSquared, K:138-206 (AVX path): per block of 8, d += ((s0+s1) + (s2+s3)) ... as "F0 + F1 + F4 + F5" after hadd.
-inline float distance_squared(int dim, const float *a, const float *b) {
-  float d = 0;
-  int i = 0;
-  for (; i + 7 < dim; i += 8) {
-    float v[8];
-    for (int k = 0; k < 8; ++k) { float t = a[i + k] - b[i + k]; v[k] = t * t; }
-    d += (v[0] + v[1]) + (v[2] + v[3]) + (v[4] + v[5]) + (v[6] + v[7]);
-  }
-  for (; i < dim; ++i) { float t = a[i] - b[i]; d += t * t; }
-  return d;
-}
+using namespace gs;
 
 // The same arithmetic for L candidate means at once.  `mt` is dimension-major: mt[c * stride + j] = means[j][c].
 template <int L>
@@ -150,18 +121,9 @@ inline int nearest_mean(const MeansT &m, const float *p, float *min_dist_out) {
 // MakeBatchJob, K:456-477: distinct random points in draw order
 void make_random_batch(int dim, const float *data, uint32_t data_size, uint32_t &rng, float *out, uint32_t batch,
                        std::vector<uint8_t> &picked) {
-  uint32_t seed = pcg_random(rng);
-  std::vector<uint32_t> chosen;
-  chosen.reserve(batch);
-  while (chosen.size() < batch) {
-    uint32_t index = pcg_hash(seed++) % data_size;
-    if (!picked[index]) {
-      std::memcpy(out + (size_t)chosen.size() * dim, data + (size_t)index * dim, (size_t)dim * 4);
-      picked[index] = 1;
-      chosen.push_back(index);
-    }
-  }
-  for (uint32_t i : chosen) picked[i] = 0;
+  std::vector<uint32_t> chosen(batch);
+  random_batch(data_size, rng, batch, picked.data(), chosen.data());
+  for (uint32_t i = 0; i < batch; ++i) std::memcpy(out + (size_t)i * dim, data + (size_t)chosen[i] * dim, (size_t)dim * 4);
 }
 
 // KMeansPlusPlus, K:325-411 (+ PickPointIndex K:273-323, CalcDistSqJob K:249-271)
@@ -174,7 +136,7 @@ void kmeans_plus_plus(int dim, int k, const float *data, uint32_t data_size, flo
   std::memcpy(means, data + (size_t)point * dim, (size_t)dim * 4);
 #pragma omp parallel for schedule(static) num_threads(team)
   for (int64_t i = 0; i < (int64_t)data_size; ++i)
-    if (i != point) min_dist_sq[i] = distance_squared(dim, data + (size_t)i * dim, means);
+    if (i != point) min_dist_sq[i] = distance_squared(data + (size_t)i * dim, means, dim);
   constexpr int kSumBatch = 1024;
   const int sum_batches = (int)((data_size + kSumBatch - 1) / kSumBatch);
   std::vector<float> partial(sum_batches);
@@ -189,7 +151,7 @@ void kmeans_plus_plus(int dim, int k, const float *data, uint32_t data_size, flo
       float sum = 0;
       for (uint32_t i = i0; i < i1; ++i) {
         if (taken[i]) continue;
-        if (new_mean) min_dist_sq[i] = std::min(min_dist_sq[i], distance_squared(dim, data + (size_t)i * dim, new_mean));
+        if (new_mean) min_dist_sq[i] = std::min(min_dist_sq[i], distance_squared(data + (size_t)i * dim, new_mean, dim));
         sum += min_dist_sq[i];
       }
       partial[b] = sum;
@@ -289,103 +251,9 @@ int gsa_kmeans(uint32_t dim, const float *data, uint32_t data_size, uint32_t bat
 
 // One 4x4 block of float RGBA in [0,1] (raster order) -> 16 bytes of BC7 mode 6.
 void gsa_bc7_encode_block(const float rgba[64], uint8_t out[16]) {
-  // endpoints: extremes of the block's pixels along their principal axis (power iteration on the 4x4 covariance), then one
-  // least-squares refit against the chosen indices; each endpoint is 7 bits per channel + one p-bit shared by its channels
-  float px[16][4], mean[4] = {0, 0, 0, 0};
-  for (int i = 0; i < 16; ++i)
-    for (int c = 0; c < 4; ++c) {
-      float v = rgba[i * 4 + c];
-      v = (v > 0.0f) ? (v < 1.0f ? v : 1.0f) : 0.0f;  // NaN -> 0
-      px[i][c] = v * 255.0f;
-      mean[c] += px[i][c] * (1.0f / 16.0f);
-    }
-  float cov[4][4] = {};
-  for (int i = 0; i < 16; ++i)
-    for (int r = 0; r < 4; ++r)
-      for (int c = 0; c < 4; ++c) cov[r][c] += (px[i][r] - mean[r]) * (px[i][c] - mean[c]);
-  float axis[4] = {1.0f, 1.0f, 1.0f, 1.0f};
-  for (int it = 0; it < 8; ++it) {
-    float n[4] = {0, 0, 0, 0}, len = 0;
-    for (int r = 0; r < 4; ++r) { for (int c = 0; c < 4; ++c) n[r] += cov[r][c] * axis[c]; len += n[r] * n[r]; }
-    if (len < 1e-12f) break;
-    len = 1.0f / std::sqrt(len);
-    for (int r = 0; r < 4; ++r) axis[r] = n[r] * len;
-  }
-  float tmin = 1e30f, tmax = -1e30f;
-  for (int i = 0; i < 16; ++i) {
-    float t = 0;
-    for (int c = 0; c < 4; ++c) t += (px[i][c] - mean[c]) * axis[c];
-    tmin = std::min(tmin, t); tmax = std::max(tmax, t);
-  }
-  float target[2][4];
-  for (int c = 0; c < 4; ++c) { target[0][c] = mean[c] + axis[c] * tmin; target[1][c] = mean[c] + axis[c] * tmax; }
-  static const int kW4[16] = {0, 4, 9, 13, 17, 21, 26, 30, 34, 38, 43, 47, 51, 55, 60, 64};
-  int ep[2][4], pbit[2] = {0, 0}, idx[16];
-  float best_total = 1e30f;
-  int best_ep[2][4] = {}, best_p[2] = {0, 0}, best_idx[16] = {};
-  for (int round = 0; round < 2; ++round) {
-    for (int e = 0; e < 2; ++e) {
-      float best_err = 1e30f;
-      for (int p = 0; p < 2; ++p) {
-        int q[4]; float err = 0;
-        for (int c = 0; c < 4; ++c) {
-          const float t = std::min(255.0f, std::max(0.0f, target[e][c]));
-          int v = (int)std::lround((t - (float)p) * 0.5f);
-          v = std::min(127, std::max(0, v));
-          q[c] = (v << 1) | p;
-          float d = (float)q[c] - t;
-          err += d * d;
-        }
-        if (err < best_err) { best_err = err; pbit[e] = p; for (int c = 0; c < 4; ++c) ep[e][c] = q[c]; }
-      }
-    }
-    int pal[16][4];
-    for (int w = 0; w < 16; ++w)
-      for (int c = 0; c < 4; ++c) pal[w][c] = ((64 - kW4[w]) * ep[0][c] + kW4[w] * ep[1][c] + 32) >> 6;
-    float total = 0;
-    for (int i = 0; i < 16; ++i) {
-      float best = 1e30f; int bi = 0;
-      for (int w = 0; w < 16; ++w) {
-        float err = 0;
-        for (int c = 0; c < 4; ++c) { float d = (float)pal[w][c] - px[i][c]; err += d * d; }
-        if (err < best) { best = err; bi = w; }
-      }
-      idx[i] = bi; total += best;
-    }
-    if (total < best_total) {
-      best_total = total;
-      std::memcpy(best_ep, ep, sizeof(ep)); std::memcpy(best_p, pbit, sizeof(pbit)); std::memcpy(best_idx, idx, sizeof(idx));
-    }
-    if (round == 1) break;
-    // least squares for the two endpoints given the weights w_i = kW4[idx_i] / 64: minimise sum |(1-w) A + w B - px|^2
-    float saa = 0, sab = 0, sbb = 0, ra[4] = {0, 0, 0, 0}, rb[4] = {0, 0, 0, 0};
-    for (int i = 0; i < 16; ++i) {
-      const float w = (float)kW4[idx[i]] * (1.0f / 64.0f), u = 1.0f - w;
-      saa += u * u; sab += u * w; sbb += w * w;
-      for (int c = 0; c < 4; ++c) { ra[c] += u * px[i][c]; rb[c] += w * px[i][c]; }
-    }
-    const float det = saa * sbb - sab * sab;
-    if (std::fabs(det) < 1e-6f) break;
-    for (int c = 0; c < 4; ++c) {
-      target[0][c] = (ra[c] * sbb - rb[c] * sab) / det;
-      target[1][c] = (rb[c] * saa - ra[c] * sab) / det;
-    }
-  }
-  std::memcpy(ep, best_ep, sizeof(ep)); std::memcpy(pbit, best_p, sizeof(pbit)); std::memcpy(idx, best_idx, sizeof(idx));
-  if (idx[0] >= 8) {  // the anchor (pixel 0) stores 3 bits: swap the endpoints so that its index has a zero top bit
-    for (int c = 0; c < 4; ++c) std::swap(ep[0][c], ep[1][c]);
-    std::swap(pbit[0], pbit[1]);
-    for (int i = 0; i < 16; ++i) idx[i] = 15 - idx[i];
-  }
-  unsigned __int128 bits = 0;
-  int pos = 0;
-  auto put = [&](uint32_t v, int n) { bits |= (unsigned __int128)v << pos; pos += n; };
-  put(1u << 6, 7);
-  for (int c = 0; c < 4; ++c) { put((uint32_t)ep[0][c] >> 1, 7); put((uint32_t)ep[1][c] >> 1, 7); }
-  put((uint32_t)pbit[0], 1); put((uint32_t)pbit[1], 1);
-  put((uint32_t)idx[0], 3);
-  for (int i = 1; i < 16; ++i) put((uint32_t)idx[i], 4);
-  std::memcpy(out, &bits, 16);
+  const Bc7Block b = bc7_encode_block(rgba);
+  std::memcpy(out, &b.lo, 8);
+  std::memcpy(out + 8, &b.hi, 8);
 }
 
 }  // extern "C"

@@ -5,15 +5,10 @@
 // function below as E/...:line).  This is new code: a flat, OpenMP-parallel C++ pipeline
 // over one contiguous record array, not a translation of the Burst job structs.
 //
-// Third-party arithmetic that is not in /root/reference: Unity.Mathematics 1.2.6
-// (package/package.json:3) math.f32tof16 / math.pow / math.min / math.max / math.saturate.
-// f32tof16 is restated below from its published source (truncate the low 12 mantissa bits,
-// add half, shift; i.e. round half up on bit 12); pow(float,float) is System.Math.Pow in
-// double, narrowed to float; min / max return their second operand unless the first wins
-// strictly or the second is NaN, so saturate(NaN) = max(0, min(1, NaN)) = 1.
-// oracle/refcs/ compiles the reference's own C# against these semantics and
-// tests/test_reference_cs.py compares this file's bytes with it.
+// The format's rules and encoders are gs_asset_format.h, shared with the GPU packer (gs_pack.cu).
+// oracle/refcs/ compiles the reference's own C# and tests/test_reference_cs.py compares this file's bytes with it.
 #include "../../include/gsplat_asset.h"
+#include "gs_asset_format.h"
 
 #include <algorithm>
 #include <cmath>
@@ -35,24 +30,15 @@ int gsa_usable_threads();  // asset_cluster_bc7.cpp: OpenMP default capped by af
 
 namespace {
 
-constexpr uint32_t kChunkSize = 256;   // R/GaussianSplatAsset.cs:14
-constexpr uint32_t kTexWidth = 2048;   // R/GaussianSplatAsset.cs:15
+using namespace gs;
 
-inline uint32_t as_u32(float f) { uint32_t u; std::memcpy(&u, &f, 4); return u; }
-inline float as_f32(uint32_t u) { float f; std::memcpy(&f, &u, 4); return f; }
-
-// ---- counter-based RNG (pcg hash, same family as E/Utils/KMeansClustering.cs:573-592) ----
-inline uint32_t pcg_hash(uint32_t input) {
-  uint32_t state = input * 747796405u + 2891336453u;
-  uint32_t word = ((state >> ((state >> 28) + 4u)) ^ state) * 277803737u;
-  return (word >> 22) ^ word;
-}
+// ---- counter-based RNG for the synthetic scenes (pcg hash, same family as the k-means') ----
 struct Rng {
   uint32_t base;
   uint32_t ctr;
   Rng(uint32_t seed, uint32_t index) : base(pcg_hash(seed ^ pcg_hash(index * 0x9E3779B9u + 0x7F4A7C15u))), ctr(0) {}
   uint32_t next() { return pcg_hash(base + (ctr++) * 0x85EBCA6Bu); }
-  float uniform() { return as_f32(0x3f800000u | (next() >> 9)) - 1.0f; }  // [0,1)
+  float uniform() { return f32_from_bits(0x3f800000u | (next() >> 9)) - 1.0f; }  // [0,1)
   float range(float lo, float hi) { return lo + (hi - lo) * uniform(); }
   float normal() {  // Box-Muller
     float u1 = std::max(uniform(), 1.0e-7f);
@@ -62,66 +48,6 @@ struct Rng {
 };
 
 inline float sigmoid(float v) { return 1.0f / (1.0f + std::exp(-v)); }  // R/GaussianUtils.cs:9-12
-
-// Unity.Mathematics math.f32tof16 (restated; see file header).
-inline uint32_t unity_f32tof16(float x) {
-  const int32_t infinity_32 = 255 << 23;
-  const uint32_t msk = 0x7FFFF000u;
-  uint32_t ux = as_u32(x);
-  uint32_t uux = ux & msk;
-  float scaled = std::min(as_f32(uux) * 1.92592994e-34f, 260042752.0f);
-  uint32_t h = (as_u32(scaled) + 0x1000u) >> 13;
-  if ((int32_t)uux >= infinity_32) h = ((int32_t)uux > infinity_32) ? 0x7e00u : 0x7c00u;
-  return h | ((ux & ~msk) >> 16);
-}
-
-// Unity.Mathematics math.min / max / saturate (see file header): of two equal values (+0 / -0) the second is kept, a NaN
-// second operand is ignored.  Every min / max fold of the importer (bounds, chunk ranges) goes through these.
-inline float unity_min(float x, float y) { return (std::isnan(y) || x < y) ? x : y; }
-inline float unity_max(float x, float y) { return (std::isnan(y) || x > y) ? x : y; }
-inline float saturate(float v) { return unity_max(0.0f, unity_min(1.0f, v)); }   // clamp(v, 0, 1); NaN -> 1
-
-// R/GaussianUtils.cs:25-30
-inline float square_centered01(float x) {
-  x -= 0.5f;
-  float sgn = (x > 0.0f) ? 1.0f : ((x < 0.0f) ? -1.0f : 0.0f);
-  x *= x * sgn;
-  return x * 2.0f + 0.5f;
-}
-
-// R/GaussianUtils.cs:81-95
-inline uint64_t morton_part1by2(uint64_t x) {
-  x &= 0x1fffff;
-  x = (x ^ (x << 32)) & 0x1f00000000ffffULL;
-  x = (x ^ (x << 16)) & 0x1f0000ff0000ffULL;
-  x = (x ^ (x << 8)) & 0x100f00f00f00f00fULL;
-  x = (x ^ (x << 4)) & 0x10c30c30c30c30c3ULL;
-  x = (x ^ (x << 2)) & 0x1249249249249249ULL;
-  return x;
-}
-inline uint64_t morton_encode3(uint32_t x, uint32_t y, uint32_t z) {
-  return (morton_part1by2(z) << 2) | (morton_part1by2(y) << 1) | morton_part1by2(x);
-}
-
-// R/GaussianUtils.cs:98-105 / S/GaussianSplatting.hlsl:120-127
-inline void decode_morton2d_16x16(uint32_t t, uint32_t &x, uint32_t &y) {
-  t = (t & 0xFF) | ((t & 0xFE) << 7);
-  t &= 0x5555;
-  t = (t ^ (t >> 1)) & 0x3333;
-  t = (t ^ (t >> 2)) & 0x0f0f;
-  x = t & 0xF;
-  y = t >> 8;
-}
-// E/GaussianSplatAssetCreator.cs:863-871
-inline uint32_t splat_index_to_texture_index(uint32_t idx) {
-  uint32_t mx, my;
-  decode_morton2d_16x16(idx, mx, my);
-  uint32_t width = kTexWidth / 16;
-  idx >>= 8;
-  uint32_t x = (idx % width) * 16 + mx;
-  uint32_t y = (idx / width) * 16 + my;
-  return y * kTexWidth + x;
-}
 
 // R/GaussianUtils.cs:46-76
 inline void pack_smallest3(const float qin[4], float out[4]) {
@@ -142,73 +68,11 @@ inline void pack_smallest3(const float qin[4], float out[4]) {
   out[3] = (float)index / 3.0f;
 }
 
-// E/GaussianSplatAssetCreator.cs:705-725 -- all truncating casts
-inline uint64_t enc_norm16(const float v[3]) {
-  return (uint64_t)(v[0] * 65535.5f) | ((uint64_t)(v[1] * 65535.5f) << 16) | ((uint64_t)(v[2] * 65535.5f) << 32);
-}
-inline uint32_t enc_norm11(const float v[3]) {
-  return (uint32_t)(v[0] * 2047.5f) | ((uint32_t)(v[1] * 1023.5f) << 11) | ((uint32_t)(v[2] * 2047.5f) << 21);
-}
-inline uint16_t enc_norm655(const float v[3]) {
-  return (uint16_t)((uint32_t)(v[0] * 63.5f) | ((uint32_t)(v[1] * 31.5f) << 6) | ((uint32_t)(v[2] * 31.5f) << 11));
-}
-inline uint16_t enc_norm565(const float v[3]) {
-  return (uint16_t)((uint32_t)(v[0] * 31.5f) | ((uint32_t)(v[1] * 63.5f) << 5) | ((uint32_t)(v[2] * 31.5f) << 11));
-}
-inline uint32_t enc_quat10(const float v[4]) {
-  return (uint32_t)(v[0] * 1023.5f) | ((uint32_t)(v[1] * 1023.5f) << 10) | ((uint32_t)(v[2] * 1023.5f) << 20) |
-         ((uint32_t)(v[3] * 3.5f) << 30);
-}
-
-inline uint32_t vector_size(uint32_t fmt) {  // R/GaussianSplatAsset.cs:39-49
-  switch (fmt) { case 0: return 12; case 1: return 6; case 2: return 4; case 3: return 2; default: return 0; }
-}
-inline uint32_t color_size(uint32_t fmt) {  // R/GaussianSplatAsset.cs:58-68
-  switch (fmt) { case 0: return 16; case 1: return 8; case 2: return 4; case 3: return 1; default: return 0; }
-}
-inline uint32_t sh_stride(uint32_t fmt) {  // R/GaussianSplatAsset.cs:83-101 (clustered formats: SHTableItemFloat16 palette entries)
-  switch (fmt) { case 0: return 192; case 1: return 96; case 2: return 60; case 3: return 32; default: return fmt <= 8 ? 96 : 0; }
-}
-inline uint32_t sh_count(uint32_t fmt, uint32_t n) {  // GetSHCount, R/GaussianSplatAsset.cs:135-150
-  return fmt <= 3 ? n : (65536u >> (fmt - 4));
-}
-inline uint64_t next_multiple(uint64_t v, uint64_t m) { return (v + m - 1) / m * m; }
-
-// E/GaussianSplatAssetCreator.cs:727-758
-inline void emit_vector(const float v[3], uint8_t *dst, uint32_t fmt) {
-  switch (fmt) {
-    case 0: std::memcpy(dst, v, 12); break;
-    case 1: {
-      float s[3] = {saturate(v[0]), saturate(v[1]), saturate(v[2])};
-      uint64_t e = enc_norm16(s);
-      uint32_t lo = (uint32_t)e; uint16_t hi = (uint16_t)(e >> 32);
-      std::memcpy(dst, &lo, 4); std::memcpy(dst + 4, &hi, 2);
-    } break;
-    case 2: {
-      float s[3] = {saturate(v[0]), saturate(v[1]), saturate(v[2])};
-      uint32_t e = enc_norm11(s);
-      std::memcpy(dst, &e, 4);
-    } break;
-    case 3: {
-      float s[3] = {saturate(v[0]), saturate(v[1]), saturate(v[2])};
-      uint16_t e = enc_norm655(s);
-      std::memcpy(dst, &e, 2);
-    } break;
-  }
-}
-
-struct ChunkInfo {  // R/GaussianSplatAsset.cs:231-237 (64 bytes)
-  uint32_t colR, colG, colB, colA;
-  float posX[2], posY[2], posZ[2];
-  uint32_t sclX, sclY, sclZ;
-  uint32_t shR, shG, shB;
-};
-static_assert(sizeof(ChunkInfo) == 64, "ChunkInfo must be 64 bytes");
-static_assert(sizeof(GsaInputSplat) == 248, "InputSplatData must be 248 bytes");
-
-inline bool uses_chunks(uint32_t pf, uint32_t sf, uint32_t cf, uint32_t shf) {  // E/...:54-58
-  return pf != 0 || sf != 0 || cf != 0 || shf != 0;
-}
+static_assert(sizeof(GsaInputSplat) == kRecFloats * 4, "InputSplatData must be 248 bytes");
+static_assert(offsetof(GsaInputSplat, dc0) == kOffDc0 * 4 && offsetof(GsaInputSplat, sh) == kOffSh * 4 &&
+                  offsetof(GsaInputSplat, opacity) == kOffOpacity * 4 && offsetof(GsaInputSplat, scale) == kOffScale * 4 &&
+                  offsetof(GsaInputSplat, rot) == kOffRot * 4,
+              "GsaInputSplat is the record emit_splat reads");
 
 void normalize4(float q[4]) {
   float l = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
@@ -221,7 +85,7 @@ void normalize4(float q[4]) {
 extern "C" {
 
 uint64_t gsa_morton_encode3(uint32_t x, uint32_t y, uint32_t z) { return morton_encode3(x, y, z); }
-uint32_t gsa_splat_index_to_texture_index(uint32_t idx) { return splat_index_to_texture_index(idx); }
+uint32_t gsa_splat_index_to_texture_index(uint32_t idx) { return splat_index_to_texel(idx); }
 void gsa_pack_smallest3(const float q[4], float out[4]) { pack_smallest3(q, out); }
 uint32_t gsa_f32tof16(float v) { return unity_f32tof16(v); }
 
@@ -287,21 +151,7 @@ int gsa_generate(uint32_t kind, uint32_t n, uint32_t seed, GsaInputSplat *out) {
 }
 
 int gsa_calc_sizes(uint32_t n, uint32_t pf, uint32_t sf, uint32_t cf, uint32_t shf, GsaSizes *out) {
-  if (!out || pf > 3 || sf > 3 || cf > 3 || shf > 8) return -1;
-  // the reference skips clustering when the palette would not be smaller than the data (E/...:480-482) and then writes an
-  // asset its own shader mis-reads (no index in `other`, empty SH blob); refuse that combination instead
-  if (shf > 3 && n <= sh_count(shf, n)) return -1;
-  uint32_t width = kTexWidth;
-  uint32_t height = std::max<uint32_t>(1, (n + width - 1) / width);
-  height = (height + 15) / 16 * 16;  // R/GaussianSplatAsset.cs:152-160
-  out->tex_width = width;
-  out->tex_height = height;
-  out->pos_bytes = next_multiple((uint64_t)n * vector_size(pf), 8);          // E/...:815
-  out->other_bytes = next_multiple((uint64_t)n * (4 + vector_size(sf) + (shf > 3 ? 2 : 0)), 8);  // E/...:837-842
-  out->color_bytes = (uint64_t)width * height * color_size(cf);
-  out->sh_bytes = (uint64_t)sh_count(shf, n) * sh_stride(shf);  // clustered: the palette only (E/...:1048-1051)
-  out->chunk_bytes = uses_chunks(pf, sf, cf, shf) ? (uint64_t)((n + kChunkSize - 1) / kChunkSize) * 64 : 0;
-  return 0;
+  return out && calc_sizes(n, pf, sf, cf, shf, out) ? 0 : -1;
 }
 
 int gsa_create_asset(GsaInputSplat *splats, uint32_t n, uint32_t pf, uint32_t sf, uint32_t cf, uint32_t shf,
@@ -372,118 +222,48 @@ int gsa_create_asset(GsaInputSplat *splats, uint32_t n, uint32_t pf, uint32_t sf
     const int64_t chunk_count = (n + kChunkSize - 1) / kChunkSize;
 #pragma omp parallel for schedule(dynamic, 64) num_threads(gsa_usable_threads())
     for (int64_t c = 0; c < chunk_count; ++c) {
-      float mnp[3], mns[3], mnc[4], mnh[3], mxp[3], mxs[3], mxc[4], mxh[3];
-      for (int k = 0; k < 3; ++k) { mnp[k] = mns[k] = mnh[k] = INFINITY; mxp[k] = mxs[k] = mxh[k] = -INFINITY; }
-      for (int k = 0; k < 4; ++k) { mnc[k] = INFINITY; mxc[k] = -INFINITY; }
+      float mn[13], mx[13];   // 0..2 position, 3..5 scale, 6..9 colour (dc0 rgb, opacity), 10..12 SH channel
+      for (int q = 0; q < 13; ++q) { mn[q] = INFINITY; mx[q] = -INFINITY; }
       uint32_t b = (uint32_t)std::min<int64_t>(c * kChunkSize, n), e = (uint32_t)std::min<int64_t>((c + 1) * kChunkSize, n);
       for (uint32_t i = b; i < e; ++i) {
         GsaInputSplat &s = splats[i];
         for (int k = 0; k < 3; ++k) s.scale[k] = (float)std::pow((double)s.scale[k], (double)(1.0f / 8.0f));
         s.opacity = square_centered01(s.opacity);
-        float col[4] = {s.dc0[0], s.dc0[1], s.dc0[2], s.opacity};
-        for (int k = 0; k < 3; ++k) {
-          mnp[k] = unity_min(mnp[k], s.pos[k]); mxp[k] = unity_max(mxp[k], s.pos[k]);
-          mns[k] = unity_min(mns[k], s.scale[k]); mxs[k] = unity_max(mxs[k], s.scale[k]);
-        }
-        for (int k = 0; k < 4; ++k) { mnc[k] = unity_min(mnc[k], col[k]); mxc[k] = unity_max(mxc[k], col[k]); }
+        const float v[10] = {s.pos[0], s.pos[1], s.pos[2], s.scale[0], s.scale[1], s.scale[2], s.dc0[0], s.dc0[1], s.dc0[2], s.opacity};
+        for (int q = 0; q < 10; ++q) { mn[q] = unity_min(mn[q], v[q]); mx[q] = unity_max(mx[q], v[q]); }
         for (int j = 0; j < 15; ++j)
           for (int k = 0; k < 3; ++k) {
-            mnh[k] = unity_min(mnh[k], s.sh[j * 3 + k]); mxh[k] = unity_max(mxh[k], s.sh[j * 3 + k]);
+            mn[10 + k] = unity_min(mn[10 + k], s.sh[j * 3 + k]); mx[10 + k] = unity_max(mx[10 + k], s.sh[j * 3 + k]);
           }
       }
-      for (int k = 0; k < 3; ++k) {
-        mxp[k] = unity_max(mxp[k], mnp[k] + 1.0e-5f);
-        mxs[k] = unity_max(mxs[k], mns[k] + 1.0e-5f);
-        mxh[k] = unity_max(mxh[k], mnh[k] + 1.0e-5f);
-      }
-      for (int k = 0; k < 4; ++k) mxc[k] = unity_max(mxc[k], mnc[k] + 1.0e-5f);
-      ChunkInfo info;
-      info.posX[0] = mnp[0]; info.posX[1] = mxp[0];
-      info.posY[0] = mnp[1]; info.posY[1] = mxp[1];
-      info.posZ[0] = mnp[2]; info.posZ[1] = mxp[2];
-      info.sclX = unity_f32tof16(mns[0]) | (unity_f32tof16(mxs[0]) << 16);
-      info.sclY = unity_f32tof16(mns[1]) | (unity_f32tof16(mxs[1]) << 16);
-      info.sclZ = unity_f32tof16(mns[2]) | (unity_f32tof16(mxs[2]) << 16);
-      info.colR = unity_f32tof16(mnc[0]) | (unity_f32tof16(mxc[0]) << 16);
-      info.colG = unity_f32tof16(mnc[1]) | (unity_f32tof16(mxc[1]) << 16);
-      info.colB = unity_f32tof16(mnc[2]) | (unity_f32tof16(mxc[2]) << 16);
-      info.colA = unity_f32tof16(mnc[3]) | (unity_f32tof16(mxc[3]) << 16);
-      info.shR = unity_f32tof16(mnh[0]) | (unity_f32tof16(mxh[0]) << 16);
-      info.shG = unity_f32tof16(mnh[1]) | (unity_f32tof16(mxh[1]) << 16);
-      info.shB = unity_f32tof16(mnh[2]) | (unity_f32tof16(mxh[2]) << 16);
-      chunks[c] = info;
+      for (int q = 0; q < 13; ++q) mx[q] = unity_max(mx[q], mn[q] + 1.0e-5f);
+      chunks[c] = encode_chunk(mn, mx);
       for (uint32_t i = b; i < e; ++i) {
         GsaInputSplat &s = splats[i];
         for (int k = 0; k < 3; ++k) {
-          s.pos[k] = (s.pos[k] - mnp[k]) / (mxp[k] - mnp[k]);
-          s.scale[k] = (s.scale[k] - mns[k]) / (mxs[k] - mns[k]);
-          s.dc0[k] = (s.dc0[k] - mnc[k]) / (mxc[k] - mnc[k]);
+          s.pos[k] = (s.pos[k] - mn[k]) / (mx[k] - mn[k]);
+          s.scale[k] = (s.scale[k] - mn[3 + k]) / (mx[3 + k] - mn[3 + k]);
+          s.dc0[k] = (s.dc0[k] - mn[6 + k]) / (mx[6 + k] - mn[6 + k]);
         }
-        s.opacity = (s.opacity - mnc[3]) / (mxc[3] - mnc[3]);
+        s.opacity = (s.opacity - mn[9]) / (mx[9] - mn[9]);
         for (int j = 0; j < 15; ++j)
-          for (int k = 0; k < 3; ++k) s.sh[j * 3 + k] = (s.sh[j * 3 + k] - mnh[k]) / (mxh[k] - mnh[k]);
+          for (int k = 0; k < 3; ++k) s.sh[j * 3 + k] = (s.sh[j * 3 + k] - mn[10 + k]) / (mx[10 + k] - mn[10 + k]);
       }
     }
   }
 
-  // ---- positions (E/...:760-774, 807-829) ----
+  // ---- positions, other, colour, SH (E/...:705-1066) ----
   std::memset(pos_out, 0, sz.pos_bytes);
   std::memset(other_out, 0, sz.other_bytes);
   std::memset(color_out, 0, sz.color_bytes);
   if (shf <= 3) std::memset(sh_out, 0, sz.sh_bytes);
-  const uint32_t pstride = vector_size(pf), ostride = 4 + vector_size(sf) + (shf > 3 ? 2 : 0), cstride = color_size(cf),
-                 hstride = sh_stride(shf);
   // BC7 is encoded from the float image, 4x4 texels at a time (E/...:887-912)
   std::vector<float> image;
   if (cf == 3) image.assign((size_t)sz.tex_width * sz.tex_height * 4, 0.0f);
+  const EmitTarget to{(uint8_t *)pos_out, (uint8_t *)other_out, (uint8_t *)color_out, (uint8_t *)sh_out, image.data(), pf, sf, cf, shf};
 #pragma omp parallel for schedule(static) num_threads(gsa_usable_threads())
-  for (int64_t i = 0; i < (int64_t)n; ++i) {
-    const GsaInputSplat &s = splats[i];
-    emit_vector(s.pos, (uint8_t *)pos_out + (uint64_t)i * pstride, pf);
-    // other: rotation 10.10.10.2 + scale (E/...:776-805)
-    uint8_t *o = (uint8_t *)other_out + (uint64_t)i * ostride;
-    uint32_t rq = enc_quat10(s.rot);
-    std::memcpy(o, &rq, 4);
-    emit_vector(s.scale, o + 4, sf);
-    if (shf > 3) { uint16_t l = (uint16_t)sh_labels[i]; std::memcpy(o + ostride - 2, &l, 2); }  // E/...:801-803
-    // colour texel, Morton-swizzled (E/...:873-885, 661-703)
-    const uint64_t texel = splat_index_to_texture_index((uint32_t)i);
-    uint8_t *cdst = (uint8_t *)color_out + texel * cstride;
-    float pix[4] = {s.dc0[0], s.dc0[1], s.dc0[2], s.opacity};
-    if (cf == 3) {
-      std::memcpy(&image[texel * 4], pix, 16);
-    } else if (cf == 0) {
-      std::memcpy(cdst, pix, 16);
-    } else if (cf == 1) {
-      uint16_t h[4];
-      for (int k = 0; k < 4; ++k) h[k] = (uint16_t)unity_f32tof16(pix[k]);
-      std::memcpy(cdst, h, 8);
-    } else {
-      for (int k = 0; k < 4; ++k) pix[k] = saturate(pix[k]);
-      uint32_t enc = (uint32_t)(pix[0] * 255.5f) | ((uint32_t)(pix[1] * 255.5f) << 8) |
-                     ((uint32_t)(pix[2] * 255.5f) << 16) | ((uint32_t)(pix[3] * 255.5f) << 24);
-      std::memcpy(cdst, &enc, 4);
-    }
-    // SH table item (E/...:934-1037)
-    if (shf > 3) continue;  // palette already written
-    uint8_t *h = (uint8_t *)sh_out + (uint64_t)i * hstride;
-    if (shf == 0) {
-      std::memcpy(h, s.sh, 180);  // 12 bytes of padding stay zero
-    } else if (shf == 1) {
-      uint16_t t[45];
-      for (int k = 0; k < 45; ++k) t[k] = (uint16_t)unity_f32tof16(s.sh[k]);
-      std::memcpy(h, t, 90);
-    } else if (shf == 2) {
-      uint32_t t[15];
-      for (int j = 0; j < 15; ++j) t[j] = enc_norm11(&s.sh[j * 3]);  // no saturate in the reference (E/...:990-1008)
-      std::memcpy(h, t, 60);
-    } else {
-      uint16_t t[16];
-      for (int j = 0; j < 15; ++j) t[j] = enc_norm565(&s.sh[j * 3]);
-      t[15] = 0;
-      std::memcpy(h, t, 32);
-    }
-  }
+  for (int64_t i = 0; i < (int64_t)n; ++i)
+    emit_splat(to, (uint32_t)i, reinterpret_cast<const float *>(&splats[i]), shf > 3 ? (uint32_t)sh_labels[i] : 0u);
   if (cf == 3) {
     const uint32_t bw = sz.tex_width / 4, bh = sz.tex_height / 4;
 #pragma omp parallel for schedule(static) num_threads(gsa_usable_threads())

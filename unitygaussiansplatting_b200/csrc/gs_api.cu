@@ -528,17 +528,12 @@ int gs_asset_upload(GsContext *ctx, const GsAssetDesc *d, GsAsset **out) {
   if (d->color_format > GS_COL_BC7) return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "unknown colour format");
   if (d->sh_format > GS_SH_CLUSTER4K) return fail(ctx, GS_ERR_UNSUPPORTED_FORMAT, "unknown SH format");
   const uint64_t n = d->splat_count;
-  // bytes per texel: Float32x4 16, Float16x4 8, Norm8x4 4, BC7 1 (16-byte 4x4 blocks), R/GaussianSplatAsset.cs:58-68
-  const uint32_t colsz = d->color_format == 0 ? 16u : d->color_format == 1 ? 8u : d->color_format == 2 ? 4u : 1u;
   // clustered SH (R/GaussianSplatAsset.cs:135-150,187-198): the blob is a palette of 64k..4k Float16 entries and every
   // splat carries a u16 palette index at the end of its `other` record (S/GaussianSplatting.hlsl:447-448,467-470)
   const bool clustered = d->sh_format > GS_SH_NORM6;
-  const uint64_t sh_items = clustered ? (uint64_t)(65536u >> (d->sh_format - GS_SH_CLUSTER64K)) : n;
-  const uint32_t shst = d->sh_format == 0 ? 192u : (d->sh_format == 1 || clustered) ? 96u : d->sh_format == 2 ? 60u : 32u;
-  uint32_t th = (uint32_t)((n + kTexWidth - 1) / kTexWidth);
-  th = (th + 15) / 16 * 16;
-  if (d->pos_bytes < n * vec_stride(d->pos_format) || d->other_bytes < n * (4 + vec_stride(d->scale_format) + (clustered ? 2u : 0u)) ||
-      d->sh_bytes < sh_items * shst || d->color_bytes < (uint64_t)kTexWidth * th * colsz)
+  if (d->pos_bytes < n * vec_stride(d->pos_format) || d->other_bytes < n * other_stride(d->scale_format, d->sh_format) ||
+      d->sh_bytes < (uint64_t)sh_count(d->sh_format, d->splat_count) * sh_stride(d->sh_format) ||
+      d->color_bytes < (uint64_t)kTexWidth * tex_height(n) * color_size(d->color_format))
     return fail(ctx, GS_ERR_INVALID_ARGUMENT, "asset blob smaller than its format requires");
   const uint32_t chunk_count = (d->chunks && d->chunk_bytes) ? (uint32_t)(d->chunk_bytes / 64) : 0;
   GS_CUDA_TRY(ctx, cudaSetDevice(ctx->device));

@@ -11,23 +11,25 @@
 #include <stdint.h>
 
 #include "../../include/gsplat_b200.h"
+#include "gs_asset_format.h"   // kChunkSize, kTexWidth, vec_stride, splat_index_to_texel, ChunkInfo
 
 namespace gs {
 
-constexpr int kChunkSize = 256;     // R/GaussianSplatAsset.cs:14, S/GaussianSplatting.hlsl:207
-constexpr int kTexWidth = 2048;     // R/GaussianSplatAsset.cs:15, S/GaussianSplatting.hlsl:181
 constexpr int kTile = 16;           // raster CTA tile edge in pixels
 constexpr int kBin = 64;            // binning cell edge in pixels: one list per 64x64 cell, shared by its sixteen 16x16 raster tiles
 constexpr int kViewStride = 40;     // sizeof(SplatViewData), S/GaussianSplatting.hlsl:610-615
 
-// SplatChunkInfo, S/GaussianSplatting.hlsl:196-202 (64 bytes)
+// SplatChunkInfo as the frame kernels read it (S/GaussianSplatting.hlsl:196-202): ChunkInfo with float2 ranges, 16-byte aligned
 struct __align__(16) Chunk {
   uint32_t colR, colG, colB, colA;
   float2 posX, posY, posZ;
   uint32_t sclX, sclY, sclZ;
   uint32_t shR, shG, shB;
 };
-static_assert(sizeof(Chunk) == 64, "chunk layout");
+static_assert(sizeof(Chunk) == sizeof(ChunkInfo) && offsetof(Chunk, posX) == offsetof(ChunkInfo, posX) &&
+                  offsetof(Chunk, posZ) == offsetof(ChunkInfo, posZ) && offsetof(Chunk, sclX) == offsetof(ChunkInfo, sclX) &&
+                  offsetof(Chunk, shB) == offsetof(ChunkInfo, shB),
+              "Chunk is ChunkInfo's layout");
 static_assert(kBin == (int)GS_BAND_PIXELS, "the public header documents the partition row height");
 
 // SplatViewData as two 16-byte vectors + one 8-byte vector
@@ -61,10 +63,6 @@ struct AssetView {     // device pointers + formats of one uploaded asset
   const uint8_t *pos, *other, *sh, *color;
   const Chunk *chunks;
 };
-
-__host__ __device__ __forceinline__ uint32_t vec_stride(uint32_t fmt) {
-  return fmt == 0 ? 12u : fmt == 1 ? 6u : fmt == 2 ? 4u : 2u;
-}
 
 // Pixels the +-2 quad of a splat can reach from its centre, given the bound `l1sq` on lambda1 of its 2-D covariance:
 // 2 (|a1x| + |a2x|) <= 2 sqrt(2) |axis1|, |axis1| = min(sqrt(2 lambda1), 4096); 2.9 instead of 2.83 and the two extra pixels
@@ -127,18 +125,6 @@ __device__ __forceinline__ uint32_t float_to_sortable_uint(float f) {
   uint32_t fu = __float_as_uint(f);
   uint32_t mask = (uint32_t)(-(int32_t)(fu >> 31)) | 0x80000000u;
   return fu ^ mask;
-}
-
-// S/GaussianSplatting.hlsl:120-127 + :183-194 -> linear texel index in the 2048-wide image
-__device__ __forceinline__ uint32_t splat_index_to_texel(uint32_t idx) {
-  uint32_t t = (idx & 0xFF) | ((idx & 0xFE) << 7);
-  t &= 0x5555;
-  t = (t ^ (t >> 1)) & 0x3333;
-  t = (t ^ (t >> 2)) & 0x0f0f;
-  uint32_t mx = t & 0xF, my = t >> 8;
-  uint32_t tile = idx >> 8;
-  uint32_t x = (tile % (kTexWidth / 16)) * 16 + mx, y = (tile / (kTexWidth / 16)) * 16 + my;
-  return y * kTexWidth + x;
 }
 
 // Deterministic exp for x <= 0 (see DESIGN.md): 2^(x*log2e), magic-number rint, degree-5 polynomial.

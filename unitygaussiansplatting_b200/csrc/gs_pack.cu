@@ -1,17 +1,20 @@
 // gs_pack.cu -- the asset packer on the GPU: gs_pack_asset / gs_kmeans / gs_pack_sizes (include/gsplat_b200.h).
 //
-// The host packer (csrc/asset_creator.cpp gsa_create_asset, csrc/asset_cluster_bc7.cpp gsa_kmeans / gsa_bc7_encode_block) is
-// the specification: for finite input every stage below produces the same floats, and so the same bytes.  What that takes:
-//   * sequential std::min / std::max folds become (value, index) reductions where the earliest index wins among equal values
+// Writes the same bytes as the host packer (csrc/asset_creator.cpp gsa_create_asset, csrc/asset_cluster_bc7.cpp gsa_kmeans)
+// for finite input.  The format itself -- sizes, the chunk record, the pcg stream, the scalar encoders, one splat's records,
+// the chunk header, the k-means squared distance, the BC7 block encoder -- is gs_asset_format.h, shared with the host
+// packer.  What this file does its own way, and what keeps it equal to the host's sequential code:
+//   * sequential math.min / math.max folds become (value, index) reductions where the earliest index wins among equal values
 //     (so -0 vs +0 comes out as the fold leaves it) and NaN never wins;
 //   * every float sum the host evaluates sequentially is evaluated sequentially here too (per-1024 k-means++ block sums, the
 //     prefix over blocks, the in-block pick scan); the host sums that are cheap stay on the host (validation distance sum);
-//   * the squared distance keeps the host's grouping: pairs of squares, ((h0+h1)+h2)+h3 per 8 dimensions, tail left to right;
-//   * no contraction anywhere (-fmad=false), IEEE division and square root;
+//   * the tiled nearest-mean kernel keeps distance_squared's grouping: pairs of squares, ((h0+h1)+h2)+h3 per 8 dimensions,
+//     tail left to right;
+//   * a chunk whose range is 0 / 0 normalises to x86's default NaN (host_div);
 //   * scale^(1/8) is a double pow narrowed to float; CUDA's pow may differ from glibc's in the last double ulp, which changes
 //     the float only next to a float rounding midpoint.  Such values are flagged and recomputed on the host with std::pow.
-//   * every random draw of the k-means is independent of the data, so the host replays gsa_kmeans' RNG and uploads the
-//     batch index lists; the device never runs a sequential RNG.
+//   * every random draw of the k-means is independent of the data, so the host replays gsa_kmeans' pcg stream and uploads
+//     the batch index lists; the device never runs a sequential RNG.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -25,61 +28,8 @@
 namespace gs {
 namespace {
 
-constexpr uint32_t kRecFloats = 62;   // GsInputSplat
-constexpr uint32_t kOffDc0 = 6, kOffSh = 9, kOffOpacity = 54, kOffScale = 55, kOffRot = 58;
 constexpr uint32_t kMaxKmeansDim = 128;
 static_assert(sizeof(GsInputSplat) == kRecFloats * 4, "InputSplatData must be 248 bytes");
-
-// ---- format arithmetic (gsa_calc_sizes, R/GaussianSplatAsset.cs) ---------------------------------------------------
-inline uint32_t color_size(uint32_t f) { return f == 0 ? 16u : f == 1 ? 8u : f == 2 ? 4u : 1u; }
-__host__ __device__ inline uint32_t sh_stride(uint32_t f) { return f == 0 ? 192u : f == 1 ? 96u : f == 2 ? 60u : f == 3 ? 32u : 96u; }
-inline uint32_t sh_count(uint32_t f, uint32_t n) { return f <= 3 ? n : (65536u >> (f - 4)); }
-inline bool uses_chunks(uint32_t pf, uint32_t sf, uint32_t cf, uint32_t shf) { return pf != 0 || sf != 0 || cf != 0 || shf != 0; }
-inline uint64_t next_multiple(uint64_t v, uint64_t m) { return (v + m - 1) / m * m; }
-
-bool calc_sizes(uint32_t n, uint32_t pf, uint32_t sf, uint32_t cf, uint32_t shf, GsPackSizes *out) {
-  if (pf > 3 || sf > 3 || cf > 3 || shf > 8) return false;
-  if (shf > 3 && n <= sh_count(shf, n)) return false;
-  uint32_t h = std::max<uint32_t>(1, (n + kTexWidth - 1) / kTexWidth);
-  h = (h + 15) / 16 * 16;
-  out->tex_width = kTexWidth;
-  out->tex_height = h;
-  out->pos_bytes = next_multiple((uint64_t)n * vec_stride(pf), 8);
-  out->other_bytes = next_multiple((uint64_t)n * (4 + vec_stride(sf) + (shf > 3 ? 2 : 0)), 8);
-  out->color_bytes = (uint64_t)kTexWidth * h * color_size(cf);
-  out->sh_bytes = (uint64_t)sh_count(shf, n) * sh_stride(shf);
-  out->chunk_bytes = uses_chunks(pf, sf, cf, shf) ? (uint64_t)((n + kChunkSize - 1) / kChunkSize) * 64 : 0;
-  return true;
-}
-
-// ---- the k-means RNG, replayed on the host (K:571-593 of the reference, gsa_kmeans) -------------------------------------
-inline uint32_t pcg_hash(uint32_t input) {
-  uint32_t state = input * 747796405u + 2891336453u;
-  uint32_t word = ((state >> ((state >> 28) + 4u)) ^ state) * 277803737u;
-  return (word >> 22) ^ word;
-}
-inline uint32_t pcg_random(uint32_t &rng_state) {
-  uint32_t state = rng_state;
-  rng_state = rng_state * 747796405u + 2891336453u;
-  uint32_t word = ((state >> ((state >> 28) + 4u)) ^ state) * 277803737u;
-  return (word >> 22) ^ word;
-}
-// make_random_batch: distinct random points in draw order
-void random_batch(uint32_t n, uint32_t &rng, uint32_t batch, std::vector<uint8_t> &picked, uint32_t *out) {
-  uint32_t seed = pcg_random(rng);
-  uint32_t got = 0;
-  while (got < batch) {
-    uint32_t index = pcg_hash(seed++) % n;
-    if (!picked[index]) { picked[index] = 1; out[got++] = index; }
-  }
-  for (uint32_t i = 0; i < batch; ++i) picked[out[i]] = 0;
-}
-
-__device__ __forceinline__ uint32_t d_pcg_hash(uint32_t input) {
-  uint32_t state = input * 747796405u + 2891336453u;
-  uint32_t word = ((state >> ((state >> 28) + 4u)) ^ state) * 277803737u;
-  return (word >> 22) ^ word;
-}
 
 // ---- ordered reductions: the result of a sequential Unity.Mathematics math.min / math.max fold ------------------------
 // `acc = math.min(acc, x)` keeps acc only when acc < x strictly (or x is NaN): of equal values (+0 / -0) the LATER one wins.
@@ -159,15 +109,6 @@ __global__ void __launch_bounds__(256) k_bounds_final(const float *part_v, const
 }
 
 // ---- 2. Morton reorder (E/...:387-429) ----------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t part1by2(uint64_t x) {
-  x &= 0x1fffff;
-  x = (x ^ (x << 32)) & 0x1f00000000ffffULL;
-  x = (x ^ (x << 16)) & 0x1f0000ff0000ffULL;
-  x = (x ^ (x << 8)) & 0x100f00f00f00f00fULL;
-  x = (x ^ (x << 4)) & 0x10c30c30c30c30c3ULL;
-  x = (x ^ (x << 2)) & 0x1249249249249249ULL;
-  return x;
-}
 __global__ void __launch_bounds__(256) k_morton(const float *__restrict__ rec, uint32_t n, const float *__restrict__ bounds,
                                                 uint32_t *lo, uint32_t *hi, uint32_t *idx) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -179,7 +120,7 @@ __global__ void __launch_bounds__(256) k_morton(const float *__restrict__ rec, u
     const float p = (rec[(size_t)i * kRecFloats + k] - bounds[k]) * inv * kScaler;
     ip[k] = (p >= 0.0f && p < 4294967296.0f) ? (uint32_t)p : 0u;
   }
-  const uint64_t code = (part1by2(ip[2]) << 2) | (part1by2(ip[1]) << 1) | part1by2(ip[0]);
+  const uint64_t code = morton_encode3(ip[0], ip[1], ip[2]);
   lo[i] = (uint32_t)code;
   hi[i] = (uint32_t)(code >> 32);
   idx[i] = i;
@@ -198,20 +139,6 @@ __global__ void k_gather_rows(const float *__restrict__ src, uint32_t src_stride
 }
 
 // ---- 3. k-means (K:29-136 of the reference, gsa_kmeans) --------------------------------------------------------------------
-// DistanceSquared with the host's grouping
-__device__ __forceinline__ float dist_sq(const float *a, const float *b, uint32_t dim) {
-  float d = 0.0f;
-  uint32_t i = 0;
-  for (; i + 7 < dim; i += 8) {
-    float v[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) { const float t = a[i + k] - b[i + k]; v[k] = t * t; }
-    d += (v[0] + v[1]) + (v[2] + v[3]) + (v[4] + v[5]) + (v[6] + v[7]);
-  }
-  for (; i < dim; ++i) { const float t = a[i] - b[i]; d += t * t; }
-  return d;
-}
-
 // Nearest mean of every point (AssignClustersJob, K:423-441: strict <, the first of equal distances wins, start FLT_MAX / 0).
 // A CTA takes 64 points (all their dimensions in shared memory) against 64-centre tiles; a thread owns 4 points x 4 centres.
 // gridDim.y splits the centre tiles (tile t goes to split t % gridDim.y); each split writes its (best, index) per point and
@@ -337,7 +264,7 @@ __global__ void __launch_bounds__(1024) k_kpp_round(const float *__restrict__ pt
   if (i < m) {
     tk = taken[i];
     if (!tk) {
-      const float d = dist_sq(pts + (size_t)i * dim, newest, dim);
+      const float d = distance_squared(pts + (size_t)i * dim, newest, dim);
       const float old = min_dist[i];
       v = first ? d : ((d < old) ? d : old);   // std::min(min_dist, d)
       min_dist[i] = v;
@@ -361,8 +288,7 @@ __global__ void __launch_bounds__(1024) k_kpp_round(const float *__restrict__ pt
   if (t == 0) {
     float total = 0.0f;
     for (uint32_t bb = 0; bb < nb; ++bb) { total += __ldcg(&partial[bb]); partial[bb] = total; }
-    const float f = __uint_as_float(0x3f800000u | (d_pcg_hash(rng + rc) >> 9)) - 1.0f;   // pcg_hash_float(rng + rc, total)
-    const float rval = f * total;
+    const float rval = pcg_hash_float(rng + rc, total);
     uint32_t lo = 0, hi = nb;
     while (lo < hi) {
       const uint32_t mid = (lo + hi) / 2;
@@ -459,25 +385,6 @@ __global__ void k_scatter_scales(float *rec, const uint32_t *idx, const float *v
   if (t < count) rec[(size_t)(idx[t] / 3u) * kRecFloats + kOffScale + idx[t] % 3u] = val[t];
 }
 
-// Unity.Mathematics math.f32tof16, as restated by the host packer
-__device__ __forceinline__ uint32_t unity_f32tof16(float x) {
-  const int32_t infinity_32 = 255 << 23;
-  const uint32_t msk = 0x7FFFF000u;
-  const uint32_t ux = __float_as_uint(x), uux = ux & msk;
-  const float a = __uint_as_float(uux) * 1.92592994e-34f;
-  const float scaled = (260042752.0f < a) ? 260042752.0f : a;   // std::min(a, 260042752)
-  uint32_t h = (__float_as_uint(scaled) + 0x1000u) >> 13;
-  if ((int32_t)uux >= infinity_32) h = ((int32_t)uux > infinity_32) ? 0x7e00u : 0x7c00u;
-  return h | ((ux & ~msk) >> 16);
-}
-__device__ __forceinline__ float square_centered01(float x) {
-  x -= 0.5f;
-  const float sgn = (x > 0.0f) ? 1.0f : ((x < 0.0f) ? -1.0f : 0.0f);
-  x *= x * sgn;
-  return x * 2.0f + 0.5f;
-}
-__device__ __forceinline__ float unity_max(float x, float y) { return (isnan(y) || x > y) ? x : y; }   // math.max(x, y)
-
 // a / b as an x86 host computes it: a chunk whose range is 0 (|min| >= 256, where min + 1e-5 rounds back to min) divides
 // 0 by 0, and the NaN that writes into Float32 / Float16 blobs is x86's default NaN 0xFFC00000, not the GPU's 0x7FFFFFFF
 __device__ __forceinline__ float host_div(float a, float b) { const float q = a / b; return isnan(q) ? __uint_as_float(0xFFC00000u) : q; }
@@ -515,21 +422,10 @@ __global__ void __launch_bounds__(256) k_chunks(float *rec, uint32_t n, Chunk *c
     if (t == 0) { s_mn[q] = mn; s_mx[q] = unity_max(mx, mn + 1.0e-5f); }
   }
   __syncthreads();
-  if (t == 0) {
+  if (t == 0) {   // stored through the 16-byte aligned device view: four 16-byte stores
+    const ChunkInfo info = encode_chunk(s_mn, s_mx);
     Chunk c;
-    c.posX = make_float2(s_mn[0], s_mx[0]);
-    c.posY = make_float2(s_mn[1], s_mx[1]);
-    c.posZ = make_float2(s_mn[2], s_mx[2]);
-    c.sclX = unity_f32tof16(s_mn[3]) | (unity_f32tof16(s_mx[3]) << 16);
-    c.sclY = unity_f32tof16(s_mn[4]) | (unity_f32tof16(s_mx[4]) << 16);
-    c.sclZ = unity_f32tof16(s_mn[5]) | (unity_f32tof16(s_mx[5]) << 16);
-    c.colR = unity_f32tof16(s_mn[6]) | (unity_f32tof16(s_mx[6]) << 16);
-    c.colG = unity_f32tof16(s_mn[7]) | (unity_f32tof16(s_mx[7]) << 16);
-    c.colB = unity_f32tof16(s_mn[8]) | (unity_f32tof16(s_mx[8]) << 16);
-    c.colA = unity_f32tof16(s_mn[9]) | (unity_f32tof16(s_mx[9]) << 16);
-    c.shR = unity_f32tof16(s_mn[10]) | (unity_f32tof16(s_mx[10]) << 16);
-    c.shG = unity_f32tof16(s_mn[11]) | (unity_f32tof16(s_mx[11]) << 16);
-    c.shB = unity_f32tof16(s_mn[12]) | (unity_f32tof16(s_mx[12]) << 16);
+    memcpy(&c, &info, sizeof(c));
     chunks[blockIdx.x] = c;
   }
   if (!live) return;
@@ -544,76 +440,16 @@ __global__ void __launch_bounds__(256) k_chunks(float *rec, uint32_t n, Chunk *c
 }
 
 // ---- 5. emit (E/...:705-1066) ---------------------------------------------------------------------------------------------
-// Every record stride of `other` is even but not always a multiple of 4: all stores are 16-bit.
-__device__ __forceinline__ void put16(uint8_t *p, uint32_t v) { *(uint16_t *)p = (uint16_t)v; }
-__device__ __forceinline__ void put32(uint8_t *p, uint32_t v) { put16(p, v & 0xffffu); put16(p + 2, v >> 16); }
-// math.saturate = max(0, min(1, v)) with math.min / max: NaN -> 1 (a chunk whose range is 0 / 0)
-__device__ __forceinline__ float sat(float v) { const float m = (isnan(v) || 1.0f < v) ? 1.0f : v; return (0.0f > m) ? 0.0f : m; }
-__device__ __forceinline__ uint32_t enc_norm11(const float *v) {
-  return (uint32_t)(v[0] * 2047.5f) | ((uint32_t)(v[1] * 1023.5f) << 11) | ((uint32_t)(v[2] * 2047.5f) << 21);
-}
-__device__ __forceinline__ uint32_t enc_norm565(const float *v) {
-  return ((uint32_t)(v[0] * 31.5f) | ((uint32_t)(v[1] * 63.5f) << 5) | ((uint32_t)(v[2] * 31.5f) << 11)) & 0xffffu;
-}
-__device__ void emit_vector(const float *v, uint8_t *dst, uint32_t fmt) {
-  if (fmt == 0) {
-    for (int k = 0; k < 3; ++k) put32(dst + 4 * k, __float_as_uint(v[k]));
-    return;
-  }
-  const float s[3] = {sat(v[0]), sat(v[1]), sat(v[2])};
-  if (fmt == 1) {
-    for (int k = 0; k < 3; ++k) put16(dst + 2 * k, (uint32_t)(uint64_t)(s[k] * 65535.5f));
-  } else if (fmt == 2) {
-    put32(dst, enc_norm11(s));
-  } else {
-    put16(dst, (uint32_t)(s[0] * 63.5f) | ((uint32_t)(s[1] * 31.5f) << 6) | ((uint32_t)(s[2] * 31.5f) << 11));
-  }
-}
-
 struct EmitArgs {
   const float *rec;
-  uint32_t n, pf, sf, cf, shf;
-  uint8_t *pos, *other, *color, *sh;
-  float4 *image;           // BC7: the float image the blocks are encoded from
+  uint32_t n;
+  EmitTarget to;           // image: BC7's float image, of float4 texels
   const int32_t *labels;   // clustered SH: palette index per splat
 };
 __global__ void __launch_bounds__(256) k_emit(EmitArgs a) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.n) return;
-  const float *s = a.rec + (size_t)i * kRecFloats;
-  emit_vector(s, a.pos + (size_t)i * vec_stride(a.pf), a.pf);
-  const uint32_t ostride = 4 + vec_stride(a.sf) + (a.shf > 3 ? 2 : 0);
-  uint8_t *o = a.other + (size_t)i * ostride;
-  const float *q = s + kOffRot;
-  put32(o, (uint32_t)(q[0] * 1023.5f) | ((uint32_t)(q[1] * 1023.5f) << 10) | ((uint32_t)(q[2] * 1023.5f) << 20) |
-               ((uint32_t)(q[3] * 3.5f) << 30));
-  emit_vector(s + kOffScale, o + 4, a.sf);
-  if (a.shf > 3) put16(o + ostride - 2, (uint32_t)a.labels[i] & 0xffffu);
-  const uint32_t texel = splat_index_to_texel(i);
-  float pix[4] = {s[kOffDc0], s[kOffDc0 + 1], s[kOffDc0 + 2], s[kOffOpacity]};
-  if (a.cf == 3) {
-    a.image[texel] = make_float4(pix[0], pix[1], pix[2], pix[3]);
-  } else if (a.cf == 0) {
-    for (int k = 0; k < 4; ++k) put32(a.color + (size_t)texel * 16 + 4 * k, __float_as_uint(pix[k]));
-  } else if (a.cf == 1) {
-    for (int k = 0; k < 4; ++k) put16(a.color + (size_t)texel * 8 + 2 * k, unity_f32tof16(pix[k]));
-  } else {
-    for (int k = 0; k < 4; ++k) pix[k] = sat(pix[k]);
-    put32(a.color + (size_t)texel * 4, (uint32_t)(pix[0] * 255.5f) | ((uint32_t)(pix[1] * 255.5f) << 8) |
-                                          ((uint32_t)(pix[2] * 255.5f) << 16) | ((uint32_t)(pix[3] * 255.5f) << 24));
-  }
-  if (a.shf > 3) return;   // palette written by k_palette
-  const float *h = s + kOffSh;
-  uint8_t *d = a.sh + (size_t)i * sh_stride(a.shf);
-  if (a.shf == 0) {
-    for (int k = 0; k < 45; ++k) put32(d + 4 * k, __float_as_uint(h[k]));
-  } else if (a.shf == 1) {
-    for (int k = 0; k < 45; ++k) put16(d + 2 * k, unity_f32tof16(h[k]));
-  } else if (a.shf == 2) {
-    for (int j = 0; j < 15; ++j) put32(d + 4 * j, enc_norm11(h + j * 3));
-  } else {
-    for (int j = 0; j < 15; ++j) put16(d + 2 * j, enc_norm565(h + j * 3));
-  }
+  emit_splat(a.to, i, a.rec + (size_t)i * kRecFloats, a.to.shf > 3 ? (uint32_t)a.labels[i] : 0u);
 }
 // ConvertSHClustersJob (E/...:443-468): 15 x half3 + one zero half3 per palette entry
 __global__ void k_palette(const float *means, uint32_t k, uint8_t *sh) {
@@ -622,118 +458,20 @@ __global__ void k_palette(const float *means, uint32_t k, uint8_t *sh) {
   put16(sh + (size_t)(t / 45) * 96 + (t % 45) * 2, unity_f32tof16(means[t]));
 }
 
-// ---- 6. BC7 mode 6, gsa_bc7_encode_block's arithmetic (csrc/asset_cluster_bc7.cpp) ------------------------------------
-__constant__ int kW4[16] = {0, 4, 9, 13, 17, 21, 26, 30, 34, 38, 43, 47, 51, 55, 60, 64};
+// ---- 6. BC7 mode 6: one thread per 4x4 block ----------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) k_bc7(const float4 *__restrict__ image, uint32_t bw, uint32_t nblocks, uint8_t *out) {
   const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= nblocks) return;
   const uint32_t bx = b % bw, by = b / bw;
-  float px[16][4], mean[4] = {0, 0, 0, 0};
+  float rgba[64];
   for (int i = 0; i < 16; ++i) {
     const float4 p = image[(size_t)(by * 4 + i / 4) * kTexWidth + bx * 4 + i % 4];
-    const float c4[4] = {p.x, p.y, p.z, p.w};
-    for (int c = 0; c < 4; ++c) {
-      float v = c4[c];
-      v = (v > 0.0f) ? (v < 1.0f ? v : 1.0f) : 0.0f;
-      px[i][c] = v * 255.0f;
-      mean[c] += px[i][c] * (1.0f / 16.0f);
-    }
+    rgba[i * 4] = p.x; rgba[i * 4 + 1] = p.y; rgba[i * 4 + 2] = p.z; rgba[i * 4 + 3] = p.w;
   }
-  float cov[4][4] = {};
-  for (int i = 0; i < 16; ++i)
-    for (int r = 0; r < 4; ++r)
-      for (int c = 0; c < 4; ++c) cov[r][c] += (px[i][r] - mean[r]) * (px[i][c] - mean[c]);
-  float axis[4] = {1.0f, 1.0f, 1.0f, 1.0f};
-  for (int it = 0; it < 8; ++it) {
-    float nv[4] = {0, 0, 0, 0}, len = 0;
-    for (int r = 0; r < 4; ++r) { for (int c = 0; c < 4; ++c) nv[r] += cov[r][c] * axis[c]; len += nv[r] * nv[r]; }
-    if (len < 1e-12f) break;
-    len = 1.0f / sqrtf(len);
-    for (int r = 0; r < 4; ++r) axis[r] = nv[r] * len;
-  }
-  float tmin = 1e30f, tmax = -1e30f;
-  for (int i = 0; i < 16; ++i) {
-    float tt = 0;
-    for (int c = 0; c < 4; ++c) tt += (px[i][c] - mean[c]) * axis[c];
-    tmin = (tt < tmin) ? tt : tmin;
-    tmax = (tmax < tt) ? tt : tmax;
-  }
-  float target[2][4];
-  for (int c = 0; c < 4; ++c) { target[0][c] = mean[c] + axis[c] * tmin; target[1][c] = mean[c] + axis[c] * tmax; }
-  int ep[2][4], pbit[2] = {0, 0}, idx[16];
-  float best_total = 1e30f;
-  int best_ep[2][4] = {}, best_p[2] = {0, 0}, best_idx[16] = {};
-  for (int round = 0; round < 2; ++round) {
-    for (int e = 0; e < 2; ++e) {
-      float best_err = 1e30f;
-      for (int p = 0; p < 2; ++p) {
-        int q[4];
-        float err = 0;
-        for (int c = 0; c < 4; ++c) {
-          const float m0 = (0.0f < target[e][c]) ? target[e][c] : 0.0f;   // std::max(0, target)
-          const float tc = (m0 < 255.0f) ? m0 : 255.0f;                     // std::min(255, .)
-          int v = (int)lroundf((tc - (float)p) * 0.5f);
-          v = v < 0 ? 0 : (v > 127 ? 127 : v);
-          q[c] = (v << 1) | p;
-          const float d = (float)q[c] - tc;
-          err += d * d;
-        }
-        if (err < best_err) { best_err = err; pbit[e] = p; for (int c = 0; c < 4; ++c) ep[e][c] = q[c]; }
-      }
-    }
-    int pal[16][4];
-    for (int w = 0; w < 16; ++w)
-      for (int c = 0; c < 4; ++c) pal[w][c] = ((64 - kW4[w]) * ep[0][c] + kW4[w] * ep[1][c] + 32) >> 6;
-    float total = 0;
-    for (int i = 0; i < 16; ++i) {
-      float bst = 1e30f;
-      int bi = 0;
-      for (int w = 0; w < 16; ++w) {
-        float err = 0;
-        for (int c = 0; c < 4; ++c) { const float d = (float)pal[w][c] - px[i][c]; err += d * d; }
-        if (err < bst) { bst = err; bi = w; }
-      }
-      idx[i] = bi;
-      total += bst;
-    }
-    if (total < best_total) {
-      best_total = total;
-      for (int e = 0; e < 2; ++e) { best_p[e] = pbit[e]; for (int c = 0; c < 4; ++c) best_ep[e][c] = ep[e][c]; }
-      for (int i = 0; i < 16; ++i) best_idx[i] = idx[i];
-    }
-    if (round == 1) break;
-    float saa = 0, sab = 0, sbb = 0, ra[4] = {0, 0, 0, 0}, rb[4] = {0, 0, 0, 0};
-    for (int i = 0; i < 16; ++i) {
-      const float w = (float)kW4[idx[i]] * (1.0f / 64.0f), u = 1.0f - w;
-      saa += u * u; sab += u * w; sbb += w * w;
-      for (int c = 0; c < 4; ++c) { ra[c] += u * px[i][c]; rb[c] += w * px[i][c]; }
-    }
-    const float det = saa * sbb - sab * sab;
-    if (fabsf(det) < 1e-6f) break;
-    for (int c = 0; c < 4; ++c) {
-      target[0][c] = (ra[c] * sbb - rb[c] * sab) / det;
-      target[1][c] = (rb[c] * saa - ra[c] * sab) / det;
-    }
-  }
-  if (best_idx[0] >= 8) {   // the anchor stores 3 bits: swap the endpoints so that its index has a zero top bit
-    for (int c = 0; c < 4; ++c) { const int tmp = best_ep[0][c]; best_ep[0][c] = best_ep[1][c]; best_ep[1][c] = tmp; }
-    const int tp = best_p[0]; best_p[0] = best_p[1]; best_p[1] = tp;
-    for (int i = 0; i < 16; ++i) best_idx[i] = 15 - best_idx[i];
-  }
-  uint64_t w[2] = {0, 0};
-  int pos = 0;
-  auto put = [&](uint32_t v, int nbits) {
-    for (int k = 0; k < nbits; ++k, ++pos)
-      if ((v >> k) & 1u) w[pos >> 6] |= 1ull << (pos & 63);
-  };
-  put(1u << 6, 7);
-  for (int c = 0; c < 4; ++c) { put((uint32_t)best_ep[0][c] >> 1, 7); put((uint32_t)best_ep[1][c] >> 1, 7); }
-  put((uint32_t)best_p[0], 1); put((uint32_t)best_p[1], 1);
-  put((uint32_t)best_idx[0], 3);
-  for (int i = 1; i < 16; ++i) put((uint32_t)best_idx[i], 4);
+  const Bc7Block e = bc7_encode_block(rgba);
   uint64_t *o = (uint64_t *)(out + (size_t)b * 16);
-  o[0] = w[0];
-  o[1] = w[1];
+  o[0] = e.lo;
+  o[1] = e.hi;
 }
 
 // ---- host side ----------------------------------------------------------------------------------------------------------
@@ -770,15 +508,15 @@ int kmeans_device(GsContext *ctx, const float *data, uint32_t stride, uint32_t d
   uint32_t rng = 1;
   std::vector<uint8_t> picked(n, 0);
   std::vector<uint32_t> cb(m), vb(m);
-  random_batch(n, rng, m, picked, cb.data());
-  random_batch(n, rng, m, picked, vb.data());
+  random_batch(n, rng, m, picked.data(), cb.data());
+  random_batch(n, rng, m, picked.data(), vb.data());
   uint32_t point0[3], rng_at[3];
   for (int a = 0; a < 3; ++a) { point0[a] = pcg_random(rng) % m; rng_at[a] = rng; }
   uint32_t iters = 0;
   const float calc_limit = (float)n * passes;
   for (float done = 0.0f; done < calc_limit; done += (float)batch) ++iters;
   std::vector<uint32_t> mb((size_t)iters * batch);
-  for (uint32_t it = 0; it < iters; ++it) random_batch(n, rng, batch, picked, mb.data() + (size_t)it * batch);
+  for (uint32_t it = 0; it < iters; ++it) random_batch(n, rng, batch, picked.data(), mb.data() + (size_t)it * batch);
   ctx->pack_stats[1] = iters;
   ctx->pack_stats[2] = 3ull * (k - 1);
 
@@ -1008,7 +746,7 @@ int gs_pack_asset(GsContext *ctx, const GsPackDesc *desc, GsPackedAsset *blobs_o
     GS_CUDA_TRY(ctx, image.reserve(texels, {st}));
     GS_CUDA_TRY(ctx, cudaMemsetAsync(image.get(), 0, texels * 16, st));
   }
-  EmitArgs ea{recs.get(), n, pf, sf, cf, shf, b_pos.get(), b_other.get(), b_color.get(), b_sh.get(), image.get(), labels.get()};
+  EmitArgs ea{recs.get(), n, {b_pos.get(), b_other.get(), b_color.get(), b_sh.get(), (float *)image.get(), pf, sf, cf, shf}, labels.get()};
   k_emit<<<blocks_for(n, 256), 256, 0, st>>>(ea);
   if (cf == GS_COL_BC7) {
     const uint32_t bw = sz.tex_width / 4, nblocks = bw * (sz.tex_height / 4);
